@@ -115,7 +115,9 @@ int mbar_b200_last_pass_ms(mbar_b200_ctx* ctx, double* ms);
 /* ---- data in / out -------------------------------------------------------------------------- */
 /* Replaces the host copies at mbar.py:243 and mbar_solvers.py:1003: u_host is [K, N_local]
  * row-major with row stride `ld` (elements).  Pinned memory is DMA'd directly; pageable memory is
- * staged through internal pinned buffers.  NaN anywhere -> MBAR_B200_ERR_NAN. */
+ * staged through internal pinned buffers.  NaN anywhere -> MBAR_B200_ERR_NAN.  Once a communicator is
+ * attached (mbar_b200_comm_init) the uploads and mbar_b200_synthesize are collective: every rank calls them, since
+ * the ranks agree on each state's lowest shifted energy, which decides the kernel of all-state passes. */
 int mbar_b200_upload_u_kn(mbar_b200_ctx* ctx, const double* u_host, int64_t ld);
 /* Same, from a row-major DEVICE buffer on ctx's device (e.g. a torch tensor's data_ptr). */
 int mbar_b200_upload_u_kn_dev(mbar_b200_ctx* ctx, const double* u_dev, int64_t ld);
@@ -210,6 +212,11 @@ int mbar_b200_last_hessian_ms(mbar_b200_ctx* ctx, double* weights_ms, double* he
 /* fp64 ceilings of this GPU measured in place (register-only DMMA.8x8x4 and DFMA loops), in TFLOP/s: the
  * roofline denominator of mbar_b200_hessian (MEASURED_PEAKS.json has no fp64 figure). */
 int mbar_b200_measure_fp64_peak(int device, double* dmma_tflops, double* dfma_tflops);
+/* Development probe of the device exp: out[i] = exp(a[i]) for n host arguments, evaluated by
+ * which = 0: exp_fast (generic pass, Hessian weights); 1: the fused pass's exp with the state constant in the
+ * exponent (MODE=1); 2: its multiplicative form e0 = exp(-u') (MODE=3).  Arguments below about -707.7 return
+ * a value in [0, 2^-1020]; arguments above 709.7 are outside the contract (the host never passes them). */
+int mbar_b200_probe_exp(int device, int which, int64_t n, const double* a_host, double* out_host);
 
 /* ---- one-shot, host-buffer entry (what a binding without residency would call) --------------- */
 /* self_consistent_update on host buffers: upload u_kn, one pass, f_out — copies inside the call. */

@@ -78,6 +78,7 @@ SIGNATURES = {
     "mbar_b200_last_kernels": (C.c_int, [_ctx, C.c_char_p, C.c_char_p, C.c_int32]),
     "mbar_b200_last_hessian_ms": (C.c_int, [_ctx, _dp, _dp]),
     "mbar_b200_measure_fp64_peak": (C.c_int, [C.c_int, _dp, _dp]),
+    "mbar_b200_probe_exp": (C.c_int, [C.c_int, C.c_int, C.c_int64, _dp, _dp]),
     "mbar_b200_sci_iterate": (C.c_int, [_ctx, _dp, C.c_int32]),
     "mbar_b200_last_loop_ms": (C.c_int, [_ctx, _dp, _dp, C.POINTER(C.c_int32)]),
     "mbar_b200_self_consistent_update_host": (C.c_int, [C.c_int, C.c_int32, C.c_int64, C.c_void_p, C.c_int64,

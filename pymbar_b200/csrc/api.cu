@@ -57,6 +57,23 @@ int comm_allreduce(mbar_b200_ctx* ctx, double* d_buf, int count, int op) {
     return MBAR_B200_OK;
 }
 
+// The lowest shifted energy of every row over all shards (max of its negation), so that every rank makes the same
+// fused / log-domain choice for its all-state passes and issues the same collectives.
+int agree_row_minima(mbar_b200_ctx* c) {
+    if (!c->comm || c->nranks == 1) return MBAR_B200_OK;
+    const int K = c->K;
+    std::vector<double> neg(K);
+    for (int k = 0; k < K; ++k) neg[k] = -c->h_urowmin[k];
+    MBAR_CUDA(cudaMemcpyAsync(c->d_scratch, neg.data(), (size_t)K * sizeof(double), cudaMemcpyHostToDevice,
+                              c->stream));
+    MBAR_TRY(comm_allreduce(c, c->d_scratch, K, 2));
+    MBAR_CUDA(cudaMemcpyAsync(neg.data(), c->d_scratch, (size_t)K * sizeof(double), cudaMemcpyDeviceToHost,
+                              c->stream));
+    MBAR_CUDA(cudaStreamSynchronize(c->stream));
+    for (int k = 0; k < K; ++k) c->h_urowmin[k] = -neg[k];
+    return MBAR_B200_OK;
+}
+
 // logS of unsampled states across ranks: logsumexp over ranks of the local log-sums.
 __global__ void logs_to_scaled(double* logS, const double* mx, double* scaled, int K) {
     const int k = blockIdx.x * blockDim.x + threadIdx.x;
@@ -895,15 +912,7 @@ int mbar_b200_comm_init(mbar_b200_ctx* c, int32_t nranks, int32_t rank, const vo
     c->nranks = nranks;
     c->rank = rank;
     // kernel-selection inputs must be identical on every rank (all ranks issue the same collectives)
-    {
-        double flag = c->unsampledExtreme ? 1.0 : 0.0;
-        MBAR_CUDA(cudaMemcpyAsync(c->d_scratch, &flag, sizeof(double), cudaMemcpyHostToDevice, c->stream));
-        MBAR_TRY(comm_allreduce(c, c->d_scratch, 1, 2));
-        MBAR_CUDA(cudaMemcpyAsync(&flag, c->d_scratch, sizeof(double), cudaMemcpyDeviceToHost, c->stream));
-        MBAR_CUDA(cudaStreamSynchronize(c->stream));
-        c->unsampledExtreme = flag != 0.0;
-    }
-    return MBAR_B200_OK;
+    return agree_row_minima(c);
 }
 
 static size_t inbox_doubles(int K) { return (size_t)2 * MAX_PEERS * 2 * (K + 2); }   // (2 candidates per launch)

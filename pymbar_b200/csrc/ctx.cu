@@ -197,6 +197,14 @@ static void* pool_park(Parked& slot, void* ptr, size_t bytes) {
     return old;
 }
 
+// Running minimum of one row's negative shifted energies (rounded down), one atomic per warp and row at most.
+// Sampled rows are >= 0 after the shift, so in practice only unsampled rows below the sampled minimum report.
+__device__ __forceinline__ void row_min_push(int* rowMin, double v, int lane) {
+    int vi = v < 0.0 ? (int)fmax(floor(v), -1073741824.0) : 0;
+    vi = __reduce_min_sync(0xffffffffu, vi);
+    if (lane == 0 && vi < 0) atomicMin(rowMin, vi);
+}
+
 // ------------------------------------------------------------------------------------------
 // Re-tile + shift kernel.  One CTA (8 warps) per tile; lane = sample, warp w owns rows w, w+8, ...
 // ------------------------------------------------------------------------------------------
@@ -205,7 +213,7 @@ __global__ void __launch_bounds__(256) retile_kernel(const double* __restrict__ 
                                                      const unsigned long long* __restrict__ rowmask,
                                                      double* __restrict__ dst,
                                                      double* __restrict__ xshift,
-                                                     int* __restrict__ flags) {
+                                                     int* __restrict__ flags, int* __restrict__ urowmin) {
     __shared__ double s_min[8][TILE_N];
     __shared__ int s_bad[8];
     const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
@@ -238,14 +246,12 @@ __global__ void __launch_bounds__(256) retile_kernel(const double* __restrict__ 
     if (!valid || !finiteShift) x = 0.0;
 
     double* out = dst + (tile0 + tileLocal) * (int64_t)K * TILE_N + lane;
-    int extreme = 0;
     for (int k = warp; k < K; k += 8) {
         double v = valid ? colp[(int64_t)k * ld] : 0.0;
         v = fmin(v - x, U_CLAMP);
-        if (valid && v < -1.0e5) extreme = 4;   // only possible for unsampled rows (sampled rows are >= 0)
+        row_min_push(urowmin + k, valid ? v : 0.0, lane);
         out[(int64_t)k * TILE_N] = valid ? v : 0.0;
     }
-    if (__any_sync(0xffffffffu, extreme) && lane == 0) atomicOr(&flags[1], 1);
     if (warp == 0) xshift[(tile0 + tileLocal) * TILE_N + lane] = x;
     if (anyBad && threadIdx.x == 0) atomicOr(&flags[0], anyBad);
 }
@@ -255,7 +261,7 @@ int retile_chunk(mbar_b200_ctx* ctx, const double* d_rowmajor, int64_t ldCols, i
     if (nTilesChunk <= 0) return MBAR_B200_OK;
     retile_kernel<<<(unsigned)nTilesChunk, 256, 0, s>>>(d_rowmajor, ldCols, ctx->K, tile0, validCols,
                                                        ctx->d_rowmask, ctx->d_u, ctx->d_xshift,
-                                                       ctx->d_flag);
+                                                       ctx->d_flag, ctx->d_urowmin);
     ctx->launches++;
     MBAR_CUDA(cudaGetLastError());
     return MBAR_B200_OK;
@@ -399,7 +405,7 @@ __global__ void __launch_bounds__(256) synth_kernel(int K, int64_t N, int64_t nO
                                                     const double* __restrict__ cumN,  // [K+1]
                                                     const unsigned long long* __restrict__ rowmask,
                                                     double* __restrict__ dst,
-                                                    double* __restrict__ xshift) {
+                                                    double* __restrict__ xshift, int* __restrict__ urowmin) {
     __shared__ double s_min[8][TILE_N];
     const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
     const int64_t tile = blockIdx.x;
@@ -436,6 +442,7 @@ __global__ void __launch_bounds__(256) synth_kernel(int K, int64_t N, int64_t nO
     for (int k = warp; k < K; k += 8) {
         const double d = x - O_k[k];
         const double v = fmin(0.5 * k_k[k] * d * d - sh, U_CLAMP);
+        row_min_push(urowmin + k, valid ? v : 0.0, lane);
         out[(int64_t)k * TILE_N] = valid ? v : 0.0;
     }
     if (warp == 0) xshift[nl] = sh;
@@ -459,7 +466,7 @@ int launch_synth(mbar_b200_ctx* ctx, const mbar_b200_synth* spec) {
                               ctx->stream));
     synth_kernel<<<(unsigned)ctx->nTiles, 256, 0, ctx->stream>>>(
         K, ctx->N, spec->n_offset, spec->seed, d, d + K, d + 2 * K, ctx->d_rowmask, ctx->d_u,
-        ctx->d_xshift);
+        ctx->d_xshift, ctx->d_urowmin);
     ctx->launches++;
     MBAR_CUDA(cudaGetLastError());
     MBAR_CUDA(cudaStreamSynchronize(ctx->stream));
@@ -629,6 +636,8 @@ int mbar_b200_create(mbar_b200_ctx** out, int device, int32_t K, int64_t N_local
     ALLOC(c->d_out, (size_t)lay.size(true) * sizeof(double));
     ALLOC(c->d_ticket, 4 * sizeof(unsigned int));
     ALLOC(c->d_flag, 4 * sizeof(int));
+    ALLOC(c->d_urowmin, (size_t)K * sizeof(int));
+    c->h_urowmin.assign(K, 0.0);
     ALLOC(c->d_f, 8 * (size_t)K * sizeof(double));
     ALLOC(c->d_scratch, ((size_t)K * K + 4 * (size_t)K + 1024) * sizeof(double));
     ALLOC(c->d_loop, sizeof(mbar::LoopState));
@@ -679,6 +688,7 @@ int mbar_b200_create(mbar_b200_ctx** out, int device, int32_t K, int64_t N_local
     CREATE_CUDA(cudaMemset(c->d_onesmask, 0xff, mask.size() * sizeof(unsigned long long)));
     CREATE_CUDA(cudaMemset(c->d_ticket, 0, 4 * sizeof(unsigned int)));
     CREATE_CUDA(cudaMemset(c->d_flag, 0, 4 * sizeof(int)));
+    CREATE_CUDA(cudaMemset(c->d_urowmin, 0, (size_t)K * sizeof(int)));
 #undef CREATE_CUDA
     *out = c;
     return MBAR_B200_OK;
@@ -711,7 +721,7 @@ int mbar_b200_destroy(mbar_b200_ctx* c) {
     }
     cudaFree(c->d_xshift); cudaFree(c->d_wgt); cudaFree(c->d_sqrtw); cudaFree(c->d_c); cudaFree(c->d_Nk); cudaFree(c->d_NkEff);
     cudaFree(c->d_rowmask); cudaFree(c->d_zeromask); cudaFree(c->d_onesmask); cudaFree(c->d_partial); cudaFree(c->d_out); cudaFree(c->d_L);
-    cudaFree(c->d_W); cudaFree(c->d_ticket); cudaFree(c->d_flag); cudaFree(c->d_f);
+    cudaFree(c->d_W); cudaFree(c->d_ticket); cudaFree(c->d_flag); cudaFree(c->d_urowmin); cudaFree(c->d_f);
     cudaFree(c->d_scratch);
     cudaFree(c->d_loop); cudaFree(c->d_av); cudaFree(c->d_outM); cudaFree(c->d_A); cudaFree(c->d_active);
     cudaFree(c->d_seq); cudaFree(c->d_Wt);
@@ -825,13 +835,21 @@ static int ensure_staging(mbar_b200_ctx* c, bool needPinned) {
     return MBAR_B200_OK;
 }
 
+// Row minima of the shifted energies written by the last upload: to the host, agreed over the shards (the upload is
+// collective once a communicator is attached), device accumulators reset for the next upload.
+static int collect_row_minima(mbar_b200_ctx* c) {
+    std::vector<int> m(c->K);
+    MBAR_CUDA(cudaMemcpy(m.data(), c->d_urowmin, (size_t)c->K * sizeof(int), cudaMemcpyDeviceToHost));
+    MBAR_CUDA(cudaMemset(c->d_urowmin, 0, (size_t)c->K * sizeof(int)));
+    for (int k = 0; k < c->K; ++k) c->h_urowmin[k] = (double)m[k];
+    return agree_row_minima(c);
+}
+
 static int finish_upload(mbar_b200_ctx* c) {
     int flags[4];
     MBAR_CUDA(cudaStreamSynchronize(c->copyStream));
     MBAR_CUDA(cudaStreamSynchronize(c->stream));
     MBAR_CUDA(cudaMemcpy(flags, c->d_flag, sizeof(flags), cudaMemcpyDeviceToHost));
-    c->unsampledExtreme = flags[1] != 0;
-    if (flags[1]) MBAR_CUDA(cudaMemset(c->d_flag + 1, 0, sizeof(int)));
     if (flags[0]) {
         MBAR_CUDA(cudaMemset(c->d_flag, 0, 4 * sizeof(int)));
         c->ready = false;
@@ -840,6 +858,7 @@ static int finish_upload(mbar_b200_ctx* c) {
         return MBAR_B200_ERR_NAN;
     }
     MBAR_TRY(reduce_sumx(c));
+    MBAR_TRY(collect_row_minima(c));
     c->ready = true;
     return MBAR_B200_OK;
 }
@@ -931,23 +950,23 @@ __global__ void __launch_bounds__(256) widen_tiles_kernel(const double* __restri
 __global__ void __launch_bounds__(256) append_rows_kernel(const double* __restrict__ stage, int64_t ldCols, int E,
                                                           int K, int Knew, int64_t tile0, int64_t validCols,
                                                           const double* __restrict__ xshift,
-                                                          double* __restrict__ dst, int* __restrict__ flags) {
+                                                          double* __restrict__ dst, int* __restrict__ flags,
+                                                          int* __restrict__ urowmin) {
     const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
     const int64_t tl = blockIdx.x;
     const int64_t col = tl * TILE_N + lane;
     const bool valid = col < validCols;
     const double x = xshift[(tile0 + tl) * TILE_N + lane];
     double* out = dst + (tile0 + tl) * (int64_t)Knew * TILE_N + (int64_t)K * TILE_N + lane;
-    int bad = 0, extreme = 0;
+    int bad = 0;
     for (int r = warp; r < E; r += 8) {
         double v = valid ? stage[(int64_t)r * ldCols + col] : 0.0;
         if (v != v) bad = 1;
         v = fmin(v - x, U_CLAMP);
-        if (valid && v < -1.0e5) extreme = 1;
+        row_min_push(urowmin + K + r, valid ? v : 0.0, lane);
         out[(int64_t)r * TILE_N] = valid ? v : 0.0;
     }
     if (__any_sync(0xffffffffu, bad) && lane == 0) atomicOr(&flags[0], 1);
-    if (__any_sync(0xffffffffu, extreme) && lane == 0) atomicOr(&flags[1], 1);
 }
 
 int mbar_b200_create_augmented(mbar_b200_ctx* base, int32_t n_extra, const double* u_extra_host, int64_t ld,
@@ -1032,7 +1051,7 @@ int mbar_b200_create_augmented(mbar_b200_ctx* base, int32_t n_extra, const doubl
         c->h2dBytes += (int64_t)w * E * 8;
         const int64_t nT = (w + TILE_N - 1) / TILE_N;
         append_rows_kernel<<<(unsigned)nT, 256, 0, c->stream>>>(d_stage, cols, E, K, Kn, n0 / TILE_N, w,
-                                                              c->d_xshift, c->d_u, c->d_flag);
+                                                              c->d_xshift, c->d_u, c->d_flag, c->d_urowmin);
         c->launches++;
         if (pinned) cudaStreamSynchronize(c->stream);   // one device staging block: consume before refilling
     }
@@ -1047,7 +1066,13 @@ int mbar_b200_create_augmented(mbar_b200_ctx* base, int32_t n_extra, const doubl
         set_error("appended energies contain NaN");
         return fail(MBAR_B200_ERR_NAN);
     }
-    c->unsampledExtreme = base->unsampledExtreme || flags[1] != 0;
+    {
+        std::vector<int> m(E);
+        AUG_CUDA(cudaMemcpy(m.data(), c->d_urowmin + K, (size_t)E * sizeof(int), cudaMemcpyDeviceToHost));
+        AUG_CUDA(cudaMemset(c->d_urowmin, 0, (size_t)Kn * sizeof(int)));
+        for (int k = 0; k < K; ++k) c->h_urowmin[k] = base->h_urowmin[k];
+        for (int r = 0; r < E; ++r) c->h_urowmin[K + r] = (double)m[r];
+    }
     if (base->d_wgt) {
         // bootstrap multiplicities travel with the samples
         AUG_CUDA(cudaMalloc((void**)&c->d_wgt, nPad * sizeof(double)));
@@ -1076,6 +1101,7 @@ int mbar_b200_synthesize(mbar_b200_ctx* c, const mbar_b200_synth* spec) {
     MBAR_CUDA(cudaSetDevice(c->device));
     MBAR_TRY(launch_synth(c, spec));
     MBAR_TRY(reduce_sumx(c));
+    MBAR_TRY(collect_row_minima(c));
     c->ready = true;
     return MBAR_B200_OK;
 }

@@ -21,6 +21,15 @@ constexpr int MAX_GRID = 132 * 4;
 // Unsampled states ride through the fused kernel as "sampled with weight e^-80": their share of any
 // denominator is below 2^-53 as long as their sum of weights stays below 1e12 (checked by the host).
 constexpr double LOG_EPS_UNSAMPLED = -80.0;
+// The device exp (exp_split + scale2) is accurate for arguments in [-707.7, 709.7].  Below, the result is floored
+// into [0, 2^-1020] instead of underflowing; above ~709.78 the binary exponent wraps, so the host never lets an
+// argument above FUSED_MAX_ARG reach the fused pass (unsampled rows below the sampled minimum: fused_applicable).
+// Sampled rows have u' >= 0 and spread(c) < 1200, so their arguments stay below 600.
+constexpr double FUSED_MAX_ARG = 700.0;
+// A floored entry enters S_k's raw sum sum_n e_kn / D_n divided by D_n >= e^(c_min - mid), c_min over the SAMPLED
+// states (every sample has one with u' = 0): the fused pass treats a raw sum below 2^53 * N * 2^-1020 * e^(mid - c_min)
+// as underflowed (S_k = NaN) and the host redoes the pass in the log domain.  log(2^53 * 2^-1020) = -967 ln 2:
+constexpr double LOG_FLOOR_S = -670.273323601467;
 
 void set_error(const char* fmt, ...);
 #define MBAR_CUDA(call)                                                                     \
@@ -100,7 +109,10 @@ struct mbar_b200_ctx {
     std::vector<double> h_logNk;    // [K], -inf for unsampled
     std::vector<double> h_logNkEff; // [K], LOG_EPS_UNSAMPLED for unsampled
     double* d_NkEff = nullptr;      // [K], exp(LOG_EPS_UNSAMPLED) for unsampled
-    bool unsampledExtreme = false;  // an unsampled state lies > 1e5 kT below every sampled one somewhere
+    // [K] min over samples of each row's shifted energy u'_kn, rounded down, 0 when none is negative (only
+    // unsampled rows can be): bounds the exp argument an unsampled row presents to the fused pass
+    std::vector<double> h_urowmin;
+    int* d_urowmin = nullptr;       // [K] the same, accumulated on the device during upload / append
     std::vector<int> active;        // indices of sampled states
     int firstActive = 0;
     double N_total_states = 0;      // sum_k N_k (global N)
@@ -189,6 +201,7 @@ struct FusedParams {
     double mid2;
     int M;                                 // candidates evaluated per launch (1 or 2)
     const unsigned long long* rowmask;
+    const unsigned long long* sampledmask;  // sampled states (the rows that bound D_n from below)
     const double* Nk;
     double* partial;                       // [grid][K + 2]
     double* out;
@@ -204,6 +217,7 @@ struct FusedParams {
     int epi, first;
     int64_t N, nTiles, nStages;
     double mid;
+    double logFloorN;                      // LOG_FLOOR_S + log N (global sample count): underflow test of S_k
     int K, Wk, Wn, Rw, TPW, NS, CW, batch, debugSkip, mode, CL, Kh, allStates;
     uint32_t tileBytes, stageBytes;
 };
@@ -273,8 +287,11 @@ int launch_logw(mbar_b200_ctx* ctx, const double* h_f, double* logW_host, int64_
 int launch_synth(mbar_b200_ctx* ctx, const mbar_b200_synth* spec);
 int launch_untile(mbar_b200_ctx* ctx, int64_t n0, int64_t n, double* d_dst, int64_t ld);
 int comm_allreduce(mbar_b200_ctx* ctx, double* d_buf, int count, int op /*0 sum, 2 max*/);
+// h_urowmin made identical on every rank (collective; a no-op without a communicator)
+int agree_row_minima(mbar_b200_ctx* ctx);
 int reduce_sumx(mbar_b200_ctx* ctx);
 int set_weights(mbar_b200_ctx* ctx, const double* w_host);
+int probe_exp_launch(int which, int64_t n, const double* d_a, double* d_out);   // mbar_b200_probe_exp
 
 // ---- device helpers ----
 #ifdef __CUDACC__
@@ -342,7 +359,9 @@ constexpr double EXP_MAGIC = 6755399441055744.0;  // 1.5 * 2^52
 
 // exp(a) with the binary exponent kept apart:  exp(a) = v * 2^q,  v in [1, 2).
 // a in [-5e7, 5e7]; `tab` = 32-entry table of 2^(j/32) in shared memory (conflict-free: 256 B).
-// 9 fp64 pipe ops (FMA t, ADD nf, FMA r, 4 FMA Horner, MUL, FMA) + integer work on the ALU pipe.
+// 9 fp64 pipe ops (FMA t, ADD nf, FMA r, 4 FMA Horner, MUL, FMA) + integer work on the ALU pipe.  The reduction
+// subtracts n ln2/32 as ONE double (MBAR_EXP_LN2N_LO is not applied): the result is exp(a (1 + 3.35e-17)), up to
+// 108 ulp off at |a| = 708 but 1.5 ulp from that (DESIGN.md 3.1: the second FMA would cost the fused pass time).
 __device__ __forceinline__ void exp_split(double a, const double* __restrict__ tab, double& v, int& q) {
     const double t = fma(a, MBAR_EXP_SCALE, EXP_MAGIC);
     const int n = __double2loint(t);
@@ -357,8 +376,9 @@ __device__ __forceinline__ void exp_split(double a, const double* __restrict__ t
     v = fma(T, p, T);
     q = n >> 5;
 }
-// v * 2^q with q clamped to the normal range from below (result >= ~2^-1021, never denormal) and
-// assumed < 1023 from above.
+// v * 2^q with q clamped to the normal range from below (result in [2^-1021, 2^-1020), never denormal: callers
+// must treat sums that such entries could dominate as underflowed, see LOG_FLOOR_S) and assumed <= 1023 from
+// above (arguments <= 709.7, see FUSED_MAX_ARG).
 __device__ __forceinline__ double scale2(double v, int q) {
     q = max(q, -1021);
     const int hi = __double2hiint(v) + (q << 20);

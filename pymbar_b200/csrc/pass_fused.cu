@@ -121,7 +121,7 @@ __device__ __forceinline__ void exp_batch(const double (&cu)[B], const double (&
         for (int i = 0; i < B; ++i) pl[i] = fma(pl[i], r[i], -MBAR_EXP_C1);
     } else {
 #pragma unroll
-        for (int i = 0; i < B; ++i) r[i] = fma(t[i] - EXP_MAGIC, -MBAR_EXP_LN2N, r[i]);
+        for (int i = 0; i < B; ++i) r[i] = fma(t[i] - EXP_MAGIC, -MBAR_EXP_LN2N, r[i]);   // (see exp_split)
 #pragma unroll
         for (int i = 0; i < B; ++i) pl[i] = fma(MBAR_EXP_C5, r[i], MBAR_EXP_C4);
 #pragma unroll
@@ -556,6 +556,29 @@ __global__ void __launch_bounds__(CW * 32, 1) pass_fused_kernel(const FusedParam
     double* tot = reinterpret_cast<double*>(stages);     // [M][K + 2] (the ring is idle now)
     constexpr int TW = M;
     const int totN = TW * (K + 2);
+    // Entries whose exp argument lay below the normal range were floored at up to 2^-1020 (scale2), and
+    // D_n >= exp(c_min - mid) amplifies each by at most exp(mid - c_min), c_min over the sampled states (each
+    // sample has a sampled state with u' = 0; unsampled rows only add to D_n): a raw sum sum_n e_kn / D_n below
+    // 2^53 * N times that bound could be made of floored entries.  Such an S_k is poisoned (NaN) and every
+    // consumer treats it as underflowed (log-domain redo).  (In S_k = E_k * sum / N_k the bound carries the
+    // same factor E_k / N_k as S_k itself, so one threshold, floorSum, serves all states.)
+    __shared__ double s_cmin[2][32];
+    {
+        double m1 = INFINITY, m2 = INFINITY;
+        for (int k = threadIdx.x; k < K; k += blockDim.x)
+            if ((p.sampledmask[k >> 6] >> (k & 63)) & 1ull) {
+                m1 = fmin(m1, p.c[k]);
+                if constexpr (M == 2) m2 = fmin(m2, p.c2[k]);
+            }
+        for (int o = 16; o > 0; o >>= 1) {
+            m1 = fmin(m1, __shfl_xor_sync(0xffffffffu, m1, o));
+            m2 = fmin(m2, __shfl_xor_sync(0xffffffffu, m2, o));
+        }
+        if (lane == 0) {
+            s_cmin[0][warp] = m1;
+            s_cmin[1][warp] = m2;
+        }
+    }
     for (int k = threadIdx.x; k < totN; k += blockDim.x) {
         double t = 0.0;
         for (unsigned b = 0; b < nGroups; ++b) t += p.partial[(size_t)b * totN + k];
@@ -564,6 +587,13 @@ __global__ void __launch_bounds__(CW * 32, 1) pass_fused_kernel(const FusedParam
         tot[k] = t;
     }
     __syncthreads();
+    double floorSum[2] = {INFINITY, INFINITY};
+    for (int w2 = 0; w2 < (int)(blockDim.x >> 5); ++w2) {
+        floorSum[0] = fmin(floorSum[0], s_cmin[0][w2]);
+        floorSum[1] = fmin(floorSum[1], s_cmin[1][w2]);
+    }
+    floorSum[0] = exp(p.logFloorN - floorSum[0]);
+    if (M == 2) floorSum[1] = exp(p.logFloorN - floorSum[1]);
     if (p.peer.nranks > 1) {
         // One-shot all-gather of the K+2 partial sums through peer memory (NVLink stores into every
         // rank's inbox, then a release flag), followed by a sum in RANK ORDER so that every GPU
@@ -621,8 +651,10 @@ __global__ void __launch_bounds__(CW * 32, 1) pass_fused_kernel(const FusedParam
     for (int k = threadIdx.x; k < K; k += blockDim.x) {
         const bool act = (p.rowmask[k >> 6] >> (k & 63)) & 1ull;
         double t = tot[k];
+        // (floor-aware underflow test on the raw sum, see floorSum)
+        const bool under = !(t > floorSum[0]);
         if ((MODE & 2) && act) t *= exp(p.c[k]);      // S_k = E_k * sum_n e0_kn / D_n / N_k
-        t = act ? t / p.Nk[k] : 0.0;
+        t = act ? (under ? NAN : t / p.Nk[k]) : 0.0;
         p.out[lay.S() + k] = t;
         p.out[lay.logS() + k] = 0.0;
         tot[k] = t;
@@ -635,8 +667,9 @@ __global__ void __launch_bounds__(CW * 32, 1) pass_fused_kernel(const FusedParam
         for (int k = threadIdx.x; k < K; k += blockDim.x) {
             const bool act = (p.rowmask[k >> 6] >> (k & 63)) & 1ull;
             double t = tot[K + 2 + k];
+            const bool under = !(t > floorSum[1]);
             if (act) t *= exp(p.c2[k]);
-            p.out2[lay.S() + k] = act ? t / p.Nk[k] : 0.0;
+            p.out2[lay.S() + k] = act ? (under ? NAN : t / p.Nk[k]) : 0.0;
             p.out2[lay.logS() + k] = 0.0;
         }
         if (threadIdx.x == 0) {
@@ -705,10 +738,19 @@ __global__ void __launch_bounds__(CW * 32, 1) pass_fused_kernel(const FusedParam
     }
 }
 
+// kernel mode (see TabRef): bit 0 = LDS-replicated exp table, bit 1 = multiplicative state constant.
+// MBAR_B200_FUSED_MODE overrides the default for experiments.
+static int fused_mode(double spread) {
+    int mode = 3;
+    if (const char* v = std::getenv("MBAR_B200_FUSED_MODE")) mode = std::atoi(v) & 3;
+    mode |= 1;   // the shuffle-gathered table (bit 0 clear) was measured 10 % slower and is retired
+    if (spread > 600.0) mode &= 1;   // exp(c_k) * exp(-u') needs the spread inside the exponent range
+    return mode;
+}
+
 bool fused_applicable(const mbar_b200_ctx* ctx, const double* h_f, bool allStates, double* midOut,
                       double* spreadOut) {
     if (ctx->K > 2048) return false;
-    if (allStates && ctx->unsampledExtreme) return false;
     double lo = INFINITY, hi = -INFINITY;
     for (int k = 0; k < ctx->K; ++k) {
         if (!allStates && !(ctx->h_Nk[k] > 0)) continue;
@@ -719,6 +761,19 @@ bool fused_applicable(const mbar_b200_ctx* ctx, const double* h_f, bool allState
     }
     if (hi - lo >= FUSED_SPREAD) return false;
     if (std::fabs(hi) > C_RANGE || std::fabs(lo) > C_RANGE) return false;
+    if (allStates) {
+        // Sampled rows have u' >= 0, unsampled rows may lie far below the sampled minimum.  An exp argument above
+        // ~709.78 would overflow the binary exponent that scale2 adds to the high word and wrap it into the sign
+        // bit (NaN, negative, or a small positive number that no later check can tell from a right answer): such
+        // all-state passes take the log-domain kernel.
+        const bool mult = fused_mode(hi - lo) & 2;
+        const double mid = 0.5 * (hi + lo);
+        for (int k = 0; k < ctx->K; ++k) {
+            if (ctx->h_Nk[k] > 0) continue;
+            const double arg = (mult ? 0.0 : h_f[k] + ctx->h_logNkEff[k] - mid) - ctx->h_urowmin[k];
+            if (arg > FUSED_MAX_ARG) return false;
+        }
+    }
     if (midOut) *midOut = 0.5 * (hi + lo);
     if (spreadOut) *spreadOut = hi - lo;
     return true;
@@ -738,12 +793,8 @@ int fused_prepare(mbar_b200_ctx* ctx, const double* h_f, bool wantL, bool allSta
     const int K = ctx->K;
     FusedParams p{};
     p.K = K;
-    // kernel mode (see TabRef): bit 0 = LDS-replicated exp table, bit 1 = multiplicative state constant.
-    // MBAR_B200_FUSED_MODE overrides the default for experiments.
-    int mode = 3;
-    if (const char* v = std::getenv("MBAR_B200_FUSED_MODE")) mode = std::atoi(v) & 3;
-    mode |= 1;   // the shuffle-gathered table (bit 0 clear) was measured 10 % slower and is retired
-    if (spread > 600.0) mode &= 1;   // exp(c_k) * exp(-u') needs the spread inside the exponent range
+    const int mode = fused_mode(spread);
+    p.logFloorN = LOG_FLOOR_S + std::log(ctx->N_total_states);
     p.allStates = allStates ? 1 : 0;
     p.M = M;
     // two candidates per launch: second accumulator set -> at most 16 states per thread, hence K <= 1024, and the
@@ -802,6 +853,7 @@ int fused_prepare(mbar_b200_ctx* ctx, const double* h_f, bool wantL, bool allSta
     p.c = d_cdst;
     // allStates: unsampled rows take part with weight e^-80 (see LOG_EPS_UNSAMPLED)
     p.rowmask = allStates ? ctx->d_onesmask : ctx->d_rowmask;
+    p.sampledmask = ctx->d_rowmask;
     p.Nk = allStates ? ctx->d_NkEff : ctx->d_Nk;
     p.partial = ctx->d_partial;
     p.out = ctx->d_out;
@@ -915,6 +967,48 @@ int launch_pass_fused(mbar_b200_ctx* ctx, const double* h_f, bool wantL, bool al
     if (!*usedOut) return MBAR_B200_OK;
     if (wroteW) *wroteW = p.Wout != nullptr;
     return fused_enqueue(ctx, p);
+}
+
+// Development probe (mbar_b200_probe_exp): exp(a[i]) through exactly the device code the passes run.
+// which = 0: exp_fast; 1: the fused exp_batch body with the constant in the exponent (MODE=1, c = a, u' = 0);
+// 2: its multiplicative form (MODE=3, e0 = exp(-u') with u' = -a).  One warp per 256 arguments, 8 per lane.
+__global__ void __launch_bounds__(32) probe_exp_kernel(int which, int64_t n, const double* __restrict__ a,
+                                                       double* __restrict__ out) {
+    __shared__ double tab[MBAR_EXP_NT];
+    __shared__ double rep[2 * 32 * 32];    // holds the lane-replicated table 8 KB aligned, as in the pass
+    const int lane = threadIdx.x;
+    tab[lane] = MBAR_EXP_TABLE[lane];
+    const uint32_t tabRep = (smem_u32(rep) + 8191u) & ~8191u;
+    for (int i = lane; i < 32 * 32; i += 32)
+        asm volatile("st.shared.f64 [%0], %1;" ::"r"(tabRep + i * 8), "d"(MBAR_EXP_TABLE[i >> 5]));
+    __syncwarp();
+    TabRef tr;
+    tr.hi = __double2hiint(MBAR_EXP_TABLE[lane]);
+    tr.lo = __double2loint(MBAR_EXP_TABLE[lane]);
+    tr.laneBase = tabRep + lane * 8;
+    const int64_t base = (int64_t)blockIdx.x * 256;
+    double cu[8], uu[8], e[8], cn[8], un[8], Dp = 0.0;
+#pragma unroll
+    for (int i = 0; i < 8; ++i) {
+        const int64_t j = base + i * 32 + lane;
+        const double x = j < n ? a[j] : 0.0;
+        cu[i] = which == 1 ? x : 0.0;
+        uu[i] = which == 1 ? 0.0 : -x;
+        e[i] = which == 0 ? exp_fast(x, tab) : 0.0;
+    }
+    if (which == 1) exp_batch<8, 8, 0, false, 1, false>(cu, uu, tr, e, Dp, nullptr, nullptr, cn, un, 0u);
+    if (which == 2) exp_batch<8, 8, 0, false, 3, false>(cu, uu, tr, e, Dp, nullptr, nullptr, cn, un, 0u);
+#pragma unroll
+    for (int i = 0; i < 8; ++i) {
+        const int64_t j = base + i * 32 + lane;
+        if (j < n) out[j] = e[i];
+    }
+}
+
+int probe_exp_launch(int which, int64_t n, const double* d_a, double* d_out) {
+    probe_exp_kernel<<<(unsigned)((n + 255) / 256), 32>>>(which, n, d_a, d_out);
+    MBAR_CUDA(cudaGetLastError());
+    return MBAR_B200_OK;
 }
 
 }  // namespace mbar

@@ -84,3 +84,32 @@ extern "C" int mbar_b200_measure_fp64_peak(int device, double* dmma_tflops, doub
     if (dfma_tflops) *dfma_tflops = best[1];
     return MBAR_B200_OK;
 }
+
+extern "C" int mbar_b200_probe_exp(int device, int which, int64_t n, const double* a_host, double* out_host) {
+    MBAR_REQUIRE(a_host && out_host && n >= 0, MBAR_B200_ERR_INVALID, "bad argument");
+    MBAR_REQUIRE(which >= 0 && which <= 2, MBAR_B200_ERR_INVALID, "which=%d: 0, 1 or 2", which);
+    int ndev = 0;
+    if (cudaGetDeviceCount(&ndev) != cudaSuccess || device < 0 || device >= ndev) {
+        cudaGetLastError();
+        set_error("no CUDA device %d", device);
+        return MBAR_B200_ERR_NO_DEVICE;
+    }
+    if (n == 0) return MBAR_B200_OK;
+    MBAR_CUDA(cudaSetDevice(device));
+    double* d = nullptr;
+    MBAR_CUDA(cudaMalloc((void**)&d, 2 * (size_t)n * sizeof(double)));
+    int rc = MBAR_B200_OK;
+    if (cudaMemcpy(d, a_host, (size_t)n * sizeof(double), cudaMemcpyHostToDevice) != cudaSuccess) {
+        set_error("probe_exp: H2D copy failed");
+        rc = MBAR_B200_ERR_CUDA;
+    }
+    if (rc == MBAR_B200_OK) rc = probe_exp_launch(which, n, d, d + n);
+    if (rc == MBAR_B200_OK &&
+        cudaMemcpy(out_host, d + n, (size_t)n * sizeof(double), cudaMemcpyDeviceToHost) != cudaSuccess) {
+        set_error("probe_exp: D2H copy failed");
+        rc = MBAR_B200_ERR_CUDA;
+    }
+    cudaFree(d);
+    cudaGetLastError();
+    return rc;
+}

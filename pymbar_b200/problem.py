@@ -351,6 +351,15 @@ def measure_fp64_peak(device=0):
     return a.value, b.value
 
 
+def probe_exp(a, which=0, device=0):
+    """exp(a) through the device's own exp (mbar_b200_probe_exp): which = 0 exp_fast, 1 the fused pass with the
+    constant in the exponent (MODE=1), 2 the fused pass's multiplicative form (MODE=3).  Development aid."""
+    a = np.ascontiguousarray(a, dtype=np.float64).ravel()
+    out = np.empty_like(a)
+    check(_lib.load().mbar_b200_probe_exp(int(device), int(which), a.size, _dptr(a), _dptr(out)))
+    return out
+
+
 def gpu_numa_node(device=0):
     """NUMA node of the GPU's PCI function (-1: the host exposes none)."""
     n = C.c_int(-1)
