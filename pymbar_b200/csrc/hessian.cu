@@ -23,7 +23,8 @@
 //             Diagonal pairs run their 6 full + 4 triangular 32 x 32 sub-blocks on 10 warps placed so that
 //             the four schedulers carry 32/32/36/36 DMMA per k-step (off-diagonal pairs: 64).
 //   fallback  hessian_inplace_kernel (round 1: in-place conversion) when the 8*K*N weight buffer cannot be
-//             allocated.
+//             allocated (on an 80 GB part: once u_kn and the weights, 16*K*N bytes, no longer fit, e.g. K = 512,
+//             N = 1.25e7), for every K.
 // Per-CTA partial blocks are reduced by a second kernel in CTA order (deterministic).
 #include <cmath>
 #include <cstdlib>
@@ -66,7 +67,8 @@ __global__ void __launch_bounds__(512, 1)
 hessian_inplace_kernel(const double* __restrict__ u, const double* __restrict__ Lp,
                const double* __restrict__ c, const unsigned long long* __restrict__ rowmask, int K,
                int64_t N, int64_t nTiles, const HessSplit split, double* __restrict__ Gpart,
-               const double* __restrict__ sqrtw) {
+               const double* __restrict__ sqrtw, const LoopState* loop) {
+    if (loop && *reinterpret_cast<const volatile int*>(&loop->done)) return;
     extern __shared__ __align__(128) unsigned char smem_raw[];
     double* tab = reinterpret_cast<double*>(smem_raw);                      // [32]
     uint64_t* bar_full = reinterpret_cast<uint64_t*>(tab + 32);             // [HNS]
@@ -224,7 +226,9 @@ hessian_inplace_kernel(const double* __restrict__ u, const double* __restrict__ 
 // Sum the partial blocks of each pair over its CTAs (in order: deterministic) and scatter to the full
 // symmetric K x K matrix.  Diagonal pairs only hold sub-blocks with row-block >= column-block.
 __global__ void __launch_bounds__(256)
-hessian_reduce_kernel(const double* __restrict__ Gpart, int K, const HessSplit split, double* __restrict__ G) {
+hessian_reduce_kernel(const double* __restrict__ Gpart, int K, const HessSplit split, double* __restrict__ G,
+                      const LoopState* loop) {
+    if (loop && *reinterpret_cast<const volatile int*>(&loop->done)) return;
     const int pair = blockIdx.x;
     int bi = 0, rem = pair + split.pairBase;
     while (rem > bi) { rem -= bi + 1; ++bi; }
@@ -736,9 +740,10 @@ int launch_hessian_dev(mbar_b200_ctx* ctx, const double* d_ch, bool allRows, Loo
                 attr[ctx->device & 15][1] = true;
             }
             hessian_inplace_kernel<<<nCtas, 512, smem, ctx->stream>>>(ctx->d_u, ctx->d_L, d_ch, mask, K, ctx->N,
-                                                                     ctx->nTiles, split, ctx->d_W, ctx->d_sqrtw);
+                                                                     ctx->nTiles, split, ctx->d_W, ctx->d_sqrtw, loop);
             MBAR_CUDA(cudaGetLastError());
-            hessian_reduce_kernel<<<dim3(nPairs, 16), 256, 0, ctx->stream>>>(ctx->d_W, K, split, ctx->d_out + lay.G());
+            hessian_reduce_kernel<<<dim3(nPairs, 16), 256, 0, ctx->stream>>>(ctx->d_W, K, split, ctx->d_out + lay.G(),
+                                                                            loop);
             MBAR_CUDA(cudaGetLastError());
         }
         ctx->launches += 2;
