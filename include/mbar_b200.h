@@ -174,6 +174,21 @@ int mbar_b200_log_W_nk_rows(mbar_b200_ctx* ctx, const double* f_k, int64_t n0, i
 int mbar_b200_weight_moments(mbar_b200_ctx* ctx, const double* f_k, double* S_out, double* G_out);
 /* Per-sample log denominators L_n [N_local] (the logsumexp at mbar_solvers.py:238). */
 int mbar_b200_log_denominator(mbar_b200_ctx* ctx, const double* f_k, double* L_host);
+/* Histogram FES of one target state (pymbar fes.py:388-600 and :1382-1415).  u_n [N_local] is the target
+ * state's reduced potential for every sample (+inf allowed = weight 0, NaN -> MBAR_B200_ERR_NAN); bin_n
+ * [N_local] is a dense bin index in [0, nbins) (anything else -> MBAR_B200_ERR_INVALID).  With
+ * multiplicities c_n (mbar_b200_set_sample_weights, default 1):
+ *   f_bin[nbins]  f_i  = -log sum_{n in i} c_n exp(-u_n - L_n)                          (required)
+ *   C[K*nbins]    C_ki = sum_{n in i} c_n W_nk w^_n,  w^_n = exp(-u_n - L_n + f_i)      (row-major, may be NULL)
+ *   D[nbins]      D_i  = sum_{n in i} c_n w^_n^2                                         (may be NULL)
+ * W_nk covers ALL K states, sampled or not, as Log_W_nk does.  Together with mbar_b200_weight_moments this is
+ * W_aug^T W_aug of the augmented matrix W_aug = [W | B], B_ni = w^_n [bin(n) = i], without materialising it.
+ * Range: at the converged f_k every W_nk <= 1 and w^_n <= 1 / c_n.  An exponent of W_nk or w^_n above 700 (f_k
+ * far from the solution), or a bin with no sample of finite weight (empty, all u_n = +inf or all c_n = 0),
+ * returns MBAR_B200_ERR_RANGE.  Two calls on the same inputs return bit-identical results.  Sharded contexts
+ * (communicator attached) are not supported: MBAR_B200_ERR_INVALID. */
+int mbar_b200_bin_moments(mbar_b200_ctx* ctx, const double* f_k, const double* u_n, const int32_t* bin_n,
+                          int32_t nbins, double* f_bin, double* C, double* D);
 
 /* ---- native solver loops (no Python between iterations) ------------------------------------- */
 /* Plain self-consistent iteration f <- f - log S(f), gauge f[first sampled] = 0 each step, until
@@ -209,6 +224,9 @@ int mbar_b200_last_loop_ms(mbar_b200_ctx* ctx, double* total_ms, double* kernel_
 int mbar_b200_last_kernels(const mbar_b200_ctx* ctx, char* pass_kernel, char* hessian_kernel, int32_t len);
 /* CUDA-event durations of the last Hessian evaluation: weight materialisation and DMMA kernel + reduction. */
 int mbar_b200_last_hessian_ms(mbar_b200_ctx* ctx, double* weights_ms, double* hessian_ms);
+/* CUDA-event duration of the kernels of the last mbar_b200_bin_moments after its pass (bin sums, C and D), and
+ * the number of bin chunks (reads of u_kn) its C / D step took (0 when C and D were not requested). */
+int mbar_b200_last_bin_stats(mbar_b200_ctx* ctx, double* ms, int32_t* chunks);
 /* fp64 ceilings of this GPU measured in place (register-only DMMA.8x8x4 and DFMA loops), in TFLOP/s: the
  * roofline denominator of mbar_b200_hessian (MEASURED_PEAKS.json has no fp64 figure). */
 int mbar_b200_measure_fp64_peak(int device, double* dmma_tflops, double* dfma_tflops);

@@ -70,6 +70,13 @@ def install(target=None, patch_layout_helpers=True, patch_mbar=True):
         from . import facade
 
         facade.install_on(mbar_mod.MBAR)
+        # histogram free-energy surfaces from the same resident problem (pymbar.FES, when importable)
+        try:
+            import pymbar.fes as fes_mod
+        except ImportError:
+            fes_mod = None
+        if fes_mod is not None and hasattr(fes_mod, "FES"):
+            facade.install_fes_on(fes_mod.FES)
     return target
 
 

@@ -69,6 +69,7 @@ SIGNATURES = {
     "mbar_b200_log_W_nk": (C.c_int, [_ctx, _dp, C.c_void_p, C.c_int64, C.c_int]),
     "mbar_b200_log_W_nk_rows": (C.c_int, [_ctx, _dp, C.c_int64, C.c_int64, C.c_void_p, C.c_int64, C.c_int]),
     "mbar_b200_log_denominator": (C.c_int, [_ctx, _dp, _dp]),
+    "mbar_b200_bin_moments": (C.c_int, [_ctx, _dp, _dp, C.POINTER(C.c_int32), C.c_int32, _dp, _dp, _dp]),
     "mbar_b200_solve_sci": (C.c_int, [_ctx, _dp, C.c_double, C.c_int32, C.POINTER(SolveResult)]),
     "mbar_b200_solve_adaptive": (C.c_int, [_ctx, _dp, C.c_double, C.c_int32, C.c_int32, C.c_double,
                                            C.POINTER(SolveResult)]),
@@ -77,6 +78,7 @@ SIGNATURES = {
     "mbar_b200_get_graph_stats": (C.c_int, [_ctx, C.POINTER(C.c_int64), C.POINTER(C.c_int64)]),
     "mbar_b200_last_kernels": (C.c_int, [_ctx, C.c_char_p, C.c_char_p, C.c_int32]),
     "mbar_b200_last_hessian_ms": (C.c_int, [_ctx, _dp, _dp]),
+    "mbar_b200_last_bin_stats": (C.c_int, [_ctx, _dp, C.POINTER(C.c_int32)]),
     "mbar_b200_measure_fp64_peak": (C.c_int, [C.c_int, _dp, _dp]),
     "mbar_b200_probe_exp": (C.c_int, [C.c_int, C.c_int, C.c_int64, _dp, _dp]),
     "mbar_b200_sci_iterate": (C.c_int, [_ctx, _dp, C.c_int32]),

@@ -181,6 +181,8 @@ struct mbar_b200_ctx {
     char lastKernel[200] = "";           // description of the pass-kernel variant launched last
     char lastHessKernel[200] = "";       // ... and of the Hessian kernel path
     double lastHessMs = 0.0, lastWeightsMs = 0.0;
+    double lastBinMs = 0.0;              // mbar_b200_bin_moments: kernels after the pass (CUDA events)
+    int lastBinChunks = 0;               // ... and the reads of u_kn its moments step took
     cudaEvent_t evH0 = nullptr, evH1 = nullptr, evH2 = nullptr;
 
     // counters

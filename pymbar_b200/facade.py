@@ -18,12 +18,22 @@ the CPU.  With the facade installed:
 * `_initialize_with_bar` (:1936-1988, `MBAR(initialize="BAR")`) uses `pymbar_b200.initialize` (samples grouped by
   state once, Brent on Bennett's equation).
 
+* `_computeUnnormalizedLogWeights` (:1919-1934) is -u_n - L_n with L_n from the device's log denominators.
+
 Anything outside what the device path implements (bootstrap uncertainties, `uncertainty_method="svd"`) calls
 the original method, which then reads `self.Log_W_nk` and materialises it.  `uninstall()` restores the class.
+
+`install_fes_on` does the same for `pymbar.FES` (fes.py): `generate_fes` without bootstraps takes its log weights
+from the device and, for fes_type="histogram", builds the bin free energies with `pymbar_b200.fes.histogram_fes`;
+`FES.w_kn` (np.exp(mbar.Log_W_nk), fes.py:416) becomes lazy like `Log_W_nk`.  `_get_fes_histogram` with
+`uncertainty_method="analytical"` takes Theta from `pymbar_b200.fes.histogram_theta` (K x nbins moments on the
+device) instead of the N x (K + nbins) augmented weight matrix (fes.py:1382-1406).  FES bootstraps, KDE / spline
+uncertainties, and any call whose weights leave the device's range contract go to the original methods.
 """
 from __future__ import annotations
 
 import threading
+from timeit import default_timer as _timer
 
 import numpy as np
 
@@ -31,7 +41,8 @@ from . import estimators as est
 
 _TLS = threading.local()
 _SAVED = {}
-STATS = {"tickets": 0, "redeemed": 0, "moments": 0, "expectations": 0}
+STATS = {"tickets": 0, "redeemed": 0, "moments": 0, "expectations": 0, "log_weights": 0, "fes_histograms": 0,
+         "fes_theta": 0, "fes_w_kn": 0}
 
 
 class LogWeightTicket:
@@ -68,6 +79,17 @@ def _moments(mbar):
     return S, G
 
 
+def _device_log_weights(mbar, u_n):
+    """-u_n - L_n: the unnormalised log weights of the target state u_n (mbar.py:1919-1934)."""
+    from . import mbar_solvers as ms
+
+    STATS["log_weights"] += 1
+    u_n = np.asarray(u_n, dtype=np.float64)
+    with ms._borrow(mbar.u_kn, np.asarray(mbar.N_k, dtype=np.float64)) as p:
+        L = p.log_denominator(np.asarray(mbar.f_k, dtype=np.float64))
+    return -u_n - L
+
+
 def _check_normalised(S, tolerance=1.0e-4):
     # utils.check_w_normalized (utils.py:340-388): column sums of W must be 1
     from . import utils as u
@@ -84,7 +106,8 @@ def install_on(MBAR):
         return
     saved = {name: MBAR.__dict__.get(name) for name in
              ("__init__", "Log_W_nk", "compute_effective_sample_number", "compute_overlap",
-              "compute_free_energy_differences", "compute_expectations_inner", "_initialize_with_bar")}
+              "compute_free_energy_differences", "compute_expectations_inner", "_initialize_with_bar",
+              "_computeUnnormalizedLogWeights")}
     _SAVED[MBAR] = saved
     orig_init = saved["__init__"]
     orig_fed = saved["compute_free_energy_differences"]
@@ -163,6 +186,10 @@ def install_on(MBAR):
 
         return init.initialize_with_bar(u_kn, self.N_k, self.x_kindices, f_k_init)
 
+    def _computeUnnormalizedLogWeights(self, u_n):
+        return _device_log_weights(self, u_n)
+
+    MBAR._computeUnnormalizedLogWeights = _computeUnnormalizedLogWeights
     MBAR._initialize_with_bar = _initialize_with_bar
     MBAR.__init__ = __init__
     MBAR.Log_W_nk = property(_get_logw, _set_logw, doc="log weights [N, K] (mbar.py:455), downloaded on first use")
@@ -170,6 +197,132 @@ def install_on(MBAR):
     MBAR.compute_overlap = compute_overlap
     MBAR.compute_free_energy_differences = compute_free_energy_differences
     MBAR.compute_expectations_inner = compute_expectations_inner
+
+
+class WeightMatrixTicket:
+    """Stands for FES.w_kn = np.exp(mbar.Log_W_nk) (fes.py:416) until somebody reads it."""
+
+    __slots__ = ("mbar",)
+
+    def __init__(self, mbar):
+        self.mbar = mbar
+
+    def redeem(self):
+        STATS["fes_w_kn"] += 1
+        return np.exp(self.mbar.Log_W_nk)
+
+
+def _out_of_range(err):
+    from . import _lib
+
+    return isinstance(err, _lib.MbarB200Error) and err.status == -6     # MBAR_B200_ERR_RANGE
+
+
+def install_fes_on(FES):
+    """Patch the class object `FES` (pymbar.fes.FES)."""
+    if FES in _SAVED:
+        return
+    saved = {name: FES.__dict__.get(name) for name in ("generate_fes", "_get_fes_histogram", "w_kn")}
+    _SAVED[FES] = saved
+    orig_generate = saved["generate_fes"]
+    orig_get_hist = saved["_get_fes_histogram"]
+
+    def generate_fes(self, u_n, x_n, fes_type="histogram", histogram_parameters=None, kde_parameters=None,
+                     spline_parameters=None, n_bootstraps=0, seed=-1):
+        args = (u_n, x_n, fes_type, histogram_parameters, kde_parameters, spline_parameters, n_bootstraps, seed)
+        single = isinstance(n_bootstraps, (int, np.integer)) and not isinstance(n_bootstraps, bool) and n_bootstraps == 0
+        if not single or fes_type not in ("histogram", "kde", "spline"):
+            return orig_generate(self, *args)
+        from . import fes as hist
+        from . import mbar_solvers as ms
+        from .utils import kn_to_n
+
+        # fes.py:335-438 for the one, non-bootstrap, sample set
+        result_vals = {}
+        self.fes_type = fes_type
+        if len(np.shape(u_n)) == 2:
+            u_n = kn_to_n(u_n, N_k=self.N_k)
+        self.u_n = u_n
+        if seed >= 0:
+            np.random.seed(seed)
+        self.n_bootstraps = n_bootstraps
+        timings = getattr(self, "timings", False)
+        start = _timer() if timings else None
+        self.fes_function = list()
+        self.mc_data = None
+        if fes_type == "histogram":
+            self._setup_fes_histogram(histogram_parameters)
+        elif fes_type == "kde":
+            self._setup_fes_kde(kde_parameters)
+        else:
+            self._setup_fes_spline(spline_parameters)
+        mbar = self.mbar
+        f_k = np.asarray(mbar.f_k, dtype=np.float64)
+        u = np.asarray(u_n, dtype=np.float64)
+        try:
+            log_w = _device_log_weights(mbar, u)
+            if fes_type == "histogram":
+                with ms._borrow(mbar.u_kn, np.asarray(mbar.N_k, dtype=np.float64)) as p:
+                    data = hist.histogram_fes(p, f_k, u, x_n, self.histogram_parameters["bin_edges"])
+                STATS["fes_histograms"] += 1
+        except Exception as err:
+            if _out_of_range(err):
+                return orig_generate(self, *args)
+            raise
+        w_n = np.exp(log_w - np.max(log_w))
+        self.w_n = w_n / np.sum(w_n)
+        self.w_kn = WeightMatrixTicket(mbar)
+        if fes_type == "histogram":
+            self.histogram_data = data
+        elif fes_type == "kde":
+            self._generate_fes_kde(0, x_n, self.w_n)
+        else:
+            self._generate_fes_spline(0, x_n, self.w_n)
+        if timings:
+            result_vals["timing"] = _timer() - start
+        return result_vals
+
+    def _get_fes_histogram(self, x, reference_point="from-lowest", fes_reference=None, uncertainty_method=None):
+        if uncertainty_method not in (None, "analytical") or reference_point not in ("from-lowest", "from-specified"):
+            return orig_get_hist(self, x, reference_point=reference_point, fes_reference=fes_reference,
+                                 uncertainty_method=uncertainty_method)
+        from . import fes as hist
+        from . import mbar_solvers as ms
+
+        mbar = self.mbar
+        K = mbar.K
+
+        def df_fn(j):
+            STATS["fes_theta"] += 1
+            with ms._borrow(mbar.u_kn, np.asarray(mbar.N_k, dtype=np.float64)) as p:
+                Theta, S, _ = hist.histogram_theta(p, np.asarray(mbar.f_k, dtype=np.float64), mbar.N_k,
+                                                   np.asarray(self.u_n, dtype=np.float64), self.histogram_data,
+                                                   return_moments=True)
+            _check_normalised(S)
+            return hist.bin_uncertainties(Theta, K, j, len(self.histogram_data["f"]))
+
+        try:
+            return hist.query(self.histogram_data, x, reference_point, fes_reference,
+                              df_fn if uncertainty_method == "analytical" else None)
+        except Exception as err:
+            if _out_of_range(err):
+                return orig_get_hist(self, x, reference_point=reference_point, fes_reference=fes_reference,
+                                     uncertainty_method=uncertainty_method)
+            raise
+
+    def _get_w_kn(self):
+        v = self.__dict__.get("_b200_w_kn")
+        if isinstance(v, WeightMatrixTicket):
+            v = v.redeem()
+            self.__dict__["_b200_w_kn"] = v
+        return v
+
+    def _set_w_kn(self, value):
+        self.__dict__["_b200_w_kn"] = value
+
+    FES.generate_fes = generate_fes
+    FES._get_fes_histogram = _get_fes_histogram
+    FES.w_kn = property(_get_w_kn, _set_w_kn, doc="weights [N, K] of all states (fes.py:416), computed on first use")
 
 
 def uninstall_from(MBAR):

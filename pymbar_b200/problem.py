@@ -296,6 +296,31 @@ class DeviceProblem:
         check(self._lib.mbar_b200_log_denominator(self._h, _dptr(f), _dptr(out)))
         return out
 
+    def bin_moments(self, f_k, u_n, bin_n, nbins, want_C=True):
+        """Histogram FES of the target state `u_n` [N] over the dense bin index `bin_n` [N] in [0, nbins):
+        (f_bin [nbins], C [K, nbins], D [nbins]) with f_i = -log sum_{n in i} exp(-u_n - L_n),
+        C_ki = sum_{n in i} W_nk w^_n, D_i = sum_{n in i} w^_n^2 and w^_n = exp(-u_n - L_n + f_i)
+        (mbar_b200_bin_moments).  want_C=False skips the moments: (f_bin, None, None)."""
+        f = _f64(f_k, self.K)
+        u = _f64(u_n)
+        b = np.ascontiguousarray(bin_n, dtype=np.int32)
+        nbins = int(nbins)
+        if u.shape != (self.N,) or b.shape != (self.N,):
+            raise ValueError(f"u_n and bin_n must have shape ({self.N},), got {u.shape} and {b.shape}")
+        f_bin = np.empty(nbins)
+        C_ = np.empty((self.K, nbins)) if want_C else None
+        D = np.empty(nbins) if want_C else None
+        check(self._lib.mbar_b200_bin_moments(self._h, _dptr(f), _dptr(u), b.ctypes.data_as(C.POINTER(C.c_int32)),
+                                              nbins, _dptr(f_bin), _dptr(C_) if want_C else None,
+                                              _dptr(D) if want_C else None))
+        return f_bin, C_, D
+
+    def last_bin_stats(self):
+        """CUDA-event time of the last bin_moments' kernels after its pass, and its reads of u_kn for C / D."""
+        ms, chunks = C.c_double(0), C.c_int32(0)
+        check(self._lib.mbar_b200_last_bin_stats(self._h, C.byref(ms), C.byref(chunks)))
+        return dict(ms=ms.value, chunks=chunks.value)
+
     # ---- native loops ---------------------------------------------------------------------------
     @staticmethod
     def _result(r):
