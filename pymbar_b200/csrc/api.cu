@@ -1,4 +1,5 @@
-// C ABI: the streaming pass, the reference primitives built on it, native solver loops, NCCL glue.
+// C ABI: the streaming pass (run_pass, pass_multi), the reference primitives built on it, the communicator.
+// The solver loops and their entry points are in loops.cu.
 #include <dlfcn.h>
 #include <nccl.h>
 
@@ -82,41 +83,6 @@ __global__ void logs_to_scaled(double* logS, const double* mx, double* scaled, i
 __global__ void scaled_to_logs(double* logS, const double* mx, const double* scaled, int K) {
     const int k = blockIdx.x * blockDim.x + threadIdx.x;
     if (k < K) logS[k] = (mx[k] > -INFINITY && mx[k] < INFINITY) ? mx[k] + log(scaled[k]) : mx[k];
-}
-
-// Device epilogue of a self-consistent iteration kept entirely on the GPU:
-//   f <- f - log S (sampled states), gauge f[first sampled] = 0, c <- f + log N - mid.
-__global__ void sci_epilogue_kernel(const double* __restrict__ out, double* __restrict__ f,
-                                    double* __restrict__ c, const double* __restrict__ Nk, int K,
-                                    int first, double mid, double* __restrict__ delta) {
-    __shared__ double s_f0;
-    __shared__ double s_max[32];
-    if (threadIdx.x == 0) s_f0 = f[first] - log(out[first]);
-    __syncthreads();
-    double md = 0.0;
-    for (int k = threadIdx.x; k < K; k += blockDim.x) {
-        if (Nk[k] > 0.0) {
-            const double fo = f[k];
-            // an underflowed S_k (linear-domain sums) poisons the result so the host redoes the
-            // iteration with the log-domain path
-            const double fn = (out[k] > 1e-280) ? fo - log(out[k]) - s_f0 : NAN;
-            f[k] = fn;
-            c[k] = fn + log(Nk[k]) - mid;
-            if (k != first) {
-                double div = fabs(fn);
-                if (div < 1e-8) div = 1.0;
-                md = fmax(md, fabs(fn - fo) / div);
-            }
-        }
-    }
-    for (int o = 16; o > 0; o >>= 1) md = fmax(md, __shfl_xor_sync(0xffffffffu, md, o));
-    if ((threadIdx.x & 31) == 0) s_max[threadIdx.x >> 5] = md;
-    __syncthreads();
-    if (threadIdx.x == 0) {
-        double m = 0.0;
-        for (int w = 0; w < (int)(blockDim.x >> 5); ++w) m = fmax(m, s_max[w]);
-        delta[0] = m;
-    }
 }
 
 }  // namespace mbar
@@ -236,41 +202,6 @@ double global_sumx(mbar_b200_ctx* c, int* rc) {
 
 }  // namespace mbar
 
-// ------------------------------------------------------------------------------------------
-// small dense helpers for the Newton step (host-stepped fallback loop, K x K)
-// ------------------------------------------------------------------------------------------
-// In-place Cholesky of the n x n SPD matrix A (row-major, lower); returns false if not PD.
-static bool cholesky(std::vector<double>& A, int n) {
-    for (int j = 0; j < n; ++j) {
-        double d = A[(size_t)j * n + j];
-        for (int k = 0; k < j; ++k) d -= A[(size_t)j * n + k] * A[(size_t)j * n + k];
-        if (!(d > 0.0) || !std::isfinite(d)) return false;
-        d = std::sqrt(d);
-        A[(size_t)j * n + j] = d;
-        const double inv = 1.0 / d;
-        for (int i = j + 1; i < n; ++i) {
-            double s = A[(size_t)i * n + j];
-            const double* ai = &A[(size_t)i * n];
-            const double* aj = &A[(size_t)j * n];
-            for (int k = 0; k < j; ++k) s -= ai[k] * aj[k];
-            A[(size_t)i * n + j] = s * inv;
-        }
-    }
-    return true;
-}
-static void chol_solve(const std::vector<double>& Lc, int n, std::vector<double>& b) {
-    for (int i = 0; i < n; ++i) {
-        double s = b[i];
-        for (int k = 0; k < i; ++k) s -= Lc[(size_t)i * n + k] * b[k];
-        b[i] = s / Lc[(size_t)i * n + i];
-    }
-    for (int i = n - 1; i >= 0; --i) {
-        double s = b[i];
-        for (int k = i + 1; k < n; ++k) s -= Lc[(size_t)k * n + i] * b[k];
-        b[i] = s / Lc[(size_t)i * n + i];
-    }
-}
-
 extern "C" {
 
 int mbar_b200_pass(mbar_b200_ctx* c, const double* f, double* S, double* sumL, double* G) {
@@ -320,10 +251,9 @@ int mbar_b200_pass_multi(mbar_b200_ctx* c, int32_t M, const double* f, double* S
     if (fast && M == 2 && !noM2) {
         // one launch for both candidates (pass_fused_kernel<..., M = 2>): one read of u_kn, one exp per entry
         bool ok0 = false, ok1 = false;
-        MBAR_TRY(fused_prepare(c, f, false, false, &p[0], &ok0, c->d_c, c->h_f, false, 2));
+        MBAR_TRY(fused_prepare(c, f, false, false, &p[0], &ok0, c->dc(ROW_C), c->hf(ROW_C), false, 2));
         if (ok0)
-            MBAR_TRY(fused_prepare(c, f + K, false, false, &p[1], &ok1, c->d_av + 4 * (size_t)K, c->h_f + 6 * (size_t)K,
-                                   false, 2));
+            MBAR_TRY(fused_prepare(c, f + K, false, false, &p[1], &ok1, c->dc(ROW_C2), c->hf(ROW_C2), false, 2));
         if (ok0 && ok1) {
             p[0].c2 = p[1].c;
             p[0].mid2 = p[1].mid;
@@ -335,8 +265,8 @@ int mbar_b200_pass_multi(mbar_b200_ctx* c, int32_t M, const double* f, double* S
     for (int m = 0; m < M && fast && !batched; ++m) {
         bool ok = false;
         // candidate m stages its constants in its own device row / pinned row (the copies are asynchronous)
-        MBAR_TRY(fused_prepare(c, f + (size_t)m * K, false, false, &p[m], &ok,
-                               m == 0 ? c->d_c : c->d_av + 4 * (size_t)K, m == 0 ? c->h_f : c->h_f + 6 * (size_t)K));
+        const int row = m == 0 ? ROW_C : ROW_C2;
+        MBAR_TRY(fused_prepare(c, f + (size_t)m * K, false, false, &p[m], &ok, c->dc(row), c->hf(row)));
         p[m].out = c->d_outM + (size_t)m * lay.size(false);
         fast = ok;
     }
@@ -395,21 +325,6 @@ int mbar_b200_last_hessian_ms(mbar_b200_ctx* c, double* weights_ms, double* hess
     if (cudaEventElapsedTime(&b, c->evH1, c->evH2) != cudaSuccess) { cudaGetLastError(); b = 0.f; }
     if (weights_ms) *weights_ms = a;
     if (hessian_ms) *hessian_ms = b;
-    return MBAR_B200_OK;
-}
-
-int mbar_b200_get_loop_stats(const mbar_b200_ctx* c, int64_t* polls, int32_t* mode, int32_t* batch) {
-    MBAR_REQUIRE(c, MBAR_B200_ERR_INVALID, "ctx is NULL");
-    if (polls) *polls = c->loopPolls;
-    if (mode) *mode = c->loopMode;
-    if (batch) *batch = c->loopBatch;
-    return MBAR_B200_OK;
-}
-
-int mbar_b200_get_graph_stats(const mbar_b200_ctx* c, int64_t* captures, int64_t* launches) {
-    MBAR_REQUIRE(c, MBAR_B200_ERR_INVALID, "ctx is NULL");
-    if (captures) *captures = c->graphCaptures;
-    if (launches) *launches = c->graphLaunches;
     return MBAR_B200_OK;
 }
 
@@ -517,359 +432,6 @@ int mbar_b200_log_denominator(mbar_b200_ctx* c, const double* f, double* L_host)
     MBAR_CUDA(cudaStreamSynchronize(c->stream));
     c->d2hBytes += 2 * c->N * 8;
     for (int64_t n = 0; n < c->N; ++n) L_host[n] -= x[n];
-    return MBAR_B200_OK;
-}
-
-// ------------------------------------------------------------------------------------------
-// native solver loops
-// ------------------------------------------------------------------------------------------
-static double rel_delta(const mbar_b200_ctx* c, const std::vector<double>& fn, const std::vector<double>& fo,
-                        double tol) {
-    // mbar_solvers.py:627-631 on the sampled states other than the gauge state
-    double md = 0.0;
-    const double thr = std::min(1e-8, tol);
-    for (size_t i = 1; i < c->active.size(); ++i) {
-        const int k = c->active[i];
-        double div = std::fabs(fn[k]);
-        if (div < thr) div = 1.0;
-        const double d = std::fabs(fn[k] - fo[k]) / div;
-        if (std::isnan(d)) return NAN;
-        md = std::max(md, d);
-    }
-    return md;
-}
-
-}  // extern "C"
-
-namespace mbar {
-// Host-stepped loops (round 1): one host round trip per pass.  They are the robust fallback of the
-// device-resident loops in loops.cu (generic kernel, log-domain sums, ridge retries) and stay selectable with
-// mbar_b200_set_loop_mode(ctx, 1).
-int solve_sci_stepped(mbar_b200_ctx* c, double* f, double tol, int32_t maxiter, mbar_b200_solve_result* res) {
-    MBAR_REQUIRE(c && f, MBAR_B200_ERR_INVALID, "NULL argument");
-    const int K = c->K;
-    const PassLayout lay{K};
-    std::vector<double> cur(f, f + K), nxt(K);
-    mbar_b200_solve_result r{};
-    cudaEvent_t e0, e1;
-    cudaEventCreate(&e0); cudaEventCreate(&e1);
-    cudaEventRecord(e0, c->stream);
-    const int g0 = c->firstActive;
-    for (int k : c->active) cur[k] -= f[g0];
-    int rc = MBAR_B200_OK;
-    for (int it = 0; it < maxiter; ++it) {
-        rc = run_pass(c, cur.data(), PassWant{});
-        if (rc != MBAR_B200_OK) break;
-        r.passes++;
-        nxt = cur;
-        for (int k : c->active) nxt[k] = cur[k] - c->h_out[lay.logS() + k];
-        const double shift = nxt[g0];
-        for (int k : c->active) nxt[k] -= shift;
-        r.max_delta = rel_delta(c, nxt, cur, tol);
-        cur.swap(nxt);
-        r.iterations = it + 1;
-        r.sci_iterations = it + 1;
-        if (std::isnan(r.max_delta) || r.max_delta < tol) {
-            r.success = 1;
-            break;
-        }
-    }
-    if (rc == MBAR_B200_OK) {
-        rc = run_pass(c, cur.data(), PassWant{});
-        r.passes++;
-        double gn = 0.0;
-        for (int k : c->active) {
-            const double g = c->h_Nk[k] * (c->h_out[k] - 1.0);
-            gn += g * g;
-        }
-        r.gnorm = std::sqrt(gn);
-    }
-    cudaEventRecord(e1, c->stream);
-    cudaEventSynchronize(e1);
-    float ms = 0.f;
-    cudaEventElapsedTime(&ms, e0, e1);
-    r.device_ms = ms;
-    cudaEventDestroy(e0); cudaEventDestroy(e1);
-    if (rc == MBAR_B200_OK) std::memcpy(f, cur.data(), K * sizeof(double));
-    if (res) *res = r;
-    return rc;
-}
-
-int solve_adaptive_stepped(mbar_b200_ctx* c, double* f, double tol, int32_t maxiter, int32_t min_sc_iter,
-                           double gamma, mbar_b200_solve_result* res) {
-    MBAR_REQUIRE(c && f, MBAR_B200_ERR_INVALID, "NULL argument");
-    const int K = c->K;
-    const PassLayout lay{K};
-    const int na = (int)c->active.size();
-    const int g0 = c->firstActive;
-    std::vector<double> cur(f, f + K), f_sci(K), f_nr(K), g(K, 0.0), g_sci(K), g_nr(K);
-    std::vector<double> A, rhs;
-    mbar_b200_solve_result r{};
-    cudaEvent_t e0, e1;
-    cudaEventCreate(&e0); cudaEventCreate(&e1);
-    cudaEventRecord(e0, c->stream);
-    {
-        const double s0 = cur[g0];
-        for (int k : c->active) cur[k] -= s0;
-    }
-    int rc = MBAR_B200_OK;
-    auto grad_from_out = [&](std::vector<double>& out) {
-        double gn = 0.0;
-        for (int k = 0; k < K; ++k) {
-            out[k] = c->h_Nk[k] > 0 ? c->h_Nk[k] * (c->h_out[k] - 1.0) : 0.0;
-            gn += out[k] * out[k];
-        }
-        return gn;
-    };
-    for (int it = 0; it < maxiter && rc == MBAR_B200_OK; ++it) {
-        // pass at f with the second moments: gives g, H and the self-consistent candidate at once
-        PassWant w;
-        w.G = true;
-        rc = run_pass(c, cur.data(), w);
-        if (rc != MBAR_B200_OK) break;
-        r.passes++;
-        r.hessian_passes++;
-        grad_from_out(g);
-        f_sci = cur;
-        for (int k : c->active) f_sci[k] = cur[k] - c->h_out[lay.logS() + k];
-        {
-            const double s0 = f_sci[g0];
-            for (int k : c->active) f_sci[k] -= s0;
-        }
-        // Newton step in the reduced coordinates (gauge state dropped): H[1:,1:] x = g[1:]
-        // (mbar_solvers.py:581-584 uses the min-norm lstsq of the singular full H minus its first
-        // component — the same step in exact arithmetic, SURVEY.md Appendix A).
-        bool haveNr = false;
-        if (na > 1) {
-            const int n = na - 1;
-            const double* Gh = c->h_out + lay.G();
-            double ridge = 0.0, ridgeRel = 0.0, tr = 0.0;
-            for (int a = 1; a < na; ++a) {
-                const int i = c->active[a];
-                tr += c->h_Nk[i] * c->h_out[i];
-            }
-            for (int attempt = 0; attempt < 4 && !haveNr; ++attempt) {
-                A.assign((size_t)n * n, 0.0);
-                for (int a = 1; a < na; ++a) {
-                    const int i = c->active[a];
-                    for (int b = 1; b <= a; ++b) {
-                        const int j = c->active[b];
-                        double v = -Gh[(size_t)i * K + j];
-                        if (i == j) v += c->h_Nk[i] * c->h_out[i] + ridge;
-                        A[(size_t)(a - 1) * n + (b - 1)] = v;
-                    }
-                }
-                if (cholesky(A, n)) {
-                    rhs.resize(n);
-                    for (int a = 1; a < na; ++a) rhs[a - 1] = g[c->active[a]];
-                    chol_solve(A, n, rhs);
-                    f_nr = cur;
-                    for (int a = 1; a < na; ++a) f_nr[c->active[a]] = cur[c->active[a]] - gamma * rhs[a - 1];
-                    haveNr = true;
-                    for (int a = 1; a < na; ++a)
-                        if (!std::isfinite(f_nr[c->active[a]]) || std::fabs(f_nr[c->active[a]]) > 0.5 * C_RANGE)
-                            haveNr = false;
-                } else {
-                    ridgeRel = (ridgeRel == 0.0) ? 1e-12 : ridgeRel * 1e3;   // relative to the mean diagonal
-                    ridge = ridgeRel * (tr / n + 1e-300);
-                }
-            }
-        }
-        rc = run_pass(c, f_sci.data(), PassWant{});
-        if (rc != MBAR_B200_OK) break;
-        r.passes++;
-        const double gn_sci = grad_from_out(g_sci);
-        double gn_nr = INFINITY;
-        if (haveNr) {
-            rc = run_pass(c, f_nr.data(), PassWant{});
-            if (rc != MBAR_B200_OK) break;
-            r.passes++;
-            gn_nr = grad_from_out(g_nr);
-            if (std::isnan(gn_nr)) gn_nr = INFINITY;
-        } else {
-            f_nr = f_sci;
-        }
-        std::vector<double> f_old = cur;
-        if (gn_sci < gn_nr || r.sci_iterations < min_sc_iter) {     // mbar_solvers.py:607
-            cur = f_sci;
-            r.sci_iterations++;
-            r.gnorm = std::sqrt(gn_sci);
-        } else {
-            cur = f_nr;
-            r.nr_iterations++;
-            r.gnorm = std::sqrt(gn_nr);
-        }
-        r.iterations = it + 1;
-        r.max_delta = rel_delta(c, cur, f_old, tol);
-        // max |f_sci - f_nr| / |f|  (mbar_solvers.py:632)
-        double max_diff = 0.0;
-        {
-            const double thr = std::min(1e-8, tol);
-            for (size_t i = 1; i < c->active.size(); ++i) {
-                const int k = c->active[i];
-                double div = std::fabs(cur[k]);
-                if (div < thr) div = 1.0;
-                max_diff = std::max(max_diff, std::fabs(f_sci[k] - f_nr[k]) / div);
-            }
-        }
-        if (std::isnan(r.max_delta) || (r.max_delta < tol && max_diff < std::sqrt(tol))) {
-            r.success = 1;
-            break;
-        }
-    }
-    cudaEventRecord(e1, c->stream);
-    cudaEventSynchronize(e1);
-    float ms = 0.f;
-    cudaEventElapsedTime(&ms, e0, e1);
-    r.device_ms = ms;
-    cudaEventDestroy(e0); cudaEventDestroy(e1);
-    if (rc == MBAR_B200_OK) std::memcpy(f, cur.data(), K * sizeof(double));
-    if (res) *res = r;
-    return rc;
-}
-
-}  // namespace mbar
-
-extern "C" {
-
-int mbar_b200_solve_sci(mbar_b200_ctx* c, double* f, double tol, int32_t maxiter, mbar_b200_solve_result* res) {
-    MBAR_REQUIRE(c && f, MBAR_B200_ERR_INVALID, "NULL argument");
-    NvtxRange nvtx_("mbar_b200::solve_sci");
-    if (c->loopMode == 1) return solve_sci_stepped(c, f, tol, maxiter, res);
-    return solve_sci_device(c, f, tol, maxiter, res);
-}
-
-int mbar_b200_solve_adaptive(mbar_b200_ctx* c, double* f, double tol, int32_t maxiter, int32_t min_sc_iter,
-                             double gamma, mbar_b200_solve_result* res) {
-    MBAR_REQUIRE(c && f, MBAR_B200_ERR_INVALID, "NULL argument");
-    NvtxRange nvtx_("mbar_b200::solve_adaptive");
-    if (c->loopMode == 1) return solve_adaptive_stepped(c, f, tol, maxiter, min_sc_iter, gamma, res);
-    return solve_adaptive_device(c, f, tol, maxiter, min_sc_iter, gamma, res);
-}
-
-int mbar_b200_set_loop_mode(mbar_b200_ctx* c, int32_t mode, int32_t batch) {
-    MBAR_REQUIRE(c, MBAR_B200_ERR_INVALID, "ctx is NULL");
-    MBAR_REQUIRE(mode == 0 || mode == 1, MBAR_B200_ERR_INVALID, "mode=%d (0 device-resident, 1 host-stepped)", mode);
-    c->loopMode = mode;
-    if (batch >= 1) c->loopBatch = batch > 64 ? 64 : batch;
-    return MBAR_B200_OK;
-}
-
-int mbar_b200_sci_iterate(mbar_b200_ctx* c, double* f, int32_t iters) {
-    MBAR_REQUIRE(c && f && iters >= 0, MBAR_B200_ERR_INVALID, "bad argument");
-    MBAR_REQUIRE(c->ready, MBAR_B200_ERR_NOT_READY, "u_kn has not been uploaded");
-    MBAR_CUDA(cudaSetDevice(c->device));
-    MBAR_TRY(check_range(c, f));
-    const int K = c->K;
-    FusedParams p;
-    bool ok = false;
-    if (c->kernelChoice != MBAR_B200_KERNEL_GENERIC) MBAR_TRY(fused_prepare(c, f, false, false, &p, &ok));
-    if (!ok) {
-        // host-stepped fallback with the generic kernel
-        std::vector<double> cur(f, f + K);
-        for (int it = 0; it < iters; ++it) {
-            MBAR_TRY(run_pass(c, cur.data(), PassWant{}));
-            const PassLayout lay2{K};
-            const double s0 = cur[c->firstActive] - c->h_out[lay2.logS() + c->firstActive];
-            for (int k : c->active) cur[k] = cur[k] - c->h_out[lay2.logS() + k] - s0;
-        }
-        std::memcpy(f, cur.data(), K * sizeof(double));
-        return MBAR_B200_OK;
-    }
-    std::memcpy(c->h_f + 4 * K, f, K * sizeof(double));
-    MBAR_CUDA(cudaMemcpyAsync(c->d_f, c->h_f + 4 * K, K * sizeof(double), cudaMemcpyHostToDevice, c->stream));
-    c->h2dBytes += K * 8;
-    const int threads = K >= 256 ? 256 : ((K + 31) / 32) * 32;
-    // per-launch CUDA events of the pass kernel (bench: average launch duration over the loop)
-    std::vector<cudaEvent_t> ev;
-    const bool perLaunch = c->timePasses && iters > 0 && iters <= 4096;
-    if (perLaunch) {
-        ev.resize(2 * (size_t)iters);
-        for (auto& e : ev) MBAR_CUDA(cudaEventCreate(&e));
-    }
-    cudaEvent_t l0, l1;
-    MBAR_CUDA(cudaEventCreate(&l0));
-    MBAR_CUDA(cudaEventCreate(&l1));
-    MBAR_CUDA(cudaEventRecord(l0, c->stream));
-    // One kernel per iteration when the exchange can live inside the pass kernel (single GPU, or peers
-    // attached through mbar_b200_peer_attach); otherwise pass -> ncclAllReduce -> epilogue kernel.
-    const bool inKernel = (c->nranks == 1 || c->peerReady) && !std::getenv("MBAR_B200_NO_FUSED_EPILOGUE");
-    MBAR_REQUIRE(c->nranks == 1 || c->comm, MBAR_B200_ERR_NOT_READY,
-                 "sharded problem (%d ranks) without a communicator: call mbar_b200_comm_init", c->nranks);
-    if (inKernel && c->peerReady) MBAR_TRY(comm_rendezvous(c));
-    NvtxRange nvtx_("mbar_b200::sci_iterate");
-    if (inKernel) {
-        p.epi = 1;
-        p.f = c->d_f;
-        p.cnext = c->d_c;
-        p.first = c->firstActive;
-        if (c->peerReady) p.peer = c->peer;
-    }
-    for (int it = 0; it < iters; ++it) {
-        if (perLaunch) MBAR_CUDA(cudaEventRecord(ev[2 * it], c->stream));
-        MBAR_TRY(fused_enqueue(c, p));
-        if (perLaunch) MBAR_CUDA(cudaEventRecord(ev[2 * it + 1], c->stream));
-        if (!inKernel) {
-            MBAR_TRY(comm_allreduce(c, c->d_out, K + 2, 0));
-            sci_epilogue_kernel<<<1, threads, 0, c->stream>>>(c->d_out, c->d_f, c->d_c, c->d_Nk, K,
-                                                             c->firstActive, p.mid, c->d_scratch);
-            c->launches++;
-        }
-    }
-    MBAR_CUDA(cudaEventRecord(l1, c->stream));
-    MBAR_CUDA(cudaEventSynchronize(l1));
-    {
-        float ms = 0.f;
-        cudaEventElapsedTime(&ms, l0, l1);
-        c->lastLoopMs = ms;
-        double ksum = 0.0;
-        for (int it = 0; perLaunch && it < iters; ++it) {
-            float k = 0.f;
-            cudaEventElapsedTime(&k, ev[2 * it], ev[2 * it + 1]);
-            ksum += k;
-        }
-        c->lastLoopKernelMs = ksum;
-        c->lastLoopIters = iters;
-        for (auto& e : ev) cudaEventDestroy(e);
-        cudaEventDestroy(l0);
-        cudaEventDestroy(l1);
-    }
-    MBAR_CUDA(cudaGetLastError());
-    MBAR_CUDA(cudaMemcpyAsync(c->h_f + 4 * K, c->d_f, K * sizeof(double), cudaMemcpyDeviceToHost, c->stream));
-    const PassLayout lay{K};
-    MBAR_CUDA(cudaMemcpyAsync(c->h_out, c->d_out, (size_t)lay.size(false) * sizeof(double),
-                              cudaMemcpyDeviceToHost, c->stream));
-    MBAR_CUDA(cudaStreamSynchronize(c->stream));
-    c->d2hBytes += K * 8 + lay.size(false) * 8;
-    float ms = 0.f;
-    if (cudaEventElapsedTime(&ms, c->evA, c->evB) == cudaSuccess) c->lastPassMs = ms;
-    MBAR_REQUIRE(!(iters > 0 && c->h_out[lay.flag()] >= 1.0e6), MBAR_B200_ERR_COMM,
-                 "peer exchange timed out inside the pass kernel (a rank did not arrive)");
-    if (p.debugSkip) return MBAR_B200_OK;   // memory-pipeline probe: the arithmetic was skipped, nothing to return
-    if (iters > 0 && c->h_out[lay.flag()] != 0.0) c->h_f[4 * K + c->firstActive] = NAN;  // force the robust redo
-    bool finite = true;
-    for (int k : c->active) finite = finite && std::isfinite(c->h_f[4 * K + k]);
-    if (!finite) {
-        // some S_k underflowed in the linear-domain fused kernel: redo with the robust stepped path
-        std::vector<double> cur(f, f + K);
-        for (int it = 0; it < iters; ++it) {
-            MBAR_TRY(run_pass(c, cur.data(), PassWant{}));
-            const double s0 = cur[c->firstActive] - c->h_out[lay.logS() + c->firstActive];
-            for (int k : c->active) cur[k] = cur[k] - c->h_out[lay.logS() + k] - s0;
-        }
-        std::memcpy(f, cur.data(), K * sizeof(double));
-        return MBAR_B200_OK;
-    }
-    for (int k = 0; k < K; ++k)
-        if (c->h_Nk[k] > 0) f[k] = c->h_f[4 * K + k];
-    return MBAR_B200_OK;
-}
-
-int mbar_b200_last_loop_ms(mbar_b200_ctx* c, double* total_ms, double* kernel_ms_sum, int32_t* iters) {
-    MBAR_REQUIRE(c, MBAR_B200_ERR_INVALID, "ctx is NULL");
-    if (total_ms) *total_ms = c->lastLoopMs;
-    if (kernel_ms_sum) *kernel_ms_sum = c->lastLoopKernelMs;
-    if (iters) *iters = c->lastLoopIters;
     return MBAR_B200_OK;
 }
 

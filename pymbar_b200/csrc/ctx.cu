@@ -626,7 +626,7 @@ int mbar_b200_create(mbar_b200_ctx** out, int device, int32_t K, int64_t N_local
     }
     if (!c->d_u) ALLOC(c->d_u, uBytes);
     ALLOC(c->d_xshift, nPad * sizeof(double));
-    ALLOC(c->d_c, 4 * (size_t)K * sizeof(double));
+    ALLOC(c->d_c, DC_ROWS * (size_t)K * sizeof(double));
     ALLOC(c->d_Nk, (size_t)K * sizeof(double));
     ALLOC(c->d_NkEff, (size_t)K * sizeof(double));
     ALLOC(c->d_rowmask, mask.size() * sizeof(unsigned long long));
@@ -638,8 +638,8 @@ int mbar_b200_create(mbar_b200_ctx** out, int device, int32_t K, int64_t N_local
     ALLOC(c->d_flag, 4 * sizeof(int));
     ALLOC(c->d_urowmin, (size_t)K * sizeof(int));
     c->h_urowmin.assign(K, 0.0);
-    ALLOC(c->d_f, 8 * (size_t)K * sizeof(double));
-    ALLOC(c->d_scratch, ((size_t)K * K + 4 * (size_t)K + 1024) * sizeof(double));
+    ALLOC(c->d_f, (size_t)K * sizeof(double));
+    ALLOC(c->d_scratch, (scratch_rendezvous(K) + 1024) * sizeof(double));
     ALLOC(c->d_loop, sizeof(mbar::LoopState));
     ALLOC(c->d_av, 8 * (size_t)K * sizeof(double));
     ALLOC(c->d_outM, 2 * (size_t)lay.size(false) * sizeof(double));
@@ -669,7 +669,7 @@ int mbar_b200_create(mbar_b200_ctx** out, int device, int32_t K, int64_t N_local
     CREATE_CUDA(cudaHostAlloc((void**)&c->h_out,
                               (size_t)std::max(lay.size(true), 2 * lay.size(false)) * sizeof(double),
                               cudaHostAllocDefault));
-    CREATE_CUDA(cudaHostAlloc((void**)&c->h_f, 8 * (size_t)K * sizeof(double), cudaHostAllocDefault));
+    CREATE_CUDA(cudaHostAlloc((void**)&c->h_f, HF_ROWS * (size_t)K * sizeof(double), cudaHostAllocDefault));
     CREATE_CUDA(cudaStreamCreateWithFlags(&c->stream, cudaStreamNonBlocking));
     CREATE_CUDA(cudaStreamCreateWithFlags(&c->copyStream, cudaStreamNonBlocking));
     CREATE_CUDA(cudaEventCreate(&c->evA));

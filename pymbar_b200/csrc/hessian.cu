@@ -763,11 +763,12 @@ int launch_hessian_dev(mbar_b200_ctx* ctx, const double* d_ch, bool allRows, Loo
 int launch_hessian(mbar_b200_ctx* ctx, const double* h_f, bool allRows, bool weightsReady) {
     const int K = ctx->K;
     // sampled rows carry N_k W_nk (c = f + log N); with allRows the unsampled rows carry W_nk (c = f)
+    double* c = ctx->hf(ROW_HESS_C);
     for (int k = 0; k < K; ++k)
-        ctx->h_f[2 * K + k] = std::isinf(ctx->h_logNk[k]) ? (allRows ? h_f[k] : 0.0) : h_f[k] + ctx->h_logNk[k];
-    MBAR_CUDA(cudaMemcpyAsync(ctx->d_c + 2 * K, ctx->h_f + 2 * K, (size_t)K * sizeof(double),
-                              cudaMemcpyHostToDevice, ctx->stream));
-    return launch_hessian_dev(ctx, ctx->d_c + 2 * K, allRows, nullptr, weightsReady);
+        c[k] = std::isinf(ctx->h_logNk[k]) ? (allRows ? h_f[k] : 0.0) : h_f[k] + ctx->h_logNk[k];
+    MBAR_CUDA(cudaMemcpyAsync(ctx->dc(ROW_HESS_C), c, (size_t)K * sizeof(double), cudaMemcpyHostToDevice,
+                              ctx->stream));
+    return launch_hessian_dev(ctx, ctx->dc(ROW_HESS_C), allRows, nullptr, weightsReady);
 }
 
 }  // namespace mbar

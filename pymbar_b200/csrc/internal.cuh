@@ -94,6 +94,11 @@ struct LoopState {
     double gn_sci, gn_nr;
 };
 
+// Rows of the staging buffers d_c ([DC_ROWS][K]) and h_f ([HF_ROWS][K], pinned; its row r stages d_c's row r, and is not
+// rewritten while a copy out of it is in flight): c of the fused or generic pass, f of the generic pass, c of the Hessian,
+// f of log W, c of a second candidate; pinned only: f to and from d_f, f of each LoopState poll.
+enum { ROW_C, ROW_GEN_F, ROW_HESS_C, ROW_LOGW_F, ROW_C2, DC_ROWS, ROW_F = DC_ROWS, ROW_POLL, HF_ROWS };
+
 }  // namespace mbar
 
 struct mbar_b200_ctx {
@@ -125,7 +130,7 @@ struct mbar_b200_ctx {
     double sumW = 0.0;              // sum_n w_n over valid local samples (= N when unweighted)
     double sumXw = 0.0;             // sum_n w_n x_n
     double sumX = 0.0;              // sum_n x_n over valid local samples
-    double* d_c = nullptr;          // [2][K] c_k = f_k + log N_k - mid (fused) | f_k (row K..2K)
+    double* d_c = nullptr;          // [DC_ROWS][K] pass constants, rows ROW_*
     double* d_Nk = nullptr;         // [K]
     unsigned long long* d_rowmask = nullptr;  // [ceil(K/64)] bit per sampled state
     unsigned long long* d_zeromask = nullptr; // same size, all zero (log-domain for every row)
@@ -137,9 +142,9 @@ struct mbar_b200_ctx {
     double* d_W = nullptr;          // per-CTA partial blocks of the Hessian kernels (gpartBytes)
     unsigned int* d_ticket = nullptr;
     int* d_flag = nullptr;          // [4] error/diagnostic flags
-    double* d_f = nullptr;          // [4][K] device-resident f vectors for native loops
-    double* h_f = nullptr;          // pinned [4][K]
-    double* d_scratch = nullptr;    // misc K*K scratch
+    double* d_f = nullptr;          // [K] device-resident f of the native loops
+    double* h_f = nullptr;          // pinned [HF_ROWS][K] staging, rows ROW_*
+    double* d_scratch = nullptr;    // misc scratch (see scratch_rendezvous)
     cudaStream_t stream = nullptr;
     cudaStream_t copyStream = nullptr;
     cudaEvent_t evA = nullptr, evB = nullptr;
@@ -161,7 +166,7 @@ struct mbar_b200_ctx {
     // device-resident solver loops
     mbar::LoopState* d_loop = nullptr;   // device
     mbar::LoopState* h_loop = nullptr;   // pinned mirror
-    double* d_av = nullptr;              // [8][K] adaptive work vectors (f_sci, f_nr, g, c_sci, c_nr, c_hess, x, -)
+    double* d_av = nullptr;              // [8][K] adaptive work vectors, rows AV_* (loops.cu)
     double* d_outM = nullptr;            // [2][2K+2] pass outputs of the two candidates
     double* d_A = nullptr;               // [K*K] Newton matrix / Cholesky factor
     int* d_active = nullptr;             // [K] indices of the sampled states
@@ -191,6 +196,9 @@ struct mbar_b200_ctx {
     double lastLoopMs = 0.0, lastLoopKernelMs = 0.0;
     int lastLoopIters = 0;
     bool timePasses = true;
+
+    double* dc(int row) const { return d_c + (size_t)row * K; }
+    double* hf(int row) const { return h_f + (size_t)row * K; }
 };
 
 namespace mbar {
@@ -257,20 +265,12 @@ struct NumaPrefer {
 int check_range(mbar_b200_ctx* c, const double* f);
 int run_pass(mbar_b200_ctx* c, const double* f, PassWant want);   // pass + all-reduce + D2H into ctx->h_out
 double global_sumx(mbar_b200_ctx* c, int* rc);
-int solve_sci_stepped(mbar_b200_ctx* c, double* f, double tol, int32_t maxiter, mbar_b200_solve_result* res);
-int solve_adaptive_stepped(mbar_b200_ctx* c, double* f, double tol, int32_t maxiter, int32_t min_sc_iter,
-                           double gamma, mbar_b200_solve_result* res);
-int solve_sci_device(mbar_b200_ctx* c, double* f, double tol, int32_t maxiter, mbar_b200_solve_result* res);
-int solve_adaptive_device(mbar_b200_ctx* c, double* f, double tol, int32_t maxiter, int32_t min_sc_iter,
-                          double gamma, mbar_b200_solve_result* res);
-// stream-ordered rendezvous of all ranks (one tiny all-reduce) before the first in-kernel peer exchange of a loop
-int comm_rendezvous(mbar_b200_ctx* ctx);
 int retile_chunk(mbar_b200_ctx* ctx, const double* d_rowmajor, int64_t ldCols, int64_t tile0,
                  int64_t nTilesChunk, int64_t validCols, cudaStream_t s);
 int launch_pass_generic(mbar_b200_ctx* ctx, const double* h_f, bool wantL, bool logAll);
 int launch_pass_fused(mbar_b200_ctx* ctx, const double* h_f, bool wantL, bool allStates, bool* usedOut,
                       bool wantW = false, bool* wroteW = nullptr);
-// d_cdst / h_stage: where c = f + log N - mid is staged (default: ctx->d_c / ctx->h_f); midForce: reuse the
+// d_cdst / h_stage: where c = f + log N - mid is staged (default: row ROW_C of ctx->d_c / ctx->h_f); midForce: reuse the
 // centring of a previous prepare (candidates evaluated against the same exp(c) range), NaN = derive from f
 int fused_prepare(mbar_b200_ctx* ctx, const double* h_f, bool wantL, bool allStates, FusedParams* out, bool* ok,
                   double* d_cdst = nullptr, double* h_stage = nullptr, bool wantW = false, int M = 1,
@@ -398,5 +398,18 @@ __device__ __forceinline__ double warp_sum(double x) {
     return x;
 }
 #endif
+
+// Relative change |a - b| / |ref| of one entry (mbar_solvers.py:627-632); entries with |ref| below thr = min(1e-8, tol)
+// compare absolutely.  Subtraction, fabs, division and a comparison are correctly rounded on host and device alike,
+// so every solver loop gets the same value.  The reduction and its NaN policy stay with each caller.
+__host__ __device__ __forceinline__ double rel_change(double a, double b, double ref, double thr) {
+    double div = fabs(ref);
+    if (div < thr) div = 1.0;
+    return fabs(a - b) / div;
+}
+
+// d_scratch holds K*K + 4K + 1024 doubles of call-local scratch; the rendezvous all-reduce of the device-resident
+// loops owns the word at this offset
+inline size_t scratch_rendezvous(int K) { return (size_t)K * K + 4 * (size_t)K; }
 
 }  // namespace mbar

@@ -53,8 +53,8 @@ int launch_logw(mbar_b200_ctx* ctx, const double* h_f, double* logW_host, int64_
     MBAR_REQUIRE(n0 >= 0 && n >= 1 && n0 + n <= ctx->N && n0 % TILE_N == 0, MBAR_B200_ERR_INVALID,
                  "log_W rows [%lld, +%lld): n0 must be a multiple of 32 inside [0, N)", (long long)n0, (long long)n);
     NvtxRange nvtx_("mbar_b200::log_W download");
-    for (int k = 0; k < K; ++k) ctx->h_f[3 * K + k] = h_f[k];
-    MBAR_CUDA(cudaMemcpyAsync(ctx->d_c + 3 * K, ctx->h_f + 3 * K, (size_t)K * sizeof(double),
+    std::memcpy(ctx->hf(ROW_LOGW_F), h_f, (size_t)K * sizeof(double));
+    MBAR_CUDA(cudaMemcpyAsync(ctx->dc(ROW_LOGW_F), ctx->hf(ROW_LOGW_F), (size_t)K * sizeof(double),
                               cudaMemcpyHostToDevice, ctx->stream));
     cudaPointerAttributes attr;
     bool pinnedDst = false;
@@ -116,7 +116,7 @@ int launch_logw(mbar_b200_ctx* ctx, const double* h_f, double* logW_host, int64_
         if (!pinnedDst) drain(buf);     // the staging buffer of two chunks ago must be empty again
         // kernel on `stream` must wait until the previous D2H out of this buffer finished
         cudaStreamWaitEvent(ctx->stream, done[buf], 0);
-        logw_kernel<<<(unsigned)nt, 128, 0, ctx->stream>>>(ctx->d_u, ctx->d_L, ctx->d_c + 3 * K, K, ctx->N,
+        logw_kernel<<<(unsigned)nt, 128, 0, ctx->stream>>>(ctx->d_u, ctx->d_L, ctx->dc(ROW_LOGW_F), K, ctx->N,
                                                           tileFirst + t0, d_out[buf], expo);
         ctx->launches++;
         cudaEvent_t ready;

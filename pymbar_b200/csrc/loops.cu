@@ -14,10 +14,16 @@
 // Every kernel starts with `if (loop->done) return;`, so the host enqueues `loopBatch` iterations at a time and
 // reads the 96-byte LoopState once per batch.  Anything the fast path cannot represent (range flag of the fused
 // kernel, an underflowing S_k, non-finite candidates) sets status = 1 and the host finishes on the robust
-// host-stepped loop (api.cu), starting from the last good f.
+// host-stepped loop, starting from the last good f.
+//
+// This file holds every solver loop and its C entry points: the device-resident loops, the host-stepped loops
+// (one run_pass per step; the fallback of the device-resident ones and mbar_b200_set_loop_mode(ctx, 1)), and
+// mbar_b200_sci_iterate.
 #include <nvtx3/nvToolsExt.h>
 
+#include <algorithm>
 #include <cmath>
+#include <cstdlib>
 #include <cstring>
 #include <vector>
 
@@ -73,32 +79,31 @@ __device__ double block_max_nan(double v, double* s_buf) {
 // ------------------------------------------------------------------------------------------------
 // self-consistent iteration, NCCL flavour (no peer memory): epilogue kernel after the all-reduce
 // ------------------------------------------------------------------------------------------------
-// f <- f - log S (sampled states), gauge f[first] = 0, c <- f + log N - mid, convergence test.
+// f <- f - log S (sampled states), gauge f[first] = 0, c <- f + log N - mid, convergence test.  With loop == NULL
+// (as in the fused pass's epilogue) every launch runs and nothing is tested or counted.
 __global__ void __launch_bounds__(256)
 sci_loop_epilogue_kernel(const double* __restrict__ out, double* __restrict__ f, double* __restrict__ c,
                          const double* __restrict__ Nk, const unsigned long long* __restrict__ rowmask, int K,
                          int first, double mid, LoopState* loop) {
-    if (loop_done(loop)) return;
+    if (loop && loop_done(loop)) return;
     __shared__ double s_buf[64];
     __shared__ double s_f0;
     if (threadIdx.x == 0) s_f0 = f[first] - log(out[first]);
     __syncthreads();
-    const double thr = fmin(1.0e-8, loop->tol);
+    const double thr = loop ? fmin(1.0e-8, loop->tol) : 1.0e-8;
     double md = 0.0;
     for (int k = threadIdx.x; k < K; k += blockDim.x) {
         if (row_on(rowmask, k)) {
             const double fo = f[k];
+            // an underflowed S_k poisons the result so the host redoes the step in the log domain
             const double fn = (out[k] > 1e-280) ? fo - log(out[k]) - s_f0 : NAN;
             f[k] = fn;
             c[k] = fn + log(Nk[k]) - mid;
             if (fn != fn) md = NAN;
-            if (k != first && md == md) {
-                double div = fabs(fn);
-                if (div < thr) div = 1.0;
-                md = fmax(md, fabs(fn - fo) / div);
-            }
+            if (k != first && md == md) md = fmax(md, rel_change(fn, fo, fn, thr));
         }
     }
+    if (!loop) return;
     md = block_max_nan(md, s_buf);
     if (threadIdx.x == 0) {
         const int it = loop->iterations + 1;
@@ -334,9 +339,7 @@ adapt_post_kernel(const double* __restrict__ outS, const double* __restrict__ ou
     for (int k = threadIdx.x; k < K; k += blockDim.x)
         if (row_on(rowmask, k) && k != first) {
             const double v = fnew[k];
-            double div = fabs(v);
-            if (div < thr) div = 1.0;
-            const double d1 = fabs(v - f[k]) / div, d2 = fabs(fsci[k] - fnr[k]) / div;
+            const double d1 = rel_change(v, f[k], v, thr), d2 = rel_change(fsci[k], fnr[k], v, thr);
             if (d1 != d1 || md != md) md = NAN; else md = fmax(md, d1);
             if (d2 == d2) mx = fmax(mx, d2);
         }
@@ -374,10 +377,48 @@ adapt_post_kernel(const double* __restrict__ outS, const double* __restrict__ ou
 // ------------------------------------------------------------------------------------------------
 // host side
 // ------------------------------------------------------------------------------------------------
-int comm_rendezvous(mbar_b200_ctx* c) {
+// CUDA events, destroyed with the object on every return path.  As the timer of a solve: start() creates two and
+// records the first on the stream, stop() records the second, waits for it and returns the elapsed ms.
+struct Events {
+    std::vector<cudaEvent_t> ev;
+    cudaStream_t s = nullptr;
+    Events() = default;
+    Events(const Events&) = delete;
+    Events& operator=(const Events&) = delete;
+    ~Events() {
+        for (cudaEvent_t e : ev) cudaEventDestroy(e);
+    }
+    int create(size_t n) {
+        for (size_t i = 0; i < n; ++i) {
+            cudaEvent_t e;
+            MBAR_CUDA(cudaEventCreate(&e));
+            ev.push_back(e);
+        }
+        return MBAR_B200_OK;
+    }
+    float ms(size_t a, size_t b) const {
+        float m = 0.f;
+        cudaEventElapsedTime(&m, ev[a], ev[b]);
+        return m;
+    }
+    int start(cudaStream_t stream) {
+        s = stream;
+        MBAR_TRY(create(2));
+        MBAR_CUDA(cudaEventRecord(ev[0], s));
+        return MBAR_B200_OK;
+    }
+    float stop() {
+        cudaEventRecord(ev[1], s);
+        cudaEventSynchronize(ev[1]);
+        return ms(0, 1);
+    }
+};
+
+// stream-ordered rendezvous of all ranks (one tiny all-reduce) before the first in-kernel peer exchange of a loop
+static int comm_rendezvous(mbar_b200_ctx* c) {
     if (!c->comm || c->nranks == 1) return MBAR_B200_OK;
     // every rank's stream reaches the first in-kernel exchange within microseconds of the others
-    return comm_allreduce(c, c->d_scratch + (size_t)c->K * c->K + 4 * (size_t)c->K, 1, 0);
+    return comm_allreduce(c, c->d_scratch + scratch_rendezvous(c->K), 1, 0);
 }
 
 static int loop_begin(mbar_b200_ctx* c, double tol, int maxiter, int min_sc_iter, double gamma) {
@@ -391,117 +432,355 @@ static int loop_begin(mbar_b200_ctx* c, double tol, int maxiter, int min_sc_iter
     return MBAR_B200_OK;
 }
 
-// download LoopState + f (pinned row 5) and wait: the ONE synchronisation per batch
-static int loop_poll(mbar_b200_ctx* c) {
-    const int K = c->K;
-    MBAR_CUDA(cudaMemcpyAsync(c->h_loop, c->d_loop, sizeof(LoopState), cudaMemcpyDeviceToHost, c->stream));
-    MBAR_CUDA(cudaMemcpyAsync(c->h_f + 5 * K, c->d_f, (size_t)K * sizeof(double), cudaMemcpyDeviceToHost, c->stream));
-    MBAR_CUDA(cudaStreamSynchronize(c->stream));
-    c->d2hBytes += (int64_t)K * 8 + (int64_t)sizeof(LoopState);
-    c->loopPolls++;
-    MBAR_CUDA(cudaGetLastError());
-    return MBAR_B200_OK;
-}
-
 static bool device_loop_possible(const mbar_b200_ctx* c) {
     if (c->kernelChoice == MBAR_B200_KERNEL_GENERIC) return false;
     if (c->nranks > 1 && !c->comm) return false;
     return c->K <= 2048;
 }
 
-int solve_sci_device(mbar_b200_ctx* c, double* f, double tol, int32_t maxiter, mbar_b200_solve_result* res) {
-    MBAR_REQUIRE(c->ready, MBAR_B200_ERR_NOT_READY, "u_kn has not been uploaded");
-    MBAR_CUDA(cudaSetDevice(c->device));
-    MBAR_TRY(check_range(c, f));
+// One kernel per self-consistent iteration when the exchange can live inside the pass kernel (single GPU, or peers
+// attached through mbar_b200_peer_attach); otherwise pass -> all-reduce -> sci_loop_epilogue_kernel.
+static bool sci_epilogue_in_kernel(const mbar_b200_ctx* c) {
+    return (c->nranks == 1 || c->peerReady) && !std::getenv("MBAR_B200_NO_FUSED_EPILOGUE");
+}
+
+// f -> pinned row ROW_F -> ctx->d_f (asynchronous)
+static int upload_f(mbar_b200_ctx* c, const double* f) {
     const int K = c->K;
+    std::memcpy(c->hf(ROW_F), f, K * sizeof(double));
+    MBAR_CUDA(cudaMemcpyAsync(c->d_f, c->hf(ROW_F), K * sizeof(double), cudaMemcpyHostToDevice, c->stream));
+    c->h2dBytes += K * 8;
+    return MBAR_B200_OK;
+}
+
+// Largest relative change over the sampled states other than the gauge state (mbar_solvers.py:627-631), NaN if any
+// entry is NaN.
+static double rel_delta(const mbar_b200_ctx* c, const std::vector<double>& fn, const std::vector<double>& fo,
+                        double tol) {
+    double md = 0.0;
+    const double thr = std::min(1e-8, tol);
+    for (size_t i = 1; i < c->active.size(); ++i) {
+        const int k = c->active[i];
+        const double d = rel_change(fn[k], fo[k], fn[k], thr);
+        if (std::isnan(d)) return NAN;
+        md = std::max(md, d);
+    }
+    return md;
+}
+
+// The self-consistent step (Eq. C3) from the packed output of run_pass at cur: f_k - log S_k over the sampled
+// states, gauge-fixed so that f[firstActive] = 0; unsampled states keep cur.  nxt may be cur.
+static void sci_step(const mbar_b200_ctx* c, const std::vector<double>& cur, std::vector<double>& nxt) {
+    const double* logS = c->h_out + PassLayout{c->K}.logS();
     const int g0 = c->firstActive;
-    if (!device_loop_possible(c) || maxiter < 1 || c->active.size() < 2)
-        return solve_sci_stepped(c, f, tol, maxiter, res);
-    std::vector<double> cur(f, f + K), snap(K);
-    for (int k : c->active) cur[k] -= f[g0];
-    mbar_b200_solve_result r{};
-    cudaEvent_t e0, e1;
-    MBAR_CUDA(cudaEventCreate(&e0));
-    MBAR_CUDA(cudaEventCreate(&e1));
-    MBAR_CUDA(cudaEventRecord(e0, c->stream));
-    MBAR_TRY(loop_begin(c, tol, maxiter, 0, 1.0));
-    const bool inKernel = (c->nranks == 1 || c->peerReady) && !std::getenv("MBAR_B200_NO_FUSED_EPILOGUE");
-    if (c->peerReady && inKernel) MBAR_TRY(comm_rendezvous(c));
-    const int threads = 256;
-    bool fallback = false;
-    int itersBefore = 0;
-    int rc = MBAR_B200_OK;
-    for (;;) {
-        snap = cur;
-        itersBefore = c->h_loop->iterations;
-        FusedParams p;
-        bool ok = false;
-        MBAR_TRY(fused_prepare(c, cur.data(), false, false, &p, &ok));
-        if (!ok) { fallback = true; break; }
-        std::memcpy(c->h_f + 4 * K, cur.data(), K * sizeof(double));
-        MBAR_CUDA(cudaMemcpyAsync(c->d_f, c->h_f + 4 * K, K * sizeof(double), cudaMemcpyHostToDevice, c->stream));
-        c->h2dBytes += K * 8;
-        p.loop = c->d_loop;
-        p.first = g0;
-        if (inKernel) {
-            p.epi = 1;
-            p.f = c->d_f;
-            p.cnext = c->d_c;
-            if (c->peerReady) p.peer = c->peer;
+    const double shift = cur[g0] - logS[g0];
+    nxt = cur;
+    for (int k : c->active) nxt[k] = (cur[k] - logS[k]) - shift;
+}
+
+// gradient norm at f over the sampled states (mbar_solvers.py:938-940): one more pass
+static int final_gnorm(mbar_b200_ctx* c, const std::vector<double>& f, mbar_b200_solve_result* r) {
+    const int rc = run_pass(c, f.data(), PassWant{});
+    r->passes++;
+    double gn = 0.0;
+    for (int k : c->active) {
+        const double g = c->h_Nk[k] * (c->h_out[k] - 1.0);
+        gn += g * g;
+    }
+    r->gnorm = std::sqrt(gn);
+    return rc;
+}
+
+// In-place Cholesky of the n x n SPD matrix A (row-major, lower); returns false if not PD.
+static bool cholesky(std::vector<double>& A, int n) {
+    for (int j = 0; j < n; ++j) {
+        double d = A[(size_t)j * n + j];
+        for (int k = 0; k < j; ++k) d -= A[(size_t)j * n + k] * A[(size_t)j * n + k];
+        if (!(d > 0.0) || !std::isfinite(d)) return false;
+        d = std::sqrt(d);
+        A[(size_t)j * n + j] = d;
+        const double inv = 1.0 / d;
+        for (int i = j + 1; i < n; ++i) {
+            double s = A[(size_t)i * n + j];
+            const double* ai = &A[(size_t)i * n];
+            const double* aj = &A[(size_t)j * n];
+            for (int k = 0; k < j; ++k) s -= ai[k] * aj[k];
+            A[(size_t)i * n + j] = s * inv;
         }
-        for (int b = 0; b < c->loopBatch; ++b) {
-            MBAR_TRY(fused_enqueue(c, p));
-            if (!inKernel) {
-                MBAR_TRY(comm_allreduce(c, c->d_out, K + 2, 0));
-                sci_loop_epilogue_kernel<<<1, threads, 0, c->stream>>>(c->d_out, c->d_f, c->d_c, c->d_Nk, c->d_rowmask,
-                                                                      K, g0, p.mid, c->d_loop);
-                c->launches++;
+    }
+    return true;
+}
+static void chol_solve(const std::vector<double>& Lc, int n, std::vector<double>& b) {
+    for (int i = 0; i < n; ++i) {
+        double s = b[i];
+        for (int k = 0; k < i; ++k) s -= Lc[(size_t)i * n + k] * b[k];
+        b[i] = s / Lc[(size_t)i * n + i];
+    }
+    for (int i = n - 1; i >= 0; --i) {
+        double s = b[i];
+        for (int k = i + 1; k < n; ++k) s -= Lc[(size_t)k * n + i] * b[k];
+        b[i] = s / Lc[(size_t)i * n + i];
+    }
+}
+
+// ---- host-stepped loops: one host round trip per pass.  They are the robust fallback of the device-resident loops
+// (generic kernel, log-domain sums, ridge retries) and stay selectable with mbar_b200_set_loop_mode(ctx, 1).
+static int solve_sci_stepped(mbar_b200_ctx* c, double* f, double tol, int32_t maxiter, mbar_b200_solve_result* res) {
+    const int K = c->K;
+    std::vector<double> cur(f, f + K), nxt(K);
+    mbar_b200_solve_result r{};
+    Events timer;
+    MBAR_TRY(timer.start(c->stream));
+    for (int k : c->active) cur[k] -= f[c->firstActive];
+    int rc = MBAR_B200_OK;
+    for (int it = 0; it < maxiter; ++it) {
+        rc = run_pass(c, cur.data(), PassWant{});
+        if (rc != MBAR_B200_OK) break;
+        r.passes++;
+        sci_step(c, cur, nxt);
+        r.max_delta = rel_delta(c, nxt, cur, tol);
+        cur.swap(nxt);
+        r.iterations = it + 1;
+        r.sci_iterations = it + 1;
+        if (std::isnan(r.max_delta) || r.max_delta < tol) {
+            r.success = 1;
+            break;
+        }
+    }
+    if (rc == MBAR_B200_OK) rc = final_gnorm(c, cur, &r);
+    r.device_ms = timer.stop();
+    if (rc == MBAR_B200_OK) std::memcpy(f, cur.data(), K * sizeof(double));
+    if (res) *res = r;
+    return rc;
+}
+
+static int solve_adaptive_stepped(mbar_b200_ctx* c, double* f, double tol, int32_t maxiter, int32_t min_sc_iter,
+                                  double gamma, mbar_b200_solve_result* res) {
+    const int K = c->K;
+    const PassLayout lay{K};
+    const int na = (int)c->active.size();
+    std::vector<double> cur(f, f + K), f_sci(K), f_nr(K), g(K, 0.0), g_sci(K), g_nr(K);
+    std::vector<double> A, rhs;
+    mbar_b200_solve_result r{};
+    Events timer;
+    MBAR_TRY(timer.start(c->stream));
+    for (int k : c->active) cur[k] -= f[c->firstActive];
+    int rc = MBAR_B200_OK;
+    auto grad_from_out = [&](std::vector<double>& out) {
+        double gn = 0.0;
+        for (int k = 0; k < K; ++k) {
+            out[k] = c->h_Nk[k] > 0 ? c->h_Nk[k] * (c->h_out[k] - 1.0) : 0.0;
+            gn += out[k] * out[k];
+        }
+        return gn;
+    };
+    for (int it = 0; it < maxiter && rc == MBAR_B200_OK; ++it) {
+        // pass at f with the second moments: gives g, H and the self-consistent candidate at once
+        PassWant w;
+        w.G = true;
+        rc = run_pass(c, cur.data(), w);
+        if (rc != MBAR_B200_OK) break;
+        r.passes++;
+        r.hessian_passes++;
+        grad_from_out(g);
+        sci_step(c, cur, f_sci);
+        // Newton step in the reduced coordinates (gauge state dropped): H[1:,1:] x = g[1:]
+        // (mbar_solvers.py:581-584 uses the min-norm lstsq of the singular full H minus its first
+        // component — the same step in exact arithmetic, SURVEY.md Appendix A).
+        bool haveNr = false;
+        if (na > 1) {
+            const int n = na - 1;
+            const double* Gh = c->h_out + lay.G();
+            double ridge = 0.0, ridgeRel = 0.0, tr = 0.0;
+            for (int a = 1; a < na; ++a) {
+                const int i = c->active[a];
+                tr += c->h_Nk[i] * c->h_out[i];
+            }
+            for (int attempt = 0; attempt < 4 && !haveNr; ++attempt) {
+                A.assign((size_t)n * n, 0.0);
+                for (int a = 1; a < na; ++a) {
+                    const int i = c->active[a];
+                    for (int b = 1; b <= a; ++b) {
+                        const int j = c->active[b];
+                        double v = -Gh[(size_t)i * K + j];
+                        if (i == j) v += c->h_Nk[i] * c->h_out[i] + ridge;
+                        A[(size_t)(a - 1) * n + (b - 1)] = v;
+                    }
+                }
+                if (cholesky(A, n)) {
+                    rhs.resize(n);
+                    for (int a = 1; a < na; ++a) rhs[a - 1] = g[c->active[a]];
+                    chol_solve(A, n, rhs);
+                    f_nr = cur;
+                    for (int a = 1; a < na; ++a) f_nr[c->active[a]] = cur[c->active[a]] - gamma * rhs[a - 1];
+                    haveNr = true;
+                    for (int a = 1; a < na; ++a)
+                        if (!std::isfinite(f_nr[c->active[a]]) || std::fabs(f_nr[c->active[a]]) > 0.5 * C_RANGE)
+                            haveNr = false;
+                } else {
+                    ridgeRel = (ridgeRel == 0.0) ? 1e-12 : ridgeRel * 1e3;   // relative to the mean diagonal
+                    ridge = ridgeRel * (tr / n + 1e-300);
+                }
             }
         }
-        MBAR_TRY(loop_poll(c));
+        rc = run_pass(c, f_sci.data(), PassWant{});
+        if (rc != MBAR_B200_OK) break;
+        r.passes++;
+        const double gn_sci = grad_from_out(g_sci);
+        double gn_nr = INFINITY;
+        if (haveNr) {
+            rc = run_pass(c, f_nr.data(), PassWant{});
+            if (rc != MBAR_B200_OK) break;
+            r.passes++;
+            gn_nr = grad_from_out(g_nr);
+            if (std::isnan(gn_nr)) gn_nr = INFINITY;
+        } else {
+            f_nr = f_sci;
+        }
+        std::vector<double> f_old = cur;
+        if (gn_sci < gn_nr || r.sci_iterations < min_sc_iter) {     // mbar_solvers.py:607
+            cur = f_sci;
+            r.sci_iterations++;
+            r.gnorm = std::sqrt(gn_sci);
+        } else {
+            cur = f_nr;
+            r.nr_iterations++;
+            r.gnorm = std::sqrt(gn_nr);
+        }
+        r.iterations = it + 1;
+        r.max_delta = rel_delta(c, cur, f_old, tol);
+        // max |f_sci - f_nr| / |f|  (mbar_solvers.py:632)
+        double max_diff = 0.0;
+        const double thr = std::min(1e-8, tol);
+        for (size_t i = 1; i < c->active.size(); ++i) {
+            const int k = c->active[i];
+            max_diff = std::max(max_diff, rel_change(f_sci[k], f_nr[k], cur[k], thr));
+        }
+        if (std::isnan(r.max_delta) || (r.max_delta < tol && max_diff < std::sqrt(tol))) {
+            r.success = 1;
+            break;
+        }
+    }
+    r.device_ms = timer.stop();
+    if (rc == MBAR_B200_OK) std::memcpy(f, cur.data(), K * sizeof(double));
+    if (res) *res = r;
+    return rc;
+}
+
+// `iters` host-stepped self-consistent iterations, no convergence test (mbar_b200_sci_iterate's robust path)
+static int sci_iterate_stepped(mbar_b200_ctx* c, double* f, int iters) {
+    std::vector<double> cur(f, f + c->K);
+    for (int it = 0; it < iters; ++it) {
+        MBAR_TRY(run_pass(c, cur.data(), PassWant{}));
+        sci_step(c, cur, cur);
+    }
+    std::memcpy(f, cur.data(), c->K * sizeof(double));
+    return MBAR_B200_OK;
+}
+
+// ---- device-resident loops
+// Enqueues `n` self-consistent iterations on the f in ctx->d_f with the pass p (from fused_prepare): the fused pass
+// with its in-kernel epilogue, or pass -> all-reduce -> epilogue kernel.  loop: early exit and convergence test, or
+// NULL (every iteration runs).  ev, optional: two events per iteration recorded around the pass launch.
+static int enqueue_sci(mbar_b200_ctx* c, FusedParams p, bool inKernel, int n, LoopState* loop,
+                       const cudaEvent_t* ev) {
+    const int K = c->K;
+    p.loop = loop;
+    p.first = c->firstActive;
+    if (inKernel) {
+        p.epi = 1;
+        p.f = c->d_f;
+        p.cnext = c->dc(ROW_C);
+        if (c->peerReady) p.peer = c->peer;
+    }
+    for (int it = 0; it < n; ++it) {
+        if (ev) MBAR_CUDA(cudaEventRecord(ev[2 * it], c->stream));
+        MBAR_TRY(fused_enqueue(c, p));
+        if (ev) MBAR_CUDA(cudaEventRecord(ev[2 * it + 1], c->stream));
+        if (!inKernel) {
+            MBAR_TRY(comm_allreduce(c, c->d_out, K + 2, 0));
+            sci_loop_epilogue_kernel<<<1, 256, 0, c->stream>>>(c->d_out, c->d_f, c->dc(ROW_C), c->d_Nk, c->d_rowmask,
+                                                               K, p.first, p.mid, loop);
+            c->launches++;
+        }
+    }
+    return MBAR_B200_OK;
+}
+
+// The batches of a device-resident solver.  batch(f, &ok) configures the fused pass at f (ok = false: it does not
+// apply), uploads f and enqueues one batch of iterations; then LoopState and f come back in the batch's one
+// synchronisation.  On return cur holds the last f the device reported.  *fallback: the fast path gave up, cur is
+// the f that batch started from, after *itersBefore iterations, and the caller finishes on its host-stepped loop.
+static int poll_batches(mbar_b200_ctx* c, std::vector<double>& cur, int* itersBefore, bool* fallback,
+                        const std::function<int(const double*, bool*)>& batch) {
+    const int K = c->K;
+    *fallback = false;
+    for (;;) {
+        *itersBefore = c->h_loop->iterations;
+        bool ok = false;
+        MBAR_TRY(batch(cur.data(), &ok));
+        if (!ok) {
+            *fallback = true;
+            return MBAR_B200_OK;
+        }
+        MBAR_CUDA(cudaMemcpyAsync(c->h_loop, c->d_loop, sizeof(LoopState), cudaMemcpyDeviceToHost, c->stream));
+        MBAR_CUDA(cudaMemcpyAsync(c->hf(ROW_POLL), c->d_f, (size_t)K * sizeof(double), cudaMemcpyDeviceToHost,
+                                  c->stream));
+        MBAR_CUDA(cudaStreamSynchronize(c->stream));
+        c->d2hBytes += (int64_t)K * 8 + (int64_t)sizeof(LoopState);
+        c->loopPolls++;
+        MBAR_CUDA(cudaGetLastError());
         const LoopState& st = *c->h_loop;
         if (st.status != 0) {
             MBAR_REQUIRE(st.status != 2, MBAR_B200_ERR_COMM,
                          "peer exchange timed out inside the pass kernel (a rank did not arrive)");
-            fallback = true;
-            break;
+            *fallback = true;
+            return MBAR_B200_OK;
         }
-        std::memcpy(cur.data(), c->h_f + 5 * K, K * sizeof(double));
-        if (st.done) break;
+        std::memcpy(cur.data(), c->hf(ROW_POLL), K * sizeof(double));
+        if (st.done) return MBAR_B200_OK;
     }
-    const LoopState st = *c->h_loop;
-    r.iterations = r.sci_iterations = st.iterations;
-    r.passes = st.iterations;
-    r.success = st.success;
-    r.max_delta = st.max_delta;
+}
+
+static int solve_sci_device(mbar_b200_ctx* c, double* f, double tol, int32_t maxiter, mbar_b200_solve_result* res) {
+    MBAR_REQUIRE(c->ready, MBAR_B200_ERR_NOT_READY, "u_kn has not been uploaded");
+    MBAR_CUDA(cudaSetDevice(c->device));
+    MBAR_TRY(check_range(c, f));
+    if (!device_loop_possible(c) || maxiter < 1 || c->active.size() < 2)
+        return solve_sci_stepped(c, f, tol, maxiter, res);
+    std::vector<double> cur(f, f + c->K);
+    for (int k : c->active) cur[k] -= f[c->firstActive];
+    Events timer;
+    MBAR_TRY(timer.start(c->stream));
+    MBAR_TRY(loop_begin(c, tol, maxiter, 0, 1.0));
+    const bool inKernel = sci_epilogue_in_kernel(c);
+    if (c->peerReady && inKernel) MBAR_TRY(comm_rendezvous(c));
+    int itersBefore = 0;
+    bool fallback = false;
+    MBAR_TRY(poll_batches(c, cur, &itersBefore, &fallback, [&](const double* fb, bool* ok) -> int {
+        FusedParams p;
+        MBAR_TRY(fused_prepare(c, fb, false, false, &p, ok));
+        if (!*ok) return MBAR_B200_OK;
+        MBAR_TRY(upload_f(c, fb));
+        return enqueue_sci(c, p, inKernel, c->loopBatch, c->d_loop, nullptr);
+    }));
+    mbar_b200_solve_result r{};
+    int rc;
     if (fallback) {
         // redo from the last good f on the robust path (generic kernel, log-domain sums)
-        mbar_b200_solve_result r2{};
-        const int done = itersBefore;
-        rc = solve_sci_stepped(c, snap.data(), tol, maxiter - done > 1 ? maxiter - done : 1, &r2);
-        cur = snap;
-        r2.iterations += done;
-        r2.sci_iterations += done;
-        r2.passes += done;
-        r = r2;
+        rc = solve_sci_stepped(c, cur.data(), tol, std::max(maxiter - itersBefore, 1), &r);
+        r.iterations += itersBefore;
+        r.sci_iterations += itersBefore;
+        r.passes += itersBefore;
     } else {
-        // gradient norm at the returned f (mbar_solvers.py:938-940): one more pass
-        rc = run_pass(c, cur.data(), PassWant{});
-        r.passes++;
-        double gn = 0.0;
-        for (int k : c->active) {
-            const double g = c->h_Nk[k] * (c->h_out[k] - 1.0);
-            gn += g * g;
-        }
-        r.gnorm = std::sqrt(gn);
+        const LoopState& st = *c->h_loop;
+        r.iterations = r.sci_iterations = st.iterations;
+        r.passes = st.iterations;
+        r.success = st.success;
+        r.max_delta = st.max_delta;
+        rc = final_gnorm(c, cur, &r);
     }
-    cudaEventRecord(e1, c->stream);
-    cudaEventSynchronize(e1);
-    float ms = 0.f;
-    cudaEventElapsedTime(&ms, e0, e1);
-    r.device_ms = ms;
-    cudaEventDestroy(e0);
-    cudaEventDestroy(e1);
+    r.device_ms = timer.stop();
     if (rc == MBAR_B200_OK)
         for (int k : c->active) f[k] = cur[k];
     if (res) *res = r;
@@ -559,7 +838,7 @@ static int enqueue_adaptive_iteration(mbar_b200_ctx* c, const FusedParams& pF, c
         if (nccl) MBAR_TRY(comm_allreduce(c, pN.out, K + 2, 0));
     }
     // (5) choice + convergence + next iteration's vectors
-    adapt_post_kernel<<<1, 256, 0, c->stream>>>(pS.out, pN.out, av, c->d_f, c->d_c, c->d_Nk, c->d_rowmask, K, g0,
+    adapt_post_kernel<<<1, 256, 0, c->stream>>>(pS.out, pN.out, av, c->d_f, c->dc(ROW_C), c->d_Nk, c->d_rowmask, K, g0,
                                                pF.mid, c->d_loop);
     MBAR_CUDA(cudaGetLastError());
     c->launches += 6;
@@ -642,40 +921,30 @@ static int run_adaptive_batch(mbar_b200_ctx* c, const FusedParams& pF, const Fus
     return MBAR_B200_OK;
 }
 
-int solve_adaptive_device(mbar_b200_ctx* c, double* f, double tol, int32_t maxiter, int32_t min_sc_iter,
-                          double gamma, mbar_b200_solve_result* res) {
+static int solve_adaptive_device(mbar_b200_ctx* c, double* f, double tol, int32_t maxiter, int32_t min_sc_iter,
+                                 double gamma, mbar_b200_solve_result* res) {
     MBAR_REQUIRE(c->ready, MBAR_B200_ERR_NOT_READY, "u_kn has not been uploaded");
     MBAR_CUDA(cudaSetDevice(c->device));
     MBAR_TRY(check_range(c, f));
     const int K = c->K;
-    const int g0 = c->firstActive;
-    const int na = (int)c->active.size();
-    if (!device_loop_possible(c) || maxiter < 1 || na < 2)
+    if (!device_loop_possible(c) || maxiter < 1 || c->active.size() < 2)
         return solve_adaptive_stepped(c, f, tol, maxiter, min_sc_iter, gamma, res);
-    std::vector<double> cur(f, f + K), snap(K);
-    for (int k : c->active) cur[k] -= f[g0];
-    mbar_b200_solve_result r{};
-    cudaEvent_t e0, e1;
-    MBAR_CUDA(cudaEventCreate(&e0));
-    MBAR_CUDA(cudaEventCreate(&e1));
-    MBAR_CUDA(cudaEventRecord(e0, c->stream));
+    std::vector<double> cur(f, f + K);
+    for (int k : c->active) cur[k] -= f[c->firstActive];
+    Events timer;
+    MBAR_TRY(timer.start(c->stream));
     MBAR_TRY(loop_begin(c, tol, maxiter, min_sc_iter, gamma));
     if (c->peerReady) MBAR_TRY(comm_rendezvous(c));
-    bool fallback = false, usedM2 = false;
+    bool usedM2 = false;
     int itersBefore = 0;
-    int rc = MBAR_B200_OK;
-    for (;;) {
-        snap = cur;
-        itersBefore = c->h_loop->iterations;
+    bool fallback = false;
+    MBAR_TRY(poll_batches(c, cur, &itersBefore, &fallback, [&](const double* fb, bool* ok) -> int {
         FusedParams pF;
-        bool ok = false;
-        MBAR_TRY(fused_prepare(c, cur.data(), true, false, &pF, &ok, nullptr, nullptr, true, 1, 16.0));
-        if (!ok) { fallback = true; break; }
-        std::memcpy(c->h_f + 4 * K, cur.data(), K * sizeof(double));
-        MBAR_CUDA(cudaMemcpyAsync(c->d_f, c->h_f + 4 * K, K * sizeof(double), cudaMemcpyHostToDevice, c->stream));
-        c->h2dBytes += K * 8;
+        MBAR_TRY(fused_prepare(c, fb, true, false, &pF, ok, nullptr, nullptr, true, 1, 16.0));
+        if (!*ok) return MBAR_B200_OK;
+        MBAR_TRY(upload_f(c, fb));
         pF.loop = c->d_loop;
-        pF.first = g0;
+        pF.first = c->firstActive;
         if (c->peerReady) pF.peer = c->peer;
         FusedParams pS = pF, pN = pF;
         pS.Wout = pN.Wout = nullptr;
@@ -690,11 +959,11 @@ int solve_adaptive_device(mbar_b200_ctx* c, double* f, double tol, int32_t maxit
         bool okM = false;
         static const bool noM2 = std::getenv("MBAR_B200_NO_M2") != nullptr;
         if (!noM2)
-            MBAR_TRY(fused_prepare(c, cur.data(), false, false, &pM, &okM, c->d_av + AV_CSCI * K, c->h_f + 6 * K,
-                                   false, 2, 16.0));
+            MBAR_TRY(fused_prepare(c, fb, false, false, &pM, &okM, c->d_av + AV_CSCI * K, c->hf(ROW_C2), false, 2,
+                                   16.0));
         if (okM) {
             pM.loop = c->d_loop;
-            pM.first = g0;
+            pM.first = c->firstActive;
             if (c->peerReady) pM.peer = c->peer;
             pM.c = c->d_av + AV_CSCI * K;
             pM.c2 = c->d_av + AV_CNR * K;
@@ -702,46 +971,30 @@ int solve_adaptive_device(mbar_b200_ctx* c, double* f, double tol, int32_t maxit
             pM.out = pS.out;
             pM.out2 = pN.out;
         }
-        MBAR_TRY(run_adaptive_batch(c, pF, pS, pN, okM ? &pM : nullptr, c->loopBatch));
         usedM2 = usedM2 || okM;
-        MBAR_TRY(loop_poll(c));
-        const LoopState& st = *c->h_loop;
-        if (st.status != 0) {
-            MBAR_REQUIRE(st.status != 2, MBAR_B200_ERR_COMM,
-                         "peer exchange timed out inside the pass kernel (a rank did not arrive)");
-            fallback = true;
-            break;
-        }
-        std::memcpy(cur.data(), c->h_f + 5 * K, K * sizeof(double));
-        if (st.done) break;
-    }
+        return run_adaptive_batch(c, pF, pS, pN, okM ? &pM : nullptr, c->loopBatch);
+    }));
+    const int passesPerIter = usedM2 ? 2 : 3;
     const LoopState st = *c->h_loop;
-    r.iterations = st.iterations;
-    r.nr_iterations = st.nr_iterations;
-    r.sci_iterations = st.sci_iterations;
-    r.passes = (usedM2 ? 2 : 3) * st.iterations;
-    r.hessian_passes = st.iterations;
-    r.success = st.success;
-    r.max_delta = st.max_delta;
-    r.gnorm = st.gnorm;
+    mbar_b200_solve_result r{};
+    int rc = MBAR_B200_OK;
     if (fallback) {
-        mbar_b200_solve_result r2{};
-        const int left = maxiter - itersBefore > 1 ? maxiter - itersBefore : 1;
-        const int msi = min_sc_iter - st.sci_iterations > 0 ? min_sc_iter - st.sci_iterations : 0;
-        rc = solve_adaptive_stepped(c, snap.data(), tol, left, msi, gamma, &r2);
-        cur = snap;
-        r2.iterations += itersBefore;
-        r2.passes += (usedM2 ? 2 : 3) * itersBefore;
-        r2.hessian_passes += itersBefore;
-        r = r2;
+        const int msi = std::max(min_sc_iter - st.sci_iterations, 0);
+        rc = solve_adaptive_stepped(c, cur.data(), tol, std::max(maxiter - itersBefore, 1), msi, gamma, &r);
+        r.iterations += itersBefore;
+        r.passes += passesPerIter * itersBefore;
+        r.hessian_passes += itersBefore;
+    } else {
+        r.iterations = st.iterations;
+        r.nr_iterations = st.nr_iterations;
+        r.sci_iterations = st.sci_iterations;
+        r.passes = passesPerIter * st.iterations;
+        r.hessian_passes = st.iterations;
+        r.success = st.success;
+        r.max_delta = st.max_delta;
+        r.gnorm = st.gnorm;
     }
-    cudaEventRecord(e1, c->stream);
-    cudaEventSynchronize(e1);
-    float ms = 0.f;
-    cudaEventElapsedTime(&ms, e0, e1);
-    r.device_ms = ms;
-    cudaEventDestroy(e0);
-    cudaEventDestroy(e1);
+    r.device_ms = timer.stop();
     if (rc == MBAR_B200_OK)
         for (int k : c->active) f[k] = cur[k];
     if (res) *res = r;
@@ -749,3 +1002,106 @@ int solve_adaptive_device(mbar_b200_ctx* c, double* f, double tol, int32_t maxit
 }
 
 }  // namespace mbar
+
+using namespace mbar;
+
+extern "C" {
+
+int mbar_b200_solve_sci(mbar_b200_ctx* c, double* f, double tol, int32_t maxiter, mbar_b200_solve_result* res) {
+    MBAR_REQUIRE(c && f, MBAR_B200_ERR_INVALID, "NULL argument");
+    NvtxRange nvtx_("mbar_b200::solve_sci");
+    if (c->loopMode == 1) return solve_sci_stepped(c, f, tol, maxiter, res);
+    return solve_sci_device(c, f, tol, maxiter, res);
+}
+
+int mbar_b200_solve_adaptive(mbar_b200_ctx* c, double* f, double tol, int32_t maxiter, int32_t min_sc_iter,
+                             double gamma, mbar_b200_solve_result* res) {
+    MBAR_REQUIRE(c && f, MBAR_B200_ERR_INVALID, "NULL argument");
+    NvtxRange nvtx_("mbar_b200::solve_adaptive");
+    if (c->loopMode == 1) return solve_adaptive_stepped(c, f, tol, maxiter, min_sc_iter, gamma, res);
+    return solve_adaptive_device(c, f, tol, maxiter, min_sc_iter, gamma, res);
+}
+
+int mbar_b200_set_loop_mode(mbar_b200_ctx* c, int32_t mode, int32_t batch) {
+    MBAR_REQUIRE(c, MBAR_B200_ERR_INVALID, "ctx is NULL");
+    MBAR_REQUIRE(mode == 0 || mode == 1, MBAR_B200_ERR_INVALID, "mode=%d (0 device-resident, 1 host-stepped)", mode);
+    c->loopMode = mode;
+    if (batch >= 1) c->loopBatch = batch > 64 ? 64 : batch;
+    return MBAR_B200_OK;
+}
+
+int mbar_b200_get_loop_stats(const mbar_b200_ctx* c, int64_t* polls, int32_t* mode, int32_t* batch) {
+    MBAR_REQUIRE(c, MBAR_B200_ERR_INVALID, "ctx is NULL");
+    if (polls) *polls = c->loopPolls;
+    if (mode) *mode = c->loopMode;
+    if (batch) *batch = c->loopBatch;
+    return MBAR_B200_OK;
+}
+
+int mbar_b200_get_graph_stats(const mbar_b200_ctx* c, int64_t* captures, int64_t* launches) {
+    MBAR_REQUIRE(c, MBAR_B200_ERR_INVALID, "ctx is NULL");
+    if (captures) *captures = c->graphCaptures;
+    if (launches) *launches = c->graphLaunches;
+    return MBAR_B200_OK;
+}
+
+int mbar_b200_sci_iterate(mbar_b200_ctx* c, double* f, int32_t iters) {
+    MBAR_REQUIRE(c && f && iters >= 0, MBAR_B200_ERR_INVALID, "bad argument");
+    MBAR_REQUIRE(c->ready, MBAR_B200_ERR_NOT_READY, "u_kn has not been uploaded");
+    MBAR_CUDA(cudaSetDevice(c->device));
+    MBAR_TRY(check_range(c, f));
+    const int K = c->K;
+    FusedParams p;
+    bool ok = false;
+    if (c->kernelChoice != MBAR_B200_KERNEL_GENERIC) MBAR_TRY(fused_prepare(c, f, false, false, &p, &ok));
+    if (!ok) return sci_iterate_stepped(c, f, iters);
+    MBAR_TRY(upload_f(c, f));
+    // per-launch CUDA events of the pass kernel (bench: average launch duration over the loop)
+    Events ev;
+    const bool perLaunch = c->timePasses && iters > 0 && iters <= 4096;
+    if (perLaunch) MBAR_TRY(ev.create(2 * (size_t)iters));
+    Events timer;
+    MBAR_TRY(timer.start(c->stream));
+    const bool inKernel = sci_epilogue_in_kernel(c);
+    MBAR_REQUIRE(c->nranks == 1 || c->comm, MBAR_B200_ERR_NOT_READY,
+                 "sharded problem (%d ranks) without a communicator: call mbar_b200_comm_init", c->nranks);
+    if (inKernel && c->peerReady) MBAR_TRY(comm_rendezvous(c));
+    NvtxRange nvtx_("mbar_b200::sci_iterate");
+    MBAR_TRY(enqueue_sci(c, p, inKernel, iters, nullptr, perLaunch ? ev.ev.data() : nullptr));
+    c->lastLoopMs = timer.stop();
+    double ksum = 0.0;
+    for (int it = 0; perLaunch && it < iters; ++it) ksum += ev.ms(2 * it, 2 * it + 1);
+    c->lastLoopKernelMs = ksum;
+    c->lastLoopIters = iters;
+    MBAR_CUDA(cudaGetLastError());
+    double* fh = c->hf(ROW_F);
+    MBAR_CUDA(cudaMemcpyAsync(fh, c->d_f, K * sizeof(double), cudaMemcpyDeviceToHost, c->stream));
+    const PassLayout lay{K};
+    MBAR_CUDA(cudaMemcpyAsync(c->h_out, c->d_out, (size_t)lay.size(false) * sizeof(double),
+                              cudaMemcpyDeviceToHost, c->stream));
+    MBAR_CUDA(cudaStreamSynchronize(c->stream));
+    c->d2hBytes += K * 8 + lay.size(false) * 8;
+    float ms = 0.f;
+    if (cudaEventElapsedTime(&ms, c->evA, c->evB) == cudaSuccess) c->lastPassMs = ms;
+    MBAR_REQUIRE(!(iters > 0 && c->h_out[lay.flag()] >= 1.0e6), MBAR_B200_ERR_COMM,
+                 "peer exchange timed out inside the pass kernel (a rank did not arrive)");
+    if (p.debugSkip) return MBAR_B200_OK;   // memory-pipeline probe: the arithmetic was skipped, nothing to return
+    if (iters > 0 && c->h_out[lay.flag()] != 0.0) fh[c->firstActive] = NAN;  // force the robust redo
+    bool finite = true;
+    for (int k : c->active) finite = finite && std::isfinite(fh[k]);
+    // some S_k underflowed in the linear-domain fused kernel: redo on the robust stepped path
+    if (!finite) return sci_iterate_stepped(c, f, iters);
+    for (int k = 0; k < K; ++k)
+        if (c->h_Nk[k] > 0) f[k] = fh[k];
+    return MBAR_B200_OK;
+}
+
+int mbar_b200_last_loop_ms(mbar_b200_ctx* c, double* total_ms, double* kernel_ms_sum, int32_t* iters) {
+    MBAR_REQUIRE(c, MBAR_B200_ERR_INVALID, "ctx is NULL");
+    if (total_ms) *total_ms = c->lastLoopMs;
+    if (kernel_ms_sum) *kernel_ms_sum = c->lastLoopKernelMs;
+    if (iters) *iters = c->lastLoopIters;
+    return MBAR_B200_OK;
+}
+
+}  // extern "C"

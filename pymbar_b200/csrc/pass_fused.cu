@@ -782,8 +782,8 @@ bool fused_applicable(const mbar_b200_ctx* ctx, const double* h_f, bool allState
 // Configure the fused kernel for f (host) and stage c = f + log N - mid on the device.
 int fused_prepare(mbar_b200_ctx* ctx, const double* h_f, bool wantL, bool allStates, FusedParams* out,
                   bool* ok, double* d_cdst, double* h_stage, bool wantW, int M, double midQuantum) {
-    if (!d_cdst) d_cdst = ctx->d_c;
-    if (!h_stage) h_stage = ctx->h_f;
+    if (!d_cdst) d_cdst = ctx->dc(ROW_C);
+    if (!h_stage) h_stage = ctx->hf(ROW_C);
     *ok = false;
     double mid = 0.0, spread = 0.0;
     if (!fused_applicable(ctx, h_f, allStates, &mid, &spread)) return MBAR_B200_OK;

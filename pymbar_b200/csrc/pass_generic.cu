@@ -214,12 +214,15 @@ pass_generic_kernel(const double* __restrict__ u, int K, int64_t N, int64_t nTil
 int launch_pass_generic(mbar_b200_ctx* ctx, const double* h_f, bool wantL, bool logAll) {
     const int K = ctx->K;
     // c (sampled) and f (all) to the device
+    double* c = ctx->hf(ROW_C);
+    double* f = ctx->hf(ROW_GEN_F);
     for (int k = 0; k < K; ++k) {
         const double fk = h_f[k];
-        ctx->h_f[k] = std::isinf(ctx->h_logNk[k]) ? -1.0e300 : fk + ctx->h_logNk[k];   // (-1e300: not in the denominator)
-        ctx->h_f[K + k] = fk;
+        c[k] = std::isinf(ctx->h_logNk[k]) ? -1.0e300 : fk + ctx->h_logNk[k];   // (-1e300: not in the denominator)
+        f[k] = fk;
     }
-    MBAR_CUDA(cudaMemcpyAsync(ctx->d_c, ctx->h_f, 2 * (size_t)K * sizeof(double), cudaMemcpyHostToDevice,
+    static_assert(ROW_GEN_F == ROW_C + 1, "one copy uploads c and f");
+    MBAR_CUDA(cudaMemcpyAsync(ctx->dc(ROW_C), c, 2 * (size_t)K * sizeof(double), cudaMemcpyHostToDevice,
                               ctx->stream));
     ctx->h2dBytes += 2 * K * 8;
     const size_t perWarp = 32 * 33 * 8 + (size_t)K * 16;
@@ -239,8 +242,8 @@ int launch_pass_generic(mbar_b200_ctx* ctx, const double* h_f, bool wantL, bool 
     snprintf(ctx->lastKernel, sizeof(ctx->lastKernel), "pass_generic_kernel<%s> grid=%lld warps=%d",
              needUnsampled ? "log-domain rows" : "linear rows", (long long)grid, W);
     MBAR_CUDA(cudaEventRecord(ctx->evA, ctx->stream));
-    kern<<<(unsigned)grid, W * 32, smem, ctx->stream>>>(ctx->d_u, K, ctx->N, ctx->nTiles, ctx->d_c,
-                                                       ctx->d_c + K, ctx->d_rowmask,
+    kern<<<(unsigned)grid, W * 32, smem, ctx->stream>>>(ctx->d_u, K, ctx->N, ctx->nTiles, ctx->dc(ROW_C),
+                                                       ctx->dc(ROW_GEN_F), ctx->d_rowmask,
                                                        logAll ? ctx->d_zeromask : ctx->d_rowmask, ctx->d_Nk,
                                                        ctx->d_partial, ctx->d_out, ctx->d_ticket,
                                                        wantL ? ctx->d_L : nullptr, ctx->d_wgt, W);

@@ -81,6 +81,32 @@ def test_sci_device_resident(lib, name):
         np.testing.assert_allclose(f7[s], f_host[s], atol=1e-11)
 
 
+@pytest.mark.parametrize("name", ["small_osc_8x40", "small_empty_state"])
+def test_sci_epilogue_kernel_path_matches_in_kernel_epilogue(lib, name, monkeypatch):
+    """MBAR_B200_NO_FUSED_EPILOGUE=1 takes the path of sharded problems without peer memory (pass, all-reduce,
+    sci_loop_epilogue_kernel) on one GPU: the same f, bit for bit, as the pass kernel's own epilogue."""
+    z = _cases.load(name)
+    u, N = z["u_kn"], z["N_k"].astype(float)
+    K = len(N)
+    f0 = np.zeros(K)
+    with lib.DeviceProblem(u, N) as p:
+        p.set_loop_mode("device", 4)
+        out = {}
+        for epilogue in ("in-kernel", "kernel"):
+            if epilogue == "kernel":
+                monkeypatch.setenv("MBAR_B200_NO_FUSED_EPILOGUE", "1")
+            launches0 = p.counters()["launches"]
+            f_it = p.sci_iterate(f0, 5)
+            launches = p.counters()["launches"] - launches0
+            f_sol, r = p.solve_sci(f0, tol=1e-12, maxiter=5000)
+            out[epilogue] = (f_it, launches, f_sol, r)
+    (f_it, launches, f_sol, r), (g_it, g_launches, g_sol, g_r) = out["in-kernel"], out["kernel"]
+    assert (launches, g_launches) == (5, 10)      # one launch per iteration | pass + epilogue kernel
+    assert g_it.tobytes() == f_it.tobytes()
+    assert r["success"] and g_r["success"] and g_r["iterations"] == r["iterations"]
+    assert g_sol.tobytes() == f_sol.tobytes()
+
+
 def _random_problem(K, N, seed, empty=()):
     u, N_k = ots.oscillators(K, max(1, N // K), seed=seed)
     N_k = N_k.astype(float)
