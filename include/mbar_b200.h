@@ -19,7 +19,15 @@
  *     In HBM it is re-tiled to [N/32][K][32] and shifted per sample (see DESIGN.md "HBM layout");
  *   - states with N_k == 0 are "unsampled": they never enter a denominator and only
  *     mbar_b200_self_consistent_update / mbar_b200_log_W_nk produce values for them, exactly as in
- *     the reference (mbar_solvers.py:1002-1012).
+ *     the reference (mbar_solvers.py:1002-1012);
+ *   - stored range: every sample is shifted by x_n (its lowest sampled-state energy) and stored as
+ *     min(u_kn - x_n, 1e6).  +inf is legal anywhere and has weight exactly 0 (an unsampled state whose
+ *     energies are all +inf gets f = +inf, log W = -inf).  An unsampled or appended state whose energies
+ *     all lie 1e6 - 800 or more above x_n, at least one of them finite, is outside the stored range: the
+ *     entry points that read unsampled rows (self_consistent_update, weight_moments, log_W_nk, bin_moments
+ *     with C / D) return MBAR_B200_ERR_RANGE; the sampled-state entry points are unaffected.  -inf in any
+ *     row is rejected at upload / append with MBAR_B200_ERR_NAN (in a sampled row the sample has "no finite
+ *     energy"; in an unsampled row the reference's f would be -inf).
  */
 #ifndef MBAR_B200_H
 #define MBAR_B200_H
@@ -119,7 +127,9 @@ int mbar_b200_last_pass_ms(mbar_b200_ctx* ctx, double* ms);
  * attached (mbar_b200_comm_init) the uploads and mbar_b200_synthesize are collective: every rank calls them, since
  * the ranks agree on each state's lowest shifted energy, which decides the kernel of all-state passes. */
 int mbar_b200_upload_u_kn(mbar_b200_ctx* ctx, const double* u_host, int64_t ld);
-/* Same, from a row-major DEVICE buffer on ctx's device (e.g. a torch tensor's data_ptr). */
+/* Same, from a row-major DEVICE buffer on ctx's device (e.g. a torch tensor's data_ptr).  Ordered after all work
+ * already submitted to the device, on any stream (it synchronises the device first): a tensor filled
+ * asynchronously just before the call is read complete.  The caller may reuse u_dev once the call returns. */
 int mbar_b200_upload_u_kn_dev(mbar_b200_ctx* ctx, const double* u_dev, int64_t ld);
 /* A new context holding the samples of `base` plus n_extra UNSAMPLED states whose energies are u_extra_host
  * [n_extra, N_local] (row stride ld).  The resident tiles are copied device-to-device; only the new rows cross

@@ -59,19 +59,40 @@ int comm_allreduce(mbar_b200_ctx* ctx, double* d_buf, int count, int op) {
 }
 
 // The lowest shifted energy of every row over all shards (max of its negation), so that every rank makes the same
-// fused / log-domain choice for its all-state passes and issues the same collectives.
+// fused / log-domain choice for its all-state passes and issues the same collectives; likewise the clamp flags (any
+// shard) and the far rows (every shard), so that every rank gives the same all-state answers.
 int agree_row_minima(mbar_b200_ctx* c) {
     if (!c->comm || c->nranks == 1) return MBAR_B200_OK;
     const int K = c->K;
-    std::vector<double> neg(K);
-    for (int k = 0; k < K; ++k) neg[k] = -c->h_urowmin[k];
-    MBAR_CUDA(cudaMemcpyAsync(c->d_scratch, neg.data(), (size_t)K * sizeof(double), cudaMemcpyHostToDevice,
+    std::vector<double> v(3 * (size_t)K);
+    for (int k = 0; k < K; ++k) {
+        v[k] = -c->h_urowmin[k];
+        v[K + k] = c->h_uclamp[k];
+        v[2 * K + k] = 1.0 - c->h_ufar[k];
+    }
+    MBAR_CUDA(cudaMemcpyAsync(c->d_scratch, v.data(), v.size() * sizeof(double), cudaMemcpyHostToDevice,
                               c->stream));
-    MBAR_TRY(comm_allreduce(c, c->d_scratch, K, 2));
-    MBAR_CUDA(cudaMemcpyAsync(neg.data(), c->d_scratch, (size_t)K * sizeof(double), cudaMemcpyDeviceToHost,
+    MBAR_TRY(comm_allreduce(c, c->d_scratch, 3 * K, 2));
+    MBAR_CUDA(cudaMemcpyAsync(v.data(), c->d_scratch, v.size() * sizeof(double), cudaMemcpyDeviceToHost,
                               c->stream));
     MBAR_CUDA(cudaStreamSynchronize(c->stream));
-    for (int k = 0; k < K; ++k) c->h_urowmin[k] = -neg[k];
+    for (int k = 0; k < K; ++k) {
+        c->h_urowmin[k] = -v[k];
+        c->h_uclamp[k] = v[K + k];
+        c->h_ufar[k] = 1.0 - v[2 * K + k];
+    }
+    return MBAR_B200_OK;
+}
+
+// A row stores min(u - x, 1e6), and the passes weigh a stored 1e6 (+inf in the caller's array) e^(c - 1e6) rather than
+// 0.  An unsampled row whose entries all lie at or above U_NEAR_CLAMP, some finite, is answered by those clamped values
+// (f = 1e6 + const where the reference gives 2e6 for a copy u_0 + 2e6): refused.  Sampled rows are exempt: every
+// sample has an entry 0 in some sampled row, so with |c| < 1e6 (check_range) such entries weigh nothing.
+int check_unsampled_clamp(const mbar_b200_ctx* c) {
+    for (int k = 0; k < c->K; ++k)
+        MBAR_REQUIRE(c->h_Nk[k] > 0 || c->h_uclamp[k] == 0.0 || c->h_ufar[k] == 0.0, MBAR_B200_ERR_RANGE,
+                     "unsampled state %d: every energy lies 999200 or more above its sample's lowest sampled-state "
+                     "energy, some finite: beyond the stored range (1e6)", k);
     return MBAR_B200_OK;
 }
 
@@ -110,6 +131,7 @@ int run_pass(mbar_b200_ctx* c, const double* f, PassWant want) {
                  "sharded problem (%d ranks) without a communicator: call mbar_b200_comm_init", c->nranks);
     MBAR_CUDA(cudaSetDevice(c->device));
     MBAR_TRY(check_range(c, f));
+    if (want.unsampled || want.Gall) MBAR_TRY(check_unsampled_clamp(c));
     NvtxRange nvtx_("mbar_b200::pass");
     const int K = c->K;
     const PassLayout lay{K};
@@ -147,7 +169,7 @@ int run_pass(mbar_b200_ctx* c, const double* f, PassWant want) {
         MBAR_CUDA(cudaStreamSynchronize(c->stream));
         c->d2hBytes += (int64_t)lay.size(false) * 8;
         float ms = 0.f;
-        if (cudaEventElapsedTime(&ms, c->evA, c->evB) == cudaSuccess) c->lastPassMs = ms;
+        if (event_ms(c->evA, c->evB, &ms)) c->lastPassMs = ms;
         if (fused && c->h_out[lay.flag()] != 0.0) continue;   // range assumption failed on a sample
         if (fused && needUnsampled) {
             // unsampled states rode along with weight e^-80: valid only while their weight sums are
@@ -175,6 +197,10 @@ int run_pass(mbar_b200_ctx* c, const double* f, PassWant want) {
         if (!underflow) break;
         if (attempt == 0) ++attempt;   // skip the linear generic pass: it would underflow the same way
     }
+    // an unsampled row of +inf only was weighed e^(c - 1e6) per entry; the reference's S is exactly 0 (f = +inf)
+    if (needUnsampled)
+        for (int k = 0; k < K; ++k)
+            if (!(c->h_Nk[k] > 0) && c->h_ufar[k] != 0.0 && c->h_uclamp[k] == 0.0) c->h_out[lay.logS() + k] = -INFINITY;
     if (want.G || want.Gall) {
         NvtxRange nvtxH("mbar_b200::hessian");
         MBAR_TRY(launch_hessian(c, f, want.Gall, fused && wroteW));

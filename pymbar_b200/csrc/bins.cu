@@ -310,6 +310,7 @@ int mbar_b200_bin_moments(mbar_b200_ctx* c, const double* f_k, const double* u_n
     PassWant w;
     w.L = true;
     MBAR_TRY(run_pass(c, f_k, w));
+    if (C || D) MBAR_TRY(check_unsampled_clamp(c));   // C covers every state
     NvtxRange nvtx_("mbar_b200::bin_moments");
     const int K = c->K;
     const int64_t N = c->N, nPad = c->nTiles * TILE_N;
@@ -384,7 +385,7 @@ int mbar_b200_bin_moments(mbar_b200_ctx* c, const double* f_k, const double* u_n
     MBAR_CUDA(cudaMemcpyAsync(&flag, d_flag, sizeof(int), cudaMemcpyDeviceToHost, s));
     MBAR_CUDA(cudaStreamSynchronize(s));
     float ms = 0.f;
-    if (cudaEventElapsedTime(&ms, ev.e[0], ev.e[1]) == cudaSuccess) c->lastBinMs = ms;
+    if (event_ms(ev.e[0], ev.e[1], &ms)) c->lastBinMs = ms;
     c->lastBinChunks = wantC ? momPlan.chunks : 0;
     MBAR_REQUIRE(!(flag & BINF_INVALID), MBAR_B200_ERR_INVALID, "bin_moments: a bin index lies outside [0, %d)",
                  (int)nbins);

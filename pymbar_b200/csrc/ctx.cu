@@ -204,6 +204,28 @@ __device__ __forceinline__ void row_min_push(int* rowMin, double v, int lane) {
     vi = __reduce_min_sync(0xffffffffu, vi);
     if (lane == 0 && vi < 0) atomicMin(rowMin, vi);
 }
+// Per row, from d = u - x before the clamp: a flag when a finite d reaches U_NEAR_CLAMP, and the count of entries at or
+// above U_NEAR_CLAMP, +inf included (a row that counts every sample holds clamped or near-clamp entries only, see
+// h_ufar).  The atomics are issued only by warps that hold such an entry.
+__device__ __forceinline__ void row_clamp_push(int* rowClamp, unsigned long long* rowFar, double d, bool valid,
+                                               int lane) {
+    const unsigned far = __ballot_sync(0xffffffffu, valid && d >= U_NEAR_CLAMP);
+    if (far == 0u) return;
+    const bool finite = __any_sync(0xffffffffu, valid && d >= U_NEAR_CLAMP && d < INFINITY);
+    if (lane == 0) {
+        atomicAdd(rowFar, (unsigned long long)__popc(far));
+        if (finite) atomicOr(rowClamp, 1);
+    }
+}
+
+// Upload flags (d_flag[0]): NaN anywhere; a sample without a finite energy in any sampled state; -inf in an unsampled
+// row (the reference would return f = -inf for that state; the library rejects the input instead)
+enum { BAD_NAN = 1, BAD_NO_FINITE = 2, BAD_NEG_INF = 4 };
+static const char* upload_error(int flags) {
+    return flags & BAD_NAN ? "u_kn contains NaN"
+         : flags & BAD_NO_FINITE ? "a sample has no finite energy in any sampled state"
+                                 : "an unsampled state has an energy of -inf (its free energy would be -inf)";
+}
 
 // ------------------------------------------------------------------------------------------
 // Re-tile + shift kernel.  One CTA (8 warps) per tile; lane = sample, warp w owns rows w, w+8, ...
@@ -213,7 +235,8 @@ __global__ void __launch_bounds__(256) retile_kernel(const double* __restrict__ 
                                                      const unsigned long long* __restrict__ rowmask,
                                                      double* __restrict__ dst,
                                                      double* __restrict__ xshift,
-                                                     int* __restrict__ flags, int* __restrict__ urowmin) {
+                                                     int* __restrict__ flags, int* __restrict__ urowmin,
+                                                     unsigned long long* __restrict__ urowfar) {
     __shared__ double s_min[8][TILE_N];
     __shared__ int s_bad[8];
     const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
@@ -223,16 +246,17 @@ __global__ void __launch_bounds__(256) retile_kernel(const double* __restrict__ 
     const double* colp = src + col;
 
     double mn = INFINITY;
-    int bad = 0;
+    unsigned bad = 0;
     for (int k = warp; k < K; k += 8) {
         double v = valid ? colp[(int64_t)k * ld] : 0.0;
-        if (v != v) bad = 1;
+        if (v != v) bad |= BAD_NAN;
         const bool act = (rowmask[k >> 6] >> (k & 63)) & 1ull;
         if (act) mn = fmin(mn, v);
+        else if (v == -INFINITY) bad |= BAD_NEG_INF;
     }
     s_min[warp][lane] = mn;
-    bad = __any_sync(0xffffffffu, bad);
-    if (lane == 0) s_bad[warp] = bad;
+    bad = __reduce_or_sync(0xffffffffu, bad);
+    if (lane == 0) s_bad[warp] = (int)bad;
     __syncthreads();
     double x = s_min[0][lane];
 #pragma unroll
@@ -242,13 +266,16 @@ __global__ void __launch_bounds__(256) retile_kernel(const double* __restrict__ 
     for (int w = 0; w < 8; ++w) anyBad |= s_bad[w];
     // a sample whose sampled-state energies are all +inf (or contain -inf) has no finite weight
     const bool finiteShift = isfinite(x);
-    if (valid && !finiteShift) anyBad |= 2;
+    // (a per-lane condition: every lane reports its own sample; warp 0 suffices, all warps hold the same x)
+    if (valid && !finiteShift && warp == 0) atomicOr(&flags[0], BAD_NO_FINITE);
     if (!valid || !finiteShift) x = 0.0;
 
     double* out = dst + (tile0 + tileLocal) * (int64_t)K * TILE_N + lane;
     for (int k = warp; k < K; k += 8) {
         double v = valid ? colp[(int64_t)k * ld] : 0.0;
-        v = fmin(v - x, U_CLAMP);
+        const double d = v - x;
+        row_clamp_push(urowmin + K + k, urowfar + k, d, valid, lane);
+        v = fmin(d, U_CLAMP);
         row_min_push(urowmin + k, valid ? v : 0.0, lane);
         out[(int64_t)k * TILE_N] = valid ? v : 0.0;
     }
@@ -261,7 +288,7 @@ int retile_chunk(mbar_b200_ctx* ctx, const double* d_rowmajor, int64_t ldCols, i
     if (nTilesChunk <= 0) return MBAR_B200_OK;
     retile_kernel<<<(unsigned)nTilesChunk, 256, 0, s>>>(d_rowmajor, ldCols, ctx->K, tile0, validCols,
                                                        ctx->d_rowmask, ctx->d_u, ctx->d_xshift,
-                                                       ctx->d_flag, ctx->d_urowmin);
+                                                       ctx->d_flag, ctx->d_urowmin, ctx->d_urowfar);
     ctx->launches++;
     MBAR_CUDA(cudaGetLastError());
     return MBAR_B200_OK;
@@ -354,6 +381,12 @@ int set_weights(mbar_b200_ctx* ctx, const double* w_host) {
     MBAR_CUDA(cudaMemcpyAsync(ctx->d_wgt, w_host, (size_t)ctx->N * sizeof(double), cudaMemcpyHostToDevice,
                               ctx->stream));
     ctx->h2dBytes += ctx->N * 8;
+    return reduce_sumxw(ctx);
+}
+
+// sum_n w_n x_n depends on the shifts: every upload or synthesis into a weighted context recomputes it
+int reduce_sumxw(mbar_b200_ctx* ctx) {
+    if (!ctx->d_wgt) return MBAR_B200_OK;
     const int grid = 256;
     wprep_kernel<<<grid, 256, 0, ctx->stream>>>(ctx->d_wgt, ctx->d_xshift, ctx->N, ctx->d_sqrtw, ctx->d_scratch);
     ctx->launches++;
@@ -405,7 +438,8 @@ __global__ void __launch_bounds__(256) synth_kernel(int K, int64_t N, int64_t nO
                                                     const double* __restrict__ cumN,  // [K+1]
                                                     const unsigned long long* __restrict__ rowmask,
                                                     double* __restrict__ dst,
-                                                    double* __restrict__ xshift, int* __restrict__ urowmin) {
+                                                    double* __restrict__ xshift, int* __restrict__ urowmin,
+                                                    unsigned long long* __restrict__ urowfar) {
     __shared__ double s_min[8][TILE_N];
     const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
     const int64_t tile = blockIdx.x;
@@ -441,7 +475,9 @@ __global__ void __launch_bounds__(256) synth_kernel(int K, int64_t N, int64_t nO
     double* out = dst + tile * (int64_t)K * TILE_N + lane;
     for (int k = warp; k < K; k += 8) {
         const double d = x - O_k[k];
-        const double v = fmin(0.5 * k_k[k] * d * d - sh, U_CLAMP);
+        const double e = 0.5 * k_k[k] * d * d - sh;
+        row_clamp_push(urowmin + K + k, urowfar + k, e, valid, lane);
+        const double v = fmin(e, U_CLAMP);
         row_min_push(urowmin + k, valid ? v : 0.0, lane);
         out[(int64_t)k * TILE_N] = valid ? v : 0.0;
     }
@@ -466,7 +502,7 @@ int launch_synth(mbar_b200_ctx* ctx, const mbar_b200_synth* spec) {
                               ctx->stream));
     synth_kernel<<<(unsigned)ctx->nTiles, 256, 0, ctx->stream>>>(
         K, ctx->N, spec->n_offset, spec->seed, d, d + K, d + 2 * K, ctx->d_rowmask, ctx->d_u,
-        ctx->d_xshift, ctx->d_urowmin);
+        ctx->d_xshift, ctx->d_urowmin, ctx->d_urowfar);
     ctx->launches++;
     MBAR_CUDA(cudaGetLastError());
     MBAR_CUDA(cudaStreamSynchronize(ctx->stream));
@@ -636,8 +672,11 @@ int mbar_b200_create(mbar_b200_ctx** out, int device, int32_t K, int64_t N_local
     ALLOC(c->d_out, (size_t)lay.size(true) * sizeof(double));
     ALLOC(c->d_ticket, 4 * sizeof(unsigned int));
     ALLOC(c->d_flag, 4 * sizeof(int));
-    ALLOC(c->d_urowmin, (size_t)K * sizeof(int));
+    ALLOC(c->d_urowmin, 2 * (size_t)K * sizeof(int));
+    ALLOC(c->d_urowfar, (size_t)K * sizeof(unsigned long long));
     c->h_urowmin.assign(K, 0.0);
+    c->h_uclamp.assign(K, 0.0);
+    c->h_ufar.assign(K, 0.0);
     ALLOC(c->d_f, (size_t)K * sizeof(double));
     ALLOC(c->d_scratch, (scratch_rendezvous(K) + 1024) * sizeof(double));
     ALLOC(c->d_loop, sizeof(mbar::LoopState));
@@ -688,7 +727,8 @@ int mbar_b200_create(mbar_b200_ctx** out, int device, int32_t K, int64_t N_local
     CREATE_CUDA(cudaMemset(c->d_onesmask, 0xff, mask.size() * sizeof(unsigned long long)));
     CREATE_CUDA(cudaMemset(c->d_ticket, 0, 4 * sizeof(unsigned int)));
     CREATE_CUDA(cudaMemset(c->d_flag, 0, 4 * sizeof(int)));
-    CREATE_CUDA(cudaMemset(c->d_urowmin, 0, (size_t)K * sizeof(int)));
+    CREATE_CUDA(cudaMemset(c->d_urowmin, 0, 2 * (size_t)K * sizeof(int)));
+    CREATE_CUDA(cudaMemset(c->d_urowfar, 0, (size_t)K * sizeof(unsigned long long)));
 #undef CREATE_CUDA
     *out = c;
     return MBAR_B200_OK;
@@ -721,7 +761,7 @@ int mbar_b200_destroy(mbar_b200_ctx* c) {
     }
     cudaFree(c->d_xshift); cudaFree(c->d_wgt); cudaFree(c->d_sqrtw); cudaFree(c->d_c); cudaFree(c->d_Nk); cudaFree(c->d_NkEff);
     cudaFree(c->d_rowmask); cudaFree(c->d_zeromask); cudaFree(c->d_onesmask); cudaFree(c->d_partial); cudaFree(c->d_out); cudaFree(c->d_L);
-    cudaFree(c->d_W); cudaFree(c->d_ticket); cudaFree(c->d_flag); cudaFree(c->d_urowmin); cudaFree(c->d_f);
+    cudaFree(c->d_W); cudaFree(c->d_ticket); cudaFree(c->d_flag); cudaFree(c->d_urowmin); cudaFree(c->d_urowfar); cudaFree(c->d_f);
     cudaFree(c->d_scratch);
     cudaFree(c->d_loop); cudaFree(c->d_av); cudaFree(c->d_outM); cudaFree(c->d_A); cudaFree(c->d_active);
     cudaFree(c->d_seq); cudaFree(c->d_Wt);
@@ -801,8 +841,7 @@ int mbar_b200_last_pass_ms(mbar_b200_ctx* c, double* ms) {
     // launched it)
     cudaSetDevice(c->device);
     float t = 0.f;
-    if (c->stream && cudaStreamSynchronize(c->stream) == cudaSuccess &&
-        cudaEventElapsedTime(&t, c->evA, c->evB) == cudaSuccess)
+    if (c->stream && cudaStreamSynchronize(c->stream) == cudaSuccess && event_ms(c->evA, c->evB, &t))
         c->lastPassMs = t;
     else
         cudaGetLastError();
@@ -835,16 +874,30 @@ static int ensure_staging(mbar_b200_ctx* c, bool needPinned) {
     return MBAR_B200_OK;
 }
 
-// Row minima of the shifted energies written by the last upload: to the host, agreed over the shards (the upload is
-// collective once a communicator is attached), device accumulators reset for the next upload.
+static int reset_row_stats(mbar_b200_ctx* c) {
+    MBAR_CUDA(cudaMemset(c->d_urowmin, 0, 2 * (size_t)c->K * sizeof(int)));
+    MBAR_CUDA(cudaMemset(c->d_urowfar, 0, (size_t)c->K * sizeof(unsigned long long)));
+    return MBAR_B200_OK;
+}
+
+// Row minima, clamp flags and far rows of the shifted energies written by the last upload: to the host, agreed
+// over the shards (the upload is collective once a communicator is attached), device accumulators reset.
 static int collect_row_minima(mbar_b200_ctx* c) {
-    std::vector<int> m(c->K);
-    MBAR_CUDA(cudaMemcpy(m.data(), c->d_urowmin, (size_t)c->K * sizeof(int), cudaMemcpyDeviceToHost));
-    MBAR_CUDA(cudaMemset(c->d_urowmin, 0, (size_t)c->K * sizeof(int)));
-    for (int k = 0; k < c->K; ++k) c->h_urowmin[k] = (double)m[k];
+    std::vector<int> m(2 * (size_t)c->K);
+    std::vector<unsigned long long> far(c->K);
+    MBAR_CUDA(cudaMemcpy(m.data(), c->d_urowmin, m.size() * sizeof(int), cudaMemcpyDeviceToHost));
+    MBAR_CUDA(cudaMemcpy(far.data(), c->d_urowfar, far.size() * sizeof(unsigned long long), cudaMemcpyDeviceToHost));
+    MBAR_TRY(reset_row_stats(c));
+    for (int k = 0; k < c->K; ++k) {
+        c->h_urowmin[k] = (double)m[k];
+        c->h_uclamp[k] = (double)m[c->K + k];
+        c->h_ufar[k] = far[k] == (unsigned long long)c->N ? 1.0 : 0.0;
+    }
     return agree_row_minima(c);
 }
 
+// After the copies of an upload or a synthesis: on success the sums over the new shifts and the row minima; on a
+// rejected input every accumulator is reset, so the next upload starts from the state of a fresh context.
 static int finish_upload(mbar_b200_ctx* c) {
     int flags[4];
     MBAR_CUDA(cudaStreamSynchronize(c->copyStream));
@@ -852,12 +905,13 @@ static int finish_upload(mbar_b200_ctx* c) {
     MBAR_CUDA(cudaMemcpy(flags, c->d_flag, sizeof(flags), cudaMemcpyDeviceToHost));
     if (flags[0]) {
         MBAR_CUDA(cudaMemset(c->d_flag, 0, 4 * sizeof(int)));
+        MBAR_TRY(reset_row_stats(c));
         c->ready = false;
-        set_error(flags[0] & 1 ? "u_kn contains NaN"
-                               : "a sample has no finite energy in any sampled state");
+        set_error("%s", upload_error(flags[0]));
         return MBAR_B200_ERR_NAN;
     }
     MBAR_TRY(reduce_sumx(c));
+    MBAR_TRY(reduce_sumxw(c));
     MBAR_TRY(collect_row_minima(c));
     c->ready = true;
     return MBAR_B200_OK;
@@ -951,22 +1005,27 @@ __global__ void __launch_bounds__(256) append_rows_kernel(const double* __restri
                                                           int K, int Knew, int64_t tile0, int64_t validCols,
                                                           const double* __restrict__ xshift,
                                                           double* __restrict__ dst, int* __restrict__ flags,
-                                                          int* __restrict__ urowmin) {
+                                                          int* __restrict__ urowmin,
+                                                          unsigned long long* __restrict__ urowfar) {
     const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
     const int64_t tl = blockIdx.x;
     const int64_t col = tl * TILE_N + lane;
     const bool valid = col < validCols;
     const double x = xshift[(tile0 + tl) * TILE_N + lane];
     double* out = dst + (tile0 + tl) * (int64_t)Knew * TILE_N + (int64_t)K * TILE_N + lane;
-    int bad = 0;
+    unsigned bad = 0;
     for (int r = warp; r < E; r += 8) {
         double v = valid ? stage[(int64_t)r * ldCols + col] : 0.0;
-        if (v != v) bad = 1;
-        v = fmin(v - x, U_CLAMP);
+        if (v != v) bad |= BAD_NAN;
+        if (v == -INFINITY) bad |= BAD_NEG_INF;
+        const double d = v - x;
+        row_clamp_push(urowmin + Knew + K + r, urowfar + K + r, d, valid, lane);
+        v = fmin(d, U_CLAMP);
         row_min_push(urowmin + K + r, valid ? v : 0.0, lane);
         out[(int64_t)r * TILE_N] = valid ? v : 0.0;
     }
-    if (__any_sync(0xffffffffu, bad) && lane == 0) atomicOr(&flags[0], 1);
+    bad = __reduce_or_sync(0xffffffffu, bad);
+    if (bad && lane == 0) atomicOr(&flags[0], (int)bad);
 }
 
 int mbar_b200_create_augmented(mbar_b200_ctx* base, int32_t n_extra, const double* u_extra_host, int64_t ld,
@@ -1051,7 +1110,8 @@ int mbar_b200_create_augmented(mbar_b200_ctx* base, int32_t n_extra, const doubl
         c->h2dBytes += (int64_t)w * E * 8;
         const int64_t nT = (w + TILE_N - 1) / TILE_N;
         append_rows_kernel<<<(unsigned)nT, 256, 0, c->stream>>>(d_stage, cols, E, K, Kn, n0 / TILE_N, w,
-                                                              c->d_xshift, c->d_u, c->d_flag, c->d_urowmin);
+                                                              c->d_xshift, c->d_u, c->d_flag, c->d_urowmin,
+                                                              c->d_urowfar);
         c->launches++;
         if (pinned) cudaStreamSynchronize(c->stream);   // one device staging block: consume before refilling
     }
@@ -1063,15 +1123,26 @@ int mbar_b200_create_augmented(mbar_b200_ctx* base, int32_t n_extra, const doubl
     AUG_CUDA(cudaMemcpy(flags, c->d_flag, sizeof(flags), cudaMemcpyDeviceToHost));
     AUG_CUDA(cudaMemset(c->d_flag, 0, 4 * sizeof(int)));
     if (flags[0]) {
-        set_error("appended energies contain NaN");
+        set_error(flags[0] & BAD_NAN ? "appended energies contain NaN"
+                                     : "an appended state has an energy of -inf (its free energy would be -inf)");
         return fail(MBAR_B200_ERR_NAN);
     }
     {
-        std::vector<int> m(E);
-        AUG_CUDA(cudaMemcpy(m.data(), c->d_urowmin + K, (size_t)E * sizeof(int), cudaMemcpyDeviceToHost));
-        AUG_CUDA(cudaMemset(c->d_urowmin, 0, (size_t)Kn * sizeof(int)));
-        for (int k = 0; k < K; ++k) c->h_urowmin[k] = base->h_urowmin[k];
-        for (int r = 0; r < E; ++r) c->h_urowmin[K + r] = (double)m[r];
+        std::vector<int> m(2 * (size_t)Kn);
+        std::vector<unsigned long long> far(Kn);
+        AUG_CUDA(cudaMemcpy(m.data(), c->d_urowmin, m.size() * sizeof(int), cudaMemcpyDeviceToHost));
+        AUG_CUDA(cudaMemcpy(far.data(), c->d_urowfar, far.size() * sizeof(unsigned long long), cudaMemcpyDeviceToHost));
+        if (reset_row_stats(c) != MBAR_B200_OK) return fail(MBAR_B200_ERR_CUDA);
+        for (int k = 0; k < K; ++k) {
+            c->h_urowmin[k] = base->h_urowmin[k];
+            c->h_uclamp[k] = base->h_uclamp[k];
+            c->h_ufar[k] = base->h_ufar[k];
+        }
+        for (int r = 0; r < E; ++r) {
+            c->h_urowmin[K + r] = (double)m[K + r];
+            c->h_uclamp[K + r] = (double)m[Kn + K + r];
+            c->h_ufar[K + r] = far[K + r] == (unsigned long long)c->N ? 1.0 : 0.0;
+        }
     }
     if (base->d_wgt) {
         // bootstrap multiplicities travel with the samples
@@ -1092,6 +1163,9 @@ int mbar_b200_upload_u_kn_dev(mbar_b200_ctx* c, const double* u_dev, int64_t ld)
     MBAR_REQUIRE(c && u_dev, MBAR_B200_ERR_INVALID, "NULL argument");
     MBAR_REQUIRE(ld >= c->N, MBAR_B200_ERR_INVALID, "ld=%lld < N_local", (long long)ld);
     MBAR_CUDA(cudaSetDevice(c->device));
+    // the context's stream does not wait for the legacy default stream (it is non-blocking), which is where torch
+    // writes a tensor unless told otherwise: finish all prior work on the device before the re-tile reads u_dev
+    MBAR_CUDA(cudaDeviceSynchronize());
     MBAR_TRY(retile_chunk(c, u_dev, ld, 0, c->nTiles, c->N, c->stream));
     return finish_upload(c);
 }
@@ -1101,6 +1175,7 @@ int mbar_b200_synthesize(mbar_b200_ctx* c, const mbar_b200_synth* spec) {
     MBAR_CUDA(cudaSetDevice(c->device));
     MBAR_TRY(launch_synth(c, spec));
     MBAR_TRY(reduce_sumx(c));
+    MBAR_TRY(reduce_sumxw(c));
     MBAR_TRY(collect_row_minima(c));
     c->ready = true;
     return MBAR_B200_OK;

@@ -15,6 +15,10 @@ namespace mbar {
 
 constexpr int TILE_N = 32;              // samples per tile (one warp lane each)
 constexpr double U_CLAMP = 1.0e6;       // shifted energies are clamped to [.., 1e6] at upload
+// +inf and everything past 1e6 are stored as U_CLAMP and weighed e^(c - 1e6) by the passes.  In a row with an entry
+// below U_NEAR_CLAMP such entries are negligible next to it (e^-800 each), as in the reference; a row with none has
+// only clamped or near-clamp entries, which decide its answer (h_ufar, h_uclamp).
+constexpr double U_NEAR_CLAMP = U_CLAMP - 800.0;
 constexpr double C_RANGE = 1.0e6;       // |f_k + log N_k| must stay below this
 constexpr double FUSED_SPREAD = 1200.0; // fused kernel needs max(c) - min(c) below this
 constexpr int MAX_GRID = 132 * 4;
@@ -117,7 +121,14 @@ struct mbar_b200_ctx {
     // [K] min over samples of each row's shifted energy u'_kn, rounded down, 0 when none is negative (only
     // unsampled rows can be): bounds the exp argument an unsampled row presents to the fused pass
     std::vector<double> h_urowmin;
-    int* d_urowmin = nullptr;       // [K] the same, accumulated on the device during upload / append
+    // [K] 1 where some sample's FINITE shifted energy reached U_NEAR_CLAMP (on any shard)
+    std::vector<double> h_uclamp;
+    // [K] 1 where every shifted energy of the row is at or above U_NEAR_CLAMP, +inf included (on every shard).  An
+    // unsampled row with both flags cannot be answered (ERR_RANGE, check_unsampled_clamp); with this one alone it is
+    // all +inf: S = 0, f = +inf
+    std::vector<double> h_ufar;
+    int* d_urowmin = nullptr;       // [2K] the row minima, then the clamp flags, accumulated during upload / append
+    unsigned long long* d_urowfar = nullptr;  // [K] entries per row at or above U_NEAR_CLAMP (+inf included)
     std::vector<int> active;        // indices of sampled states
     int firstActive = 0;
     double N_total_states = 0;      // sum_k N_k (global N)
@@ -289,9 +300,12 @@ int launch_logw(mbar_b200_ctx* ctx, const double* h_f, double* logW_host, int64_
 int launch_synth(mbar_b200_ctx* ctx, const mbar_b200_synth* spec);
 int launch_untile(mbar_b200_ctx* ctx, int64_t n0, int64_t n, double* d_dst, int64_t ld);
 int comm_allreduce(mbar_b200_ctx* ctx, double* d_buf, int count, int op /*0 sum, 2 max*/);
-// h_urowmin made identical on every rank (collective; a no-op without a communicator)
+// h_urowmin and h_uclamp made identical on every rank (collective; a no-op without a communicator)
 int agree_row_minima(mbar_b200_ctx* ctx);
+// ERR_RANGE when an unsampled row holds a clamped finite energy (h_uclamp): for entry points that read those rows
+int check_unsampled_clamp(const mbar_b200_ctx* ctx);
 int reduce_sumx(mbar_b200_ctx* ctx);
+int reduce_sumxw(mbar_b200_ctx* ctx);   // sum_n w_n x_n with the current shifts (no-op without multiplicities)
 int set_weights(mbar_b200_ctx* ctx, const double* w_host);
 int probe_exp_launch(int which, int64_t n, const double* d_a, double* d_out);   // mbar_b200_probe_exp
 
@@ -406,6 +420,14 @@ __host__ __device__ __forceinline__ double rel_change(double a, double b, double
     double div = fabs(ref);
     if (div < thr) div = 1.0;
     return fabs(a - b) / div;
+}
+
+// Elapsed ms between two events.  False when either was never recorded (e.g. no pass has run yet); the runtime's
+// error is then cleared, or the next MBAR_CUDA(cudaGetLastError()) of an unrelated call would report it.
+inline bool event_ms(cudaEvent_t a, cudaEvent_t b, float* ms) {
+    if (cudaEventElapsedTime(ms, a, b) == cudaSuccess) return true;
+    cudaGetLastError();
+    return false;
 }
 
 // d_scratch holds K*K + 4K + 1024 doubles of call-local scratch; the rendezvous all-reduce of the device-resident

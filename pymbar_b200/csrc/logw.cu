@@ -50,6 +50,7 @@ int launch_logw(mbar_b200_ctx* ctx, const double* h_f, double* logW_host, int64_
                 int64_t n) {
     const int K = ctx->K;
     MBAR_REQUIRE(ctx->d_L, MBAR_B200_ERR_NOT_READY, "log_W: per-sample L not available");
+    MBAR_TRY(check_unsampled_clamp(ctx));
     MBAR_REQUIRE(n0 >= 0 && n >= 1 && n0 + n <= ctx->N && n0 % TILE_N == 0, MBAR_B200_ERR_INVALID,
                  "log_W rows [%lld, +%lld): n0 must be a multiple of 32 inside [0, N)", (long long)n0, (long long)n);
     NvtxRange nvtx_("mbar_b200::log_W download");

@@ -398,7 +398,7 @@ struct Events {
     }
     float ms(size_t a, size_t b) const {
         float m = 0.f;
-        cudaEventElapsedTime(&m, ev[a], ev[b]);
+        event_ms(ev[a], ev[b], &m);
         return m;
     }
     int start(cudaStream_t stream) {
@@ -1082,7 +1082,7 @@ int mbar_b200_sci_iterate(mbar_b200_ctx* c, double* f, int32_t iters) {
     MBAR_CUDA(cudaStreamSynchronize(c->stream));
     c->d2hBytes += K * 8 + lay.size(false) * 8;
     float ms = 0.f;
-    if (cudaEventElapsedTime(&ms, c->evA, c->evB) == cudaSuccess) c->lastPassMs = ms;
+    if (event_ms(c->evA, c->evB, &ms)) c->lastPassMs = ms;   // (no pass has run on a fresh context with iters = 0)
     MBAR_REQUIRE(!(iters > 0 && c->h_out[lay.flag()] >= 1.0e6), MBAR_B200_ERR_COMM,
                  "peer exchange timed out inside the pass kernel (a rank did not arrive)");
     if (p.debugSkip) return MBAR_B200_OK;   // memory-pipeline probe: the arithmetic was skipped, nothing to return
