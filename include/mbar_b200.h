@@ -200,6 +200,38 @@ int mbar_b200_log_denominator(mbar_b200_ctx* ctx, const double* f_k, double* L_h
 int mbar_b200_bin_moments(mbar_b200_ctx* ctx, const double* f_k, const double* u_n, const int32_t* bin_n,
                           int32_t nbins, double* f_bin, double* C, double* D);
 
+/* ---- kernel-density sums (pymbar FES with fes_type="kde", independent of any u_kn context) ------ */
+/* For the resident samples x_n in R^D with weights w_n >= 0 and query points y_q:
+ *   out[q] = log sum_n w_n k(d_qn / h),   d_qn = sqrt(sum_{j<D} (y_qj - x_nj)^2),
+ * the unnormalised log kernel sum behind sklearn's KernelDensity.score_samples (fes.py:1566): the caller adds the
+ * kernel's normalisation and subtracts log sum_n w_n.  The log-kernels are sklearn's: gaussian -d^2/(2h^2),
+ * exponential -d/h; tophat 0, epanechnikov log(1 - d^2/h^2), linear log(1 - d/h), cosine log cos(pi d / (2h)), each
+ * for d < h only, with d the correctly rounded square root of the rounded squares summed in dimension order, as
+ * sklearn computes it.  out[q] is finite whenever some w_n k > 0, however far below the fp64 range the linear sum
+ * lies, and -inf when none is.  A query's result depends only on it and the samples (not on Q or the other queries),
+ * and repeat calls are bit-identical. */
+typedef enum mbar_b200_kde_kernel {
+    MBAR_B200_KDE_GAUSSIAN = 0,
+    MBAR_B200_KDE_TOPHAT = 1,
+    MBAR_B200_KDE_EPANECHNIKOV = 2,
+    MBAR_B200_KDE_EXPONENTIAL = 3,
+    MBAR_B200_KDE_LINEAR = 4,
+    MBAR_B200_KDE_COSINE = 5
+} mbar_b200_kde_kernel;
+typedef struct mbar_b200_kde mbar_b200_kde;
+/* Upload N samples x_host [N, D] row-major and their weights w_host [N] once.  D outside 1..4, a negative, NaN or
+ * infinite weight, or weights that sum to 0 -> MBAR_B200_ERR_INVALID; a NaN or infinite coordinate ->
+ * MBAR_B200_ERR_NAN. */
+int mbar_b200_kde_create(int device, int64_t N, int32_t D, const double* x_host, const double* w_host,
+                         mbar_b200_kde** out);
+int mbar_b200_kde_destroy(mbar_b200_kde* kde);
+/* out [Q] for the queries y_host [Q, D] row-major.  An unknown kernel (mbar_b200_kde_kernel), or h <= 0 or not finite
+ * -> MBAR_B200_ERR_INVALID; a NaN or infinite query coordinate -> MBAR_B200_ERR_NAN.  A failed call leaves the object
+ * usable. */
+int mbar_b200_kde_log_sum(mbar_b200_kde* kde, int32_t kernel, double h, int64_t Q, const double* y_host, double* out);
+/* CUDA-event time of the kernels of the last mbar_b200_kde_log_sum and the number of sample chunks they split N into. */
+int mbar_b200_last_kde_stats(mbar_b200_kde* kde, double* ms, int32_t* chunks);
+
 /* ---- native solver loops (no Python between iterations) ------------------------------------- */
 /* Plain self-consistent iteration f <- f - log S(f), gauge f[first sampled] = 0 each step, until
  * max |delta f / f| < tol (the convergence rule of mbar_solvers.py:627-640) or maxiter. */

@@ -70,6 +70,10 @@ SIGNATURES = {
     "mbar_b200_log_W_nk_rows": (C.c_int, [_ctx, _dp, C.c_int64, C.c_int64, C.c_void_p, C.c_int64, C.c_int]),
     "mbar_b200_log_denominator": (C.c_int, [_ctx, _dp, _dp]),
     "mbar_b200_bin_moments": (C.c_int, [_ctx, _dp, _dp, C.POINTER(C.c_int32), C.c_int32, _dp, _dp, _dp]),
+    "mbar_b200_kde_create": (C.c_int, [C.c_int, C.c_int64, C.c_int32, _dp, _dp, C.POINTER(_ctx)]),
+    "mbar_b200_kde_destroy": (C.c_int, [_ctx]),
+    "mbar_b200_kde_log_sum": (C.c_int, [_ctx, C.c_int32, C.c_double, C.c_int64, _dp, _dp]),
+    "mbar_b200_last_kde_stats": (C.c_int, [_ctx, _dp, C.POINTER(C.c_int32)]),
     "mbar_b200_solve_sci": (C.c_int, [_ctx, _dp, C.c_double, C.c_int32, C.POINTER(SolveResult)]),
     "mbar_b200_solve_adaptive": (C.c_int, [_ctx, _dp, C.c_double, C.c_int32, C.c_int32, C.c_double,
                                            C.POINTER(SolveResult)]),

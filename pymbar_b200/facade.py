@@ -27,8 +27,13 @@ the original method, which then reads `self.Log_W_nk` and materialises it.  `uni
 from the device and, for fes_type="histogram", builds the bin free energies with `pymbar_b200.fes.histogram_fes`;
 `FES.w_kn` (np.exp(mbar.Log_W_nk), fes.py:416) becomes lazy like `Log_W_nk`.  `_get_fes_histogram` with
 `uncertainty_method="analytical"` takes Theta from `pymbar_b200.fes.histogram_theta` (K x nbins moments on the
-device) instead of the N x (K + nbins) augmented weight matrix (fes.py:1382-1406).  FES bootstraps, KDE / spline
-uncertainties, and any call whose weights leave the device's range contract go to the original methods.
+device) instead of the N x (K + nbins) augmented weight matrix (fes.py:1382-1406).
+
+For fes_type="kde" (sklearn parameters the device serves, `pymbar_b200.fes.kde_settings`) `generate_fes` uploads x_n
+and w_n to a `DeviceKde` instead of fitting sklearn's tree, and `_get_fes_kde` without uncertainties answers from
+it (`pymbar_b200.fes.kde_query`).  `FES.kde` becomes lazy: the first read by anything else (`get_kde()`, the original
+methods) fits it exactly as fes.py:696 does.  FES bootstraps, bootstrap uncertainties, spline fits, device errors
+and any call whose weights leave the device's range contract go to the original methods.
 """
 from __future__ import annotations
 
@@ -42,7 +47,7 @@ from . import estimators as est
 _TLS = threading.local()
 _SAVED = {}
 STATS = {"tickets": 0, "redeemed": 0, "moments": 0, "expectations": 0, "log_weights": 0, "fes_histograms": 0,
-         "fes_theta": 0, "fes_w_kn": 0}
+         "fes_theta": 0, "fes_w_kn": 0, "fes_kde_fits": 0, "fes_kde_queries": 0}
 
 
 class LogWeightTicket:
@@ -218,18 +223,57 @@ def _out_of_range(err):
     return isinstance(err, _lib.MbarB200Error) and err.status == -6     # MBAR_B200_ERR_RANGE
 
 
+def _drop_device_kde(fes):
+    dev = fes.__dict__.pop("_b200_kde_dev", None)
+    if dev is not None and hasattr(dev[0], "close"):
+        dev[0].close()
+
+
+def _device_kde(fes, x_n):
+    """The KDE of fes.py:650-699 (b = 0) for the device: upload x_n and fes.w_n to a DeviceKde and leave FES.kde
+    unfitted until something reads it.  False when the device does not serve these parameters or cannot take the
+    samples; the caller then fits sklearn's tree as the reference does."""
+    from . import _lib
+    from . import fes as hist
+    from . import mbar_solvers as ms
+
+    if np.ndim(x_n) == 1 and not hasattr(x_n, "reshape"):
+        return False                    # fes.py:677 reshapes 1-D samples with x_n.reshape: let the original raise
+    x = np.asarray(x_n)
+    if x.ndim == 1:
+        x = x.reshape(-1, 1)
+    kde = fes.__dict__.get("_b200_kde")
+    if x.ndim != 2 or not hasattr(kde, "get_params"):
+        return False
+    settings = hist.kde_settings(kde.get_params(), x.shape[0], x.shape[1])
+    if settings is None:
+        return False
+    w = fes.w_n
+    try:
+        dev = ms.DeviceKde(x, w, device=ms._DEVICE)
+    except (_lib.MbarB200Error, ValueError, TypeError):
+        return False
+    fes.__dict__["_b200_kde_dev"] = (dev, settings, float(np.log(np.sum(w))))
+    fes.__dict__["_b200_kde_fit"] = (x_n if np.ndim(x_n) != 1 else x, w)
+    return True
+
+
 def install_fes_on(FES):
     """Patch the class object `FES` (pymbar.fes.FES)."""
     if FES in _SAVED:
         return
-    saved = {name: FES.__dict__.get(name) for name in ("generate_fes", "_get_fes_histogram", "w_kn")}
+    saved = {name: FES.__dict__.get(name) for name in ("generate_fes", "_get_fes_histogram", "w_kn", "_get_fes_kde",
+                                                         "kde")}
     _SAVED[FES] = saved
     orig_generate = saved["generate_fes"]
     orig_get_hist = saved["_get_fes_histogram"]
+    orig_get_kde = saved["_get_fes_kde"]
 
     def generate_fes(self, u_n, x_n, fes_type="histogram", histogram_parameters=None, kde_parameters=None,
                      spline_parameters=None, n_bootstraps=0, seed=-1):
         args = (u_n, x_n, fes_type, histogram_parameters, kde_parameters, spline_parameters, n_bootstraps, seed)
+        # a DeviceKde answers only for the surface the last generate_fes built
+        _drop_device_kde(self)
         single = isinstance(n_bootstraps, (int, np.integer)) and not isinstance(n_bootstraps, bool) and n_bootstraps == 0
         if not single or fes_type not in ("histogram", "kde", "spline"):
             return orig_generate(self, *args)
@@ -275,7 +319,8 @@ def install_fes_on(FES):
         if fes_type == "histogram":
             self.histogram_data = data
         elif fes_type == "kde":
-            self._generate_fes_kde(0, x_n, self.w_n)
+            if not _device_kde(self, x_n):
+                self._generate_fes_kde(0, x_n, self.w_n)
         else:
             self._generate_fes_spline(0, x_n, self.w_n)
         if timings:
@@ -310,6 +355,38 @@ def install_fes_on(FES):
                                      uncertainty_method=uncertainty_method)
             raise
 
+    def _get_fes_kde(self, x, reference_point="from-normalization", fes_reference=None, uncertainty_method=None):
+        dev = self.__dict__.get("_b200_kde_dev")
+        if dev is not None and uncertainty_method is None:
+            from . import _lib
+            from . import fes as hist
+
+            kde, settings, log_sum_w = dev
+            try:
+                out = hist.kde_query(kde, settings, x, reference_point, fes_reference, log_sum_w)
+            except _lib.MbarB200Error:
+                out = None
+            if out is not None:
+                STATS["fes_kde_queries"] += 1
+                return out
+        return orig_get_kde(self, x, reference_point=reference_point, fes_reference=fes_reference,
+                            uncertainty_method=uncertainty_method)
+
+    def _get_kde(self):
+        try:
+            kde = self.__dict__["_b200_kde"]
+        except KeyError:
+            raise AttributeError(f"{type(self).__name__!r} object has no attribute 'kde'") from None
+        pending = self.__dict__.pop("_b200_kde_fit", None)
+        if pending is not None:
+            STATS["fes_kde_fits"] += 1
+            kde.fit(pending[0], sample_weight=pending[1])
+        return kde
+
+    def _set_kde(self, value):
+        self.__dict__["_b200_kde"] = value
+        self.__dict__.pop("_b200_kde_fit", None)
+
     def _get_w_kn(self):
         v = self.__dict__.get("_b200_w_kn")
         if isinstance(v, WeightMatrixTicket):
@@ -322,6 +399,8 @@ def install_fes_on(FES):
 
     FES.generate_fes = generate_fes
     FES._get_fes_histogram = _get_fes_histogram
+    FES._get_fes_kde = _get_fes_kde
+    FES.kde = property(_get_kde, _set_kde, doc="the sklearn KernelDensity (fes.py:648), fitted on first use")
     FES.w_kn = property(_get_w_kn, _set_w_kn, doc="weights [N, K] of all states (fes.py:416), computed on first use")
 
 

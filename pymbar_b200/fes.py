@@ -1,4 +1,4 @@
-"""Histogram free-energy surfaces from the resident MBAR problem (pymbar.FES with fes_type="histogram").
+"""Free-energy surfaces from the resident MBAR problem: pymbar.FES with fes_type="histogram" and with "kde".
 
 pymbar's FES builds a histogram PMF from the log weights of one target state, log w_n = -u_n - L_n (mbar.py:1919-1934),
 and its analytical uncertainty from the augmented weight matrix W_aug = [W | B] with B_ni = w^_n [bin(n) = i] and
@@ -13,6 +13,11 @@ and everything comes from the resident u_kn plus two O(N) vectors (u_n and a den
 vectorised restatement of fes.py:513-573, quirks included: samples below the grid share the label -1, samples above
 the top edge of a dimension get that dimension's bin count, and both pseudo-bins are bins in their own right.
 The (K + nbins)^2 covariance algebra is the reference's own (estimators.asymptotic_covariance, "svd-ew").
+
+A KDE surface is -score_samples of an sklearn KernelDensity fitted to x_n with the target state's weights w_n
+(fes.py:650-699, :1566).  The N x Q part, l_q = log sum_n w_n k(|y_q - x_n| / h), is DeviceKde.log_sum; this module
+holds sklearn's host algebra around it: the kernel and bandwidth (kde_settings), the kernel normalisation
+(kde_log_norm) and the reference points of _get_fes_kde (kde_query).
 """
 from __future__ import annotations
 
@@ -180,3 +185,140 @@ def query(histogram_data, x, reference_point, fes_reference, df_fn=None):
     if df_fn is not None:
         out["df_i"] = dfx
     return out
+
+
+KDE_KERNELS = ("gaussian", "tophat", "epanechnikov", "exponential", "linear", "cosine")
+_LOG_PI = math.log(math.pi)
+_LOG_2PI = math.log(2 * math.pi)
+
+
+def _log_vn(n):
+    # log volume of the unit n-ball
+    return 0.5 * n * _LOG_PI - math.lgamma(0.5 * n + 1)
+
+
+def _log_sn(n):
+    # log surface of the unit n-sphere
+    return _LOG_2PI + _log_vn(n - 1)
+
+
+def kde_log_norm(kernel, D, h):
+    """log of the normalisation sklearn multiplies its unnormalised kernel sum by (its _log_kernel_norm), for one of
+    KDE_KERNELS in D dimensions at bandwidth h."""
+    if kernel == "gaussian":
+        factor = 0.5 * D * _LOG_2PI
+    elif kernel == "tophat":
+        factor = _log_vn(D)
+    elif kernel == "epanechnikov":
+        factor = _log_vn(D) + math.log(2.0 / (D + 2.0))
+    elif kernel == "exponential":
+        factor = _log_sn(D - 1) + math.lgamma(D)
+    elif kernel == "linear":
+        factor = _log_vn(D) - math.log(D + 1.0)
+    elif kernel == "cosine":
+        factor = 0.0
+        tmp = 2.0 / math.pi
+        for k in range(1, D + 1, 2):
+            factor += tmp
+            tmp *= -(D - k) * (D - k - 1) * (2.0 / math.pi) ** 2
+        # negative for D = 4: sklearn's log then gives NaN, and so does this
+        factor = (math.log(factor) if factor > 0 else math.nan) + _log_sn(D - 1)
+    else:
+        raise ValueError(f"kernel {kernel!r} not recognized")
+    return -factor - D * math.log(h)
+
+
+def _nonnegative_real(v):
+    return isinstance(v, (int, float, np.integer, np.floating)) and not isinstance(v, bool) and v >= 0
+
+
+def kde_settings(params, N, D):
+    """What the device needs of a KernelDensity with parameters `params` (its get_params()) fitted to N samples in
+    D dimensions: {"kernel", "h", "D"}, or None when the device does not serve it (a metric other than euclidean,
+    metric_params, D outside 1..4, or any parameter sklearn's fit would reject, so that the caller's fall-back
+    raises sklearn's own error).  The bandwidth of "scott" / "silverman" is sklearn's, from N and D.
+
+    atol, rtol, algorithm, leaf_size and breadth_first only choose how sklearn's tree approximates the sum: the
+    device sums every pair, an exact answer that lies within the tolerance of any such setting."""
+    kernel = params.get("kernel")
+    bw = params.get("bandwidth")
+    if kernel not in KDE_KERNELS or params.get("metric") != "euclidean" or params.get("metric_params") is not None:
+        return None
+    if not 1 <= D <= 4 or N < 1:
+        return None
+    if not (_nonnegative_real(params.get("atol")) and _nonnegative_real(params.get("rtol"))):
+        return None
+    leaf = params.get("leaf_size")
+    if params.get("algorithm") not in ("auto", "kd_tree", "ball_tree"):
+        return None
+    if not isinstance(params.get("breadth_first"), (bool, np.bool_)):
+        return None
+    if not isinstance(leaf, (int, np.integer)) or isinstance(leaf, bool) or leaf < 1:
+        return None
+    # sklearn KernelDensity.fit: N = X.shape[0] counts every sample, zero weights included
+    if isinstance(bw, str):
+        if bw == "scott":
+            h = N ** (-1 / (D + 4))
+        elif bw == "silverman":
+            h = (N * (D + 2) / 4) ** (-1 / (D + 4))
+        else:
+            return None
+    elif isinstance(bw, (int, float, np.integer, np.floating)) and not isinstance(bw, bool):
+        h = float(bw)
+        if not (math.isfinite(h) and h > 0):
+            return None
+    else:
+        return None
+    return {"kernel": kernel, "h": float(h), "D": int(D)}
+
+
+def _draw_as_sample(kernel, D):
+    """What KernelDensity.sample() does to its caller, without the sample: _get_fes_kde calls it only for its shape
+    (fes.py:1560).  Other kernels than gaussian and tophat raise NotImplementedError there; those two take one
+    uniform and D normals from numpy's global generator."""
+    if kernel not in ("gaussian", "tophat"):
+        raise NotImplementedError()
+    rng = np.random.mtrand._rand
+    rng.uniform(0, 1, size=1)
+    rng.normal(size=(1, D))
+
+
+def kde_query(kde, settings, x, reference_point, fes_reference, log_sum_w):
+    """_get_fes_kde (fes.py:1523-1609) without uncertainties, from kde.log_sum (a DeviceKde): {"f_i", "df_i": None}
+    with f_i = -score_samples(x) relative to the reference point, log_sum_w = log sum_n w_n of the fitted weights.
+
+    "from-specified" evaluates its reference point in the same call as the queries (a query's result does not
+    depend on the others).  Raises what the reference raises: IndexError for 1-D x, NotImplementedError for kernels
+    sklearn cannot sample from, DataError on a dimension mismatch, ParameterError for another reference point."""
+    try:
+        from pymbar.utils import DataError, ParameterError
+    except ImportError:
+        from .utils import ParameterError
+
+        DataError = ParameterError
+    kernel, h, D = settings["kernel"], settings["h"], settings["D"]
+    dims = np.shape(x)[1]
+    _draw_as_sample(kernel, D)
+    if dims != D:
+        raise DataError("query coordinates have inconsistent dimension with the data the FES is fit to.")
+    y = np.asarray(x, dtype=np.float64).reshape(-1, D)
+    Q = len(y)
+    if reference_point == "from-specified":
+        ref = np.asarray(fes_reference, dtype=np.float64).reshape(1, -1)
+        if ref.shape[1] != D:
+            raise ValueError(f"X has {ref.shape[1]} features, but KernelDensity is expecting {D} features as input.")
+        y = np.vstack([y, ref])
+    # sklearn: the tree's log sum, += the kernel's normalisation, -= log of the weight sum
+    score = kde.log_sum(kernel, h, y)
+    score += kde_log_norm(kernel, D, h)
+    score -= log_sum_w
+    f_i = -score[:Q]
+    if reference_point == "from-lowest":
+        f_i = f_i - np.min(f_i)
+    elif reference_point == "from-specified":
+        f_i = f_i - (-score[Q:])
+    elif reference_point == "from-normalization":
+        pass
+    else:
+        raise ParameterError(f"reference point choice {reference_point} for kde is unavailable")
+    return {"f_i": f_i, "df_i": None}

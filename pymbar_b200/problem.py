@@ -369,6 +369,68 @@ class DeviceProblem:
         return f
 
 
+KDE_KERNELS = ("gaussian", "tophat", "epanechnikov", "exponential", "linear", "cosine")   # mbar_b200_kde_kernel
+
+
+class DeviceKde:
+    """Weighted samples x_n [N, D] (D = 1..4) resident on one H100 for kernel-density sums (mbar_b200_kde_*).
+
+    `log_sum(kernel, h, y)` returns l_q = log sum_n w_n k(|y_q - x_n| / h) for the query points y [Q, D], with
+    sklearn's unnormalised kernels; pymbar_b200.fes adds the normalisation.  Independent of any DeviceProblem."""
+
+    def __init__(self, x_n, w_n, device=0):
+        self._lib = _lib.load()
+        self._h = C.c_void_p()
+        x = np.asarray(x_n, dtype=np.float64)
+        if x.ndim == 1:
+            x = x.reshape(-1, 1)
+        if x.ndim != 2:
+            raise ValueError(f"x_n must be [N] or [N, D], got shape {np.shape(x_n)}")
+        x = np.ascontiguousarray(x)
+        w = _f64(w_n, x.shape[0])
+        self.N, self.D = x.shape
+        self.device = int(device)
+        check(self._lib.mbar_b200_kde_create(self.device, self.N, self.D, _dptr(x), _dptr(w), C.byref(self._h)))
+
+    def close(self):
+        if self._h is not None and self._h.value:
+            self._lib.mbar_b200_kde_destroy(self._h)
+            self._h = None
+
+    def __del__(self):
+        try:
+            self.close()
+        except Exception:
+            pass
+
+    def __enter__(self):
+        return self
+
+    def __exit__(self, *exc):
+        self.close()
+
+    def log_sum(self, kernel, h, y):
+        """l_q [Q] for the queries y [Q, D] (or [Q] when D = 1); kernel is a name of KDE_KERNELS or its code."""
+        code = KDE_KERNELS.index(kernel) if isinstance(kernel, str) and kernel in KDE_KERNELS else kernel
+        if isinstance(code, str):
+            code = -1                      # unknown name: the library reports ERR_INVALID
+        y = np.asarray(y, dtype=np.float64)
+        if y.ndim == 1 and self.D == 1:
+            y = y.reshape(-1, 1)
+        if y.ndim != 2 or y.shape[1] != self.D:
+            raise ValueError(f"queries must be [Q, {self.D}], got shape {y.shape}")
+        y = np.ascontiguousarray(y)
+        out = np.empty(y.shape[0])
+        check(self._lib.mbar_b200_kde_log_sum(self._h, int(code), float(h), y.shape[0], _dptr(y), _dptr(out)))
+        return out
+
+    def last_stats(self):
+        """CUDA-event time (ms) of the last log_sum's kernels and the number of sample chunks."""
+        ms, chunks = C.c_double(0), C.c_int32(0)
+        check(self._lib.mbar_b200_last_kde_stats(self._h, C.byref(ms), C.byref(chunks)))
+        return dict(ms=ms.value, chunks=chunks.value)
+
+
 def measure_fp64_peak(device=0):
     """(DMMA TFLOP/s, DFMA TFLOP/s) of this GPU from register-only loops (mbar_b200_measure_fp64_peak)."""
     a, b = C.c_double(0), C.c_double(0)
