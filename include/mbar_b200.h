@@ -232,6 +232,31 @@ int mbar_b200_kde_log_sum(mbar_b200_kde* kde, int32_t kernel, double h, int64_t 
 /* CUDA-event time of the kernels of the last mbar_b200_kde_log_sum and the number of sample chunks they split N into. */
 int mbar_b200_last_kde_stats(mbar_b200_kde* kde, double* ms, int32_t* chunks);
 
+/* ---- B-spline basis sums (pymbar FES with fes_type="spline", independent of any u_kn context) --- */
+/* For the resident samples x_n with weights w_n and state labels s_n, and the nb = n_knots - degree - 1 basis
+ * functions B_i of the knot vector t:
+ *   S_ki = sum_{n: s_n = k} B_i(x_n),   A_i = sum_n w_n B_i(x_n),
+ * the sums that the sample terms of the spline fit's objective, gradient and MC likelihood are linear in
+ * (fes.py:2102-2306, :1954-2010).  B_i(x) is scipy.interpolate.BSpline(t, e_i, degree)(x) with extrapolate=True, bit
+ * for bit: the interval scipy picks (x on a knot, repeated knots, x outside [t_k, t_nb] on the end polynomials) and
+ * its Cox-de Boor arithmetic.  Repeat calls are bit-identical, S and A do not depend on whether the other is asked for
+ * or on earlier knot vectors, and there are no floating-point atomics. */
+typedef struct mbar_b200_bspline mbar_b200_bspline;
+/* Upload N samples x [N], weights w [N] (NULL: no A) and labels s [N] in [0, K) (NULL: no S) once.  A negative, NaN
+ * or infinite weight, or a label outside [0, K) -> MBAR_B200_ERR_INVALID; a NaN or infinite x -> MBAR_B200_ERR_NAN. */
+int mbar_b200_bspline_create(int device, int64_t N, const double* x, const double* w, const int32_t* s, int32_t K,
+                             mbar_b200_bspline** out);
+int mbar_b200_bspline_destroy(mbar_b200_bspline* bspline);
+/* S [K * nb] row-major and A [nb]; either may be NULL.  degree outside 0..7, a non-finite or decreasing knot,
+ * n_knots < 2 (degree + 1), t[degree] = t[nb], nb + n_knots above 13824 (one shared-memory accumulator), or S / A
+ * asked of an object created without labels / weights -> MBAR_B200_ERR_INVALID.  A failed call leaves the object
+ * usable.  When K * nb does not fit one accumulator, further state chunks cover the rest (tiles without a sample of
+ * a chunk's states are skipped). */
+int mbar_b200_bspline_moments(mbar_b200_bspline* bspline, int32_t degree, int64_t n_knots, const double* t, double* S,
+                              double* A);
+/* CUDA-event time of the kernels of the last mbar_b200_bspline_moments and the number of row chunks they took. */
+int mbar_b200_last_bspline_stats(mbar_b200_bspline* bspline, double* ms, int32_t* chunks);
+
 /* ---- native solver loops (no Python between iterations) ------------------------------------- */
 /* Plain self-consistent iteration f <- f - log S(f), gauge f[first sampled] = 0 each step, until
  * max |delta f / f| < tol (the convergence rule of mbar_solvers.py:627-640) or maxiter. */

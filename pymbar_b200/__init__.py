@@ -4,15 +4,16 @@ Public surface:
   * :mod:`pymbar_b200.mbar_solvers` — same names/signatures as ``pymbar.mbar_solvers``;
   * :class:`pymbar_b200.DeviceProblem` — explicit residency handle (one GPU, one shard of samples);
   * :class:`pymbar_b200.DeviceKde` — weighted samples resident for kernel-density sums (FES with fes_type="kde");
+  * :class:`pymbar_b200.DeviceBSpline` — samples resident for B-spline basis sums (FES with fes_type="spline");
   * :func:`pymbar_b200.install` — rebind ``pymbar.mbar_solvers`` so unmodified ``pymbar.MBAR`` uses it.
 
 Everything numerical runs in libmbar_b200.so (C ABI in include/mbar_b200.h).  No CPU fallback.
 """
 from . import _lib
-from .problem import DeviceKde, DeviceProblem, PinnedArray
+from .problem import DeviceBSpline, DeviceKde, DeviceProblem, PinnedArray
 from .utils import ParameterError
 
-__all__ = ["DeviceProblem", "DeviceKde", "PinnedArray", "ParameterError", "install", "uninstall", "trim", "mbar_solvers"]
+__all__ = ["DeviceProblem", "DeviceKde", "DeviceBSpline", "PinnedArray", "ParameterError", "install", "uninstall", "trim", "mbar_solvers"]
 
 _SAVED = {}
 _PATCHED = (

@@ -74,6 +74,11 @@ SIGNATURES = {
     "mbar_b200_kde_destroy": (C.c_int, [_ctx]),
     "mbar_b200_kde_log_sum": (C.c_int, [_ctx, C.c_int32, C.c_double, C.c_int64, _dp, _dp]),
     "mbar_b200_last_kde_stats": (C.c_int, [_ctx, _dp, C.POINTER(C.c_int32)]),
+    "mbar_b200_bspline_create": (C.c_int, [C.c_int, C.c_int64, _dp, _dp, C.POINTER(C.c_int32), C.c_int32,
+                                           C.POINTER(_ctx)]),
+    "mbar_b200_bspline_destroy": (C.c_int, [_ctx]),
+    "mbar_b200_bspline_moments": (C.c_int, [_ctx, C.c_int32, C.c_int64, _dp, _dp, _dp]),
+    "mbar_b200_last_bspline_stats": (C.c_int, [_ctx, _dp, C.POINTER(C.c_int32)]),
     "mbar_b200_solve_sci": (C.c_int, [_ctx, _dp, C.c_double, C.c_int32, C.POINTER(SolveResult)]),
     "mbar_b200_solve_adaptive": (C.c_int, [_ctx, _dp, C.c_double, C.c_int32, C.c_int32, C.c_double,
                                            C.POINTER(SolveResult)]),

@@ -32,8 +32,19 @@ device) instead of the N x (K + nbins) augmented weight matrix (fes.py:1382-1406
 For fes_type="kde" (sklearn parameters the device serves, `pymbar_b200.fes.kde_settings`) `generate_fes` uploads x_n
 and w_n to a `DeviceKde` instead of fitting sklearn's tree, and `_get_fes_kde` without uncertainties answers from
 it (`pymbar_b200.fes.kde_query`).  `FES.kde` becomes lazy: the first read by anything else (`get_kde()`, the original
-methods) fits it exactly as fes.py:696 does.  FES bootstraps, bootstrap uncertainties, spline fits, device errors
-and any call whose weights leave the device's range contract go to the original methods.
+methods) fits it exactly as fes.py:696 does.
+
+For fes_type="spline" with 1-D samples, `generate_fes` makes one pass over x_n on a `DeviceBSpline` for the fit's
+knots: the per-state basis sums S and the weighted sums A (`SplineMoments`).  The fit's sample terms are linear in
+the spline coefficients, so `_bspline_calculate_f`, `_bspline_calculate_g` and `_get_MC_loglikelihood` answer from
+them (`pymbar_b200.fes.spline_objective` / `spline_gradient` / `spline_mc_loglikelihood`) with O(K nb) arithmetic
+and the reference's quadratures, where the reference evaluates the spline on every sample at every step.  They do
+so only for the very x_n and w_n arrays the moments were built from and for splines on the same knots and degree;
+any other call (bootstrap replicates, another x_n passed to `sample_parameter_distribution`, 2-D samples) runs the
+original method.  The optimiser, the Hessian, the information criteria and `_get_fes_spline` stay the reference's.
+
+FES bootstraps, bootstrap uncertainties, device errors and any call whose weights leave the device's range contract
+go to the original methods.
 """
 from __future__ import annotations
 
@@ -47,7 +58,8 @@ from . import estimators as est
 _TLS = threading.local()
 _SAVED = {}
 STATS = {"tickets": 0, "redeemed": 0, "moments": 0, "expectations": 0, "log_weights": 0, "fes_histograms": 0,
-         "fes_theta": 0, "fes_w_kn": 0, "fes_kde_fits": 0, "fes_kde_queries": 0}
+         "fes_theta": 0, "fes_w_kn": 0, "fes_kde_fits": 0, "fes_kde_queries": 0, "fes_spline_moments": 0,
+         "fes_spline_calls": 0}
 
 
 class LogWeightTicket:
@@ -258,22 +270,84 @@ def _device_kde(fes, x_n):
     return True
 
 
+class SplineMoments:
+    """The basis sums of one spline fit: S [K, nb] (or None) and A [nb] (or None) of the samples x_n, weights w_n
+    and state labels, for the knots t and degree k, with their sample terms v (fes.spline_sample_terms).  F_k, the
+    per-state sums of the bias callables, is computed on first use by the MC likelihood."""
+
+    __slots__ = ("x", "w", "labels", "t", "k", "weights", "S", "A", "N_k", "v", "F_k")
+
+    def __init__(self, x, w, labels, t, k, weights, S, A, N):
+        from . import fes as hist
+
+        self.x, self.w, self.labels, self.t, self.k, self.weights, self.S, self.A = x, w, labels, t, k, weights, S, A
+        self.N_k = None if S is None else np.bincount(labels, minlength=S.shape[0])
+        self.v = hist.spline_sample_terms(S, A, weights, N, self.N_k)
+        self.F_k = None
+
+    def serves(self, x_n, w_n, t, k):
+        return x_n is self.x and w_n is self.w and k == self.k and np.array_equal(t, self.t)
+
+
+def _device_spline(fes, x_n):
+    """One DeviceBSpline pass over x_n for the knots of fes.spline_data["bspline"] (after _setup_fes_spline and the
+    device weights); the moments are kept in fes.__dict__["_b200_spline"].  Nothing is kept for 2-D samples, an
+    unknown spline_weights or a device error (NaN samples, labels outside [0, K)): the fit then runs the original
+    methods."""
+    from . import _lib
+    from . import fes as hist
+    from . import mbar_solvers as ms
+
+    weights = fes.spline_parameters.get("spline_weights")
+    if np.ndim(x_n) != 1 or weights not in hist.SPLINE_WEIGHTS:
+        return
+    b = fes.spline_data["bspline"]
+    t, k = np.array(b.t, dtype=np.float64), int(b.k)
+    want_S = weights != "unbiasedstate"
+    K = fes.mbar.K
+    labels = np.asarray(fes.mbar.x_kindices) if want_S else None
+    try:
+        dev = ms.DeviceBSpline(np.asarray(x_n, dtype=np.float64), None if want_S else fes.w_n, labels,
+                               K=K if want_S else None, device=ms._DEVICE)
+        try:
+            S, A = dev.moments(t, k, want_S=want_S, want_A=not want_S)
+        finally:
+            dev.close()
+    except (_lib.MbarB200Error, ValueError, TypeError):
+        return
+    STATS["fes_spline_moments"] += 1
+    fes.__dict__["_b200_spline"] = SplineMoments(x_n, fes.w_n, labels, t, k, weights, S, A, fes.N)
+
+
+def _spline_moments_for(fes, x_n, w_n, t, k, weights):
+    m = fes.__dict__.get("_b200_spline")
+    if m is None or weights != m.weights or not m.serves(x_n, w_n, t, k):
+        return None
+    return m
+
+
 def install_fes_on(FES):
     """Patch the class object `FES` (pymbar.fes.FES)."""
     if FES in _SAVED:
         return
     saved = {name: FES.__dict__.get(name) for name in ("generate_fes", "_get_fes_histogram", "w_kn", "_get_fes_kde",
-                                                         "kde")}
+                                                         "kde", "_bspline_calculate_f", "_bspline_calculate_g",
+                                                         "_get_MC_loglikelihood")}
     _SAVED[FES] = saved
     orig_generate = saved["generate_fes"]
     orig_get_hist = saved["_get_fes_histogram"]
     orig_get_kde = saved["_get_fes_kde"]
+    # the class's own spline methods, or those it inherits
+    orig_spline_f = FES._bspline_calculate_f if hasattr(FES, "_bspline_calculate_f") else None
+    orig_spline_g = FES._bspline_calculate_g if hasattr(FES, "_bspline_calculate_g") else None
+    orig_mc_ll = FES._get_MC_loglikelihood if hasattr(FES, "_get_MC_loglikelihood") else None
 
     def generate_fes(self, u_n, x_n, fes_type="histogram", histogram_parameters=None, kde_parameters=None,
                      spline_parameters=None, n_bootstraps=0, seed=-1):
         args = (u_n, x_n, fes_type, histogram_parameters, kde_parameters, spline_parameters, n_bootstraps, seed)
-        # a DeviceKde answers only for the surface the last generate_fes built
+        # a DeviceKde, or spline moments, answer only for the surface the last generate_fes built
         _drop_device_kde(self)
+        self.__dict__.pop("_b200_spline", None)
         single = isinstance(n_bootstraps, (int, np.integer)) and not isinstance(n_bootstraps, bool) and n_bootstraps == 0
         if not single or fes_type not in ("histogram", "kde", "spline"):
             return orig_generate(self, *args)
@@ -322,6 +396,7 @@ def install_fes_on(FES):
             if not _device_kde(self, x_n):
                 self._generate_fes_kde(0, x_n, self.w_n)
         else:
+            _device_spline(self, x_n)
             self._generate_fes_spline(0, x_n, self.w_n)
         if timings:
             result_vals["timing"] = _timer() - start
@@ -372,6 +447,39 @@ def install_fes_on(FES):
         return orig_get_kde(self, x, reference_point=reference_point, fes_reference=fes_reference,
                             uncertainty_method=uncertainty_method)
 
+    def _fit_moments(self, x_n, w_n):
+        b = self.spline_data["bspline"]
+        return _spline_moments_for(self, x_n, w_n, b.t, b.k, self.spline_parameters.get("spline_weights"))
+
+    def _bspline_calculate_f(self, xi, x_n, w_n):
+        m = _fit_moments(self, x_n, w_n)
+        if m is None:
+            return orig_spline_f(self, xi, x_n, w_n)
+        from . import fes as hist
+
+        STATS["fes_spline_calls"] += 1
+        return hist.spline_objective(self, xi, m.v)
+
+    def _bspline_calculate_g(self, xi, x_n, w_n):
+        m = _fit_moments(self, x_n, w_n)
+        if m is None:
+            return orig_spline_g(self, xi, x_n, w_n)
+        from . import fes as hist
+
+        STATS["fes_spline_calls"] += 1
+        return hist.spline_gradient(self, xi, m.v)
+
+    def _get_MC_loglikelihood(self, x_n, w_n, spline_weights, spline, xrange):
+        m = _spline_moments_for(self, x_n, w_n, spline.t, spline.k, spline_weights)
+        if m is None:
+            return orig_mc_ll(self, x_n, w_n, spline_weights, spline, xrange)
+        from . import fes as hist
+
+        if m.S is not None and m.F_k is None:
+            m.F_k = hist.state_bias_sums(self.spline_parameters["fkbias"], m.x, m.labels, m.S.shape[0])
+        STATS["fes_spline_calls"] += 1
+        return hist.spline_mc_loglikelihood(self, spline, spline_weights, xrange, m.S, m.A, m.F_k, m.N_k)
+
     def _get_kde(self):
         try:
             kde = self.__dict__["_b200_kde"]
@@ -400,6 +508,11 @@ def install_fes_on(FES):
     FES.generate_fes = generate_fes
     FES._get_fes_histogram = _get_fes_histogram
     FES._get_fes_kde = _get_fes_kde
+    if orig_spline_f is not None:
+        FES._bspline_calculate_f = _bspline_calculate_f
+        FES._bspline_calculate_g = _bspline_calculate_g
+    if orig_mc_ll is not None:
+        FES._get_MC_loglikelihood = _get_MC_loglikelihood
     FES.kde = property(_get_kde, _set_kde, doc="the sklearn KernelDensity (fes.py:648), fitted on first use")
     FES.w_kn = property(_get_w_kn, _set_w_kn, doc="weights [N, K] of all states (fes.py:416), computed on first use")
 

@@ -1,4 +1,4 @@
-"""Free-energy surfaces from the resident MBAR problem: pymbar.FES with fes_type="histogram" and with "kde".
+"""Free-energy surfaces from the resident MBAR problem: pymbar.FES with fes_type="histogram", "kde" and "spline".
 
 pymbar's FES builds a histogram PMF from the log weights of one target state, log w_n = -u_n - L_n (mbar.py:1919-1934),
 and its analytical uncertainty from the augmented weight matrix W_aug = [W | B] with B_ni = w^_n [bin(n) = i] and
@@ -18,6 +18,13 @@ A KDE surface is -score_samples of an sklearn KernelDensity fitted to x_n with t
 (fes.py:650-699, :1566).  The N x Q part, l_q = log sum_n w_n k(|y_q - x_n| / h), is DeviceKde.log_sum; this module
 holds sklearn's host algebra around it: the kernel and bandwidth (kde_settings), the kernel normalisation
 (kde_log_norm) and the reference points of _get_fes_kde (kde_query).
+
+A spline surface is fitted by minimising an objective whose sample term is linear in the B-spline coefficients c
+(fes.py:2102-2306): c . A with A_i = sum_n w_n B_i(x_n), or c . S_k per state with S_ki = sum_{n in k} B_i(x_n).
+DeviceBSpline.moments computes S and A in one pass; spline_sample_terms turns them into the term of each weighting,
+and spline_objective / spline_gradient / spline_mc_loglikelihood restate the reference's objective, gradient and MC
+log-likelihood around it with the reference's own quadratures, so that the fit costs O(K nb) arithmetic per step
+instead of a spline evaluation on every sample.
 """
 from __future__ import annotations
 
@@ -322,3 +329,159 @@ def kde_query(kde, settings, x, reference_point, fes_reference, log_sum_w):
     else:
         raise ParameterError(f"reference point choice {reference_point} for kde is unavailable")
     return {"f_i": f_i, "df_i": None}
+
+
+SPLINE_WEIGHTS = ("unbiasedstate", "biasedstates", "simplesum")
+
+
+def spline_sample_terms(S, A, spline_weights, N, N_k):
+    """v [nb] such that the sample term of the spline fit's objective (fes.py:2135-2167) is c . v, with c the full
+    coefficient vector, and that of its gradient (:2242-2249) is v[1:].
+
+    S [K, nb] and A [nb] are DeviceBSpline.moments of the fit's knots (S_ki = sum over state k's samples of B_i,
+    A_i = sum_n w_n B_i); N_k [K] counts the samples of each state.  A state without samples makes "simplesum"
+    NaN, as np.mean of an empty array does in the reference."""
+    if spline_weights == "unbiasedstate":
+        return N * np.asarray(A, np.float64)
+    S = np.asarray(S, np.float64)
+    if spline_weights == "biasedstates":
+        return S.sum(axis=0)
+    if spline_weights == "simplesum":
+        K = S.shape[0]
+        with np.errstate(invalid="ignore", divide="ignore"):
+            return ((N / K) * (S / np.asarray(N_k, np.float64)[:, None])).sum(axis=0)
+    raise ValueError(f"spline_weights {spline_weights!r} is not one of {SPLINE_WEIGHTS}")
+
+
+def _spline_setup(fes):
+    p = fes.spline_parameters
+    K = fes.mbar.K
+    N = fes.N
+    weights = p["spline_weights"]
+    scaling = (N / K) * np.ones(K) if weights == "simplesum" else fes.mbar.N_k
+    return p, K, N, weights, scaling
+
+
+def spline_objective(fes, xi, v):
+    """The spline fit's objective at the coefficients xi (the last nspline - 1; fes.py:2102-2186) from the sample
+    terms v of spline_sample_terms.  The partition functions are the reference's quadratures of the same integrands
+    in the same order, stored in fes.spline_data["bspline_expf"] / ["bspline_pF"] as the reference stores them, so
+    that the unpatched Hessian reads what it expects."""
+    p, K, N, weights, scaling = _spline_setup(fes)
+    xrange, fkbias = p["xrange"], p["fkbias"]
+    bloc = fes._val_to_spline(xi)
+    f = np.dot(bloc.c, v)
+    if weights == "unbiasedstate":
+        def expf(x):
+            return np.exp(-bloc(x))
+
+        pF = fes._integrate(expf, xrange[0], xrange[1])
+        f += N * np.log(pF)
+    else:
+        pF = np.zeros(K)
+        expf = []
+        for k in range(K):
+            def expfk(x, kf=k):
+                return np.exp(-bloc(x) - fkbias[kf](x))
+
+            pF[k] = fes._integrate(expfk, xrange[0], xrange[1], args=(k,))
+            expf.append(expfk)
+        f += np.dot(scaling, np.log(pF))
+    fes.spline_data["bspline_expf"] = expf
+    fes.spline_data["bspline_pF"] = pF
+    logprior = p["map_data"]["logprior"]
+    if logprior is not None:
+        f -= logprior(np.concatenate([[0], xi], axis=None))
+    return f
+
+
+def spline_gradient(fes, xi, v):
+    """The gradient of spline_objective (fes.py:2188-2306) from the sample terms v: v[1:] minus the Boltzmann-weighted
+    basis integrals, computed and stored (spline_data["bspline_gkquad"] / ["bspline_pE"]) as the reference does."""
+    p, K, N, weights, scaling = _spline_setup(fes)
+    xrange, fkbias = p["xrange"], p["fkbias"]
+    nspline = p["nspline"]
+    db_c = fes.spline_data["bspline_derivatives"]
+    xrangei = fes.spline_data["xrangei"]
+    bloc = fes._val_to_spline(xi)
+    g = np.array(v[1:], dtype=np.float64)
+    if weights == "unbiasedstate":
+        gkquad = 0
+
+        def expf(x):
+            return np.exp(-bloc(x))
+
+        pF = fes._integrate(expf, xrange[0], xrange[1])
+        pE = np.zeros(nspline - 1)
+
+        def dexpf(x, index):
+            return db_c[index + 1](x) * expf(x)
+
+        for i in range(nspline - 1):
+            pE[i] = fes._integrate(dexpf, xrangei[i + 1, 0], xrangei[i + 1, 1], args=(i,))
+            pE[i] /= pF
+        g -= N * pE
+    else:
+        pF = np.zeros(K)
+        gkquad = np.zeros([nspline - 1, K])
+
+        def expf(x, k):
+            return np.exp(-bloc(x) - fkbias[k](x))
+
+        pE = None
+        for k in range(K):
+            pF[k] = fes._integrate(expf, xrange[0], xrange[1], args=(k,))
+            for i in range(nspline - 1):
+                def dexpf(x, k, i=i):
+                    return db_c[i + 1](x) * expf(x, k)
+
+                # the reference keeps the last of these scalars in spline_data["bspline_pE"]
+                pE = fes._integrate(dexpf, xrangei[i + 1, 0], xrangei[i + 1, 1], args=(k,))
+                gkquad[i, k] = pE / pF[k]
+        g -= np.dot(gkquad, scaling)
+    dlogprior = p["map_data"]["dlogprior"]
+    if dlogprior is not None:
+        g -= dlogprior(np.concatenate([[0], xi], axis=None))
+    fes.spline_data["bspline_gkquad"] = gkquad
+    fes.spline_data["bspline_pE"] = pE
+    return g
+
+
+def state_bias_sums(fkbias, x_n, state_n, K):
+    """F_k = sum over state k's samples of fkbias[k](x_n): one pass of the user's bias callables over the samples."""
+    x = np.asarray(x_n)
+    s = np.asarray(state_n)
+    order = np.argsort(s, kind="stable")
+    bounds = np.concatenate([[0], np.cumsum(np.bincount(s, minlength=K))])
+    xs = x[order]
+    return np.array([np.sum(fkbias[k](xs[bounds[k]:bounds[k + 1]])) for k in range(K)], dtype=np.float64)
+
+
+def spline_mc_loglikelihood(fes, spline, spline_weights, xrange, S, A, F_k, N_k):
+    """The MC chain's log-likelihood of `spline` (a BSpline on the fit's knots; fes.py:1954-2010) from the moments
+    S, A, the per-state bias sums F_k (state_bias_sums) and the per-state sample counts N_k.  The per-state
+    normalisations are the reference's quadratures."""
+    N, K = fes.N, fes.K
+    c = spline.c
+    if spline_weights == "unbiasedstate":
+        return N * np.dot(c, A)
+    fkbias = fes.spline_parameters["fkbias"]
+
+    def splinek(x, kf):
+        return spline(x) + fkbias[kf](x)
+
+    def expk(x, kf):
+        return np.exp(-splinek(x, kf))
+
+    loglikelihood = 0
+    for k in range(K):
+        normalize = np.log(fes._integrate(expk, xrange[0], xrange[1], args=(k,)))
+        total = np.dot(S[k], c) + F_k[k]
+        if spline_weights == "simplesum":
+            with np.errstate(invalid="ignore", divide="ignore"):
+                loglikelihood += (N / K) * (total / N_k[k])
+            loglikelihood += (N / K) * normalize
+        else:
+            loglikelihood += total
+            loglikelihood += fes.N_k[k] * normalize
+    return loglikelihood

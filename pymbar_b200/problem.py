@@ -431,6 +431,73 @@ class DeviceKde:
         return dict(ms=ms.value, chunks=chunks.value)
 
 
+class DeviceBSpline:
+    """Samples x_n [N] with optional weights w_n and state labels state_n in [0, K) resident on one H100 for B-spline
+    basis sums (mbar_b200_bspline_*).
+
+    `moments(t, k)` returns (S [K, nb], A [nb]) with S_ki = sum_{n: state_n = k} B_i(x_n) and A_i = sum_n w_n B_i(x_n),
+    B_i the basis functions of scipy's BSpline(t, e_i, k).  One upload serves any number of knot vectors.  Independent
+    of any DeviceProblem."""
+
+    def __init__(self, x_n, w_n=None, state_n=None, K=None, device=0):
+        self._lib = _lib.load()
+        self._h = C.c_void_p()
+        x = np.ascontiguousarray(x_n, dtype=np.float64)
+        if x.ndim != 1:
+            raise ValueError(f"x_n must be one-dimensional, got shape {np.shape(x_n)}")
+        self.N = x.shape[0]
+        w = None if w_n is None else _f64(w_n, self.N)
+        s = None
+        if state_n is not None:
+            s_raw = np.asarray(state_n)
+            if s_raw.shape != (self.N,) or not np.issubdtype(s_raw.dtype, np.integer):
+                raise ValueError(f"state_n must be [{self.N}] integers, got {s_raw.dtype} {s_raw.shape}")
+            K = int(s_raw.max()) + 1 if K is None else int(K)
+            # labels beyond int32 become -1, which the library rejects
+            s = np.ascontiguousarray(np.where((s_raw >= -1) & (s_raw < 2 ** 31 - 1), s_raw, -1), dtype=np.int32)
+        self.K = int(K) if s is not None else 0
+        self.has_weights, self.has_labels = w is not None, s is not None
+        self.device = int(device)
+        check(self._lib.mbar_b200_bspline_create(
+            self.device, self.N, _dptr(x), None if w is None else _dptr(w),
+            None if s is None else s.ctypes.data_as(C.POINTER(C.c_int32)), self.K, C.byref(self._h)))
+
+    def close(self):
+        if self._h is not None and self._h.value:
+            self._lib.mbar_b200_bspline_destroy(self._h)
+            self._h = None
+
+    def __del__(self):
+        try:
+            self.close()
+        except Exception:
+            pass
+
+    def __enter__(self):
+        return self
+
+    def __exit__(self, *exc):
+        self.close()
+
+    def moments(self, t, k, want_S=True, want_A=True):
+        """(S [K, nb] or None, A [nb] or None) for the knots t and degree k."""
+        t = np.ascontiguousarray(t, dtype=np.float64)
+        if t.ndim != 1:
+            raise ValueError(f"knots must be one-dimensional, got shape {t.shape}")
+        nb = max(t.shape[0] - int(k) - 1, 0)
+        S = np.empty((self.K, nb)) if want_S else None
+        A = np.empty(nb) if want_A else None
+        check(self._lib.mbar_b200_bspline_moments(self._h, int(k), t.shape[0], _dptr(t),
+                                                  None if S is None else _dptr(S), None if A is None else _dptr(A)))
+        return S, A
+
+    def last_stats(self):
+        """CUDA-event time (ms) of the last moments call's kernels and the number of row chunks."""
+        ms, chunks = C.c_double(0), C.c_int32(0)
+        check(self._lib.mbar_b200_last_bspline_stats(self._h, C.byref(ms), C.byref(chunks)))
+        return dict(ms=ms.value, chunks=chunks.value)
+
+
 def measure_fp64_peak(device=0):
     """(DMMA TFLOP/s, DFMA TFLOP/s) of this GPU from register-only loops (mbar_b200_measure_fp64_peak)."""
     a, b = C.c_double(0), C.c_double(0)
