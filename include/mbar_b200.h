@@ -257,6 +257,44 @@ int mbar_b200_bspline_moments(mbar_b200_bspline* bspline, int32_t degree, int64_
 /* CUDA-event time of the kernels of the last mbar_b200_bspline_moments and the number of row chunks they took. */
 int mbar_b200_last_bspline_stats(mbar_b200_bspline* bspline, double* ms, int32_t* chunks);
 
+/* ---- lag sums of timeseries (pymbar.timeseries, independent of any u_kn context) --------------- */
+/* For a start s of the resident series A (and B; NULL: B = A) of length T, m = T - s, the means mu_A, mu_B of A[s:],
+ * B[s:], dA = A - mu_A, dB = B - mu_B, and
+ *   sigma^2 = sum_{n >= s} dA[n] dB[n] / m,
+ *   C(t) = sum_{n = s}^{T-1-t} (dA[n] dB[n+t] + dB[n] dA[n+t]) / (2.0 (m - t) sigma^2),
+ * with every term and quotient rounded as numpy rounds the reference's (timeseries.py:156-196, :474-497); only the
+ * sums run in another order (sequential within chunks whose bounds depend on T alone, the chunks in order).  A
+ * start's results do not depend on the other starts of a call or on how its lags were batched, and repeat calls are
+ * bit-identical; there are no floating-point atomics. */
+typedef struct mbar_b200_acf mbar_b200_acf;
+/* Upload A [T] and B [T] (or NULL) once.  n_segments > 0: A is K concatenated series with offsets [K + 1] (0 = offsets[0]
+ * < offsets[1] < ... < offsets[K] = T), and no lag pair crosses a series (statistical_inefficiency_multiple).  NaN or
+ * infinite values -> MBAR_B200_ERR_NAN; T < 1 or bad offsets -> MBAR_B200_ERR_INVALID. */
+int mbar_b200_acf_create(int device, int64_t T, const double* a, const double* b, int32_t n_segments,
+                         const int64_t* offsets, mbar_b200_acf** out);
+int mbar_b200_acf_destroy(mbar_b200_acf* acf);
+/* The reference's statistical-inefficiency loop for every start: t = 1, 2, ... (fast: increments 1, 2, 3, ...) while
+ * t < m - 1, stopping after the first C(t) <= 0 with t > mintime, g += 2.0 * C * (1.0 - t / m) * increment.
+ * rule 1 (a segmented autocorrelation object, the single start 0) is statistical_inefficiency_multiple's loop instead:
+ * C(t) = (sum of single products over the series / sum_k max(N_k - t, 0)) / sigma^2, t < max N_k - 1, stop at
+ * C <= 0 with t > 10, g += 2.0 * C * (1.0 - t / navg) * increment.  Per start: mean_a, mean_b, sigma2 (may be NULL),
+ * g before the g >= 1 clamp, last_lag (the last t whose C was computed, 0 if none) and status (1: sigma^2 == 0, the
+ * reference's ParameterError; g = 1 and no lag evaluated).  trace [n_starts][trace_cap] (trace_cap may be 0) gets
+ * C at the first trace_cap lag indices evaluated, NaN after the last.  Lags are evaluated in rounds of 8, 8, 16, 32,
+ * ... lag indices for all active starts, with one host poll per round.  A start outside [0, T) or a rule the object
+ * cannot take -> MBAR_B200_ERR_INVALID.  A failed call leaves the object usable. */
+int mbar_b200_acf_inefficiency(mbar_b200_acf* acf, int64_t n_starts, const int64_t* starts, int32_t fast,
+                               int32_t mintime, int32_t rule, double navg, int64_t trace_cap, double* mean_a,
+                               double* mean_b, double* sigma2, double* g, int64_t* last_lag, int32_t* status,
+                               double* trace);
+/* C(t) for t = 0 .. n_max of one start (normalized_fluctuation_correlation_function), with its means and sigma^2.
+ * n_max outside [0, T - start - 1], a segmented object or sigma^2 == 0 -> MBAR_B200_ERR_INVALID. */
+int mbar_b200_acf_correlation(mbar_b200_acf* acf, int64_t start, int64_t n_max, double* C, double* mean_a,
+                              double* mean_b, double* sigma2);
+/* CUDA-event time of the last call, its lag rounds (host polls), and the (start, lag, n) terms of lags >= 1 it
+ * evaluated and of those up to each start's last lag; terms / useful_terms is the speculative batches' waste. */
+int mbar_b200_last_acf_stats(mbar_b200_acf* acf, double* ms, int32_t* rounds, int64_t* terms, int64_t* useful_terms);
+
 /* ---- native solver loops (no Python between iterations) ------------------------------------- */
 /* Plain self-consistent iteration f <- f - log S(f), gauge f[first sampled] = 0 each step, until
  * max |delta f / f| < tol (the convergence rule of mbar_solvers.py:627-640) or maxiter. */

@@ -5,15 +5,17 @@ Public surface:
   * :class:`pymbar_b200.DeviceProblem` — explicit residency handle (one GPU, one shard of samples);
   * :class:`pymbar_b200.DeviceKde` — weighted samples resident for kernel-density sums (FES with fes_type="kde");
   * :class:`pymbar_b200.DeviceBSpline` — samples resident for B-spline basis sums (FES with fes_type="spline");
+  * :class:`pymbar_b200.DeviceAcf` — a series resident for the lag sums of ``pymbar.timeseries``
+    (:mod:`pymbar_b200.timeseries`);
   * :func:`pymbar_b200.install` — rebind ``pymbar.mbar_solvers`` so unmodified ``pymbar.MBAR`` uses it.
 
 Everything numerical runs in libmbar_b200.so (C ABI in include/mbar_b200.h).  No CPU fallback.
 """
 from . import _lib
-from .problem import DeviceBSpline, DeviceKde, DeviceProblem, PinnedArray
+from .problem import DeviceAcf, DeviceBSpline, DeviceKde, DeviceProblem, PinnedArray
 from .utils import ParameterError
 
-__all__ = ["DeviceProblem", "DeviceKde", "DeviceBSpline", "PinnedArray", "ParameterError", "install", "uninstall", "trim", "mbar_solvers"]
+__all__ = ["DeviceProblem", "DeviceKde", "DeviceBSpline", "DeviceAcf", "PinnedArray", "ParameterError", "install", "uninstall", "trim", "mbar_solvers"]
 
 _SAVED = {}
 _PATCHED = (
@@ -79,6 +81,13 @@ def install(target=None, patch_layout_helpers=True, patch_mbar=True):
             fes_mod = None
         if fes_mod is not None and hasattr(fes_mod, "FES"):
             facade.install_fes_on(fes_mod.FES)
+        # pymbar.timeseries (statistical inefficiencies, equilibration detection), when importable
+        try:
+            import pymbar.timeseries as ts_mod
+        except ImportError:
+            ts_mod = None
+        if ts_mod is not None:
+            facade.install_timeseries_on(ts_mod)
     return target
 
 

@@ -1,0 +1,705 @@
+// mbar_b200_acf_*: the centred lag sums behind pymbar.timeseries (statistical_inefficiency, _multiple,
+// normalized_fluctuation_correlation_function and detect_equilibration, timeseries.py:83-836).  For a start s of a
+// series of length T (m = T - s) and a lag t the reference evaluates
+//
+//   S(s, t) = sum_{n = s}^{T - 1 - t} dA[n] dB[n + t] (+ dB[n] dA[n + t] for a cross-correlation),
+//   dA[n] = A[n] - mean(A[s:]),
+//
+// and walks t = 1, 2, ... (fast: increments 1, 2, 3, ...) until C(t) = S / (2 (m - t) sigma^2) <= 0 past mintime.
+//
+// Decomposition.  n is cut into chunks of NC samples, NC a function of T alone.  The partial of one (start, lag,
+// chunk) is a sequential sum, from 0.0, over the chunk's n >= s with n + t inside the series (or its segment), and a
+// (start, lag) sum adds the partials of chunks chunk(s), chunk(s) + 1, ... in that order, from 0.0.  The means are
+// the same construction with the term A[n].  Every term is the reference's, rounded as numpy rounds it (__dmul_rn /
+// __dadd_rn, no contraction); only the order of the sums differs from numpy's pairwise one.  Nothing depends on the
+// other starts of a call, on the lag batches or on the launch shapes: a start's results are the same bits in any call.
+//
+// Rounds.  The stop rule is sequential, so each round evaluates a batch of lag indices for every active start (one
+// CTA thread owns a start and ACF_RL consecutive lags of one chunk), and acf_walk_kernel then walks each start's batch
+// in lag order, applies the rule, accumulates g and retires the start.  The batches are 8, 8, 16, 32, ... lag
+// indices, so the lags evaluated never exceed twice those needed plus 8, and the host polls once per round: the
+// number of rounds grows like log L.
+#include <algorithm>
+#include <cmath>
+#include <vector>
+
+#include "internal.cuh"
+
+namespace mbar {
+
+constexpr int ACF_THREADS = 256;
+constexpr int ACF_RL = 4;                          // lags per thread
+constexpr int ACF_B0 = 8;                          // lag indices of the first round
+constexpr int64_t ACF_MAX_CHUNKS = 1024;           // NC = max(512, ceil(T / 1024))
+constexpr int64_t ACF_MIN_NC = 512;
+constexpr int64_t ACF_PART_BUDGET = int64_t(1) << 25;   // doubles of (start, lag, chunk) partials per launch
+
+}  // namespace mbar
+
+struct mbar_b200_acf {
+    int device = 0;
+    int64_t T = 0;
+    int64_t NC = 0, nChunks = 0;
+    int cross = 0;
+    int nSeg = 0;                       // 0: one series
+    double* d_a = nullptr;
+    double* d_b = nullptr;              // == d_a for an autocorrelation
+    int64_t* d_segEnd = nullptr;        // [T] end of the segment holding n, or NULL
+    int64_t* d_segLen = nullptr;        // [nSeg]
+    std::vector<int64_t> segLen;
+    cudaStream_t stream = nullptr;
+    cudaEvent_t ev0 = nullptr, ev1 = nullptr;
+    double lastMs = 0.0;
+    int lastRounds = 0;
+    int64_t lastTerms = 0, lastUseful = 0;
+};
+
+namespace mbar {
+
+__host__ __device__ __forceinline__ int64_t acf_lag(int64_t i, int fast) {
+    return fast ? 1 + i * (i + 1) / 2 : i + 1;
+}
+
+// chunk totals of A and B: tot[c] = 0.0 + sum over the chunk, in n order
+__global__ void acf_chunk_total_kernel(const double* __restrict__ a, const double* __restrict__ b, int64_t T,
+                                       int64_t NC, int64_t nChunks, double* totA, double* totB) {
+    const int64_t c = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (c >= nChunks) return;
+    const int64_t c1 = min(T, (c + 1) * NC);
+    double sa = 0.0, sb = 0.0;
+    for (int64_t n = c * NC; n < c1; ++n) {
+        sa = __dadd_rn(sa, a[n]);
+        sb = __dadd_rn(sb, b[n]);
+    }
+    totA[c] = sa;
+    totB[c] = sb;
+}
+
+// means of A[s:] and B[s:]: the head of chunk(s) from s, then the following chunk totals in order
+__global__ void acf_mean_kernel(const double* __restrict__ a, const double* __restrict__ b, int64_t T, int64_t NC,
+                                int64_t nChunks, const double* __restrict__ totA, const double* __restrict__ totB,
+                                const int64_t* __restrict__ starts, int64_t nStarts, double* muA, double* muB) {
+    const int64_t j = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (j >= nStarts) return;
+    const int64_t s = starts[j];
+    const int64_t c = s / NC, c1 = min(T, (c + 1) * NC);
+    double ha = 0.0, hb = 0.0;
+    for (int64_t n = s; n < c1; ++n) {
+        ha = __dadd_rn(ha, a[n]);
+        hb = __dadd_rn(hb, b[n]);
+    }
+    double sa = __dadd_rn(0.0, ha), sb = __dadd_rn(0.0, hb);
+    for (int64_t k = c + 1; k < nChunks; ++k) {
+        sa = __dadd_rn(sa, totA[k]);
+        sb = __dadd_rn(sb, totB[k]);
+    }
+    muA[j] = __ddiv_rn(sa, (double)(T - s));
+    muB[j] = __ddiv_rn(sb, (double)(T - s));
+}
+
+struct AcfLagParams {
+    const double* a;
+    const double* b;
+    const int64_t* segEnd;
+    const int64_t* starts;      // [call starts]
+    const double* muA;
+    const double* muB;
+    const int32_t* act;         // active call-start indices of this launch: act[0 .. nAct)
+    const int64_t* lags;        // this launch's lags, ascending: lags[0 .. nLags)
+    double* partial;            // [nChunks][nAct * nLags]
+    int64_t T, NC;
+    int nAct, nLags, LG;        // LG = ceil(nLags / ACF_RL) lag groups per start
+};
+
+// one (start, ACF_RL lags) per thread, one chunk per blockIdx.x
+template <bool CROSS, bool SEG>
+__global__ void __launch_bounds__(ACF_THREADS) acf_lag_partial_kernel(AcfLagParams p) {
+    const int64_t q = (int64_t)blockIdx.y * ACF_THREADS + threadIdx.x;
+    const int si = (int)(q / p.LG), lg = (int)(q % p.LG);
+    if (si >= p.nAct) return;
+    const int j = p.act[si];
+    const int64_t s = p.starts[j];
+    const int64_t c = blockIdx.x;
+    const int64_t c0 = c * p.NC, c1 = min(p.T, c0 + p.NC);
+    if (s >= c1) return;                       // a chunk before the start: never read
+    const double mua = p.muA[j], mub = p.muB[j];
+    int64_t t[ACF_RL];
+    double acc[ACF_RL];
+    const int jl0 = lg * ACF_RL;
+#pragma unroll
+    for (int r = 0; r < ACF_RL; ++r) {
+        t[r] = (jl0 + r < p.nLags) ? p.lags[jl0 + r] : INT64_MAX / 2;
+        acc[r] = 0.0;
+    }
+    const int64_t lo = max(c0, s);
+    const int64_t hi = SEG ? c1 : min(c1, p.T - t[0]);
+    for (int64_t n = lo; n < hi; ++n) {
+        const double da = __dsub_rn(__ldg(p.a + n), mua);
+        const double db = CROSS ? __dsub_rn(__ldg(p.b + n), mub) : da;
+        const int64_t end = SEG ? __ldg(p.segEnd + n) : p.T;
+#pragma unroll
+        for (int r = 0; r < ACF_RL; ++r) {
+            if (n + t[r] < end) {
+                double term = __dmul_rn(da, __dsub_rn(__ldg(p.b + n + t[r]), mub));
+                if (CROSS) term = __dadd_rn(term, __dmul_rn(db, __dsub_rn(__ldg(p.a + n + t[r]), mua)));
+                acc[r] = __dadd_rn(acc[r], term);
+            }
+        }
+    }
+    const int64_t pairs = (int64_t)p.nAct * p.nLags;
+#pragma unroll
+    for (int r = 0; r < ACF_RL; ++r)
+        if (jl0 + r < p.nLags) p.partial[c * pairs + (int64_t)si * p.nLags + jl0 + r] = acc[r];
+}
+
+// S[si * ldS + col0 + jl] = 0.0 + partials of chunks chunk(s), chunk(s) + 1, ... in order
+__global__ void acf_reduce_kernel(const double* __restrict__ partial, const int64_t* __restrict__ starts,
+                                  const int32_t* __restrict__ act, int nAct, int nLags, int64_t NC, int64_t nChunks,
+                                  double* S, int ldS, int col0) {
+    const int64_t q = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    const int64_t pairs = (int64_t)nAct * nLags;
+    if (q >= pairs) return;
+    const int si = (int)(q / nLags), jl = (int)(q % nLags);
+    const int64_t s = starts[act[si]];
+    double sum = 0.0;
+    for (int64_t c = s / NC; c < nChunks; ++c) sum = __dadd_rn(sum, partial[c * pairs + q]);
+    S[(int64_t)si * ldS + col0 + jl] = sum;
+}
+
+// sigma^2 from the lag-0 sums; status 1 where it is 0 (the reference's ParameterError)
+__global__ void acf_sigma_kernel(const double* __restrict__ S0, const int64_t* __restrict__ starts, int64_t nStarts,
+                                 int64_t T, int cross, double* sigma2, int32_t* status, int8_t* done) {
+    const int64_t j = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (j >= nStarts) return;
+    const double sum = cross ? __dmul_rn(0.5, S0[j]) : S0[j];
+    const double s2 = __ddiv_rn(sum, (double)(T - starts[j]));
+    sigma2[j] = s2;
+    status[j] = s2 == 0.0 ? 1 : 0;
+    done[j] = s2 == 0.0 ? 1 : 0;
+}
+
+struct AcfWalkParams {
+    const int64_t* starts;
+    const int32_t* act;
+    const double* S;            // [nAct][B]
+    const double* sigma2;
+    const int64_t* segLen;      // multiple rule
+    int nSeg;
+    int nAct, B;
+    int64_t i0;                 // first lag index of the batch
+    int64_t T;
+    int fast, multiple, cross;
+    int64_t mintime;
+    double navg;
+    int64_t limitMultiple;      // max N_k (multiple rule)
+    double* g;
+    int64_t* lastLag;
+    int8_t* done;
+    double* trace;
+    int64_t traceCap;
+};
+
+// the reference's loop over this batch's lags, for one start, in the reference's fp64 operations
+__global__ void acf_walk_kernel(AcfWalkParams p) {
+    const int si = blockIdx.x * blockDim.x + threadIdx.x;
+    if (si >= p.nAct) return;
+    const int j = p.act[si];
+    const int64_t s = p.starts[j];
+    const int64_t m = p.T - s;
+    const int64_t limit = p.multiple ? p.limitMultiple : m;
+    const double s2 = p.sigma2[j];
+    double g = p.g[j];
+    int64_t last = p.lastLag[j];
+    int8_t fin = 0;
+    for (int k = 0; k < p.B && !fin; ++k) {
+        const int64_t i = p.i0 + k;
+        const int64_t t = acf_lag(i, p.fast);
+        if (t >= limit - 1) {
+            fin = 1;
+            break;
+        }
+        const double sum = p.S[(int64_t)si * p.B + k];
+        double C;
+        if (p.multiple) {
+            int64_t den = 0;
+            for (int q = 0; q < p.nSeg; ++q)
+                if (t < p.segLen[q]) den += p.segLen[q] - t;
+            C = __ddiv_rn(__ddiv_rn(sum, (double)den), s2);
+        } else {
+            const double num = p.cross ? sum : __dmul_rn(2.0, sum);
+            C = __ddiv_rn(num, __dmul_rn(__dmul_rn(2.0, (double)(m - t)), s2));
+        }
+        if (p.trace && i < p.traceCap) p.trace[(int64_t)j * p.traceCap + i] = C;
+        last = t;
+        if (C <= 0.0 && t > (p.multiple ? 10 : p.mintime)) {
+            fin = 1;
+            break;
+        }
+        const double frac = p.multiple ? __ddiv_rn((double)t, p.navg) : __ddiv_rn((double)t, (double)m);
+        const double inc = p.fast ? (double)(i + 1) : 1.0;
+        g = __dadd_rn(g, __dmul_rn(__dmul_rn(__dmul_rn(2.0, C), __dsub_rn(1.0, frac)), inc));
+    }
+    if (!fin && acf_lag(p.i0 + p.B, p.fast) >= limit - 1) fin = 1;
+    p.g[j] = g;
+    p.lastLag[j] = last;
+    p.done[j] = fin;
+}
+
+// C(t) = S / (2 (m - t) sigma^2) for the lags of one start
+__global__ void acf_corr_kernel(const double* __restrict__ S, const int64_t* __restrict__ lags, int nLags, int64_t m,
+                                int cross, const double* __restrict__ sigma2, double* C) {
+    const int k = blockIdx.x * blockDim.x + threadIdx.x;
+    if (k >= nLags) return;
+    const double num = cross ? S[k] : __dmul_rn(2.0, S[k]);
+    C[k] = __ddiv_rn(num, __dmul_rn(__dmul_rn(2.0, (double)(m - lags[k])), sigma2[0]));
+}
+
+static void acf_release(mbar_b200_acf* o) {
+    for (void* p : {(void*)o->d_a, (void*)(o->d_b == o->d_a ? nullptr : o->d_b), (void*)o->d_segEnd,
+                    (void*)o->d_segLen})
+        if (p) cudaFree(p);
+    if (o->ev0) cudaEventDestroy(o->ev0);
+    if (o->ev1) cudaEventDestroy(o->ev1);
+    if (o->stream) cudaStreamDestroy(o->stream);
+    delete o;
+}
+
+// Device buffers of one call, released on every return path.
+struct AcfBuffers {
+    std::vector<void*> ptrs;
+    ~AcfBuffers() {
+        for (void* p : ptrs) cudaFree(p);
+    }
+    template <class T>
+    int alloc(T** p, size_t count) {
+        *p = nullptr;
+        const cudaError_t e = cudaMalloc((void**)p, std::max<size_t>(count, 1) * sizeof(T));
+        if (e != cudaSuccess) {
+            cudaGetLastError();
+            set_error("acf: cannot allocate %zu bytes", count * sizeof(T));
+            return e == cudaErrorMemoryAllocation ? MBAR_B200_ERR_NOMEM : MBAR_B200_ERR_CUDA;
+        }
+        ptrs.push_back((void*)*p);
+        return MBAR_B200_OK;
+    }
+};
+
+// Lag sums of the call starts act_h[] (indices into d_starts) for the ascending lags lags_h[], into d_S [nAct][B]
+// at columns col0.. (B = row stride).  Splits starts and lags so that one launch's partials fit the budget.
+struct AcfLagRunner {
+    mbar_b200_acf* o;
+    const int64_t* d_starts;
+    const double* d_muA;
+    const double* d_muB;
+    int32_t* d_act;       // [capacity]
+    int64_t* d_lags;      // [capacity]
+    double* d_partial;    // [ACF_PART_BUDGET or less]
+    int64_t partCap;
+
+    int run(const int32_t* act_h, int nAct, const int64_t* lags_h, int nLags, double* d_S, int ldS) {
+        const int64_t pairsMax = std::max<int64_t>(ACF_RL, partCap / o->nChunks);
+        const int lagStep = (int)std::min<int64_t>(nLags, std::max<int64_t>(ACF_RL, pairsMax / ACF_RL * ACF_RL));
+        MBAR_CUDA(cudaMemcpyAsync(d_lags, lags_h, (size_t)nLags * sizeof(int64_t), cudaMemcpyHostToDevice, o->stream));
+        MBAR_CUDA(cudaMemcpyAsync(d_act, act_h, (size_t)nAct * sizeof(int32_t), cudaMemcpyHostToDevice, o->stream));
+        for (int l0 = 0; l0 < nLags; l0 += lagStep) {
+            const int nl = std::min(lagStep, nLags - l0);
+            const int startStep = (int)std::max<int64_t>(1, std::min<int64_t>(nAct, pairsMax / nl));
+            for (int a0 = 0; a0 < nAct; a0 += startStep) {
+                const int na = std::min(startStep, nAct - a0);
+                AcfLagParams p{};
+                p.a = o->d_a;
+                p.b = o->d_b;
+                p.segEnd = o->d_segEnd;
+                p.starts = d_starts;
+                p.muA = d_muA;
+                p.muB = d_muB;
+                p.act = d_act + a0;
+                p.lags = d_lags + l0;
+                p.partial = d_partial;
+                p.T = o->T;
+                p.NC = o->NC;
+                p.nAct = na;
+                p.nLags = nl;
+                p.LG = (nl + ACF_RL - 1) / ACF_RL;
+                const int64_t threads = (int64_t)na * p.LG;
+                const dim3 grid((unsigned)o->nChunks, (unsigned)((threads + ACF_THREADS - 1) / ACF_THREADS));
+                if (o->cross) {
+                    if (o->d_segEnd) acf_lag_partial_kernel<true, true><<<grid, ACF_THREADS, 0, o->stream>>>(p);
+                    else acf_lag_partial_kernel<true, false><<<grid, ACF_THREADS, 0, o->stream>>>(p);
+                } else {
+                    if (o->d_segEnd) acf_lag_partial_kernel<false, true><<<grid, ACF_THREADS, 0, o->stream>>>(p);
+                    else acf_lag_partial_kernel<false, false><<<grid, ACF_THREADS, 0, o->stream>>>(p);
+                }
+                const int64_t pairs = (int64_t)na * nl;
+                acf_reduce_kernel<<<(unsigned)((pairs + 255) / 256), 256, 0, o->stream>>>(
+                    d_partial, d_starts, d_act + a0, na, nl, o->NC, o->nChunks, d_S + (int64_t)a0 * ldS, ldS, l0);
+                MBAR_CUDA(cudaGetLastError());
+            }
+        }
+        return MBAR_B200_OK;
+    }
+};
+
+}  // namespace mbar
+
+using namespace mbar;
+
+int mbar_b200_acf_create(int device, int64_t T, const double* a, const double* b, int32_t n_segments,
+                         const int64_t* offsets, mbar_b200_acf** out) {
+    MBAR_REQUIRE(out && a, MBAR_B200_ERR_INVALID, "acf_create: NULL argument");
+    *out = nullptr;
+    MBAR_REQUIRE(T >= 1, MBAR_B200_ERR_INVALID, "acf_create: T=%lld must be >= 1", (long long)T);
+    MBAR_REQUIRE(T < (int64_t(1) << 40), MBAR_B200_ERR_INVALID, "acf_create: T=%lld too large", (long long)T);
+    MBAR_REQUIRE(n_segments >= 0, MBAR_B200_ERR_INVALID, "acf_create: %d segments", (int)n_segments);
+    MBAR_REQUIRE(n_segments == 0 || offsets, MBAR_B200_ERR_INVALID, "acf_create: NULL segment offsets");
+    if (n_segments > 0) {
+        MBAR_REQUIRE(offsets[0] == 0 && offsets[n_segments] == T, MBAR_B200_ERR_INVALID,
+                     "acf_create: segment offsets must run from 0 to T=%lld", (long long)T);
+        for (int k = 0; k < n_segments; ++k)
+            MBAR_REQUIRE(offsets[k + 1] > offsets[k], MBAR_B200_ERR_INVALID,
+                         "acf_create: segment %d is empty or offsets decrease", k);
+    }
+    for (int64_t n = 0; n < T; ++n) {
+        MBAR_REQUIRE(std::isfinite(a[n]), MBAR_B200_ERR_NAN, "acf_create: A[%lld] is %g", (long long)n, a[n]);
+        MBAR_REQUIRE(!b || std::isfinite(b[n]), MBAR_B200_ERR_NAN, "acf_create: B[%lld] is %g", (long long)n,
+                     b ? b[n] : 0.0);
+    }
+    int ndev = 0;
+    if (cudaGetDeviceCount(&ndev) != cudaSuccess || ndev == 0) {
+        cudaGetLastError();
+        set_error("no CUDA device visible: libmbar_b200 has no CPU fallback");
+        return MBAR_B200_ERR_NO_DEVICE;
+    }
+    MBAR_REQUIRE(device >= 0 && device < ndev, MBAR_B200_ERR_INVALID, "device %d of %d", device, ndev);
+    MBAR_CUDA(cudaSetDevice(device));
+    cudaDeviceProp prop;
+    MBAR_CUDA(cudaGetDeviceProperties(&prop, device));
+    if (prop.major != 9 || prop.minor != 0) {
+        set_error("device %d is sm_%d%d; this library is built for sm_90a (H100) only", device, prop.major, prop.minor);
+        return MBAR_B200_ERR_NO_DEVICE;
+    }
+    mbar_b200_acf* o = new mbar_b200_acf();
+    o->device = device;
+    o->T = T;
+    o->NC = std::max<int64_t>(ACF_MIN_NC, (T + ACF_MAX_CHUNKS - 1) / ACF_MAX_CHUNKS);
+    o->nChunks = (T + o->NC - 1) / o->NC;
+    o->cross = b ? 1 : 0;
+    o->nSeg = n_segments;
+    auto fail = [&](int status) {
+        acf_release(o);
+        return status;
+    };
+    if (cudaStreamCreateWithFlags(&o->stream, cudaStreamNonBlocking) != cudaSuccess ||
+        cudaEventCreate(&o->ev0) != cudaSuccess || cudaEventCreate(&o->ev1) != cudaSuccess) {
+        set_error("acf_create: %s", cudaGetErrorString(cudaGetLastError()));
+        return fail(MBAR_B200_ERR_CUDA);
+    }
+    auto put = [&](auto** dst, const auto* src, size_t count) -> int {
+        using T_ = typename std::remove_const<typename std::remove_pointer<decltype(src)>::type>::type;
+        if (cudaMalloc((void**)dst, count * sizeof(T_)) != cudaSuccess) {
+            *dst = nullptr;
+            cudaGetLastError();
+            set_error("acf_create: cannot allocate %zu bytes", count * sizeof(T_));
+            return MBAR_B200_ERR_NOMEM;
+        }
+        if (cudaMemcpyAsync(*dst, src, count * sizeof(T_), cudaMemcpyHostToDevice, o->stream) != cudaSuccess) {
+            set_error("acf_create: %s", cudaGetErrorString(cudaGetLastError()));
+            return MBAR_B200_ERR_CUDA;
+        }
+        return MBAR_B200_OK;
+    };
+    std::vector<int64_t> segEnd;
+    int rc = put(&o->d_a, a, (size_t)T);
+    if (!rc && b) rc = put(&o->d_b, b, (size_t)T);
+    if (!rc && !b) o->d_b = o->d_a;
+    if (!rc && n_segments > 0) {
+        segEnd.resize((size_t)T);
+        o->segLen.resize((size_t)n_segments);
+        for (int k = 0; k < n_segments; ++k) {
+            o->segLen[k] = offsets[k + 1] - offsets[k];
+            for (int64_t n = offsets[k]; n < offsets[k + 1]; ++n) segEnd[n] = offsets[k + 1];
+        }
+        rc = put(&o->d_segEnd, segEnd.data(), (size_t)T);
+        if (!rc) rc = put(&o->d_segLen, o->segLen.data(), (size_t)n_segments);
+    }
+    if (rc) return fail(rc);
+    if (cudaStreamSynchronize(o->stream) != cudaSuccess) {
+        set_error("acf_create: %s", cudaGetErrorString(cudaGetLastError()));
+        return fail(MBAR_B200_ERR_CUDA);
+    }
+    *out = o;
+    return MBAR_B200_OK;
+}
+
+int mbar_b200_acf_destroy(mbar_b200_acf* o) {
+    if (!o) return MBAR_B200_OK;
+    cudaSetDevice(o->device);
+    if (o->stream) cudaStreamSynchronize(o->stream);
+    acf_release(o);
+    return MBAR_B200_OK;
+}
+
+// means and sigma^2 of the call's starts (device arrays d_starts [n]); done[j] = 1 where sigma^2 == 0
+static int acf_moments(mbar_b200_acf* o, AcfBuffers& buf, const int64_t* d_starts, const std::vector<int64_t>& starts,
+                       AcfLagRunner& run, double* d_muA, double* d_muB, double* d_s2, int32_t* d_status,
+                       int8_t* d_done) {
+    const int64_t n = (int64_t)starts.size();
+    double *d_totA, *d_totB, *d_S0;
+    MBAR_TRY(buf.alloc(&d_totA, (size_t)o->nChunks));
+    MBAR_TRY(buf.alloc(&d_totB, (size_t)o->nChunks));
+    MBAR_TRY(buf.alloc(&d_S0, (size_t)n));
+    acf_chunk_total_kernel<<<(unsigned)((o->nChunks + 127) / 128), 128, 0, o->stream>>>(o->d_a, o->d_b, o->T, o->NC,
+                                                                                       o->nChunks, d_totA, d_totB);
+    acf_mean_kernel<<<(unsigned)((n + 127) / 128), 128, 0, o->stream>>>(o->d_a, o->d_b, o->T, o->NC, o->nChunks,
+                                                                      d_totA, d_totB, d_starts, n, d_muA, d_muB);
+    MBAR_CUDA(cudaGetLastError());
+    std::vector<int32_t> all((size_t)n);
+    for (int64_t j = 0; j < n; ++j) all[j] = (int32_t)j;
+    const int64_t zero = 0;
+    MBAR_TRY(run.run(all.data(), (int)n, &zero, 1, d_S0, 1));
+    acf_sigma_kernel<<<(unsigned)((n + 127) / 128), 128, 0, o->stream>>>(d_S0, d_starts, n, o->T, o->cross, d_s2,
+                                                                       d_status, d_done);
+    MBAR_CUDA(cudaGetLastError());
+    return MBAR_B200_OK;
+}
+
+int mbar_b200_acf_inefficiency(mbar_b200_acf* o, int64_t n_starts, const int64_t* starts, int32_t fast,
+                               int32_t mintime, int32_t rule, double navg, int64_t trace_cap, double* mean_a,
+                               double* mean_b, double* sigma2, double* g, int64_t* last_lag, int32_t* status,
+                               double* trace) {
+    MBAR_REQUIRE(o, MBAR_B200_ERR_INVALID, "acf_inefficiency: NULL object");
+    MBAR_REQUIRE(n_starts >= 1 && n_starts < INT32_MAX && starts, MBAR_B200_ERR_INVALID,
+                 "acf_inefficiency: %lld starts", (long long)n_starts);
+    MBAR_REQUIRE(g && last_lag && status, MBAR_B200_ERR_INVALID, "acf_inefficiency: NULL output");
+    MBAR_REQUIRE(rule == 0 || rule == 1, MBAR_B200_ERR_INVALID, "acf_inefficiency: unknown rule %d", (int)rule);
+    MBAR_REQUIRE(trace_cap >= 0 && (trace_cap == 0 || trace), MBAR_B200_ERR_INVALID,
+                 "acf_inefficiency: trace_cap %lld without a trace buffer", (long long)trace_cap);
+    MBAR_REQUIRE(trace_cap <= (int64_t(1) << 31) / n_starts, MBAR_B200_ERR_INVALID,
+                 "acf_inefficiency: trace of %lld x %lld too large", (long long)n_starts, (long long)trace_cap);
+    if (rule == 1) {
+        MBAR_REQUIRE(o->nSeg > 0 && !o->cross, MBAR_B200_ERR_INVALID,
+                     "acf_inefficiency: the multiple-series rule needs segments and an autocorrelation");
+        MBAR_REQUIRE(n_starts == 1 && starts[0] == 0, MBAR_B200_ERR_INVALID,
+                     "acf_inefficiency: the multiple-series rule takes the single start 0");
+        MBAR_REQUIRE(std::isfinite(navg) && navg > 0.0, MBAR_B200_ERR_INVALID, "acf_inefficiency: Navg = %g", navg);
+    } else {
+        MBAR_REQUIRE(o->nSeg == 0, MBAR_B200_ERR_INVALID, "acf_inefficiency: a segmented object takes rule 1");
+    }
+    for (int64_t j = 0; j < n_starts; ++j)
+        MBAR_REQUIRE(starts[j] >= 0 && starts[j] < o->T, MBAR_B200_ERR_INVALID,
+                     "acf_inefficiency: start %lld outside [0, %lld)", (long long)starts[j], (long long)o->T);
+    MBAR_CUDA(cudaSetDevice(o->device));
+    NvtxRange nvtx_("mbar_b200::acf_inefficiency");
+    const int64_t n = n_starts;
+    std::vector<int64_t> hs(starts, starts + n);
+    int64_t limitMultiple = 0;
+    for (int64_t L : o->segLen) limitMultiple = std::max(limitMultiple, L);
+    int64_t maxLimit = 0;
+    for (int64_t s : hs) maxLimit = std::max(maxLimit, rule == 1 ? limitMultiple : o->T - s);
+    AcfBuffers buf;
+    int64_t* d_starts;
+    double *d_muA, *d_muB, *d_s2, *d_g, *d_S, *d_partial, *d_trace = nullptr;
+    int64_t *d_last, *d_lags;
+    int32_t *d_status, *d_act;
+    int8_t* d_done;
+    // the largest round: every start active, one batch of B lags; keep the [active][B] sums within the budget by
+    // walking the starts in groups
+    const int64_t partCap = std::min<int64_t>(ACF_PART_BUDGET, o->nChunks * std::max<int64_t>(n, 1) * 4096);
+    MBAR_TRY(buf.alloc(&d_starts, (size_t)n));
+    MBAR_TRY(buf.alloc(&d_muA, (size_t)n));
+    MBAR_TRY(buf.alloc(&d_muB, (size_t)n));
+    MBAR_TRY(buf.alloc(&d_s2, (size_t)n));
+    MBAR_TRY(buf.alloc(&d_g, (size_t)n));
+    MBAR_TRY(buf.alloc(&d_last, (size_t)n));
+    MBAR_TRY(buf.alloc(&d_status, (size_t)n));
+    MBAR_TRY(buf.alloc(&d_done, (size_t)n));
+    MBAR_TRY(buf.alloc(&d_act, (size_t)n));
+    MBAR_TRY(buf.alloc(&d_partial, (size_t)partCap));
+    if (trace_cap > 0) MBAR_TRY(buf.alloc(&d_trace, (size_t)(n * trace_cap)));
+    MBAR_CUDA(cudaMemcpyAsync(d_starts, hs.data(), (size_t)n * sizeof(int64_t), cudaMemcpyHostToDevice, o->stream));
+    if (d_trace) MBAR_CUDA(cudaMemsetAsync(d_trace, 0xff, (size_t)(n * trace_cap) * sizeof(double), o->stream));
+    std::vector<double> ones((size_t)n, 1.0);
+    std::vector<int64_t> zeros((size_t)n, 0);
+    MBAR_CUDA(cudaMemcpyAsync(d_g, ones.data(), (size_t)n * sizeof(double), cudaMemcpyHostToDevice, o->stream));
+    MBAR_CUDA(cudaMemcpyAsync(d_last, zeros.data(), (size_t)n * sizeof(int64_t), cudaMemcpyHostToDevice, o->stream));
+    // lag batches: 8, 8, 16, 32, ... indices; the walk groups hold at most budget / B starts
+    int64_t Bmax = ACF_B0;
+    {
+        int64_t cum = ACF_B0;
+        while (acf_lag(cum, fast) < maxLimit - 1) {
+            Bmax = cum;
+            cum *= 2;
+        }
+    }
+    const int64_t walkCap = std::max<int64_t>(Bmax, std::min<int64_t>(n * Bmax, ACF_PART_BUDGET / 4));
+    MBAR_TRY(buf.alloc(&d_S, (size_t)walkCap));
+    MBAR_TRY(buf.alloc(&d_lags, (size_t)Bmax + 1));
+    AcfLagRunner run{o, d_starts, d_muA, d_muB, d_act, d_lags, d_partial, partCap};
+    MBAR_CUDA(cudaEventRecord(o->ev0, o->stream));
+    MBAR_TRY(acf_moments(o, buf, d_starts, hs, run, d_muA, d_muB, d_s2, d_status, d_done));
+    std::vector<int8_t> done((size_t)n);
+    MBAR_CUDA(cudaMemcpyAsync(done.data(), d_done, (size_t)n, cudaMemcpyDeviceToHost, o->stream));
+    MBAR_CUDA(cudaStreamSynchronize(o->stream));
+    std::vector<int32_t> active;
+    for (int64_t j = 0; j < n; ++j)
+        if (!done[j]) active.push_back((int32_t)j);
+    int rounds = 0;
+    int64_t terms = 0;
+    int64_t i0 = 0, B = ACF_B0;
+    std::vector<int64_t> lags;
+    auto termsOf = [&](int64_t s, int64_t t) -> int64_t {
+        if (rule == 1) {
+            int64_t c = 0;
+            for (int64_t L : o->segLen) c += std::max<int64_t>(L - t, 0);
+            return c;
+        }
+        return std::max<int64_t>(o->T - s - t, 0);
+    };
+    while (!active.empty()) {
+        lags.clear();
+        for (int64_t i = i0; i < i0 + B && acf_lag(i, fast) < maxLimit - 1; ++i) lags.push_back(acf_lag(i, fast));
+        const int nl = (int)lags.size();
+        const int groupMax = (int)std::max<int64_t>(1, walkCap / std::max(nl, 1));
+        for (size_t a0 = 0; a0 < active.size(); a0 += groupMax) {
+            const int na = (int)std::min<size_t>(groupMax, active.size() - a0);
+            if (nl > 0) MBAR_TRY(run.run(active.data() + a0, na, lags.data(), nl, d_S, nl));
+            else MBAR_CUDA(cudaMemcpyAsync(d_act, active.data() + a0, (size_t)na * sizeof(int32_t),
+                                           cudaMemcpyHostToDevice, o->stream));
+            AcfWalkParams w{};
+            w.starts = d_starts;
+            w.act = d_act;
+            w.S = d_S;
+            w.sigma2 = d_s2;
+            w.segLen = o->d_segLen;
+            w.nSeg = o->nSeg;
+            w.nAct = na;
+            w.B = nl;
+            w.i0 = i0;
+            w.T = o->T;
+            w.fast = fast ? 1 : 0;
+            w.multiple = rule == 1;
+            w.cross = o->cross;
+            w.mintime = mintime;
+            w.navg = navg;
+            w.limitMultiple = limitMultiple;
+            w.g = d_g;
+            w.lastLag = d_last;
+            w.done = d_done;
+            w.trace = d_trace;
+            w.traceCap = trace_cap;
+            // run() copied this group's active list to d_act[0..na)
+            acf_walk_kernel<<<(unsigned)((na + 127) / 128), 128, 0, o->stream>>>(w);
+            MBAR_CUDA(cudaGetLastError());
+            for (int k = 0; k < na; ++k)
+                for (int64_t t : lags) terms += termsOf(hs[active[a0 + k]], t);
+        }
+        MBAR_CUDA(cudaMemcpyAsync(done.data(), d_done, (size_t)n, cudaMemcpyDeviceToHost, o->stream));
+        MBAR_CUDA(cudaStreamSynchronize(o->stream));
+        ++rounds;
+        std::vector<int32_t> next;
+        for (int32_t j : active)
+            if (!done[j]) next.push_back(j);
+        active.swap(next);
+        i0 += B;
+        if (rounds > 1) B *= 2;
+    }
+    MBAR_CUDA(cudaEventRecord(o->ev1, o->stream));
+    if (mean_a) MBAR_CUDA(cudaMemcpyAsync(mean_a, d_muA, (size_t)n * sizeof(double), cudaMemcpyDeviceToHost, o->stream));
+    if (mean_b) MBAR_CUDA(cudaMemcpyAsync(mean_b, d_muB, (size_t)n * sizeof(double), cudaMemcpyDeviceToHost, o->stream));
+    if (sigma2) MBAR_CUDA(cudaMemcpyAsync(sigma2, d_s2, (size_t)n * sizeof(double), cudaMemcpyDeviceToHost, o->stream));
+    MBAR_CUDA(cudaMemcpyAsync(g, d_g, (size_t)n * sizeof(double), cudaMemcpyDeviceToHost, o->stream));
+    MBAR_CUDA(cudaMemcpyAsync(last_lag, d_last, (size_t)n * sizeof(int64_t), cudaMemcpyDeviceToHost, o->stream));
+    MBAR_CUDA(cudaMemcpyAsync(status, d_status, (size_t)n * sizeof(int32_t), cudaMemcpyDeviceToHost, o->stream));
+    if (d_trace)
+        MBAR_CUDA(cudaMemcpyAsync(trace, d_trace, (size_t)(n * trace_cap) * sizeof(double), cudaMemcpyDeviceToHost,
+                                  o->stream));
+    MBAR_CUDA(cudaStreamSynchronize(o->stream));
+    // the lag terms the stop rule needed: every lag up to each start's last evaluated one
+    int64_t useful = 0;
+    for (int64_t j = 0; j < n; ++j) {
+        if (status[j]) continue;
+        for (int64_t i = 0; acf_lag(i, fast) <= last_lag[j] && last_lag[j] > 0; ++i)
+            useful += termsOf(hs[j], acf_lag(i, fast));
+    }
+    float e = 0.f;
+    o->lastMs = event_ms(o->ev0, o->ev1, &e) ? e : 0.0;
+    o->lastRounds = rounds;
+    o->lastTerms = terms;
+    o->lastUseful = useful;
+    return MBAR_B200_OK;
+}
+
+int mbar_b200_acf_correlation(mbar_b200_acf* o, int64_t start, int64_t n_max, double* C, double* mean_a,
+                              double* mean_b, double* sigma2) {
+    MBAR_REQUIRE(o, MBAR_B200_ERR_INVALID, "acf_correlation: NULL object");
+    MBAR_REQUIRE(C, MBAR_B200_ERR_INVALID, "acf_correlation: NULL output");
+    MBAR_REQUIRE(o->nSeg == 0, MBAR_B200_ERR_INVALID, "acf_correlation: the object holds segments");
+    MBAR_REQUIRE(start >= 0 && start < o->T, MBAR_B200_ERR_INVALID, "acf_correlation: start %lld outside [0, %lld)",
+                 (long long)start, (long long)o->T);
+    MBAR_REQUIRE(n_max >= 0 && n_max <= o->T - start - 1, MBAR_B200_ERR_INVALID,
+                 "acf_correlation: N_max %lld outside [0, %lld]", (long long)n_max, (long long)(o->T - start - 1));
+    MBAR_CUDA(cudaSetDevice(o->device));
+    NvtxRange nvtx_("mbar_b200::acf_correlation");
+    AcfBuffers buf;
+    int64_t *d_starts, *d_lags;
+    double *d_muA, *d_muB, *d_s2, *d_S, *d_C, *d_partial;
+    int32_t *d_status, *d_act;
+    int8_t* d_done;
+    const int64_t nl = n_max + 1;
+    const int64_t batch = std::min<int64_t>(nl, 1 << 20);
+    const int64_t partCap = std::min<int64_t>(ACF_PART_BUDGET, o->nChunks * batch);
+    MBAR_TRY(buf.alloc(&d_starts, 1));
+    MBAR_TRY(buf.alloc(&d_muA, 1));
+    MBAR_TRY(buf.alloc(&d_muB, 1));
+    MBAR_TRY(buf.alloc(&d_s2, 1));
+    MBAR_TRY(buf.alloc(&d_status, 1));
+    MBAR_TRY(buf.alloc(&d_done, 1));
+    MBAR_TRY(buf.alloc(&d_act, 1));
+    MBAR_TRY(buf.alloc(&d_lags, (size_t)batch));
+    MBAR_TRY(buf.alloc(&d_S, (size_t)batch));
+    MBAR_TRY(buf.alloc(&d_C, (size_t)nl));
+    MBAR_TRY(buf.alloc(&d_partial, (size_t)partCap));
+    MBAR_CUDA(cudaMemcpyAsync(d_starts, &start, sizeof(int64_t), cudaMemcpyHostToDevice, o->stream));
+    AcfLagRunner run{o, d_starts, d_muA, d_muB, d_act, d_lags, d_partial, partCap};
+    MBAR_CUDA(cudaEventRecord(o->ev0, o->stream));
+    std::vector<int64_t> hs{start};
+    MBAR_TRY(acf_moments(o, buf, d_starts, hs, run, d_muA, d_muB, d_s2, d_status, d_done));
+    double s2 = 0.0;
+    MBAR_CUDA(cudaMemcpyAsync(&s2, d_s2, sizeof(double), cudaMemcpyDeviceToHost, o->stream));
+    MBAR_CUDA(cudaStreamSynchronize(o->stream));
+    MBAR_REQUIRE(s2 != 0.0, MBAR_B200_ERR_INVALID, "acf_correlation: sigma^2 = 0 (constant series)");
+    const int32_t act0 = 0;
+    std::vector<int64_t> lags;
+    for (int64_t l0 = 0; l0 < nl; l0 += batch) {
+        const int64_t b = std::min(batch, nl - l0);
+        lags.resize((size_t)b);
+        for (int64_t k = 0; k < b; ++k) lags[k] = l0 + k;
+        MBAR_TRY(run.run(&act0, 1, lags.data(), (int)b, d_S, (int)b));
+        acf_corr_kernel<<<(unsigned)((b + 255) / 256), 256, 0, o->stream>>>(d_S, d_lags, (int)b, o->T - start,
+                                                                           o->cross, d_s2, d_C + l0);
+        MBAR_CUDA(cudaGetLastError());
+        MBAR_CUDA(cudaStreamSynchronize(o->stream));   // d_lags is rewritten by the next batch
+    }
+    MBAR_CUDA(cudaEventRecord(o->ev1, o->stream));
+    MBAR_CUDA(cudaMemcpyAsync(C, d_C, (size_t)nl * sizeof(double), cudaMemcpyDeviceToHost, o->stream));
+    if (mean_a) MBAR_CUDA(cudaMemcpyAsync(mean_a, d_muA, sizeof(double), cudaMemcpyDeviceToHost, o->stream));
+    if (mean_b) MBAR_CUDA(cudaMemcpyAsync(mean_b, d_muB, sizeof(double), cudaMemcpyDeviceToHost, o->stream));
+    if (sigma2) MBAR_CUDA(cudaMemcpyAsync(sigma2, d_s2, sizeof(double), cudaMemcpyDeviceToHost, o->stream));
+    MBAR_CUDA(cudaStreamSynchronize(o->stream));
+    float e = 0.f;
+    o->lastMs = event_ms(o->ev0, o->ev1, &e) ? e : 0.0;
+    o->lastRounds = 0;
+    o->lastTerms = o->lastUseful = 0;
+    for (int64_t t = 0; t < nl; ++t) o->lastTerms += o->T - start - t;
+    o->lastUseful = o->lastTerms;
+    return MBAR_B200_OK;
+}
+
+int mbar_b200_last_acf_stats(mbar_b200_acf* o, double* ms, int32_t* rounds, int64_t* terms, int64_t* useful_terms) {
+    MBAR_REQUIRE(o, MBAR_B200_ERR_INVALID, "NULL acf object");
+    if (ms) *ms = o->lastMs;
+    if (rounds) *rounds = o->lastRounds;
+    if (terms) *terms = o->lastTerms;
+    if (useful_terms) *useful_terms = o->lastUseful;
+    return MBAR_B200_OK;
+}

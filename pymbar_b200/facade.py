@@ -45,6 +45,14 @@ original method.  The optimiser, the Hessian, the information criteria and `_get
 
 FES bootstraps, bootstrap uncertainties, device errors and any call whose weights leave the device's range contract
 go to the original methods.
+
+`install_timeseries_on` rebinds `statistical_inefficiency`, `statistical_inefficiency_multiple`,
+`normalized_fluctuation_correlation_function` and `detect_equilibration` of `pymbar.timeseries` to
+`pymbar_b200.timeseries`, which answers from a `DeviceAcf`.  `subsample_correlated_data`,
+`integrated_autocorrelation_time(Multiple)` and fes.py reach them through the module's globals.  fft=True, inputs
+that are not 1-D float64 or integer arrays (float32 means differ in the reference), a constant input or sigma^2 = 0 in
+`_multiple` (the reference returns NaN or runs on rounding noise) and device errors go to the original functions;
+the FFT and binary-search functions are not touched.
 """
 from __future__ import annotations
 
@@ -59,7 +67,8 @@ _TLS = threading.local()
 _SAVED = {}
 STATS = {"tickets": 0, "redeemed": 0, "moments": 0, "expectations": 0, "log_weights": 0, "fes_histograms": 0,
          "fes_theta": 0, "fes_w_kn": 0, "fes_kde_fits": 0, "fes_kde_queries": 0, "fes_spline_moments": 0,
-         "fes_spline_calls": 0}
+         "fes_spline_calls": 0, "ts_inefficiency": 0, "ts_multiple": 0, "ts_correlation": 0, "ts_equilibration": 0,
+         "ts_fallbacks": 0}
 
 
 class LogWeightTicket:
@@ -515,6 +524,99 @@ def install_fes_on(FES):
         FES._get_MC_loglikelihood = _get_MC_loglikelihood
     FES.kde = property(_get_kde, _set_kde, doc="the sklearn KernelDensity (fes.py:648), fitted on first use")
     FES.w_kn = property(_get_w_kn, _set_w_kn, doc="weights [N, K] of all states (fes.py:416), computed on first use")
+
+
+def _ts_series(x, need_array=False):
+    """x as the device takes it: a 1-D float64 or integer array (a list becomes one), else None."""
+    if need_array and not isinstance(x, np.ndarray):
+        return None
+    a = np.asarray(x)
+    if a.ndim != 1 or a.size == 0 or not (a.dtype == np.float64 or a.dtype.kind in "iu"):
+        return None
+    return a
+
+
+def install_timeseries_on(module):
+    """Patch the module object `module` (pymbar.timeseries)."""
+    if module in _SAVED:
+        return
+    names = ("statistical_inefficiency", "statistical_inefficiency_multiple",
+             "normalized_fluctuation_correlation_function", "detect_equilibration")
+    saved = {name: module.__dict__.get(name) for name in names}
+    _SAVED[module] = saved
+    orig_si, orig_multi, orig_corr, orig_eq = (saved[n] for n in names)
+
+    def _fallback(fn, *args, **kwargs):
+        STATS["ts_fallbacks"] += 1
+        return fn(*args, **kwargs)
+
+    def statistical_inefficiency(A_n, B_n=None, fast=False, mintime=3, fft=False):
+        args = (A_n, B_n, fast, mintime, fft)
+        if fft or _ts_series(A_n) is None or (B_n is not None and _ts_series(B_n) is None):
+            return _fallback(orig_si, *args)
+        from . import _lib
+        from . import timeseries as ts
+
+        try:
+            g = ts.statistical_inefficiency(A_n, B_n, fast=fast, mintime=mintime)
+        except _lib.MbarB200Error:
+            return _fallback(orig_si, *args)
+        STATS["ts_inefficiency"] += 1
+        return g
+
+    def statistical_inefficiency_multiple(A_kn, fast=False, return_correlation_function=False):
+        args = (A_kn, fast, return_correlation_function)
+        from . import _lib
+        from . import timeseries as ts
+        from . import utils as u
+
+        if isinstance(A_kn, np.ndarray):
+            ok = A_kn.ndim in (1, 2) and _ts_series(A_kn.ravel()) is not None
+        else:
+            ok = all(_ts_series(x, need_array=True) is not None for x in A_kn) and len(A_kn) > 0
+        if not ok:
+            return _fallback(orig_multi, *args)
+        try:
+            out = ts.statistical_inefficiency_multiple(A_kn, fast=fast,
+                                                       return_correlation_function=return_correlation_function)
+        except (_lib.MbarB200Error, u.ParameterError):
+            return _fallback(orig_multi, *args)
+        STATS["ts_multiple"] += 1
+        return out
+
+    def normalized_fluctuation_correlation_function(A_n, B_n=None, N_max=None, norm=True):
+        args = (A_n, B_n, N_max, norm)
+        if _ts_series(A_n) is None or (B_n is not None and _ts_series(B_n) is None):
+            return _fallback(orig_corr, *args)
+        from . import _lib
+        from . import timeseries as ts
+
+        try:
+            C = ts.normalized_fluctuation_correlation_function(A_n, B_n, N_max=N_max, norm=norm)
+        except _lib.MbarB200Error:
+            return _fallback(orig_corr, *args)
+        STATS["ts_correlation"] += 1
+        return C
+
+    def detect_equilibration(A_t, fast=True, nskip=1):
+        args = (A_t, fast, nskip)
+        if _ts_series(A_t, need_array=True) is None or not isinstance(nskip, (int, np.integer)) or nskip < 1:
+            return _fallback(orig_eq, *args)
+        from . import _lib
+        from . import timeseries as ts
+
+        try:
+            out = ts.detect_equilibration(A_t, fast=fast, nskip=nskip)
+        except _lib.MbarB200Error:
+            return _fallback(orig_eq, *args)
+        STATS["ts_equilibration"] += 1
+        return out
+
+    for name, fn in zip(names, (statistical_inefficiency, statistical_inefficiency_multiple,
+                                normalized_fluctuation_correlation_function, detect_equilibration)):
+        if saved[name] is not None:
+            fn.__doc__ = saved[name].__doc__
+            setattr(module, name, fn)
 
 
 def uninstall_from(MBAR):

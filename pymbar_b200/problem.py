@@ -498,6 +498,88 @@ class DeviceBSpline:
         return dict(ms=ms.value, chunks=chunks.value)
 
 
+class DeviceAcf:
+    """A series A [T] (and B [T] for a cross-correlation; optionally K concatenated series given by their lengths)
+    resident on one H100 for the centred lag sums of pymbar.timeseries (mbar_b200_acf_*).  Independent of any
+    DeviceProblem.
+
+    `inefficiency(starts, fast, mintime)` runs the reference's statistical-inefficiency loop for every start at once;
+    `correlation(start, n_max)` returns C(t), t = 0 .. n_max."""
+
+    def __init__(self, A_n, B_n=None, lengths=None, device=0):
+        self._lib = _lib.load()
+        self._h = C.c_void_p()
+        a = np.ascontiguousarray(A_n, dtype=np.float64)
+        if a.ndim != 1:
+            raise ValueError(f"A_n must be one-dimensional, got shape {np.shape(A_n)}")
+        self.T = a.shape[0]
+        b = None if B_n is None else _f64(B_n, self.T)
+        offsets = None
+        if lengths is not None:
+            offsets = np.ascontiguousarray(np.concatenate([[0], np.cumsum(np.asarray(lengths, dtype=np.int64))]),
+                                           dtype=np.int64)
+        self.lengths = None if lengths is None else np.asarray(lengths, dtype=np.int64)
+        self.cross = b is not None
+        self.device = int(device)
+        check(self._lib.mbar_b200_acf_create(
+            self.device, self.T, _dptr(a), None if b is None else _dptr(b), 0 if offsets is None else len(offsets) - 1,
+            None if offsets is None else offsets.ctypes.data_as(C.POINTER(C.c_int64)), C.byref(self._h)))
+
+    def close(self):
+        if self._h is not None and self._h.value:
+            self._lib.mbar_b200_acf_destroy(self._h)
+            self._h = None
+
+    def __del__(self):
+        try:
+            self.close()
+        except Exception:
+            pass
+
+    def __enter__(self):
+        return self
+
+    def __exit__(self, *exc):
+        self.close()
+
+    def inefficiency(self, starts, fast=False, mintime=3, multiple=False, navg=0.0, trace_cap=0):
+        """dict of per-start arrays: mean_a, mean_b, sigma2, g (before the g >= 1 clamp), last_lag, status
+        (1: sigma^2 == 0) and, with trace_cap > 0, trace [n, trace_cap] (C at the first lag indices, NaN after the
+        last).  multiple=True: statistical_inefficiency_multiple's loop (start 0 of a segmented object, navg the
+        mean series length)."""
+        s = np.ascontiguousarray(np.atleast_1d(starts), dtype=np.int64)
+        n = s.shape[0]
+        out = {k: np.empty(n) for k in ("mean_a", "mean_b", "sigma2", "g")}
+        out["last_lag"] = np.empty(n, np.int64)
+        out["status"] = np.empty(n, np.int32)
+        trace = np.empty((n, int(trace_cap))) if trace_cap > 0 else None
+        check(self._lib.mbar_b200_acf_inefficiency(
+            self._h, n, s.ctypes.data_as(C.POINTER(C.c_int64)), int(bool(fast)), int(mintime), 1 if multiple else 0,
+            float(navg), int(trace_cap), _dptr(out["mean_a"]), _dptr(out["mean_b"]), _dptr(out["sigma2"]),
+            _dptr(out["g"]), out["last_lag"].ctypes.data_as(C.POINTER(C.c_int64)),
+            out["status"].ctypes.data_as(C.POINTER(C.c_int32)), None if trace is None else _dptr(trace)))
+        if trace is not None:
+            out["trace"] = trace
+        return out
+
+    def correlation(self, start, n_max):
+        """(C [n_max + 1], mean_a, mean_b, sigma2) of the series from `start`."""
+        Cn = np.empty(int(n_max) + 1)
+        ma, mb, s2 = C.c_double(0), C.c_double(0), C.c_double(0)
+        check(self._lib.mbar_b200_acf_correlation(self._h, int(start), int(n_max), _dptr(Cn), C.byref(ma),
+                                                  C.byref(mb), C.byref(s2)))
+        return Cn, ma.value, mb.value, s2.value
+
+    def last_stats(self):
+        """CUDA-event time (ms) of the last call, its lag rounds, the lag terms evaluated and those the stop rule
+        needed (waste = terms / useful_terms)."""
+        ms, rounds, terms, useful = C.c_double(0), C.c_int32(0), C.c_int64(0), C.c_int64(0)
+        check(self._lib.mbar_b200_last_acf_stats(self._h, C.byref(ms), C.byref(rounds), C.byref(terms),
+                                                 C.byref(useful)))
+        return dict(ms=ms.value, rounds=rounds.value, terms=terms.value, useful_terms=useful.value,
+                    waste=terms.value / useful.value if useful.value else 1.0)
+
+
 def measure_fp64_peak(device=0):
     """(DMMA TFLOP/s, DFMA TFLOP/s) of this GPU from register-only loops (mbar_b200_measure_fp64_peak)."""
     a, b = C.c_double(0), C.c_double(0)

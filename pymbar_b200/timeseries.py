@@ -1,0 +1,228 @@
+"""The host side of pymbar.timeseries (timeseries.py:83-836) over the lag sums of a `DeviceAcf`.
+
+`statistical_inefficiency`, `statistical_inefficiency_multiple`, `normalized_fluctuation_correlation_function` and
+`detect_equilibration` take the reference's arguments and return what it returns.  The device evaluates every
+centred lag sum, the stop rule and the g accumulation in the reference's fp64 operations; only the order of the sums
+differs from numpy's pairwise one, so g, C and sigma^2 agree to a few ulps times the chunk length (DESIGN.md §3.5d),
+and `detect_equilibration` gets every start of the series in one device call instead of one numpy pass per start
+and lag.
+
+Starts whose remaining series is constant are the one place where the order of a sum changes the answer: the
+reference raises ParameterError (sigma^2 = 0, g = T - t + 1 in detect_equilibration, pymbar issue #122) when numpy's
+mean of the repeated value is exact, and otherwise runs its loop on the rounding noise of that mean.  Such starts are
+answered on the host: g = T - t + 1 when the mean is exact in any order (the value has at most 53 - ceil(log2 T)
+significant bits), else `_host_inefficiency`, the reference's loop in the reference's numpy operations.  They have
+Neff close to 1, and a long inexact constant tail costs what it costs in the reference.
+"""
+from __future__ import annotations
+
+import math
+
+import numpy as np
+
+from . import utils as _u
+
+DeviceAcf = None          # the device class; resolved on first use (a test may put a stand-in here)
+
+
+def _device(A, B=None, lengths=None):
+    global DeviceAcf
+    from . import mbar_solvers as ms
+
+    if DeviceAcf is None:
+        DeviceAcf = ms.DeviceAcf
+    return DeviceAcf(A, B, lengths=lengths, device=ms._DEVICE)
+
+
+def _parameter_error(msg):
+    # looked up at raise time: install() makes it pymbar's own ParameterError
+    return _u.ParameterError(msg)
+
+
+def lag(i, fast):
+    """The lag of lag index i (0, 1, ...): 1, 2, 3, ... or, fast, 1, 2, 4, 7, 11, ... (increments 1, 2, 3, ...)."""
+    i = np.asarray(i, dtype=np.int64)
+    return 1 + i * (i + 1) // 2 if fast else i + 1
+
+
+def lag_count(last_lag, fast):
+    """How many lags the loop evaluated when the last one was last_lag (0: none)."""
+    if last_lag <= 0:
+        return 0
+    if not fast:
+        return int(last_lag)
+    i = int(math.isqrt(2 * int(last_lag)))
+    while lag(i, True) > last_lag:
+        i -= 1
+    while lag(i + 1, True) <= last_lag:
+        i += 1
+    return i + 1
+
+
+def mean_is_exact(value, T):
+    """True when the mean of up to T copies of `value` is exact whatever the order of the sum: its significand has at
+    most 53 - ceil(log2 T) significant bits, so every partial sum k * value is representable."""
+    if value == 0.0:
+        return True
+    mant, _ = math.frexp(float(value))
+    bits = int(abs(mant) * 2 ** 53)
+    sig = 53 - ((bits & -bits).bit_length() - 1)
+    return sig <= 53 - math.ceil(math.log2(max(int(T), 2)))
+
+
+def _constant(x):
+    return x.size > 0 and bool(np.all(x == x[0]))
+
+
+def _host_inefficiency(A, B, fast, mintime):
+    """The reference's statistical_inefficiency loop (timeseries.py:152-196) in its own numpy operations, for series
+    whose device answer would differ only because of the order of a sum (constant series).  g before the clamp, or
+    None where sigma^2 == 0."""
+    B = A if B is None else B
+    N = A.size
+    dA = A.astype(np.float64) - A.mean()
+    dB = B.astype(np.float64) - B.mean()
+    s2 = (dA * dB).mean()
+    if s2 == 0:
+        return None
+    g, t, inc = 1.0, 1, 1
+    while t < N - 1:
+        C = np.sum(dA[0:N - t] * dB[t:N] + dB[0:N - t] * dA[t:N]) / (2.0 * float(N - t) * s2)
+        if C <= 0.0 and t > mintime:
+            break
+        g += 2.0 * C * (1.0 - float(t) / float(N)) * float(inc)
+        t += inc
+        if fast:
+            inc += 1
+    return g
+
+
+def neff(count, g32):
+    """(T - t + 1) / g_t[t] as detect_equilibration evaluates it (a Python int over a float32 scalar), elementwise:
+    a float32 division under numpy >= 2 (NEP 50); under numpy 1 a float32 division for counts below 2**16 and a
+    float64 one, rounded to float32, above."""
+    count = np.asarray(count, dtype=np.int64)
+    g32 = np.asarray(g32, dtype=np.float32)
+    if int(np.__version__.split(".")[0]) >= 2:
+        return count.astype(np.float32) / g32
+    small = count < 2 ** 16
+    out = (count.astype(np.float64) / g32.astype(np.float64)).astype(np.float32)
+    out[small] = count[small].astype(np.float32) / g32[small]
+    return out
+
+
+def statistical_inefficiency(A_n, B_n=None, fast=False, mintime=3):
+    """statistical_inefficiency (timeseries.py:83-203) without fft: g >= 1 of one series, or of two."""
+    A = np.array(A_n)
+    B = None if B_n is None else np.array(B_n)
+    if B is not None and A.shape != B.shape:
+        raise _parameter_error("A_n and B_n must have same dimensions.")
+    a = np.ascontiguousarray(A.ravel(), dtype=np.float64)
+    b = None if B is None else np.ascontiguousarray(B.ravel(), dtype=np.float64)
+    if _constant(a) or (b is not None and _constant(b)):
+        g = _host_inefficiency(A.ravel(), None if B is None else B.ravel(), fast, mintime)
+    else:
+        with _device(a, b) as dev:
+            r = dev.inefficiency([0], fast=fast, mintime=mintime)
+        g = None if r["status"][0] else float(r["g"][0])
+    if g is None:
+        raise _parameter_error("Sample covariance sigma_AB^2 = 0 -- cannot compute statistical inefficiency")
+    return 1.0 if g < 1.0 else g
+
+
+def _series_list(A_kn):
+    if isinstance(A_kn, np.ndarray):
+        return [A_kn.copy()] if A_kn.ndim == 1 else [A_kn[k, :].copy() for k in range(A_kn.shape[0])]
+    return list(A_kn)
+
+
+def statistical_inefficiency_multiple(A_kn, fast=False, return_correlation_function=False):
+    """statistical_inefficiency_multiple (timeseries.py:209-365): g of K series of possibly different lengths, and
+    with return_correlation_function the reference's [(t, C), ...].  A constant input (sigma^2 = 0 or rounding noise
+    in the reference) raises ParameterError."""
+    series = _series_list(A_kn)
+    N_k = np.array([np.asarray(x).size for x in series], np.int32)
+    navg = np.array(N_k, np.float64).mean()
+    a = np.concatenate([np.asarray(x, dtype=np.float64).ravel() for x in series])
+    if _constant(a):
+        raise _parameter_error("constant series: sigma^2 is 0 or rounding noise")
+    nmax = int(N_k.max())
+    cap = 0
+    if return_correlation_function:
+        cap = lag_count(nmax - 2, fast) if nmax > 2 else 0
+    with _device(a, lengths=N_k.astype(np.int64)) as dev:
+        r = dev.inefficiency([0], fast=fast, multiple=True, navg=navg, trace_cap=cap)
+    if r["status"][0]:
+        raise _parameter_error("Sample covariance sigma^2 = 0 -- cannot compute statistical inefficiency")
+    g = float(r["g"][0])
+    g = 1.0 if g < 1.0 else g
+    if not return_correlation_function:
+        return g
+    n = lag_count(int(r["last_lag"][0]), fast)
+    ts = lag(np.arange(n), fast)
+    return g, [(int(t), np.float64(C)) for t, C in zip(ts, r["trace"][0, :n])] if cap else []
+
+
+def normalized_fluctuation_correlation_function(A_n, B_n=None, N_max=None, norm=True):
+    """normalized_fluctuation_correlation_function (timeseries.py:405-503): C(t), t = 0 .. N_max, or with
+    norm=False C(t) sigma^2 + mu_A mu_B."""
+    A = np.array(A_n)
+    B = None if B_n is None else np.array(B_n)
+    N = A.size
+    if (not N_max) or (N_max > N - 1):
+        N_max = N - 1
+    if B is not None and A.shape != B.shape:
+        raise _parameter_error("A_n and B_n must have same dimensions.")
+    a = np.ascontiguousarray(A.ravel(), dtype=np.float64)
+    b = None if B is None else np.ascontiguousarray(B.ravel(), dtype=np.float64)
+    if _constant(a) or (b is not None and _constant(b)):
+        Bh = A if B is None else B
+        dA = A.astype(np.float64) - A.mean()
+        dB = Bh.astype(np.float64) - Bh.mean()
+        s2 = (dA * dB).mean()
+        if s2 == 0:
+            raise _parameter_error("Sample covariance sigma_AB^2 = 0 -- cannot compute statistical inefficiency")
+        dA, dB = dA.ravel(), dB.ravel()
+        C = np.array([np.sum(dA[0:N - t] * dB[t:N] + dB[0:N - t] * dA[t:N]) / (2.0 * float(N - t) * s2)
+                      for t in range(N_max + 1)])
+        mu_a, mu_b = A.mean(), Bh.mean()
+    else:
+        with _device(a, b) as dev:
+            C, mu_a, mu_b, s2 = dev.correlation(0, N_max)
+    return C if norm else C * s2 + mu_a * mu_b
+
+
+def detect_equilibration(A_t, fast=True, nskip=1):
+    """detect_equilibration (timeseries.py:771-836): (t, g, Neff_max) as np.int64, np.float32, np.float32, every
+    start in one device call."""
+    T = A_t.size
+    if A_t.std() == 0.0:
+        return 0, 1, 1
+    a = np.ascontiguousarray(np.asarray(A_t).ravel(), dtype=np.float64)
+    g_t = np.ones([T - 1], np.float32)
+    Neff_t = np.ones([T - 1], np.float32)
+    starts = np.arange(0, T - 1, nskip, dtype=np.int64)
+    differs = np.flatnonzero(a != a[-1])
+    tail = int(differs[-1]) + 1 if differs.size else 0          # A[t:] is constant for t >= tail
+    g = np.ones(starts.size)
+    zero = np.zeros(starts.size, bool)
+    on_dev = starts < tail
+    if on_dev.any():
+        with _device(a) as dev:
+            r = dev.inefficiency(starts[on_dev], fast=fast, mintime=3)
+        g[on_dev] = r["g"]
+        zero[on_dev] = r["status"] != 0
+    exact = mean_is_exact(a[-1], T)
+    for k in np.flatnonzero(~on_dev):
+        t = int(starts[k])
+        gk = None if exact else _host_inefficiency(np.asarray(A_t).ravel()[t:T], None, fast, 3)
+        if gk is None:
+            zero[k] = True
+        else:
+            g[k] = gk
+    g_t[starts] = np.where(g < 1.0, 1.0, g)
+    g_t[starts[zero]] = T - starts[zero] + 1
+    Neff_t[starts] = neff(T - starts + 1, g_t[starts])
+    Neff_max = Neff_t.max()
+    t = Neff_t.argmax()
+    return t, g_t[t], Neff_max
