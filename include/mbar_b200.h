@@ -40,6 +40,9 @@ extern "C" {
 
 #define MBAR_B200_ABI_VERSION 1
 
+/* Largest number of states a context takes: mbar_b200_create's K and create_augmented's K + n_extra. */
+#define MBAR_B200_MAX_STATES 8192
+
 #if defined(__GNUC__)
 #pragma GCC visibility push(default)
 #endif

@@ -9,6 +9,7 @@ _HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.path.join(_HERE, "libmbar_b200.so")
 
 UNIQUE_ID_BYTES = 128
+MAX_STATES = 8192            # MBAR_B200_MAX_STATES: largest K of a context, augmented ones included
 KERNEL_AUTO, KERNEL_FUSED, KERNEL_GENERIC = 0, 1, 2
 
 STATUS = {

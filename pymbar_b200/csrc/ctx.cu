@@ -592,7 +592,8 @@ int mbar_b200_host_hash(const void* base, int64_t rows, int64_t row_bytes, int64
 int mbar_b200_create(mbar_b200_ctx** out, int device, int32_t K, int64_t N_local, const double* N_k) {
     MBAR_REQUIRE(out && N_k, MBAR_B200_ERR_INVALID, "NULL argument");
     *out = nullptr;
-    MBAR_REQUIRE(K >= 1 && K <= 8192, MBAR_B200_ERR_INVALID, "K=%d outside [1, 8192]", K);
+    MBAR_REQUIRE(K >= 1 && K <= MBAR_B200_MAX_STATES, MBAR_B200_ERR_INVALID, "K=%d outside [1, %d]", K,
+                 MBAR_B200_MAX_STATES);
     MBAR_REQUIRE(N_local >= 1, MBAR_B200_ERR_INVALID, "N_local=%lld must be >= 1", (long long)N_local);
     int ndev = 0;
     if (cudaGetDeviceCount(&ndev) != cudaSuccess || ndev == 0) {
@@ -1033,7 +1034,8 @@ int mbar_b200_create_augmented(mbar_b200_ctx* base, int32_t n_extra, const doubl
     MBAR_REQUIRE(base && u_extra_host && out, MBAR_B200_ERR_INVALID, "NULL argument");
     *out = nullptr;
     MBAR_REQUIRE(base->ready, MBAR_B200_ERR_NOT_READY, "base problem has no u_kn yet");
-    MBAR_REQUIRE(n_extra >= 1 && base->K + n_extra <= 8192, MBAR_B200_ERR_INVALID, "n_extra=%d", n_extra);
+    MBAR_REQUIRE(n_extra >= 1 && base->K + n_extra <= MBAR_B200_MAX_STATES, MBAR_B200_ERR_INVALID,
+                 "n_extra=%d: K + n_extra must lie in [K + 1, %d]", n_extra, MBAR_B200_MAX_STATES);
     MBAR_REQUIRE(ld >= base->N, MBAR_B200_ERR_INVALID, "ld=%lld < N_local", (long long)ld);
     NvtxRange nvtx_("mbar_b200::create_augmented");
     const int K = base->K, E = n_extra, Kn = K + E;

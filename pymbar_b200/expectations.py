@@ -25,6 +25,25 @@ def _as_rows(a):
     return a.reshape(1, -1) if a.ndim == 1 else a
 
 
+def _appended(state_map):
+    """(of_state, of_obs, wanted_states) of a state map: the u_ln row and the observable of every (state, observable)
+    pair, and the distinct states of interest.  The augmented problem appends one row per wanted state and one per
+    pair."""
+    table = np.asarray(state_map)
+    if table.ndim >= 2:
+        of_state, of_obs = table[0].astype(int), table[1].astype(int)
+    else:
+        of_state, of_obs = table.astype(int), np.zeros(0, dtype=int)
+    return of_state, of_obs, np.unique(of_state)
+
+
+def augmented_states(K, state_map):
+    """K plus the rows expectations_inner appends for `state_map`.  A context holds at most `_lib.MAX_STATES`
+    states."""
+    _, of_obs, wanted = _appended(state_map)
+    return int(K) + len(wanted) + len(of_obs)
+
+
 def expectations_inner(u_kn, N_k, f_k, A_n, u_ln, state_map, uncertainty_method=None, return_theta=False,
                        device=0, problem=None):
     """MBAR.compute_expectations_inner (mbar.py:766-1012) for the analytical (non-bootstrap) methods.
@@ -43,13 +62,8 @@ def expectations_inner(u_kn, N_k, f_k, A_n, u_ln, state_map, uncertainty_method=
     K = u_kn.shape[0]
     energies = _as_rows(u_ln)
     obs = _as_rows(A_n)
-    table = np.asarray(state_map)
-    if table.ndim >= 2:
-        of_state, of_obs = table[0].astype(int), table[1].astype(int)
-    else:
-        of_state, of_obs = table.astype(int), np.zeros(0, dtype=int)
+    of_state, of_obs, wanted_states = _appended(state_map)     # wanted: rows of u_ln that become appended states
     n_pairs = len(of_obs)
-    wanted_states = np.unique(of_state)                  # rows of u_ln that become appended states
     n_states = len(wanted_states)
 
     # observables must be positive to live in the exponent: shift each one used by its minimum (plus a guard

@@ -20,8 +20,9 @@ the CPU.  With the facade installed:
 
 * `_computeUnnormalizedLogWeights` (:1919-1934) is -u_n - L_n with L_n from the device's log denominators.
 
-Anything outside what the device path implements (bootstrap uncertainties, `uncertainty_method="svd"`) calls
-the original method, which then reads `self.Log_W_nk` and materialises it.  `uninstall()` restores the class.
+Anything outside what the device path implements (bootstrap uncertainties, `uncertainty_method="svd"`, an
+augmented problem of more than `_lib.MAX_STATES` states) calls the original method, which then reads
+`self.Log_W_nk` and materialises it.  `uninstall()` restores the class.
 
 `install_fes_on` does the same for `pymbar.FES` (fes.py): `generate_fes` without bootstraps takes its log weights
 from the device and, for fes_type="histogram", builds the bin free energies with `pymbar_b200.fes.histogram_fes`;
@@ -65,10 +66,10 @@ from . import estimators as est
 
 _TLS = threading.local()
 _SAVED = {}
-STATS = {"tickets": 0, "redeemed": 0, "moments": 0, "expectations": 0, "log_weights": 0, "fes_histograms": 0,
-         "fes_theta": 0, "fes_w_kn": 0, "fes_kde_fits": 0, "fes_kde_queries": 0, "fes_spline_moments": 0,
-         "fes_spline_calls": 0, "ts_inefficiency": 0, "ts_multiple": 0, "ts_correlation": 0, "ts_equilibration": 0,
-         "ts_fallbacks": 0}
+STATS = {"tickets": 0, "redeemed": 0, "moments": 0, "expectations": 0, "expectations_fallbacks": 0, "log_weights": 0,
+         "fes_histograms": 0, "fes_theta": 0, "fes_w_kn": 0, "fes_kde_fits": 0, "fes_kde_queries": 0,
+         "fes_spline_moments": 0, "fes_spline_calls": 0, "ts_inefficiency": 0, "ts_multiple": 0, "ts_correlation": 0,
+         "ts_equilibration": 0, "ts_fallbacks": 0}
 
 
 class LogWeightTicket:
@@ -199,9 +200,16 @@ def install_on(MBAR):
         if uncertainty_method not in (None, "svd-ew", "approximate"):
             return orig_inner(self, A_n, u_ln, state_map, uncertainty_method=uncertainty_method,
                               warning_cutoff=warning_cutoff, return_theta=return_theta)
+        from . import _lib
         from . import expectations as ex
         from . import mbar_solvers as ms
 
+        # the augmented problem holds K + one row per state of interest + one per (state, observable) pair; past
+        # what a context takes, the original answers (checked up front: ERR_INVALID may also mean a bad argument)
+        if ex.augmented_states(np.shape(self.u_kn)[0], state_map) > _lib.MAX_STATES:
+            STATS["expectations_fallbacks"] += 1
+            return orig_inner(self, A_n, u_ln, state_map, uncertainty_method=uncertainty_method,
+                              warning_cutoff=warning_cutoff, return_theta=return_theta)
         STATS["expectations"] += 1
         return ex.expectations_inner(self.u_kn, self.N_k, self.f_k, A_n, u_ln, state_map,
                                      uncertainty_method=uncertainty_method, return_theta=return_theta,

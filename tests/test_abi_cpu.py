@@ -42,6 +42,14 @@ def test_ctypes_table_matches_header(lib):
     assert lib.load().mbar_b200_abi_version() == 1
 
 
+def test_max_states_matches_header():
+    """The facade decides up front whether an augmented problem fits a context: its limit must be the library's."""
+    from pymbar_b200 import _lib
+
+    m = re.search(r"#define\s+MBAR_B200_MAX_STATES\s+(\d+)", open(HEADER).read())
+    assert m and int(m.group(1)) == _lib.MAX_STATES
+
+
 def test_no_internal_symbols_leak(lib):
     import subprocess
 
