@@ -298,6 +298,35 @@ int mbar_b200_acf_correlation(mbar_b200_acf* acf, int64_t start, int64_t n_max, 
  * evaluated and of those up to each start's last lag; terms / useful_terms is the speculative batches' waste. */
 int mbar_b200_last_acf_stats(mbar_b200_acf* acf, double* ms, int32_t* rounds, int64_t* terms, int64_t* useful_terms);
 
+/* ---- sums over work vectors (pymbar.other_estimators: BAR, EXP, Gaussian EXP; no u_kn context) -- */
+/* A request (vector v, kind, c1, c2) over the resident vector w = w_v of n values returns out [3], every term in the
+ * reference's fp64 formula with its own max shifts (other_estimators.py:120-145, :489-504, :617-636, :694-696), and
+ * logsumexp(t) = log(sum exp(t - M)) + M with M = max t, replaced by 0 when it is not finite (utils.py:315-320):
+ *   FERMI:          a = (w + c1) + c2, m = max(a, 0), t = -m - log(exp(-m) + exp(a - m)):  logsumexp(t), 0, 0
+ *   FERMI_MOMENTS:  a = w + c1, A = max(a), t = -log(exp(-A) + exp(a - A)):  logsumexp(t), logsumexp(2 t), A
+ *   EXP:            x = exp(-w - max(-w)):  log(sum x) + max(-w), sum x, sum (x - sum x / n)^2
+ *   GAUSS:          sum w, sum (w - sum w / n)^2, 0
+ * Each sum runs over chunks whose bounds depend on n alone (sequential per thread, a fixed tree per chunk, the chunks
+ * in order): a request's out is the same bits whichever requests share the call, repeat calls are bit-identical, and
+ * there are no floating-point atomics. */
+#define MBAR_B200_WORK_FERMI 0
+#define MBAR_B200_WORK_FERMI_MOMENTS 1
+#define MBAR_B200_WORK_EXP 2
+#define MBAR_B200_WORK_GAUSS 3
+typedef struct mbar_b200_work mbar_b200_work;
+/* Upload V concatenated vectors w [n_total] with offsets [V + 1] once; each vector's min and max are kept.  NaN or
+ * infinite values -> MBAR_B200_ERR_NAN; an empty vector or bad offsets -> MBAR_B200_ERR_INVALID. */
+int mbar_b200_work_create(int device, int64_t n_total, const double* w, int32_t n_vectors, const int64_t* offsets,
+                          mbar_b200_work** out);
+int mbar_b200_work_destroy(mbar_b200_work* work);
+/* out [n_requests][3] for the requests (vector[r], kind[r], c1[r], c2[r]): two passes over each requested vector,
+ * four launches and one host synchronisation per call.  A vector outside [0, V) or an unknown kind ->
+ * MBAR_B200_ERR_INVALID.  A failed call leaves the object usable. */
+int mbar_b200_work_evaluate(mbar_b200_work* work, int32_t n_requests, const int32_t* vector, const int32_t* kind,
+                            const double* c1, const double* c2, double* out);
+/* CUDA-event time of the kernels of the last mbar_b200_work_evaluate, its launches and the work values it read. */
+int mbar_b200_last_work_stats(mbar_b200_work* work, double* ms, int32_t* launches, int64_t* values_read);
+
 /* ---- native solver loops (no Python between iterations) ------------------------------------- */
 /* Plain self-consistent iteration f <- f - log S(f), gauge f[first sampled] = 0 each step, until
  * max |delta f / f| < tol (the convergence rule of mbar_solvers.py:627-640) or maxiter. */

@@ -7,15 +7,17 @@ Public surface:
   * :class:`pymbar_b200.DeviceBSpline` — samples resident for B-spline basis sums (FES with fes_type="spline");
   * :class:`pymbar_b200.DeviceAcf` — a series resident for the lag sums of ``pymbar.timeseries``
     (:mod:`pymbar_b200.timeseries`);
+  * :class:`pymbar_b200.DeviceWork` — work vectors resident for the sums of ``pymbar.other_estimators`` (BAR, EXP,
+    Gaussian EXP; :mod:`pymbar_b200.other_estimators`, including ``bar_many`` for many pairs in lockstep);
   * :func:`pymbar_b200.install` — rebind ``pymbar.mbar_solvers`` so unmodified ``pymbar.MBAR`` uses it.
 
 Everything numerical runs in libmbar_b200.so (C ABI in include/mbar_b200.h).  No CPU fallback.
 """
 from . import _lib
-from .problem import DeviceAcf, DeviceBSpline, DeviceKde, DeviceProblem, PinnedArray
+from .problem import DeviceAcf, DeviceBSpline, DeviceKde, DeviceProblem, DeviceWork, PinnedArray
 from .utils import ParameterError
 
-__all__ = ["DeviceProblem", "DeviceKde", "DeviceBSpline", "DeviceAcf", "PinnedArray", "ParameterError", "install", "uninstall", "trim", "mbar_solvers"]
+__all__ = ["DeviceProblem", "DeviceKde", "DeviceBSpline", "DeviceAcf", "DeviceWork", "PinnedArray", "ParameterError", "install", "uninstall", "trim", "mbar_solvers"]
 
 _SAVED = {}
 _PATCHED = (
@@ -88,6 +90,21 @@ def install(target=None, patch_layout_helpers=True, patch_mbar=True):
             ts_mod = None
         if ts_mod is not None:
             facade.install_timeseries_on(ts_mod)
+        # pymbar.other_estimators (BAR, EXP, Gaussian EXP), when importable; pymbar re-exports those names at import
+        try:
+            import pymbar.other_estimators as oe_mod
+        except ImportError:
+            oe_mod = None
+        if oe_mod is not None:
+            import pymbar as pkg
+
+            originals = {name: oe_mod.__dict__.get(name) for name in facade.OE_NAMES}
+            facade.install_other_estimators_on(oe_mod)
+            for name in facade.OE_NAMES:
+                if originals[name] is not None and pkg.__dict__.get(name) is originals[name]:
+                    if (pkg, name) not in _SAVED:
+                        _SAVED[(pkg, name)] = originals[name]
+                    setattr(pkg, name, getattr(oe_mod, name))
     return target
 
 

@@ -54,6 +54,13 @@ go to the original methods.
 that are not 1-D float64 or integer arrays (float32 means differ in the reference), a constant input or sigma^2 = 0 in
 `_multiple` (the reference returns NaN or runs on rounding noise) and device errors go to the original functions;
 the FFT and binary-search functions are not touched.
+
+`install_other_estimators_on` rebinds `bar`, `bar_zero`, `exp` and `exp_gauss` of `pymbar.other_estimators` to
+`pymbar_b200.other_estimators`, which answers from a `DeviceWork`; `install()` rebinds the same names on the `pymbar`
+package, which bound them at import.  `bar_overlap` stays the reference's and reaches the patched `bar` through the
+module's globals.  Input that is not a 1-D float64 or signed integer ndarray (the reference fails on lists in `bar`,
+and float32 changes its arithmetic), empty or non-finite input, `verbose=True`, an unknown `method` or
+`uncertainty_method` (the original raises its own error) and device errors go to the original functions.
 """
 from __future__ import annotations
 
@@ -69,7 +76,8 @@ _SAVED = {}
 STATS = {"tickets": 0, "redeemed": 0, "moments": 0, "expectations": 0, "expectations_fallbacks": 0, "log_weights": 0,
          "fes_histograms": 0, "fes_theta": 0, "fes_w_kn": 0, "fes_kde_fits": 0, "fes_kde_queries": 0,
          "fes_spline_moments": 0, "fes_spline_calls": 0, "ts_inefficiency": 0, "ts_multiple": 0, "ts_correlation": 0,
-         "ts_equilibration": 0, "ts_fallbacks": 0}
+         "ts_equilibration": 0, "ts_fallbacks": 0, "oe_bar": 0, "oe_bar_zero": 0, "oe_exp": 0, "oe_exp_gauss": 0,
+         "oe_evaluations": 0, "oe_fallbacks": 0}
 
 
 class LogWeightTicket:
@@ -622,6 +630,106 @@ def install_timeseries_on(module):
 
     for name, fn in zip(names, (statistical_inefficiency, statistical_inefficiency_multiple,
                                 normalized_fluctuation_correlation_function, detect_equilibration)):
+        if saved[name] is not None:
+            fn.__doc__ = saved[name].__doc__
+            setattr(module, name, fn)
+
+
+OE_NAMES = ("bar", "bar_zero", "exp", "exp_gauss")
+
+
+def _oe_work(x):
+    """x if the device takes it as the reference computes it: a non-empty 1-D float64 ndarray, or a signed integer one
+    (32 or 64 bit) whose values, and -w - max(-w), are exact in fp64; else None."""
+    if not isinstance(x, np.ndarray) or x.ndim != 1 or x.size == 0:
+        return None
+    if x.dtype == np.float64:
+        return x
+    if x.dtype.kind == "i" and x.dtype.itemsize in (4, 8):
+        lim = min(2 ** 52, 2 ** (8 * x.dtype.itemsize - 3))
+        if int(x.min()) >= -lim and int(x.max()) <= lim:
+            return x
+    return None
+
+
+def install_other_estimators_on(module):
+    """Patch the module object `module` (pymbar.other_estimators): bar, bar_zero, exp and exp_gauss."""
+    if module in _SAVED:
+        return
+    saved = {name: module.__dict__.get(name) for name in OE_NAMES}
+    _SAVED[module] = saved
+    orig_bar, orig_zero, orig_exp, orig_gauss = (saved[n] for n in OE_NAMES)
+
+    def _fallback(fn, *args):
+        STATS["oe_fallbacks"] += 1
+        return fn(*args)
+
+    def _device_call(counter, fn, *args, **kwargs):
+        """fn on the device; None when the device refuses the input.  The reference's own exceptions are raised as the
+        patched module's classes."""
+        from . import _lib
+        from . import other_estimators as oe
+        from . import utils as u
+
+        n0 = oe.EVALUATIONS[0]
+        try:
+            out = fn(*args, **kwargs)
+        except _lib.MbarB200Error:
+            return None
+        except (u.ParameterError, u.ConvergenceError, u.BoundsError) as e:
+            for name in ("ParameterError", "ConvergenceError", "BoundsError"):
+                theirs = module.__dict__.get(name)
+                if isinstance(e, getattr(u, name)) and isinstance(theirs, type) and not isinstance(e, theirs):
+                    raise theirs(*e.args) from None
+            raise
+        finally:
+            STATS["oe_evaluations"] += oe.EVALUATIONS[0] - n0
+        STATS[counter] += 1
+        return (out,)
+
+    def bar(w_F, w_R, DeltaF=0.0, compute_uncertainty=True, uncertainty_method="BAR", maximum_iterations=500,
+            relative_tolerance=1.0e-12, verbose=False, method="false-position", iterated_solution=True):
+        from . import other_estimators as oe
+
+        args = (w_F, w_R, DeltaF, compute_uncertainty, uncertainty_method, maximum_iterations, relative_tolerance,
+                verbose, method, iterated_solution)
+        solver = method if iterated_solution else "self-consistent-iteration"
+        if (verbose or _oe_work(w_F) is None or _oe_work(w_R) is None or not isinstance(solver, str)
+                or solver not in oe.METHODS or not isinstance(uncertainty_method, str)
+                or uncertainty_method not in oe.UNCERTAINTY_METHODS):
+            return _fallback(orig_bar, *args)
+        r = _device_call("oe_bar", oe.bar, w_F, w_R, DeltaF=DeltaF, compute_uncertainty=compute_uncertainty,
+                         uncertainty_method=uncertainty_method, maximum_iterations=maximum_iterations,
+                         relative_tolerance=relative_tolerance, method=method, iterated_solution=iterated_solution)
+        return _fallback(orig_bar, *args) if r is None else r[0]
+
+    def bar_zero(w_F, w_R, DeltaF):
+        from . import other_estimators as oe
+
+        if _oe_work(w_F) is None or _oe_work(w_R) is None:
+            return _fallback(orig_zero, w_F, w_R, DeltaF)
+        r = _device_call("oe_bar_zero", oe.bar_zero, w_F, w_R, DeltaF)
+        return _fallback(orig_zero, w_F, w_R, DeltaF) if r is None else r[0]
+
+    def exp(w_F, compute_uncertainty=True, is_timeseries=False):
+        from . import other_estimators as oe
+
+        args = (w_F, compute_uncertainty, is_timeseries)
+        if _oe_work(w_F) is None:
+            return _fallback(orig_exp, *args)
+        r = _device_call("oe_exp", oe.exp, *args)
+        return _fallback(orig_exp, *args) if r is None else r[0]
+
+    def exp_gauss(w_F, compute_uncertainty=True, is_timeseries=False):
+        from . import other_estimators as oe
+
+        args = (w_F, compute_uncertainty, is_timeseries)
+        if _oe_work(w_F) is None:
+            return _fallback(orig_gauss, *args)
+        r = _device_call("oe_exp_gauss", oe.exp_gauss, *args)
+        return _fallback(orig_gauss, *args) if r is None else r[0]
+
+    for name, fn in zip(OE_NAMES, (bar, bar_zero, exp, exp_gauss)):
         if saved[name] is not None:
             fn.__doc__ = saved[name].__doc__
             setattr(module, name, fn)

@@ -27,7 +27,7 @@ from collections import OrderedDict
 import numpy as np
 import scipy.optimize
 
-from .problem import DeviceAcf, DeviceBSpline, DeviceKde, DeviceProblem  # noqa: F401  (DeviceKde, DeviceBSpline, DeviceAcf: looked up here by the facade)
+from .problem import DeviceAcf, DeviceBSpline, DeviceKde, DeviceProblem, DeviceWork  # noqa: F401  (DeviceKde, DeviceBSpline, DeviceAcf, DeviceWork: looked up here by the facade)
 from .utils import ParameterError, ensure_type
 
 logger = logging.getLogger(__name__)

@@ -580,6 +580,70 @@ class DeviceAcf:
                     waste=terms.value / useful.value if useful.value else 1.0)
 
 
+WORK_KINDS = ("fermi", "fermi_moments", "exp", "gauss")      # MBAR_B200_WORK_* in this order
+
+
+class DeviceWork:
+    """V work vectors resident on one H100 for the sums of pymbar.other_estimators (mbar_b200_work_*).  Independent of
+    any DeviceProblem.
+
+    `evaluate(vector, kind, c1, c2)` answers R requests in one device call and returns out [R, 3]: for kind "fermi"
+    logsumexp of bar_zero's term at a = (w + c1) + c2, for "fermi_moments" logsumexp(t), logsumexp(2 t) and
+    A = max(w + c1) of bar's uncertainty sums, for "exp" log(sum x) + max(-w), sum x and sum (x - mean x)^2 with
+    x = exp(-w - max(-w)), for "gauss" sum w and sum (w - mean w)^2 (include/mbar_b200.h)."""
+
+    def __init__(self, vectors, device=0):
+        self._lib = _lib.load()
+        self._h = C.c_void_p()
+        vs = [np.asarray(v) for v in vectors]
+        if not vs or any(v.ndim != 1 for v in vs):
+            raise ValueError("vectors must be a non-empty list of one-dimensional arrays")
+        self.lengths = np.array([v.size for v in vs], dtype=np.int64)
+        offsets = np.ascontiguousarray(np.concatenate([[0], np.cumsum(self.lengths)]), dtype=np.int64)
+        w = np.ascontiguousarray(np.concatenate(vs) if vs else np.zeros(0), dtype=np.float64)
+        self.device = int(device)
+        check(self._lib.mbar_b200_work_create(self.device, w.shape[0], _dptr(w), len(vs),
+                                              offsets.ctypes.data_as(C.POINTER(C.c_int64)), C.byref(self._h)))
+
+    def close(self):
+        if self._h is not None and self._h.value:
+            self._lib.mbar_b200_work_destroy(self._h)
+            self._h = None
+
+    def __del__(self):
+        try:
+            self.close()
+        except Exception:
+            pass
+
+    def __enter__(self):
+        return self
+
+    def __exit__(self, *exc):
+        self.close()
+
+    def evaluate(self, vector, kind, c1, c2):
+        """out [R, 3] for the requests (vector[r], kind[r], c1[r], c2[r]); a kind is a name of WORK_KINDS or its code."""
+        v = np.ascontiguousarray(np.atleast_1d(vector), dtype=np.int32)
+        k = np.ascontiguousarray([WORK_KINDS.index(x) if isinstance(x, str) and x in WORK_KINDS else
+                                  (-1 if isinstance(x, str) else int(x)) for x in np.atleast_1d(kind)], dtype=np.int32)
+        a = np.ascontiguousarray(np.broadcast_to(np.asarray(c1, dtype=np.float64), v.shape))
+        b = np.ascontiguousarray(np.broadcast_to(np.asarray(c2, dtype=np.float64), v.shape))
+        if k.shape != v.shape:
+            raise ValueError("vector and kind must have the same length")
+        out = np.empty((v.shape[0], 3))
+        i32 = C.POINTER(C.c_int32)
+        check(self._lib.mbar_b200_work_evaluate(self._h, v.shape[0], v.ctypes.data_as(i32), k.ctypes.data_as(i32),
+                                                _dptr(a), _dptr(b), _dptr(out)))
+        return out
+
+    def last_stats(self):
+        """CUDA-event time (ms) of the last evaluate's kernels, its launches, the work values and bytes it read."""
+        ms, launches, values = C.c_double(0), C.c_int32(0), C.c_int64(0)
+        check(self._lib.mbar_b200_last_work_stats(self._h, C.byref(ms), C.byref(launches), C.byref(values)))
+        return dict(ms=ms.value, launches=launches.value, values_read=values.value, bytes_read=8 * values.value)
+
+
 def measure_fp64_peak(device=0):
     """(DMMA TFLOP/s, DFMA TFLOP/s) of this GPU from register-only loops (mbar_b200_measure_fp64_peak)."""
     a, b = C.c_double(0), C.c_double(0)

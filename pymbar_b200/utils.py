@@ -12,6 +12,10 @@ class ConvergenceError(Exception):
     """pymbar.utils.ConvergenceError (utils.py:408)."""
 
 
+class BoundsError(Exception):
+    """pymbar.utils.BoundsError (utils.py:413)."""
+
+
 class TypeCastPerformanceWarning(RuntimeWarning):
     """pymbar.utils.TypeCastPerformanceWarning (utils.py:36)."""
 
