@@ -232,7 +232,27 @@ int mbar_b200_kde_destroy(mbar_b200_kde* kde);
  * -> MBAR_B200_ERR_INVALID; a NaN or infinite query coordinate -> MBAR_B200_ERR_NAN.  A failed call leaves the object
  * usable. */
 int mbar_b200_kde_log_sum(mbar_b200_kde* kde, int32_t kernel, double h, int64_t Q, const double* y_host, double* out);
-/* CUDA-event time of the kernels of the last mbar_b200_kde_log_sum and the number of sample chunks they split N into. */
+/* Bootstrap replicates of the resident samples (pymbar FES with fes_type="kde" and n_bootstraps > 0, fes.py:388-430,
+ * :690-699, :1590-1601): replicate b puts weight V_host[b, n] >= 0 on sample n (row-major [B, N]).  The reference fits
+ * replicate b to x_n[idx_b] with the weights of b = 0 by position, so V_bn is the sum of w_m over the positions m with
+ * idx_b[m] = n.  The weights stay on the device until the next call replaces them: 8 nPad (9 ceil(B/8) + 1) bytes,
+ * nPad = N rounded up to 256.  The host side is built one batch of 8 replicates at a time (8 * 9 nPad bytes).
+ * B < 1, or a negative, NaN or infinite weight -> MBAR_B200_ERR_INVALID (the object then holds no replicates). */
+int mbar_b200_kde_set_replicates(mbar_b200_kde* kde, int64_t B, const double* V_host);
+/* out [B, Q] row-major: out[b, q] = log sum_n V_bn k(d_qn / h), the log sum of mbar_b200_kde_log_sum with replicate
+ * b's weights, behind score_samples of the reference's B replicate KernelDensity objects (fes.py:1598-1601).  Every
+ * batch of 8 replicates is one pass over the samples: the distance, the kernel and one exp per (query, sample) pair
+ * serve the whole batch, under one running scale per query (the largest log V_bn + log k_qn of the batch).  Where
+ * that shared scale may have cut a replicate short (its log sum more than 549 - log N below the batch's scale at
+ * the query, -inf included: far queries), the entry is recomputed with the single-replicate pass, so every out[b, q]
+ * agrees with mbar_b200_kde_log_sum on weights V_b to 1e-12 relative and is -inf exactly when no V_bn k is nonzero.
+ * Results do not depend on Q, on the other queries or on replicates of other batches, and repeat calls are
+ * bit-identical.
+ * Errors as mbar_b200_kde_log_sum; no replicates uploaded -> MBAR_B200_ERR_NOT_READY. */
+int mbar_b200_kde_log_sum_replicates(mbar_b200_kde* kde, int32_t kernel, double h, int64_t Q, const double* y_host,
+                                     double* out);
+/* CUDA-event time of the kernels of the last mbar_b200_kde_log_sum or mbar_b200_kde_log_sum_replicates, and the number
+ * of sample chunks they split N into. */
 int mbar_b200_last_kde_stats(mbar_b200_kde* kde, double* ms, int32_t* chunks);
 
 /* ---- B-spline basis sums (pymbar FES with fes_type="spline", independent of any u_kn context) --- */

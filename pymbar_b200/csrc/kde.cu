@@ -45,6 +45,16 @@ struct mbar_b200_kde {
     cudaEvent_t ev0 = nullptr, ev1 = nullptr;
     double lastMs = 0.0;
     int lastChunks = 0;
+    // bootstrap replicates (mbar_b200_kde_set_replicates), in batches of KDE_REP_W
+    int64_t B = 0;
+    double* d_lvm = nullptr;     // [nRepBatches][nPad] log vmax_n = log max_b V_bn over the batch, -inf when 0
+    double* d_rat = nullptr;     // [nRepBatches * KDE_REP_W][nPad] V_bn / vmax_n (0 where vmax_n = 0, and padding rows)
+    double* d_rpm = nullptr;     // [nChunks][KDE_REP_W][rqCap] partials of one (replicate batch, query batch)
+    double* d_rps = nullptr;
+    double* d_rout = nullptr;    // [KDE_REP_W][rqCap]
+    double* d_rflag = nullptr;   // [KDE_REP_W][rqCap] 1 where the batch's shared scale may have lost digits
+    double* d_rlw = nullptr;     // [nPad] log V_bn of one replicate, for the exact pass over flagged queries
+    int64_t rqCap = 0;
 };
 
 namespace mbar {
@@ -57,6 +67,13 @@ constexpr size_t KDE_PART_BYTES = 64ull << 20;   // cap of the (m, s) partials o
 constexpr double KDE_RESCALE = 128.0;         // raise m when a term exceeds it by more than this
 constexpr double KDE_FLOOR = -1000.0;         // exp arguments are clamped here (result exactly 0)
 constexpr double KDE_HALF_PI = 1.5707963267948966;   // 0.5 * pi as sklearn's 0.5 * PI folds it
+constexpr int KDE_REP_W = 8;                  // bootstrap replicates served by one pass over the samples
+// What the shared scale of a replicate batch can lose (kde_replicates_kernel): a term or a rescaled partial sum is
+// flushed only when it lies below 2^-1021 ~ e^-707 of the running scale m, and a partial sum is at most (terms) e^128
+// of m (KDE_RESCALE), so all that is lost at a query is below N e^(M - 579), M the batch's final scale.  A replicate
+// whose log sum l >= M - (KDE_REP_EXACT - log N) therefore has lost less than e^-30 of its sum; every other entry
+// is recomputed by the single-replicate pass.
+constexpr double KDE_REP_EXACT = 707.0 - KDE_RESCALE - 30.0;
 
 enum { KDE_GAUSSIAN = 0, KDE_TOPHAT, KDE_EPANECHNIKOV, KDE_EXPONENTIAL, KDE_LINEAR, KDE_COSINE, KDE_NKERNELS };
 
@@ -163,6 +180,140 @@ __global__ void kde_combine_kernel(const double* __restrict__ pm, const double* 
     out[q] = M + log(S);
 }
 
+// kde_combine_kernel's rule for the W * Qb entries of a replicate batch, and flag[i] = 1 where the entry lies more
+// than thr below the batch's scale M (or is -inf while M is finite): there the shared scale may have lost digits
+__global__ void kde_rep_combine_kernel(const double* __restrict__ pm, const double* __restrict__ ps, int nChunks,
+                                       int nOut, double thr, double* __restrict__ out, double* __restrict__ flag) {
+    const int i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= nOut) return;
+    double M = -INFINITY;
+    for (int c = 0; c < nChunks; ++c) M = fmax(M, pm[(int64_t)c * nOut + i]);
+    if (M == -INFINITY) {
+        out[i] = -INFINITY;
+        flag[i] = 0.0;
+        return;
+    }
+    double S = 0.0;
+    for (int c = 0; c < nChunks; ++c) S += ps[(int64_t)c * nOut + i] * exp(pm[(int64_t)c * nOut + i] - M);
+    const double l = M + log(S);
+    out[i] = l;
+    flag[i] = l >= M - thr ? 0.0 : 1.0;
+}
+
+// log V_bn of one replicate from its batch's log vmax_n and ratio r_bn (-inf where r_bn = 0)
+__global__ void kde_rep_log_weight_kernel(const double* __restrict__ lvm, const double* __restrict__ rat,
+                                          int64_t nPad, double* __restrict__ lw) {
+    const int64_t n = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (n >= nPad) return;
+    const double r = rat[n];
+    lw[n] = r > 0.0 ? lvm[n] + log(r) : -INFINITY;
+}
+
+// kde_partial_kernel for a batch of KDE_REP_W bootstrap replicates with weights V_bn on the same samples
+// (mbar_b200_kde_log_sum_replicates).  p.lw holds log vmax_n, vmax_n = max_b V_bn over the batch, and rat [W][nPad]
+// the ratios r_bn = V_bn / vmax_n in [0, 1].  The distance, the kernel and one exp per (query, sample) pair serve all
+// W replicates: e = exp(log vmax_n + log k_qn - m) with one running scale m per query shared by the batch, and
+// s_b += r_bn e (r_bn e k for the compact kernels).  Partials are written [chunk][b][Qb], so that kde_combine_kernel
+// over W * Qb entries combines every replicate by its rule; m is stored once per replicate.
+template <int D, int KERN>
+__global__ void __launch_bounds__(KDE_THREADS) kde_replicates_kernel(KdeParams p, const double* __restrict__ rat) {
+    __shared__ double sx[D][KDE_TILE];
+    __shared__ double slv[KDE_TILE];
+    __shared__ double sr[KDE_REP_W][KDE_TILE];
+    __shared__ double tab[MBAR_EXP_NT];
+    if (threadIdx.x < MBAR_EXP_NT) tab[threadIdx.x] = MBAR_EXP_TABLE[threadIdx.x];
+    const int q = blockIdx.x * KDE_THREADS + threadIdx.x;
+    const int64_t n0 = (int64_t)blockIdx.y * p.chunkLen, n1 = min(n0 + p.chunkLen, p.nPad);
+    double y[D];
+#pragma unroll
+    for (int j = 0; j < D; ++j) y[j] = q < p.Qb ? p.y[(int64_t)j * p.Qb + q] : 0.0;
+    double m = -INFINITY, s[KDE_REP_W];
+#pragma unroll
+    for (int b = 0; b < KDE_REP_W; ++b) s[b] = 0.0;
+    for (int64_t t0 = n0; t0 < n1; t0 += KDE_TILE) {
+        __syncthreads();
+        for (int i = threadIdx.x; i < KDE_TILE; i += KDE_THREADS) {
+#pragma unroll
+            for (int j = 0; j < D; ++j) sx[j][i] = p.x[(int64_t)j * p.nPad + t0 + i];
+            slv[i] = p.lw[t0 + i];
+#pragma unroll
+            for (int b = 0; b < KDE_REP_W; ++b) sr[b][i] = rat[(int64_t)b * p.nPad + t0 + i];
+        }
+        __syncthreads();
+#pragma unroll 4
+        for (int i = 0; i < KDE_TILE; ++i) {
+            // distance, support and kernel exactly as kde_partial_kernel
+            double t = __dsub_rn(y[0], sx[0][i]);
+            double r = __dmul_rn(t, t);
+#pragma unroll
+            for (int j = 1; j < D; ++j) {
+                t = __dsub_rn(y[j], sx[j][i]);
+                r = __dadd_rn(r, __dmul_rn(t, t));
+            }
+            const double lv = slv[i];
+            double a, k = 1.0;
+            if (KERN == KDE_GAUSSIAN) {
+                a = fma(-r, p.c, lv);
+            } else if (KERN == KDE_TOPHAT) {
+                a = r < p.T ? lv : -INFINITY;
+            } else if (KERN == KDE_EXPONENTIAL) {
+                a = fma(-__dsqrt_rn(r), p.c, lv);
+            } else {
+                const double d = __dsqrt_rn(r);
+                const bool in = d < p.h;
+                a = in ? lv : -INFINITY;
+                if (KERN == KDE_EPANECHNIKOV) k = __dsub_rn(1.0, __ddiv_rn(__dmul_rn(d, d), p.hh));
+                if (KERN == KDE_LINEAR) k = __dsub_rn(1.0, __ddiv_rn(d, p.h));
+                if (KERN == KDE_COSINE) k = cos(__ddiv_rn(__dmul_rn(KDE_HALF_PI, d), p.h));
+                k = in ? k : 0.0;
+            }
+            double dl = a - m;
+            if (dl > KDE_RESCALE) {
+                const double g = exp_flush(fmax(m - a, KDE_FLOOR), tab);
+#pragma unroll
+                for (int b = 0; b < KDE_REP_W; ++b) s[b] *= g;
+                m = a;
+                dl = 0.0;
+            }
+            double e = exp_flush(fmax(dl, KDE_FLOOR), tab);
+            if (KERN == KDE_EPANECHNIKOV || KERN == KDE_LINEAR || KERN == KDE_COSINE) e *= k;
+#pragma unroll
+            for (int b = 0; b < KDE_REP_W; ++b) s[b] = fma(sr[b][i], e, s[b]);
+        }
+    }
+    if (q < p.Qb) {
+#pragma unroll
+        for (int b = 0; b < KDE_REP_W; ++b) {
+            const int64_t o = ((int64_t)blockIdx.y * KDE_REP_W + b) * p.Qb + q;
+            p.pm[o] = m;
+            p.ps[o] = s[b];
+        }
+    }
+}
+
+typedef void (*KdeRepKernelFn)(KdeParams, const double*);
+
+template <int D>
+static KdeRepKernelFn kde_rep_kernel_for(int kernel) {
+    switch (kernel) {
+        case KDE_GAUSSIAN: return kde_replicates_kernel<D, KDE_GAUSSIAN>;
+        case KDE_TOPHAT: return kde_replicates_kernel<D, KDE_TOPHAT>;
+        case KDE_EPANECHNIKOV: return kde_replicates_kernel<D, KDE_EPANECHNIKOV>;
+        case KDE_EXPONENTIAL: return kde_replicates_kernel<D, KDE_EXPONENTIAL>;
+        case KDE_LINEAR: return kde_replicates_kernel<D, KDE_LINEAR>;
+        default: return kde_replicates_kernel<D, KDE_COSINE>;
+    }
+}
+
+static KdeRepKernelFn kde_rep_kernel_for(int D, int kernel) {
+    switch (D) {
+        case 1: return kde_rep_kernel_for<1>(kernel);
+        case 2: return kde_rep_kernel_for<2>(kernel);
+        case 3: return kde_rep_kernel_for<3>(kernel);
+        default: return kde_rep_kernel_for<4>(kernel);
+    }
+}
+
 typedef void (*KdeKernelFn)(KdeParams);
 
 template <int D>
@@ -196,7 +347,8 @@ static double sqrt_threshold(double h) {
 }
 
 static void kde_release(mbar_b200_kde* k) {
-    for (double* p : {k->d_x, k->d_lw, k->d_y, k->d_pm, k->d_ps, k->d_out})
+    for (double* p : {k->d_x, k->d_lw, k->d_y, k->d_pm, k->d_ps, k->d_out, k->d_lvm, k->d_rat, k->d_rpm, k->d_rps,
+                      k->d_rout, k->d_rflag, k->d_rlw})
         if (p) cudaFree(p);
     if (k->ev0) cudaEventDestroy(k->ev0);
     if (k->ev1) cudaEventDestroy(k->ev1);
@@ -229,6 +381,30 @@ static int kde_reserve(mbar_b200_kde* k, int64_t qb) {
     MBAR_TRY(kde_alloc(&k->d_out, (size_t)qb));
     k->qCap = qb;
     return MBAR_B200_OK;
+}
+
+// the replicate pass's partials and results for up to qb queries, as kde_reserve
+static int kde_rep_reserve(mbar_b200_kde* k, int64_t qb) {
+    if (qb <= k->rqCap) return MBAR_B200_OK;
+    for (double** p : {&k->d_rpm, &k->d_rps, &k->d_rout, &k->d_rflag}) {
+        if (*p) cudaFree(*p);
+        *p = nullptr;
+    }
+    k->rqCap = 0;
+    MBAR_TRY(kde_alloc(&k->d_rpm, (size_t)k->nChunks * KDE_REP_W * qb));
+    MBAR_TRY(kde_alloc(&k->d_rps, (size_t)k->nChunks * KDE_REP_W * qb));
+    MBAR_TRY(kde_alloc(&k->d_rout, (size_t)KDE_REP_W * qb));
+    MBAR_TRY(kde_alloc(&k->d_rflag, (size_t)KDE_REP_W * qb));
+    k->rqCap = qb;
+    return MBAR_B200_OK;
+}
+
+static void kde_drop_replicates(mbar_b200_kde* k) {
+    for (double** p : {&k->d_lvm, &k->d_rat, &k->d_rlw}) {
+        if (*p) cudaFree(*p);
+        *p = nullptr;
+    }
+    k->B = 0;
 }
 
 }  // namespace mbar
@@ -365,6 +541,164 @@ int mbar_b200_kde_log_sum(mbar_b200_kde* k, int32_t kernel, double h, int64_t Q,
         MBAR_CUDA(cudaStreamSynchronize(k->stream));
         float e = 0.f;
         if (event_ms(k->ev0, k->ev1, &e)) ms += e;
+    }
+    k->lastMs = ms;
+    k->lastChunks = k->nChunks;
+    return MBAR_B200_OK;
+}
+
+int mbar_b200_kde_set_replicates(mbar_b200_kde* k, int64_t B, const double* V_host) {
+    MBAR_REQUIRE(k, MBAR_B200_ERR_INVALID, "kde_set_replicates: NULL object");
+    MBAR_CUDA(cudaSetDevice(k->device));
+    kde_drop_replicates(k);
+    MBAR_REQUIRE(B >= 1 && V_host, MBAR_B200_ERR_INVALID, "kde_set_replicates: B=%lld, V=%p", (long long)B,
+                 (const void*)V_host);
+    const int64_t N = k->N, nPad = k->nPad;
+    for (int64_t i = 0; i < B * N; ++i)
+        MBAR_REQUIRE(V_host[i] >= 0.0 && V_host[i] < INFINITY, MBAR_B200_ERR_INVALID, "kde_set_replicates: weight "
+                     "(%lld, %lld) is %g (negative, NaN or infinite)", (long long)(i / N), (long long)(i % N), V_host[i]);
+    // device: log vmax_n per batch of KDE_REP_W replicates, the ratios V_bn / vmax_n (rows past B stay 0), and one
+    // replicate's log weights for the exact pass: 8 nPad (9 nRB + 1) bytes
+    const int64_t nRB = (B + KDE_REP_W - 1) / KDE_REP_W;
+    int rc = MBAR_B200_OK;
+    if ((rc = kde_alloc(&k->d_lvm, (size_t)(nRB * nPad))) ||
+        (rc = kde_alloc(&k->d_rat, (size_t)(nRB * KDE_REP_W * nPad))) || (rc = kde_alloc(&k->d_rlw, (size_t)nPad))) {
+        kde_drop_replicates(k);
+        return rc;
+    }
+    // host: one batch at a time (8 nPad (1 + KDE_REP_W) bytes), rows read in order
+    std::vector<double> hl((size_t)nPad), hr((size_t)(KDE_REP_W * nPad));
+    for (int64_t rb = 0; rb < nRB; ++rb) {
+        const int64_t b0 = rb * KDE_REP_W, b1 = std::min(B, b0 + KDE_REP_W);
+        std::fill(hl.begin(), hl.end(), 0.0);
+        std::fill(hr.begin(), hr.end(), 0.0);
+        for (int64_t b = b0; b < b1; ++b)
+            for (int64_t n = 0; n < N; ++n) hl[(size_t)n] = std::max(hl[(size_t)n], V_host[b * N + n]);
+        for (int64_t b = b0; b < b1; ++b) {
+            double* r = hr.data() + (b - b0) * nPad;
+            for (int64_t n = 0; n < N; ++n)
+                if (hl[(size_t)n] > 0.0) r[n] = V_host[b * N + n] / hl[(size_t)n];
+        }
+        for (int64_t n = 0; n < nPad; ++n) hl[(size_t)n] = hl[(size_t)n] > 0.0 ? std::log(hl[(size_t)n]) : -INFINITY;
+        // synchronous per batch: the host buffers are reused by the next batch
+        if (cudaMemcpyAsync(k->d_lvm + rb * nPad, hl.data(), hl.size() * sizeof(double), cudaMemcpyHostToDevice,
+                            k->stream) != cudaSuccess ||
+            cudaMemcpyAsync(k->d_rat + rb * KDE_REP_W * nPad, hr.data(), hr.size() * sizeof(double),
+                            cudaMemcpyHostToDevice, k->stream) != cudaSuccess ||
+            cudaStreamSynchronize(k->stream) != cudaSuccess) {
+            set_error("kde_set_replicates: %s", cudaGetErrorString(cudaGetLastError()));
+            kde_drop_replicates(k);
+            return MBAR_B200_ERR_CUDA;
+        }
+    }
+    k->B = B;
+    return MBAR_B200_OK;
+}
+
+int mbar_b200_kde_log_sum_replicates(mbar_b200_kde* k, int32_t kernel, double h, int64_t Q, const double* y_host,
+                                     double* out) {
+    MBAR_REQUIRE(k, MBAR_B200_ERR_INVALID, "kde_log_sum_replicates: NULL object");
+    MBAR_REQUIRE(k->B >= 1, MBAR_B200_ERR_NOT_READY, "kde_log_sum_replicates: no replicates uploaded");
+    MBAR_REQUIRE(kernel >= 0 && kernel < KDE_NKERNELS, MBAR_B200_ERR_INVALID,
+                 "kde_log_sum_replicates: unknown kernel %d", (int)kernel);
+    MBAR_REQUIRE(std::isfinite(h) && h > 0.0, MBAR_B200_ERR_INVALID, "kde_log_sum_replicates: bandwidth %g must be "
+                 "finite and positive", h);
+    MBAR_REQUIRE(Q >= 0, MBAR_B200_ERR_INVALID, "kde_log_sum_replicates: Q=%lld", (long long)Q);
+    if (Q == 0) return MBAR_B200_OK;
+    MBAR_REQUIRE(y_host && out, MBAR_B200_ERR_INVALID, "kde_log_sum_replicates: NULL argument");
+    const int D = k->D;
+    for (int64_t i = 0; i < Q * D; ++i)
+        MBAR_REQUIRE(std::isfinite(y_host[i]), MBAR_B200_ERR_NAN, "kde_log_sum_replicates: query coordinate "
+                     "(%lld, %d) is %g", (long long)(i / D), (int)(i % D), y_host[i]);
+    MBAR_CUDA(cudaSetDevice(k->device));
+    NvtxRange nvtx_("mbar_b200::kde_log_sum_replicates");
+    int64_t cap = (int64_t)(KDE_PART_BYTES / (2 * sizeof(double) * KDE_REP_W * (size_t)k->nChunks));
+    cap = std::max<int64_t>(KDE_THREADS, cap / KDE_THREADS * KDE_THREADS);
+    const int64_t qb = std::min(Q, cap);
+    MBAR_TRY(kde_reserve(k, qb));
+    MBAR_TRY(kde_rep_reserve(k, qb));
+    KdeParams p{};
+    p.x = k->d_x;
+    p.y = k->d_y;
+    p.pm = k->d_rpm;
+    p.ps = k->d_rps;
+    p.nPad = k->nPad;
+    p.chunkLen = k->chunkLen;
+    p.h = h;
+    p.hh = h * h;
+    p.c = kernel == KDE_GAUSSIAN ? 0.5 / (h * h) : 1.0 / h;
+    p.T = sqrt_threshold(h);
+    const KdeRepKernelFn fn = kde_rep_kernel_for(D, kernel);
+    const int64_t nRB = (k->B + KDE_REP_W - 1) / KDE_REP_W;
+    const double thr = KDE_REP_EXACT - std::log((double)k->N);
+    std::vector<double> hy((size_t)D * qb), hflag((size_t)KDE_REP_W * qb);
+    std::vector<std::vector<int64_t>> redo((size_t)k->B);     // per replicate: queries for the exact pass
+    double ms = 0.0;
+    float e = 0.f;
+    for (int64_t q0 = 0; q0 < Q; q0 += qb) {
+        const int Qb = (int)std::min(qb, Q - q0);
+        for (int64_t i = 0; i < Qb; ++i)
+            for (int j = 0; j < D; ++j) hy[(size_t)j * Qb + i] = y_host[(q0 + i) * D + j];
+        MBAR_CUDA(cudaMemcpyAsync(k->d_y, hy.data(), (size_t)D * Qb * sizeof(double), cudaMemcpyHostToDevice,
+                                  k->stream));
+        p.Qb = Qb;
+        for (int64_t rb = 0; rb < nRB; ++rb) {
+            p.lw = k->d_lvm + rb * k->nPad;
+            const int64_t nb = std::min<int64_t>(KDE_REP_W, k->B - rb * KDE_REP_W);
+            MBAR_CUDA(cudaEventRecord(k->ev0, k->stream));
+            const dim3 grid((unsigned)((Qb + KDE_THREADS - 1) / KDE_THREADS), (unsigned)k->nChunks);
+            fn<<<grid, KDE_THREADS, 0, k->stream>>>(p, k->d_rat + rb * KDE_REP_W * k->nPad);
+            const int nOut = KDE_REP_W * Qb;
+            kde_rep_combine_kernel<<<(nOut + 127) / 128, 128, 0, k->stream>>>(k->d_rpm, k->d_rps, k->nChunks, nOut,
+                                                                              thr, k->d_rout, k->d_rflag);
+            MBAR_CUDA(cudaGetLastError());
+            MBAR_CUDA(cudaEventRecord(k->ev1, k->stream));
+            // rows b of the batch go to out[(rb W + b) Q + q0 ...]
+            MBAR_CUDA(cudaMemcpy2DAsync(out + rb * KDE_REP_W * Q + q0, (size_t)Q * sizeof(double), k->d_rout,
+                                        (size_t)Qb * sizeof(double), (size_t)Qb * sizeof(double), (size_t)nb,
+                                        cudaMemcpyDeviceToHost, k->stream));
+            MBAR_CUDA(cudaMemcpyAsync(hflag.data(), k->d_rflag, (size_t)(nb * Qb) * sizeof(double),
+                                      cudaMemcpyDeviceToHost, k->stream));
+            MBAR_CUDA(cudaStreamSynchronize(k->stream));
+            if (event_ms(k->ev0, k->ev1, &e)) ms += e;
+            for (int64_t b = 0; b < nb; ++b)
+                for (int64_t i = 0; i < Qb; ++i)
+                    if (hflag[(size_t)(b * Qb + i)] != 0.0) redo[(size_t)(rb * KDE_REP_W + b)].push_back(q0 + i);
+        }
+    }
+    // the entries the shared scale may have cut short: the single-replicate pass (kde_partial_kernel) on log V_bn
+    KdeParams p1 = p;
+    p1.lw = k->d_rlw;
+    p1.pm = k->d_pm;
+    p1.ps = k->d_ps;
+    const KdeKernelFn fn1 = kde_kernel_for(D, kernel);
+    std::vector<double> hout((size_t)qb);
+    for (int64_t b = 0; b < k->B; ++b) {
+        const std::vector<int64_t>& qs = redo[(size_t)b];
+        if (qs.empty()) continue;
+        const int64_t rb = b / KDE_REP_W;
+        kde_rep_log_weight_kernel<<<(unsigned)((k->nPad + 255) / 256), 256, 0, k->stream>>>(
+            k->d_lvm + rb * k->nPad, k->d_rat + b * k->nPad, k->nPad, k->d_rlw);
+        MBAR_CUDA(cudaGetLastError());
+        for (size_t i0 = 0; i0 < qs.size(); i0 += (size_t)qb) {
+            const int Qb = (int)std::min<size_t>((size_t)qb, qs.size() - i0);
+            for (int64_t i = 0; i < Qb; ++i)
+                for (int j = 0; j < D; ++j) hy[(size_t)j * Qb + i] = y_host[qs[i0 + i] * D + j];
+            MBAR_CUDA(cudaMemcpyAsync(k->d_y, hy.data(), (size_t)D * Qb * sizeof(double), cudaMemcpyHostToDevice,
+                                      k->stream));
+            p1.Qb = Qb;
+            MBAR_CUDA(cudaEventRecord(k->ev0, k->stream));
+            const dim3 grid((unsigned)((Qb + KDE_THREADS - 1) / KDE_THREADS), (unsigned)k->nChunks);
+            fn1<<<grid, KDE_THREADS, 0, k->stream>>>(p1);
+            kde_combine_kernel<<<(Qb + 127) / 128, 128, 0, k->stream>>>(k->d_pm, k->d_ps, k->nChunks, Qb, k->d_out);
+            MBAR_CUDA(cudaGetLastError());
+            MBAR_CUDA(cudaEventRecord(k->ev1, k->stream));
+            MBAR_CUDA(cudaMemcpyAsync(hout.data(), k->d_out, (size_t)Qb * sizeof(double), cudaMemcpyDeviceToHost,
+                                      k->stream));
+            MBAR_CUDA(cudaStreamSynchronize(k->stream));
+            if (event_ms(k->ev0, k->ev1, &e)) ms += e;
+            for (int64_t i = 0; i < Qb; ++i) out[b * Q + qs[i0 + i]] = hout[(size_t)i];
+        }
     }
     k->lastMs = ms;
     k->lastChunks = k->nChunks;

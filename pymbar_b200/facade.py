@@ -44,8 +44,19 @@ so only for the very x_n and w_n arrays the moments were built from and for spli
 any other call (bootstrap replicates, another x_n passed to `sample_parameter_distribution`, 2-D samples) runs the
 original method.  The optimiser, the Hessian, the information criteria and `_get_fes_spline` stay the reference's.
 
-FES bootstraps, bootstrap uncertainties, device errors and any call whose weights leave the device's range contract
-go to the original methods.
+`generate_fes` with n_bootstraps >= 2 for fes_type="histogram" or "kde" draws the replicates from numpy's global
+generator as fes.py:395-406 does (one MBAR seed draw after every block included) and keeps the generator's state
+before each replicate instead of its indices (`pymbar_b200.fes_bootstrap`).  A histogram replicate is one weighted
+solve on the resident problem and one bin pass with the replicate's multiplicities; `histogram_datas[b]` builds
+`bin_n`, `sample_label` and `nonzero_bins` on first read.  A KDE replicate has no solve: the replicate weights go to
+the DeviceKde once, `FES.kdes` fits replicate b only when read, and `_get_fes_kde(uncertainty_method="bootstrap")`
+answers "from-lowest" and "from-specified" from one `log_sum_replicates` call; `_get_fes_histogram` takes the std
+over the replicates as fes.py:1417-1422 does.  A replicate that empties a bin tuple of b = 0, a state without
+samples, spline bootstraps, other reference points, and device errors call the original with numpy's generator
+restored to its state at entry (`STATS["fes_boot_*"]`).
+
+Bootstrap uncertainties of surfaces generated without device replicates, device errors and any call whose weights
+leave the device's range contract go to the original methods.
 
 `install_timeseries_on` rebinds `statistical_inefficiency`, `statistical_inefficiency_multiple`,
 `normalized_fluctuation_correlation_function` and `detect_equilibration` of `pymbar.timeseries` to
@@ -77,7 +88,7 @@ STATS = {"tickets": 0, "redeemed": 0, "moments": 0, "expectations": 0, "expectat
          "fes_histograms": 0, "fes_theta": 0, "fes_w_kn": 0, "fes_kde_fits": 0, "fes_kde_queries": 0,
          "fes_spline_moments": 0, "fes_spline_calls": 0, "ts_inefficiency": 0, "ts_multiple": 0, "ts_correlation": 0,
          "ts_equilibration": 0, "ts_fallbacks": 0, "oe_bar": 0, "oe_bar_zero": 0, "oe_exp": 0, "oe_exp_gauss": 0,
-         "oe_evaluations": 0, "oe_fallbacks": 0}
+         "oe_evaluations": 0, "oe_fallbacks": 0, "fes_boot_solves": 0, "fes_boot_passes": 0, "fes_boot_fallbacks": 0}
 
 
 class LogWeightTicket:
@@ -351,6 +362,68 @@ def _spline_moments_for(fes, x_n, w_n, t, k, weights):
     return m
 
 
+def _histogram_bootstraps(fes, u_n, n_bootstraps):
+    """fes.histogram_datas for n_bootstraps replicates (fes.py:388-430), each one weighted solve and one bin pass on
+    the resident problem.  False, with numpy's generator advanced, when a replicate empties a bin tuple of b = 0 or
+    the device fails: the caller then restores the generator and runs the original."""
+    from . import _lib
+    from . import fes_bootstrap as fb
+    from . import mbar_solvers as ms
+
+    mbar = fes.mbar
+    N_k = np.asarray(mbar.N_k)
+    tuples, n_tuples = fb.tuple_index(fes.histogram_data["bin_n"])
+    covered = []
+    states = fb.draw_replicates(N_k, n_bootstraps,
+                                lambda b, idx: covered.append(fb.covers_every_tuple(idx, tuples, n_tuples)))
+    if not all(covered):
+        return False
+    protocol = fb.solver_protocol(ms.DEFAULT_SOLVER_PROTOCOL)
+
+    def solved():
+        STATS["fes_boot_solves"] += 1
+
+    try:
+        with ms._borrow(mbar.u_kn, np.asarray(N_k, dtype=np.float64)) as p:
+            if not hasattr(p, "set_sample_weights"):      # a backend without multiplicities (the tests' stand-in)
+                return False
+            datas = fb.histogram_replicates(p, np.asarray(mbar.f_k, dtype=np.float64), N_k, u_n,
+                                            fes.histogram_data, states, protocol, on_solve=solved)
+    except _lib.MbarB200Error:
+        return False
+    fes.histogram_datas = datas
+    return True
+
+
+def _kde_bootstraps(fes, x_n, n_bootstraps):
+    """The replicate weights V [B, N] of n_bootstraps KDE replicates (fes.py:388-430, :689-699) on fes's DeviceKde,
+    and fes.kdes as a ReplicateKdes.  False, with numpy's generator advanced, when the device refuses them."""
+    from . import _lib
+    from . import fes_bootstrap as fb
+
+    dev = fes.__dict__["_b200_kde_dev"][0]
+    if not hasattr(dev, "set_replicates"):         # a KDE backend without replicates (the tests' numpy stand-in)
+        return False
+    N_k = np.asarray(fes.mbar.N_k)
+    w = np.asarray(fes.w_n, dtype=np.float64)
+    V = np.empty((int(n_bootstraps), len(w)))
+
+    def weights(b, idx):
+        V[b] = np.bincount(idx, weights=w, minlength=len(w))
+
+    states = fb.draw_replicates(N_k, n_bootstraps, weights)
+    try:
+        dev.set_replicates(V)
+    except (_lib.MbarB200Error, ValueError):
+        return False
+
+    def fitted():
+        STATS["fes_kde_fits"] += 1
+
+    fes.kdes = fb.ReplicateKdes(fes.__dict__["_b200_kde"].get_params(), x_n, fes.w_n, N_k, states, on_fit=fitted)
+    return True
+
+
 def install_fes_on(FES):
     """Patch the class object `FES` (pymbar.fes.FES)."""
     if FES in _SAVED:
@@ -373,9 +446,23 @@ def install_fes_on(FES):
         # a DeviceKde, or spline moments, answer only for the surface the last generate_fes built
         _drop_device_kde(self)
         self.__dict__.pop("_b200_spline", None)
-        single = isinstance(n_bootstraps, (int, np.integer)) and not isinstance(n_bootstraps, bool) and n_bootstraps == 0
-        if not single or fes_type not in ("histogram", "kde", "spline"):
+        counted = isinstance(n_bootstraps, (int, np.integer)) and not isinstance(n_bootstraps, bool)
+        boot = counted and n_bootstraps >= 2
+        if not (boot or (counted and n_bootstraps == 0)) or fes_type not in ("histogram", "kde", "spline"):
             return orig_generate(self, *args)
+        entry = np.random.get_state() if boot else None
+
+        def fallback():
+            # the original from where the caller left numpy's generator: the same replicates, the same errors
+            STATS["fes_boot_fallbacks"] += 1
+            _drop_device_kde(self)
+            np.random.set_state(entry)
+            return orig_generate(self, *args)
+
+        # spline bootstraps need per-replicate basis sums; randint(0, 0) raises for an empty state, and the
+        # reference indexes x_n with the replicate's indices
+        if boot and (fes_type == "spline" or not isinstance(x_n, np.ndarray) or np.any(np.asarray(self.mbar.N_k) < 1)):
+            return fallback()
         from . import fes as hist
         from . import mbar_solvers as ms
         from .utils import kn_to_n
@@ -410,16 +497,22 @@ def install_fes_on(FES):
                 STATS["fes_histograms"] += 1
         except Exception as err:
             if _out_of_range(err):
-                return orig_generate(self, *args)
+                return fallback() if boot else orig_generate(self, *args)
             raise
         w_n = np.exp(log_w - np.max(log_w))
         self.w_n = w_n / np.sum(w_n)
         self.w_kn = WeightMatrixTicket(mbar)
         if fes_type == "histogram":
             self.histogram_data = data
+            if boot and not _histogram_bootstraps(self, u, n_bootstraps):
+                return fallback()
         elif fes_type == "kde":
             if not _device_kde(self, x_n):
+                if boot:
+                    return fallback()
                 self._generate_fes_kde(0, x_n, self.w_n)
+            elif boot and not _kde_bootstraps(self, x_n, n_bootstraps):
+                return fallback()
         else:
             _device_spline(self, x_n)
             self._generate_fes_spline(0, x_n, self.w_n)
@@ -428,7 +521,16 @@ def install_fes_on(FES):
         return result_vals
 
     def _get_fes_histogram(self, x, reference_point="from-lowest", fes_reference=None, uncertainty_method=None):
-        if uncertainty_method not in (None, "analytical") or reference_point not in ("from-lowest", "from-specified"):
+        from . import fes_bootstrap as fb
+
+        boot = uncertainty_method == "bootstrap"
+        datas = getattr(self, "histogram_datas", None)
+        served = boot and isinstance(datas, list) and len(datas) > 0 and \
+            all(isinstance(h, fb.ReplicateHistogram) for h in datas)
+        if (uncertainty_method not in (None, "analytical") and not served) or \
+                reference_point not in ("from-lowest", "from-specified"):
+            if boot:
+                STATS["fes_boot_fallbacks"] += 1
             return orig_get_hist(self, x, reference_point=reference_point, fes_reference=fes_reference,
                                  uncertainty_method=uncertainty_method)
         from . import fes as hist
@@ -436,6 +538,12 @@ def install_fes_on(FES):
 
         mbar = self.mbar
         K = mbar.K
+
+        if boot:
+            def df_fn(j):
+                return fb.bootstrap_df(datas, j, len(self.histogram_data["f"]))
+
+            return hist.query(self.histogram_data, x, reference_point, fes_reference, df_fn)
 
         def df_fn(j):
             STATS["fes_theta"] += 1
@@ -469,6 +577,21 @@ def install_fes_on(FES):
             if out is not None:
                 STATS["fes_kde_queries"] += 1
                 return out
+        if uncertainty_method == "bootstrap":
+            from . import _lib
+            from . import fes_bootstrap as fb
+
+            kdes = getattr(self, "kdes", None)
+            if (dev is not None and reference_point in ("from-lowest", "from-specified")
+                    and isinstance(kdes, fb.ReplicateKdes) and dev[0].B == len(kdes)):
+                try:
+                    out = fb.kde_bootstrap_query(dev[0], dev[1], x, reference_point, fes_reference, dev[2])
+                except _lib.MbarB200Error:
+                    out = None
+                if out is not None:
+                    STATS["fes_boot_passes"] += 1
+                    return out
+            STATS["fes_boot_fallbacks"] += 1
         return orig_get_kde(self, x, reference_point=reference_point, fes_reference=fes_reference,
                             uncertainty_method=uncertainty_method)
 

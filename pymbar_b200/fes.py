@@ -42,6 +42,12 @@ def _edges(bin_edges):
     return bin_edges
 
 
+def _first_rows(bin_n):
+    """Index of the first sample of each distinct row of bin_n, in order of first appearance."""
+    _, first = np.unique(bin_n, axis=0, return_index=True)
+    return np.sort(first)
+
+
 def histogram_labels(x_n, bin_edges):
     """Bin every sample as fes.py:513-573 does, without a Python loop over samples.
 
@@ -61,8 +67,7 @@ def histogram_labels(x_n, bin_edges):
     for d in range(dims):
         sample_label += bin_n[:, d] * len(bins[d]) ** d
     sample_label[np.any(bin_n < 0, axis=1)] = -1
-    _, first = np.unique(bin_n, axis=0, return_index=True)
-    first = np.sort(first)
+    first = _first_rows(bin_n)
     nonzero_bins = [tuple(int(v) for v in bin_n[n]) for n in first]
     bin_label = {t: int(sample_label[n]) for t, n in zip(nonzero_bins, first)}
     bin_order = {}
@@ -290,9 +295,11 @@ def _draw_as_sample(kernel, D):
     rng.normal(size=(1, D))
 
 
-def kde_query(kde, settings, x, reference_point, fes_reference, log_sum_w):
+def kde_query(kde, settings, x, reference_point, fes_reference, log_sum_w, with_fmin=False):
     """_get_fes_kde (fes.py:1523-1609) without uncertainties, from kde.log_sum (a DeviceKde): {"f_i", "df_i": None}
     with f_i = -score_samples(x) relative to the reference point, log_sum_w = log sum_n w_n of the fitted weights.
+    with_fmin=True also returns the reference's fmin, the -score_samples subtracted for "from-lowest" and
+    "from-specified" (None for "from-normalization"): (out, fmin).
 
     "from-specified" evaluates its reference point in the same call as the queries (a query's result does not
     depend on the others).  Raises what the reference raises: IndexError for 1-D x, NotImplementedError for kernels
@@ -320,15 +327,19 @@ def kde_query(kde, settings, x, reference_point, fes_reference, log_sum_w):
     score += kde_log_norm(kernel, D, h)
     score -= log_sum_w
     f_i = -score[:Q]
+    fmin = None
     if reference_point == "from-lowest":
-        f_i = f_i - np.min(f_i)
+        fmin = np.min(f_i)
+        f_i = f_i - fmin
     elif reference_point == "from-specified":
-        f_i = f_i - (-score[Q:])
+        fmin = -score[Q:]
+        f_i = f_i - fmin
     elif reference_point == "from-normalization":
         pass
     else:
         raise ParameterError(f"reference point choice {reference_point} for kde is unavailable")
-    return {"f_i": f_i, "df_i": None}
+    out = {"f_i": f_i, "df_i": None}
+    return (out, fmin) if with_fmin else out
 
 
 SPLINE_WEIGHTS = ("unbiasedstate", "biasedstates", "simplesum")

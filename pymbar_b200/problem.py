@@ -389,6 +389,7 @@ class DeviceKde:
         x = np.ascontiguousarray(x)
         w = _f64(w_n, x.shape[0])
         self.N, self.D = x.shape
+        self.B = 0                         # replicates uploaded by set_replicates
         self.device = int(device)
         check(self._lib.mbar_b200_kde_create(self.device, self.N, self.D, _dptr(x), _dptr(w), C.byref(self._h)))
 
@@ -409,8 +410,7 @@ class DeviceKde:
     def __exit__(self, *exc):
         self.close()
 
-    def log_sum(self, kernel, h, y):
-        """l_q [Q] for the queries y [Q, D] (or [Q] when D = 1); kernel is a name of KDE_KERNELS or its code."""
+    def _kernel_and_queries(self, kernel, y):
         code = KDE_KERNELS.index(kernel) if isinstance(kernel, str) and kernel in KDE_KERNELS else kernel
         if isinstance(code, str):
             code = -1                      # unknown name: the library reports ERR_INVALID
@@ -419,13 +419,35 @@ class DeviceKde:
             y = y.reshape(-1, 1)
         if y.ndim != 2 or y.shape[1] != self.D:
             raise ValueError(f"queries must be [Q, {self.D}], got shape {y.shape}")
-        y = np.ascontiguousarray(y)
+        return code, np.ascontiguousarray(y)
+
+    def log_sum(self, kernel, h, y):
+        """l_q [Q] for the queries y [Q, D] (or [Q] when D = 1); kernel is a name of KDE_KERNELS or its code."""
+        code, y = self._kernel_and_queries(kernel, y)
         out = np.empty(y.shape[0])
         check(self._lib.mbar_b200_kde_log_sum(self._h, int(code), float(h), y.shape[0], _dptr(y), _dptr(out)))
         return out
 
+    def set_replicates(self, V):
+        """Upload the weights V [B, N] of B bootstrap replicates of the resident samples (V_bn >= 0); they replace any
+        uploaded before and stay on the device for log_sum_replicates."""
+        V = np.ascontiguousarray(V, dtype=np.float64)
+        if V.ndim != 2 or V.shape[1] != self.N:
+            raise ValueError(f"replicate weights must be [B, {self.N}], got shape {V.shape}")
+        self.B = 0                         # a failed upload leaves none
+        check(self._lib.mbar_b200_kde_set_replicates(self._h, V.shape[0], _dptr(V)))
+        self.B = V.shape[0]
+
+    def log_sum_replicates(self, kernel, h, y):
+        """[B, Q]: log_sum with the weights of each uploaded replicate, all replicates in one device call."""
+        code, y = self._kernel_and_queries(kernel, y)
+        out = np.empty((self.B, y.shape[0]))
+        check(self._lib.mbar_b200_kde_log_sum_replicates(self._h, int(code), float(h), y.shape[0], _dptr(y),
+                                                         _dptr(out)))
+        return out
+
     def last_stats(self):
-        """CUDA-event time (ms) of the last log_sum's kernels and the number of sample chunks."""
+        """CUDA-event time (ms) of the last log_sum's or log_sum_replicates' kernels and the number of sample chunks."""
         ms, chunks = C.c_double(0), C.c_int32(0)
         check(self._lib.mbar_b200_last_kde_stats(self._h, C.byref(ms), C.byref(chunks)))
         return dict(ms=ms.value, chunks=chunks.value)
