@@ -277,7 +277,21 @@ int mbar_b200_bspline_destroy(mbar_b200_bspline* bspline);
  * a chunk's states are skipped). */
 int mbar_b200_bspline_moments(mbar_b200_bspline* bspline, int32_t degree, int64_t n_knots, const double* t, double* S,
                               double* A);
-/* CUDA-event time of the kernels of the last mbar_b200_bspline_moments and the number of row chunks they took. */
+/* Upload the weights V [B, N] row-major (V_bn >= 0) of B bootstrap replicates of the resident samples, replacing any
+ * uploaded before; they stay on the device (8 B nPad bytes, nPad = N rounded up to 32) until the next call or destroy.
+ * B < 1, or a negative, NaN or infinite weight -> MBAR_B200_ERR_INVALID, and the object then holds no replicates.
+ * The weights w and labels s of create are not touched. */
+int mbar_b200_bspline_set_replicates(mbar_b200_bspline* bspline, int64_t B, const double* V_host);
+/* out [B, nb] row-major: out[b, i] = sum_n V_bn B_i(x_n), the A of mbar_b200_bspline_moments with replicate b's
+ * weights, for every uploaded replicate in one call.  Each pass over the samples evaluates the basis once per sample
+ * for a batch of replicates.  Row b is summed in an order fixed by N and nb alone: it does not depend on B or on the
+ * other rows, and repeat calls are bit-identical; there are no floating-point atomics.  Degree and knot errors are
+ * those of mbar_b200_bspline_moments; no replicates uploaded -> MBAR_B200_ERR_NOT_READY.  A failed call leaves the
+ * object usable. */
+int mbar_b200_bspline_replicate_sums(mbar_b200_bspline* bspline, int32_t degree, int64_t n_knots, const double* t,
+                                     double* out);
+/* CUDA-event time of the kernels of the last mbar_b200_bspline_moments or mbar_b200_bspline_replicate_sums and the
+ * number of row chunks (moments) or replicate batches (replicate_sums) they took. */
 int mbar_b200_last_bspline_stats(mbar_b200_bspline* bspline, double* ms, int32_t* chunks);
 
 /* ---- lag sums of timeseries (pymbar.timeseries, independent of any u_kn context) --------------- */

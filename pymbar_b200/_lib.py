@@ -81,6 +81,8 @@ SIGNATURES = {
                                            C.POINTER(_ctx)]),
     "mbar_b200_bspline_destroy": (C.c_int, [_ctx]),
     "mbar_b200_bspline_moments": (C.c_int, [_ctx, C.c_int32, C.c_int64, _dp, _dp, _dp]),
+    "mbar_b200_bspline_set_replicates": (C.c_int, [_ctx, C.c_int64, _dp]),
+    "mbar_b200_bspline_replicate_sums": (C.c_int, [_ctx, C.c_int32, C.c_int64, _dp, _dp]),
     "mbar_b200_last_bspline_stats": (C.c_int, [_ctx, _dp, C.POINTER(C.c_int32)]),
     "mbar_b200_acf_create": (C.c_int, [C.c_int, C.c_int64, _dp, _dp, C.c_int32, C.POINTER(C.c_int64),
                                        C.POINTER(_ctx)]),

@@ -18,6 +18,14 @@
 // first index alone.  The per-CTA blocks are then summed in CTA order.  There are no atomics: the order of every
 // sum is fixed by N and the inputs, so repeat calls, and S-only, A-only or both, give the same bits.  Tiles without a
 // sample in a chunk's states are skipped (with the default labels every state's samples are contiguous).
+//
+// Replicate sums (mbar_b200_bspline_replicate_sums): R_bi = sum_n V_bn B_i(x_n) for B weight rows V uploaded once,
+// the sample terms of B bootstrap replicates of the fit.  A pass serves a batch of replicates: each warp evaluates a
+// tile's Cox-de Boor triangle once, groups its lanes by first basis index once, and then for every replicate of the
+// batch reads 32 consecutive V_bn and adds the segmented sums of V_bn B_{first + a} to its own [batch x nb]
+// accumulator, so the warps of a CTA never wait for each other.  Each CTA adds its warps' accumulators in warp order
+// and the CTAs are summed in CTA order.  The tiles a warp owns are fixed by N and the warps per CTA by nb, so row b's
+// sum is ordered by (N, nb) alone: it does not depend on B, on the batch it falls in or on the other rows.
 #include <algorithm>
 #include <cmath>
 #include <vector>
@@ -31,6 +39,7 @@ constexpr int BSP_WARPS = BSP_THREADS / 32;
 constexpr int BSP_MAX_DEGREE = 7;
 constexpr int BSP_ACC_DOUBLES = (108 * 1024) / 8;   // shared accumulator per CTA
 constexpr int64_t BSP_MAX_GROUPS = 264;              // CTAs per chunk: two per SM on an H100 SXM
+constexpr int BSP_REP_MAX_WARPS = 8;                 // warps per CTA of the replicate kernel (fewer for a large nb)
 
 }  // namespace mbar
 
@@ -45,6 +54,8 @@ struct mbar_b200_bspline {
     int32_t* d_s = nullptr;    // [nTiles * 32], -1 in the padding, or NULL
     int32_t* d_tmin = nullptr; // [nTiles] smallest / largest label of a tile (padding excluded)
     int32_t* d_tmax = nullptr;
+    int64_t B = 0;             // replicate rows uploaded by mbar_b200_bspline_set_replicates
+    double* d_V = nullptr;     // [B][nTiles * 32], 0 in the padding
     cudaStream_t stream = nullptr;
     cudaEvent_t ev0 = nullptr, ev1 = nullptr;
     double lastMs = 0.0;
@@ -220,6 +231,98 @@ __global__ void bsp_reduce_kernel(const double* __restrict__ partial, int nGroup
     else S[(int64_t)(k0 + r - hasA) * nb + b] = s;
 }
 
+struct BspRepParams {
+    const double* x;
+    const double* V;        // [B][nPad]
+    const double* t;        // knots [nKnots]
+    double* partial;        // [nGroups][rows][nb]
+    int64_t N, nTiles, nPad;
+    int64_t b0;             // first replicate of this pass
+    int nKnots, nb;
+    int nGroups;
+    int rows;               // replicates in this pass
+};
+
+// One pass over the samples for replicates [b0, b0 + rows): blockDim.x / 32 warps, each with its own accumulator.
+template <int KD>
+__global__ void __launch_bounds__(BSP_REP_MAX_WARPS * 32) bsp_replicate_kernel(BspRepParams p) {
+    extern __shared__ double smem[];
+    __shared__ int perm[BSP_REP_MAX_WARPS][32];
+    const unsigned FULL = 0xffffffffu;
+    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5, nWarps = blockDim.x >> 5;
+    const int cells = p.rows * p.nb;
+    double* st = smem;                                   // knots
+    double* acc = smem + p.nKnots;                       // [nWarps][rows][nb]
+    for (int i = threadIdx.x; i < nWarps * cells; i += blockDim.x) acc[i] = 0.0;
+    for (int i = threadIdx.x; i < p.nKnots; i += blockDim.x) st[i] = p.t[i];
+    __syncthreads();
+    double* wacc = acc + (size_t)warp * cells;
+    const int64_t g = blockIdx.x;
+    const int64_t t0 = g * p.nTiles / p.nGroups, t1 = (g + 1) * p.nTiles / p.nGroups;
+    for (int64_t tile = t0 + warp; tile < t1; tile += nWarps) {
+        const int64_t n = tile * TILE_N + lane;
+        double h[KD + 1];
+        const int first = bsp_basis<KD>(st, p.nKnots, p.nb, p.x[n], h);
+        int skey, steps;
+        unsigned same;
+        const int src = bsp_sort(n < p.N ? first : -1, lane, perm[warp], skey, same, steps);
+        // the basis values in sorted order, once per tile
+        double hs[KD + 1];
+#pragma unroll
+        for (int a = 0; a <= KD; ++a) hs[a] = __shfl_sync(FULL, h[a], src);
+        const int next = __shfl_down_sync(FULL, skey, 1);
+        const bool tail = skey >= 0 && (lane == 31 || next != skey);
+        const double* vrow = p.V + p.b0 * p.nPad + n;
+        for (int r = 0; r < p.rows; ++r) {
+            const double v = __shfl_sync(FULL, vrow[(int64_t)r * p.nPad], src);
+            const int cell = r * p.nb + skey;
+#pragma unroll
+            for (int a = 0; a <= KD; ++a) {
+                double y = __dmul_rn(v, hs[a]);
+                // segmented inclusive sum over the sorted groups: the group's last lane holds its total
+                for (int s = 0; s < steps; ++s) {
+                    const double z = __shfl_up_sync(FULL, y, 1 << s);
+                    if ((same >> s) & 1u) y += z;
+                }
+                if (tail) wacc[cell + a] += y;
+                __syncwarp();
+            }
+        }
+    }
+    __syncthreads();
+    double* dst = p.partial + g * cells;
+    for (int i = threadIdx.x; i < cells; i += blockDim.x) {
+        double s = 0.0;
+        for (int w = 0; w < nWarps; ++w) s += acc[(size_t)w * cells + i];
+        dst[i] = s;
+    }
+}
+
+// out[(b0 + r) * nb + i] = partials of (r, i) summed in CTA order
+__global__ void bsp_replicate_reduce_kernel(const double* __restrict__ partial, int nGroups, int cells, int64_t b0,
+                                            int nb, double* __restrict__ out) {
+    const int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= cells) return;
+    double s = 0.0;
+    for (int g = 0; g < nGroups; ++g) s += partial[(int64_t)g * cells + i];
+    out[b0 * nb + i] = s;
+}
+
+typedef void (*BspRepKernelFn)(BspRepParams);
+
+static BspRepKernelFn bsp_replicate_kernel_for(int degree) {
+    switch (degree) {
+        case 0: return bsp_replicate_kernel<0>;
+        case 1: return bsp_replicate_kernel<1>;
+        case 2: return bsp_replicate_kernel<2>;
+        case 3: return bsp_replicate_kernel<3>;
+        case 4: return bsp_replicate_kernel<4>;
+        case 5: return bsp_replicate_kernel<5>;
+        case 6: return bsp_replicate_kernel<6>;
+        default: return bsp_replicate_kernel<7>;
+    }
+}
+
 typedef void (*BspKernelFn)(BspParams);
 
 static BspKernelFn bsp_kernel_for(int degree) {
@@ -236,7 +339,7 @@ static BspKernelFn bsp_kernel_for(int degree) {
 }
 
 static void bsp_release(mbar_b200_bspline* b) {
-    for (void* p : {(void*)b->d_x, (void*)b->d_w, (void*)b->d_s, (void*)b->d_tmin, (void*)b->d_tmax})
+    for (void* p : {(void*)b->d_x, (void*)b->d_w, (void*)b->d_s, (void*)b->d_tmin, (void*)b->d_tmax, (void*)b->d_V})
         if (p) cudaFree(p);
     if (b->ev0) cudaEventDestroy(b->ev0);
     if (b->ev1) cudaEventDestroy(b->ev1);
@@ -367,25 +470,31 @@ int mbar_b200_bspline_destroy(mbar_b200_bspline* b) {
     return MBAR_B200_OK;
 }
 
-int mbar_b200_bspline_moments(mbar_b200_bspline* b, int32_t degree, int64_t n_knots, const double* t, double* S,
-                              double* A) {
-    MBAR_REQUIRE(b, MBAR_B200_ERR_INVALID, "bspline_moments: NULL object");
-    MBAR_REQUIRE(degree >= 0 && degree <= BSP_MAX_DEGREE, MBAR_B200_ERR_INVALID,
-                 "bspline_moments: degree %d outside [0, %d]", (int)degree, BSP_MAX_DEGREE);
-    MBAR_REQUIRE(t, MBAR_B200_ERR_INVALID, "bspline_moments: NULL knots");
+// The degree and knot checks of mbar_b200_bspline_moments and mbar_b200_bspline_replicate_sums.
+static int bsp_check_knots(const char* fn, int32_t degree, int64_t n_knots, const double* t) {
+    MBAR_REQUIRE(degree >= 0 && degree <= BSP_MAX_DEGREE, MBAR_B200_ERR_INVALID, "%s: degree %d outside [0, %d]", fn,
+                 (int)degree, BSP_MAX_DEGREE);
+    MBAR_REQUIRE(t, MBAR_B200_ERR_INVALID, "%s: NULL knots", fn);
     MBAR_REQUIRE(n_knots >= 2 * (int64_t)(degree + 1), MBAR_B200_ERR_INVALID,
-                 "bspline_moments: %lld knots, degree %d needs at least %d", (long long)n_knots, (int)degree,
-                 2 * (degree + 1));
+                 "%s: %lld knots, degree %d needs at least %d", fn, (long long)n_knots, (int)degree, 2 * (degree + 1));
     for (int64_t i = 0; i < n_knots; ++i) {
-        MBAR_REQUIRE(std::isfinite(t[i]), MBAR_B200_ERR_INVALID, "bspline_moments: knot %lld is %g", (long long)i, t[i]);
-        MBAR_REQUIRE(i == 0 || t[i] >= t[i - 1], MBAR_B200_ERR_INVALID, "bspline_moments: knots decrease at %lld",
+        MBAR_REQUIRE(std::isfinite(t[i]), MBAR_B200_ERR_INVALID, "%s: knot %lld is %g", fn, (long long)i, t[i]);
+        MBAR_REQUIRE(i == 0 || t[i] >= t[i - 1], MBAR_B200_ERR_INVALID, "%s: knots decrease at %lld", fn,
                      (long long)i);
     }
     const int64_t nb64 = n_knots - degree - 1;
-    MBAR_REQUIRE(t[degree] < t[nb64], MBAR_B200_ERR_INVALID, "bspline_moments: t[k] = t[nb] = %g (empty base interval)",
+    MBAR_REQUIRE(t[degree] < t[nb64], MBAR_B200_ERR_INVALID, "%s: t[k] = t[nb] = %g (empty base interval)", fn,
                  t[degree]);
     MBAR_REQUIRE(nb64 <= BSP_ACC_DOUBLES - n_knots, MBAR_B200_ERR_INVALID,
-                 "bspline_moments: %lld basis functions exceed one accumulator", (long long)nb64);
+                 "%s: %lld basis functions exceed one accumulator", fn, (long long)nb64);
+    return MBAR_B200_OK;
+}
+
+int mbar_b200_bspline_moments(mbar_b200_bspline* b, int32_t degree, int64_t n_knots, const double* t, double* S,
+                              double* A) {
+    MBAR_REQUIRE(b, MBAR_B200_ERR_INVALID, "bspline_moments: NULL object");
+    MBAR_TRY(bsp_check_knots("bspline_moments", degree, n_knots, t));
+    const int64_t nb64 = n_knots - degree - 1;
     MBAR_REQUIRE(!S || b->d_s, MBAR_B200_ERR_INVALID, "bspline_moments: S requested but no labels were uploaded");
     MBAR_REQUIRE(!A || b->d_w, MBAR_B200_ERR_INVALID, "bspline_moments: A requested but no weights were uploaded");
     MBAR_REQUIRE((int64_t)b->K * nb64 < INT32_MAX, MBAR_B200_ERR_INVALID, "bspline_moments: K * nb too large");
@@ -442,6 +551,102 @@ int mbar_b200_bspline_moments(mbar_b200_bspline* b, int32_t degree, int64_t n_kn
     float e = 0.f;
     b->lastMs = event_ms(b->ev0, b->ev1, &e) ? e : 0.0;
     b->lastChunks = chunks;
+    return MBAR_B200_OK;
+}
+
+int mbar_b200_bspline_set_replicates(mbar_b200_bspline* b, int64_t B, const double* V_host) {
+    MBAR_REQUIRE(b, MBAR_B200_ERR_INVALID, "bspline_set_replicates: NULL object");
+    MBAR_CUDA(cudaSetDevice(b->device));
+    // a failed upload leaves no replicates
+    if (b->d_V) {
+        cudaStreamSynchronize(b->stream);
+        cudaFree(b->d_V);
+        b->d_V = nullptr;
+    }
+    b->B = 0;
+    MBAR_REQUIRE(B >= 1 && V_host, MBAR_B200_ERR_INVALID, "bspline_set_replicates: B=%lld, V=%p", (long long)B,
+                 (const void*)V_host);
+    const int64_t N = b->N, nPad = b->nTiles * TILE_N;
+    for (int64_t i = 0; i < B * N; ++i)
+        MBAR_REQUIRE(V_host[i] >= 0.0 && V_host[i] < INFINITY, MBAR_B200_ERR_INVALID, "bspline_set_replicates: weight "
+                     "(%lld, %lld) is %g (negative, NaN or infinite)", (long long)(i / N), (long long)(i % N),
+                     V_host[i]);
+    const size_t bytes = (size_t)B * nPad * sizeof(double);
+    const cudaError_t e = cudaMalloc((void**)&b->d_V, bytes);
+    if (e != cudaSuccess) {
+        b->d_V = nullptr;
+        cudaGetLastError();
+        set_error("bspline_set_replicates: cannot allocate %zu bytes", bytes);
+        return e == cudaErrorMemoryAllocation ? MBAR_B200_ERR_NOMEM : MBAR_B200_ERR_CUDA;
+    }
+    // rows of N into rows of nPad, the padding zeroed
+    bool ok = cudaMemcpy2DAsync(b->d_V, nPad * sizeof(double), V_host, N * sizeof(double), N * sizeof(double),
+                                (size_t)B, cudaMemcpyHostToDevice, b->stream) == cudaSuccess;
+    if (ok && nPad > N)
+        ok = cudaMemset2DAsync(b->d_V + N, nPad * sizeof(double), 0, (nPad - N) * sizeof(double), (size_t)B,
+                               b->stream) == cudaSuccess;
+    if (!ok || cudaStreamSynchronize(b->stream) != cudaSuccess) {
+        set_error("bspline_set_replicates: %s", cudaGetErrorString(cudaGetLastError()));
+        cudaFree(b->d_V);
+        b->d_V = nullptr;
+        return MBAR_B200_ERR_CUDA;
+    }
+    b->B = B;
+    return MBAR_B200_OK;
+}
+
+int mbar_b200_bspline_replicate_sums(mbar_b200_bspline* b, int32_t degree, int64_t n_knots, const double* t,
+                                     double* out) {
+    MBAR_REQUIRE(b, MBAR_B200_ERR_INVALID, "bspline_replicate_sums: NULL object");
+    MBAR_TRY(bsp_check_knots("bspline_replicate_sums", degree, n_knots, t));
+    MBAR_REQUIRE(out, MBAR_B200_ERR_INVALID, "bspline_replicate_sums: NULL output");
+    MBAR_REQUIRE(b->d_V && b->B >= 1, MBAR_B200_ERR_NOT_READY, "bspline_replicate_sums: no replicates uploaded");
+    const int nb = (int)(n_knots - degree - 1), nk = (int)n_knots;
+    MBAR_CUDA(cudaSetDevice(b->device));
+    NvtxRange nvtx_("mbar_b200::bspline_replicate_sums");
+    // warps per CTA from nb alone (each warp holds a [rows x nb] accumulator), then as many replicates per pass as
+    // the shared accumulator holds
+    int warps = BSP_REP_MAX_WARPS;
+    while (warps > 1 && (int64_t)warps * nb + nk > BSP_ACC_DOUBLES) warps >>= 1;
+    const int rowsPer = (int)std::max<int64_t>(1, std::min<int64_t>(b->B, (BSP_ACC_DOUBLES - nk) / ((int64_t)warps * nb)));
+    BspBuffers buf;
+    double *d_t, *d_partial, *d_out;
+    MBAR_TRY(buf.alloc(&d_t, (size_t)nk));
+    MBAR_TRY(buf.alloc(&d_partial, (size_t)b->nGroups * rowsPer * nb));
+    MBAR_TRY(buf.alloc(&d_out, (size_t)b->B * nb));
+    MBAR_CUDA(cudaMemcpyAsync(d_t, t, (size_t)nk * sizeof(double), cudaMemcpyHostToDevice, b->stream));
+    const BspRepKernelFn fn = bsp_replicate_kernel_for(degree);
+    const size_t smem = ((size_t)warps * rowsPer * nb + nk) * sizeof(double);
+    MBAR_CUDA(cudaFuncSetAttribute(fn, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+    BspRepParams p{};
+    p.x = b->d_x;
+    p.V = b->d_V;
+    p.t = d_t;
+    p.partial = d_partial;
+    p.N = b->N;
+    p.nTiles = b->nTiles;
+    p.nPad = b->nTiles * TILE_N;
+    p.nKnots = nk;
+    p.nb = nb;
+    p.nGroups = b->nGroups;
+    MBAR_CUDA(cudaEventRecord(b->ev0, b->stream));
+    int passes = 0;
+    for (int64_t b0 = 0; b0 < b->B; b0 += rowsPer) {
+        p.b0 = b0;
+        p.rows = (int)std::min<int64_t>(rowsPer, b->B - b0);
+        fn<<<b->nGroups, warps * 32, smem, b->stream>>>(p);
+        const int cells = p.rows * nb;
+        bsp_replicate_reduce_kernel<<<(unsigned)((cells + 255) / 256), 256, 0, b->stream>>>(d_partial, b->nGroups,
+                                                                                           cells, b0, nb, d_out);
+        MBAR_CUDA(cudaGetLastError());
+        ++passes;
+    }
+    MBAR_CUDA(cudaEventRecord(b->ev1, b->stream));
+    MBAR_CUDA(cudaMemcpyAsync(out, d_out, (size_t)b->B * nb * sizeof(double), cudaMemcpyDeviceToHost, b->stream));
+    MBAR_CUDA(cudaStreamSynchronize(b->stream));
+    float e = 0.f;
+    b->lastMs = event_ms(b->ev0, b->ev1, &e) ? e : 0.0;
+    b->lastChunks = passes;
     return MBAR_B200_OK;
 }
 

@@ -41,8 +41,17 @@ the spline coefficients, so `_bspline_calculate_f`, `_bspline_calculate_g` and `
 them (`pymbar_b200.fes.spline_objective` / `spline_gradient` / `spline_mc_loglikelihood`) with O(K nb) arithmetic
 and the reference's quadratures, where the reference evaluates the spline on every sample at every step.  They do
 so only for the very x_n and w_n arrays the moments were built from and for splines on the same knots and degree;
-any other call (bootstrap replicates, another x_n passed to `sample_parameter_distribution`, 2-D samples) runs the
-original method.  The optimiser, the Hessian, the information criteria and `_get_fes_spline` stay the reference's.
+any other call (another x_n passed to `sample_parameter_distribution`, 2-D samples) runs the original method.  The
+optimiser, the Hessian, the information criteria and `_get_fes_spline` stay the reference's.
+
+`generate_fes(fes_type="spline", n_bootstraps >= 2)` with 1-D samples in block order fits b = 0 as above, then draws
+the replicates as the reference does and gives every replicate's sample terms from one
+`DeviceBSpline.replicate_sums` call over weights V_b built on the host (`pymbar_b200.fes_bootstrap.spline_replicates`;
+"unbiasedstate" runs one weighted solve per replicate for its log denominators, the other weightings none).  Each
+replicate is fitted by the reference's `_generate_fes_spline(b, x_nb, w_nb)`, whose objective and gradient answer
+from that replicate's terms, and appended to `fes_functions`; `_get_fes_spline` takes its bootstrap std from them
+as the reference does.  Samples out of block order, 2-D samples, an unknown spline_weights and device errors call
+the original with numpy's generator and the spline_parameters restored (`STATS["fes_boot_spline_*"]`).
 
 `generate_fes` with n_bootstraps >= 2 for fes_type="histogram" or "kde" draws the replicates from numpy's global
 generator as fes.py:395-406 does (one MBAR seed draw after every block included) and keeps the generator's state
@@ -52,8 +61,8 @@ solve on the resident problem and one bin pass with the replicate's multipliciti
 the DeviceKde once, `FES.kdes` fits replicate b only when read, and `_get_fes_kde(uncertainty_method="bootstrap")`
 answers "from-lowest" and "from-specified" from one `log_sum_replicates` call; `_get_fes_histogram` takes the std
 over the replicates as fes.py:1417-1422 does.  A replicate that empties a bin tuple of b = 0, a state without
-samples, spline bootstraps, other reference points, and device errors call the original with numpy's generator
-restored to its state at entry (`STATS["fes_boot_*"]`).
+samples, other reference points, and device errors call the original with numpy's generator restored to its state at
+entry (`STATS["fes_boot_*"]`).
 
 Bootstrap uncertainties of surfaces generated without device replicates, device errors and any call whose weights
 leave the device's range contract go to the original methods.
@@ -88,7 +97,8 @@ STATS = {"tickets": 0, "redeemed": 0, "moments": 0, "expectations": 0, "expectat
          "fes_histograms": 0, "fes_theta": 0, "fes_w_kn": 0, "fes_kde_fits": 0, "fes_kde_queries": 0,
          "fes_spline_moments": 0, "fes_spline_calls": 0, "ts_inefficiency": 0, "ts_multiple": 0, "ts_correlation": 0,
          "ts_equilibration": 0, "ts_fallbacks": 0, "oe_bar": 0, "oe_bar_zero": 0, "oe_exp": 0, "oe_exp_gauss": 0,
-         "oe_evaluations": 0, "oe_fallbacks": 0, "fes_boot_solves": 0, "fes_boot_passes": 0, "fes_boot_fallbacks": 0}
+         "oe_evaluations": 0, "oe_fallbacks": 0, "fes_boot_solves": 0, "fes_boot_passes": 0, "fes_boot_fallbacks": 0,
+         "fes_boot_spline_solves": 0, "fes_boot_spline_sums": 0}
 
 
 class LogWeightTicket:
@@ -355,11 +365,101 @@ def _device_spline(fes, x_n):
     fes.__dict__["_b200_spline"] = SplineMoments(x_n, fes.w_n, labels, t, k, weights, S, A, fes.N)
 
 
-def _spline_moments_for(fes, x_n, w_n, t, k, weights):
-    m = fes.__dict__.get("_b200_spline")
+class ReplicateSplineTerms:
+    """The sample terms v of one bootstrap replicate's spline fit, for the replicate's own x_nb and w_nb arrays (the
+    ones passed to _generate_fes_spline) on the fit's knots t and degree k."""
+
+    __slots__ = ("x", "w", "t", "k", "weights", "v")
+
+    def __init__(self, x, w, t, k, weights, v):
+        self.x, self.w, self.t, self.k, self.weights, self.v = x, w, t, k, weights, v
+
+    def serves(self, x_n, w_n, t, k):
+        return x_n is self.x and w_n is self.w and k == self.k and np.array_equal(t, self.t)
+
+
+def _spline_moments_for(fes, x_n, w_n, t, k, weights, slot="_b200_spline"):
+    m = fes.__dict__.get(slot)
     if m is None or weights != m.weights or not m.serves(x_n, w_n, t, k):
         return None
     return m
+
+
+def _spline_boot_served(fes, x_n, spline_parameters):
+    """True when the device serves the spline replicates: 1-D samples, a known spline_weights, and samples in block
+    order (the reference labels replicate positions with b = 0's x_kindices, which are the replicate's samples' own
+    labels only in block order)."""
+    from . import fes as hist
+    from . import fes_bootstrap as fb
+
+    mbar = fes.mbar
+    return (np.ndim(x_n) == 1 and isinstance(spline_parameters, dict)
+            and spline_parameters.get("spline_weights") in hist.SPLINE_WEIGHTS
+            and fb.in_block_order(mbar.x_kindices, mbar.N_k))
+
+
+def _spline_bootstraps(fes, x_n, u_n, n_bootstraps):
+    """fes.fes_functions for n_bootstraps spline replicates (fes.py:388-430, :971-1098).  The replicates are drawn as
+    the reference draws them; "unbiasedstate" runs one weighted solve per replicate on the resident problem for its
+    log denominators, the other weightings none.  One DeviceBSpline.replicate_sums call gives every replicate's sample
+    terms, and each replicate is then fitted by fes._generate_fes_spline(b, x_nb, w_nb) with its objective and
+    gradient answered from them.  False, with numpy's generator advanced, when the device refuses: the caller then
+    restores the generator and runs the original."""
+    from . import _lib
+    from . import fes_bootstrap as fb
+    from . import mbar_solvers as ms
+    from .bootstrap import bootstrap_f_k
+
+    mbar = fes.mbar
+    N_k = np.asarray(mbar.N_k)
+    weights = fes.spline_parameters["spline_weights"]
+    spline = fes.spline_data["bspline"]
+    t, k = np.array(spline.t, dtype=np.float64), int(spline.k)
+    f_k = np.asarray(mbar.f_k, dtype=np.float64)
+    times = {"solves": 0.0}
+    try:
+        start = _timer()
+        with ms._borrow(mbar.u_kn, np.asarray(N_k, dtype=np.float64)) as p:
+            if weights == "unbiasedstate" and not hasattr(p, "set_sample_weights"):
+                return False                    # a backend without multiplicities (the tests' stand-in)
+            protocol = fb.solver_protocol(ms.DEFAULT_SOLVER_PROTOCOL)
+
+            def log_weights(idx):
+                t0 = _timer()
+                f_b = bootstrap_f_k(p, f_k, N_k, rints=idx[None], solver_protocol=protocol)[0]
+                L = p.log_denominator(f_b)
+                STATS["fes_boot_spline_solves"] += 1
+                times["solves"] += _timer() - t0
+                return -u_n - L
+
+            states, V = fb.spline_replicates(N_k, n_bootstraps, weights, log_weights)
+        times["draws"] = _timer() - start - times["solves"]
+        start = _timer()
+        dev = ms.DeviceBSpline(np.asarray(x_n, dtype=np.float64), device=ms._DEVICE)
+        try:
+            if not hasattr(dev, "replicate_sums"):
+                return False                    # a backend without replicates (the tests' plain numpy stand-in)
+            dev.set_replicates(V)
+            R = dev.replicate_sums(t, k)
+            times["sums_kernel_ms"] = dev.last_stats()["ms"] if hasattr(dev, "last_stats") else None
+        finally:
+            dev.close()
+    except (_lib.MbarB200Error, ValueError, TypeError):
+        return False
+    STATS["fes_boot_spline_sums"] += 1
+    times["sums"] = _timer() - start
+    v = fes.N * R if weights == "unbiasedstate" else R
+    start = _timer()
+    try:
+        for b, state in enumerate(states):
+            x_nb, w_nb = fb.spline_replicate_samples(state, N_k, x_n, V[b], weights)
+            fes.__dict__["_b200_spline_replicate"] = ReplicateSplineTerms(x_nb, w_nb, t, k, weights, v[b])
+            fes._generate_fes_spline(b + 1, x_nb, w_nb)
+    finally:
+        fes.__dict__.pop("_b200_spline_replicate", None)
+    times["fits"] = _timer() - start
+    fes.__dict__["_b200_spline_boot_times"] = times
+    return True
 
 
 def _histogram_bootstraps(fes, u_n, n_bootstraps):
@@ -446,23 +546,38 @@ def install_fes_on(FES):
         # a DeviceKde, or spline moments, answer only for the surface the last generate_fes built
         _drop_device_kde(self)
         self.__dict__.pop("_b200_spline", None)
+        self.__dict__.pop("_b200_spline_boot_times", None)
         counted = isinstance(n_bootstraps, (int, np.integer)) and not isinstance(n_bootstraps, bool)
         boot = counted and n_bootstraps >= 2
         if not (boot or (counted and n_bootstraps == 0)) or fes_type not in ("histogram", "kde", "spline"):
             return orig_generate(self, *args)
         entry = np.random.get_state() if boot else None
+        restore = []
 
         def fallback():
-            # the original from where the caller left numpy's generator: the same replicates, the same errors
+            # the original from where the caller left numpy's generator (the same replicates, the same errors) and
+            # with the spline_parameters it was given (_setup_fes_spline edits them in place)
             STATS["fes_boot_fallbacks"] += 1
             _drop_device_kde(self)
+            self.__dict__.pop("_b200_spline", None)
+            for undo in restore:
+                undo()
             np.random.set_state(entry)
             return orig_generate(self, *args)
 
-        # spline bootstraps need per-replicate basis sums; randint(0, 0) raises for an empty state, and the
-        # reference indexes x_n with the replicate's indices
-        if boot and (fes_type == "spline" or not isinstance(x_n, np.ndarray) or np.any(np.asarray(self.mbar.N_k) < 1)):
+        # randint(0, 0) raises for an empty state, and the reference indexes x_n with the replicate's indices
+        if boot and (not isinstance(x_n, np.ndarray) or np.any(np.asarray(self.mbar.N_k) < 1)):
             return fallback()
+        if boot and fes_type == "spline":
+            if not _spline_boot_served(self, x_n, spline_parameters):
+                return fallback()
+            given = {key: (dict(v) if isinstance(v, dict) else v) for key, v in spline_parameters.items()}
+
+            def undo_setup():
+                spline_parameters.clear()
+                spline_parameters.update(given)
+
+            restore.append(undo_setup)
         from . import fes as hist
         from . import mbar_solvers as ms
         from .utils import kn_to_n
@@ -515,7 +630,11 @@ def install_fes_on(FES):
                 return fallback()
         else:
             _device_spline(self, x_n)
+            if boot and "_b200_spline" not in self.__dict__:
+                return fallback()
             self._generate_fes_spline(0, x_n, self.w_n)
+            if boot and not _spline_bootstraps(self, x_n, u, n_bootstraps):
+                return fallback()
         if timings:
             result_vals["timing"] = _timer() - start
         return result_vals
@@ -596,8 +715,13 @@ def install_fes_on(FES):
                             uncertainty_method=uncertainty_method)
 
     def _fit_moments(self, x_n, w_n):
+        # b = 0's moments, or the sample terms of the bootstrap replicate being fitted
         b = self.spline_data["bspline"]
-        return _spline_moments_for(self, x_n, w_n, b.t, b.k, self.spline_parameters.get("spline_weights"))
+        weights = self.spline_parameters.get("spline_weights")
+        m = _spline_moments_for(self, x_n, w_n, b.t, b.k, weights)
+        if m is None:
+            m = _spline_moments_for(self, x_n, w_n, b.t, b.k, weights, slot="_b200_spline_replicate")
+        return m
 
     def _bspline_calculate_f(self, xi, x_n, w_n):
         m = _fit_moments(self, x_n, w_n)

@@ -1,4 +1,5 @@
-"""Bootstrap replicates of pymbar's FES (fes.py:388-430) for fes_type="histogram" and "kde", from the resident problem.
+"""Bootstrap replicates of pymbar's FES (fes.py:388-430) for fes_type="histogram", "kde" and "spline", from the
+resident problem.
 
 The reference resamples every state's block of samples and, inside the loop over states, builds a full MBAR on the
 gathered u_kn[:, idx] for each block (fes.py:395-406): K solves, K gathers of 8 K N bytes and K draws of the MBAR
@@ -15,7 +16,12 @@ constructor's seed (mbar.py:273-274) per replicate, of which only the last solve
 * a KDE replicate needs no solve: the reference fits replicate b to x_n[idx_b] with the weights of b = 0 by position
   (fes.py:696), so its weight on sample n is V_bn = sum of w_m over the positions m with idx_b[m] = n, and
   DeviceKde.log_sum_replicates scores every replicate in one device call.  FES.kdes becomes a ReplicateKdes whose
-  item b is fitted as the reference fits it when something reads it.
+  item b is fitted as the reference fits it when something reads it;
+* a spline replicate's fit needs only its sample terms v_b (fes.spline_sample_terms): with samples in block order and
+  c_bn = #{m : idx_b[m] = n}, v_b[i] = sum_n V_bn B_i(x_n) with V_bn = c_bn ("biasedstates"), c_bn N / (K N_{s_n})
+  ("simplesum") or N c_bn e^{-u_n - L^{(b)}_n} / Z_b ("unbiasedstate", where L^{(b)} comes from one weighted solve
+  and Z_b normalises as fes.py:412-414 does).  spline_replicates draws the stream and builds V; one
+  DeviceBSpline.replicate_sums call then gives every v_b.
 """
 from __future__ import annotations
 
@@ -181,6 +187,58 @@ class ReplicateKdes(Sequence):
             if self._on_fit is not None:
                 self._on_fit()
         return self._fitted[b]
+
+
+def in_block_order(x_kindices, N_k):
+    """True when the samples are in block order (state k's N_k[k] samples after those of states < k)."""
+    N_k = np.asarray(N_k, dtype=np.int64)
+    return np.array_equal(np.asarray(x_kindices), np.repeat(np.arange(len(N_k)), N_k))
+
+
+def replicate_weights(c, log_w):
+    """V_n = c_n e^{log_w_n} / sum_m c_m e^{log_w_m}: the reference's normalised replicate weights w_nb (fes.py:410-414)
+    summed over the positions that repeat sample n.  Samples the replicate does not draw get 0."""
+    V = np.zeros(len(c))
+    sel = c > 0
+    e = c[sel] * np.exp(log_w[sel] - np.max(log_w[sel]))
+    V[sel] = e / np.sum(e)
+    return V
+
+
+def spline_replicates(N_k, n_bootstraps, spline_weights, replicate_log_weights=None):
+    """(states, V [B, N]): the generator states of n_bootstraps replicates drawn as the reference draws them
+    (draw_replicates) and the weight of every resident sample in each replicate's spline sample terms, with samples in
+    block order.  V_b is c_b ("biasedstates"), c_b N / (K N_{s_n}) ("simplesum"), or replicate_weights(c_b,
+    replicate_log_weights(idx_b)) ("unbiasedstate"; the callable returns -u_n - L^{(b)}_n of the replicate's solve,
+    and the caller multiplies the sums by N).  Every N_k[k] must be >= 1."""
+    N_k = np.asarray(N_k, dtype=np.int64)
+    K, N = len(N_k), int(np.sum(N_k))
+    V = np.empty((int(n_bootstraps), N))
+    scale = np.repeat(N / (K * N_k.astype(np.float64)), N_k) if spline_weights == "simplesum" else None
+
+    def each(b, idx):
+        c = np.bincount(idx, minlength=N).astype(np.float64)
+        if spline_weights == "unbiasedstate":
+            V[b] = replicate_weights(c, replicate_log_weights(idx))
+        elif spline_weights == "simplesum":
+            V[b] = c * scale
+        elif spline_weights == "biasedstates":
+            V[b] = c
+        else:
+            raise ValueError(f"spline_weights {spline_weights!r} is not one of {hist.SPLINE_WEIGHTS}")
+
+    return draw_replicates(N_k, n_bootstraps, each), V
+
+
+def spline_replicate_samples(state, N_k, x_n, V_b, spline_weights):
+    """(x_nb, w_nb): the samples and weights the reference passes to _generate_fes_spline for the replicate drawn from
+    `state` (fes.py:406-430).  w_nb is rebuilt from V_b for "unbiasedstate"; the other weightings never read it and
+    get None, as no solve is run for them."""
+    idx = replicate_indices(state, N_k)
+    if spline_weights != "unbiasedstate":
+        return x_n[idx], None
+    c = np.bincount(idx, minlength=len(V_b)).astype(np.float64)
+    return x_n[idx], V_b[idx] / c[idx]
 
 
 def kde_bootstrap_query(kde, settings, x, reference_point, fes_reference, log_sum_w):

@@ -478,6 +478,7 @@ class DeviceBSpline:
             # labels beyond int32 become -1, which the library rejects
             s = np.ascontiguousarray(np.where((s_raw >= -1) & (s_raw < 2 ** 31 - 1), s_raw, -1), dtype=np.int32)
         self.K = int(K) if s is not None else 0
+        self.B = 0                         # replicates uploaded by set_replicates
         self.has_weights, self.has_labels = w is not None, s is not None
         self.device = int(device)
         check(self._lib.mbar_b200_bspline_create(
@@ -513,8 +514,30 @@ class DeviceBSpline:
                                                   None if S is None else _dptr(S), None if A is None else _dptr(A)))
         return S, A
 
+    def set_replicates(self, V):
+        """Upload the weights V [B, N] of B bootstrap replicates of the resident samples (V_bn >= 0); they replace any
+        uploaded before and stay on the device for replicate_sums.  The weights and labels of the constructor are
+        kept."""
+        V = np.ascontiguousarray(V, dtype=np.float64)
+        if V.ndim != 2 or V.shape[1] != self.N:
+            raise ValueError(f"replicate weights must be [B, {self.N}], got shape {V.shape}")
+        self.B = 0                         # a failed upload leaves none
+        check(self._lib.mbar_b200_bspline_set_replicates(self._h, V.shape[0], _dptr(V)))
+        self.B = V.shape[0]
+
+    def replicate_sums(self, t, k):
+        """[B, nb]: row b is sum_n V_bn B_i(x_n), the A of moments with replicate b's weights, for every uploaded
+        replicate in one device call."""
+        t = np.ascontiguousarray(t, dtype=np.float64)
+        if t.ndim != 1:
+            raise ValueError(f"knots must be one-dimensional, got shape {t.shape}")
+        out = np.empty((self.B, max(t.shape[0] - int(k) - 1, 0)))
+        check(self._lib.mbar_b200_bspline_replicate_sums(self._h, int(k), t.shape[0], _dptr(t), _dptr(out)))
+        return out
+
     def last_stats(self):
-        """CUDA-event time (ms) of the last moments call's kernels and the number of row chunks."""
+        """CUDA-event time (ms) of the last moments or replicate_sums call's kernels and the number of row chunks
+        (moments) or replicate batches (replicate_sums)."""
         ms, chunks = C.c_double(0), C.c_int32(0)
         check(self._lib.mbar_b200_last_bspline_stats(self._h, C.byref(ms), C.byref(chunks)))
         return dict(ms=ms.value, chunks=chunks.value)
