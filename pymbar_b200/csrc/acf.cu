@@ -21,6 +21,7 @@
 // number of rounds grows like log L.
 #include <algorithm>
 #include <cmath>
+#include <memory>
 #include <vector>
 
 #include "internal.cuh"
@@ -36,20 +37,17 @@ constexpr int64_t ACF_PART_BUDGET = int64_t(1) << 25;   // doubles of (start, la
 
 }  // namespace mbar
 
-struct mbar_b200_acf {
-    int device = 0;
+struct mbar_b200_acf : mbar::Resident {
     int64_t T = 0;
     int64_t NC = 0, nChunks = 0;
     int cross = 0;
     int nSeg = 0;                       // 0: one series
-    double* d_a = nullptr;
-    double* d_b = nullptr;              // == d_a for an autocorrelation
-    int64_t* d_segEnd = nullptr;        // [T] end of the segment holding n, or NULL
-    int64_t* d_segLen = nullptr;        // [nSeg]
+    mbar::DevArray<double> d_a;
+    mbar::DevArray<double> d_bOwn;      // B of a cross-correlation
+    double* d_b = nullptr;              // the B the kernels read: d_bOwn, or d_a for an autocorrelation
+    mbar::DevArray<int64_t> d_segEnd;   // [T] end of the segment holding n, or NULL
+    mbar::DevArray<int64_t> d_segLen;   // [nSeg]
     std::vector<int64_t> segLen;
-    cudaStream_t stream = nullptr;
-    cudaEvent_t ev0 = nullptr, ev1 = nullptr;
-    double lastMs = 0.0;
     int lastRounds = 0;
     int64_t lastTerms = 0, lastUseful = 0;
 };
@@ -254,36 +252,6 @@ __global__ void acf_corr_kernel(const double* __restrict__ S, const int64_t* __r
     C[k] = __ddiv_rn(num, __dmul_rn(__dmul_rn(2.0, (double)(m - lags[k])), sigma2[0]));
 }
 
-static void acf_release(mbar_b200_acf* o) {
-    for (void* p : {(void*)o->d_a, (void*)(o->d_b == o->d_a ? nullptr : o->d_b), (void*)o->d_segEnd,
-                    (void*)o->d_segLen})
-        if (p) cudaFree(p);
-    if (o->ev0) cudaEventDestroy(o->ev0);
-    if (o->ev1) cudaEventDestroy(o->ev1);
-    if (o->stream) cudaStreamDestroy(o->stream);
-    delete o;
-}
-
-// Device buffers of one call, released on every return path.
-struct AcfBuffers {
-    std::vector<void*> ptrs;
-    ~AcfBuffers() {
-        for (void* p : ptrs) cudaFree(p);
-    }
-    template <class T>
-    int alloc(T** p, size_t count) {
-        *p = nullptr;
-        const cudaError_t e = cudaMalloc((void**)p, std::max<size_t>(count, 1) * sizeof(T));
-        if (e != cudaSuccess) {
-            cudaGetLastError();
-            set_error("acf: cannot allocate %zu bytes", count * sizeof(T));
-            return e == cudaErrorMemoryAllocation ? MBAR_B200_ERR_NOMEM : MBAR_B200_ERR_CUDA;
-        }
-        ptrs.push_back((void*)*p);
-        return MBAR_B200_OK;
-    }
-};
-
 // Lag sums of the call starts act_h[] (indices into d_starts) for the ascending lags lags_h[], into d_S [nAct][B]
 // at columns col0.. (B = row stride).  Splits starts and lags so that one launch's partials fit the budget.
 struct AcfLagRunner {
@@ -364,83 +332,36 @@ int mbar_b200_acf_create(int device, int64_t T, const double* a, const double* b
         MBAR_REQUIRE(!b || std::isfinite(b[n]), MBAR_B200_ERR_NAN, "acf_create: B[%lld] is %g", (long long)n,
                      b ? b[n] : 0.0);
     }
-    int ndev = 0;
-    if (cudaGetDeviceCount(&ndev) != cudaSuccess || ndev == 0) {
-        cudaGetLastError();
-        set_error("no CUDA device visible: libmbar_b200 has no CPU fallback");
-        return MBAR_B200_ERR_NO_DEVICE;
-    }
-    MBAR_REQUIRE(device >= 0 && device < ndev, MBAR_B200_ERR_INVALID, "device %d of %d", device, ndev);
-    MBAR_CUDA(cudaSetDevice(device));
-    cudaDeviceProp prop;
-    MBAR_CUDA(cudaGetDeviceProperties(&prop, device));
-    if (prop.major != 9 || prop.minor != 0) {
-        set_error("device %d is sm_%d%d; this library is built for sm_90a (H100) only", device, prop.major, prop.minor);
-        return MBAR_B200_ERR_NO_DEVICE;
-    }
-    mbar_b200_acf* o = new mbar_b200_acf();
-    o->device = device;
+    MBAR_TRY(open_device(device, nullptr));
+    std::unique_ptr<mbar_b200_acf> o(new mbar_b200_acf());
     o->T = T;
     o->NC = std::max<int64_t>(ACF_MIN_NC, (T + ACF_MAX_CHUNKS - 1) / ACF_MAX_CHUNKS);
     o->nChunks = (T + o->NC - 1) / o->NC;
     o->cross = b ? 1 : 0;
     o->nSeg = n_segments;
-    auto fail = [&](int status) {
-        acf_release(o);
-        return status;
-    };
-    if (cudaStreamCreateWithFlags(&o->stream, cudaStreamNonBlocking) != cudaSuccess ||
-        cudaEventCreate(&o->ev0) != cudaSuccess || cudaEventCreate(&o->ev1) != cudaSuccess) {
-        set_error("acf_create: %s", cudaGetErrorString(cudaGetLastError()));
-        return fail(MBAR_B200_ERR_CUDA);
-    }
-    auto put = [&](auto** dst, const auto* src, size_t count) -> int {
-        using T_ = typename std::remove_const<typename std::remove_pointer<decltype(src)>::type>::type;
-        if (cudaMalloc((void**)dst, count * sizeof(T_)) != cudaSuccess) {
-            *dst = nullptr;
-            cudaGetLastError();
-            set_error("acf_create: cannot allocate %zu bytes", count * sizeof(T_));
-            return MBAR_B200_ERR_NOMEM;
-        }
-        if (cudaMemcpyAsync(*dst, src, count * sizeof(T_), cudaMemcpyHostToDevice, o->stream) != cudaSuccess) {
-            set_error("acf_create: %s", cudaGetErrorString(cudaGetLastError()));
-            return MBAR_B200_ERR_CUDA;
-        }
-        return MBAR_B200_OK;
-    };
-    std::vector<int64_t> segEnd;
-    int rc = put(&o->d_a, a, (size_t)T);
-    if (!rc && b) rc = put(&o->d_b, b, (size_t)T);
-    if (!rc && !b) o->d_b = o->d_a;
-    if (!rc && n_segments > 0) {
-        segEnd.resize((size_t)T);
+    const char* who = "acf_create";
+    MBAR_TRY(o->open(device, who));
+    MBAR_TRY(o->upload(o->d_a, a, (size_t)T, who));
+    if (b) MBAR_TRY(o->upload(o->d_bOwn, b, (size_t)T, who));
+    o->d_b = b ? o->d_bOwn : o->d_a;
+    if (n_segments > 0) {
+        std::vector<int64_t> segEnd((size_t)T);
         o->segLen.resize((size_t)n_segments);
         for (int k = 0; k < n_segments; ++k) {
             o->segLen[k] = offsets[k + 1] - offsets[k];
             for (int64_t n = offsets[k]; n < offsets[k + 1]; ++n) segEnd[n] = offsets[k + 1];
         }
-        rc = put(&o->d_segEnd, segEnd.data(), (size_t)T);
-        if (!rc) rc = put(&o->d_segLen, o->segLen.data(), (size_t)n_segments);
+        MBAR_TRY(o->upload(o->d_segEnd, segEnd.data(), (size_t)T, who));
+        MBAR_TRY(o->upload(o->d_segLen, o->segLen.data(), (size_t)n_segments, who));
     }
-    if (rc) return fail(rc);
-    if (cudaStreamSynchronize(o->stream) != cudaSuccess) {
-        set_error("acf_create: %s", cudaGetErrorString(cudaGetLastError()));
-        return fail(MBAR_B200_ERR_CUDA);
-    }
-    *out = o;
+    *out = o.release();
     return MBAR_B200_OK;
 }
 
-int mbar_b200_acf_destroy(mbar_b200_acf* o) {
-    if (!o) return MBAR_B200_OK;
-    cudaSetDevice(o->device);
-    if (o->stream) cudaStreamSynchronize(o->stream);
-    acf_release(o);
-    return MBAR_B200_OK;
-}
+int mbar_b200_acf_destroy(mbar_b200_acf* o) { return destroy_resident(o); }
 
 // means and sigma^2 of the call's starts (device arrays d_starts [n]); done[j] = 1 where sigma^2 == 0
-static int acf_moments(mbar_b200_acf* o, AcfBuffers& buf, const int64_t* d_starts, const std::vector<int64_t>& starts,
+static int acf_moments(mbar_b200_acf* o, CallBuffers& buf, const int64_t* d_starts, const std::vector<int64_t>& starts,
                        AcfLagRunner& run, double* d_muA, double* d_muB, double* d_s2, int32_t* d_status,
                        int8_t* d_done) {
     const int64_t n = (int64_t)starts.size();
@@ -496,7 +417,7 @@ int mbar_b200_acf_inefficiency(mbar_b200_acf* o, int64_t n_starts, const int64_t
     for (int64_t L : o->segLen) limitMultiple = std::max(limitMultiple, L);
     int64_t maxLimit = 0;
     for (int64_t s : hs) maxLimit = std::max(maxLimit, rule == 1 ? limitMultiple : o->T - s);
-    AcfBuffers buf;
+    CallBuffers buf("acf");
     int64_t* d_starts;
     double *d_muA, *d_muB, *d_s2, *d_g, *d_S, *d_partial, *d_trace = nullptr;
     int64_t *d_last, *d_lags;
@@ -640,7 +561,7 @@ int mbar_b200_acf_correlation(mbar_b200_acf* o, int64_t start, int64_t n_max, do
                  "acf_correlation: N_max %lld outside [0, %lld]", (long long)n_max, (long long)(o->T - start - 1));
     MBAR_CUDA(cudaSetDevice(o->device));
     NvtxRange nvtx_("mbar_b200::acf_correlation");
-    AcfBuffers buf;
+    CallBuffers buf("acf");
     int64_t *d_starts, *d_lags;
     double *d_muA, *d_muB, *d_s2, *d_S, *d_C, *d_partial;
     int32_t *d_status, *d_act;

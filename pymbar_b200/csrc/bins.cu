@@ -252,26 +252,6 @@ static BinPlan plan_bins(int nrows, int nbins, int64_t nTiles, int smCount) {
     return best;
 }
 
-// Device buffers of one call, released on every return path.
-struct DevBuffers {
-    std::vector<void*> ptrs;
-    ~DevBuffers() {
-        for (void* p : ptrs) cudaFree(p);
-    }
-    template <class T>
-    int alloc(T** p, size_t count) {
-        *p = nullptr;
-        const cudaError_t e = cudaMalloc((void**)p, std::max<size_t>(count, 1) * sizeof(T));
-        if (e != cudaSuccess) {
-            cudaGetLastError();
-            set_error("bin_moments: cannot allocate %zu bytes", count * sizeof(T));
-            return e == cudaErrorMemoryAllocation ? MBAR_B200_ERR_NOMEM : MBAR_B200_ERR_CUDA;
-        }
-        ptrs.push_back((void*)*p);
-        return MBAR_B200_OK;
-    }
-};
-
 // nrows x nbins sums of a * right over the bins: rows [0, Kw) are W_nk, row Kw the auxiliary row.
 static int run_accum(mbar_b200_ctx* c, BinParams p, int nbins, double* d_out, double* d_partial, const BinPlan& pl) {
     p.partial = d_partial;
@@ -317,7 +297,7 @@ int mbar_b200_bin_moments(mbar_b200_ctx* c, const double* f_k, const double* u_n
     const bool wantC = C || D;
     const BinPlan sumPlan = plan_bins(1, nbins, c->nTiles, c->smCount);
     const BinPlan momPlan = plan_bins(K + 1, nbins, c->nTiles, c->smCount);
-    DevBuffers buf;
+    CallBuffers buf("bin_moments");
     int* d_bin;
     int* d_flag;
     double *d_lw, *d_f, *d_m, *d_o, *d_s, *d_fbin, *d_partial, *d_out = nullptr;

@@ -28,6 +28,7 @@
 // sum is ordered by (N, nb) alone: it does not depend on B, on the batch it falls in or on the other rows.
 #include <algorithm>
 #include <cmath>
+#include <memory>
 #include <vector>
 
 #include "internal.cuh"
@@ -43,22 +44,18 @@ constexpr int BSP_REP_MAX_WARPS = 8;                 // warps per CTA of the rep
 
 }  // namespace mbar
 
-struct mbar_b200_bspline {
-    int device = 0;
+struct mbar_b200_bspline : mbar::Resident {
     int64_t N = 0;
     int64_t nTiles = 0;        // ceil(N / 32)
     int K = 0;                 // states (0: no labels)
     int nGroups = 1;           // CTAs per chunk, a function of N alone
-    double* d_x = nullptr;     // [nTiles * 32], 0 in the padding
-    double* d_w = nullptr;     // [nTiles * 32] or NULL
-    int32_t* d_s = nullptr;    // [nTiles * 32], -1 in the padding, or NULL
-    int32_t* d_tmin = nullptr; // [nTiles] smallest / largest label of a tile (padding excluded)
-    int32_t* d_tmax = nullptr;
-    int64_t B = 0;             // replicate rows uploaded by mbar_b200_bspline_set_replicates
-    double* d_V = nullptr;     // [B][nTiles * 32], 0 in the padding
-    cudaStream_t stream = nullptr;
-    cudaEvent_t ev0 = nullptr, ev1 = nullptr;
-    double lastMs = 0.0;
+    mbar::DevArray<double> d_x;      // [nTiles * 32], 0 in the padding
+    mbar::DevArray<double> d_w;      // [nTiles * 32] or NULL
+    mbar::DevArray<int32_t> d_s;     // [nTiles * 32], -1 in the padding, or NULL
+    mbar::DevArray<int32_t> d_tmin;  // [nTiles] smallest / largest label of a tile (padding excluded)
+    mbar::DevArray<int32_t> d_tmax;
+    int64_t B = 0;                   // replicate rows uploaded by mbar_b200_bspline_set_replicates
+    mbar::DevArray<double> d_V;      // [B][nTiles * 32], 0 in the padding
     int lastChunks = 0;
 };
 
@@ -338,35 +335,6 @@ static BspKernelFn bsp_kernel_for(int degree) {
     }
 }
 
-static void bsp_release(mbar_b200_bspline* b) {
-    for (void* p : {(void*)b->d_x, (void*)b->d_w, (void*)b->d_s, (void*)b->d_tmin, (void*)b->d_tmax, (void*)b->d_V})
-        if (p) cudaFree(p);
-    if (b->ev0) cudaEventDestroy(b->ev0);
-    if (b->ev1) cudaEventDestroy(b->ev1);
-    if (b->stream) cudaStreamDestroy(b->stream);
-    delete b;
-}
-
-// Device buffers of one call, released on every return path.
-struct BspBuffers {
-    std::vector<void*> ptrs;
-    ~BspBuffers() {
-        for (void* p : ptrs) cudaFree(p);
-    }
-    template <class T>
-    int alloc(T** p, size_t count) {
-        *p = nullptr;
-        const cudaError_t e = cudaMalloc((void**)p, std::max<size_t>(count, 1) * sizeof(T));
-        if (e != cudaSuccess) {
-            cudaGetLastError();
-            set_error("bspline: cannot allocate %zu bytes", count * sizeof(T));
-            return e == cudaErrorMemoryAllocation ? MBAR_B200_ERR_NOMEM : MBAR_B200_ERR_CUDA;
-        }
-        ptrs.push_back((void*)*p);
-        return MBAR_B200_OK;
-    }
-};
-
 }  // namespace mbar
 
 using namespace mbar;
@@ -384,31 +352,13 @@ int mbar_b200_bspline_create(int device, int64_t N, const double* x, const doubl
                      "[0, %d)", (long long)n, s ? (int)s[n] : 0, (int)K);
         MBAR_REQUIRE(std::isfinite(x[n]), MBAR_B200_ERR_NAN, "bspline_create: x[%lld] is %g", (long long)n, x[n]);
     }
-    int ndev = 0;
-    if (cudaGetDeviceCount(&ndev) != cudaSuccess || ndev == 0) {
-        cudaGetLastError();
-        set_error("no CUDA device visible: libmbar_b200 has no CPU fallback");
-        return MBAR_B200_ERR_NO_DEVICE;
-    }
-    MBAR_REQUIRE(device >= 0 && device < ndev, MBAR_B200_ERR_INVALID, "device %d of %d", device, ndev);
-    MBAR_CUDA(cudaSetDevice(device));
-    cudaDeviceProp prop;
-    MBAR_CUDA(cudaGetDeviceProperties(&prop, device));
-    if (prop.major != 9 || prop.minor != 0) {
-        set_error("device %d is sm_%d%d; this library is built for sm_90a (H100) only", device, prop.major, prop.minor);
-        return MBAR_B200_ERR_NO_DEVICE;
-    }
-    mbar_b200_bspline* b = new mbar_b200_bspline();
-    b->device = device;
+    MBAR_TRY(open_device(device, nullptr));
+    std::unique_ptr<mbar_b200_bspline> b(new mbar_b200_bspline());
     b->N = N;
     b->nTiles = (N + TILE_N - 1) / TILE_N;
     b->K = s ? K : 0;
     b->nGroups = (int)std::max<int64_t>(1, std::min<int64_t>(BSP_MAX_GROUPS, b->nTiles / 4));
     const int64_t nPad = b->nTiles * TILE_N;
-    auto fail = [&](int status) {
-        bsp_release(b);
-        return status;
-    };
     std::vector<double> hx((size_t)nPad, 0.0);
     std::copy(x, x + N, hx.begin());
     std::vector<double> hw;
@@ -427,48 +377,20 @@ int mbar_b200_bspline_create(int device, int64_t N, const double* x, const doubl
             tmax[n / TILE_N] = std::max(tmax[n / TILE_N], s[n]);
         }
     }
-    auto put = [&](auto** dst, const auto& src) -> int {
-        using T = typename std::remove_reference<decltype(src)>::type::value_type;
-        if (cudaMalloc((void**)dst, src.size() * sizeof(T)) != cudaSuccess) {
-            *dst = nullptr;
-            cudaGetLastError();
-            set_error("bspline_create: cannot allocate %zu bytes", src.size() * sizeof(T));
-            return MBAR_B200_ERR_NOMEM;
-        }
-        if (cudaMemcpyAsync(*dst, src.data(), src.size() * sizeof(T), cudaMemcpyHostToDevice, b->stream) !=
-            cudaSuccess) {
-            set_error("bspline_create: %s", cudaGetErrorString(cudaGetLastError()));
-            return MBAR_B200_ERR_CUDA;
-        }
-        return MBAR_B200_OK;
-    };
-    // the copies go on the object's own (non-blocking) stream and are waited for, as in mbar_b200_kde_create
-    if (cudaStreamCreateWithFlags(&b->stream, cudaStreamNonBlocking) != cudaSuccess ||
-        cudaEventCreate(&b->ev0) != cudaSuccess || cudaEventCreate(&b->ev1) != cudaSuccess) {
-        set_error("bspline_create: %s", cudaGetErrorString(cudaGetLastError()));
-        return fail(MBAR_B200_ERR_CUDA);
+    const char* who = "bspline_create";
+    MBAR_TRY(b->open(device, who));
+    MBAR_TRY(b->upload(b->d_x, hx.data(), hx.size(), who));
+    if (w) MBAR_TRY(b->upload(b->d_w, hw.data(), hw.size(), who));
+    if (s) {
+        MBAR_TRY(b->upload(b->d_s, hs.data(), hs.size(), who));
+        MBAR_TRY(b->upload(b->d_tmin, tmin.data(), tmin.size(), who));
+        MBAR_TRY(b->upload(b->d_tmax, tmax.data(), tmax.size(), who));
     }
-    int rc = put(&b->d_x, hx);
-    if (!rc && w) rc = put(&b->d_w, hw);
-    if (!rc && s) rc = put(&b->d_s, hs);
-    if (!rc && s) rc = put(&b->d_tmin, tmin);
-    if (!rc && s) rc = put(&b->d_tmax, tmax);
-    if (rc) return fail(rc);
-    if (cudaStreamSynchronize(b->stream) != cudaSuccess) {
-        set_error("bspline_create: %s", cudaGetErrorString(cudaGetLastError()));
-        return fail(MBAR_B200_ERR_CUDA);
-    }
-    *out = b;
+    *out = b.release();
     return MBAR_B200_OK;
 }
 
-int mbar_b200_bspline_destroy(mbar_b200_bspline* b) {
-    if (!b) return MBAR_B200_OK;
-    cudaSetDevice(b->device);
-    if (b->stream) cudaStreamSynchronize(b->stream);
-    bsp_release(b);
-    return MBAR_B200_OK;
-}
+int mbar_b200_bspline_destroy(mbar_b200_bspline* b) { return destroy_resident(b); }
 
 // The degree and knot checks of mbar_b200_bspline_moments and mbar_b200_bspline_replicate_sums.
 static int bsp_check_knots(const char* fn, int32_t degree, int64_t n_knots, const double* t) {
@@ -505,7 +427,7 @@ int mbar_b200_bspline_moments(mbar_b200_bspline* b, int32_t degree, int64_t n_kn
     const int Kw = S ? b->K : 0;
     const int totalRows = (A ? 1 : 0) + Kw;
     const int rowsPer = std::max(1, std::min(totalRows, (BSP_ACC_DOUBLES - nk) / nb));
-    BspBuffers buf;
+    CallBuffers buf("bspline");
     double *d_t, *d_partial, *d_S = nullptr, *d_A = nullptr;
     MBAR_TRY(buf.alloc(&d_t, (size_t)nk));
     MBAR_TRY(buf.alloc(&d_partial, (size_t)b->nGroups * rowsPer * nb));
@@ -560,25 +482,12 @@ int mbar_b200_bspline_set_replicates(mbar_b200_bspline* b, int64_t B, const doub
     // a failed upload leaves no replicates
     if (b->d_V) {
         cudaStreamSynchronize(b->stream);
-        cudaFree(b->d_V);
-        b->d_V = nullptr;
+        b->d_V.reset();
     }
     b->B = 0;
-    MBAR_REQUIRE(B >= 1 && V_host, MBAR_B200_ERR_INVALID, "bspline_set_replicates: B=%lld, V=%p", (long long)B,
-                 (const void*)V_host);
+    MBAR_TRY(check_replicate_weights("bspline_set_replicates", B, b->N, V_host));
     const int64_t N = b->N, nPad = b->nTiles * TILE_N;
-    for (int64_t i = 0; i < B * N; ++i)
-        MBAR_REQUIRE(V_host[i] >= 0.0 && V_host[i] < INFINITY, MBAR_B200_ERR_INVALID, "bspline_set_replicates: weight "
-                     "(%lld, %lld) is %g (negative, NaN or infinite)", (long long)(i / N), (long long)(i % N),
-                     V_host[i]);
-    const size_t bytes = (size_t)B * nPad * sizeof(double);
-    const cudaError_t e = cudaMalloc((void**)&b->d_V, bytes);
-    if (e != cudaSuccess) {
-        b->d_V = nullptr;
-        cudaGetLastError();
-        set_error("bspline_set_replicates: cannot allocate %zu bytes", bytes);
-        return e == cudaErrorMemoryAllocation ? MBAR_B200_ERR_NOMEM : MBAR_B200_ERR_CUDA;
-    }
+    MBAR_TRY(b->d_V.reserve((size_t)B * nPad, "bspline_set_replicates"));
     // rows of N into rows of nPad, the padding zeroed
     bool ok = cudaMemcpy2DAsync(b->d_V, nPad * sizeof(double), V_host, N * sizeof(double), N * sizeof(double),
                                 (size_t)B, cudaMemcpyHostToDevice, b->stream) == cudaSuccess;
@@ -587,8 +496,7 @@ int mbar_b200_bspline_set_replicates(mbar_b200_bspline* b, int64_t B, const doub
                                b->stream) == cudaSuccess;
     if (!ok || cudaStreamSynchronize(b->stream) != cudaSuccess) {
         set_error("bspline_set_replicates: %s", cudaGetErrorString(cudaGetLastError()));
-        cudaFree(b->d_V);
-        b->d_V = nullptr;
+        b->d_V.reset();
         return MBAR_B200_ERR_CUDA;
     }
     b->B = B;
@@ -609,7 +517,7 @@ int mbar_b200_bspline_replicate_sums(mbar_b200_bspline* b, int32_t degree, int64
     int warps = BSP_REP_MAX_WARPS;
     while (warps > 1 && (int64_t)warps * nb + nk > BSP_ACC_DOUBLES) warps >>= 1;
     const int rowsPer = (int)std::max<int64_t>(1, std::min<int64_t>(b->B, (BSP_ACC_DOUBLES - nk) / ((int64_t)warps * nb)));
-    BspBuffers buf;
+    CallBuffers buf("bspline");
     double *d_t, *d_partial, *d_out;
     MBAR_TRY(buf.alloc(&d_t, (size_t)nk));
     MBAR_TRY(buf.alloc(&d_partial, (size_t)b->nGroups * rowsPer * nb));

@@ -509,6 +509,26 @@ int launch_synth(mbar_b200_ctx* ctx, const mbar_b200_synth* spec) {
     return MBAR_B200_OK;
 }
 
+int open_device(int device, cudaDeviceProp* propOut) {
+    int ndev = 0;
+    if (cudaGetDeviceCount(&ndev) != cudaSuccess || ndev == 0) {
+        cudaGetLastError();
+        set_error("no CUDA device visible: libmbar_b200 has no CPU fallback");
+        return MBAR_B200_ERR_NO_DEVICE;
+    }
+    MBAR_REQUIRE(device >= 0 && device < ndev, MBAR_B200_ERR_INVALID, "device %d of %d", device, ndev);
+    MBAR_CUDA(cudaSetDevice(device));
+    cudaDeviceProp prop;
+    MBAR_CUDA(cudaGetDeviceProperties(&prop, device));
+    if (prop.major != 9 || prop.minor != 0) {
+        set_error("device %d is sm_%d%d; this library is built for sm_90a (H100) only", device,
+                  prop.major, prop.minor);
+        return MBAR_B200_ERR_NO_DEVICE;
+    }
+    if (propOut) *propOut = prop;
+    return MBAR_B200_OK;
+}
+
 }  // namespace mbar
 
 using namespace mbar;
@@ -595,21 +615,8 @@ int mbar_b200_create(mbar_b200_ctx** out, int device, int32_t K, int64_t N_local
     MBAR_REQUIRE(K >= 1 && K <= MBAR_B200_MAX_STATES, MBAR_B200_ERR_INVALID, "K=%d outside [1, %d]", K,
                  MBAR_B200_MAX_STATES);
     MBAR_REQUIRE(N_local >= 1, MBAR_B200_ERR_INVALID, "N_local=%lld must be >= 1", (long long)N_local);
-    int ndev = 0;
-    if (cudaGetDeviceCount(&ndev) != cudaSuccess || ndev == 0) {
-        cudaGetLastError();
-        set_error("no CUDA device visible: libmbar_b200 has no CPU fallback");
-        return MBAR_B200_ERR_NO_DEVICE;
-    }
-    MBAR_REQUIRE(device >= 0 && device < ndev, MBAR_B200_ERR_INVALID, "device %d of %d", device, ndev);
-    MBAR_CUDA(cudaSetDevice(device));
     cudaDeviceProp prop;
-    MBAR_CUDA(cudaGetDeviceProperties(&prop, device));
-    if (prop.major != 9 || prop.minor != 0) {
-        set_error("device %d is sm_%d%d; this library is built for sm_90a (H100) only", device,
-                  prop.major, prop.minor);
-        return MBAR_B200_ERR_NO_DEVICE;
-    }
+    MBAR_TRY(open_device(device, &prop));
     mbar_b200_ctx* c = new mbar_b200_ctx();
     c->device = device;
     c->K = K;

@@ -434,4 +434,135 @@ inline bool event_ms(cudaEvent_t a, cudaEvent_t b, float* ms) {
 // loops owns the word at this offset
 inline size_t scratch_rendezvous(int K) { return (size_t)K * K + 4 * (size_t)K; }
 
+// ---- host scaffold of the resident device objects (mbar_b200_kde, _bspline, _acf, _work) ----
+
+// Checks that `device` is visible and is an sm_90 part, makes it current and fills *prop unless it is NULL (ctx.cu).
+int open_device(int device, cudaDeviceProp* prop);
+
+// cudaMalloc of max(count, 1) elements.  On failure *p is NULL, the runtime's error is cleared and the status is
+// ERR_NOMEM when the device is out of memory, ERR_CUDA otherwise.
+template <class T>
+int dev_alloc(T** p, size_t count, const char* who) {
+    const cudaError_t e = cudaMalloc((void**)p, (count > 0 ? count : 1) * sizeof(T));
+    if (e == cudaSuccess) return MBAR_B200_OK;
+    *p = nullptr;
+    cudaGetLastError();
+    set_error("%s: cannot allocate %zu bytes", who, count * sizeof(T));
+    return e == cudaErrorMemoryAllocation ? MBAR_B200_ERR_NOMEM : MBAR_B200_ERR_CUDA;
+}
+
+// Device buffers of one call, freed on every return path.
+struct CallBuffers {
+    const char* who;
+    std::vector<void*> ptrs;
+    explicit CallBuffers(const char* who_) : who(who_) {}
+    CallBuffers(const CallBuffers&) = delete;
+    CallBuffers& operator=(const CallBuffers&) = delete;
+    ~CallBuffers() {
+        for (void* p : ptrs) cudaFree(p);
+    }
+    template <class T>
+    int alloc(T** p, size_t count) {
+        MBAR_TRY(dev_alloc(p, count, who));
+        ptrs.push_back((void*)*p);
+        return MBAR_B200_OK;
+    }
+};
+
+// A device array owned by a resident object and freed with it.  reserve(n) keeps the buffer when it already holds n
+// elements; otherwise it drops the contents and allocates n, and a failure leaves the array empty with capacity 0.
+template <class T>
+struct DevArray {
+    T* ptr = nullptr;
+    size_t cap = 0;
+    DevArray() = default;
+    DevArray(DevArray&& o) noexcept : ptr(o.ptr), cap(o.cap) {
+        o.ptr = nullptr;
+        o.cap = 0;
+    }
+    DevArray& operator=(DevArray&& o) noexcept {
+        std::swap(ptr, o.ptr);
+        std::swap(cap, o.cap);
+        return *this;
+    }
+    ~DevArray() { reset(); }
+    void reset() {
+        if (ptr) cudaFree(ptr);
+        ptr = nullptr;
+        cap = 0;
+    }
+    int reserve(size_t n, const char* who) {
+        if (ptr && n <= cap) return MBAR_B200_OK;
+        reset();
+        MBAR_TRY(dev_alloc(&ptr, n, who));
+        cap = n;
+        return MBAR_B200_OK;
+    }
+    operator T*() const { return ptr; }
+};
+
+// Device, stream and timing events of a resident device object.  mbar_b200_kde, _bspline, _acf and _work derive from
+// it and hold their device memory in DevArray members; each create holds its object in a std::unique_ptr until it
+// succeeds, and each destroy goes through destroy_resident.
+struct Resident {
+    int device = 0;
+    cudaStream_t stream = nullptr;            // non-blocking: work on the legacy stream does not serialise with it
+    cudaEvent_t ev0 = nullptr, ev1 = nullptr; // the timed window of the last call
+    double lastMs = 0.0;
+
+    Resident() = default;
+    Resident(const Resident&) = delete;
+    Resident& operator=(const Resident&) = delete;
+    ~Resident() {
+        if (ev0) cudaEventDestroy(ev0);
+        if (ev1) cudaEventDestroy(ev1);
+        if (stream) cudaStreamDestroy(stream);
+    }
+    // the stream and the events, on `dev` (made current by open_device)
+    int open(int dev, const char* who) {
+        device = dev;
+        if (cudaStreamCreateWithFlags(&stream, cudaStreamNonBlocking) != cudaSuccess ||
+            cudaEventCreate(&ev0) != cudaSuccess || cudaEventCreate(&ev1) != cudaSuccess) {
+            set_error("%s: %s", who, cudaGetErrorString(cudaGetLastError()));
+            return MBAR_B200_ERR_CUDA;
+        }
+        return MBAR_B200_OK;
+    }
+    // count elements of src into dst (allocated to fit).  The copy goes on the object's own stream and is waited for:
+    // a pageable cudaMemcpy on the legacy stream may return before its DMA lands, and the kernels' stream would not
+    // wait for it.
+    template <class T>
+    int upload(DevArray<T>& dst, const T* src, size_t count, const char* who) {
+        MBAR_TRY(dst.reserve(count, who));
+        if (cudaMemcpyAsync(dst, src, count * sizeof(T), cudaMemcpyHostToDevice, stream) != cudaSuccess ||
+            cudaStreamSynchronize(stream) != cudaSuccess) {
+            set_error("%s: %s", who, cudaGetErrorString(cudaGetLastError()));
+            return MBAR_B200_ERR_CUDA;
+        }
+        return MBAR_B200_OK;
+    }
+};
+
+// Deletes a resident object once its stream has drained.  C++ destroys the derived object's DevArrays before ~Resident
+// runs, so the wait has to come before the delete.
+template <class T>
+int destroy_resident(T* o) {
+    if (!o) return MBAR_B200_OK;
+    cudaSetDevice(o->device);
+    if (o->stream) cudaStreamSynchronize(o->stream);
+    delete o;
+    return MBAR_B200_OK;
+}
+
+// The replicate weights V [B, N] of mbar_b200_kde_set_replicates and mbar_b200_bspline_set_replicates: B >= 1 and
+// every V_bn finite and >= 0.
+inline int check_replicate_weights(const char* who, int64_t B, int64_t N, const double* V) {
+    MBAR_REQUIRE(B >= 1 && V, MBAR_B200_ERR_INVALID, "%s: B=%lld, V=%p", who, (long long)B, (const void*)V);
+    for (int64_t i = 0; i < B * N; ++i)
+        MBAR_REQUIRE(V[i] >= 0.0 && V[i] < INFINITY, MBAR_B200_ERR_INVALID,
+                     "%s: weight (%lld, %lld) is %g (negative, NaN or infinite)", who, (long long)(i / N),
+                     (long long)(i % N), V[i]);
+    return MBAR_B200_OK;
+}
+
 }  // namespace mbar

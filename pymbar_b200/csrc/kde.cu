@@ -23,38 +23,33 @@
 // square root reaches h (computed on the host).
 #include <algorithm>
 #include <cmath>
+#include <memory>
 #include <vector>
 
 #include "internal.cuh"
 
-struct mbar_b200_kde {
-    int device = 0;
+struct mbar_b200_kde : mbar::Resident {
     int D = 0;
     int64_t N = 0;
     int64_t nPad = 0;            // N rounded up to a tile
     int64_t chunkLen = 0;        // samples per chunk (a multiple of KDE_TILE)
     int nChunks = 0;
-    double* d_x = nullptr;       // [D][nPad] coordinates, 0 in the padding
-    double* d_lw = nullptr;      // [nPad] log w_n, -inf for zero weights and the padding
-    double* d_y = nullptr;       // [D][qCap] queries of one batch
-    double* d_pm = nullptr;      // [nChunks][qCap] running maxima
-    double* d_ps = nullptr;      // [nChunks][qCap] sums relative to them
-    double* d_out = nullptr;     // [qCap]
-    int64_t qCap = 0;
-    cudaStream_t stream = nullptr;
-    cudaEvent_t ev0 = nullptr, ev1 = nullptr;
-    double lastMs = 0.0;
+    mbar::DevArray<double> d_x;    // [D][nPad] coordinates, 0 in the padding
+    mbar::DevArray<double> d_lw;   // [nPad] log w_n, -inf for zero weights and the padding
+    mbar::DevArray<double> d_y;    // [D][qb] queries of one batch
+    mbar::DevArray<double> d_pm;   // [nChunks][qb] running maxima
+    mbar::DevArray<double> d_ps;   // [nChunks][qb] sums relative to them
+    mbar::DevArray<double> d_out;  // [qb]
     int lastChunks = 0;
     // bootstrap replicates (mbar_b200_kde_set_replicates), in batches of KDE_REP_W
     int64_t B = 0;
-    double* d_lvm = nullptr;     // [nRepBatches][nPad] log vmax_n = log max_b V_bn over the batch, -inf when 0
-    double* d_rat = nullptr;     // [nRepBatches * KDE_REP_W][nPad] V_bn / vmax_n (0 where vmax_n = 0, and padding rows)
-    double* d_rpm = nullptr;     // [nChunks][KDE_REP_W][rqCap] partials of one (replicate batch, query batch)
-    double* d_rps = nullptr;
-    double* d_rout = nullptr;    // [KDE_REP_W][rqCap]
-    double* d_rflag = nullptr;   // [KDE_REP_W][rqCap] 1 where the batch's shared scale may have lost digits
-    double* d_rlw = nullptr;     // [nPad] log V_bn of one replicate, for the exact pass over flagged queries
-    int64_t rqCap = 0;
+    mbar::DevArray<double> d_lvm;  // [nRepBatches][nPad] log vmax_n = log max_b V_bn over the batch, -inf when 0
+    mbar::DevArray<double> d_rat;  // [nRepBatches * KDE_REP_W][nPad] V_bn / vmax_n (0 where vmax_n = 0, padding rows)
+    mbar::DevArray<double> d_rpm;  // [nChunks][KDE_REP_W][qb] partials of one (replicate batch, query batch)
+    mbar::DevArray<double> d_rps;
+    mbar::DevArray<double> d_rout;   // [KDE_REP_W][qb]
+    mbar::DevArray<double> d_rflag;  // [KDE_REP_W][qb] 1 where the batch's shared scale may have lost digits
+    mbar::DevArray<double> d_rlw;    // [nPad] log V_bn of one replicate, for the exact pass over flagged queries
 };
 
 namespace mbar {
@@ -346,64 +341,26 @@ static double sqrt_threshold(double h) {
     return r;
 }
 
-static void kde_release(mbar_b200_kde* k) {
-    for (double* p : {k->d_x, k->d_lw, k->d_y, k->d_pm, k->d_ps, k->d_out, k->d_lvm, k->d_rat, k->d_rpm, k->d_rps,
-                      k->d_rout, k->d_rflag, k->d_rlw})
-        if (p) cudaFree(p);
-    if (k->ev0) cudaEventDestroy(k->ev0);
-    if (k->ev1) cudaEventDestroy(k->ev1);
-    if (k->stream) cudaStreamDestroy(k->stream);
-    delete k;
-}
-
-static int kde_alloc(double** p, size_t count) {
-    const cudaError_t e = cudaMalloc((void**)p, std::max<size_t>(count, 1) * sizeof(double));
-    if (e != cudaSuccess) {
-        *p = nullptr;
-        cudaGetLastError();
-        set_error("kde: cannot allocate %zu bytes", count * sizeof(double));
-        return e == cudaErrorMemoryAllocation ? MBAR_B200_ERR_NOMEM : MBAR_B200_ERR_CUDA;
-    }
-    return MBAR_B200_OK;
-}
-
 // per-batch buffers for up to qb queries; on failure the object keeps no (or its previous) buffers and stays usable
 static int kde_reserve(mbar_b200_kde* k, int64_t qb) {
-    if (qb <= k->qCap) return MBAR_B200_OK;
-    for (double** p : {&k->d_y, &k->d_pm, &k->d_ps, &k->d_out}) {
-        if (*p) cudaFree(*p);
-        *p = nullptr;
-    }
-    k->qCap = 0;
-    MBAR_TRY(kde_alloc(&k->d_y, (size_t)k->D * qb));
-    MBAR_TRY(kde_alloc(&k->d_pm, (size_t)k->nChunks * qb));
-    MBAR_TRY(kde_alloc(&k->d_ps, (size_t)k->nChunks * qb));
-    MBAR_TRY(kde_alloc(&k->d_out, (size_t)qb));
-    k->qCap = qb;
-    return MBAR_B200_OK;
+    MBAR_TRY(k->d_y.reserve((size_t)k->D * qb, "kde"));
+    MBAR_TRY(k->d_pm.reserve((size_t)k->nChunks * qb, "kde"));
+    MBAR_TRY(k->d_ps.reserve((size_t)k->nChunks * qb, "kde"));
+    return k->d_out.reserve((size_t)qb, "kde");
 }
 
 // the replicate pass's partials and results for up to qb queries, as kde_reserve
 static int kde_rep_reserve(mbar_b200_kde* k, int64_t qb) {
-    if (qb <= k->rqCap) return MBAR_B200_OK;
-    for (double** p : {&k->d_rpm, &k->d_rps, &k->d_rout, &k->d_rflag}) {
-        if (*p) cudaFree(*p);
-        *p = nullptr;
-    }
-    k->rqCap = 0;
-    MBAR_TRY(kde_alloc(&k->d_rpm, (size_t)k->nChunks * KDE_REP_W * qb));
-    MBAR_TRY(kde_alloc(&k->d_rps, (size_t)k->nChunks * KDE_REP_W * qb));
-    MBAR_TRY(kde_alloc(&k->d_rout, (size_t)KDE_REP_W * qb));
-    MBAR_TRY(kde_alloc(&k->d_rflag, (size_t)KDE_REP_W * qb));
-    k->rqCap = qb;
-    return MBAR_B200_OK;
+    MBAR_TRY(k->d_rpm.reserve((size_t)k->nChunks * KDE_REP_W * qb, "kde"));
+    MBAR_TRY(k->d_rps.reserve((size_t)k->nChunks * KDE_REP_W * qb, "kde"));
+    MBAR_TRY(k->d_rout.reserve((size_t)KDE_REP_W * qb, "kde"));
+    return k->d_rflag.reserve((size_t)KDE_REP_W * qb, "kde");
 }
 
 static void kde_drop_replicates(mbar_b200_kde* k) {
-    for (double** p : {&k->d_lvm, &k->d_rat, &k->d_rlw}) {
-        if (*p) cudaFree(*p);
-        *p = nullptr;
-    }
+    k->d_lvm.reset();
+    k->d_rat.reset();
+    k->d_rlw.reset();
     k->B = 0;
 }
 
@@ -417,20 +374,7 @@ int mbar_b200_kde_create(int device, int64_t N, int32_t D, const double* x_host,
     *out = nullptr;
     MBAR_REQUIRE(N >= 1, MBAR_B200_ERR_INVALID, "kde_create: N=%lld must be >= 1", (long long)N);
     MBAR_REQUIRE(D >= 1 && D <= 4, MBAR_B200_ERR_INVALID, "kde_create: D=%d outside [1, 4]", (int)D);
-    int ndev = 0;
-    if (cudaGetDeviceCount(&ndev) != cudaSuccess || ndev == 0) {
-        cudaGetLastError();
-        set_error("no CUDA device visible: libmbar_b200 has no CPU fallback");
-        return MBAR_B200_ERR_NO_DEVICE;
-    }
-    MBAR_REQUIRE(device >= 0 && device < ndev, MBAR_B200_ERR_INVALID, "device %d of %d", device, ndev);
-    MBAR_CUDA(cudaSetDevice(device));
-    cudaDeviceProp prop;
-    MBAR_CUDA(cudaGetDeviceProperties(&prop, device));
-    if (prop.major != 9 || prop.minor != 0) {
-        set_error("device %d is sm_%d%d; this library is built for sm_90a (H100) only", device, prop.major, prop.minor);
-        return MBAR_B200_ERR_NO_DEVICE;
-    }
+    MBAR_TRY(open_device(device, nullptr));
     const int64_t nPad = (N + KDE_TILE - 1) / KDE_TILE * KDE_TILE;
     std::vector<double> hx((size_t)D * nPad, 0.0), hlw((size_t)nPad, -INFINITY);
     bool any = false;
@@ -448,8 +392,7 @@ int mbar_b200_kde_create(int device, int64_t N, int32_t D, const double* x_host,
         }
     }
     MBAR_REQUIRE(any, MBAR_B200_ERR_INVALID, "kde_create: the weights sum to 0");
-    mbar_b200_kde* k = new mbar_b200_kde();
-    k->device = device;
+    std::unique_ptr<mbar_b200_kde> k(new mbar_b200_kde());
     k->D = D;
     k->N = N;
     k->nPad = nPad;
@@ -457,35 +400,14 @@ int mbar_b200_kde_create(int device, int64_t N, int32_t D, const double* x_host,
     int64_t nc = std::min<int64_t>(KDE_MAX_CHUNKS, std::max<int64_t>(1, (N + KDE_MIN_CHUNK - 1) / KDE_MIN_CHUNK));
     k->chunkLen = ((N + nc - 1) / nc + KDE_TILE - 1) / KDE_TILE * KDE_TILE;
     k->nChunks = (int)((nPad + k->chunkLen - 1) / k->chunkLen);
-    int rc = MBAR_B200_OK;
-    auto fail = [&](int status) {
-        kde_release(k);
-        return status;
-    };
-    if ((rc = kde_alloc(&k->d_x, hx.size())) || (rc = kde_alloc(&k->d_lw, hlw.size()))) return fail(rc);
-    // the copies go on the object's own (non-blocking) stream and are waited for: a pageable cudaMemcpy on the legacy
-    // stream may return before its DMA lands, and the kernels' stream would not wait for it
-    if (cudaStreamCreateWithFlags(&k->stream, cudaStreamNonBlocking) != cudaSuccess ||
-        cudaEventCreate(&k->ev0) != cudaSuccess || cudaEventCreate(&k->ev1) != cudaSuccess ||
-        cudaMemcpyAsync(k->d_x, hx.data(), hx.size() * sizeof(double), cudaMemcpyHostToDevice, k->stream) !=
-            cudaSuccess ||
-        cudaMemcpyAsync(k->d_lw, hlw.data(), hlw.size() * sizeof(double), cudaMemcpyHostToDevice, k->stream) !=
-            cudaSuccess ||
-        cudaStreamSynchronize(k->stream) != cudaSuccess) {
-        set_error("kde_create: %s", cudaGetErrorString(cudaGetLastError()));
-        return fail(MBAR_B200_ERR_CUDA);
-    }
-    *out = k;
+    MBAR_TRY(k->open(device, "kde_create"));
+    MBAR_TRY(k->upload(k->d_x, hx.data(), hx.size(), "kde_create"));
+    MBAR_TRY(k->upload(k->d_lw, hlw.data(), hlw.size(), "kde_create"));
+    *out = k.release();
     return MBAR_B200_OK;
 }
 
-int mbar_b200_kde_destroy(mbar_b200_kde* k) {
-    if (!k) return MBAR_B200_OK;
-    cudaSetDevice(k->device);
-    if (k->stream) cudaStreamSynchronize(k->stream);
-    kde_release(k);
-    return MBAR_B200_OK;
-}
+int mbar_b200_kde_destroy(mbar_b200_kde* k) { return destroy_resident(k); }
 
 int mbar_b200_kde_log_sum(mbar_b200_kde* k, int32_t kernel, double h, int64_t Q, const double* y_host,
                           double* out) {
@@ -551,18 +473,15 @@ int mbar_b200_kde_set_replicates(mbar_b200_kde* k, int64_t B, const double* V_ho
     MBAR_REQUIRE(k, MBAR_B200_ERR_INVALID, "kde_set_replicates: NULL object");
     MBAR_CUDA(cudaSetDevice(k->device));
     kde_drop_replicates(k);
-    MBAR_REQUIRE(B >= 1 && V_host, MBAR_B200_ERR_INVALID, "kde_set_replicates: B=%lld, V=%p", (long long)B,
-                 (const void*)V_host);
+    MBAR_TRY(check_replicate_weights("kde_set_replicates", B, k->N, V_host));
     const int64_t N = k->N, nPad = k->nPad;
-    for (int64_t i = 0; i < B * N; ++i)
-        MBAR_REQUIRE(V_host[i] >= 0.0 && V_host[i] < INFINITY, MBAR_B200_ERR_INVALID, "kde_set_replicates: weight "
-                     "(%lld, %lld) is %g (negative, NaN or infinite)", (long long)(i / N), (long long)(i % N), V_host[i]);
     // device: log vmax_n per batch of KDE_REP_W replicates, the ratios V_bn / vmax_n (rows past B stay 0), and one
     // replicate's log weights for the exact pass: 8 nPad (9 nRB + 1) bytes
     const int64_t nRB = (B + KDE_REP_W - 1) / KDE_REP_W;
     int rc = MBAR_B200_OK;
-    if ((rc = kde_alloc(&k->d_lvm, (size_t)(nRB * nPad))) ||
-        (rc = kde_alloc(&k->d_rat, (size_t)(nRB * KDE_REP_W * nPad))) || (rc = kde_alloc(&k->d_rlw, (size_t)nPad))) {
+    if ((rc = k->d_lvm.reserve((size_t)(nRB * nPad), "kde")) ||
+        (rc = k->d_rat.reserve((size_t)(nRB * KDE_REP_W * nPad), "kde")) ||
+        (rc = k->d_rlw.reserve((size_t)nPad, "kde"))) {
         kde_drop_replicates(k);
         return rc;
     }

@@ -24,6 +24,7 @@
 // there are no atomics, and repeat calls are bit-identical.
 #include <algorithm>
 #include <cmath>
+#include <memory>
 #include <vector>
 
 #include "internal.cuh"
@@ -47,25 +48,17 @@ struct WorkReq {
 
 }  // namespace mbar
 
-struct mbar_b200_work {
-    int device = 0;
+struct mbar_b200_work : mbar::Resident {
     int64_t nTotal = 0;
     int nVec = 0;
     std::vector<int64_t> offsets;
     std::vector<double> vmin, vmax;
-    double* d_w = nullptr;
+    mbar::DevArray<double> d_w;
     // per-call buffers, grown on demand
-    mbar::WorkReq* d_req = nullptr;
-    int64_t reqCap = 0;
-    double* d_part = nullptr;      // [items][2]
-    int64_t partCap = 0;
-    double* d_shift = nullptr;     // [requests][2]: pass-1 results (shifts, or sum and mean)
-    int64_t shiftCap = 0;
-    double* d_out = nullptr;       // [requests][3]
-    int64_t outCap = 0;
-    cudaStream_t stream = nullptr;
-    cudaEvent_t ev0 = nullptr, ev1 = nullptr;
-    double lastMs = 0.0;
+    mbar::DevArray<mbar::WorkReq> d_req;
+    mbar::DevArray<double> d_part;   // [items][2]
+    mbar::DevArray<double> d_shift;  // [requests][2]: pass-1 results (shifts, or sum and mean)
+    mbar::DevArray<double> d_out;    // [requests][3]
     int32_t lastLaunches = 0;
     int64_t lastValues = 0;
 };
@@ -242,32 +235,11 @@ __global__ void work_finalize2_kernel(const WorkReq* __restrict__ req, int nReq,
     }
 }
 
-static void work_release(mbar_b200_work* o) {
-    for (void* p : {(void*)o->d_w, (void*)o->d_req, (void*)o->d_part, (void*)o->d_shift, (void*)o->d_out})
-        if (p) cudaFree(p);
-    if (o->ev0) cudaEventDestroy(o->ev0);
-    if (o->ev1) cudaEventDestroy(o->ev1);
-    if (o->stream) cudaStreamDestroy(o->stream);
-    delete o;
-}
-
-// grow *p to hold `count` elements (old contents are dropped); on failure the buffer is empty and cap 0
+// grow a per-call buffer to hold `count` elements, with room to spare for a somewhat larger call
 template <class T>
-static int work_grow(T** p, int64_t* cap, int64_t count) {
-    if (count <= *cap) return MBAR_B200_OK;
-    if (*p) cudaFree(*p);
-    *p = nullptr;
-    *cap = 0;
-    const int64_t want = count + count / 2 + 64;
-    const cudaError_t e = cudaMalloc((void**)p, (size_t)want * sizeof(T));
-    if (e != cudaSuccess) {
-        *p = nullptr;
-        cudaGetLastError();
-        set_error("work: cannot allocate %zu bytes", (size_t)want * sizeof(T));
-        return e == cudaErrorMemoryAllocation ? MBAR_B200_ERR_NOMEM : MBAR_B200_ERR_CUDA;
-    }
-    *cap = want;
-    return MBAR_B200_OK;
+static int work_grow(DevArray<T>& a, int64_t count) {
+    if ((size_t)count <= a.cap) return MBAR_B200_OK;
+    return a.reserve((size_t)(count + count / 2 + 64), "work");
 }
 
 }  // namespace mbar
@@ -297,59 +269,20 @@ int mbar_b200_work_create(int device, int64_t n_total, const double* w, int32_t 
         vmin[v] = lo;
         vmax[v] = hi;
     }
-    int ndev = 0;
-    if (cudaGetDeviceCount(&ndev) != cudaSuccess || ndev == 0) {
-        cudaGetLastError();
-        set_error("no CUDA device visible: libmbar_b200 has no CPU fallback");
-        return MBAR_B200_ERR_NO_DEVICE;
-    }
-    MBAR_REQUIRE(device >= 0 && device < ndev, MBAR_B200_ERR_INVALID, "device %d of %d", device, ndev);
-    MBAR_CUDA(cudaSetDevice(device));
-    cudaDeviceProp prop;
-    MBAR_CUDA(cudaGetDeviceProperties(&prop, device));
-    if (prop.major != 9 || prop.minor != 0) {
-        set_error("device %d is sm_%d%d; this library is built for sm_90a (H100) only", device, prop.major, prop.minor);
-        return MBAR_B200_ERR_NO_DEVICE;
-    }
-    mbar_b200_work* o = new mbar_b200_work();
-    o->device = device;
+    MBAR_TRY(open_device(device, nullptr));
+    std::unique_ptr<mbar_b200_work> o(new mbar_b200_work());
     o->nTotal = n_total;
     o->nVec = n_vectors;
     o->offsets.assign(offsets, offsets + n_vectors + 1);
     o->vmin.swap(vmin);
     o->vmax.swap(vmax);
-    auto fail = [&](int status) {
-        work_release(o);
-        return status;
-    };
-    if (cudaStreamCreateWithFlags(&o->stream, cudaStreamNonBlocking) != cudaSuccess ||
-        cudaEventCreate(&o->ev0) != cudaSuccess || cudaEventCreate(&o->ev1) != cudaSuccess) {
-        set_error("work_create: %s", cudaGetErrorString(cudaGetLastError()));
-        return fail(MBAR_B200_ERR_CUDA);
-    }
-    if (cudaMalloc((void**)&o->d_w, (size_t)n_total * sizeof(double)) != cudaSuccess) {
-        o->d_w = nullptr;
-        cudaGetLastError();
-        set_error("work_create: cannot allocate %zu bytes", (size_t)n_total * sizeof(double));
-        return fail(MBAR_B200_ERR_NOMEM);
-    }
-    if (cudaMemcpyAsync(o->d_w, w, (size_t)n_total * sizeof(double), cudaMemcpyHostToDevice, o->stream) !=
-            cudaSuccess ||
-        cudaStreamSynchronize(o->stream) != cudaSuccess) {
-        set_error("work_create: %s", cudaGetErrorString(cudaGetLastError()));
-        return fail(MBAR_B200_ERR_CUDA);
-    }
-    *out = o;
+    MBAR_TRY(o->open(device, "work_create"));
+    MBAR_TRY(o->upload(o->d_w, w, (size_t)n_total, "work_create"));
+    *out = o.release();
     return MBAR_B200_OK;
 }
 
-int mbar_b200_work_destroy(mbar_b200_work* o) {
-    if (!o) return MBAR_B200_OK;
-    cudaSetDevice(o->device);
-    if (o->stream) cudaStreamSynchronize(o->stream);
-    work_release(o);
-    return MBAR_B200_OK;
-}
+int mbar_b200_work_destroy(mbar_b200_work* o) { return destroy_resident(o); }
 
 int mbar_b200_work_evaluate(mbar_b200_work* o, int32_t n_requests, const int32_t* vector, const int32_t* kind,
                             const double* c1, const double* c2, double* out) {
@@ -380,10 +313,10 @@ int mbar_b200_work_evaluate(mbar_b200_work* o, int32_t n_requests, const int32_t
     MBAR_REQUIRE(items < INT32_MAX, MBAR_B200_ERR_INVALID, "work_evaluate: %lld chunks in one call", (long long)items);
     MBAR_CUDA(cudaSetDevice(o->device));
     NvtxRange nvtx_("mbar_b200::work_evaluate");
-    MBAR_TRY(work_grow(&o->d_req, &o->reqCap, (int64_t)n_requests));
-    MBAR_TRY(work_grow(&o->d_part, &o->partCap, 2 * items));
-    MBAR_TRY(work_grow(&o->d_shift, &o->shiftCap, 2 * (int64_t)n_requests));
-    MBAR_TRY(work_grow(&o->d_out, &o->outCap, 3 * (int64_t)n_requests));
+    MBAR_TRY(work_grow(o->d_req, (int64_t)n_requests));
+    MBAR_TRY(work_grow(o->d_part, 2 * items));
+    MBAR_TRY(work_grow(o->d_shift, 2 * (int64_t)n_requests));
+    MBAR_TRY(work_grow(o->d_out, 3 * (int64_t)n_requests));
     MBAR_CUDA(cudaMemcpyAsync(o->d_req, req.data(), req.size() * sizeof(WorkReq), cudaMemcpyHostToDevice, o->stream));
     const unsigned rb = (unsigned)((n_requests + 127) / 128);
     MBAR_CUDA(cudaEventRecord(o->ev0, o->stream));

@@ -17,11 +17,60 @@ def _dptr(a):
     return a.ctypes.data_as(C.POINTER(C.c_double))
 
 
+def _i32p(a):
+    return a.ctypes.data_as(C.POINTER(C.c_int32))
+
+
+def _i64p(a):
+    return a.ctypes.data_as(C.POINTER(C.c_int64))
+
+
 def _f64(a, K=None):
     a = np.ascontiguousarray(a, dtype=np.float64)
     if K is not None and a.shape != (K,):
         raise ValueError(f"expected shape ({K},), got {a.shape}")
     return a
+
+
+def _set_replicates(obj, upload, V):
+    """Upload the replicate weights V [B, obj.N] with `upload` (a *_set_replicates entry point) and set obj.B."""
+    V = np.ascontiguousarray(V, dtype=np.float64)
+    if V.ndim != 2 or V.shape[1] != obj.N:
+        raise ValueError(f"replicate weights must be [B, {obj.N}], got shape {V.shape}")
+    obj.B = 0                              # a failed upload leaves none
+    check(upload(obj._h, V.shape[0], _dptr(V)))
+    obj.B = V.shape[0]
+
+
+def _knots(t, k):
+    """(t as contiguous float64, nb): the knot vector and its number of basis functions of degree k."""
+    t = np.ascontiguousarray(t, dtype=np.float64)
+    if t.ndim != 1:
+        raise ValueError(f"knots must be one-dimensional, got shape {t.shape}")
+    return t, max(t.shape[0] - int(k) - 1, 0)
+
+
+class _Resident:
+    """Owner of one library object: the handle `_h` and `_destroy`, the name of the entry point that frees it."""
+
+    _destroy = None
+
+    def close(self):
+        if self._h is not None and self._h.value:
+            getattr(self._lib, self._destroy)(self._h)
+            self._h = None
+
+    def __del__(self):
+        try:
+            self.close()
+        except Exception:
+            pass
+
+    def __enter__(self):
+        return self
+
+    def __exit__(self, *exc):
+        self.close()
 
 
 class PinnedArray:
@@ -48,7 +97,7 @@ class PinnedArray:
             pass
 
 
-class DeviceProblem:
+class DeviceProblem(_Resident):
     """u_kn [K, N_local] + global N_k [K] on one H100.
 
     Parameters
@@ -59,6 +108,8 @@ class DeviceProblem:
     device : CUDA device ordinal.
     N_local : required when u_kn is None.
     """
+
+    _destroy = "mbar_b200_destroy"
 
     def __init__(self, u_kn, N_k, device=0, N_local=None):
         self._lib = _lib.load()
@@ -79,24 +130,6 @@ class DeviceProblem:
         check(self._lib.mbar_b200_create(C.byref(self._h), self.device, self.K, self.N, _dptr(N_k)))
         if u_kn is not None:
             self.upload(u_kn)
-
-    # ---- lifetime -------------------------------------------------------------------------
-    def close(self):
-        if self._h is not None and self._h.value:
-            self._lib.mbar_b200_destroy(self._h)
-            self._h = None
-
-    def __del__(self):
-        try:
-            self.close()
-        except Exception:
-            pass
-
-    def __enter__(self):
-        return self
-
-    def __exit__(self, *exc):
-        self.close()
 
     # ---- data -------------------------------------------------------------------------------
     def upload(self, u_kn):
@@ -310,9 +343,8 @@ class DeviceProblem:
         f_bin = np.empty(nbins)
         C_ = np.empty((self.K, nbins)) if want_C else None
         D = np.empty(nbins) if want_C else None
-        check(self._lib.mbar_b200_bin_moments(self._h, _dptr(f), _dptr(u), b.ctypes.data_as(C.POINTER(C.c_int32)),
-                                              nbins, _dptr(f_bin), _dptr(C_) if want_C else None,
-                                              _dptr(D) if want_C else None))
+        check(self._lib.mbar_b200_bin_moments(self._h, _dptr(f), _dptr(u), _i32p(b), nbins, _dptr(f_bin),
+                                              _dptr(C_) if want_C else None, _dptr(D) if want_C else None))
         return f_bin, C_, D
 
     def last_bin_stats(self):
@@ -372,11 +404,13 @@ class DeviceProblem:
 KDE_KERNELS = ("gaussian", "tophat", "epanechnikov", "exponential", "linear", "cosine")   # mbar_b200_kde_kernel
 
 
-class DeviceKde:
+class DeviceKde(_Resident):
     """Weighted samples x_n [N, D] (D = 1..4) resident on one H100 for kernel-density sums (mbar_b200_kde_*).
 
     `log_sum(kernel, h, y)` returns l_q = log sum_n w_n k(|y_q - x_n| / h) for the query points y [Q, D], with
     sklearn's unnormalised kernels; pymbar_b200.fes adds the normalisation.  Independent of any DeviceProblem."""
+
+    _destroy = "mbar_b200_kde_destroy"
 
     def __init__(self, x_n, w_n, device=0):
         self._lib = _lib.load()
@@ -392,23 +426,6 @@ class DeviceKde:
         self.B = 0                         # replicates uploaded by set_replicates
         self.device = int(device)
         check(self._lib.mbar_b200_kde_create(self.device, self.N, self.D, _dptr(x), _dptr(w), C.byref(self._h)))
-
-    def close(self):
-        if self._h is not None and self._h.value:
-            self._lib.mbar_b200_kde_destroy(self._h)
-            self._h = None
-
-    def __del__(self):
-        try:
-            self.close()
-        except Exception:
-            pass
-
-    def __enter__(self):
-        return self
-
-    def __exit__(self, *exc):
-        self.close()
 
     def _kernel_and_queries(self, kernel, y):
         code = KDE_KERNELS.index(kernel) if isinstance(kernel, str) and kernel in KDE_KERNELS else kernel
@@ -431,12 +448,7 @@ class DeviceKde:
     def set_replicates(self, V):
         """Upload the weights V [B, N] of B bootstrap replicates of the resident samples (V_bn >= 0); they replace any
         uploaded before and stay on the device for log_sum_replicates."""
-        V = np.ascontiguousarray(V, dtype=np.float64)
-        if V.ndim != 2 or V.shape[1] != self.N:
-            raise ValueError(f"replicate weights must be [B, {self.N}], got shape {V.shape}")
-        self.B = 0                         # a failed upload leaves none
-        check(self._lib.mbar_b200_kde_set_replicates(self._h, V.shape[0], _dptr(V)))
-        self.B = V.shape[0]
+        _set_replicates(self, self._lib.mbar_b200_kde_set_replicates, V)
 
     def log_sum_replicates(self, kernel, h, y):
         """[B, Q]: log_sum with the weights of each uploaded replicate, all replicates in one device call."""
@@ -453,13 +465,15 @@ class DeviceKde:
         return dict(ms=ms.value, chunks=chunks.value)
 
 
-class DeviceBSpline:
+class DeviceBSpline(_Resident):
     """Samples x_n [N] with optional weights w_n and state labels state_n in [0, K) resident on one H100 for B-spline
     basis sums (mbar_b200_bspline_*).
 
     `moments(t, k)` returns (S [K, nb], A [nb]) with S_ki = sum_{n: state_n = k} B_i(x_n) and A_i = sum_n w_n B_i(x_n),
     B_i the basis functions of scipy's BSpline(t, e_i, k).  One upload serves any number of knot vectors.  Independent
     of any DeviceProblem."""
+
+    _destroy = "mbar_b200_bspline_destroy"
 
     def __init__(self, x_n, w_n=None, state_n=None, K=None, device=0):
         self._lib = _lib.load()
@@ -483,31 +497,11 @@ class DeviceBSpline:
         self.device = int(device)
         check(self._lib.mbar_b200_bspline_create(
             self.device, self.N, _dptr(x), None if w is None else _dptr(w),
-            None if s is None else s.ctypes.data_as(C.POINTER(C.c_int32)), self.K, C.byref(self._h)))
-
-    def close(self):
-        if self._h is not None and self._h.value:
-            self._lib.mbar_b200_bspline_destroy(self._h)
-            self._h = None
-
-    def __del__(self):
-        try:
-            self.close()
-        except Exception:
-            pass
-
-    def __enter__(self):
-        return self
-
-    def __exit__(self, *exc):
-        self.close()
+            None if s is None else _i32p(s), self.K, C.byref(self._h)))
 
     def moments(self, t, k, want_S=True, want_A=True):
         """(S [K, nb] or None, A [nb] or None) for the knots t and degree k."""
-        t = np.ascontiguousarray(t, dtype=np.float64)
-        if t.ndim != 1:
-            raise ValueError(f"knots must be one-dimensional, got shape {t.shape}")
-        nb = max(t.shape[0] - int(k) - 1, 0)
+        t, nb = _knots(t, k)
         S = np.empty((self.K, nb)) if want_S else None
         A = np.empty(nb) if want_A else None
         check(self._lib.mbar_b200_bspline_moments(self._h, int(k), t.shape[0], _dptr(t),
@@ -518,20 +512,13 @@ class DeviceBSpline:
         """Upload the weights V [B, N] of B bootstrap replicates of the resident samples (V_bn >= 0); they replace any
         uploaded before and stay on the device for replicate_sums.  The weights and labels of the constructor are
         kept."""
-        V = np.ascontiguousarray(V, dtype=np.float64)
-        if V.ndim != 2 or V.shape[1] != self.N:
-            raise ValueError(f"replicate weights must be [B, {self.N}], got shape {V.shape}")
-        self.B = 0                         # a failed upload leaves none
-        check(self._lib.mbar_b200_bspline_set_replicates(self._h, V.shape[0], _dptr(V)))
-        self.B = V.shape[0]
+        _set_replicates(self, self._lib.mbar_b200_bspline_set_replicates, V)
 
     def replicate_sums(self, t, k):
         """[B, nb]: row b is sum_n V_bn B_i(x_n), the A of moments with replicate b's weights, for every uploaded
         replicate in one device call."""
-        t = np.ascontiguousarray(t, dtype=np.float64)
-        if t.ndim != 1:
-            raise ValueError(f"knots must be one-dimensional, got shape {t.shape}")
-        out = np.empty((self.B, max(t.shape[0] - int(k) - 1, 0)))
+        t, nb = _knots(t, k)
+        out = np.empty((self.B, nb))
         check(self._lib.mbar_b200_bspline_replicate_sums(self._h, int(k), t.shape[0], _dptr(t), _dptr(out)))
         return out
 
@@ -543,13 +530,15 @@ class DeviceBSpline:
         return dict(ms=ms.value, chunks=chunks.value)
 
 
-class DeviceAcf:
+class DeviceAcf(_Resident):
     """A series A [T] (and B [T] for a cross-correlation; optionally K concatenated series given by their lengths)
     resident on one H100 for the centred lag sums of pymbar.timeseries (mbar_b200_acf_*).  Independent of any
     DeviceProblem.
 
     `inefficiency(starts, fast, mintime)` runs the reference's statistical-inefficiency loop for every start at once;
     `correlation(start, n_max)` returns C(t), t = 0 .. n_max."""
+
+    _destroy = "mbar_b200_acf_destroy"
 
     def __init__(self, A_n, B_n=None, lengths=None, device=0):
         self._lib = _lib.load()
@@ -568,24 +557,7 @@ class DeviceAcf:
         self.device = int(device)
         check(self._lib.mbar_b200_acf_create(
             self.device, self.T, _dptr(a), None if b is None else _dptr(b), 0 if offsets is None else len(offsets) - 1,
-            None if offsets is None else offsets.ctypes.data_as(C.POINTER(C.c_int64)), C.byref(self._h)))
-
-    def close(self):
-        if self._h is not None and self._h.value:
-            self._lib.mbar_b200_acf_destroy(self._h)
-            self._h = None
-
-    def __del__(self):
-        try:
-            self.close()
-        except Exception:
-            pass
-
-    def __enter__(self):
-        return self
-
-    def __exit__(self, *exc):
-        self.close()
+            None if offsets is None else _i64p(offsets), C.byref(self._h)))
 
     def inefficiency(self, starts, fast=False, mintime=3, multiple=False, navg=0.0, trace_cap=0):
         """dict of per-start arrays: mean_a, mean_b, sigma2, g (before the g >= 1 clamp), last_lag, status
@@ -599,10 +571,9 @@ class DeviceAcf:
         out["status"] = np.empty(n, np.int32)
         trace = np.empty((n, int(trace_cap))) if trace_cap > 0 else None
         check(self._lib.mbar_b200_acf_inefficiency(
-            self._h, n, s.ctypes.data_as(C.POINTER(C.c_int64)), int(bool(fast)), int(mintime), 1 if multiple else 0,
-            float(navg), int(trace_cap), _dptr(out["mean_a"]), _dptr(out["mean_b"]), _dptr(out["sigma2"]),
-            _dptr(out["g"]), out["last_lag"].ctypes.data_as(C.POINTER(C.c_int64)),
-            out["status"].ctypes.data_as(C.POINTER(C.c_int32)), None if trace is None else _dptr(trace)))
+            self._h, n, _i64p(s), int(bool(fast)), int(mintime), 1 if multiple else 0, float(navg), int(trace_cap),
+            _dptr(out["mean_a"]), _dptr(out["mean_b"]), _dptr(out["sigma2"]), _dptr(out["g"]), _i64p(out["last_lag"]),
+            _i32p(out["status"]), None if trace is None else _dptr(trace)))
         if trace is not None:
             out["trace"] = trace
         return out
@@ -628,7 +599,7 @@ class DeviceAcf:
 WORK_KINDS = ("fermi", "fermi_moments", "exp", "gauss")      # MBAR_B200_WORK_* in this order
 
 
-class DeviceWork:
+class DeviceWork(_Resident):
     """V work vectors resident on one H100 for the sums of pymbar.other_estimators (mbar_b200_work_*).  Independent of
     any DeviceProblem.
 
@@ -636,6 +607,8 @@ class DeviceWork:
     logsumexp of bar_zero's term at a = (w + c1) + c2, for "fermi_moments" logsumexp(t), logsumexp(2 t) and
     A = max(w + c1) of bar's uncertainty sums, for "exp" log(sum x) + max(-w), sum x and sum (x - mean x)^2 with
     x = exp(-w - max(-w)), for "gauss" sum w and sum (w - mean w)^2 (include/mbar_b200.h)."""
+
+    _destroy = "mbar_b200_work_destroy"
 
     def __init__(self, vectors, device=0):
         self._lib = _lib.load()
@@ -647,25 +620,8 @@ class DeviceWork:
         offsets = np.ascontiguousarray(np.concatenate([[0], np.cumsum(self.lengths)]), dtype=np.int64)
         w = np.ascontiguousarray(np.concatenate(vs) if vs else np.zeros(0), dtype=np.float64)
         self.device = int(device)
-        check(self._lib.mbar_b200_work_create(self.device, w.shape[0], _dptr(w), len(vs),
-                                              offsets.ctypes.data_as(C.POINTER(C.c_int64)), C.byref(self._h)))
-
-    def close(self):
-        if self._h is not None and self._h.value:
-            self._lib.mbar_b200_work_destroy(self._h)
-            self._h = None
-
-    def __del__(self):
-        try:
-            self.close()
-        except Exception:
-            pass
-
-    def __enter__(self):
-        return self
-
-    def __exit__(self, *exc):
-        self.close()
+        check(self._lib.mbar_b200_work_create(self.device, w.shape[0], _dptr(w), len(vs), _i64p(offsets),
+                                              C.byref(self._h)))
 
     def evaluate(self, vector, kind, c1, c2):
         """out [R, 3] for the requests (vector[r], kind[r], c1[r], c2[r]); a kind is a name of WORK_KINDS or its code."""
@@ -677,9 +633,8 @@ class DeviceWork:
         if k.shape != v.shape:
             raise ValueError("vector and kind must have the same length")
         out = np.empty((v.shape[0], 3))
-        i32 = C.POINTER(C.c_int32)
-        check(self._lib.mbar_b200_work_evaluate(self._h, v.shape[0], v.ctypes.data_as(i32), k.ctypes.data_as(i32),
-                                                _dptr(a), _dptr(b), _dptr(out)))
+        check(self._lib.mbar_b200_work_evaluate(self._h, v.shape[0], _i32p(v), _i32p(k), _dptr(a), _dptr(b),
+                                                _dptr(out)))
         return out
 
     def last_stats(self):
