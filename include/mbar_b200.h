@@ -202,6 +202,22 @@ int mbar_b200_log_denominator(mbar_b200_ctx* ctx, const double* f_k, double* L_h
  * (communicator attached) are not supported: MBAR_B200_ERR_INVALID. */
 int mbar_b200_bin_moments(mbar_b200_ctx* ctx, const double* f_k, const double* u_n, const int32_t* bin_n,
                           int32_t nbins, double* f_bin, double* C, double* D);
+/* Unsampled-state updates of B bootstrap replicates of the resident samples in one call.  Replicate b draws sample n
+ * counts[b, n] times ([B, N_local] row-major) and has free energies F[b] ([B, K] row-major; only sampled entries are
+ * read).  For every replicate and every unsampled state j (N_k = 0, in index order; n_u of them):
+ *   out[b, j] = -log sum_n counts[b,n] exp(-u_jn - L_bn),   L_bn = log sum_{k: N_k > 0} N_k exp(F[b,k] - u_kn),
+ * i.e. what mbar_b200_set_sample_weights(counts[b]) + mbar_b200_self_consistent_update(F[b]) return for row j.
+ * +inf where no term is nonzero (a row of +inf energies).  Range errors are those of self_consistent_update for
+ * every replicate (check_range on each F[b]; check_unsampled_clamp).  A replicate whose counts sum to 0, B < 1, or a
+ * context with a communicator -> MBAR_B200_ERR_INVALID.  Multiplicities set by mbar_b200_set_sample_weights are
+ * neither used nor changed.  Row b is summed in an order fixed by N and K alone: it does not depend on B or on the
+ * other replicates, repeat calls are bit-identical, and there are no floating-point atomics.  A failed call leaves
+ * the context usable.  The counts go to the device one batch of 8 replicates at a time, one batch ahead of the
+ * kernels (2 * 8 * 2 * N_local bytes of device memory whatever B is). */
+int mbar_b200_replicate_unsampled(mbar_b200_ctx* ctx, int64_t B, const uint16_t* counts, const double* F,
+                                  double* out);
+/* CUDA-event time of the kernels of the last call, its replicate batches, and the exps it evaluated. */
+int mbar_b200_last_replicate_stats(mbar_b200_ctx* ctx, double* ms, int32_t* batches, int64_t* exps);
 
 /* ---- kernel-density sums (pymbar FES with fes_type="kde", independent of any u_kn context) ------ */
 /* For the resident samples x_n in R^D with weights w_n >= 0 and query points y_q:

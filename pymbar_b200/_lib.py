@@ -71,6 +71,8 @@ SIGNATURES = {
     "mbar_b200_log_W_nk_rows": (C.c_int, [_ctx, _dp, C.c_int64, C.c_int64, C.c_void_p, C.c_int64, C.c_int]),
     "mbar_b200_log_denominator": (C.c_int, [_ctx, _dp, _dp]),
     "mbar_b200_bin_moments": (C.c_int, [_ctx, _dp, _dp, C.POINTER(C.c_int32), C.c_int32, _dp, _dp, _dp]),
+    "mbar_b200_replicate_unsampled": (C.c_int, [_ctx, C.c_int64, C.POINTER(C.c_uint16), _dp, _dp]),
+    "mbar_b200_last_replicate_stats": (C.c_int, [_ctx, _dp, C.POINTER(C.c_int32), C.POINTER(C.c_int64)]),
     "mbar_b200_kde_create": (C.c_int, [C.c_int, C.c_int64, C.c_int32, _dp, _dp, C.POINTER(_ctx)]),
     "mbar_b200_kde_destroy": (C.c_int, [_ctx]),
     "mbar_b200_kde_log_sum": (C.c_int, [_ctx, C.c_int32, C.c_double, C.c_int64, _dp, _dp]),

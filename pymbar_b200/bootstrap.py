@@ -35,6 +35,61 @@ def bootstrap_indices(N_k, n_bootstraps, rseed, x_kindices=None):
     return out
 
 
+def state_members(N_k, x_kindices):
+    """[samples of state k for k < K], each in increasing order (np.where(x_kindices == k)[0] of mbar.py:430), from
+    one stable argsort; None unless x_kindices labels every sample with a state in [0, K) and state k with exactly
+    N_k[k] samples (the only labellings for which the reference's draws are well defined)."""
+    N_k = np.asarray(N_k, dtype=np.int64)
+    x = np.asarray(x_kindices)
+    if x.shape != (int(N_k.sum()),) or not (x.dtype.kind in "iu" or x.size == 0):
+        return None
+    if x.size and (x.min() < 0 or x.max() >= len(N_k)):
+        return None
+    if not np.array_equal(np.bincount(x.astype(np.int64), minlength=len(N_k)), N_k):
+        return None
+    order = np.argsort(x, kind="stable")
+    first = np.concatenate([[0], np.cumsum(N_k)])
+    return [order[first[k]:first[k + 1]] for k in range(len(N_k))]
+
+
+def _draw_rints(rng, N_k, members):
+    N = int(np.sum(N_k))
+    rints = np.zeros(N, int)
+    for k, k_indices in enumerate(members):
+        n = int(N_k[k])
+        rints[k_indices] = k_indices[rng.integers(n, size=n)]
+    return rints
+
+
+def draw_mbar_replicates(rng, N_k, members, n_bootstraps, each=None):
+    """(states, counts): MBAR.__init__'s bootstrap draws (mbar.py:424-433) from `rng` (MBAR.rng, advanced exactly as
+    the reference advances it), as the generator state before each replicate and the multiplicities
+    counts[b, n] = #{p : rints_b[p] = n} as uint16 [B, N] (2 B N bytes against the reference's 8 B N of int64
+    bootstrap_rints).  counts is None if a multiplicity exceeds 65535.  each(b, rints), when given, sees every
+    replicate's indices as they are drawn."""
+    N = int(np.sum(N_k))
+    states = []
+    counts = np.zeros((int(n_bootstraps), N), dtype=np.uint16)
+    fits = True
+    for b in range(int(n_bootstraps)):
+        states.append(rng.bit_generator.state)
+        rints = _draw_rints(rng, N_k, members)
+        c = np.bincount(rints, minlength=N)
+        fits = fits and (c.max(initial=0) <= 65535)
+        counts[b] = np.minimum(c, 65535)
+        if each is not None:
+            each(b, rints)
+    return states, (counts if fits else None)
+
+
+def replicate_rints(rng, state, N_k, members):
+    """The reference's bootstrap_rints row of the replicate drawn from `state` (a bit-generator state of `rng`'s
+    kind), regenerated on a private generator: `rng` is not advanced."""
+    bg = type(rng.bit_generator)()
+    bg.state = state
+    return _draw_rints(np.random.Generator(bg), N_k, members)
+
+
 def bootstrap_f_k(problem, f_k, N_k, rints=None, n_bootstraps=0, rseed=None, x_kindices=None,
                   solver_protocol=None):
     """f_k_boots[b, :] of mbar.py:421-443 on a resident problem.

@@ -199,6 +199,9 @@ struct mbar_b200_ctx {
     double lastHessMs = 0.0, lastWeightsMs = 0.0;
     double lastBinMs = 0.0;              // mbar_b200_bin_moments: kernels after the pass (CUDA events)
     int lastBinChunks = 0;               // ... and the reads of u_kn its moments step took
+    double lastRepMs = 0.0;              // mbar_b200_replicate_unsampled: its kernels (CUDA events),
+    int lastRepBatches = 0;              // ... its replicate batches
+    int64_t lastRepExps = 0;             // ... and the exps it evaluated
     cudaEvent_t evH0 = nullptr, evH1 = nullptr, evH2 = nullptr;
 
     // counters

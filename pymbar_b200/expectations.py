@@ -45,8 +45,8 @@ def augmented_states(K, state_map):
 
 
 def expectations_inner(u_kn, N_k, f_k, A_n, u_ln, state_map, uncertainty_method=None, return_theta=False,
-                       device=0, problem=None):
-    """MBAR.compute_expectations_inner (mbar.py:766-1012) for the analytical (non-bootstrap) methods.
+                       device=0, problem=None, replicates=None):
+    """MBAR.compute_expectations_inner (mbar.py:766-1012).
 
     Same contract as the reference: A_n [I, N] observables, u_ln [L, N] energies of the states of interest,
     state_map either a 1-D list of states (free energies only) or a [2, S] table whose columns are
@@ -54,7 +54,13 @@ def expectations_inner(u_kn, N_k, f_k, A_n, u_ln, state_map, uncertainty_method=
 
     The appended rows form an augmented problem on top of the RESIDENT u_kn (`DeviceProblem.augmented`): only
     those rows are uploaded.  `problem` may name the resident DeviceProblem of (u_kn, N_k); otherwise the
-    residency cache of `mbar_solvers` provides it."""
+    residency cache of `mbar_solvers` provides it.
+
+    `replicates` = (F [B, K], counts [B, N]) adds the bootstrap keys of mbar.py:962-971: replicate b is the samples
+    drawn counts[b, n] times with free energies F[b] (MBAR.f_k_boots[b]).  One `replicate_unsampled` call on the same
+    augmented problem gives every replicate's appended rows, from which 'bootstrapped_observables' [B, S] and
+    'bootstrapped_f' [B, len(state_list)] follow as for b = 0.  Theta stays the svd-ew one of b = 0, as the reference
+    computes it for uncertainty_method="bootstrap" (mbar.py:1796)."""
     from . import mbar_solvers as ms
 
     u_kn = np.asarray(u_kn)
@@ -88,10 +94,20 @@ def expectations_inner(u_kn, N_k, f_k, A_n, u_ln, state_map, uncertainty_method=
     f_aug = np.concatenate([f_k, np.zeros(n_states + n_pairs)])
     N_aug = np.concatenate([np.asarray(N_k, dtype=np.float64), np.zeros(n_states + n_pairs)])
 
+    n_extra = n_states + n_pairs
+    boot = {}
+
     def run(base):
         with base.augmented(extra) as q:
             f_new = q.self_consistent_update(f_aug)        # appended rows: -logsumexp_n(-v_an - L_n)
             f_aug[K:] = f_new[K:]
+            if replicates is not None:
+                F, counts = replicates
+                F = np.asarray(F, dtype=np.float64)
+                F_aug = np.concatenate([F, np.zeros((F.shape[0], n_extra))], axis=1)
+                # the appended rows are the last unsampled states of the augmented problem
+                F_aug[:, K:] = q.replicate_unsampled(counts, F_aug)[:, -n_extra:]
+                boot["f"] = F_aug
             return q.weight_moments(f_aug)[1] if return_theta else None
 
     if problem is not None:
@@ -101,10 +117,15 @@ def expectations_inner(u_kn, N_k, f_k, A_n, u_ln, state_map, uncertainty_method=
             G = run(base)
 
     out = {}
+    shift = np.array([floor[i] for i in of_obs])
     if n_pairs:
-        shift = np.array([floor[i] for i in of_obs])
         out["observables"] = np.exp(f_aug[rows_l] - f_aug[rows_s]) + shift      # mbar.py:943-953
     out["f"] = f_aug[rows_l]
+    if replicates is not None:
+        fb = boot["f"]
+        obs_b = np.exp(fb[:, rows_l] - fb[:, rows_s]) + shift if n_pairs else np.zeros((len(fb), 0))
+        out["bootstrapped_observables"] = obs_b                                             # mbar.py:963-967
+        out["bootstrapped_f"] = fb[:, rows_l]
     if return_theta:
         Theta = est.asymptotic_covariance(G, N_aug, method=uncertainty_method)
         pick = np.concatenate([rows_s, rows_l]).astype(int)        # observables first, then their states

@@ -20,9 +20,18 @@ the CPU.  With the facade installed:
 
 * `_computeUnnormalizedLogWeights` (:1919-1934) is -u_n - L_n with L_n from the device's log denominators.
 
-Anything outside what the device path implements (bootstrap uncertainties, `uncertainty_method="svd"`, an
-augmented problem of more than `_lib.MAX_STATES` states) calls the original method, which then reads
-`self.Log_W_nk` and materialises it.  `uninstall()` restores the class.
+* `MBAR(..., n_bootstraps=B)` with B a positive int runs the original constructor with n_bootstraps=0, then draws the
+  replicates from `self.rng` as mbar.py:424-433 does and solves each with one weighted solve on the resident problem
+  (`bootstrap.bootstrap_f_k`; BAR on the replicate's columns under initialize="BAR").  `bootstrap_rints` becomes lazy:
+  the generator state before each replicate is kept and the rows are regenerated on first read.
+  `compute_free_energy_differences` and `compute_expectations_inner` with `uncertainty_method="bootstrap"` answer from
+  `f_k_boots`, the replicates' counts and one `DeviceProblem.replicate_unsampled` call on the augmented problem
+  (`expectations.expectations_inner(..., replicates=...)`).  A replicate whose device solve fails is solved on the
+  gathered `u_kn[:, rints]` (`STATS["mbar_boot_*"]`).
+
+Anything outside what the device path implements (`uncertainty_method="svd"`, an augmented problem of more than
+`_lib.MAX_STATES` states, bootstrap requests without device replicates or with a count above 65535) calls the
+original method, which then reads `self.Log_W_nk` and materialises it.  `uninstall()` restores the class.
 
 `install_fes_on` does the same for `pymbar.FES` (fes.py): `generate_fes` without bootstraps takes its log weights
 from the device and, for fes_type="histogram", builds the bin free energies with `pymbar_b200.fes.histogram_fes`;
@@ -98,7 +107,8 @@ STATS = {"tickets": 0, "redeemed": 0, "moments": 0, "expectations": 0, "expectat
          "fes_spline_moments": 0, "fes_spline_calls": 0, "ts_inefficiency": 0, "ts_multiple": 0, "ts_correlation": 0,
          "ts_equilibration": 0, "ts_fallbacks": 0, "oe_bar": 0, "oe_bar_zero": 0, "oe_exp": 0, "oe_exp_gauss": 0,
          "oe_evaluations": 0, "oe_fallbacks": 0, "fes_boot_solves": 0, "fes_boot_passes": 0, "fes_boot_fallbacks": 0,
-         "fes_boot_spline_solves": 0, "fes_boot_spline_sums": 0}
+         "fes_boot_spline_solves": 0, "fes_boot_spline_sums": 0, "mbar_boot_solves": 0, "mbar_boot_fallbacks": 0,
+         "expectations_boot": 0, "boot_rints_built": 0}
 
 
 class LogWeightTicket:
@@ -156,6 +166,110 @@ def _check_normalised(S, tolerance=1.0e-4):
                                f"{int(bad[0]):d} was {S[bad[0]]:f}. {bad.size:d} other columns have similar problems")
 
 
+class RintsTicket:
+    """Stands for MBAR.bootstrap_rints [B, N] (mbar.py:423-445) until somebody reads it: the generator state before
+    each replicate's draws, from which the rows are regenerated bit for bit."""
+
+    __slots__ = ("rng", "states", "N_k", "members")
+
+    def __init__(self, rng, states, N_k, members):
+        self.rng, self.states, self.N_k, self.members = rng, states, N_k, members
+
+    def redeem(self):
+        from . import bootstrap as bs
+
+        STATS["boot_rints_built"] += 1
+        out = np.zeros((len(self.states), int(np.sum(self.N_k))), int)
+        for b, state in enumerate(self.states):
+            out[b] = bs.replicate_rints(self.rng, state, self.N_k, self.members)
+        return out
+
+
+def _solver_module(mbar):
+    """The solver module the MBAR class resolves its solves through (pymbar.mbar_solvers for pymbar.MBAR)."""
+    import sys
+
+    from . import mbar_solvers as ms
+
+    own = getattr(type(mbar), "solvers", None)
+    return own if own is not None else getattr(sys.modules.get(type(mbar).__module__), "mbar_solvers", ms)
+
+
+def _bootstrap_protocol(mbar, prot):
+    """The bootstrap_solver_protocol as mbar.py:370-411 resolves it (the original normalised the dicts in place)."""
+    import sys
+
+    from . import fes_bootstrap as fb
+
+    mod = sys.modules.get(type(mbar).__module__)
+    solvers = _solver_module(mbar)
+
+    def const(name):
+        v = getattr(mod, name, None)
+        return v if v is not None else getattr(solvers, name)
+
+    default = const("BOOTSTRAP_SOLVER_PROTOCOL")
+    if prot is None or (isinstance(prot, str) and prot == "default"):
+        prot = default
+    elif isinstance(prot, str) and prot == "robust":
+        prot = const("ROBUST_SOLVER_PROTOCOL")
+    elif isinstance(prot, str) and prot == "jax":
+        prot = const("JAX_SOLVER_PROTOCOL")
+    elif any(not isinstance(st, dict) for st in prot):
+        prot = default
+    return fb.solver_protocol(prot)
+
+
+def _mbar_bootstraps(mbar, n_bootstraps, members, arguments):
+    """f_k_boots of mbar.py:417-449 after the original constructor ran with n_bootstraps=0.  The replicates are drawn
+    from mbar.rng as the reference draws them; each is one weighted solve on the resident problem of mbar.u_kn
+    (bootstrap.bootstrap_f_k), started at mbar.f_k or, under initialize="BAR", at BAR on the replicate's columns.  A
+    replicate whose device solve raises is solved the original way, on the gathered u_kn[:, rints]."""
+    import logging
+
+    from . import _lib
+    from . import bootstrap as bs
+    from . import initialize as init
+    from . import mbar_solvers as ms
+
+    N_k = np.asarray(mbar.N_k, dtype=np.int64)
+    protocol = _bootstrap_protocol(mbar, arguments.get("bootstrap_solver_protocol"))
+    f_k = np.array(mbar.f_k, dtype=np.float64)
+    bar = arguments.get("initialize") == "BAR"
+    verbose = arguments.get("verbose")
+    maxfrac = int(max((1, 0.1 * n_bootstraps)))
+    log = logging.getLogger(type(mbar).__module__)
+    boots = np.zeros((n_bootstraps, len(N_k)))
+    with ms._borrow(mbar.u_kn, N_k.astype(np.float64)) as p:
+        def solve(b, rints):
+            start = init.initialize_with_bar(mbar.u_kn, N_k, mbar.x_kindices, f_k, columns=rints) if bar else f_k
+            try:
+                boots[b] = bs.bootstrap_f_k(p, start, N_k, rints=rints[None], solver_protocol=protocol)[0]
+                STATS["mbar_boot_solves"] += 1
+            except _lib.MbarB200Error:
+                STATS["mbar_boot_fallbacks"] += 1
+                boots[b] = _solver_module(mbar).solve_mbar_for_all_states(
+                    mbar.u_kn[:, rints], mbar.N_k, np.array(start), np.flatnonzero(N_k > 0), protocol)
+            if verbose and b % maxfrac == 0:
+                log.info(f"Calculated {b + 1:d}/{n_bootstraps:d} bootstrap samples")
+
+        states, counts = bs.draw_mbar_replicates(mbar.rng, N_k, members, n_bootstraps, solve)
+    mbar.n_bootstraps = n_bootstraps
+    mbar.f_k_boots = boots
+    mbar.__dict__["_b200_rints"] = RintsTicket(mbar.rng, states, N_k, members)
+    mbar.__dict__["_b200_boot_counts"] = counts
+
+
+def _replicate_counts(mbar):
+    """counts [B, N] of the replicates behind mbar.f_k_boots: the constructor's, or the multiplicities of whatever was
+    assigned to bootstrap_rints; None when one exceeds 65535."""
+    if "_b200_boot_counts" in mbar.__dict__:
+        return mbar.__dict__["_b200_boot_counts"]
+    rints = np.asarray(mbar.bootstrap_rints)
+    counts = np.stack([np.bincount(r, minlength=int(mbar.N)) for r in rints])
+    return counts if counts.max(initial=0) <= 65535 else None
+
+
 def install_on(MBAR):
     """Patch the class object `MBAR` (pymbar.mbar.MBAR)."""
     if MBAR in _SAVED:
@@ -163,18 +277,69 @@ def install_on(MBAR):
     saved = {name: MBAR.__dict__.get(name) for name in
              ("__init__", "Log_W_nk", "compute_effective_sample_number", "compute_overlap",
               "compute_free_energy_differences", "compute_expectations_inner", "_initialize_with_bar",
-              "_computeUnnormalizedLogWeights")}
+              "_computeUnnormalizedLogWeights", "bootstrap_rints")}
     _SAVED[MBAR] = saved
     orig_init = saved["__init__"]
     orig_fed = saved["compute_free_energy_differences"]
     orig_inner = saved["compute_expectations_inner"]
+    import inspect
+
+    try:
+        init_sig = inspect.signature(orig_init)
+    except (TypeError, ValueError):
+        init_sig = None
+
+    def _bootstrap_request(self, args, kwargs):
+        """(bound arguments, B, members) when the device draws and solves the replicates: n_bootstraps a positive
+        int (not bool) and x_kindices a labelling for which the reference's draws are defined; else None."""
+        from . import bootstrap as bs
+
+        if init_sig is None or "n_bootstraps" not in init_sig.parameters:
+            return None
+        try:
+            bound = init_sig.bind(self, *args, **kwargs)
+        except TypeError:
+            return None
+        bound.apply_defaults()
+        n = bound.arguments["n_bootstraps"]
+        if not isinstance(n, (int, np.integer)) or isinstance(n, bool) or n <= 0:
+            return None
+        try:
+            N_k = np.array(bound.arguments["N_k"], dtype=np.int64)
+            x = bound.arguments.get("x_kindices")
+            x = np.repeat(np.arange(len(N_k)), N_k) if x is None else x
+            members = bs.state_members(N_k, x)
+        except (TypeError, ValueError):
+            return None
+        return None if members is None else (bound, int(n), members)
 
     def __init__(self, *args, **kwargs):
+        boot = _bootstrap_request(self, args, kwargs)
+        if boot is not None:
+            bound = boot[0]
+            bound.arguments["n_bootstraps"] = 0
+            args, kwargs = bound.args[1:], bound.kwargs
         _TLS.defer = getattr(_TLS, "defer", 0) + 1
         try:
             orig_init(self, *args, **kwargs)
         finally:
             _TLS.defer -= 1
+        if boot is not None:
+            _mbar_bootstraps(self, boot[1], boot[2], boot[0].arguments)
+
+    def _get_rints(self):
+        try:
+            v = self.__dict__["_b200_rints"]
+        except KeyError:
+            raise AttributeError(f"{type(self).__name__!r} object has no attribute 'bootstrap_rints'") from None
+        if isinstance(v, RintsTicket):
+            v = v.redeem()
+            self.__dict__["_b200_rints"] = v
+        return v
+
+    def _set_rints(self, value):
+        self.__dict__["_b200_rints"] = value
+        self.__dict__.pop("_b200_boot_counts", None)
 
     def _get_logw(self):
         v = self.__dict__.get("_b200_logw")
@@ -205,18 +370,23 @@ def install_on(MBAR):
 
     def compute_free_energy_differences(self, compute_uncertainty=True, uncertainty_method=None,
                                         warning_cutoff=1.0e-10, return_theta=False):
-        device_ok = uncertainty_method in (None, "svd-ew", "approximate")
+        # bootstrap: the spread of the replicates' differences (mbar.py:706-714), Theta from the device's moments
+        boot = uncertainty_method == "bootstrap" and getattr(self, "f_k_boots", None) is not None
+        device_ok = uncertainty_method in (None, "svd-ew", "approximate") or boot
         if not device_ok and (compute_uncertainty or return_theta):
             return orig_fed(self, compute_uncertainty=compute_uncertainty, uncertainty_method=uncertainty_method,
                             warning_cutoff=warning_cutoff, return_theta=return_theta)
         Delta = np.array(self.f_k - np.vstack(self.f_k))
         self._zerosamestates(Delta)
         out = {"Delta_f": Delta}
-        if compute_uncertainty or return_theta:
+        if boot and compute_uncertainty:
+            F = np.asarray(self.f_k_boots)
+            out["dDelta_f"] = np.std(F[:, None, :] - F[:, :, None], axis=0)
+        if return_theta or (compute_uncertainty and not boot):
             S, G = _moments(self)
             _check_normalised(S)
             Theta = est.asymptotic_covariance(G, self.N_k, method=uncertainty_method)
-            if compute_uncertainty:
+            if compute_uncertainty and not boot:
                 d = np.array(est.error_of_differences(Theta, warning_cutoff=warning_cutoff))
                 self._zerosamestates(d)
                 out["dDelta_f"] = d
@@ -226,23 +396,40 @@ def install_on(MBAR):
 
     def compute_expectations_inner(self, A_n, u_ln, state_map, uncertainty_method=None, warning_cutoff=1.0e-10,
                                    return_theta=False):
-        if uncertainty_method not in (None, "svd-ew", "approximate"):
+        boot = uncertainty_method == "bootstrap" and getattr(self, "f_k_boots", None) is not None
+        if uncertainty_method not in (None, "svd-ew", "approximate") and not boot:
             return orig_inner(self, A_n, u_ln, state_map, uncertainty_method=uncertainty_method,
                               warning_cutoff=warning_cutoff, return_theta=return_theta)
         from . import _lib
         from . import expectations as ex
         from . import mbar_solvers as ms
 
-        # the augmented problem holds K + one row per state of interest + one per (state, observable) pair; past
-        # what a context takes, the original answers (checked up front: ERR_INVALID may also mean a bad argument)
-        if ex.augmented_states(np.shape(self.u_kn)[0], state_map) > _lib.MAX_STATES:
+        def fallback():
             STATS["expectations_fallbacks"] += 1
             return orig_inner(self, A_n, u_ln, state_map, uncertainty_method=uncertainty_method,
                               warning_cutoff=warning_cutoff, return_theta=return_theta)
-        STATS["expectations"] += 1
-        return ex.expectations_inner(self.u_kn, self.N_k, self.f_k, A_n, u_ln, state_map,
-                                     uncertainty_method=uncertainty_method, return_theta=return_theta,
-                                     device=ms._DEVICE)
+
+        # the augmented problem holds K + one row per state of interest + one per (state, observable) pair; past
+        # what a context takes, the original answers (checked up front: ERR_INVALID may also mean a bad argument)
+        if ex.augmented_states(np.shape(self.u_kn)[0], state_map) > _lib.MAX_STATES:
+            return fallback()
+        if not boot:
+            STATS["expectations"] += 1
+            return ex.expectations_inner(self.u_kn, self.N_k, self.f_k, A_n, u_ln, state_map,
+                                         uncertainty_method=uncertainty_method, return_theta=return_theta,
+                                         device=ms._DEVICE)
+        # bootstrap: every replicate's appended rows from one replicate_unsampled call (mbar.py:890-971)
+        counts = _replicate_counts(self)
+        if counts is None:
+            return fallback()
+        try:
+            out = ex.expectations_inner(self.u_kn, self.N_k, self.f_k, A_n, u_ln, state_map,
+                                        uncertainty_method=uncertainty_method, return_theta=return_theta,
+                                        device=ms._DEVICE, replicates=(self.f_k_boots, counts))
+        except _lib.MbarB200Error:
+            return fallback()
+        STATS["expectations_boot"] += 1
+        return out
 
     def _initialize_with_bar(self, u_kn, f_k_init=None):
         from . import initialize as init
@@ -256,6 +443,8 @@ def install_on(MBAR):
     MBAR._initialize_with_bar = _initialize_with_bar
     MBAR.__init__ = __init__
     MBAR.Log_W_nk = property(_get_logw, _set_logw, doc="log weights [N, K] (mbar.py:455), downloaded on first use")
+    MBAR.bootstrap_rints = property(_get_rints, _set_rints,
+                                    doc="bootstrap indices [B, N] (mbar.py:423-445), regenerated on first use")
     MBAR.compute_effective_sample_number = compute_effective_sample_number
     MBAR.compute_overlap = compute_overlap
     MBAR.compute_free_energy_differences = compute_free_energy_differences

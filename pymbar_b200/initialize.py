@@ -61,9 +61,13 @@ def bar_delta_f(w_F, w_R, guess=0.0, rtol=1.0e-5, maxiter=100):
                                  maxiter=maxiter, disp=False)
 
 
-def initialize_with_bar(u_kn, N_k, x_kindices, f_k_init=None):
+def initialize_with_bar(u_kn, N_k, x_kindices, f_k_init=None, columns=None):
     """f_k seeded by BAR along the chain of sampled states (mbar.py:1936-1988).  `x_kindices[n]` is the state
-    sample n was drawn from (mbar.py:264-268)."""
+    sample n was drawn from (mbar.py:264-268).
+
+    `columns` [N] (a bootstrap replicate's rints) makes it BAR on the gathered u_kn[:, columns] without the gather:
+    position p keeps its label x_kindices[p] and reads the energies of sample columns[p], and only the two rows of each
+    adjacent pair are read at those columns (what mbar.py:436 and :1957-1960 compute on the gathered matrix)."""
     u_kn = np.asarray(u_kn)
     N_k = np.asarray(N_k)
     K = len(N_k)
@@ -77,6 +81,8 @@ def initialize_with_bar(u_kn, N_k, x_kindices, f_k_init=None):
     members = lambda k: idx[first[k]:first[k + 1]]           # noqa: E731
     for k, l in zip(order[:-1], order[1:]):
         nk, nl = members(k), members(l)
+        if columns is not None:
+            nk, nl = np.asarray(columns)[nk], np.asarray(columns)[nl]
         if len(nk) == 0 or len(nl) == 0:
             f[l] = 0.0
             continue

@@ -353,6 +353,32 @@ class DeviceProblem(_Resident):
         check(self._lib.mbar_b200_last_bin_stats(self._h, C.byref(ms), C.byref(chunks)))
         return dict(ms=ms.value, chunks=chunks.value)
 
+    def replicate_unsampled(self, counts, F):
+        """[B, n_u]: for bootstrap replicate b with multiplicities counts[b] [N] and free energies F[b] [K], the
+        unsampled states' updates -log sum_n counts[b, n] exp(-u_jn - L_bn), what set_sample_weights(counts[b]) +
+        self_consistent_update(F[b]) give for those rows, every replicate in one device call
+        (mbar_b200_replicate_unsampled).  Counts are sent as uint16: above 65535 (or negative) raises ValueError."""
+        c = np.asarray(counts)
+        if c.ndim != 2 or c.shape[1] != self.N:
+            raise ValueError(f"counts must be [B, {self.N}], got shape {c.shape}")
+        if c.size and (c.min() < 0 or c.max() > 65535):
+            raise ValueError("replicate counts must lie in [0, 65535]")
+        c = np.ascontiguousarray(c, dtype=np.uint16)
+        F = np.ascontiguousarray(F, dtype=np.float64)
+        if F.shape != (c.shape[0], self.K):
+            raise ValueError(f"F must be [{c.shape[0]}, {self.K}], got shape {F.shape}")
+        out = np.empty((c.shape[0], int(np.sum(~(self.N_k > 0)))))
+        check(self._lib.mbar_b200_replicate_unsampled(self._h, c.shape[0], c.ctypes.data_as(C.POINTER(C.c_uint16)),
+                                                      _dptr(F), _dptr(out)))
+        return out
+
+    def last_replicate_stats(self):
+        """CUDA-event time (ms) of the last replicate_unsampled's kernels, its replicate batches and the exps it
+        evaluated."""
+        ms, batches, exps = C.c_double(0), C.c_int32(0), C.c_int64(0)
+        check(self._lib.mbar_b200_last_replicate_stats(self._h, C.byref(ms), C.byref(batches), C.byref(exps)))
+        return dict(ms=ms.value, batches=batches.value, exps=exps.value)
+
     # ---- native loops ---------------------------------------------------------------------------
     @staticmethod
     def _result(r):
