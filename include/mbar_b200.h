@@ -334,8 +334,12 @@ int mbar_b200_acf_destroy(mbar_b200_acf* acf);
  * g before the g >= 1 clamp, last_lag (the last t whose C was computed, 0 if none) and status (1: sigma^2 == 0, the
  * reference's ParameterError; g = 1 and no lag evaluated).  trace [n_starts][trace_cap] (trace_cap may be 0) gets
  * C at the first trace_cap lag indices evaluated, NaN after the last.  Lags are evaluated in rounds of 8, 8, 16, 32,
- * ... lag indices for all active starts, with one host poll per round.  A start outside [0, T) or a rule the object
- * cannot take -> MBAR_B200_ERR_INVALID.  A failed call leaves the object usable. */
+ * ... lag indices for all active starts, with one host poll per round.
+ * rule 2 (an unsegmented autocorrelation object, fast = 0, any starts) is statistical_inefficiency_fft's loop over
+ * statsmodels' acf(adjusted=True): C(t) = (S(t) / (m - t)) / sigma^2 with S(t) the single-product sum
+ * sum_{n = s}^{T-1-t} dA[n] dA[n+t], evaluated by direct lag sums (not an FFT), t = 1 .. m - 1 inclusive, stop at the
+ * first C <= 0 with t > mintime (that lag excluded), g += 2.0 * C * (1.0 - t / m).  A start outside [0, T) or a rule
+ * the object cannot take -> MBAR_B200_ERR_INVALID.  A failed call leaves the object usable. */
 int mbar_b200_acf_inefficiency(mbar_b200_acf* acf, int64_t n_starts, const int64_t* starts, int32_t fast,
                                int32_t mintime, int32_t rule, double navg, int64_t trace_cap, double* mean_a,
                                double* mean_b, double* sigma2, double* g, int64_t* last_lag, int32_t* status,
@@ -344,8 +348,22 @@ int mbar_b200_acf_inefficiency(mbar_b200_acf* acf, int64_t n_starts, const int64
  * n_max outside [0, T - start - 1], a segmented object or sigma^2 == 0 -> MBAR_B200_ERR_INVALID. */
 int mbar_b200_acf_correlation(mbar_b200_acf* acf, int64_t start, int64_t n_max, double* C, double* mean_a,
                               double* mean_b, double* sigma2);
+/* normalized_fluctuation_correlation_function_multiple of a segmented object (K series, A and optionally B): pooled
+ * means mu_A, mu_B over all N = T samples, S_k(t) = sum_{n < N_k - t} dA_k[n] dB_k[n + t] (one product, over the
+ * series with N_k > t), C(t) = ((0.0 + sum_k S_k(t)) / sum_k (N_k - t)) / sigma^2 with sigma^2 = sum_k S_k(0) / N
+ * (so C(0) == 1.0), for t = 0 .. n_max into C [n_max + 1].  Each series is cut into its own chunks of
+ * max(512, ceil(N_k / 1024)) samples; a (series, lag) sum adds its chunk partials in order and the numerator the
+ * series in list order, so results are bit-identical across calls and launch splits, with no floating-point atomics.
+ * n_out gets the length the reference returns: n_max, or with truncate the first t at which a running numerator
+ * (after each series, in list order) is negative; truncate evaluates lags in rounds of 8, 8, 16, 32, ... and leaves
+ * NaN in C past the last round.  mean_a, mean_b, sigma2 may be NULL.  An unsegmented object, n_max outside
+ * [0, max N_k - 1] or sigma^2 == 0 -> MBAR_B200_ERR_INVALID. */
+int mbar_b200_acf_correlation_multiple(mbar_b200_acf* acf, int64_t n_max, int32_t truncate, double* C, int64_t* n_out,
+                                       double* mean_a, double* mean_b, double* sigma2);
 /* CUDA-event time of the last call, its lag rounds (host polls), and the (start, lag, n) terms of lags >= 1 it
- * evaluated and of those up to each start's last lag; terms / useful_terms is the speculative batches' waste. */
+ * evaluated and of those up to each start's last lag; terms / useful_terms is the speculative batches' waste.  After
+ * mbar_b200_acf_correlation_multiple: its truncate rounds (0 without truncate) and the (series, lag, n) terms of
+ * lags >= 0 evaluated and of those through the reference's last lag. */
 int mbar_b200_last_acf_stats(mbar_b200_acf* acf, double* ms, int32_t* rounds, int64_t* terms, int64_t* useful_terms);
 
 /* ---- sums over work vectors (pymbar.other_estimators: BAR, EXP, Gaussian EXP; no u_kn context) -- */

@@ -93,6 +93,8 @@ SIGNATURES = {
                                              C.c_double, C.c_int64, _dp, _dp, _dp, _dp, C.POINTER(C.c_int64),
                                              C.POINTER(C.c_int32), _dp]),
     "mbar_b200_acf_correlation": (C.c_int, [_ctx, C.c_int64, C.c_int64, _dp, _dp, _dp, _dp]),
+    "mbar_b200_acf_correlation_multiple": (C.c_int, [_ctx, C.c_int64, C.c_int32, _dp, C.POINTER(C.c_int64), _dp, _dp,
+                                                     _dp]),
     "mbar_b200_last_acf_stats": (C.c_int, [_ctx, _dp, C.POINTER(C.c_int32), C.POINTER(C.c_int64),
                                            C.POINTER(C.c_int64)]),
     "mbar_b200_work_create": (C.c_int, [C.c_int, C.c_int64, _dp, C.c_int32, C.POINTER(C.c_int64), C.POINTER(_ctx)]),

@@ -187,6 +187,7 @@ struct AcfWalkParams {
     int64_t i0;                 // first lag index of the batch
     int64_t T;
     int fast, multiple, cross;
+    int fft;                    // rule 2: statistical_inefficiency_fft's acf and its lags 1 .. m - 1
     int64_t mintime;
     double navg;
     int64_t limitMultiple;      // max N_k (multiple rule)
@@ -204,7 +205,7 @@ __global__ void acf_walk_kernel(AcfWalkParams p) {
     const int j = p.act[si];
     const int64_t s = p.starts[j];
     const int64_t m = p.T - s;
-    const int64_t limit = p.multiple ? p.limitMultiple : m;
+    const int64_t limit = p.multiple ? p.limitMultiple : (p.fft ? m + 1 : m);
     const double s2 = p.sigma2[j];
     double g = p.g[j];
     int64_t last = p.lastLag[j];
@@ -223,6 +224,8 @@ __global__ void acf_walk_kernel(AcfWalkParams p) {
             for (int q = 0; q < p.nSeg; ++q)
                 if (t < p.segLen[q]) den += p.segLen[q] - t;
             C = __ddiv_rn(__ddiv_rn(sum, (double)den), s2);
+        } else if (p.fft) {
+            C = __ddiv_rn(__ddiv_rn(sum, (double)(m - t)), s2);       // acov(t) / acov(0), acov(0) = sigma^2
         } else {
             const double num = p.cross ? sum : __dmul_rn(2.0, sum);
             C = __ddiv_rn(num, __dmul_rn(__dmul_rn(2.0, (double)(m - t)), s2));
@@ -392,7 +395,7 @@ int mbar_b200_acf_inefficiency(mbar_b200_acf* o, int64_t n_starts, const int64_t
     MBAR_REQUIRE(n_starts >= 1 && n_starts < INT32_MAX && starts, MBAR_B200_ERR_INVALID,
                  "acf_inefficiency: %lld starts", (long long)n_starts);
     MBAR_REQUIRE(g && last_lag && status, MBAR_B200_ERR_INVALID, "acf_inefficiency: NULL output");
-    MBAR_REQUIRE(rule == 0 || rule == 1, MBAR_B200_ERR_INVALID, "acf_inefficiency: unknown rule %d", (int)rule);
+    MBAR_REQUIRE(rule >= 0 && rule <= 2, MBAR_B200_ERR_INVALID, "acf_inefficiency: unknown rule %d", (int)rule);
     MBAR_REQUIRE(trace_cap >= 0 && (trace_cap == 0 || trace), MBAR_B200_ERR_INVALID,
                  "acf_inefficiency: trace_cap %lld without a trace buffer", (long long)trace_cap);
     MBAR_REQUIRE(trace_cap <= (int64_t(1) << 31) / n_starts, MBAR_B200_ERR_INVALID,
@@ -406,6 +409,9 @@ int mbar_b200_acf_inefficiency(mbar_b200_acf* o, int64_t n_starts, const int64_t
     } else {
         MBAR_REQUIRE(o->nSeg == 0, MBAR_B200_ERR_INVALID, "acf_inefficiency: a segmented object takes rule 1");
     }
+    if (rule == 2)
+        MBAR_REQUIRE(!o->cross && !fast, MBAR_B200_ERR_INVALID,
+                     "acf_inefficiency: the FFT rule needs an autocorrelation and fast = 0");
     for (int64_t j = 0; j < n_starts; ++j)
         MBAR_REQUIRE(starts[j] >= 0 && starts[j] < o->T, MBAR_B200_ERR_INVALID,
                      "acf_inefficiency: start %lld outside [0, %lld)", (long long)starts[j], (long long)o->T);
@@ -416,7 +422,8 @@ int mbar_b200_acf_inefficiency(mbar_b200_acf* o, int64_t n_starts, const int64_t
     int64_t limitMultiple = 0;
     for (int64_t L : o->segLen) limitMultiple = std::max(limitMultiple, L);
     int64_t maxLimit = 0;
-    for (int64_t s : hs) maxLimit = std::max(maxLimit, rule == 1 ? limitMultiple : o->T - s);
+    // lags run while t < limit - 1: limit = m for rule 0, m + 1 for rule 2 (its lags include m - 1)
+    for (int64_t s : hs) maxLimit = std::max(maxLimit, rule == 1 ? limitMultiple : o->T - s + (rule == 2 ? 1 : 0));
     CallBuffers buf("acf");
     int64_t* d_starts;
     double *d_muA, *d_muB, *d_s2, *d_g, *d_S, *d_partial, *d_trace = nullptr;
@@ -500,6 +507,7 @@ int mbar_b200_acf_inefficiency(mbar_b200_acf* o, int64_t n_starts, const int64_t
             w.fast = fast ? 1 : 0;
             w.multiple = rule == 1;
             w.cross = o->cross;
+            w.fft = rule == 2;
             w.mintime = mintime;
             w.navg = navg;
             w.limitMultiple = limitMultiple;
@@ -613,6 +621,260 @@ int mbar_b200_acf_correlation(mbar_b200_acf* o, int64_t start, int64_t n_max, do
     o->lastTerms = o->lastUseful = 0;
     for (int64_t t = 0; t < nl; ++t) o->lastTerms += o->T - start - t;
     o->lastUseful = o->lastTerms;
+    return MBAR_B200_OK;
+}
+
+// ---- normalized_fluctuation_correlation_function_multiple (timeseries.py:509-658) ----------------------------------
+// Series k of a segmented object (offset o_k, length L_k) is cut into its own chunks of max(512, ceil(L_k / 1024))
+// samples: no chunk straddles two series and the bounds depend on the lengths alone.  The sum of a (series, lag) is
+// 0.0 + its chunk partials in order, and a lag's numerator 0.0 + those sums in list order, as the reference adds one
+// np.sum per series; the pooled means are the same construction.
+namespace mbar {
+
+// chunk totals of A and B: tot[c] = 0.0 + sum over [lo[c], hi[c]) in n order
+__global__ void acf_seg_total_kernel(const double* __restrict__ a, const double* __restrict__ b,
+                                     const int64_t* __restrict__ lo, const int64_t* __restrict__ hi, int64_t nChunks,
+                                     double* totA, double* totB) {
+    const int64_t c = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (c >= nChunks) return;
+    double sa = 0.0, sb = 0.0;
+    for (int64_t n = lo[c]; n < hi[c]; ++n) {
+        sa = __dadd_rn(sa, a[n]);
+        sb = __dadd_rn(sb, b[n]);
+    }
+    totA[c] = sa;
+    totB[c] = sb;
+}
+
+// pooled means (one thread): each series' chunk totals in order, the series in list order, over N
+__global__ void acf_seg_mean_kernel(const double* __restrict__ totA, const double* __restrict__ totB,
+                                    const int64_t* __restrict__ chunkOff, int K, int64_t N, double* mu) {
+    if (blockIdx.x != 0 || threadIdx.x != 0) return;
+    double pa = 0.0, pb = 0.0;
+    for (int k = 0; k < K; ++k) {
+        double sa = 0.0, sb = 0.0;
+        for (int64_t c = chunkOff[k]; c < chunkOff[k + 1]; ++c) {
+            sa = __dadd_rn(sa, totA[c]);
+            sb = __dadd_rn(sb, totB[c]);
+        }
+        pa = __dadd_rn(pa, sa);
+        pb = __dadd_rn(pb, sb);
+    }
+    mu[0] = __ddiv_rn(pa, (double)N);
+    mu[1] = __ddiv_rn(pb, (double)N);
+}
+
+struct AcfSegParams {
+    const double* a;
+    const double* b;
+    const int64_t* lo;          // [nChunks] chunk bounds
+    const int64_t* hi;
+    const int64_t* end;         // [nChunks] end of the chunk's series
+    const double* mu;           // [2] pooled means
+    double* partial;            // [nChunks][nLags]
+    int64_t l0;                 // lags l0 .. l0 + nLags - 1
+    int nLags, LG;
+};
+
+// partial[c][jl] = 0.0 + sum over the chunk's n with n + t in its series of dA[n] dB[n + t], t = l0 + jl; one thread
+// per ACF_RL consecutive lags, one chunk per blockIdx.x
+__global__ void __launch_bounds__(ACF_THREADS) acf_seg_partial_kernel(AcfSegParams p) {
+    const int lg = (int)blockIdx.y * ACF_THREADS + threadIdx.x;
+    if (lg >= p.LG) return;
+    const int64_t c = blockIdx.x;
+    const int64_t c0 = p.lo[c], c1 = p.hi[c], end = p.end[c];
+    const double mua = p.mu[0], mub = p.mu[1];
+    const int jl0 = lg * ACF_RL;
+    int64_t t[ACF_RL];
+    double acc[ACF_RL];
+#pragma unroll
+    for (int r = 0; r < ACF_RL; ++r) {
+        t[r] = (jl0 + r < p.nLags) ? p.l0 + jl0 + r : INT64_MAX / 2;
+        acc[r] = 0.0;
+    }
+    const int64_t hi = min(c1, end - t[0]);
+    for (int64_t n = c0; n < hi; ++n) {
+        const double da = __dsub_rn(__ldg(p.a + n), mua);
+#pragma unroll
+        for (int r = 0; r < ACF_RL; ++r)
+            if (n + t[r] < end) acc[r] = __dadd_rn(acc[r], __dmul_rn(da, __dsub_rn(__ldg(p.b + n + t[r]), mub)));
+    }
+#pragma unroll
+    for (int r = 0; r < ACF_RL; ++r)
+        if (jl0 + r < p.nLags) p.partial[c * p.nLags + jl0 + r] = acc[r];
+}
+
+// per lag t = l0 + jl: numerator = 0.0 + the series sums (each 0.0 + its chunk partials in order) of the series with
+// L_k > t in list order, denominator = 0.0 + (double)(L_k - t) over the same series; neg[jl] = 1 when a running
+// numerator is negative (truncate, timeseries.py:641); out[jl] = (numerator / denominator) / sigma2, or the
+// numerator itself where sigma2 is NULL (the lag-0 pass that gives sigma^2)
+__global__ void acf_seg_combine_kernel(const double* __restrict__ partial, const int64_t* __restrict__ chunkOff,
+                                       const int64_t* __restrict__ segLen, int K, int64_t l0, int nLags,
+                                       const double* __restrict__ sigma2, double* out, int8_t* neg) {
+    const int jl = blockIdx.x * blockDim.x + threadIdx.x;
+    if (jl >= nLags) return;
+    const int64_t t = l0 + jl;
+    double num = 0.0, den = 0.0;
+    int8_t negative = 0;
+    for (int k = 0; k < K; ++k) {
+        if (t >= segLen[k]) continue;
+        double s = 0.0;
+        for (int64_t c = chunkOff[k]; c < chunkOff[k + 1]; ++c) s = __dadd_rn(s, partial[c * nLags + jl]);
+        num = __dadd_rn(num, s);
+        den = __dadd_rn(den, (double)(segLen[k] - t));
+        if (num < 0.0) negative = 1;
+    }
+    out[jl] = sigma2 ? __ddiv_rn(__ddiv_rn(num, den), sigma2[0]) : num;
+    if (neg) neg[jl] = negative;
+}
+
+__global__ void acf_seg_sigma_kernel(const double* __restrict__ num0, int64_t N, double* sigma2) {
+    if (blockIdx.x == 0 && threadIdx.x == 0) sigma2[0] = __ddiv_rn(num0[0], (double)N);
+}
+
+// sum over lags t in [t0, t1) of max(L - t, 0): the lag terms of one series
+inline int64_t seg_lag_terms(int64_t L, int64_t t0, int64_t t1) {
+    const int64_t hi = std::min(t1, L);
+    if (hi <= t0) return 0;
+    const int64_t n = hi - t0;
+    return n * L - (t0 + hi - 1) * n / 2;
+}
+
+}  // namespace mbar
+
+int mbar_b200_acf_correlation_multiple(mbar_b200_acf* o, int64_t n_max, int32_t truncate, double* C,
+                                       int64_t* n_out, double* mean_a, double* mean_b, double* sigma2) {
+    MBAR_REQUIRE(o, MBAR_B200_ERR_INVALID, "acf_correlation_multiple: NULL object");
+    MBAR_REQUIRE(C && n_out, MBAR_B200_ERR_INVALID, "acf_correlation_multiple: NULL output");
+    MBAR_REQUIRE(o->nSeg > 0, MBAR_B200_ERR_INVALID, "acf_correlation_multiple: the object holds no segments");
+    const int K = o->nSeg;
+    int64_t Lmax = 0;
+    for (int64_t L : o->segLen) Lmax = std::max(Lmax, L);
+    MBAR_REQUIRE(n_max >= 0 && n_max <= Lmax - 1, MBAR_B200_ERR_INVALID,
+                 "acf_correlation_multiple: N_max %lld outside [0, %lld]", (long long)n_max, (long long)(Lmax - 1));
+    MBAR_CUDA(cudaSetDevice(o->device));
+    NvtxRange nvtx_("mbar_b200::acf_correlation_multiple");
+    std::vector<int64_t> lo, hi, end, chunkOff((size_t)K + 1, 0);
+    {
+        int64_t off = 0;
+        for (int k = 0; k < K; ++k) {
+            const int64_t L = o->segLen[k];
+            const int64_t NC = std::max<int64_t>(ACF_MIN_NC, (L + ACF_MAX_CHUNKS - 1) / ACF_MAX_CHUNKS);
+            for (int64_t x = 0; x < L; x += NC) {
+                lo.push_back(off + x);
+                hi.push_back(off + std::min(L, x + NC));
+                end.push_back(off + L);
+            }
+            chunkOff[k + 1] = (int64_t)lo.size();
+            off += L;
+        }
+    }
+    const int64_t nc = (int64_t)lo.size();
+    const int64_t nl = n_max + 1;
+    const int64_t lagStep = std::min<int64_t>(nl, std::max<int64_t>(ACF_RL, ACF_PART_BUDGET / nc / ACF_RL * ACF_RL));
+    CallBuffers buf("acf");
+    int64_t *d_lo, *d_hi, *d_end, *d_chunkOff;
+    double *d_totA, *d_totB, *d_mu, *d_num0, *d_s2, *d_C, *d_partial;
+    int8_t* d_neg;
+    MBAR_TRY(buf.alloc(&d_lo, (size_t)nc));
+    MBAR_TRY(buf.alloc(&d_hi, (size_t)nc));
+    MBAR_TRY(buf.alloc(&d_end, (size_t)nc));
+    MBAR_TRY(buf.alloc(&d_chunkOff, (size_t)K + 1));
+    MBAR_TRY(buf.alloc(&d_totA, (size_t)nc));
+    MBAR_TRY(buf.alloc(&d_totB, (size_t)nc));
+    MBAR_TRY(buf.alloc(&d_mu, 2));
+    MBAR_TRY(buf.alloc(&d_num0, 1));
+    MBAR_TRY(buf.alloc(&d_s2, 1));
+    MBAR_TRY(buf.alloc(&d_C, (size_t)nl));
+    MBAR_TRY(buf.alloc(&d_neg, (size_t)nl));
+    MBAR_TRY(buf.alloc(&d_partial, (size_t)(nc * lagStep)));
+    MBAR_CUDA(cudaMemcpyAsync(d_lo, lo.data(), (size_t)nc * sizeof(int64_t), cudaMemcpyHostToDevice, o->stream));
+    MBAR_CUDA(cudaMemcpyAsync(d_hi, hi.data(), (size_t)nc * sizeof(int64_t), cudaMemcpyHostToDevice, o->stream));
+    MBAR_CUDA(cudaMemcpyAsync(d_end, end.data(), (size_t)nc * sizeof(int64_t), cudaMemcpyHostToDevice, o->stream));
+    MBAR_CUDA(cudaMemcpyAsync(d_chunkOff, chunkOff.data(), (size_t)(K + 1) * sizeof(int64_t), cudaMemcpyHostToDevice,
+                              o->stream));
+    MBAR_CUDA(cudaMemsetAsync(d_C, 0xff, (size_t)nl * sizeof(double), o->stream));
+    // lags [t0, t1) in launches whose partials fit the budget; out / neg indexed from t0
+    auto evalLags = [&](int64_t t0, int64_t t1, const double* s2, double* out, int8_t* neg) -> int {
+        for (int64_t x = t0; x < t1; x += lagStep) {
+            const int n = (int)std::min(lagStep, t1 - x);
+            AcfSegParams p{};
+            p.a = o->d_a;
+            p.b = o->d_b;
+            p.lo = d_lo;
+            p.hi = d_hi;
+            p.end = d_end;
+            p.mu = d_mu;
+            p.partial = d_partial;
+            p.l0 = x;
+            p.nLags = n;
+            p.LG = (n + ACF_RL - 1) / ACF_RL;
+            const dim3 grid((unsigned)nc, (unsigned)((p.LG + ACF_THREADS - 1) / ACF_THREADS));
+            acf_seg_partial_kernel<<<grid, ACF_THREADS, 0, o->stream>>>(p);
+            acf_seg_combine_kernel<<<(unsigned)((n + 127) / 128), 128, 0, o->stream>>>(
+                d_partial, d_chunkOff, o->d_segLen, K, x, n, s2, out + (x - t0), neg ? neg + (x - t0) : nullptr);
+            MBAR_CUDA(cudaGetLastError());
+        }
+        return MBAR_B200_OK;
+    };
+    MBAR_CUDA(cudaEventRecord(o->ev0, o->stream));
+    acf_seg_total_kernel<<<(unsigned)((nc + 127) / 128), 128, 0, o->stream>>>(o->d_a, o->d_b, d_lo, d_hi, nc, d_totA,
+                                                                            d_totB);
+    acf_seg_mean_kernel<<<1, 32, 0, o->stream>>>(d_totA, d_totB, d_chunkOff, K, o->T, d_mu);
+    MBAR_CUDA(cudaGetLastError());
+    MBAR_TRY(evalLags(0, 1, nullptr, d_num0, nullptr));
+    acf_seg_sigma_kernel<<<1, 32, 0, o->stream>>>(d_num0, o->T, d_s2);
+    MBAR_CUDA(cudaGetLastError());
+    double s2 = 0.0;
+    MBAR_CUDA(cudaMemcpyAsync(&s2, d_s2, sizeof(double), cudaMemcpyDeviceToHost, o->stream));
+    MBAR_CUDA(cudaStreamSynchronize(o->stream));
+    MBAR_REQUIRE(s2 != 0.0, MBAR_B200_ERR_INVALID, "acf_correlation_multiple: sigma^2 = 0 (constant series)");
+    int64_t count = n_max, evaluated = nl;
+    int rounds = 0;
+    if (!truncate) {
+        MBAR_TRY(evalLags(0, nl, d_s2, d_C, nullptr));
+    } else {
+        // the reference stops at the first lag whose running numerator is negative: rounds of 8, 8, 16, 32, ... lags
+        std::vector<int8_t> neg;
+        int64_t t0 = 0, B = ACF_B0;
+        bool stop = false;
+        while (!stop && t0 < nl) {
+            const int64_t t1 = std::min(nl, t0 + B);
+            MBAR_TRY(evalLags(t0, t1, d_s2, d_C + t0, d_neg + t0));
+            neg.resize((size_t)(t1 - t0));
+            MBAR_CUDA(cudaMemcpyAsync(neg.data(), d_neg + t0, (size_t)(t1 - t0), cudaMemcpyDeviceToHost, o->stream));
+            MBAR_CUDA(cudaStreamSynchronize(o->stream));
+            ++rounds;
+            for (int64_t t = t0; t < t1; ++t)
+                if (neg[t - t0]) {
+                    count = t;
+                    stop = true;
+                    break;
+                }
+            evaluated = t1;
+            t0 = t1;
+            if (rounds > 1) B *= 2;
+        }
+    }
+    MBAR_CUDA(cudaEventRecord(o->ev1, o->stream));
+    MBAR_CUDA(cudaMemcpyAsync(C, d_C, (size_t)nl * sizeof(double), cudaMemcpyDeviceToHost, o->stream));
+    double mu[2];
+    MBAR_CUDA(cudaMemcpyAsync(mu, d_mu, 2 * sizeof(double), cudaMemcpyDeviceToHost, o->stream));
+    MBAR_CUDA(cudaStreamSynchronize(o->stream));
+    *n_out = count;
+    if (mean_a) *mean_a = mu[0];
+    if (mean_b) *mean_b = mu[1];
+    if (sigma2) *sigma2 = s2;
+    float e = 0.f;
+    o->lastMs = event_ms(o->ev0, o->ev1, &e) ? e : 0.0;
+    o->lastRounds = rounds;
+    // terms: every lag evaluated after sigma^2; useful: the lags the reference evaluates (through the stop lag)
+    const int64_t needed = (truncate && count < n_max) ? count + 1 : nl;
+    o->lastTerms = o->lastUseful = 0;
+    for (int64_t L : o->segLen) {
+        o->lastTerms += seg_lag_terms(L, 0, evaluated);
+        o->lastUseful += seg_lag_terms(L, 0, needed);
+    }
     return MBAR_B200_OK;
 }
 

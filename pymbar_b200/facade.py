@@ -81,8 +81,12 @@ leave the device's range contract go to the original methods.
 `pymbar_b200.timeseries`, which answers from a `DeviceAcf`.  `subsample_correlated_data`,
 `integrated_autocorrelation_time(Multiple)` and fes.py reach them through the module's globals.  fft=True, inputs
 that are not 1-D float64 or integer arrays (float32 means differ in the reference), a constant input or sigma^2 = 0 in
-`_multiple` (the reference returns NaN or runs on rounding noise) and device errors go to the original functions;
-the FFT and binary-search functions are not touched.
+`_multiple` (the reference returns NaN or runs on rounding noise) and device errors go to the original functions.
+Where the module has them, `normalized_fluctuation_correlation_function_multiple`, `statistical_inefficiency_fft`
+and `detect_equilibration_binary_search` are rebound too (`STATS["ts_correlation_multiple"]`, `["ts_fft"]`,
+`["ts_binary_search"]`); they need no statsmodels.  `statistical_inefficiency(fft=True)` still calls the original,
+which reaches the rebound `statistical_inefficiency_fft` through the module's globals.  Constant remaining series,
+unsupported input and device errors call their originals, which without statsmodels raise as before.
 
 `install_other_estimators_on` rebinds `bar`, `bar_zero`, `exp` and `exp_gauss` of `pymbar.other_estimators` to
 `pymbar_b200.other_estimators`, which answers from a `DeviceWork`; `install()` rebinds the same names on the `pymbar`
@@ -105,7 +109,8 @@ _SAVED = {}
 STATS = {"tickets": 0, "redeemed": 0, "moments": 0, "expectations": 0, "expectations_fallbacks": 0, "log_weights": 0,
          "fes_histograms": 0, "fes_theta": 0, "fes_w_kn": 0, "fes_kde_fits": 0, "fes_kde_queries": 0,
          "fes_spline_moments": 0, "fes_spline_calls": 0, "ts_inefficiency": 0, "ts_multiple": 0, "ts_correlation": 0,
-         "ts_equilibration": 0, "ts_fallbacks": 0, "oe_bar": 0, "oe_bar_zero": 0, "oe_exp": 0, "oe_exp_gauss": 0,
+         "ts_equilibration": 0, "ts_fft": 0, "ts_binary_search": 0, "ts_correlation_multiple": 0, "ts_fallbacks": 0,
+         "oe_bar": 0, "oe_bar_zero": 0, "oe_exp": 0, "oe_exp_gauss": 0,
          "oe_evaluations": 0, "oe_fallbacks": 0, "fes_boot_solves": 0, "fes_boot_passes": 0, "fes_boot_fallbacks": 0,
          "fes_boot_spline_solves": 0, "fes_boot_spline_sums": 0, "mbar_boot_solves": 0, "mbar_boot_fallbacks": 0,
          "expectations_boot": 0, "boot_rints_built": 0}
@@ -993,10 +998,12 @@ def install_timeseries_on(module):
     if module in _SAVED:
         return
     names = ("statistical_inefficiency", "statistical_inefficiency_multiple",
-             "normalized_fluctuation_correlation_function", "detect_equilibration")
+             "normalized_fluctuation_correlation_function", "detect_equilibration",
+             "normalized_fluctuation_correlation_function_multiple", "statistical_inefficiency_fft",
+             "detect_equilibration_binary_search")
     saved = {name: module.__dict__.get(name) for name in names}
     _SAVED[module] = saved
-    orig_si, orig_multi, orig_corr, orig_eq = (saved[n] for n in names)
+    orig_si, orig_multi, orig_corr, orig_eq, orig_corr_multi, orig_fft, orig_bs = (saved[n] for n in names)
 
     def _fallback(fn, *args, **kwargs):
         STATS["ts_fallbacks"] += 1
@@ -1064,8 +1071,50 @@ def install_timeseries_on(module):
         STATS["ts_equilibration"] += 1
         return out
 
+    # the three below: ts raises NotOnDevice where the reference's answer is not reproducible (constant remaining
+    # series, unsupported input); the original then answers, or raises as it does without statsmodels
+    def normalized_fluctuation_correlation_function_multiple(A_kn, B_kn=None, N_max=None, norm=True,
+                                                             truncate=False):
+        args = (A_kn, B_kn, N_max, norm, truncate)
+        from . import _lib
+        from . import timeseries as ts
+
+        try:
+            C = ts.normalized_fluctuation_correlation_function_multiple(A_kn, B_kn, N_max=N_max, norm=norm,
+                                                                        truncate=truncate)
+        except (_lib.MbarB200Error, ts.NotOnDevice):
+            return _fallback(orig_corr_multi, *args)
+        STATS["ts_correlation_multiple"] += 1
+        return C
+
+    def statistical_inefficiency_fft(A_n, mintime=3):
+        args = (A_n, mintime)
+        from . import _lib
+        from . import timeseries as ts
+
+        try:
+            g = ts.statistical_inefficiency_fft(A_n, mintime=mintime)
+        except (_lib.MbarB200Error, ts.NotOnDevice):
+            return _fallback(orig_fft, *args)
+        STATS["ts_fft"] += 1
+        return g
+
+    def detect_equilibration_binary_search(A_t, bs_nodes=10):
+        args = (A_t, bs_nodes)
+        from . import _lib
+        from . import timeseries as ts
+
+        try:
+            out = ts.detect_equilibration_binary_search(A_t, bs_nodes=bs_nodes)
+        except (_lib.MbarB200Error, ts.NotOnDevice):
+            return _fallback(orig_bs, *args)
+        STATS["ts_binary_search"] += 1
+        return out
+
     for name, fn in zip(names, (statistical_inefficiency, statistical_inefficiency_multiple,
-                                normalized_fluctuation_correlation_function, detect_equilibration)):
+                                normalized_fluctuation_correlation_function, detect_equilibration,
+                                normalized_fluctuation_correlation_function_multiple, statistical_inefficiency_fft,
+                                detect_equilibration_binary_search)):
         if saved[name] is not None:
             fn.__doc__ = saved[name].__doc__
             setattr(module, name, fn)

@@ -561,8 +561,9 @@ class DeviceAcf(_Resident):
     resident on one H100 for the centred lag sums of pymbar.timeseries (mbar_b200_acf_*).  Independent of any
     DeviceProblem.
 
-    `inefficiency(starts, fast, mintime)` runs the reference's statistical-inefficiency loop for every start at once;
-    `correlation(start, n_max)` returns C(t), t = 0 .. n_max."""
+    `inefficiency(starts, fast, mintime)` runs the reference's statistical-inefficiency loop for every start at once
+    (rule="fft": statistical_inefficiency_fft's); `correlation(start, n_max)` returns C(t), t = 0 .. n_max, and
+    `correlation_multiple(n_max, truncate)` the multiple-series correlation function of a segmented object."""
 
     _destroy = "mbar_b200_acf_destroy"
 
@@ -585,11 +586,16 @@ class DeviceAcf(_Resident):
             self.device, self.T, _dptr(a), None if b is None else _dptr(b), 0 if offsets is None else len(offsets) - 1,
             None if offsets is None else _i64p(offsets), C.byref(self._h)))
 
-    def inefficiency(self, starts, fast=False, mintime=3, multiple=False, navg=0.0, trace_cap=0):
+    def inefficiency(self, starts, fast=False, mintime=3, multiple=False, navg=0.0, trace_cap=0, rule=None):
         """dict of per-start arrays: mean_a, mean_b, sigma2, g (before the g >= 1 clamp), last_lag, status
         (1: sigma^2 == 0) and, with trace_cap > 0, trace [n, trace_cap] (C at the first lag indices, NaN after the
         last).  multiple=True: statistical_inefficiency_multiple's loop (start 0 of a segmented object, navg the
-        mean series length)."""
+        mean series length).  rule="fft": statistical_inefficiency_fft's loop (an autocorrelation, fast=False)."""
+        if rule not in (None, "fft"):
+            raise ValueError(f"unknown rule {rule!r}")
+        if rule == "fft" and multiple:
+            raise ValueError("rule='fft' and multiple=True exclude each other")
+        code = 2 if rule == "fft" else (1 if multiple else 0)
         s = np.ascontiguousarray(np.atleast_1d(starts), dtype=np.int64)
         n = s.shape[0]
         out = {k: np.empty(n) for k in ("mean_a", "mean_b", "sigma2", "g")}
@@ -597,7 +603,7 @@ class DeviceAcf(_Resident):
         out["status"] = np.empty(n, np.int32)
         trace = np.empty((n, int(trace_cap))) if trace_cap > 0 else None
         check(self._lib.mbar_b200_acf_inefficiency(
-            self._h, n, _i64p(s), int(bool(fast)), int(mintime), 1 if multiple else 0, float(navg), int(trace_cap),
+            self._h, n, _i64p(s), int(bool(fast)), int(mintime), code, float(navg), int(trace_cap),
             _dptr(out["mean_a"]), _dptr(out["mean_b"]), _dptr(out["sigma2"]), _dptr(out["g"]), _i64p(out["last_lag"]),
             _i32p(out["status"]), None if trace is None else _dptr(trace)))
         if trace is not None:
@@ -611,6 +617,16 @@ class DeviceAcf(_Resident):
         check(self._lib.mbar_b200_acf_correlation(self._h, int(start), int(n_max), _dptr(Cn), C.byref(ma),
                                                   C.byref(mb), C.byref(s2)))
         return Cn, ma.value, mb.value, s2.value
+
+    def correlation_multiple(self, n_max, truncate=False):
+        """(C, mean_a, mean_b, sigma2) of normalized_fluctuation_correlation_function_multiple over the object's
+        series: C holds the entries the reference returns (n_max of them, or with truncate those before the first
+        lag whose running numerator is negative)."""
+        Cn = np.empty(int(n_max) + 1)
+        count, ma, mb, s2 = C.c_int64(0), C.c_double(0), C.c_double(0), C.c_double(0)
+        check(self._lib.mbar_b200_acf_correlation_multiple(self._h, int(n_max), int(bool(truncate)), _dptr(Cn),
+                                                           C.byref(count), C.byref(ma), C.byref(mb), C.byref(s2)))
+        return Cn[:count.value].copy(), ma.value, mb.value, s2.value
 
     def last_stats(self):
         """CUDA-event time (ms) of the last call, its lag rounds, the lag terms evaluated and those the stop rule

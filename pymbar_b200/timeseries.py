@@ -13,6 +13,14 @@ mean of the repeated value is exact, and otherwise runs its loop on the rounding
 answered on the host: g = T - t + 1 when the mean is exact in any order (the value has at most 53 - ceil(log2 T)
 significant bits), else `_host_inefficiency`, the reference's loop in the reference's numpy operations.  They have
 Neff close to 1, and a long inexact constant tail costs what it costs in the reference.
+
+`normalized_fluctuation_correlation_function_multiple`, `statistical_inefficiency_fft` and
+`detect_equilibration_binary_search` (timeseries.py:509-658, :839-970) take the reference's arguments and return its
+values and types.  The FFT functions need no statsmodels: the device evaluates statsmodels' acf(adjusted=True) by
+direct lag sums up to the stop lag, which is the same C(t) in exact arithmetic and the more accurate of the two in
+fp64.  Where the reference's answer is not reproducible (a constant remaining series, whose statsmodels acf divides
+rounding noise by rounding noise, or sigma^2 = 0) or the input is not a 1-D float64 or integer array, these raise
+`NotOnDevice`, and the facade calls the original.
 """
 from __future__ import annotations
 
@@ -37,6 +45,17 @@ def _device(A, B=None, lengths=None):
 def _parameter_error(msg):
     # looked up at raise time: install() makes it pymbar's own ParameterError
     return _u.ParameterError(msg)
+
+
+class NotOnDevice(Exception):
+    """The input has no device answer that reproduces the reference's; the caller runs the reference instead."""
+
+
+def _device_series(x):
+    """x as float64 if it is a 1-D float64 or integer ndarray, else NotOnDevice."""
+    if not isinstance(x, np.ndarray) or x.ndim != 1 or not (x.dtype == np.float64 or x.dtype.kind in "iu"):
+        raise NotOnDevice("input is not a 1-D float64 or integer array")
+    return np.ascontiguousarray(x, dtype=np.float64)
 
 
 def lag(i, fast):
@@ -226,3 +245,104 @@ def detect_equilibration(A_t, fast=True, nskip=1):
     Neff_max = Neff_t.max()
     t = Neff_t.argmax()
     return t, g_t[t], Neff_max
+
+
+def normalized_fluctuation_correlation_function_multiple(A_kn, B_kn=None, N_max=None, norm=True, truncate=False):
+    """normalized_fluctuation_correlation_function_multiple (timeseries.py:509-658): C(t) over K series with pooled
+    means, in one device call; the reference's C_n[:t] (with norm=False C sigma^2 + mu_A mu_B)."""
+    cross = B_kn is not None
+    if B_kn is None:
+        B_kn = A_kn
+    if (type(A_kn) is not list) or (type(B_kn) is not list):
+        raise _parameter_error("A_kn and B_kn must each be a list of numpy arrays.")
+    if len(A_kn) != len(B_kn):
+        raise _parameter_error("A_kn and B_kn must contain corresponding timeseries -- different numbers of "
+                               "timeseries detected in each.")
+    A = [_device_series(x) for x in A_kn]
+    B = [_device_series(x) for x in B_kn] if cross else A
+    if any(x.size != y.size for x, y in zip(A, B)):
+        raise _parameter_error("A_kn and B_kn must contain corresponding timeseries -- lack of correspondence in "
+                               "timeseries lenghts detected.")
+    N_k = np.array([x.size for x in A], np.int64)
+    if N_k.size == 0 or N_k.sum() == 0:
+        raise NotOnDevice("no samples")
+    if (not N_max) or (N_max > N_k.max() - 1):
+        N_max = int(N_k.max()) - 1
+    if not isinstance(N_max, (int, np.integer)) or N_max < 0:
+        raise NotOnDevice(f"N_max = {N_max!r}")
+    keep = [k for k in range(N_k.size) if N_k[k] > 0]        # empty series add nothing to any sum
+    a = np.concatenate([A[k] for k in keep])
+    b = np.concatenate([B[k] for k in keep]) if cross else None
+    if _constant(a) or (b is not None and _constant(b)):
+        raise NotOnDevice("constant series: sigma^2 is 0 or rounding noise")
+    with _device(a, b, lengths=N_k[keep]) as dev:
+        C, mu_a, mu_b, s2 = dev.correlation_multiple(int(N_max), truncate=bool(truncate))
+    return C if norm else C * s2 + mu_a * mu_b
+
+
+def _fft_g(dev, starts, mintime):
+    """g before the clamp of statistical_inefficiency_fft for each start of the device series."""
+    mintime = min(max(int(mintime), -1), 2 ** 31 - 1)          # t >= 1: every mintime < 0 acts as -1
+    r = dev.inefficiency(starts, mintime=mintime, rule="fft")
+    if np.any(r["status"] != 0):
+        raise NotOnDevice("sigma^2 = 0")
+    return r["g"]
+
+
+def statistical_inefficiency_fft(A_n, mintime=3):
+    """statistical_inefficiency_fft (timeseries.py:839-898) without statsmodels: max(1.0, g)."""
+    a = _device_series(np.array(A_n))
+    if a.size < 2 or _constant(a):
+        raise NotOnDevice("fewer than 2 samples or a constant series")
+    if isinstance(mintime, bool) or not isinstance(mintime, (int, np.integer)):
+        raise NotOnDevice(f"mintime = {mintime!r}")
+    with _device(a) as dev:
+        g = np.float64(_fft_g(dev, [0], mintime)[0])
+    return max(1.0, g)
+
+
+def detect_equilibration_binary_search(A_t, bs_nodes=10):
+    """detect_equilibration_binary_search (timeseries.py:901-970): the reference's grid and window updates on the
+    host, each round's starts in one device call; (t, g, Neff_max) as np.int64, np.float64, np.float64."""
+    assert bs_nodes > 4, "Number of nodes for binary search must be > 4"
+    a = _device_series(A_t)
+    T = A_t.size
+    if T < 2:
+        raise NotOnDevice("fewer than 2 samples")
+    if A_t.std() == 0.0:
+        return 0, 1, T
+    if _constant(a):                 # numpy's std of a constant series is rounding noise when its mean is inexact
+        raise NotOnDevice("constant series")
+    tail = int(np.flatnonzero(a != a[-1])[-1]) + 1               # A[t:] is constant for t >= tail
+    start = 1
+    end = T - 1
+    n_grid = min(bs_nodes, T)
+    with _device(a) as dev:
+        while True:
+            time_grid = np.unique((10 ** np.linspace(np.log10(start), np.log10(end), n_grid)).round().astype("int"))
+            g_t = np.ones(time_grid.size)
+            Neff_t = np.ones(time_grid.size)
+            on = time_grid < T - 1
+            if on.any():
+                s = time_grid[on]
+                if s.max() >= tail:
+                    raise NotOnDevice("constant remaining series")
+                g = _fft_g(dev, s, 3)
+                g_t[on] = np.where(g > 1.0, g, 1.0)
+                Neff_t[on] = (T - s + 1) / g_t[on]
+            Neff_max = Neff_t.max()
+            k = Neff_t.argmax()
+            t = time_grid[k]
+            g = g_t[k]
+            if end - start < 4:
+                break
+            if k == 0:
+                start = time_grid[0]
+                end = time_grid[1]
+            elif k == time_grid.size - 1:
+                start = time_grid[-2]
+                end = time_grid[-1]
+            else:
+                start = time_grid[k - 1]
+                end = time_grid[k + 1]
+    return t, g, Neff_max
