@@ -40,7 +40,9 @@ constexpr uint32_t FUSED_COPY_CHUNK = 32768;
 
 __host__ __device__ inline size_t fused_smem_header(int K, int CL, int M = 1) {
     // tab[32] | c_s[M][K + 32] | xD[2][M][slots][32] | sred[M][256] | sumL[M][16] | bad[M][32] | full[8] | empty[8]
-    // (c_s carries 32 spare entries: the masked variants fetch constants of up to 31 rows they do not own;
+    // (c_s carries 32 spare entries.  A masked CTA zeroes c_s[Kl, max(Kl + 32, (Wk - 1) Rw + R)): it reads the
+    //  constants of all R register rows of every warp.  Wk Rw < Kh + 2 Wk and R < Rw + 8 keep the highest read
+    //  below Kh + 24, which is K + 24 for CL = 1 and at most K / 2 + 26 for CL > 1: K + 32 entries hold it.
     //  M = 2: a second candidate f-vector is evaluated on the same staged tiles)
     size_t b = 256 + (size_t)M * (((size_t)K + 32) * 8 + 2 * (size_t)fused_slots(CL) * 32 * 8 + 256 * 8 + 128 + 128) +
                64 + 64;
@@ -231,11 +233,17 @@ __global__ void __launch_bounds__(CW * 32, 1) pass_fused_kernel(const FusedParam
     // state constants: c_k, or E_k = exp(c_k) when the constant is applied multiplicatively
     for (int k = threadIdx.x; k < Kl; k += blockDim.x)
         c_s[k] = (MODE & 2) ? exp(p.c[kbase + k]) : p.c[kbase + k];
-    // masked variants read up to 31 state constants past this CTA's rows: keep those entries finite
+    // keep the constants past this CTA's rows finite (a stale inf or NaN would turn D += E_k * 0 into NaN): the
+    // masked variants read all R register rows of every warp, owned or not, up to c_s[(Wk - 1) * Rw + R - 1], which
+    // for the last CTA of a cluster (Kl < Kh) can lie past Kl + 31.  The FULL variants read their own rows only.
     for (int i = threadIdx.x; i < 32; i += blockDim.x) c_s[Kl + i] = 0.0;
+    if constexpr (!FULL)
+        for (int i = Kl + 32 + threadIdx.x; i < (p.Wk - 1) * p.Rw + R; i += blockDim.x) c_s[i] = 0.0;
     if constexpr (M == 2) {
         for (int k = threadIdx.x; k < Kl; k += blockDim.x) c_s2[k] = exp(p.c2[kbase + k]);
         for (int i = threadIdx.x; i < 32; i += blockDim.x) c_s2[Kl + i] = 0.0;
+        if constexpr (!FULL)
+            for (int i = Kl + 32 + threadIdx.x; i < (p.Wk - 1) * p.Rw + R; i += blockDim.x) c_s2[i] = 0.0;
     }
     for (int i = threadIdx.x; i < 2 * M * SLOTS * 32; i += blockDim.x) xD[i] = 0.0;
     // lane-replicated exp table, 8 KB aligned so that its address bits never overlap the index bits

@@ -139,12 +139,15 @@ def exp_rel(a):
 
 
 def reduction_depth(plan):
-    """Additions a summand of S_k passes through: 32 samples of a tile summed by one lane, the tiles of a warp, the W
-    warps of a CTA, then the CTAs in index order.  Sequential sums of positive terms: relative error <= depth eps."""
+    """Additions a summand of S_k passes through: the plan's own `depth` where it states one (tests/_fused.py), else
+    the generic pass's: 32 samples of a tile summed by one lane, the tiles of a warp, the W warps of a CTA, then the
+    CTAs in index order.  Sequential sums of positive terms: relative error <= depth eps."""
+    if "depth" in plan:
+        return plan["depth"]
     return 32 + plan["tiles_per_warp"] + plan["W"] + plan["grid"]
 
 
-def sparse_moments_ld(u, N_k, f, mult=None, all_rows=False, cut=CUT, want_G=False, chunk=None):
+def sparse_moments_ld(u, N_k, f, mult=None, all_rows=False, cut=CUT, want_G=False, chunk=None, c_abs=None):
     """The pass and the second moments in long double from the dense u [K, N], column chunk by column chunk, keeping
     the entries within `cut` of each sample's largest exponent.
 
@@ -153,7 +156,9 @@ def sparse_moments_ld(u, N_k, f, mult=None, all_rows=False, cut=CUT, want_G=Fals
     drop (bound on the dropped part of any N_k S_k or Ghat_ij), and the error budget of the device's pass:
     dL [N] (absolute, of L_n), eS [K] (sum_n m_n W_nk e_kn / S_k, the first-order relative error of S_k from its
     entries) and eLogW [K] (the same for the log-domain rows).  With want_G: Gi, Gj, Gv, the support of Ghat
-    (i >= j) in long double."""
+    (i >= j) in long double.  `c_abs` [K]: the magnitude of the state constant the device puts into each row's exp
+    arguments where it is not |f_k + log N_k| (the fused pass centres the constants on a midpoint and gives unsampled
+    rows log N = -80 in an all-state pass); the error budget then rounds on the larger of the two."""
     u = np.asarray(u, np.float64)
     K, N = u.shape
     N_k = np.asarray(N_k, np.float64)
@@ -163,6 +168,7 @@ def sparse_moments_ld(u, N_k, f, mult=None, all_rows=False, cut=CUT, want_G=Fals
     logN[s] = np.log(N_k[s].astype(LD))
     c = fL + logN                                   # unsampled rows: c = f (log N = 0)
     c64 = c.astype(np.float64)
+    cab = np.abs(c64) if c_abs is None else np.maximum(np.abs(c64), np.asarray(c_abs, np.float64))
     m = np.ones(N) if mult is None else np.asarray(mult, np.float64)
     rows = np.ones(K, bool) if all_rows else s
     chunk = chunk or max(32, (1 << 23) // K)
@@ -198,7 +204,7 @@ def sparse_moments_ld(u, N_k, f, mult=None, all_rows=False, cut=CUT, want_G=Fals
             up = np.abs(uc[kk, nn] - x[nn])
             mprime = np.abs(top + x)
             Lp = np.abs(L.astype(np.float64) + x)
-            term = ARG_ROUND * (np.abs(c64[kk]) + up + mprime[nn]) + exp_rel(aL.astype(np.float64) - top[nn])
+            term = ARG_ROUND * (cab[kk] + up + mprime[nn]) + exp_rel(aL.astype(np.float64) - top[nn])
             wD = np.exp((aL - top[nn].astype(LD)).astype(np.float64))
             num = np.zeros(n1 - n0)
             np.add.at(num, nn[sk], (wD * term)[sk])
@@ -212,7 +218,7 @@ def sparse_moments_ld(u, N_k, f, mult=None, all_rows=False, cut=CUT, want_G=Fals
             # (a weight of multiplicity 0 may lie far above its row's live ones: it must not overflow into 0 * inf)
             Wk = np.where(mm > 0, np.exp(np.where(mm > 0, fL[kk] - uc[kk, nn].astype(LD) - L[nn] - shift[kk], 0)), 0)
             np.add.at(out["S"], kk, mm * Wk)
-            e = dL[nn] + ARG_ROUND * (np.abs(c64[kk]) + up + Lp[nn]) + exp_rel(arg.astype(np.float64)) + 2 * EPS
+            e = dL[nn] + ARG_ROUND * (cab[kk] + up + Lp[nn]) + exp_rel(arg.astype(np.float64)) + 2 * EPS
             np.add.at(out["eS"], kk, mm * Wk * e.astype(LD))
             elog = e + EPS * np.abs(np.log(np.where(mc[nn] > 0, mc[nn], 1.0)))
             np.add.at(out["eLogW"], kk, mm * Wk * elog.astype(LD))
@@ -225,15 +231,18 @@ def sparse_moments_ld(u, N_k, f, mult=None, all_rows=False, cut=CUT, want_G=Fals
                 k2, n2, w2 = kk[keep], nn[keep], np.exp(arg[keep]) * np.sqrt(mm[keep])
                 order = np.argsort(n2, kind="stable")
                 k2, n2, w2 = k2[order], n2[order], w2[order]
-                starts = np.flatnonzero(np.r_[True, n2[1:] != n2[:-1]])
-                ends = np.r_[starts[1:], n2.size]
-                for a, b in zip(starts, ends):
-                    ki, wi = k2[a:b], w2[a:b]
-                    I, J = np.meshgrid(np.arange(b - a), np.arange(b - a), indexing="ij")
-                    low = ki[I] >= ki[J]
-                    Gi.append(ki[I][low])
-                    Gj.append(ki[J][low])
-                    Gv.append((wi[I] * wi[J])[low])
+                # every pair of kept entries of one sample: the entries of a sample are contiguous after the sort,
+                # so the pairs lie d = 0, 1, ... positions apart (d = 0: the diagonal)
+                d = 0
+                while d < n2.size:
+                    a = np.flatnonzero(n2[:n2.size - d] == n2[d:])
+                    if a.size == 0:
+                        break
+                    ka, kb = k2[a], k2[a + d]
+                    Gi.append(np.maximum(ka, kb))
+                    Gj.append(np.minimum(ka, kb))
+                    Gv.append(w2[a] * w2[a + d])
+                    d += 1
     out["sumL"] = (m.astype(LD) * out["L"]).sum()
     with np.errstate(divide="ignore", invalid="ignore"):
         Ssh = out["S"]
@@ -252,9 +261,11 @@ def sparse_moments_ld(u, N_k, f, mult=None, all_rows=False, cut=CUT, want_G=Fals
     return out
 
 
-def pass_tolerances(ref, N_k, plan, mult=None):
+def pass_tolerances(ref, N_k, plan, mult=None, floor=None):
     """Absolute tolerances of S (sampled rows, linear sums), of log S (log-domain rows, every row) and of L_n.
-    Either form may answer a sampled row (log-domain after an underflow), so tolS covers both."""
+    Either form may answer a sampled row (log-domain after an underflow), so tolS covers both.  `floor` [K] replaces
+    the absolute term of weights on the exp floor, N max(m) 2^-1020 / N_k, where a pass divides floored entries by
+    a denominator (the fused pass: per row sum_n m_n 2^-1020 max(1, e^(c_k - mid)) / (D_n N_k))."""
     N_k = np.asarray(N_k, np.float64)
     s = N_k > 0
     h = reduction_depth(plan)
@@ -262,12 +273,14 @@ def pass_tolerances(ref, N_k, plan, mult=None):
     S = ref["S"].astype(np.float64)
     M_ = float(plan["N"] if mult is None else np.sum(mult))
     mmax = 1.0 if mult is None else float(np.max(mult))
-    floor_abs = plan["N"] * mmax * M.FLOOR / Nd
+    floor_abs = plan["N"] * mmax * M.FLOOR / Nd if floor is None else np.asarray(floor, np.float64)
     with np.errstate(divide="ignore", invalid="ignore"):
         rel_lin = ref["eS"].astype(np.float64) + (h + 2) * EPS
         # log-domain rows: per-lane (max, sum) over 32 samples, merged over tiles, warps and CTAs
         tol_log = (ref["eLogW"].astype(np.float64) + (h + 2) * EPS + 4 * LOG_MERGE
                    + 2 * EPS * np.abs(ref["logS"].astype(np.float64)) + plan["N"] * mmax * float(np.exp(-LD(CUT))))
+        if floor is not None:           # linear sums of every row (the fused all-state pass): the floor, relative
+            tol_log = tol_log + np.where(S > 0, floor * Nd / np.where(S > 0, S * Nd, 1.0), 0.0)
         # a row whose every kept weight has multiplicity 0 sums to exactly 0 on both sides
         tolS = np.where(s, np.where(S > 0, np.maximum(S * rel_lin, S * np.expm1(np.minimum(tol_log, 1.0))), 0.0)
                         + floor_abs + float(ref["drop"]) / Nd, 0.0)
@@ -275,12 +288,16 @@ def pass_tolerances(ref, N_k, plan, mult=None):
     return dict(S=tolS, logS=tol_log, L=tolL, M=M_)
 
 
-def sumL_tolerance(ref, plan, mult=None):
-    """sum_n m_n L'_n (warp butterfly, the tiles of a thread, warps, CTAs) less sum_n m_n x_n (host, N terms)."""
+def sumL_tolerance(ref, plan, mult=None, mid=0.0):
+    """sum_n m_n L'_n (warp butterfly, the tiles of a thread, warps, CTAs) less sum_n m_n x_n (host, N terms).  A
+    plan may state its own `sumL_depth`; one with `logprod` sums log(D_n) = L'_n - mid as a product of mantissas
+    (one rounding per sample, absolute in the log) and adds sum_n m_n mid at the end."""
     m = np.ones(plan["N"]) if mult is None else np.asarray(mult, np.float64)
-    Lp = np.abs(ref["L"].astype(np.float64) + ref["x"])
-    depth = 5 + plan["tiles_per_warp"] + plan["W"] + plan["grid"] + 2
-    return float(np.sum(m * ref["dL"]) + depth * EPS * np.sum(m * Lp) + plan["N"] * EPS * np.sum(m * np.abs(ref["x"])))
+    Lp = np.abs(ref["L"].astype(np.float64) + ref["x"]) + abs(mid)
+    depth = plan.get("sumL_depth", 5 + plan.get("tiles_per_warp", 0) + plan.get("W", 0) + plan["grid"] + 2)
+    prod = 2 * EPS * float(np.sum(m)) if plan.get("logprod") else 0.0
+    return float(np.sum(m * ref["dL"]) + depth * EPS * np.sum(m * Lp) + plan["N"] * EPS * np.sum(m * np.abs(ref["x"]))
+                 + prod)
 
 
 def dense_G(ref, K):
