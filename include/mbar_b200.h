@@ -395,6 +395,38 @@ int mbar_b200_work_evaluate(mbar_b200_work* work, int32_t n_requests, const int3
 /* CUDA-event time of the kernels of the last mbar_b200_work_evaluate, its launches and the work values it read. */
 int mbar_b200_last_work_stats(mbar_b200_work* work, double* ms, int32_t* launches, int64_t* values_read);
 
+/* ---- many small MBAR problems in lockstep (pymbar_b200.mbar_many; DESIGN.md 3.5g) ------------------------------ */
+/* P problems, problem p with K_p (1 to 64) states and N_p >= 1 samples: u concatenates each problem's row-major
+ * u_kn [K_p][N_p], N_k concatenates each problem's N_k [K_p] (at least one positive entry each).  One H2D copy, then
+ * every problem is shifted per sample and tiled on the device.  NaN or -inf energies -> MBAR_B200_ERR_NAN; a bad
+ * shape or N_k -> MBAR_B200_ERR_INVALID; a batch that does not fit in device memory -> MBAR_B200_ERR_NOMEM (the
+ * message gives the allocation in bytes). */
+typedef struct mbar_b200_batch mbar_b200_batch;
+int mbar_b200_batch_create(int device, int32_t n_problems, const int32_t* K, const int64_t* N, const double* N_k,
+                           const double* u, mbar_b200_batch** out);
+int mbar_b200_batch_destroy(mbar_b200_batch* batch);
+/* For each request r (problem[r], f: the concatenation of the requests' f [K_p]): S_k = sum_n e^{f_k - u_kn - L_n},
+ * log S_k, sum_n L_n with L_n = log sum_{j sampled} N_j e^{f_j - u_jn}, a flag and, when G is not NULL, the Gram
+ * Ghat_ij = sum_n w_in w_jn with w_kn = N_k W_nk on sampled rows and W_nk on unsampled rows if all_rows (0
+ * otherwise).  S and log S cover the sampled rows, and all rows if all_rows.  flag[r] = 1: a NaN reached the sums,
+ * a sampled S_k lies outside (1e-280, 1e300), or (all_rows) an unsampled S_k is NaN or overflows.  Outputs are
+ * concatenated by request (G: K_p x K_p each, row-major).  Two kernel launches and one synchronisation; a request's
+ * results are the same bits whichever requests share the call. */
+int mbar_b200_batch_moments(mbar_b200_batch* batch, int32_t n_requests, const int32_t* problem, const double* f,
+                            int32_t all_rows, double* S, double* log_S, double* sum_L, int32_t* flag, double* G);
+/* The adaptive solver of mbar_b200_solve_adaptive's host-stepped loop (same step, Newton retries, step choice and
+ * convergence rule) for every problem at once, one moments call (both candidates of every unfinished problem) per
+ * iteration.  f [sum K_p] in/out: the sampled states of each problem, gauge f[first sampled] = 0; unsampled states
+ * are left untouched.  status[p]: 0 converged (or nothing to solve), 1 maxiter reached, 2 the batched sums could
+ * not represent an iterate (flag set or a non-finite candidate; f is then the last good iterate).  iterations[p]:
+ * the iterations problem p took.  A sampled |f_k| >= 5e5 -> MBAR_B200_ERR_RANGE. */
+int mbar_b200_batch_solve(mbar_b200_batch* batch, double* f_inout, double tol, int32_t maxiter, int32_t min_sc_iter,
+                          double gamma, int32_t* status, int32_t* iterations);
+/* CUDA-event time of the kernels of the last batch_moments or batch_solve call, its kernel launches, its iterations
+ * (solve) and the bytes of u_kn tiles its passes read. */
+int mbar_b200_last_batch_stats(mbar_b200_batch* batch, double* kernel_ms, int32_t* launches, int32_t* iterations,
+                               int64_t* bytes_read);
+
 /* ---- native solver loops (no Python between iterations) ------------------------------------- */
 /* Plain self-consistent iteration f <- f - log S(f), gauge f[first sampled] = 0 each step, until
  * max |delta f / f| < tol (the convergence rule of mbar_solvers.py:627-640) or maxiter. */

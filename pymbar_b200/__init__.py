@@ -9,15 +9,18 @@ Public surface:
     (:mod:`pymbar_b200.timeseries`);
   * :class:`pymbar_b200.DeviceWork` — work vectors resident for the sums of ``pymbar.other_estimators`` (BAR, EXP,
     Gaussian EXP; :mod:`pymbar_b200.other_estimators`, including ``bar_many`` for many pairs in lockstep);
+  * :class:`pymbar_b200.DeviceMbarBatch` — many small MBAR problems (up to 64 states each) resident together;
+    :func:`pymbar_b200.mbar_many.mbar_many` solves all of them in lockstep, one device call per iteration, and
+    returns each problem's free energies and uncertainties;
   * :func:`pymbar_b200.install` — rebind ``pymbar.mbar_solvers`` so unmodified ``pymbar.MBAR`` uses it.
 
 Everything numerical runs in libmbar_b200.so (C ABI in include/mbar_b200.h).  No CPU fallback.
 """
 from . import _lib
-from .problem import DeviceAcf, DeviceBSpline, DeviceKde, DeviceProblem, DeviceWork, PinnedArray
+from .problem import DeviceAcf, DeviceBSpline, DeviceKde, DeviceMbarBatch, DeviceProblem, DeviceWork, PinnedArray
 from .utils import ParameterError
 
-__all__ = ["DeviceProblem", "DeviceKde", "DeviceBSpline", "DeviceAcf", "DeviceWork", "PinnedArray", "ParameterError", "install", "uninstall", "trim", "mbar_solvers"]
+__all__ = ["DeviceProblem", "DeviceKde", "DeviceBSpline", "DeviceAcf", "DeviceWork", "DeviceMbarBatch", "PinnedArray", "ParameterError", "install", "uninstall", "trim", "mbar_solvers"]
 
 _SAVED = {}
 _PATCHED = (

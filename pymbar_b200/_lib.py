@@ -102,6 +102,15 @@ SIGNATURES = {
     "mbar_b200_work_evaluate": (C.c_int, [_ctx, C.c_int32, C.POINTER(C.c_int32), C.POINTER(C.c_int32), _dp, _dp,
                                           _dp]),
     "mbar_b200_last_work_stats": (C.c_int, [_ctx, _dp, C.POINTER(C.c_int32), C.POINTER(C.c_int64)]),
+    "mbar_b200_batch_create": (C.c_int, [C.c_int, C.c_int32, C.POINTER(C.c_int32), C.POINTER(C.c_int64), _dp, _dp,
+                                         C.POINTER(_ctx)]),
+    "mbar_b200_batch_destroy": (C.c_int, [_ctx]),
+    "mbar_b200_batch_moments": (C.c_int, [_ctx, C.c_int32, C.POINTER(C.c_int32), _dp, C.c_int32, _dp, _dp, _dp,
+                                          C.POINTER(C.c_int32), _dp]),
+    "mbar_b200_batch_solve": (C.c_int, [_ctx, _dp, C.c_double, C.c_int32, C.c_int32, C.c_double, C.POINTER(C.c_int32),
+                                        C.POINTER(C.c_int32)]),
+    "mbar_b200_last_batch_stats": (C.c_int, [_ctx, _dp, C.POINTER(C.c_int32), C.POINTER(C.c_int32),
+                                             C.POINTER(C.c_int64)]),
     "mbar_b200_solve_sci":(C.c_int, [_ctx, _dp, C.c_double, C.c_int32, C.POINTER(SolveResult)]),
     "mbar_b200_solve_adaptive": (C.c_int, [_ctx, _dp, C.c_double, C.c_int32, C.c_int32, C.c_double,
                                            C.POINTER(SolveResult)]),

@@ -7,7 +7,7 @@ import sys
 HERE = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(HERE, "csrc")
 LIB = os.path.join(HERE, "libmbar_b200.so")
-SOURCES = ["ctx.cu", "pass_generic.cu", "pass_fused.cu", "hessian.cu", "logw.cu", "bins.cu", "replicates.cu", "kde.cu", "bspline.cu", "acf.cu", "work.cu", "api.cu", "loops.cu", "ubench.cu"]
+SOURCES = ["ctx.cu", "pass_generic.cu", "pass_fused.cu", "hessian.cu", "logw.cu", "bins.cu", "replicates.cu", "kde.cu", "bspline.cu", "acf.cu", "work.cu", "batch.cu", "api.cu", "loops.cu", "ubench.cu"]
 NVCC_FLAGS = [
     "-O3", "-std=c++17", "-gencode", "arch=compute_90a,code=sm_90a", "-lineinfo",
     "-Xcompiler", "-fPIC", "-Xcompiler", "-fvisibility=hidden", "--use_fast_math=false",

@@ -1,0 +1,696 @@
+// mbar_b200_batch_*: many small MBAR problems (1 <= K_p <= 64 states each) resident on one GPU, their sums evaluated
+// in one launch for every problem and the adaptive solver stepped for all of them in lockstep (DESIGN.md 3.5g).
+//
+// Layout.  Problem p keeps its own tiles [nT_p][K_p][32] of shifted energies u'_kn = u_kn - x_n with
+// x_n = min over the sampled states of u_kn (0 when every such entry is +inf), as the single-problem upload stores
+// them (DESIGN.md 2).  Samples past N_p in the last tile hold +inf.  Per problem the device also keeps N_k, log N_k
+// and sum_n x_n.
+//
+// Moments.  A request names a problem and a vector f [K_p].  With c_k = f_k + log N_k over the sampled states,
+//   L'_n = log sum_{k sampled} e^{c_k - u'_kn}      (per-sample max shift, exact exp)
+//   a_kn = f_k - u'_kn - L'_n,   log S_k = logsumexp_n a_kn,   sum L = sum_n L'_n - sum_n x_n
+// and, on request, the Gram Ghat_ij = sum_n w_in w_jn with w_kn = N_k e^{a_kn} (sampled rows) and e^{a_kn} (unsampled
+// rows, only when all rows are asked for) — the row scaling of launch_hessian.  A sampled row has e^{a_kn} <= 1 / N_k
+// and is summed linearly, as the single-problem pass sums it: its S_k carries a relative error of a few ulp, which the
+// adaptive loop's relative-change test at tol = 1e-12 needs when f_k is near 0.  An unsampled row is kept as a running
+// (max, sum) pair, so it neither under- nor overflows inside the pass.  The finalize kernel sets the request's flag
+// where a sum is not a usable number (see batch_finalize_kernel).
+//
+// Determinism.  Work items are (request, chunk) pairs; a chunk is CT_p tiles with CT_p a function of (N_p, K_p) alone.
+// Warp w of a CTA takes the chunk's tiles w, w + 4, ... in order and folds each tile into its own (max, sum) pairs;
+// the four warps' pairs, the 128 thread sums of L' and the per-thread Gram sums are combined in a fixed order, and
+// the finalize kernel adds a request's chunk partials in chunk order.  There are no atomics: a request's sums are the
+// same bits whichever requests share the launch, and repeat calls are bit-identical.
+#include <algorithm>
+#include <cmath>
+#include <cstring>
+#include <memory>
+#include <vector>
+
+#include "internal.cuh"
+
+namespace mbar {
+
+constexpr int BATCH_MAX_K = 64;
+constexpr int BATCH_THREADS = 128;                  // four warps, one tile each per round
+constexpr int BATCH_WARPS = BATCH_THREADS / 32;
+constexpr int BATCH_ROUND = BATCH_THREADS;          // samples per round
+constexpr int BATCH_SW_LD = BATCH_ROUND + 1;        // leading dimension of the staged weights (bank spread)
+constexpr int BATCH_GSLOTS = (BATCH_MAX_K * (BATCH_MAX_K + 1) / 2 + BATCH_THREADS - 1) / BATCH_THREADS;
+constexpr int64_t BATCH_MAX_CHUNKS = 4096;
+
+// tiles per chunk: about 64k entries of u' per chunk, at most BATCH_MAX_CHUNKS chunks per problem
+__host__ __device__ __forceinline__ int64_t batch_chunk_tiles(int64_t nT, int K) {
+    const int64_t base = 2048 / K > 4 ? 2048 / K : 4;
+    const int64_t need = (nT + BATCH_MAX_CHUNKS - 1) / BATCH_MAX_CHUNKS;
+    return base > need ? base : need;
+}
+
+struct BatchReq {
+    int64_t uoff;     // first double of the problem's tiles
+    int64_t N, nT;    // samples and tiles of the problem
+    int64_t ct;       // tiles per chunk
+    int64_t item0;    // first (request, chunk) item
+    int64_t poff;     // first double of the request's chunk partials
+    int64_t ooff;     // first double of the request's packed output
+    int64_t voff;     // first entry of the problem's K-vectors (N_k, log N_k)
+    int64_t foff;     // first entry of the request's f
+    int32_t K, prob, allRows, wantG;
+};
+
+// per-request packed output: [0, K) S, [K, 2K) log S, [2K] sum L, [2K + 1] flag, then K x K Ghat when asked for
+__host__ __device__ __forceinline__ int64_t batch_out_size(int K, bool G) { return 2 * K + 2 + (G ? (int64_t)K * K : 0); }
+// per-chunk partial: K (max, sum) pairs, sum L', bad flag, then the K (K + 1) / 2 lower-triangle Gram entries
+__host__ __device__ __forceinline__ int64_t batch_part_size(int K, bool G) {
+    return 2 * K + 2 + (G ? (int64_t)K * (K + 1) / 2 : 0);
+}
+
+}  // namespace mbar
+
+struct mbar_b200_batch : mbar::Resident {
+    int P = 0;
+    std::vector<int> K;
+    std::vector<int64_t> N, nT, uoff, voff;
+    std::vector<double> Nk;                     // concatenated N_k
+    int64_t uTotal = 0;
+    mbar::DevArray<double> d_u, d_Nk, d_logNk, d_sumx;
+    // per-call buffers, grown on demand
+    mbar::DevArray<mbar::BatchReq> d_req;
+    mbar::DevArray<double> d_f, d_part, d_out;
+    double* h_f = nullptr;                      // pinned staging of f and of the packed output
+    double* h_out = nullptr;
+    size_t h_fCap = 0, h_outCap = 0;
+    // the last moments / solve call
+    int32_t lastLaunches = 0, lastIterations = 0;
+    int64_t lastBytes = 0;
+    ~mbar_b200_batch() {
+        if (h_f) cudaFreeHost(h_f);
+        if (h_out) cudaFreeHost(h_out);
+    }
+};
+
+namespace mbar {
+
+// ---- upload: raw row-major problems -> shifted tiles, x_n, sum x_n -------------------------------------------------
+struct BatchProbDev {
+    int64_t roff, uoff, tile0, N, voff;
+    int32_t K;
+};
+
+__device__ __forceinline__ int batch_find_tile(const BatchProbDev* __restrict__ pr, int P, int64_t tile) {
+    int lo = 0, hi = P - 1;
+    while (lo < hi) {
+        const int mid = (lo + hi + 1) >> 1;
+        if (pr[mid].tile0 <= tile) lo = mid;
+        else hi = mid - 1;
+    }
+    return lo;
+}
+
+// one warp per tile, one lane per sample; bad[0] counts NaN or -inf energies
+__global__ void __launch_bounds__(256) batch_retile_kernel(const double* __restrict__ raw,
+                                                           const BatchProbDev* __restrict__ pr, int P,
+                                                           int64_t nTiles, const double* __restrict__ Nk,
+                                                           double* __restrict__ u, double* __restrict__ x,
+                                                           unsigned int* bad) {
+    const int64_t tile = (int64_t)blockIdx.x * 8 + (threadIdx.x >> 5);
+    if (tile >= nTiles) return;
+    const int lane = threadIdx.x & 31;
+    const int p = batch_find_tile(pr, P, tile);
+    const BatchProbDev q = pr[p];
+    const int64_t t = tile - q.tile0;
+    const int64_t n = t * 32 + lane;
+    const bool valid = n < q.N;
+    double xn = INFINITY;
+    bool nan = false;
+    if (valid)
+        for (int k = 0; k < q.K; ++k) {
+            const double v = raw[q.roff + (int64_t)k * q.N + n];
+            if (v != v || v == -INFINITY) nan = true;
+            if (Nk[q.voff + k] > 0.0) xn = fmin(xn, v);
+        }
+    if (!(xn < INFINITY)) xn = 0.0;
+    double* dst = u + q.uoff + t * q.K * 32 + lane;
+    for (int k = 0; k < q.K; ++k) dst[k * 32] = valid ? raw[q.roff + (int64_t)k * q.N + n] - xn : INFINITY;
+    x[tile * 32 + lane] = valid ? xn : 0.0;
+    if (nan) atomicAdd(bad, 1u);        // an error count, not a result
+}
+
+// sum_n x_n of each problem, in a fixed order (one CTA per problem)
+__global__ void __launch_bounds__(256) batch_sumx_kernel(const double* __restrict__ x,
+                                                         const BatchProbDev* __restrict__ pr,
+                                                         double* __restrict__ sumx) {
+    __shared__ double sh[256];
+    const BatchProbDev q = pr[blockIdx.x];
+    double s = 0.0;
+    for (int64_t n = threadIdx.x; n < q.N; n += 256) s += x[q.tile0 * 32 + n];
+    sh[threadIdx.x] = s;
+    __syncthreads();
+    for (int o = 128; o > 0; o >>= 1) {
+        if (threadIdx.x < o) sh[threadIdx.x] += sh[threadIdx.x + o];
+        __syncthreads();
+    }
+    if (threadIdx.x == 0) sumx[blockIdx.x] = sh[0];
+}
+
+// ---- the moments pass ---------------------------------------------------------------------------------------------
+__device__ __forceinline__ int batch_find_item(const BatchReq* __restrict__ req, int nReq, int64_t item) {
+    int lo = 0, hi = nReq - 1;
+    while (lo < hi) {
+        const int mid = (lo + hi + 1) >> 1;
+        if (req[mid].item0 <= item) lo = mid;
+        else hi = mid - 1;
+    }
+    return lo;
+}
+
+__device__ __forceinline__ double warp_max(double x) {
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) x = fmax(x, __shfl_xor_sync(0xffffffffu, x, o));
+    return x;
+}
+
+// fold the pair (m2, s2) into (m, s): the running log-sum-exp m + log s
+__device__ __forceinline__ void pair_merge(double& m, double& s, double m2, double s2) {
+    if (!(s2 > 0.0)) return;
+    if (m2 > m) {
+        s = s * exp(m - m2) + s2;
+        m = m2;
+    } else {
+        s += s2 * exp(m2 - m);
+    }
+}
+
+__global__ void __launch_bounds__(BATCH_THREADS) batch_moments_kernel(
+    const double* __restrict__ u, const BatchReq* __restrict__ req, int nReq, const double* __restrict__ fAll,
+    const double* __restrict__ NkAll, const double* __restrict__ logNkAll, double* __restrict__ part) {
+    extern __shared__ __align__(16) double sW[];                  // [K][BATCH_SW_LD] staged Gram weights
+    __shared__ double sM[BATCH_WARPS][BATCH_MAX_K], sS[BATCH_WARPS][BATCH_MAX_K];
+    __shared__ double sF[BATCH_MAX_K], sC[BATCH_MAX_K], sLs[BATCH_MAX_K];
+    __shared__ int sRow[BATCH_MAX_K];                             // 1 sampled, 2 unsampled and asked for, 0 neither
+    __shared__ double sRed[BATCH_THREADS];
+    __shared__ int sBad;
+    const int64_t item = blockIdx.x;
+    const BatchReq q = req[batch_find_item(req, nReq, item)];
+    const int64_t chunk = item - q.item0;
+    const int K = q.K;
+    const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+    if (tid < K) {
+        const double n = NkAll[q.voff + tid];
+        sF[tid] = fAll[q.foff + tid];
+        sC[tid] = n > 0.0 ? sF[tid] + logNkAll[q.voff + tid] : -INFINITY;
+        sLs[tid] = n > 0.0 ? logNkAll[q.voff + tid] : 0.0;
+        sRow[tid] = n > 0.0 ? 1 : (q.allRows ? 2 : 0);
+    }
+    for (int k = tid; k < BATCH_WARPS * BATCH_MAX_K; k += BATCH_THREADS) {
+        (&sM[0][0])[k] = -INFINITY;
+        (&sS[0][0])[k] = 0.0;
+    }
+    if (tid == 0) sBad = 0;
+    // lower-triangle Gram entries of this thread: e = tid + BATCH_THREADS * slot, row i >= column j
+    const int E = q.wantG ? K * (K + 1) / 2 : 0;
+    int gi[BATCH_GSLOTS], gj[BATCH_GSLOTS];
+    double gacc[BATCH_GSLOTS];
+#pragma unroll
+    for (int sl = 0; sl < BATCH_GSLOTS; ++sl) {
+        const int e = tid + BATCH_THREADS * sl;
+        int i = (int)((sqrt(8.0 * e + 1.0) - 1.0) * 0.5);
+        while ((i + 1) * (i + 2) / 2 <= e) ++i;
+        while (i * (i + 1) / 2 > e) --i;
+        gi[sl] = i;
+        gj[sl] = e - i * (i + 1) / 2;
+        gacc[sl] = 0.0;
+    }
+    __syncthreads();
+    const int64_t t0 = chunk * q.ct, t1 = min(q.nT, t0 + q.ct);
+    const int rounds = (int)((q.ct + BATCH_WARPS - 1) / BATCH_WARPS);
+    double sumL = 0.0;
+    bool bad = false;
+    for (int r = 0; r < rounds; ++r) {
+        const int64_t t = t0 + (int64_t)r * BATCH_WARPS + warp;
+        const bool tileOn = t < t1;                                  // warp-uniform
+        const int64_t n = t * 32 + lane;
+        const bool valid = tileOn && n < q.N;
+        const double* ut = u + q.uoff + t * (int64_t)K * 32 + lane;
+        double Lp = 0.0;
+        if (valid) {
+            double m = -INFINITY;
+            for (int k = 0; k < K; ++k)
+                if (sRow[k] == 1) m = fmax(m, sC[k] - __ldg(ut + k * 32));
+            double D = 0.0;
+            for (int k = 0; k < K; ++k)
+                if (sRow[k] == 1) D += exp(sC[k] - __ldg(ut + k * 32) - m);
+            Lp = m + log(D);
+            sumL += Lp;
+        }
+        if (tileOn)
+            for (int k = 0; k < K; ++k) {
+                if (sRow[k] == 0) {
+                    if (q.wantG) sW[k * BATCH_SW_LD + tid] = 0.0;
+                    continue;
+                }
+                double a = valid ? sF[k] - __ldg(ut + k * 32) - Lp : -INFINITY;
+                if (a != a) {
+                    bad = true;
+                    a = -INFINITY;
+                }
+                // sampled rows: e^a <= 1 / N_k, summed linearly (the pair keeps max 0) as the single-problem pass
+                // sums them; unsampled rows: shifted by the warp's max
+                const double wm = sRow[k] == 1 ? 0.0 : warp_max(a);
+                const double e = wm > -INFINITY ? exp(a - wm) : 0.0;
+                const double ws = warp_sum(e);
+                if (lane == 0) pair_merge(sM[warp][k], sS[warp][k], wm, ws);
+                if (q.wantG) sW[k * BATCH_SW_LD + tid] = exp(a + sLs[k]);
+            }
+        else if (q.wantG)
+            for (int k = 0; k < K; ++k) sW[k * BATCH_SW_LD + tid] = 0.0;
+        if (q.wantG) {
+            __syncthreads();
+#pragma unroll
+            for (int sl = 0; sl < BATCH_GSLOTS; ++sl) {
+                if (tid + BATCH_THREADS * sl < E) {
+                    const double* wi = sW + gi[sl] * BATCH_SW_LD;
+                    const double* wj = sW + gj[sl] * BATCH_SW_LD;
+                    double acc = gacc[sl];
+                    for (int s = 0; s < BATCH_ROUND; ++s) acc = fma(wi[s], wj[s], acc);
+                    gacc[sl] = acc;
+                }
+            }
+            __syncthreads();
+        }
+    }
+    if (bad) sBad = 1;
+    sRed[tid] = sumL;
+    __syncthreads();
+    for (int o = BATCH_THREADS / 2; o > 0; o >>= 1) {
+        if (tid < o) sRed[tid] += sRed[tid + o];
+        __syncthreads();
+    }
+    const int64_t stride = batch_part_size(K, q.wantG);
+    double* pc = part + q.poff + chunk * stride;
+    if (tid < K) {
+        double m = sM[0][tid], s = sS[0][tid];
+        for (int w = 1; w < BATCH_WARPS; ++w) pair_merge(m, s, sM[w][tid], sS[w][tid]);
+        pc[2 * tid] = m;
+        pc[2 * tid + 1] = s;
+    }
+    if (tid == 0) {
+        pc[2 * K] = sRed[0];
+        pc[2 * K + 1] = sBad ? 1.0 : 0.0;
+    }
+#pragma unroll
+    for (int sl = 0; sl < BATCH_GSLOTS; ++sl) {
+        const int e = tid + BATCH_THREADS * sl;
+        if (e < E) pc[2 * K + 2 + e] = gacc[sl];
+    }
+}
+
+// A request's chunk partials in chunk order -> its packed output.  The flag is set when a NaN reached a sum, when a
+// sampled row's S_k is outside (1e-280, 1e300) (the range the fused pass and the adaptive loop accept), or when an
+// unsampled row asked for has a NaN or overflowing S_k.  An unsampled row whose every weight is zero (all its
+// energies +inf) reports S_k = 0, log S_k = -inf, as the single-problem path does.
+__global__ void __launch_bounds__(BATCH_THREADS) batch_finalize_kernel(const BatchReq* __restrict__ req,
+                                                                       const double* __restrict__ part,
+                                                                       const double* __restrict__ NkAll,
+                                                                       const double* __restrict__ sumx,
+                                                                       double* __restrict__ out) {
+    __shared__ int sFlag;
+    const BatchReq q = req[blockIdx.x];
+    const int K = q.K, tid = threadIdx.x;
+    const int64_t stride = batch_part_size(K, q.wantG);
+    const int64_t nc = (q.nT + q.ct - 1) / q.ct;
+    const double* p0 = part + q.poff;
+    double* o = out + q.ooff;
+    if (tid == 0) sFlag = 0;
+    __syncthreads();
+    if (tid < K) {
+        double m = -INFINITY, s = 0.0;
+        for (int64_t c = 0; c < nc; ++c) pair_merge(m, s, p0[c * stride + 2 * tid], p0[c * stride + 2 * tid + 1]);
+        const double logS = s > 0.0 ? m + log(s) : -INFINITY;
+        const double S = m == 0.0 ? s : exp(logS);      // sampled rows: the linear sum itself
+        o[tid] = S;
+        o[K + tid] = logS;
+        const bool sampled = NkAll[q.voff + tid] > 0.0;
+        if (sampled && !(S > 1e-280 && S < 1e300)) sFlag = 1;
+        if (!sampled && q.allRows && (logS != logS || !(S < INFINITY))) sFlag = 1;
+    }
+    if (tid == 0) {
+        double sl = 0.0, bad = 0.0;
+        for (int64_t c = 0; c < nc; ++c) {
+            sl += p0[c * stride + 2 * K];
+            bad = fmax(bad, p0[c * stride + 2 * K + 1]);
+        }
+        o[2 * K] = sl - sumx[q.prob];
+        if (bad > 0.0 || sl != sl) sFlag = 1;
+    }
+    if (q.wantG) {
+        const int E = K * (K + 1) / 2;
+        for (int e = tid; e < E; e += BATCH_THREADS) {
+            int i = (int)((sqrt(8.0 * e + 1.0) - 1.0) * 0.5);
+            while ((i + 1) * (i + 2) / 2 <= e) ++i;
+            while (i * (i + 1) / 2 > e) --i;
+            const int j = e - i * (i + 1) / 2;
+            double g = 0.0;
+            for (int64_t c = 0; c < nc; ++c) g += p0[c * stride + 2 * K + 2 + e];
+            o[2 * K + 2 + (int64_t)i * K + j] = g;
+            o[2 * K + 2 + (int64_t)j * K + i] = g;
+        }
+    }
+    __syncthreads();
+    if (tid == 0) o[2 * K + 1] = sFlag ? 1.0 : 0.0;
+}
+
+template <class T>
+static int batch_grow(DevArray<T>& a, int64_t count) {
+    if ((size_t)count <= a.cap) return MBAR_B200_OK;
+    return a.reserve((size_t)(count + count / 2 + 64), "batch");
+}
+
+static int pinned_grow(double** p, size_t* cap, size_t count) {
+    if (count <= *cap) return MBAR_B200_OK;
+    if (*p) cudaFreeHost(*p);
+    *p = nullptr;
+    *cap = 0;
+    const size_t n = count + count / 2 + 64;
+    MBAR_REQUIRE(cudaMallocHost((void**)p, n * sizeof(double)) == cudaSuccess, MBAR_B200_ERR_NOMEM,
+                 "batch: cannot allocate %zu bytes of pinned host memory", n * sizeof(double));
+    *cap = n;
+    return MBAR_B200_OK;
+}
+
+// One request of a moments launch: problem p at f (K_p values), its packed output lands at out (host).
+struct Ask {
+    int p;
+    const double* f;
+    bool G;
+};
+
+// Evaluate the requests in one launch of each kernel and one synchronisation; returns the packed outputs in
+// b->h_out, request r's at offsets[r] (batch_out_size(K_p, G) doubles each).
+static int batch_run(mbar_b200_batch* b, const std::vector<Ask>& asks, bool allRows, std::vector<int64_t>& offsets,
+                     double* msAcc) {
+    const int nReq = (int)asks.size();
+    std::vector<BatchReq> req((size_t)nReq);
+    int64_t items = 0, parts = 0, outs = 0, fs = 0, bytes = 0;
+    int maxKG = 0;
+    offsets.resize(nReq);
+    for (int r = 0; r < nReq; ++r) {
+        const int p = asks[r].p;
+        BatchReq& q = req[r];
+        q.K = b->K[p];
+        q.prob = p;
+        q.allRows = allRows ? 1 : 0;
+        q.wantG = asks[r].G ? 1 : 0;
+        q.N = b->N[p];
+        q.nT = b->nT[p];
+        q.ct = batch_chunk_tiles(q.nT, q.K);
+        q.uoff = b->uoff[p];
+        q.voff = b->voff[p];
+        q.item0 = items;
+        q.poff = parts;
+        q.ooff = outs;
+        q.foff = fs;
+        const int64_t nc = (q.nT + q.ct - 1) / q.ct;
+        items += nc;
+        parts += nc * batch_part_size(q.K, q.wantG);
+        offsets[r] = outs;
+        outs += batch_out_size(q.K, q.wantG);
+        fs += q.K;
+        bytes += q.nT * 32 * q.K * 8;
+        if (q.wantG) maxKG = std::max(maxKG, q.K);
+    }
+    MBAR_REQUIRE(items < INT32_MAX, MBAR_B200_ERR_INVALID, "batch: %lld chunks in one call", (long long)items);
+    MBAR_TRY(batch_grow(b->d_req, nReq));
+    MBAR_TRY(batch_grow(b->d_f, fs));
+    MBAR_TRY(batch_grow(b->d_part, parts));
+    MBAR_TRY(batch_grow(b->d_out, outs));
+    MBAR_TRY(pinned_grow(&b->h_f, &b->h_fCap, (size_t)fs + (size_t)nReq * sizeof(BatchReq) / 8 + 1));
+    MBAR_TRY(pinned_grow(&b->h_out, &b->h_outCap, (size_t)outs));
+    for (int r = 0; r < nReq; ++r) std::memcpy(b->h_f + req[r].foff, asks[r].f, (size_t)req[r].K * sizeof(double));
+    BatchReq* hreq = reinterpret_cast<BatchReq*>(b->h_f + fs);
+    std::memcpy(hreq, req.data(), req.size() * sizeof(BatchReq));
+    MBAR_CUDA(cudaMemcpyAsync(b->d_f, b->h_f, (size_t)fs * sizeof(double), cudaMemcpyHostToDevice, b->stream));
+    MBAR_CUDA(cudaMemcpyAsync(b->d_req, hreq, req.size() * sizeof(BatchReq), cudaMemcpyHostToDevice, b->stream));
+    const size_t shBytes = (size_t)maxKG * BATCH_SW_LD * sizeof(double);
+    static size_t attr[16] = {0};
+    if (attr[b->device & 15] < shBytes) {
+        MBAR_CUDA(cudaFuncSetAttribute(batch_moments_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                       (int)(BATCH_MAX_K * BATCH_SW_LD * sizeof(double))));
+        attr[b->device & 15] = BATCH_MAX_K * BATCH_SW_LD * sizeof(double);
+    }
+    MBAR_CUDA(cudaEventRecord(b->ev0, b->stream));
+    batch_moments_kernel<<<(unsigned)items, BATCH_THREADS, shBytes, b->stream>>>(b->d_u, b->d_req, nReq, b->d_f,
+                                                                                 b->d_Nk, b->d_logNk, b->d_part);
+    batch_finalize_kernel<<<(unsigned)nReq, BATCH_THREADS, 0, b->stream>>>(b->d_req, b->d_part, b->d_Nk, b->d_sumx,
+                                                                           b->d_out);
+    MBAR_CUDA(cudaGetLastError());
+    MBAR_CUDA(cudaEventRecord(b->ev1, b->stream));
+    MBAR_CUDA(cudaMemcpyAsync(b->h_out, b->d_out, (size_t)outs * sizeof(double), cudaMemcpyDeviceToHost, b->stream));
+    MBAR_CUDA(cudaStreamSynchronize(b->stream));
+    float e = 0.f;
+    if (event_ms(b->ev0, b->ev1, &e)) *msAcc += e;
+    b->lastLaunches += 2;
+    b->lastBytes += bytes;
+    return MBAR_B200_OK;
+}
+
+// Per-problem state of the batched adaptive loop.
+struct BatchSolver {
+    std::vector<int> active;
+    StepRows rows;
+    std::vector<double> cur, f_sci, f_nr, g, S, logS, G, A, rhs;
+    mbar_b200_solve_result r{};
+    bool haveNr = false;
+};
+
+}  // namespace mbar
+
+using namespace mbar;
+
+int mbar_b200_batch_create(int device, int32_t n_problems, const int32_t* K, const int64_t* N, const double* N_k,
+                           const double* u, mbar_b200_batch** out) {
+    MBAR_REQUIRE(out && K && N && N_k && u, MBAR_B200_ERR_INVALID, "batch_create: NULL argument");
+    *out = nullptr;
+    MBAR_REQUIRE(n_problems >= 1, MBAR_B200_ERR_INVALID, "batch_create: %d problems", (int)n_problems);
+    std::unique_ptr<mbar_b200_batch> o(new mbar_b200_batch());
+    o->P = n_problems;
+    int64_t rawTotal = 0, vTotal = 0, tiles = 0;
+    std::vector<BatchProbDev> pr((size_t)n_problems);
+    for (int p = 0; p < n_problems; ++p) {
+        MBAR_REQUIRE(K[p] >= 1 && K[p] <= BATCH_MAX_K, MBAR_B200_ERR_INVALID,
+                     "batch_create: problem %d has K=%d states (1 to %d)", p, (int)K[p], BATCH_MAX_K);
+        MBAR_REQUIRE(N[p] >= 1 && N[p] < (int64_t(1) << 36), MBAR_B200_ERR_INVALID,
+                     "batch_create: problem %d has N=%lld samples", p, (long long)N[p]);
+        bool any = false;
+        for (int k = 0; k < K[p]; ++k) {
+            const double n = N_k[vTotal + k];
+            MBAR_REQUIRE(n >= 0.0 && n < INFINITY, MBAR_B200_ERR_INVALID, "batch_create: problem %d has N_k[%d]=%g", p,
+                         k, n);
+            any = any || n > 0.0;
+        }
+        MBAR_REQUIRE(any, MBAR_B200_ERR_INVALID, "batch_create: problem %d has no sampled state", p);
+        const int64_t nT = (N[p] + 31) / 32;
+        o->K.push_back(K[p]);
+        o->N.push_back(N[p]);
+        o->nT.push_back(nT);
+        o->uoff.push_back(o->uTotal);
+        o->voff.push_back(vTotal);
+        pr[p] = BatchProbDev{rawTotal, o->uTotal, tiles, N[p], vTotal, K[p]};
+        rawTotal += (int64_t)K[p] * N[p];
+        o->uTotal += nT * 32 * K[p];
+        vTotal += K[p];
+        tiles += nT;
+    }
+    o->Nk.assign(N_k, N_k + vTotal);
+    std::vector<double> logNk((size_t)vTotal);
+    for (int64_t i = 0; i < vTotal; ++i) logNk[i] = o->Nk[i] > 0.0 ? std::log(o->Nk[i]) : -INFINITY;
+    MBAR_TRY(open_device(device, nullptr));
+    MBAR_TRY(o->open(device, "batch_create"));
+    NvtxRange nvtx_("mbar_b200::batch_create");
+    MBAR_TRY(o->upload(o->d_Nk, o->Nk.data(), (size_t)vTotal, "batch_create"));
+    MBAR_TRY(o->upload(o->d_logNk, logNk.data(), (size_t)vTotal, "batch_create"));
+    MBAR_TRY(o->d_u.reserve((size_t)o->uTotal, "batch_create (tiles)"));
+    MBAR_TRY(o->d_sumx.reserve((size_t)n_problems, "batch_create"));
+    {
+        CallBuffers cb("batch_create (staging)");
+        double *raw = nullptr, *x = nullptr;
+        BatchProbDev* dpr = nullptr;
+        unsigned int* bad = nullptr;
+        MBAR_TRY(cb.alloc(&raw, (size_t)rawTotal));
+        MBAR_TRY(cb.alloc(&x, (size_t)tiles * 32));
+        MBAR_TRY(cb.alloc(&dpr, (size_t)n_problems));
+        MBAR_TRY(cb.alloc(&bad, 1));
+        MBAR_CUDA(cudaMemcpyAsync(raw, u, (size_t)rawTotal * sizeof(double), cudaMemcpyHostToDevice, o->stream));
+        MBAR_CUDA(cudaMemcpyAsync(dpr, pr.data(), pr.size() * sizeof(BatchProbDev), cudaMemcpyHostToDevice,
+                                  o->stream));
+        MBAR_CUDA(cudaMemsetAsync(bad, 0, sizeof(unsigned int), o->stream));
+        batch_retile_kernel<<<(unsigned)((tiles + 7) / 8), 256, 0, o->stream>>>(raw, dpr, n_problems, tiles, o->d_Nk,
+                                                                               o->d_u, x, bad);
+        batch_sumx_kernel<<<(unsigned)n_problems, 256, 0, o->stream>>>(x, dpr, o->d_sumx);
+        MBAR_CUDA(cudaGetLastError());
+        unsigned int hbad = 0;
+        MBAR_CUDA(cudaMemcpyAsync(&hbad, bad, sizeof(hbad), cudaMemcpyDeviceToHost, o->stream));
+        MBAR_CUDA(cudaStreamSynchronize(o->stream));
+        MBAR_REQUIRE(hbad == 0, MBAR_B200_ERR_NAN, "batch_create: %u samples hold NaN or -inf energies", hbad);
+    }
+    *out = o.release();
+    return MBAR_B200_OK;
+}
+
+int mbar_b200_batch_destroy(mbar_b200_batch* b) { return destroy_resident(b); }
+
+int mbar_b200_batch_moments(mbar_b200_batch* b, int32_t n_requests, const int32_t* problem, const double* f,
+                            int32_t all_rows, double* S, double* logS, double* sumL, int32_t* flag, double* G) {
+    MBAR_REQUIRE(b, MBAR_B200_ERR_INVALID, "batch_moments: NULL object");
+    MBAR_REQUIRE(n_requests >= 1 && problem && f, MBAR_B200_ERR_INVALID, "batch_moments: %d requests",
+                 (int)n_requests);
+    std::vector<Ask> asks((size_t)n_requests);
+    int64_t fo = 0;
+    for (int r = 0; r < n_requests; ++r) {
+        const int p = problem[r];
+        MBAR_REQUIRE(p >= 0 && p < b->P, MBAR_B200_ERR_INVALID, "batch_moments: request %d names problem %d of %d", r,
+                     p, b->P);
+        asks[r] = Ask{p, f + fo, G != nullptr};
+        fo += b->K[p];
+    }
+    MBAR_CUDA(cudaSetDevice(b->device));
+    NvtxRange nvtx_("mbar_b200::batch_moments");
+    b->lastLaunches = 0;
+    b->lastBytes = 0;
+    b->lastIterations = 0;
+    double ms = 0.0;
+    std::vector<int64_t> off;
+    MBAR_TRY(batch_run(b, asks, all_rows != 0, off, &ms));
+    b->lastMs = ms;
+    int64_t ko = 0, go = 0;
+    for (int r = 0; r < n_requests; ++r) {
+        const int K = b->K[asks[r].p];
+        const double* o = b->h_out + off[r];
+        if (S) std::memcpy(S + ko, o, K * sizeof(double));
+        if (logS) std::memcpy(logS + ko, o + K, K * sizeof(double));
+        if (sumL) sumL[r] = o[2 * K];
+        if (flag) flag[r] = o[2 * K + 1] != 0.0;
+        if (G) std::memcpy(G + go, o + 2 * K + 2, (size_t)K * K * sizeof(double));
+        ko += K;
+        go += (int64_t)K * K;
+    }
+    return MBAR_B200_OK;
+}
+
+int mbar_b200_batch_solve(mbar_b200_batch* b, double* f, double tol, int32_t maxiter, int32_t min_sc_iter,
+                          double gamma, int32_t* status, int32_t* iterations) {
+    MBAR_REQUIRE(b && f && status && iterations, MBAR_B200_ERR_INVALID, "batch_solve: NULL argument");
+    MBAR_REQUIRE(maxiter >= 0, MBAR_B200_ERR_INVALID, "batch_solve: maxiter=%d", (int)maxiter);
+    MBAR_CUDA(cudaSetDevice(b->device));
+    NvtxRange nvtx_("mbar_b200::batch_solve");
+    b->lastLaunches = 0;
+    b->lastBytes = 0;
+    b->lastIterations = 0;
+    double ms = 0.0;
+    const int P = b->P;
+    std::vector<BatchSolver> sv((size_t)P);
+    std::vector<int> work;                    // problems still iterating, in index order
+    for (int p = 0; p < P; ++p) {
+        BatchSolver& s = sv[p];
+        const int K = b->K[p];
+        const double* Nk = b->Nk.data() + b->voff[p];
+        for (int k = 0; k < K; ++k)
+            if (Nk[k] > 0.0) s.active.push_back(k);
+        s.rows = StepRows{K, s.active.data(), (int)s.active.size(), Nk};
+        double* fp = f + b->voff[p];
+        s.cur.assign(fp, fp + K);
+        for (int k : s.active) s.cur[k] -= fp[s.active[0]];
+        for (int k : s.active)
+            MBAR_REQUIRE(std::isfinite(s.cur[k]) && std::fabs(s.cur[k]) < 0.5 * C_RANGE, MBAR_B200_ERR_RANGE,
+                         "batch_solve: problem %d has f[%d]=%g", p, k, fp[k]);
+        s.g.assign(K, 0.0);
+        status[p] = 1;
+        iterations[p] = 0;
+        if (s.active.size() < 2 || maxiter < 1) status[p] = 0;     // nothing to solve: the gauge fixes f
+        else work.push_back(p);
+    }
+    std::vector<Ask> asks;
+    std::vector<int64_t> off;
+    auto take = [&](BatchSolver& s, const double* o) {
+        const int K = s.rows.K;
+        s.S.assign(o, o + K);
+        s.logS.assign(o + K, o + 2 * K);
+        s.G.assign(o + 2 * K + 2, o + 2 * K + 2 + (size_t)K * K);
+    };
+    // the sums at the starting points
+    for (int p : work) asks.push_back(Ask{p, sv[p].cur.data(), true});
+    if (!work.empty()) MBAR_TRY(batch_run(b, asks, false, off, &ms));
+    {
+        std::vector<int> next;
+        for (size_t i = 0; i < work.size(); ++i) {
+            const int p = work[i];
+            const double* o = b->h_out + off[i];
+            if (o[2 * b->K[p] + 1] != 0.0) {
+                status[p] = 2;
+                continue;
+            }
+            take(sv[p], o);
+            next.push_back(p);
+        }
+        work.swap(next);
+    }
+    // one launch per iteration: both candidates of every problem, with their second moments, so that the chosen
+    // one's sums are the next iteration's sums at f
+    while (!work.empty()) {
+        asks.clear();
+        std::vector<int> first(work.size());
+        for (size_t i = 0; i < work.size(); ++i) {
+            BatchSolver& s = sv[work[i]];
+            step_gradient(s.rows, s.S.data(), s.g);
+            step_sci(s.rows, s.cur, s.logS.data(), s.f_sci);
+            s.haveNr = step_newton(s.rows, s.S.data(), s.G.data(), s.g, s.cur, gamma, s.A, s.rhs, s.f_nr);
+            first[i] = (int)asks.size();
+            asks.push_back(Ask{work[i], s.f_sci.data(), true});
+            if (s.haveNr) asks.push_back(Ask{work[i], s.f_nr.data(), true});
+        }
+        MBAR_TRY(batch_run(b, asks, false, off, &ms));
+        b->lastIterations++;
+        std::vector<int> next;
+        for (size_t i = 0; i < work.size(); ++i) {
+            const int p = work[i];
+            BatchSolver& s = sv[p];
+            const int K = s.rows.K;
+            const double* oS = b->h_out + off[first[i]];
+            const double* oN = s.haveNr ? b->h_out + off[first[i] + 1] : nullptr;
+            bool finite = true;
+            for (int k : s.active) finite = finite && std::isfinite(s.f_sci[k]);
+            if (oS[2 * K + 1] != 0.0 || !finite) {
+                status[p] = 2;              // the self-consistent candidate left the range this loop serves
+                iterations[p] = s.r.iterations;
+                continue;
+            }
+            std::vector<double> gtmp(K);
+            const double gn_sci = step_gradient(s.rows, oS, gtmp);
+            const bool nrOk = s.haveNr && oN[2 * K + 1] == 0.0;
+            const double gn_nr = nrOk ? step_gradient(s.rows, oN, gtmp) : INFINITY;
+            const int nrBefore = s.r.nr_iterations;
+            const bool done = step_choose(s.rows, s.f_sci, s.f_nr, nrOk, gn_sci, gn_nr, tol, min_sc_iter, s.cur, s.r);
+            take(s, s.r.nr_iterations > nrBefore ? oN : oS);
+            iterations[p] = s.r.iterations;
+            if (done) status[p] = 0;
+            else if (s.r.iterations < maxiter) next.push_back(p);
+        }
+        work.swap(next);
+    }
+    for (int p = 0; p < P; ++p) {
+        double* fp = f + b->voff[p];
+        for (int k : sv[p].active) fp[k] = sv[p].cur[k];
+    }
+    b->lastMs = ms;
+    return MBAR_B200_OK;
+}
+
+int mbar_b200_last_batch_stats(mbar_b200_batch* b, double* ms, int32_t* launches, int32_t* iterations,
+                               int64_t* bytes_read) {
+    MBAR_REQUIRE(b, MBAR_B200_ERR_INVALID, "NULL batch object");
+    if (ms) *ms = b->lastMs;
+    if (launches) *launches = b->lastLaunches;
+    if (iterations) *iterations = b->lastIterations;
+    if (bytes_read) *bytes_read = b->lastBytes;
+    return MBAR_B200_OK;
+}

@@ -312,6 +312,26 @@ int reduce_sumxw(mbar_b200_ctx* ctx);   // sum_n w_n x_n with the current shifts
 int set_weights(mbar_b200_ctx* ctx, const double* w_host);
 int probe_exp_launch(int which, int64_t n, const double* d_a, double* d_out);   // mbar_b200_probe_exp
 
+// ---- one adaptive iteration on the host (loops.cu): the rules the host-stepped loop and the batched loop of batch.cu
+// share.  A problem is K states, the indices of its sampled ones (active[0] is the gauge state) and N_k; S, log S and
+// Ghat (N-scaled second moments, row-major K x K) are the sums of a pass.
+struct StepRows {
+    int K;
+    const int* active;
+    int na;
+    const double* Nk;
+};
+StepRows step_rows(const mbar_b200_ctx* c);
+double step_rel_delta(const StepRows& s, const double* fn, const double* fo, double tol);
+void step_sci(const StepRows& s, const std::vector<double>& cur, const double* logS, std::vector<double>& nxt);
+double step_gradient(const StepRows& s, const double* S, std::vector<double>& g);
+bool step_newton(const StepRows& s, const double* S, const double* Gh, const std::vector<double>& g,
+                 const std::vector<double>& cur, double gamma, std::vector<double>& A, std::vector<double>& rhs,
+                 std::vector<double>& f_nr);
+bool step_choose(const StepRows& s, const std::vector<double>& f_sci, const std::vector<double>& f_nr, bool haveNr,
+                 double gn_sci, double gn_nr, double tol, int32_t min_sc_iter, std::vector<double>& cur,
+                 mbar_b200_solve_result& r);
+
 // ---- device helpers ----
 #ifdef __CUDACC__
 static __device__ const double MBAR_EXP_TABLE[MBAR_EXP_NT] = {MBAR_EXP_TABLE_VALUES};

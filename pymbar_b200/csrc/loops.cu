@@ -453,29 +453,51 @@ static int upload_f(mbar_b200_ctx* c, const double* f) {
     return MBAR_B200_OK;
 }
 
+StepRows step_rows(const mbar_b200_ctx* c) { return StepRows{c->K, c->active.data(), (int)c->active.size(), c->h_Nk.data()}; }
+
 // Largest relative change over the sampled states other than the gauge state (mbar_solvers.py:627-631), NaN if any
 // entry is NaN.
-static double rel_delta(const mbar_b200_ctx* c, const std::vector<double>& fn, const std::vector<double>& fo,
-                        double tol) {
+double step_rel_delta(const StepRows& s, const double* fn, const double* fo, double tol) {
     double md = 0.0;
     const double thr = std::min(1e-8, tol);
-    for (size_t i = 1; i < c->active.size(); ++i) {
-        const int k = c->active[i];
+    for (int i = 1; i < s.na; ++i) {
+        const int k = s.active[i];
         const double d = rel_change(fn[k], fo[k], fn[k], thr);
         if (std::isnan(d)) return NAN;
         md = std::max(md, d);
     }
     return md;
 }
+static double rel_delta(const mbar_b200_ctx* c, const std::vector<double>& fn, const std::vector<double>& fo,
+                        double tol) {
+    return step_rel_delta(step_rows(c), fn.data(), fo.data(), tol);
+}
 
-// The self-consistent step (Eq. C3) from the packed output of run_pass at cur: f_k - log S_k over the sampled
-// states, gauge-fixed so that f[firstActive] = 0; unsampled states keep cur.  nxt may be cur.
-static void sci_step(const mbar_b200_ctx* c, const std::vector<double>& cur, std::vector<double>& nxt) {
-    const double* logS = c->h_out + PassLayout{c->K}.logS();
-    const int g0 = c->firstActive;
+// The self-consistent step (Eq. C3) from log S_k at cur: f_k - log S_k over the sampled states, gauge-fixed so that
+// f[active[0]] = 0; unsampled states keep cur.  nxt may be cur.
+void step_sci(const StepRows& s, const std::vector<double>& cur, const double* logS, std::vector<double>& nxt) {
+    const int g0 = s.active[0];
     const double shift = cur[g0] - logS[g0];
     nxt = cur;
-    for (int k : c->active) nxt[k] = (cur[k] - logS[k]) - shift;
+    for (int i = 0; i < s.na; ++i) {
+        const int k = s.active[i];
+        nxt[k] = (cur[k] - logS[k]) - shift;
+    }
+}
+
+// The self-consistent step from the packed output of run_pass at cur.
+static void sci_step(const mbar_b200_ctx* c, const std::vector<double>& cur, std::vector<double>& nxt) {
+    step_sci(step_rows(c), cur, c->h_out + PassLayout{c->K}.logS(), nxt);
+}
+
+// g_k = N_k (S_k - 1) over every state (0 where N_k = 0) and its squared norm
+double step_gradient(const StepRows& s, const double* S, std::vector<double>& g) {
+    double gn = 0.0;
+    for (int k = 0; k < s.K; ++k) {
+        g[k] = s.Nk[k] > 0 ? s.Nk[k] * (S[k] - 1.0) : 0.0;
+        gn += g[k] * g[k];
+    }
+    return gn;
 }
 
 // gradient norm at f over the sampled states (mbar_solvers.py:938-940): one more pass
@@ -554,11 +576,92 @@ static int solve_sci_stepped(mbar_b200_ctx* c, double* f, double tol, int32_t ma
     return rc;
 }
 
+// The Newton candidate of one adaptive iteration from the sums at cur, in the reduced coordinates (gauge state
+// dropped): H[1:,1:] x = g[1:] with H_ab = delta_ab N_i S_i - Ghat_ij (mbar_solvers.py:581-584 uses the min-norm
+// lstsq of the singular full H minus its first component — the same step in exact arithmetic, SURVEY.md Appendix A).
+// A factorisation that fails is retried with a relative ridge, up to four attempts.  False: no candidate (no free
+// state, H not positive definite, or f_nr non-finite or outside C_RANGE).  A and rhs are scratch.
+bool step_newton(const StepRows& s, const double* S, const double* Gh, const std::vector<double>& g,
+                 const std::vector<double>& cur, double gamma, std::vector<double>& A, std::vector<double>& rhs,
+                 std::vector<double>& f_nr) {
+    const int K = s.K, na = s.na;
+    bool haveNr = false;
+    if (na > 1) {
+        const int n = na - 1;
+        double ridge = 0.0, ridgeRel = 0.0, tr = 0.0;
+        for (int a = 1; a < na; ++a) {
+            const int i = s.active[a];
+            tr += s.Nk[i] * S[i];
+        }
+        for (int attempt = 0; attempt < 4 && !haveNr; ++attempt) {
+            A.assign((size_t)n * n, 0.0);
+            for (int a = 1; a < na; ++a) {
+                const int i = s.active[a];
+                for (int b = 1; b <= a; ++b) {
+                    const int j = s.active[b];
+                    double v = -Gh[(size_t)i * K + j];
+                    if (i == j) v += s.Nk[i] * S[i] + ridge;
+                    A[(size_t)(a - 1) * n + (b - 1)] = v;
+                }
+            }
+            if (cholesky(A, n)) {
+                rhs.resize(n);
+                for (int a = 1; a < na; ++a) rhs[a - 1] = g[s.active[a]];
+                chol_solve(A, n, rhs);
+                f_nr = cur;
+                for (int a = 1; a < na; ++a) f_nr[s.active[a]] = cur[s.active[a]] - gamma * rhs[a - 1];
+                haveNr = true;
+                for (int a = 1; a < na; ++a)
+                    if (!std::isfinite(f_nr[s.active[a]]) || std::fabs(f_nr[s.active[a]]) > 0.5 * C_RANGE)
+                        haveNr = false;
+            } else {
+                ridgeRel = (ridgeRel == 0.0) ? 1e-12 : ridgeRel * 1e3;   // relative to the mean diagonal
+                ridge = ridgeRel * (tr / n + 1e-300);
+            }
+        }
+    }
+    return haveNr;
+}
+
+// The step choice of one adaptive iteration (mbar_solvers.py:607) and its convergence rule (:627-640), given the
+// squared gradient norms at both candidates (gn_nr is ignored without a Newton candidate; NaN counts as +inf).  cur
+// becomes the chosen candidate; r's iteration counters, gnorm and max_delta advance.  True when converged.
+bool step_choose(const StepRows& s, const std::vector<double>& f_sci, const std::vector<double>& f_nr, bool haveNr,
+                 double gn_sci, double gn_nr, double tol, int32_t min_sc_iter, std::vector<double>& cur,
+                 mbar_b200_solve_result& r) {
+    const std::vector<double>& fnr = haveNr ? f_nr : f_sci;
+    if (!haveNr || std::isnan(gn_nr)) gn_nr = INFINITY;
+    std::vector<double> f_old = cur;
+    if (gn_sci < gn_nr || r.sci_iterations < min_sc_iter) {     // mbar_solvers.py:607
+        cur = f_sci;
+        r.sci_iterations++;
+        r.gnorm = std::sqrt(gn_sci);
+    } else {
+        cur = fnr;
+        r.nr_iterations++;
+        r.gnorm = std::sqrt(gn_nr);
+    }
+    r.iterations++;
+    r.max_delta = step_rel_delta(s, cur.data(), f_old.data(), tol);
+    // max |f_sci - f_nr| / |f|  (mbar_solvers.py:632)
+    double max_diff = 0.0;
+    const double thr = std::min(1e-8, tol);
+    for (int i = 1; i < s.na; ++i) {
+        const int k = s.active[i];
+        max_diff = std::max(max_diff, rel_change(f_sci[k], fnr[k], cur[k], thr));
+    }
+    if (std::isnan(r.max_delta) || (r.max_delta < tol && max_diff < std::sqrt(tol))) {
+        r.success = 1;
+        return true;
+    }
+    return false;
+}
+
 static int solve_adaptive_stepped(mbar_b200_ctx* c, double* f, double tol, int32_t maxiter, int32_t min_sc_iter,
                                   double gamma, mbar_b200_solve_result* res) {
     const int K = c->K;
     const PassLayout lay{K};
-    const int na = (int)c->active.size();
+    const StepRows rows = step_rows(c);
     std::vector<double> cur(f, f + K), f_sci(K), f_nr(K), g(K, 0.0), g_sci(K), g_nr(K);
     std::vector<double> A, rhs;
     mbar_b200_solve_result r{};
@@ -566,14 +669,6 @@ static int solve_adaptive_stepped(mbar_b200_ctx* c, double* f, double tol, int32
     MBAR_TRY(timer.start(c->stream));
     for (int k : c->active) cur[k] -= f[c->firstActive];
     int rc = MBAR_B200_OK;
-    auto grad_from_out = [&](std::vector<double>& out) {
-        double gn = 0.0;
-        for (int k = 0; k < K; ++k) {
-            out[k] = c->h_Nk[k] > 0 ? c->h_Nk[k] * (c->h_out[k] - 1.0) : 0.0;
-            gn += out[k] * out[k];
-        }
-        return gn;
-    };
     for (int it = 0; it < maxiter && rc == MBAR_B200_OK; ++it) {
         // pass at f with the second moments: gives g, H and the self-consistent candidate at once
         PassWant w;
@@ -582,84 +677,21 @@ static int solve_adaptive_stepped(mbar_b200_ctx* c, double* f, double tol, int32
         if (rc != MBAR_B200_OK) break;
         r.passes++;
         r.hessian_passes++;
-        grad_from_out(g);
+        step_gradient(rows, c->h_out, g);
         sci_step(c, cur, f_sci);
-        // Newton step in the reduced coordinates (gauge state dropped): H[1:,1:] x = g[1:]
-        // (mbar_solvers.py:581-584 uses the min-norm lstsq of the singular full H minus its first
-        // component — the same step in exact arithmetic, SURVEY.md Appendix A).
-        bool haveNr = false;
-        if (na > 1) {
-            const int n = na - 1;
-            const double* Gh = c->h_out + lay.G();
-            double ridge = 0.0, ridgeRel = 0.0, tr = 0.0;
-            for (int a = 1; a < na; ++a) {
-                const int i = c->active[a];
-                tr += c->h_Nk[i] * c->h_out[i];
-            }
-            for (int attempt = 0; attempt < 4 && !haveNr; ++attempt) {
-                A.assign((size_t)n * n, 0.0);
-                for (int a = 1; a < na; ++a) {
-                    const int i = c->active[a];
-                    for (int b = 1; b <= a; ++b) {
-                        const int j = c->active[b];
-                        double v = -Gh[(size_t)i * K + j];
-                        if (i == j) v += c->h_Nk[i] * c->h_out[i] + ridge;
-                        A[(size_t)(a - 1) * n + (b - 1)] = v;
-                    }
-                }
-                if (cholesky(A, n)) {
-                    rhs.resize(n);
-                    for (int a = 1; a < na; ++a) rhs[a - 1] = g[c->active[a]];
-                    chol_solve(A, n, rhs);
-                    f_nr = cur;
-                    for (int a = 1; a < na; ++a) f_nr[c->active[a]] = cur[c->active[a]] - gamma * rhs[a - 1];
-                    haveNr = true;
-                    for (int a = 1; a < na; ++a)
-                        if (!std::isfinite(f_nr[c->active[a]]) || std::fabs(f_nr[c->active[a]]) > 0.5 * C_RANGE)
-                            haveNr = false;
-                } else {
-                    ridgeRel = (ridgeRel == 0.0) ? 1e-12 : ridgeRel * 1e3;   // relative to the mean diagonal
-                    ridge = ridgeRel * (tr / n + 1e-300);
-                }
-            }
-        }
+        const bool haveNr = step_newton(rows, c->h_out, c->h_out + lay.G(), g, cur, gamma, A, rhs, f_nr);
         rc = run_pass(c, f_sci.data(), PassWant{});
         if (rc != MBAR_B200_OK) break;
         r.passes++;
-        const double gn_sci = grad_from_out(g_sci);
+        const double gn_sci = step_gradient(rows, c->h_out, g_sci);
         double gn_nr = INFINITY;
         if (haveNr) {
             rc = run_pass(c, f_nr.data(), PassWant{});
             if (rc != MBAR_B200_OK) break;
             r.passes++;
-            gn_nr = grad_from_out(g_nr);
-            if (std::isnan(gn_nr)) gn_nr = INFINITY;
-        } else {
-            f_nr = f_sci;
+            gn_nr = step_gradient(rows, c->h_out, g_nr);
         }
-        std::vector<double> f_old = cur;
-        if (gn_sci < gn_nr || r.sci_iterations < min_sc_iter) {     // mbar_solvers.py:607
-            cur = f_sci;
-            r.sci_iterations++;
-            r.gnorm = std::sqrt(gn_sci);
-        } else {
-            cur = f_nr;
-            r.nr_iterations++;
-            r.gnorm = std::sqrt(gn_nr);
-        }
-        r.iterations = it + 1;
-        r.max_delta = rel_delta(c, cur, f_old, tol);
-        // max |f_sci - f_nr| / |f|  (mbar_solvers.py:632)
-        double max_diff = 0.0;
-        const double thr = std::min(1e-8, tol);
-        for (size_t i = 1; i < c->active.size(); ++i) {
-            const int k = c->active[i];
-            max_diff = std::max(max_diff, rel_change(f_sci[k], f_nr[k], cur[k], thr));
-        }
-        if (std::isnan(r.max_delta) || (r.max_delta < tol && max_diff < std::sqrt(tol))) {
-            r.success = 1;
-            break;
-        }
+        if (step_choose(rows, f_sci, f_nr, haveNr, gn_sci, gn_nr, tol, min_sc_iter, cur, r)) break;
     }
     r.device_ms = timer.stop();
     if (rc == MBAR_B200_OK) std::memcpy(f, cur.data(), K * sizeof(double));

@@ -686,6 +686,89 @@ class DeviceWork(_Resident):
         return dict(ms=ms.value, launches=launches.value, values_read=values.value, bytes_read=8 * values.value)
 
 
+class DeviceMbarBatch(_Resident):
+    """P small MBAR problems (u_kn [K_p, N_p], N_k [K_p], 1 <= K_p <= 64) resident on one H100 and evaluated together
+    (mbar_b200_batch_*).  Independent of any DeviceProblem.
+
+    `moments(f_list)` returns each problem's S_k, log S_k, sum_n L_n, range flag and optionally the N-scaled Gram
+    Ghat (two launches and one synchronisation for all of them); `solve(f_list)` runs the adaptive solver of
+    DeviceProblem.solve_adaptive on every problem in lockstep, one moments call per iteration."""
+
+    _destroy = "mbar_b200_batch_destroy"
+    MAX_K = 64
+
+    def __init__(self, u_kn_list, N_k_list, device=0):
+        self._lib = _lib.load()
+        self._h = C.c_void_p()
+        us = [np.asarray(u, dtype=np.float64) for u in u_kn_list]
+        nks = [_f64(n) for n in N_k_list]
+        if not us or len(us) != len(nks):
+            raise ValueError("u_kn_list and N_k_list must be non-empty and of the same length")
+        for p, (u, n) in enumerate(zip(us, nks)):
+            if u.ndim != 2 or n.shape != (u.shape[0],):
+                raise ValueError(f"problem {p}: u_kn {u.shape} and N_k {n.shape} do not match")
+        self.P = len(us)
+        self.K = np.ascontiguousarray([u.shape[0] for u in us], dtype=np.int32)
+        self.N = np.ascontiguousarray([u.shape[1] for u in us], dtype=np.int64)
+        self.N_k = nks
+        self.device = int(device)
+        flat = np.empty(int(np.sum(self.K.astype(np.int64) * self.N)))
+        o = 0
+        for u in us:
+            flat[o:o + u.size] = u.ravel()
+            o += u.size
+        Nk = np.ascontiguousarray(np.concatenate(nks))
+        check(self._lib.mbar_b200_batch_create(self.device, self.P, _i32p(self.K), _i64p(self.N), _dptr(Nk),
+                                               _dptr(flat), C.byref(self._h)))
+
+    def moments(self, f_list, want_G=False, all_rows=False, problems=None):
+        """One dict per request (f_list[r] at problem problems[r], by default problem r): S [K_p], log_S [K_p],
+        sum_L, flag and, with want_G, G = Ghat [K_p, K_p] (rows scaled by N_k; unsampled rows by 1 when all_rows,
+        0 otherwise).  Unsampled rows of S and log_S are filled only when all_rows."""
+        problems = np.ascontiguousarray(np.arange(len(f_list)) if problems is None else problems, dtype=np.int32)
+        if problems.shape != (len(f_list),) or len(f_list) == 0:
+            raise ValueError("need one problem index per f vector, and at least one")
+        Ks = [int(self.K[p]) if 0 <= p < self.P else -1 for p in problems]
+        f = np.ascontiguousarray(np.concatenate([_f64(v, K) for v, K in zip(f_list, Ks)]))
+        S, logS = np.empty(f.size), np.empty(f.size)
+        sumL = np.empty(len(Ks))
+        flag = np.empty(len(Ks), np.int32)
+        G = np.empty(sum(K * K for K in Ks)) if want_G else None
+        check(self._lib.mbar_b200_batch_moments(self._h, len(Ks), _i32p(problems), _dptr(f), int(bool(all_rows)),
+                                                _dptr(S), _dptr(logS), _dptr(sumL), _i32p(flag),
+                                                _dptr(G) if want_G else None))
+        out, o, g = [], 0, 0
+        for r, K in enumerate(Ks):
+            d = dict(S=S[o:o + K], log_S=logS[o:o + K], sum_L=float(sumL[r]), flag=bool(flag[r]))
+            if want_G:
+                d["G"] = G[g:g + K * K].reshape(K, K)
+            out.append(d)
+            o += K
+            g += K * K
+        return out
+
+    def solve(self, f_list=None, tol=1e-12, maxiter=10000, min_sc_iter=0, gamma=1.0):
+        """(f_list, status [P], iterations [P]): the adaptive solver from f_list (zeros by default) on every problem.
+        status 0 converged, 1 maxiter reached, 2 an iterate the batched sums could not represent (see
+        mbar_b200_batch_solve).  Sampled states come back with f[first sampled] = 0, unsampled ones untouched."""
+        if f_list is None:
+            f_list = [np.zeros(K) for K in self.K]
+        f = np.ascontiguousarray(np.concatenate([_f64(v, int(K)) for v, K in zip(f_list, self.K)]))
+        status = np.empty(self.P, np.int32)
+        iters = np.empty(self.P, np.int32)
+        check(self._lib.mbar_b200_batch_solve(self._h, _dptr(f), float(tol), int(maxiter), int(min_sc_iter),
+                                              float(gamma), _i32p(status), _i32p(iters)))
+        return np.split(f, np.cumsum(self.K)[:-1]), status, iters
+
+    def last_stats(self):
+        """CUDA-event time (ms) of the last moments or solve call's kernels, its launches, iterations and the bytes of
+        u_kn tiles it read."""
+        ms, launches, iters, nbytes = C.c_double(0), C.c_int32(0), C.c_int32(0), C.c_int64(0)
+        check(self._lib.mbar_b200_last_batch_stats(self._h, C.byref(ms), C.byref(launches), C.byref(iters),
+                                                   C.byref(nbytes)))
+        return dict(ms=ms.value, launches=launches.value, iterations=iters.value, bytes_read=nbytes.value)
+
+
 def measure_fp64_peak(device=0):
     """(DMMA TFLOP/s, DFMA TFLOP/s) of this GPU from register-only loops (mbar_b200_measure_fp64_peak)."""
     a, b = C.c_double(0), C.c_double(0)
