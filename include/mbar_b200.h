@@ -422,8 +422,28 @@ int mbar_b200_batch_moments(mbar_b200_batch* batch, int32_t n_requests, const in
  * the iterations problem p took.  A sampled |f_k| >= 5e5 -> MBAR_B200_ERR_RANGE. */
 int mbar_b200_batch_solve(mbar_b200_batch* batch, double* f_inout, double tol, int32_t maxiter, int32_t min_sc_iter,
                           double gamma, int32_t* status, int32_t* iterations);
-/* CUDA-event time of the kernels of the last batch_moments or batch_solve call, its kernel launches, its iterations
- * (solve) and the bytes of u_kn tiles its passes read. */
+/* Replicate slots (DESIGN.md 3.5g'): replaces the resident slots with n_slots bootstrap replicates, slot s of problem
+ * problem[s] with the uint16 multiplicities counts [N_p] (counts concatenates the slots), and computes each slot's
+ * sum_n c_n x_n once.  A slot naming a bad problem or whose counts do not sum to N_p -> MBAR_B200_ERR_INVALID;
+ * slots that do not fit in device memory -> MBAR_B200_ERR_NOMEM (the message gives the allocation in bytes).  A
+ * failed call leaves no slot.  n_slots = 0 drops every slot. */
+int mbar_b200_batch_set_replicates(mbar_b200_batch* batch, int32_t n_slots, const int32_t* problem,
+                                   const uint16_t* counts);
+/* mbar_b200_batch_moments with every request naming a slot (slot[r]) instead of a problem: the sums of its problem
+ * with sample n counted c_n times, S_k = sum_n c_n e^{f_k - u_kn - L_n}, Ghat_ij = sum_n c_n w_in w_jn and
+ * sum_n c_n L_n, where L_n keeps N_k.  These are the values DeviceProblem.set_sample_weights(c) and the matching
+ * single-problem call give; the flag follows the same rules.  All-ones counts give the bits of the unweighted
+ * request, and a request's results are the same bits whichever requests share the call. */
+int mbar_b200_batch_replicate_moments(mbar_b200_batch* batch, int32_t n_requests, const int32_t* slot,
+                                      const double* f, int32_t all_rows, double* S, double* log_S, double* sum_L,
+                                      int32_t* flag, double* G);
+/* mbar_b200_batch_solve over the slots: the same loop with units that are slots rather than problems.  f_inout
+ * [sum over slots of K_p], status and iterations [n_slots]; the same status codes. */
+int mbar_b200_batch_solve_replicates(mbar_b200_batch* batch, double* f_inout, double tol, int32_t maxiter,
+                                     int32_t min_sc_iter, double gamma, int32_t* status, int32_t* iterations);
+/* CUDA-event time of the kernels of the last batch_moments, batch_solve, batch_replicate_moments or
+ * batch_solve_replicates call, its kernel launches, its iterations (solves) and the bytes of u_kn tiles (and
+ * counts) its passes read. */
 int mbar_b200_last_batch_stats(mbar_b200_batch* batch, double* kernel_ms, int32_t* launches, int32_t* iterations,
                                int64_t* bytes_read);
 

@@ -16,6 +16,16 @@
 // (max, sum) pair, so it neither under- nor overflows inside the pass.  The finalize kernel sets the request's flag
 // where a sum is not a usable number (see batch_finalize_kernel).
 //
+// Replicate slots.  A slot is a bootstrap replicate of one problem: uint16 multiplicities c_n over its N_p samples,
+// padded with 0 to the problem's tiles, and sum_n c_n x_n, computed once when the slots are set (x_n stays resident
+// for that).  A weighted request names a slot and gets exactly what DeviceProblem.set_sample_weights(c) and the
+// matching single-problem call give: S_k = sum_n c_n e^{a_kn}, Ghat_ij = sum_n c_n w_in w_jn and
+// sum L = sum_n c_n L'_n - sum_n c_n x_n, with L'_n itself unweighted (the denominators keep N_k).  It is the same
+// kernel instantiated with W = true; the unweighted instantiation compiles to the code it had before slots existed.
+// Multiplying by c_n = 1 is exact and the order of operations is the same in both instantiations, so all-ones counts
+// give the bits of the unweighted request.  A zero-count sample enters no sum: its a_kn is -inf before the warp max
+// of an unsampled row, as log c_n = -inf does in the single-problem pass.
+//
 // Determinism.  Work items are (request, chunk) pairs; a chunk is CT_p tiles with CT_p a function of (N_p, K_p) alone.
 // Warp w of a CTA takes the chunk's tiles w, w + 4, ... in order and folds each tile into its own (max, sum) pairs;
 // the four warps' pairs, the 128 thread sums of L' and the per-thread Gram sums are combined in a fixed order, and
@@ -55,7 +65,9 @@ struct BatchReq {
     int64_t ooff;     // first double of the request's packed output
     int64_t voff;     // first entry of the problem's K-vectors (N_k, log N_k)
     int64_t foff;     // first entry of the request's f
-    int32_t K, prob, allRows, wantG;
+    int32_t K;
+    int32_t prob;     // the problem, or for a weighted request its replicate slot: indexes sum x (sum c x)
+    int32_t allRows, wantG;
 };
 
 // per-request packed output: [0, K) S, [K, 2K) log S, [2K] sum L, [2K + 1] flag, then K x K Ghat when asked for
@@ -64,6 +76,12 @@ __host__ __device__ __forceinline__ int64_t batch_out_size(int K, bool G) { retu
 __host__ __device__ __forceinline__ int64_t batch_part_size(int K, bool G) {
     return 2 * K + 2 + (G ? (int64_t)K * (K + 1) / 2 : 0);
 }
+
+// one problem's layout for the upload kernels: raw offset, tile offset, first tile, samples, K-vector offset, states
+struct BatchProbDev {
+    int64_t roff, uoff, tile0, N, voff;
+    int32_t K;
+};
 
 }  // namespace mbar
 
@@ -74,6 +92,16 @@ struct mbar_b200_batch : mbar::Resident {
     std::vector<double> Nk;                     // concatenated N_k
     int64_t uTotal = 0;
     mbar::DevArray<double> d_u, d_Nk, d_logNk, d_sumx;
+    mbar::DevArray<double> d_x;                 // x_n [tiles * 32], kept for the slots' sum_n c_n x_n
+    mbar::DevArray<mbar::BatchProbDev> d_prob;  // per-problem layout, as the upload kernels read it
+    // replicate slots (mbar_b200_batch_set_replicates)
+    int nSlots = 0;
+    std::vector<int> slotProb;
+    std::vector<int64_t> slotCoff;              // first count of each slot in d_counts
+    mbar::DevArray<uint16_t> d_counts;          // each slot's c_n, padded with 0 to its problem's tiles
+    mbar::DevArray<int64_t> d_slotCoff;
+    mbar::DevArray<int32_t> d_slotProb;
+    mbar::DevArray<double> d_sumxw;             // sum_n c_n x_n of each slot
     // per-call buffers, grown on demand
     mbar::DevArray<mbar::BatchReq> d_req;
     mbar::DevArray<double> d_f, d_part, d_out;
@@ -92,11 +120,6 @@ struct mbar_b200_batch : mbar::Resident {
 namespace mbar {
 
 // ---- upload: raw row-major problems -> shifted tiles, x_n, sum x_n -------------------------------------------------
-struct BatchProbDev {
-    int64_t roff, uoff, tile0, N, voff;
-    int32_t K;
-};
-
 __device__ __forceinline__ int batch_find_tile(const BatchProbDev* __restrict__ pr, int P, int64_t tile) {
     int lo = 0, hi = P - 1;
     while (lo < hi) {
@@ -136,14 +159,22 @@ __global__ void __launch_bounds__(256) batch_retile_kernel(const double* __restr
     if (nan) atomicAdd(bad, 1u);        // an error count, not a result
 }
 
-// sum_n x_n of each problem, in a fixed order (one CTA per problem)
+// sum_n x_n of each problem (W = false, one CTA per problem) or sum_n c_n x_n of each replicate slot (W = true, one
+// CTA per slot), in a fixed order that is the same for both: all-ones counts give the problem's bits
+template <bool W>
 __global__ void __launch_bounds__(256) batch_sumx_kernel(const double* __restrict__ x,
                                                          const BatchProbDev* __restrict__ pr,
+                                                         const int32_t* __restrict__ slotProb,
+                                                         const int64_t* __restrict__ slotCoff,
+                                                         const uint16_t* __restrict__ counts,
                                                          double* __restrict__ sumx) {
     __shared__ double sh[256];
-    const BatchProbDev q = pr[blockIdx.x];
+    const BatchProbDev q = pr[W ? slotProb[blockIdx.x] : blockIdx.x];
     double s = 0.0;
-    for (int64_t n = threadIdx.x; n < q.N; n += 256) s += x[q.tile0 * 32 + n];
+    for (int64_t n = threadIdx.x; n < q.N; n += 256) {
+        if constexpr (W) s += (double)counts[slotCoff[blockIdx.x] + n] * x[q.tile0 * 32 + n];
+        else s += x[q.tile0 * 32 + n];
+    }
     sh[threadIdx.x] = s;
     __syncthreads();
     for (int o = 128; o > 0; o >>= 1) {
@@ -181,9 +212,13 @@ __device__ __forceinline__ void pair_merge(double& m, double& s, double m2, doub
     }
 }
 
+// W: weighted requests (q.prob names a replicate slot; its counts start at slotCoff[q.prob]).  Every request of a
+// launch is weighted or none is.
+template <bool W>
 __global__ void __launch_bounds__(BATCH_THREADS) batch_moments_kernel(
     const double* __restrict__ u, const BatchReq* __restrict__ req, int nReq, const double* __restrict__ fAll,
-    const double* __restrict__ NkAll, const double* __restrict__ logNkAll, double* __restrict__ part) {
+    const double* __restrict__ NkAll, const double* __restrict__ logNkAll, double* __restrict__ part,
+    const int64_t* __restrict__ slotCoff, const uint16_t* __restrict__ counts) {
     extern __shared__ __align__(16) double sW[];                  // [K][BATCH_SW_LD] staged Gram weights
     __shared__ double sM[BATCH_WARPS][BATCH_MAX_K], sS[BATCH_WARPS][BATCH_MAX_K];
     __shared__ double sF[BATCH_MAX_K], sC[BATCH_MAX_K], sLs[BATCH_MAX_K];
@@ -222,6 +257,13 @@ __global__ void __launch_bounds__(BATCH_THREADS) batch_moments_kernel(
         gacc[sl] = 0.0;
     }
     __syncthreads();
+    double* sCn = nullptr;                                        // the round's counts, for the Gram
+    const uint16_t* cq = nullptr;
+    if constexpr (W) {
+        __shared__ double sCnBuf[BATCH_ROUND];
+        sCn = sCnBuf;
+        cq = counts + slotCoff[q.prob];
+    }
     const int64_t t0 = chunk * q.ct, t1 = min(q.nT, t0 + q.ct);
     const int rounds = (int)((q.ct + BATCH_WARPS - 1) / BATCH_WARPS);
     double sumL = 0.0;
@@ -232,6 +274,11 @@ __global__ void __launch_bounds__(BATCH_THREADS) batch_moments_kernel(
         const int64_t n = t * 32 + lane;
         const bool valid = tileOn && n < q.N;
         const double* ut = u + q.uoff + t * (int64_t)K * 32 + lane;
+        double cn = 1.0;
+        if constexpr (W) {
+            cn = valid ? (double)__ldg(cq + n) : 0.0;
+            if (q.wantG) sCn[tid] = cn;
+        }
         double Lp = 0.0;
         if (valid) {
             double m = -INFINITY;
@@ -241,7 +288,8 @@ __global__ void __launch_bounds__(BATCH_THREADS) batch_moments_kernel(
             for (int k = 0; k < K; ++k)
                 if (sRow[k] == 1) D += exp(sC[k] - __ldg(ut + k * 32) - m);
             Lp = m + log(D);
-            sumL += Lp;
+            if constexpr (W) sumL += cn * Lp;
+            else sumL += Lp;
         }
         if (tileOn)
             for (int k = 0; k < K; ++k) {
@@ -254,10 +302,13 @@ __global__ void __launch_bounds__(BATCH_THREADS) batch_moments_kernel(
                     bad = true;
                     a = -INFINITY;
                 }
+                if constexpr (W)
+                    if (cn == 0.0) a = -INFINITY;
                 // sampled rows: e^a <= 1 / N_k, summed linearly (the pair keeps max 0) as the single-problem pass
                 // sums them; unsampled rows: shifted by the warp's max
                 const double wm = sRow[k] == 1 ? 0.0 : warp_max(a);
-                const double e = wm > -INFINITY ? exp(a - wm) : 0.0;
+                double e = wm > -INFINITY ? exp(a - wm) : 0.0;
+                if constexpr (W) e *= cn;
                 const double ws = warp_sum(e);
                 if (lane == 0) pair_merge(sM[warp][k], sS[warp][k], wm, ws);
                 if (q.wantG) sW[k * BATCH_SW_LD + tid] = exp(a + sLs[k]);
@@ -272,7 +323,10 @@ __global__ void __launch_bounds__(BATCH_THREADS) batch_moments_kernel(
                     const double* wi = sW + gi[sl] * BATCH_SW_LD;
                     const double* wj = sW + gj[sl] * BATCH_SW_LD;
                     double acc = gacc[sl];
-                    for (int s = 0; s < BATCH_ROUND; ++s) acc = fma(wi[s], wj[s], acc);
+                    if constexpr (W)
+                        for (int s = 0; s < BATCH_ROUND; ++s) acc = fma(wi[s] * sCn[s], wj[s], acc);
+                    else
+                        for (int s = 0; s < BATCH_ROUND; ++s) acc = fma(wi[s], wj[s], acc);
                     gacc[sl] = acc;
                 }
             }
@@ -378,27 +432,46 @@ static int pinned_grow(double** p, size_t* cap, size_t count) {
     return MBAR_B200_OK;
 }
 
-// One request of a moments launch: problem p at f (K_p values), its packed output lands at out (host).
+// One request of a moments launch: f (K_p values) at unit `id` — problem id, or replicate slot id when the launch is
+// weighted.
 struct Ask {
-    int p;
+    int id;
     const double* f;
     bool G;
 };
 
+// the problem of unit `id`
+static inline int unit_problem(const mbar_b200_batch* b, bool weighted, int id) {
+    return weighted ? b->slotProb[id] : id;
+}
+
+// Sets the kernel's dynamic shared memory limit once per device and instantiation.
+template <bool W>
+static int batch_smem_attr(int device) {
+    static size_t attr[16] = {0};
+    const size_t need = BATCH_MAX_K * BATCH_SW_LD * sizeof(double);
+    if (attr[device & 15] < need) {
+        MBAR_CUDA(cudaFuncSetAttribute(batch_moments_kernel<W>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)need));
+        attr[device & 15] = need;
+    }
+    return MBAR_B200_OK;
+}
+
 // Evaluate the requests in one launch of each kernel and one synchronisation; returns the packed outputs in
-// b->h_out, request r's at offsets[r] (batch_out_size(K_p, G) doubles each).
-static int batch_run(mbar_b200_batch* b, const std::vector<Ask>& asks, bool allRows, std::vector<int64_t>& offsets,
-                     double* msAcc) {
+// b->h_out, request r's at offsets[r] (batch_out_size(K_p, G) doubles each).  weighted: every request names a
+// replicate slot.
+static int batch_run(mbar_b200_batch* b, const std::vector<Ask>& asks, bool allRows, bool weighted,
+                     std::vector<int64_t>& offsets, double* msAcc) {
     const int nReq = (int)asks.size();
     std::vector<BatchReq> req((size_t)nReq);
     int64_t items = 0, parts = 0, outs = 0, fs = 0, bytes = 0;
     int maxKG = 0;
     offsets.resize(nReq);
     for (int r = 0; r < nReq; ++r) {
-        const int p = asks[r].p;
+        const int p = unit_problem(b, weighted, asks[r].id);
         BatchReq& q = req[r];
         q.K = b->K[p];
-        q.prob = p;
+        q.prob = asks[r].id;
         q.allRows = allRows ? 1 : 0;
         q.wantG = asks[r].G ? 1 : 0;
         q.N = b->N[p];
@@ -416,7 +489,7 @@ static int batch_run(mbar_b200_batch* b, const std::vector<Ask>& asks, bool allR
         offsets[r] = outs;
         outs += batch_out_size(q.K, q.wantG);
         fs += q.K;
-        bytes += q.nT * 32 * q.K * 8;
+        bytes += q.nT * 32 * q.K * 8 + (weighted ? q.nT * 32 * 2 : 0);
         if (q.wantG) maxKG = std::max(maxKG, q.K);
     }
     MBAR_REQUIRE(items < INT32_MAX, MBAR_B200_ERR_INVALID, "batch: %lld chunks in one call", (long long)items);
@@ -432,17 +505,16 @@ static int batch_run(mbar_b200_batch* b, const std::vector<Ask>& asks, bool allR
     MBAR_CUDA(cudaMemcpyAsync(b->d_f, b->h_f, (size_t)fs * sizeof(double), cudaMemcpyHostToDevice, b->stream));
     MBAR_CUDA(cudaMemcpyAsync(b->d_req, hreq, req.size() * sizeof(BatchReq), cudaMemcpyHostToDevice, b->stream));
     const size_t shBytes = (size_t)maxKG * BATCH_SW_LD * sizeof(double);
-    static size_t attr[16] = {0};
-    if (attr[b->device & 15] < shBytes) {
-        MBAR_CUDA(cudaFuncSetAttribute(batch_moments_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                       (int)(BATCH_MAX_K * BATCH_SW_LD * sizeof(double))));
-        attr[b->device & 15] = BATCH_MAX_K * BATCH_SW_LD * sizeof(double);
-    }
+    if (shBytes > 0) MBAR_TRY(weighted ? batch_smem_attr<true>(b->device) : batch_smem_attr<false>(b->device));
     MBAR_CUDA(cudaEventRecord(b->ev0, b->stream));
-    batch_moments_kernel<<<(unsigned)items, BATCH_THREADS, shBytes, b->stream>>>(b->d_u, b->d_req, nReq, b->d_f,
-                                                                                 b->d_Nk, b->d_logNk, b->d_part);
-    batch_finalize_kernel<<<(unsigned)nReq, BATCH_THREADS, 0, b->stream>>>(b->d_req, b->d_part, b->d_Nk, b->d_sumx,
-                                                                           b->d_out);
+    if (weighted)
+        batch_moments_kernel<true><<<(unsigned)items, BATCH_THREADS, shBytes, b->stream>>>(
+            b->d_u, b->d_req, nReq, b->d_f, b->d_Nk, b->d_logNk, b->d_part, b->d_slotCoff, b->d_counts);
+    else
+        batch_moments_kernel<false><<<(unsigned)items, BATCH_THREADS, shBytes, b->stream>>>(
+            b->d_u, b->d_req, nReq, b->d_f, b->d_Nk, b->d_logNk, b->d_part, nullptr, nullptr);
+    batch_finalize_kernel<<<(unsigned)nReq, BATCH_THREADS, 0, b->stream>>>(b->d_req, b->d_part, b->d_Nk,
+                                                                           weighted ? b->d_sumxw : b->d_sumx, b->d_out);
     MBAR_CUDA(cudaGetLastError());
     MBAR_CUDA(cudaEventRecord(b->ev1, b->stream));
     MBAR_CUDA(cudaMemcpyAsync(b->h_out, b->d_out, (size_t)outs * sizeof(double), cudaMemcpyDeviceToHost, b->stream));
@@ -454,7 +526,7 @@ static int batch_run(mbar_b200_batch* b, const std::vector<Ask>& asks, bool allR
     return MBAR_B200_OK;
 }
 
-// Per-problem state of the batched adaptive loop.
+// Per-unit state of the batched adaptive loop.
 struct BatchSolver {
     std::vector<int> active;
     StepRows rows;
@@ -462,6 +534,158 @@ struct BatchSolver {
     mbar_b200_solve_result r{};
     bool haveNr = false;
 };
+
+// The adaptive loop of mbar_b200_batch_solve over U units: the problems (weighted = false, U = P) or the replicate
+// slots (weighted = true, U = nSlots), each unit with its problem's K_p entries of f in unit order.  Every iteration
+// evaluates both candidates of every unfinished unit in one batch_run.
+static int batch_solve_units(mbar_b200_batch* b, bool weighted, double* f, double tol, int32_t maxiter,
+                             int32_t min_sc_iter, double gamma, int32_t* status, int32_t* iterations, const char* who) {
+    MBAR_REQUIRE(maxiter >= 0, MBAR_B200_ERR_INVALID, "%s: maxiter=%d", who, (int)maxiter);
+    MBAR_CUDA(cudaSetDevice(b->device));
+    b->lastLaunches = 0;
+    b->lastBytes = 0;
+    b->lastIterations = 0;
+    double ms = 0.0;
+    const int U = weighted ? b->nSlots : b->P;
+    std::vector<BatchSolver> sv((size_t)U);
+    std::vector<int64_t> foff((size_t)U + 1, 0);
+    std::vector<int> work;                    // units still iterating, in index order
+    for (int u = 0; u < U; ++u) {
+        BatchSolver& s = sv[u];
+        const int p = unit_problem(b, weighted, u);
+        const int K = b->K[p];
+        foff[u + 1] = foff[u] + K;
+        const double* Nk = b->Nk.data() + b->voff[p];
+        for (int k = 0; k < K; ++k)
+            if (Nk[k] > 0.0) s.active.push_back(k);
+        s.rows = StepRows{K, s.active.data(), (int)s.active.size(), Nk};
+        double* fp = f + foff[u];
+        s.cur.assign(fp, fp + K);
+        for (int k : s.active) s.cur[k] -= fp[s.active[0]];
+        for (int k : s.active)
+            MBAR_REQUIRE(std::isfinite(s.cur[k]) && std::fabs(s.cur[k]) < 0.5 * C_RANGE, MBAR_B200_ERR_RANGE,
+                         "%s: %s %d has f[%d]=%g", who, weighted ? "slot" : "problem", u, k, fp[k]);
+        s.g.assign(K, 0.0);
+        status[u] = 1;
+        iterations[u] = 0;
+        if (s.active.size() < 2 || maxiter < 1) status[u] = 0;     // nothing to solve: the gauge fixes f
+        else work.push_back(u);
+    }
+    std::vector<Ask> asks;
+    std::vector<int64_t> off;
+    auto take = [&](BatchSolver& s, const double* o) {
+        const int K = s.rows.K;
+        s.S.assign(o, o + K);
+        s.logS.assign(o + K, o + 2 * K);
+        s.G.assign(o + 2 * K + 2, o + 2 * K + 2 + (size_t)K * K);
+    };
+    // the sums at the starting points
+    for (int u : work) asks.push_back(Ask{u, sv[u].cur.data(), true});
+    if (!work.empty()) MBAR_TRY(batch_run(b, asks, false, weighted, off, &ms));
+    {
+        std::vector<int> next;
+        for (size_t i = 0; i < work.size(); ++i) {
+            const int u = work[i];
+            const double* o = b->h_out + off[i];
+            if (o[2 * sv[u].rows.K + 1] != 0.0) {
+                status[u] = 2;
+                continue;
+            }
+            take(sv[u], o);
+            next.push_back(u);
+        }
+        work.swap(next);
+    }
+    // one launch per iteration: both candidates of every unit, with their second moments, so that the chosen one's
+    // sums are the next iteration's sums at f
+    while (!work.empty()) {
+        asks.clear();
+        std::vector<int> first(work.size());
+        for (size_t i = 0; i < work.size(); ++i) {
+            BatchSolver& s = sv[work[i]];
+            step_gradient(s.rows, s.S.data(), s.g);
+            step_sci(s.rows, s.cur, s.logS.data(), s.f_sci);
+            s.haveNr = step_newton(s.rows, s.S.data(), s.G.data(), s.g, s.cur, gamma, s.A, s.rhs, s.f_nr);
+            first[i] = (int)asks.size();
+            asks.push_back(Ask{work[i], s.f_sci.data(), true});
+            if (s.haveNr) asks.push_back(Ask{work[i], s.f_nr.data(), true});
+        }
+        MBAR_TRY(batch_run(b, asks, false, weighted, off, &ms));
+        b->lastIterations++;
+        std::vector<int> next;
+        for (size_t i = 0; i < work.size(); ++i) {
+            const int u = work[i];
+            BatchSolver& s = sv[u];
+            const int K = s.rows.K;
+            const double* oS = b->h_out + off[first[i]];
+            const double* oN = s.haveNr ? b->h_out + off[first[i] + 1] : nullptr;
+            bool finite = true;
+            for (int k : s.active) finite = finite && std::isfinite(s.f_sci[k]);
+            if (oS[2 * K + 1] != 0.0 || !finite) {
+                status[u] = 2;              // the self-consistent candidate left the range this loop serves
+                iterations[u] = s.r.iterations;
+                continue;
+            }
+            std::vector<double> gtmp(K);
+            const double gn_sci = step_gradient(s.rows, oS, gtmp);
+            const bool nrOk = s.haveNr && oN[2 * K + 1] == 0.0;
+            const double gn_nr = nrOk ? step_gradient(s.rows, oN, gtmp) : INFINITY;
+            const int nrBefore = s.r.nr_iterations;
+            const bool done = step_choose(s.rows, s.f_sci, s.f_nr, nrOk, gn_sci, gn_nr, tol, min_sc_iter, s.cur, s.r);
+            take(s, s.r.nr_iterations > nrBefore ? oN : oS);
+            iterations[u] = s.r.iterations;
+            if (done) status[u] = 0;
+            else if (s.r.iterations < maxiter) next.push_back(u);
+        }
+        work.swap(next);
+    }
+    for (int u = 0; u < U; ++u) {
+        double* fp = f + foff[u];
+        for (int k : sv[u].active) fp[k] = sv[u].cur[k];
+    }
+    b->lastMs = ms;
+    return MBAR_B200_OK;
+}
+
+// The moments of mbar_b200_batch_moments (weighted = false, ids name problems) or of
+// mbar_b200_batch_replicate_moments (ids name slots), unpacked into the caller's arrays.
+static int batch_moments_call(mbar_b200_batch* b, bool weighted, int32_t n, const int32_t* ids, const double* f,
+                              int32_t all_rows, double* S, double* logS, double* sumL, int32_t* flag, double* G,
+                              const char* who) {
+    MBAR_REQUIRE(b, MBAR_B200_ERR_INVALID, "%s: NULL object", who);
+    MBAR_REQUIRE(n >= 1 && ids && f, MBAR_B200_ERR_INVALID, "%s: %d requests", who, (int)n);
+    const int U = weighted ? b->nSlots : b->P;
+    std::vector<Ask> asks((size_t)n);
+    int64_t fo = 0;
+    for (int r = 0; r < n; ++r) {
+        const int id = ids[r];
+        MBAR_REQUIRE(id >= 0 && id < U, MBAR_B200_ERR_INVALID, "%s: request %d names %s %d of %d", who, r,
+                     weighted ? "slot" : "problem", id, U);
+        asks[r] = Ask{id, f + fo, G != nullptr};
+        fo += b->K[unit_problem(b, weighted, id)];
+    }
+    MBAR_CUDA(cudaSetDevice(b->device));
+    b->lastLaunches = 0;
+    b->lastBytes = 0;
+    b->lastIterations = 0;
+    double ms = 0.0;
+    std::vector<int64_t> off;
+    MBAR_TRY(batch_run(b, asks, all_rows != 0, weighted, off, &ms));
+    b->lastMs = ms;
+    int64_t ko = 0, go = 0;
+    for (int r = 0; r < n; ++r) {
+        const int K = b->K[unit_problem(b, weighted, asks[r].id)];
+        const double* o = b->h_out + off[r];
+        if (S) std::memcpy(S + ko, o, K * sizeof(double));
+        if (logS) std::memcpy(logS + ko, o + K, K * sizeof(double));
+        if (sumL) sumL[r] = o[2 * K];
+        if (flag) flag[r] = o[2 * K + 1] != 0.0;
+        if (G) std::memcpy(G + go, o + 2 * K + 2, (size_t)K * K * sizeof(double));
+        ko += K;
+        go += (int64_t)K * K;
+    }
+    return MBAR_B200_OK;
+}
 
 }  // namespace mbar
 
@@ -511,22 +735,20 @@ int mbar_b200_batch_create(int device, int32_t n_problems, const int32_t* K, con
     MBAR_TRY(o->upload(o->d_logNk, logNk.data(), (size_t)vTotal, "batch_create"));
     MBAR_TRY(o->d_u.reserve((size_t)o->uTotal, "batch_create (tiles)"));
     MBAR_TRY(o->d_sumx.reserve((size_t)n_problems, "batch_create"));
+    MBAR_TRY(o->d_x.reserve((size_t)tiles * 32, "batch_create (x_n)"));
+    MBAR_TRY(o->upload(o->d_prob, pr.data(), pr.size(), "batch_create"));
     {
         CallBuffers cb("batch_create (staging)");
-        double *raw = nullptr, *x = nullptr;
-        BatchProbDev* dpr = nullptr;
+        double* raw = nullptr;
         unsigned int* bad = nullptr;
         MBAR_TRY(cb.alloc(&raw, (size_t)rawTotal));
-        MBAR_TRY(cb.alloc(&x, (size_t)tiles * 32));
-        MBAR_TRY(cb.alloc(&dpr, (size_t)n_problems));
         MBAR_TRY(cb.alloc(&bad, 1));
         MBAR_CUDA(cudaMemcpyAsync(raw, u, (size_t)rawTotal * sizeof(double), cudaMemcpyHostToDevice, o->stream));
-        MBAR_CUDA(cudaMemcpyAsync(dpr, pr.data(), pr.size() * sizeof(BatchProbDev), cudaMemcpyHostToDevice,
-                                  o->stream));
         MBAR_CUDA(cudaMemsetAsync(bad, 0, sizeof(unsigned int), o->stream));
-        batch_retile_kernel<<<(unsigned)((tiles + 7) / 8), 256, 0, o->stream>>>(raw, dpr, n_problems, tiles, o->d_Nk,
-                                                                               o->d_u, x, bad);
-        batch_sumx_kernel<<<(unsigned)n_problems, 256, 0, o->stream>>>(x, dpr, o->d_sumx);
+        batch_retile_kernel<<<(unsigned)((tiles + 7) / 8), 256, 0, o->stream>>>(raw, o->d_prob, n_problems, tiles,
+                                                                               o->d_Nk, o->d_u, o->d_x, bad);
+        batch_sumx_kernel<false><<<(unsigned)n_problems, 256, 0, o->stream>>>(o->d_x, o->d_prob, nullptr, nullptr,
+                                                                               nullptr, o->d_sumx);
         MBAR_CUDA(cudaGetLastError());
         unsigned int hbad = 0;
         MBAR_CUDA(cudaMemcpyAsync(&hbad, bad, sizeof(hbad), cudaMemcpyDeviceToHost, o->stream));
@@ -541,148 +763,76 @@ int mbar_b200_batch_destroy(mbar_b200_batch* b) { return destroy_resident(b); }
 
 int mbar_b200_batch_moments(mbar_b200_batch* b, int32_t n_requests, const int32_t* problem, const double* f,
                             int32_t all_rows, double* S, double* logS, double* sumL, int32_t* flag, double* G) {
-    MBAR_REQUIRE(b, MBAR_B200_ERR_INVALID, "batch_moments: NULL object");
-    MBAR_REQUIRE(n_requests >= 1 && problem && f, MBAR_B200_ERR_INVALID, "batch_moments: %d requests",
-                 (int)n_requests);
-    std::vector<Ask> asks((size_t)n_requests);
-    int64_t fo = 0;
-    for (int r = 0; r < n_requests; ++r) {
-        const int p = problem[r];
-        MBAR_REQUIRE(p >= 0 && p < b->P, MBAR_B200_ERR_INVALID, "batch_moments: request %d names problem %d of %d", r,
-                     p, b->P);
-        asks[r] = Ask{p, f + fo, G != nullptr};
-        fo += b->K[p];
-    }
-    MBAR_CUDA(cudaSetDevice(b->device));
     NvtxRange nvtx_("mbar_b200::batch_moments");
-    b->lastLaunches = 0;
-    b->lastBytes = 0;
-    b->lastIterations = 0;
-    double ms = 0.0;
-    std::vector<int64_t> off;
-    MBAR_TRY(batch_run(b, asks, all_rows != 0, off, &ms));
-    b->lastMs = ms;
-    int64_t ko = 0, go = 0;
-    for (int r = 0; r < n_requests; ++r) {
-        const int K = b->K[asks[r].p];
-        const double* o = b->h_out + off[r];
-        if (S) std::memcpy(S + ko, o, K * sizeof(double));
-        if (logS) std::memcpy(logS + ko, o + K, K * sizeof(double));
-        if (sumL) sumL[r] = o[2 * K];
-        if (flag) flag[r] = o[2 * K + 1] != 0.0;
-        if (G) std::memcpy(G + go, o + 2 * K + 2, (size_t)K * K * sizeof(double));
-        ko += K;
-        go += (int64_t)K * K;
-    }
-    return MBAR_B200_OK;
+    return batch_moments_call(b, false, n_requests, problem, f, all_rows, S, logS, sumL, flag, G, "batch_moments");
 }
 
 int mbar_b200_batch_solve(mbar_b200_batch* b, double* f, double tol, int32_t maxiter, int32_t min_sc_iter,
                           double gamma, int32_t* status, int32_t* iterations) {
     MBAR_REQUIRE(b && f && status && iterations, MBAR_B200_ERR_INVALID, "batch_solve: NULL argument");
-    MBAR_REQUIRE(maxiter >= 0, MBAR_B200_ERR_INVALID, "batch_solve: maxiter=%d", (int)maxiter);
-    MBAR_CUDA(cudaSetDevice(b->device));
     NvtxRange nvtx_("mbar_b200::batch_solve");
-    b->lastLaunches = 0;
-    b->lastBytes = 0;
-    b->lastIterations = 0;
-    double ms = 0.0;
-    const int P = b->P;
-    std::vector<BatchSolver> sv((size_t)P);
-    std::vector<int> work;                    // problems still iterating, in index order
-    for (int p = 0; p < P; ++p) {
-        BatchSolver& s = sv[p];
-        const int K = b->K[p];
-        const double* Nk = b->Nk.data() + b->voff[p];
-        for (int k = 0; k < K; ++k)
-            if (Nk[k] > 0.0) s.active.push_back(k);
-        s.rows = StepRows{K, s.active.data(), (int)s.active.size(), Nk};
-        double* fp = f + b->voff[p];
-        s.cur.assign(fp, fp + K);
-        for (int k : s.active) s.cur[k] -= fp[s.active[0]];
-        for (int k : s.active)
-            MBAR_REQUIRE(std::isfinite(s.cur[k]) && std::fabs(s.cur[k]) < 0.5 * C_RANGE, MBAR_B200_ERR_RANGE,
-                         "batch_solve: problem %d has f[%d]=%g", p, k, fp[k]);
-        s.g.assign(K, 0.0);
-        status[p] = 1;
-        iterations[p] = 0;
-        if (s.active.size() < 2 || maxiter < 1) status[p] = 0;     // nothing to solve: the gauge fixes f
-        else work.push_back(p);
+    return batch_solve_units(b, false, f, tol, maxiter, min_sc_iter, gamma, status, iterations, "batch_solve");
+}
+
+int mbar_b200_batch_set_replicates(mbar_b200_batch* b, int32_t n_slots, const int32_t* problem,
+                                   const uint16_t* counts) {
+    MBAR_REQUIRE(b, MBAR_B200_ERR_INVALID, "batch_set_replicates: NULL object");
+    b->nSlots = 0;                            // a failed call leaves no slot
+    MBAR_REQUIRE(n_slots >= 0 && (n_slots == 0 || (problem && counts)), MBAR_B200_ERR_INVALID,
+                 "batch_set_replicates: %d slots", (int)n_slots);
+    std::vector<int64_t> coff((size_t)n_slots);
+    int64_t padded = 0, src = 0;
+    for (int s = 0; s < n_slots; ++s) {
+        const int p = problem[s];
+        MBAR_REQUIRE(p >= 0 && p < b->P, MBAR_B200_ERR_INVALID, "batch_set_replicates: slot %d names problem %d of %d",
+                     s, p, b->P);
+        int64_t sum = 0;
+        for (int64_t n = 0; n < b->N[p]; ++n) sum += counts[src + n];
+        MBAR_REQUIRE(sum == b->N[p], MBAR_B200_ERR_INVALID,
+                     "batch_set_replicates: slot %d counts sum to %lld, problem %d has %lld samples", s,
+                     (long long)sum, p, (long long)b->N[p]);
+        coff[s] = padded;
+        padded += b->nT[p] * 32;
+        src += b->N[p];
     }
-    std::vector<Ask> asks;
-    std::vector<int64_t> off;
-    auto take = [&](BatchSolver& s, const double* o) {
-        const int K = s.rows.K;
-        s.S.assign(o, o + K);
-        s.logS.assign(o + K, o + 2 * K);
-        s.G.assign(o + 2 * K + 2, o + 2 * K + 2 + (size_t)K * K);
-    };
-    // the sums at the starting points
-    for (int p : work) asks.push_back(Ask{p, sv[p].cur.data(), true});
-    if (!work.empty()) MBAR_TRY(batch_run(b, asks, false, off, &ms));
-    {
-        std::vector<int> next;
-        for (size_t i = 0; i < work.size(); ++i) {
-            const int p = work[i];
-            const double* o = b->h_out + off[i];
-            if (o[2 * b->K[p] + 1] != 0.0) {
-                status[p] = 2;
-                continue;
-            }
-            take(sv[p], o);
-            next.push_back(p);
-        }
-        work.swap(next);
+    MBAR_CUDA(cudaSetDevice(b->device));
+    NvtxRange nvtx_("mbar_b200::batch_set_replicates");
+    b->slotProb.assign(problem, problem + n_slots);
+    b->slotCoff = coff;
+    if (n_slots == 0) return MBAR_B200_OK;
+    std::vector<uint16_t> hc((size_t)padded, 0);
+    src = 0;
+    for (int s = 0; s < n_slots; ++s) {
+        const int64_t N = b->N[problem[s]];
+        std::memcpy(hc.data() + coff[s], counts + src, (size_t)N * sizeof(uint16_t));
+        src += N;
     }
-    // one launch per iteration: both candidates of every problem, with their second moments, so that the chosen
-    // one's sums are the next iteration's sums at f
-    while (!work.empty()) {
-        asks.clear();
-        std::vector<int> first(work.size());
-        for (size_t i = 0; i < work.size(); ++i) {
-            BatchSolver& s = sv[work[i]];
-            step_gradient(s.rows, s.S.data(), s.g);
-            step_sci(s.rows, s.cur, s.logS.data(), s.f_sci);
-            s.haveNr = step_newton(s.rows, s.S.data(), s.G.data(), s.g, s.cur, gamma, s.A, s.rhs, s.f_nr);
-            first[i] = (int)asks.size();
-            asks.push_back(Ask{work[i], s.f_sci.data(), true});
-            if (s.haveNr) asks.push_back(Ask{work[i], s.f_nr.data(), true});
-        }
-        MBAR_TRY(batch_run(b, asks, false, off, &ms));
-        b->lastIterations++;
-        std::vector<int> next;
-        for (size_t i = 0; i < work.size(); ++i) {
-            const int p = work[i];
-            BatchSolver& s = sv[p];
-            const int K = s.rows.K;
-            const double* oS = b->h_out + off[first[i]];
-            const double* oN = s.haveNr ? b->h_out + off[first[i] + 1] : nullptr;
-            bool finite = true;
-            for (int k : s.active) finite = finite && std::isfinite(s.f_sci[k]);
-            if (oS[2 * K + 1] != 0.0 || !finite) {
-                status[p] = 2;              // the self-consistent candidate left the range this loop serves
-                iterations[p] = s.r.iterations;
-                continue;
-            }
-            std::vector<double> gtmp(K);
-            const double gn_sci = step_gradient(s.rows, oS, gtmp);
-            const bool nrOk = s.haveNr && oN[2 * K + 1] == 0.0;
-            const double gn_nr = nrOk ? step_gradient(s.rows, oN, gtmp) : INFINITY;
-            const int nrBefore = s.r.nr_iterations;
-            const bool done = step_choose(s.rows, s.f_sci, s.f_nr, nrOk, gn_sci, gn_nr, tol, min_sc_iter, s.cur, s.r);
-            take(s, s.r.nr_iterations > nrBefore ? oN : oS);
-            iterations[p] = s.r.iterations;
-            if (done) status[p] = 0;
-            else if (s.r.iterations < maxiter) next.push_back(p);
-        }
-        work.swap(next);
-    }
-    for (int p = 0; p < P; ++p) {
-        double* fp = f + b->voff[p];
-        for (int k : sv[p].active) fp[k] = sv[p].cur[k];
-    }
-    b->lastMs = ms;
+    MBAR_TRY(b->upload(b->d_counts, hc.data(), hc.size(), "batch_set_replicates (counts)"));
+    MBAR_TRY(b->upload(b->d_slotCoff, coff.data(), coff.size(), "batch_set_replicates"));
+    MBAR_TRY(b->upload(b->d_slotProb, problem, (size_t)n_slots, "batch_set_replicates"));
+    MBAR_TRY(b->d_sumxw.reserve((size_t)n_slots, "batch_set_replicates"));
+    batch_sumx_kernel<true><<<(unsigned)n_slots, 256, 0, b->stream>>>(b->d_x, b->d_prob, b->d_slotProb, b->d_slotCoff,
+                                                                       b->d_counts, b->d_sumxw);
+    MBAR_CUDA(cudaGetLastError());
+    MBAR_CUDA(cudaStreamSynchronize(b->stream));
+    b->nSlots = n_slots;
     return MBAR_B200_OK;
+}
+
+int mbar_b200_batch_replicate_moments(mbar_b200_batch* b, int32_t n_requests, const int32_t* slot, const double* f,
+                                      int32_t all_rows, double* S, double* logS, double* sumL, int32_t* flag,
+                                      double* G) {
+    NvtxRange nvtx_("mbar_b200::batch_replicate_moments");
+    return batch_moments_call(b, true, n_requests, slot, f, all_rows, S, logS, sumL, flag, G,
+                              "batch_replicate_moments");
+}
+
+int mbar_b200_batch_solve_replicates(mbar_b200_batch* b, double* f, double tol, int32_t maxiter,
+                                     int32_t min_sc_iter, double gamma, int32_t* status, int32_t* iterations) {
+    MBAR_REQUIRE(b && f && status && iterations, MBAR_B200_ERR_INVALID, "batch_solve_replicates: NULL argument");
+    NvtxRange nvtx_("mbar_b200::batch_solve_replicates");
+    return batch_solve_units(b, true, f, tol, maxiter, min_sc_iter, gamma, status, iterations,
+                             "batch_solve_replicates");
 }
 
 int mbar_b200_last_batch_stats(mbar_b200_batch* b, double* ms, int32_t* launches, int32_t* iterations,

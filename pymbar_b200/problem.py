@@ -692,7 +692,12 @@ class DeviceMbarBatch(_Resident):
 
     `moments(f_list)` returns each problem's S_k, log S_k, sum_n L_n, range flag and optionally the N-scaled Gram
     Ghat (two launches and one synchronisation for all of them); `solve(f_list)` runs the adaptive solver of
-    DeviceProblem.solve_adaptive on every problem in lockstep, one moments call per iteration."""
+    DeviceProblem.solve_adaptive on every problem in lockstep, one moments call per iteration.
+
+    Bootstrap replicates live in replicate slots (`set_replicates`): uint16 multiplicities c_n over one problem's
+    samples.  `moments(..., slots=)` and `solve_replicates` evaluate a slot exactly as
+    DeviceProblem.set_sample_weights(c) followed by the matching single-problem call would, in the same batched
+    launches: S_k = sum_n c_n e^{a_kn}, Ghat_ij = sum_n c_n w_in w_jn and sum_L = sum_n c_n L_n."""
 
     _destroy = "mbar_b200_batch_destroy"
     MAX_K = 64
@@ -708,6 +713,7 @@ class DeviceMbarBatch(_Resident):
             if u.ndim != 2 or n.shape != (u.shape[0],):
                 raise ValueError(f"problem {p}: u_kn {u.shape} and N_k {n.shape} do not match")
         self.P = len(us)
+        self.slot_problems = np.zeros(0, np.int32)
         self.K = np.ascontiguousarray([u.shape[0] for u in us], dtype=np.int32)
         self.N = np.ascontiguousarray([u.shape[1] for u in us], dtype=np.int64)
         self.N_k = nks
@@ -721,22 +727,50 @@ class DeviceMbarBatch(_Resident):
         check(self._lib.mbar_b200_batch_create(self.device, self.P, _i32p(self.K), _i64p(self.N), _dptr(Nk),
                                                _dptr(flat), C.byref(self._h)))
 
-    def moments(self, f_list, want_G=False, all_rows=False, problems=None):
+    def set_replicates(self, problems, counts):
+        """Replace the resident replicate slots: slot s holds the multiplicities counts[s] [N_p] of problem
+        problems[s] (a sequence of 1-D arrays, or one [S, N] array when every slot's problem has N samples).  Counts
+        lie in [0, 65535] (ValueError before anything changes) and sum to N_p; a bad problem index or sum raises the
+        library's error and leaves no slot.  Each slot's sum_n c_n x_n is computed once, here.  An empty `problems`
+        drops every slot."""
+        problems = np.ascontiguousarray(problems, dtype=np.int32).reshape(-1)
+        if len(counts) != problems.size:
+            raise ValueError(f"need one count vector per slot: {problems.size} problems, {len(counts)} count vectors")
+        parts = [np.asarray(c).reshape(-1) for c in counts]
+        for s, c in enumerate(parts):
+            if c.size and (c.min() < 0 or c.max() > 65535):
+                raise ValueError(f"slot {s}: replicate counts must lie in [0, 65535]")
+        flat = np.ascontiguousarray(np.concatenate(parts) if parts else np.zeros(0), dtype=np.uint16)
+        self.slot_problems = np.zeros(0, np.int32)
+        check(self._lib.mbar_b200_batch_set_replicates(self._h, problems.size, _i32p(problems),
+                                                       flat.ctypes.data_as(C.POINTER(C.c_uint16))))
+        self.slot_problems = problems
+
+    def moments(self, f_list, want_G=False, all_rows=False, problems=None, slots=None):
         """One dict per request (f_list[r] at problem problems[r], by default problem r): S [K_p], log_S [K_p],
         sum_L, flag and, with want_G, G = Ghat [K_p, K_p] (rows scaled by N_k; unsampled rows by 1 when all_rows,
-        0 otherwise).  Unsampled rows of S and log_S are filled only when all_rows."""
-        problems = np.ascontiguousarray(np.arange(len(f_list)) if problems is None else problems, dtype=np.int32)
-        if problems.shape != (len(f_list),) or len(f_list) == 0:
-            raise ValueError("need one problem index per f vector, and at least one")
-        Ks = [int(self.K[p]) if 0 <= p < self.P else -1 for p in problems]
+        0 otherwise).  Unsampled rows of S and log_S are filled only when all_rows.
+
+        slots: the requests name replicate slots instead (f_list[r] at slot slots[r], of problem
+        slot_problems[slots[r]]) and every sum counts sample n c_n times, with the same range flag.  All-ones counts
+        give the bits of the unweighted request."""
+        if slots is not None and problems is not None:
+            raise ValueError("a moments call names problems or slots, not both")
+        weighted = slots is not None
+        ids = np.ascontiguousarray(np.arange(len(f_list)) if not weighted and problems is None
+                                   else (slots if weighted else problems), dtype=np.int32)
+        if ids.shape != (len(f_list),) or len(f_list) == 0:
+            raise ValueError("need one problem or slot index per f vector, and at least one")
+        owner = self.slot_problems if weighted else np.arange(self.P)
+        Ks = [int(self.K[owner[i]]) if 0 <= i < len(owner) else -1 for i in ids]
         f = np.ascontiguousarray(np.concatenate([_f64(v, K) for v, K in zip(f_list, Ks)]))
         S, logS = np.empty(f.size), np.empty(f.size)
         sumL = np.empty(len(Ks))
         flag = np.empty(len(Ks), np.int32)
         G = np.empty(sum(K * K for K in Ks)) if want_G else None
-        check(self._lib.mbar_b200_batch_moments(self._h, len(Ks), _i32p(problems), _dptr(f), int(bool(all_rows)),
-                                                _dptr(S), _dptr(logS), _dptr(sumL), _i32p(flag),
-                                                _dptr(G) if want_G else None))
+        call = self._lib.mbar_b200_batch_replicate_moments if weighted else self._lib.mbar_b200_batch_moments
+        check(call(self._h, len(Ks), _i32p(ids), _dptr(f), int(bool(all_rows)), _dptr(S), _dptr(logS), _dptr(sumL),
+                   _i32p(flag), _dptr(G) if want_G else None))
         out, o, g = [], 0, 0
         for r, K in enumerate(Ks):
             d = dict(S=S[o:o + K], log_S=logS[o:o + K], sum_L=float(sumL[r]), flag=bool(flag[r]))
@@ -760,9 +794,27 @@ class DeviceMbarBatch(_Resident):
                                               float(gamma), _i32p(status), _i32p(iters)))
         return np.split(f, np.cumsum(self.K)[:-1]), status, iters
 
+    def solve_replicates(self, f_list, tol=1e-12, maxiter=10000, min_sc_iter=0, gamma=1.0):
+        """(f_list, status, iterations), one entry per replicate slot: the loop of `solve` (the same code, with slots
+        as its units) on every slot in lockstep from f_list[s] [K_p], with the same status codes.  Each iteration is
+        one weighted moments call for both candidates of every unfinished slot."""
+        S = self.slot_problems.size
+        Ks = [int(self.K[p]) for p in self.slot_problems]
+        if len(f_list) != S:
+            raise ValueError(f"need one f vector per slot ({S}), got {len(f_list)}")
+        status = np.empty(S, np.int32)
+        iters = np.empty(S, np.int32)
+        if S == 0:
+            return [], status, iters
+        f = np.ascontiguousarray(np.concatenate([_f64(v, K) for v, K in zip(f_list, Ks)]))
+        check(self._lib.mbar_b200_batch_solve_replicates(self._h, _dptr(f), float(tol), int(maxiter),
+                                                         int(min_sc_iter), float(gamma), _i32p(status),
+                                                         _i32p(iters)))
+        return np.split(f, np.cumsum(Ks)[:-1]), status, iters
+
     def last_stats(self):
-        """CUDA-event time (ms) of the last moments or solve call's kernels, its launches, iterations and the bytes of
-        u_kn tiles it read."""
+        """CUDA-event time (ms) of the last moments, solve or solve_replicates call's kernels, its launches,
+        iterations and the bytes of u_kn tiles (and replicate counts) it read."""
         ms, launches, iters, nbytes = C.c_double(0), C.c_int32(0), C.c_int32(0), C.c_int64(0)
         check(self._lib.mbar_b200_last_batch_stats(self._h, C.byref(ms), C.byref(launches), C.byref(iters),
                                                    C.byref(nbytes)))
