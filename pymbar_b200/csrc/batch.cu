@@ -23,8 +23,9 @@
 // sum L = sum_n c_n L'_n - sum_n c_n x_n, with L'_n itself unweighted (the denominators keep N_k).  It is the same
 // kernel instantiated with W = true; the unweighted instantiation compiles to the code it had before slots existed.
 // Multiplying by c_n = 1 is exact and the order of operations is the same in both instantiations, so all-ones counts
-// give the bits of the unweighted request.  A zero-count sample enters no sum: its a_kn is -inf before the warp max
-// of an unsampled row, as log c_n = -inf does in the single-problem pass.
+// give the bits of the unweighted request.  A zero-count sample enters no sum: its L'_n is not added to sum L and its
+// a_kn is -inf before the NaN test and the warp max of an unsampled row, as log c_n = -inf is in the single-problem
+// pass, so an undrawn sample whose sampled energies are all +inf does not flag its replicate.
 //
 // Determinism.  Work items are (request, chunk) pairs; a chunk is CT_p tiles with CT_p a function of (N_p, K_p) alone.
 // Warp w of a CTA takes the chunk's tiles w, w + 4, ... in order and folds each tile into its own (max, sum) pairs;
@@ -288,8 +289,11 @@ __global__ void __launch_bounds__(BATCH_THREADS) batch_moments_kernel(
             for (int k = 0; k < K; ++k)
                 if (sRow[k] == 1) D += exp(sC[k] - __ldg(ut + k * 32) - m);
             Lp = m + log(D);
-            if constexpr (W) sumL += cn * Lp;
-            else sumL += Lp;
+            if constexpr (W) {
+                if (cn != 0.0) sumL += cn * Lp;
+            } else {
+                sumL += Lp;
+            }
         }
         if (tileOn)
             for (int k = 0; k < K; ++k) {
@@ -298,12 +302,12 @@ __global__ void __launch_bounds__(BATCH_THREADS) batch_moments_kernel(
                     continue;
                 }
                 double a = valid ? sF[k] - __ldg(ut + k * 32) - Lp : -INFINITY;
+                if constexpr (W)
+                    if (cn == 0.0) a = -INFINITY;      // before the NaN test: an undrawn sample enters no sum
                 if (a != a) {
                     bad = true;
                     a = -INFINITY;
                 }
-                if constexpr (W)
-                    if (cn == 0.0) a = -INFINITY;
                 // sampled rows: e^a <= 1 / N_k, summed linearly (the pair keeps max 0) as the single-problem pass
                 // sums them; unsampled rows: shifted by the warp's max
                 const double wm = sRow[k] == 1 ? 0.0 : warp_max(a);
@@ -360,9 +364,11 @@ __global__ void __launch_bounds__(BATCH_THREADS) batch_moments_kernel(
 }
 
 // A request's chunk partials in chunk order -> its packed output.  The flag is set when a NaN reached a sum, when a
-// sampled row's S_k is outside (1e-280, 1e300) (the range the fused pass and the adaptive loop accept), or when an
-// unsampled row asked for has a NaN or overflowing S_k.  An unsampled row whose every weight is zero (all its
-// energies +inf) reports S_k = 0, log S_k = -inf, as the single-problem path does.
+// sampled row's S_k is outside (1e-280, 1e300) (the range the fused pass and the adaptive loop accept), when an
+// unsampled row asked for has a NaN or overflowing S_k, or, with the Gram, when an entry of Ghat is not finite: an
+// unsampled row's Gram weight e^{a_kn} is not shifted, so a weight above about e^355 overflows Ghat_kk while S_k is
+// still finite.  An unsampled row whose every weight is zero (all its energies +inf) reports S_k = 0,
+// log S_k = -inf, as the single-problem path does.
 __global__ void __launch_bounds__(BATCH_THREADS) batch_finalize_kernel(const BatchReq* __restrict__ req,
                                                                        const double* __restrict__ part,
                                                                        const double* __restrict__ NkAll,
@@ -406,6 +412,7 @@ __global__ void __launch_bounds__(BATCH_THREADS) batch_finalize_kernel(const Bat
             const int j = e - i * (i + 1) / 2;
             double g = 0.0;
             for (int64_t c = 0; c < nc; ++c) g += p0[c * stride + 2 * K + 2 + e];
+            if (!isfinite(g)) sFlag = 1;
             o[2 * K + 2 + (int64_t)i * K + j] = g;
             o[2 * K + 2 + (int64_t)j * K + i] = g;
         }

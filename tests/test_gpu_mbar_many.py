@@ -8,6 +8,7 @@ import pytest
 from pymbar_b200 import DeviceMbarBatch, DeviceProblem
 from pymbar_b200.mbar_many import mbar_many
 from tests import _mbar_many as H
+from tests._batch_edges import predict_flag
 from tests._moments import entry_tol, excess, moments_ld
 
 pytestmark = pytest.mark.gpu
@@ -69,6 +70,7 @@ def test_moments_against_long_double(which):
                 np.testing.assert_array_equal(d["G"], d2["G"])
                 np.testing.assert_array_equal(d["S"], d2["S"])
                 if d["flag"]:
+                    assert predict_flag(u, N_k, f, all_rows, True)[0], (len(N_k), u.shape[1])
                     continue
                 S, G, A = moments_ld(u, N_k, f, all_rows=all_rows)
                 rows = np.ones(len(N_k), bool) if all_rows else N_k > 0

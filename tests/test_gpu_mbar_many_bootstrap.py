@@ -10,6 +10,7 @@ from pymbar_b200 import DeviceMbarBatch, DeviceProblem, bootstrap
 from pymbar_b200 import mbar_many as mm
 from tests import _mbar_many as H
 from tests import _mbar_many_boot as W
+from tests._batch_edges import predict_flag
 from tests._moments import entry_tol, excess, moments_ld
 
 pytestmark = pytest.mark.gpu
@@ -59,6 +60,7 @@ def test_weighted_moments_against_long_double(which):
                 np.testing.assert_array_equal(d["S"], d2["S"])
                 assert d["sum_L"] == d2["sum_L"]
                 if d["flag"]:
+                    assert predict_flag(u, N_k, f, all_rows, True, counts=c)[0], (len(N_k), u.shape[1])
                     continue
                 checked += 1
                 S, G, A = moments_ld(u, N_k, f, mult=c, all_rows=all_rows)
