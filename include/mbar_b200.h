@@ -344,6 +344,17 @@ int mbar_b200_acf_inefficiency(mbar_b200_acf* acf, int64_t n_starts, const int64
                                int32_t mintime, int32_t rule, double navg, int64_t trace_cap, double* mean_a,
                                double* mean_b, double* sigma2, double* g, int64_t* last_lag, int32_t* status,
                                double* trace);
+/* Rule 0 of mbar_b200_acf_inefficiency for n requests on a segmented object (autocorrelation or cross): request r is
+ * series series[r] taken alone, from starts[r] counted from that series' first sample.  Every output of request r is
+ * bit for bit what mbar_b200_acf_inefficiency returns for that start on an unsegmented object holding series[r] alone:
+ * each series is cut into its own chunks of max(512, ceil(N_k / 1024)) samples, the lag launch covers only the
+ * (request, chunk) pairs a request reads, and the rounds (8, 8, 16, 32, ... lag indices, one host poll each) are shared
+ * by all active requests, each retired at its own limit.  n < 1 or n >= 2^31, a series index outside [0, K), a start
+ * outside [0, N_k) or an unsegmented object -> MBAR_B200_ERR_INVALID before anything runs.  mean_a, mean_b and sigma2
+ * may be NULL.  mbar_b200_last_acf_stats reports the call's rounds and terms. */
+int mbar_b200_acf_inefficiency_series(mbar_b200_acf* acf, int64_t n, const int32_t* series, const int64_t* starts,
+                                      int32_t fast, int32_t mintime, double* mean_a, double* mean_b, double* sigma2,
+                                      double* g, int64_t* last_lag, int32_t* status);
 /* C(t) for t = 0 .. n_max of one start (normalized_fluctuation_correlation_function), with its means and sigma^2.
  * n_max outside [0, T - start - 1], a segmented object or sigma^2 == 0 -> MBAR_B200_ERR_INVALID. */
 int mbar_b200_acf_correlation(mbar_b200_acf* acf, int64_t start, int64_t n_max, double* C, double* mean_a,

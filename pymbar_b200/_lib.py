@@ -92,6 +92,9 @@ SIGNATURES = {
     "mbar_b200_acf_inefficiency": (C.c_int, [_ctx, C.c_int64, C.POINTER(C.c_int64), C.c_int32, C.c_int32, C.c_int32,
                                              C.c_double, C.c_int64, _dp, _dp, _dp, _dp, C.POINTER(C.c_int64),
                                              C.POINTER(C.c_int32), _dp]),
+    "mbar_b200_acf_inefficiency_series": (C.c_int, [_ctx, C.c_int64, C.POINTER(C.c_int32), C.POINTER(C.c_int64),
+                                                    C.c_int32, C.c_int32, _dp, _dp, _dp, _dp, C.POINTER(C.c_int64),
+                                                    C.POINTER(C.c_int32)]),
     "mbar_b200_acf_correlation": (C.c_int, [_ctx, C.c_int64, C.c_int64, _dp, _dp, _dp, _dp]),
     "mbar_b200_acf_correlation_multiple": (C.c_int, [_ctx, C.c_int64, C.c_int32, _dp, C.POINTER(C.c_int64), _dp, _dp,
                                                      _dp]),

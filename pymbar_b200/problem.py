@@ -610,6 +610,23 @@ class DeviceAcf(_Resident):
             out["trace"] = trace
         return out
 
+    def inefficiency_series(self, series, starts, fast=False, mintime=3):
+        """`inefficiency` for requests on a segmented object: request r is series series[r] alone from starts[r]
+        (counted from that series' first sample), the same bits as `inefficiency([starts[r]])` on an object holding
+        that series alone.  dict of per-request arrays mean_a, mean_b, sigma2, g, last_lag, status."""
+        k = np.ascontiguousarray(np.atleast_1d(series), dtype=np.int32)
+        s = np.ascontiguousarray(np.atleast_1d(starts), dtype=np.int64)
+        if k.shape != s.shape or k.ndim != 1:
+            raise ValueError(f"series {k.shape} and starts {s.shape} must be matching 1-D arrays")
+        n = s.shape[0]
+        out = {key: np.empty(n) for key in ("mean_a", "mean_b", "sigma2", "g")}
+        out["last_lag"] = np.empty(n, np.int64)
+        out["status"] = np.empty(n, np.int32)
+        check(self._lib.mbar_b200_acf_inefficiency_series(
+            self._h, n, _i32p(k), _i64p(s), int(bool(fast)), int(mintime), _dptr(out["mean_a"]), _dptr(out["mean_b"]),
+            _dptr(out["sigma2"]), _dptr(out["g"]), _i64p(out["last_lag"]), _i32p(out["status"])))
+        return out
+
     def correlation(self, start, n_max):
         """(C [n_max + 1], mean_a, mean_b, sigma2) of the series from `start`."""
         Cn = np.empty(int(n_max) + 1)

@@ -21,6 +21,11 @@ direct lag sums up to the stop lag, which is the same C(t) in exact arithmetic a
 fp64.  Where the reference's answer is not reproducible (a constant remaining series, whose statsmodels acf divides
 rounding noise by rounding noise, or sigma^2 = 0) or the input is not a 1-D float64 or integer array, these raise
 `NotOnDevice`, and the facade calls the original.
+
+`detect_equilibration_many`, `statistical_inefficiency_many` and `subsample_correlated_data_many` return what a loop
+of the single-series functions returns, with every start of every series in one segmented device call per wave
+(DESIGN.md §3.5d′).  The single and many-series functions share their host halves (`_si_plan` / `_si_finish`,
+`_eq_plan` / `_EqPlan.finish`).
 """
 from __future__ import annotations
 
@@ -130,8 +135,9 @@ def neff(count, g32):
     return out
 
 
-def statistical_inefficiency(A_n, B_n=None, fast=False, mintime=3):
-    """statistical_inefficiency (timeseries.py:83-203) without fft: g >= 1 of one series, or of two."""
+def _si_plan(A_n, B_n, fast, mintime):
+    """statistical_inefficiency up to the device call: (a, b, None) with the float64 series the device answers, or
+    (None, None, [g]) where the host answers (a constant series; g None where sigma^2 == 0)."""
     A = np.array(A_n)
     B = None if B_n is None else np.array(B_n)
     if B is not None and A.shape != B.shape:
@@ -139,14 +145,29 @@ def statistical_inefficiency(A_n, B_n=None, fast=False, mintime=3):
     a = np.ascontiguousarray(A.ravel(), dtype=np.float64)
     b = None if B is None else np.ascontiguousarray(B.ravel(), dtype=np.float64)
     if _constant(a) or (b is not None and _constant(b)):
-        g = _host_inefficiency(A.ravel(), None if B is None else B.ravel(), fast, mintime)
-    else:
-        with _device(a, b) as dev:
-            r = dev.inefficiency([0], fast=fast, mintime=mintime)
-        g = None if r["status"][0] else float(r["g"][0])
+        return None, None, [_host_inefficiency(A.ravel(), None if B is None else B.ravel(), fast, mintime)]
+    return a, b, None
+
+
+def _si_finish(g):
+    """statistical_inefficiency's answer from g before the clamp (None: sigma^2 == 0)."""
     if g is None:
         raise _parameter_error("Sample covariance sigma_AB^2 = 0 -- cannot compute statistical inefficiency")
     return 1.0 if g < 1.0 else g
+
+
+def _device_g(r, k):
+    return None if r["status"][k] else float(r["g"][k])
+
+
+def statistical_inefficiency(A_n, B_n=None, fast=False, mintime=3):
+    """statistical_inefficiency (timeseries.py:83-203) without fft: g >= 1 of one series, or of two."""
+    a, b, host = _si_plan(A_n, B_n, fast, mintime)
+    if host is not None:
+        return _si_finish(host[0])
+    with _device(a, b) as dev:
+        r = dev.inefficiency([0], fast=fast, mintime=mintime)
+    return _si_finish(_device_g(r, 0))
 
 
 def _series_list(A_kn):
@@ -211,40 +232,63 @@ def normalized_fluctuation_correlation_function(A_n, B_n=None, N_max=None, norm=
     return C if norm else C * s2 + mu_a * mu_b
 
 
+class _EqPlan:
+    """detect_equilibration up to the device call: the starts, which of them go to the device (`on_dev`), and g /
+    sigma^2 == 0 (`zero`) of those answered on the host (a constant remaining series)."""
+
+    def __init__(self, A_t, fast, nskip):
+        T = self.T = A_t.size
+        self.a = np.ascontiguousarray(np.asarray(A_t).ravel(), dtype=np.float64)
+        a = self.a
+        self.g_t = np.ones([T - 1], np.float32)
+        self.starts = np.arange(0, T - 1, nskip, dtype=np.int64)
+        differs = np.flatnonzero(a != a[-1])
+        tail = int(differs[-1]) + 1 if differs.size else 0          # A[t:] is constant for t >= tail
+        self.g = np.ones(self.starts.size)
+        self.zero = np.zeros(self.starts.size, bool)
+        self.on_dev = self.starts < tail
+        exact = mean_is_exact(a[-1], T)
+        for k in np.flatnonzero(~self.on_dev):
+            t = int(self.starts[k])
+            gk = None if exact else _host_inefficiency(np.asarray(A_t).ravel()[t:T], None, fast, 3)
+            if gk is None:
+                self.zero[k] = True
+            else:
+                self.g[k] = gk
+
+    def finish(self, r=None):
+        """(t, g, Neff_max) from the device's answers r (a dict of g and status over starts[on_dev])."""
+        T, starts, g, zero, g_t = self.T, self.starts, self.g, self.zero, self.g_t
+        if r is not None:
+            g[self.on_dev] = r["g"]
+            zero[self.on_dev] = r["status"] != 0
+        Neff_t = np.ones([T - 1], np.float32)
+        g_t[starts] = np.where(g < 1.0, 1.0, g)
+        g_t[starts[zero]] = T - starts[zero] + 1
+        Neff_t[starts] = neff(T - starts + 1, g_t[starts])
+        Neff_max = Neff_t.max()
+        t = Neff_t.argmax()
+        return t, g_t[t], Neff_max
+
+
+def _eq_plan(A_t, fast, nskip):
+    """detect_equilibration's early answer (a series whose numpy std is 0) or its _EqPlan."""
+    if A_t.std() == 0.0:
+        return 0, 1, 1
+    return _EqPlan(A_t, fast, nskip)
+
+
 def detect_equilibration(A_t, fast=True, nskip=1):
     """detect_equilibration (timeseries.py:771-836): (t, g, Neff_max) as np.int64, np.float32, np.float32, every
     start in one device call."""
-    T = A_t.size
-    if A_t.std() == 0.0:
-        return 0, 1, 1
-    a = np.ascontiguousarray(np.asarray(A_t).ravel(), dtype=np.float64)
-    g_t = np.ones([T - 1], np.float32)
-    Neff_t = np.ones([T - 1], np.float32)
-    starts = np.arange(0, T - 1, nskip, dtype=np.int64)
-    differs = np.flatnonzero(a != a[-1])
-    tail = int(differs[-1]) + 1 if differs.size else 0          # A[t:] is constant for t >= tail
-    g = np.ones(starts.size)
-    zero = np.zeros(starts.size, bool)
-    on_dev = starts < tail
-    if on_dev.any():
-        with _device(a) as dev:
-            r = dev.inefficiency(starts[on_dev], fast=fast, mintime=3)
-        g[on_dev] = r["g"]
-        zero[on_dev] = r["status"] != 0
-    exact = mean_is_exact(a[-1], T)
-    for k in np.flatnonzero(~on_dev):
-        t = int(starts[k])
-        gk = None if exact else _host_inefficiency(np.asarray(A_t).ravel()[t:T], None, fast, 3)
-        if gk is None:
-            zero[k] = True
-        else:
-            g[k] = gk
-    g_t[starts] = np.where(g < 1.0, 1.0, g)
-    g_t[starts[zero]] = T - starts[zero] + 1
-    Neff_t[starts] = neff(T - starts + 1, g_t[starts])
-    Neff_max = Neff_t.max()
-    t = Neff_t.argmax()
-    return t, g_t[t], Neff_max
+    plan = _eq_plan(A_t, fast, nskip)
+    if isinstance(plan, tuple):
+        return plan
+    r = None
+    if plan.on_dev.any():
+        with _device(plan.a) as dev:
+            r = dev.inefficiency(plan.starts[plan.on_dev], fast=fast, mintime=3)
+    return plan.finish(r)
 
 
 def normalized_fluctuation_correlation_function_multiple(A_kn, B_kn=None, N_max=None, norm=True, truncate=False):
@@ -346,3 +390,154 @@ def detect_equilibration_binary_search(A_t, bs_nodes=10):
                 start = time_grid[k - 1]
                 end = time_grid[k + 1]
     return t, g, Neff_max
+
+
+# ---- many series in lockstep ----------------------------------------------------------------------------------------
+# The _many functions return what a list comprehension over the single-series function returns, and raise the
+# exception of the lowest-index failing series.  Every device request (series, start) of every series goes to one
+# segmented DeviceAcf and its `inefficiency_series`, whose answers are the single-series call's bits; requests go in
+# waves of at most WAVE_BYTES // REQUEST_BYTES, which changes no bits.  A series that cannot be a segment (empty, or
+# with a non-finite value) is answered by the single-series function, so that its own error is the one raised.
+
+WAVE_BYTES = 1 << 30        # device footprint of the requests of one inefficiency_series call
+REQUEST_BYTES = 96          # device bytes per request (starts, series, means, sigma^2, g, last lag, status, order)
+LAST_MANY_STATS = {}        # waves, rounds, kernel ms, lag terms and requests of the last _many device work
+
+
+def _segmentable(a, b):
+    return a.size > 0 and bool(np.all(np.isfinite(a))) and (b is None or bool(np.all(np.isfinite(b))))
+
+
+def _many_requests(series, cross, ser, starts, fast, mintime):
+    """(g, status) of requests (series ser[r], start starts[r]) over the float64 series [(a, b)], one segmented
+    DeviceAcf (autocorrelation, or cross when `cross`) and one inefficiency_series call per wave."""
+    n = ser.size
+    g = np.empty(n)
+    status = np.empty(n, np.int32)
+    a = np.concatenate([x for x, _ in series])
+    b = np.concatenate([y for _, y in series]) if cross else None
+    lengths = np.array([x.size for x, _ in series], np.int64)
+    per = max(1, int(WAVE_BYTES) // REQUEST_BYTES)
+    st = LAST_MANY_STATS
+    with _device(a, b, lengths=lengths) as dev:
+        for w0 in range(0, n, per):
+            r = dev.inefficiency_series(ser[w0:w0 + per], starts[w0:w0 + per], fast=fast, mintime=mintime)
+            g[w0:w0 + per] = r["g"]
+            status[w0:w0 + per] = r["status"]
+            s = dev.last_stats() if hasattr(dev, "last_stats") else {}
+            st["waves"] = st.get("waves", 0) + 1
+            for k in ("rounds", "ms", "terms"):
+                st[k] = st.get(k, 0) + s.get(k, 0)
+    st["requests"] = st.get("requests", 0) + n
+    return g, status
+
+
+def _raise_lowest(errors):
+    if errors:
+        raise errors[min(errors)]
+
+
+def statistical_inefficiency_many(A_list, B_list=None, fast=False, mintime=3):
+    """`statistical_inefficiency(A_list[i], B_list[i], fast, mintime)` for every series: a float64 array of g >= 1,
+    every device series in one call per wave (autocorrelations and cross-correlations in one object each)."""
+    LAST_MANY_STATS.clear()
+    n = len(A_list)
+    if B_list is not None and len(B_list) != n:
+        raise ValueError(f"{n} series A but {len(B_list)} series B")
+    out = np.ones(n)
+    errors = {}
+    groups = {False: [], True: []}                 # cross -> [(i, a, b)]
+    for i in range(n):
+        B_i = None if B_list is None else B_list[i]
+        try:
+            a, b, host = _si_plan(A_list[i], B_i, fast, mintime)
+            if host is not None:
+                out[i] = _si_finish(host[0])
+            elif not _segmentable(a, b):
+                out[i] = statistical_inefficiency(A_list[i], B_i, fast, mintime)
+            else:
+                groups[b is not None].append((i, a, b))
+        except Exception as e:                  # noqa: BLE001  (re-raised below, lowest index first)
+            errors[i] = e
+            break                               # the series after it cannot change what is raised
+    first = min(errors) if errors else n
+    for cross, items in groups.items():
+        items = [x for x in items if x[0] < first]
+        if not items:
+            continue
+        k = np.arange(len(items), dtype=np.int32)
+        g, status = _many_requests([(a, b) for _, a, b in items], cross, k, np.zeros(k.size, np.int64), fast,
+                                   mintime)
+        for (i, _, _), gi, si in zip(items, g, status):
+            try:
+                out[i] = _si_finish(None if si else float(gi))
+            except Exception as e:              # noqa: BLE001
+                errors[i] = e
+    _raise_lowest(errors)
+    return out
+
+
+def detect_equilibration_many(A_list, fast=True, nskip=1):
+    """`detect_equilibration(A, fast, nskip)` for every series: a list of (t, g, Neff_max), every start of every series
+    in one device call per wave, with the lag rounds shared by all series."""
+    LAST_MANY_STATS.clear()
+    n = len(A_list)
+    out = [None] * n
+    errors = {}
+    plans = []                                  # (i, plan) of the series with device starts
+    for i in range(n):
+        try:
+            plan = _eq_plan(A_list[i], fast, nskip)
+            if isinstance(plan, tuple):
+                out[i] = plan
+            elif not plan.on_dev.any():
+                out[i] = plan.finish()
+            elif not _segmentable(plan.a, None):
+                out[i] = detect_equilibration(A_list[i], fast, nskip)
+            else:
+                plans.append((i, plan))
+        except Exception as e:                  # noqa: BLE001  (re-raised below, lowest index first)
+            errors[i] = e
+            break
+    if plans:
+        counts = np.array([int(p.on_dev.sum()) for _, p in plans], np.int64)
+        ser = np.repeat(np.arange(len(plans), dtype=np.int32), counts)
+        starts = np.concatenate([p.starts[p.on_dev] for _, p in plans])
+        g, status = _many_requests([(p.a, None) for _, p in plans], False, ser, starts, fast, 3)
+        off = np.concatenate([[0], np.cumsum(counts)])
+        for k, (i, p) in enumerate(plans):
+            out[i] = p.finish(dict(g=g[off[k]:off[k + 1]], status=status[off[k]:off[k + 1]]))
+    _raise_lowest(errors)
+    return out
+
+
+def _subsample_indices(T, g, conservative):
+    """The indices subsample_correlated_data keeps of T samples for a statistical inefficiency g: stride ceil(g) when
+    conservative, else round(n g) for n = 0, 1, 2, ... while below T, each index once."""
+    if conservative:
+        return list(range(0, T, int(math.ceil(g))))
+    if not g > 0:
+        raise ValueError(f"g = {g!r}: the indices round(n g) never reach T")
+    # n g as Python evaluates it for a scalar g: float64, or g's own precision for a numpy float
+    dtype = g.dtype if isinstance(g, np.floating) else np.float64
+    n = np.arange(int(math.floor((T + 0.5) / float(g))) + 2).astype(dtype)
+    t = np.round(n * g)
+    t = t[t < T]
+    return np.unique(t).astype(np.int64).tolist()
+
+
+def subsample_correlated_data_many(A_list, g=None, fast=False, conservative=False):
+    """`pymbar.timeseries.subsample_correlated_data(A_list[i], g_i, fast, conservative)` for every series: one index
+    list per series.  g is None, one value for every series or one value per series; the series whose g is falsy get
+    g from one statistical_inefficiency_many call (the reference's statistical_inefficiency(A, A, fast): a
+    cross-correlation of a series with itself is its autocorrelation, bit for bit)."""
+    A = [np.array(x) for x in A_list]
+    n = len(A)
+    gs = [g] * n if g is None or np.ndim(g) == 0 else list(g)
+    if len(gs) != n:
+        raise ValueError(f"{len(gs)} values of g for {n} series")
+    need = [i for i in range(n) if not gs[i]]
+    if need:
+        for i, gi in zip(need, statistical_inefficiency_many([A[i] for i in need], fast=fast)):
+            gs[i] = float(gi)
+    return [_subsample_indices(A[i].size, gs[i], conservative) for i in range(n)]
