@@ -47,14 +47,13 @@ constexpr int64_t ACF_PART_BUDGET = int64_t(1) << 25;   // doubles of (request, 
 inline int64_t acf_chunk_size(int64_t N) { return std::max<int64_t>(ACF_MIN_NC, (N + ACF_MAX_CHUNKS - 1) / ACF_MAX_CHUNKS); }
 
 // The chunks of a list of series: series k is [off[k], off[k + 1]), cut into its chunks [chunkOff[k], chunkOff[k + 1])
-// of NC[k] samples; chunk c is [lo[c], hi[c]) and its series ends at end[c].
-// On the device the six arrays sit in one buffer, d_all (one upload).
+// of NC[k] samples; chunk c is [lo[c], hi[c]).
+// On the device the five arrays sit in one buffer, d_all (one upload).
 struct AcfGrid {
     int K = 0;
-    std::vector<int64_t> off, NC, chunkOff, lo, hi, end;
+    std::vector<int64_t> off, NC, chunkOff, lo, hi;
     DevArray<int64_t> d_all;
-    const int64_t *d_off = nullptr, *d_NC = nullptr, *d_chunkOff = nullptr, *d_lo = nullptr, *d_hi = nullptr,
-                  *d_end = nullptr;
+    const int64_t *d_off = nullptr, *d_NC = nullptr, *d_chunkOff = nullptr, *d_lo = nullptr, *d_hi = nullptr;
     int64_t nChunks() const { return (int64_t)lo.size(); }
 };
 
@@ -66,14 +65,12 @@ inline void acf_grid(const int64_t* lengths, int K, AcfGrid& g) {
     g.chunkOff.assign((size_t)K + 1, 0);
     g.lo.clear();
     g.hi.clear();
-    g.end.clear();
     for (int k = 0; k < K; ++k) {
         const int64_t L = lengths[k], o = g.off[k];
         g.NC[k] = acf_chunk_size(L);
         for (int64_t x = 0; x < L; x += g.NC[k]) {
             g.lo.push_back(o + x);
             g.hi.push_back(o + std::min(L, x + g.NC[k]));
-            g.end.push_back(o + L);
         }
         g.off[k + 1] = o + L;
         g.chunkOff[k + 1] = (int64_t)g.lo.size();
@@ -344,24 +341,46 @@ __global__ void acf_corr_kernel(const double* __restrict__ S, const int64_t* __r
 // Lag sums of the call requests act_h[] (indices into the call's starts) for the ascending lags lags_h[], into
 // d_S [nAct][ldS] at columns col0.. (row k of d_S: act_h[k]).  Orders the requests by chunk count, largest first, and
 // splits lags and requests so that one launch's partials, counted over each request's own chunks, fit the budget.
+// alloc() makes the device arrays of a call: the requests' starts and series (uploaded), their means (the caller
+// computes them) and room for lag batches of up to lagCap lags.
 struct AcfLagRunner {
     mbar_b200_acf* o;
     const AcfGrid* grid;
-    AcfSeries v;
+    bool cross;                 // the symmetrised term dA[n] dB[n + t] + dB[n] dA[n + t]; else dA[n] dB[n + t] alone
     bool seg;                   // bound the terms by the segment of n (rule 1 on the whole-object grid)
     const int64_t* hs;          // [call requests] host starts and series (NULL: series 0)
     const int32_t* hser;
-    const int64_t* d_starts;
-    const double* d_muA;
-    const double* d_muB;
-    int32_t* d_act;       // [capacity] act_h as given (the walk kernel reads it)
-    int32_t* d_sact;      // [2 capacity] act_h ordered by chunk count, then the d_S row of each entry (if reordered)
-    int64_t* d_lags;      // [capacity]
-    int64_t* d_rowOff;    // [ACF_MAX_CHUNKS + 1]
-    double* d_partial;    // [partCap]
-    int64_t partCap;
+    AcfSeries v{};
+    int64_t* d_starts = nullptr;
+    double* d_muA = nullptr;
+    double* d_muB = nullptr;
+    int32_t* d_act = nullptr;       // [n] act_h as given (the walk kernel reads it)
+    int32_t* d_sact = nullptr;      // [2 n] act_h ordered by chunk count, then the d_S row of each entry
+    int64_t* d_lags = nullptr;      // [lagCap]
+    int64_t* d_rowOff = nullptr;    // [ACF_MAX_CHUNKS + 1]
+    double* d_partial = nullptr;    // [partCap]
+    int64_t partCap = 0;
     std::vector<int32_t> sact;       // [2 nAct]: order, then rows
     std::vector<int64_t> cnt, rowOff, bucket;
+
+    int alloc(CallBuffers& buf, int64_t n, int64_t lagCap, int64_t partCap_) {
+        int32_t* d_ser = nullptr;
+        MBAR_TRY(buf.alloc(&d_starts, (size_t)n));
+        if (hser) MBAR_TRY(buf.alloc(&d_ser, (size_t)n));
+        MBAR_TRY(buf.alloc(&d_muA, (size_t)n));
+        MBAR_TRY(buf.alloc(&d_muB, (size_t)n));
+        MBAR_TRY(buf.alloc(&d_act, 3 * (size_t)n));
+        MBAR_TRY(buf.alloc(&d_lags, (size_t)lagCap + ACF_MAX_CHUNKS + 1));
+        MBAR_TRY(buf.alloc(&d_partial, (size_t)partCap_));
+        d_sact = d_act + n;
+        d_rowOff = d_lags + lagCap;
+        partCap = partCap_;
+        v = AcfSeries{grid->d_off, grid->d_NC, grid->d_chunkOff, d_ser};
+        MBAR_CUDA(cudaMemcpyAsync(d_starts, hs, (size_t)n * sizeof(int64_t), cudaMemcpyHostToDevice, o->stream));
+        if (hser)
+            MBAR_CUDA(cudaMemcpyAsync(d_ser, hser, (size_t)n * sizeof(int32_t), cudaMemcpyHostToDevice, o->stream));
+        return MBAR_B200_OK;
+    }
 
     int64_t count(int32_t j) const {
         const int k = hser ? hser[j] : 0;
@@ -443,7 +462,7 @@ struct AcfLagRunner {
                 p.rows = rows;
                 p.nLags = nl;
                 p.LG = (nl + ACF_RL - 1) / ACF_RL;
-                if (o->cross) {
+                if (cross) {
                     if (seg) launch<true, true>(p, items);
                     else launch<true, false>(p, items);
                 } else {
@@ -514,7 +533,7 @@ int mbar_b200_acf_create(int device, int64_t T, const double* a, const double* b
     o->d_b = b ? o->d_bOwn : o->d_a;
     auto uploadGrid = [&](AcfGrid& g) -> int {
         std::vector<int64_t> all;
-        for (const std::vector<int64_t>* v : {&g.off, &g.NC, &g.chunkOff, &g.lo, &g.hi, &g.end})
+        for (const std::vector<int64_t>* v : {&g.off, &g.NC, &g.chunkOff, &g.lo, &g.hi})
             all.insert(all.end(), v->begin(), v->end());
         MBAR_TRY(o->upload(g.d_all, all.data(), all.size(), who));
         g.d_off = g.d_all;
@@ -522,7 +541,6 @@ int mbar_b200_acf_create(int device, int64_t T, const double* a, const double* b
         g.d_chunkOff = g.d_NC + g.NC.size();
         g.d_lo = g.d_chunkOff + g.chunkOff.size();
         g.d_hi = g.d_lo + g.lo.size();
-        g.d_end = g.d_hi + g.hi.size();
         return MBAR_B200_OK;
     };
     acf_grid(&T, 1, o->whole);
@@ -545,9 +563,9 @@ int mbar_b200_acf_create(int device, int64_t T, const double* a, const double* b
 
 int mbar_b200_acf_destroy(mbar_b200_acf* o) { return destroy_resident(o); }
 
-// means and sigma^2 of the call's requests (device arrays d_starts [n]); done[j] = 1 where sigma^2 == 0
-static int acf_moments(mbar_b200_acf* o, CallBuffers& buf, const int64_t* d_starts, int64_t n, AcfLagRunner& run,
-                       double* d_muA, double* d_muB, double* d_s2, int32_t* d_status, int8_t* d_done) {
+// means (into the runner's) and sigma^2 of the call's n requests; done[j] = 1 where sigma^2 == 0
+static int acf_moments(mbar_b200_acf* o, CallBuffers& buf, int64_t n, AcfLagRunner& run, double* d_s2,
+                       int32_t* d_status, int8_t* d_done) {
     const AcfGrid& grid = *run.grid;
     const int64_t nc = grid.nChunks();
     double *d_totA, *d_totB, *d_S0;
@@ -557,14 +575,14 @@ static int acf_moments(mbar_b200_acf* o, CallBuffers& buf, const int64_t* d_star
     acf_total_kernel<<<(unsigned)((nc + 127) / 128), 128, 0, o->stream>>>(o->d_a, o->d_b, grid.d_lo, grid.d_hi, nc,
                                                                         d_totA, d_totB);
     acf_mean_kernel<<<(unsigned)((n + 127) / 128), 128, 0, o->stream>>>(o->d_a, o->d_b, run.v, d_totA, d_totB,
-                                                                      d_starts, n, d_muA, d_muB);
+                                                                      run.d_starts, n, run.d_muA, run.d_muB);
     MBAR_CUDA(cudaGetLastError());
     std::vector<int32_t> all((size_t)n);
     for (int64_t j = 0; j < n; ++j) all[j] = (int32_t)j;
     const int64_t zero = 0;
     MBAR_TRY(run.run(all.data(), (int)n, &zero, 1, d_S0, 1));
-    acf_sigma_kernel<<<(unsigned)((n + 127) / 128), 128, 0, o->stream>>>(d_S0, run.v, d_starts, n, o->cross, d_s2,
-                                                                       d_status, d_done);
+    acf_sigma_kernel<<<(unsigned)((n + 127) / 128), 128, 0, o->stream>>>(d_S0, run.v, run.d_starts, n, o->cross,
+                                                                       d_s2, d_status, d_done);
     MBAR_CUDA(cudaGetLastError());
     return MBAR_B200_OK;
 }
@@ -587,28 +605,19 @@ static int acf_run(mbar_b200_acf* o, const AcfGrid& grid, int64_t n, const int64
     for (int64_t j = 0; j < n; ++j)
         maxLimit = std::max(maxLimit, rule == 1 ? limitMultiple : lenOf(j) - hs[j] + (rule == 2 ? 1 : 0));
     CallBuffers buf("acf");
-    int64_t* d_starts;
-    double *d_muA, *d_muB, *d_s2, *d_g, *d_S, *d_partial, *d_trace = nullptr;
-    int64_t *d_last, *d_lags;
-    int32_t *d_status, *d_act, *d_ser = nullptr;
+    double *d_s2, *d_g, *d_S, *d_trace = nullptr;
+    int64_t* d_last;
+    int32_t* d_status;
     int8_t* d_done;
     // the largest round: every request active, one batch of B lags; keep the [active][B] sums within the budget by
     // walking the requests in groups
     const int64_t partCap = std::min<int64_t>(ACF_PART_BUDGET, grid.nChunks() * std::max<int64_t>(n, 1) * 4096);
-    MBAR_TRY(buf.alloc(&d_starts, (size_t)n));
-    if (ser) MBAR_TRY(buf.alloc(&d_ser, (size_t)n));
-    MBAR_TRY(buf.alloc(&d_muA, (size_t)n));
-    MBAR_TRY(buf.alloc(&d_muB, (size_t)n));
     MBAR_TRY(buf.alloc(&d_s2, (size_t)n));
     MBAR_TRY(buf.alloc(&d_g, (size_t)n));
     MBAR_TRY(buf.alloc(&d_last, (size_t)n));
     MBAR_TRY(buf.alloc(&d_status, (size_t)n));
     MBAR_TRY(buf.alloc(&d_done, (size_t)n));
-    MBAR_TRY(buf.alloc(&d_act, 3 * (size_t)n));            // act, then the runner's order and rows
-    MBAR_TRY(buf.alloc(&d_partial, (size_t)partCap));
     if (trace_cap > 0) MBAR_TRY(buf.alloc(&d_trace, (size_t)(n * trace_cap)));
-    MBAR_CUDA(cudaMemcpyAsync(d_starts, hs.data(), (size_t)n * sizeof(int64_t), cudaMemcpyHostToDevice, o->stream));
-    if (ser) MBAR_CUDA(cudaMemcpyAsync(d_ser, ser, (size_t)n * sizeof(int32_t), cudaMemcpyHostToDevice, o->stream));
     if (d_trace) MBAR_CUDA(cudaMemsetAsync(d_trace, 0xff, (size_t)(n * trace_cap) * sizeof(double), o->stream));
     std::vector<double> ones((size_t)n, 1.0);
     std::vector<int64_t> zeros((size_t)n, 0);
@@ -625,12 +634,10 @@ static int acf_run(mbar_b200_acf* o, const AcfGrid& grid, int64_t n, const int64
     }
     const int64_t walkCap = std::max<int64_t>(Bmax, std::min<int64_t>(n * Bmax, ACF_PART_BUDGET / 4));
     MBAR_TRY(buf.alloc(&d_S, (size_t)walkCap));
-    MBAR_TRY(buf.alloc(&d_lags, (size_t)Bmax + 1 + ACF_MAX_CHUNKS + 1));   // lags, then the row offsets
-    const AcfSeries v{grid.d_off, grid.d_NC, grid.d_chunkOff, d_ser};
-    AcfLagRunner run{o, &grid, v, rule == 1, hs.data(), ser, d_starts, d_muA, d_muB, d_act, d_act + n, d_lags,
-                     d_lags + Bmax + 1, d_partial, partCap};
+    AcfLagRunner run{o, &grid, o->cross != 0, rule == 1, hs.data(), ser};
+    MBAR_TRY(run.alloc(buf, n, Bmax + 1, partCap));
     MBAR_CUDA(cudaEventRecord(o->ev0, o->stream));
-    MBAR_TRY(acf_moments(o, buf, d_starts, n, run, d_muA, d_muB, d_s2, d_status, d_done));
+    MBAR_TRY(acf_moments(o, buf, n, run, d_s2, d_status, d_done));
     std::vector<int8_t> done((size_t)n);
     MBAR_CUDA(cudaMemcpyAsync(done.data(), d_done, (size_t)n, cudaMemcpyDeviceToHost, o->stream));
     MBAR_CUDA(cudaStreamSynchronize(o->stream));
@@ -663,12 +670,12 @@ static int acf_run(mbar_b200_acf* o, const AcfGrid& grid, int64_t n, const int64
         for (size_t a0 = 0; a0 < active.size(); a0 += groupMax) {
             const int na = (int)std::min<size_t>(groupMax, active.size() - a0);
             if (nl > 0) MBAR_TRY(run.run(active.data() + a0, na, lags.data(), nl, d_S, nl));
-            else MBAR_CUDA(cudaMemcpyAsync(d_act, active.data() + a0, (size_t)na * sizeof(int32_t),
+            else MBAR_CUDA(cudaMemcpyAsync(run.d_act, active.data() + a0, (size_t)na * sizeof(int32_t),
                                            cudaMemcpyHostToDevice, o->stream));
             AcfWalkParams w{};
-            w.v = v;
-            w.starts = d_starts;
-            w.act = d_act;
+            w.v = run.v;
+            w.starts = run.d_starts;
+            w.act = run.d_act;
             w.S = d_S;
             w.sigma2 = d_s2;
             w.segLen = o->d_segLen;
@@ -704,8 +711,10 @@ static int acf_run(mbar_b200_acf* o, const AcfGrid& grid, int64_t n, const int64
         if (rounds > 1) B *= 2;
     }
     MBAR_CUDA(cudaEventRecord(o->ev1, o->stream));
-    if (mean_a) MBAR_CUDA(cudaMemcpyAsync(mean_a, d_muA, (size_t)n * sizeof(double), cudaMemcpyDeviceToHost, o->stream));
-    if (mean_b) MBAR_CUDA(cudaMemcpyAsync(mean_b, d_muB, (size_t)n * sizeof(double), cudaMemcpyDeviceToHost, o->stream));
+    if (mean_a)
+        MBAR_CUDA(cudaMemcpyAsync(mean_a, run.d_muA, (size_t)n * sizeof(double), cudaMemcpyDeviceToHost, o->stream));
+    if (mean_b)
+        MBAR_CUDA(cudaMemcpyAsync(mean_b, run.d_muB, (size_t)n * sizeof(double), cudaMemcpyDeviceToHost, o->stream));
     if (sigma2) MBAR_CUDA(cudaMemcpyAsync(sigma2, d_s2, (size_t)n * sizeof(double), cudaMemcpyDeviceToHost, o->stream));
     MBAR_CUDA(cudaMemcpyAsync(g, d_g, (size_t)n * sizeof(double), cudaMemcpyDeviceToHost, o->stream));
     MBAR_CUDA(cudaMemcpyAsync(last_lag, d_last, (size_t)n * sizeof(int64_t), cudaMemcpyDeviceToHost, o->stream));
@@ -800,30 +809,21 @@ int mbar_b200_acf_correlation(mbar_b200_acf* o, int64_t start, int64_t n_max, do
     MBAR_CUDA(cudaSetDevice(o->device));
     NvtxRange nvtx_("mbar_b200::acf_correlation");
     CallBuffers buf("acf");
-    int64_t *d_starts, *d_lags;
-    double *d_muA, *d_muB, *d_s2, *d_S, *d_C, *d_partial;
-    int32_t *d_status, *d_act;
+    double *d_s2, *d_S, *d_C;
+    int32_t* d_status;
     int8_t* d_done;
     const int64_t nl = n_max + 1;
     const int64_t batch = std::min<int64_t>(nl, 1 << 20);
     const int64_t partCap = std::min<int64_t>(ACF_PART_BUDGET, o->nChunks * batch);
-    MBAR_TRY(buf.alloc(&d_starts, 1));
-    MBAR_TRY(buf.alloc(&d_muA, 1));
-    MBAR_TRY(buf.alloc(&d_muB, 1));
     MBAR_TRY(buf.alloc(&d_s2, 1));
     MBAR_TRY(buf.alloc(&d_status, 1));
     MBAR_TRY(buf.alloc(&d_done, 1));
-    MBAR_TRY(buf.alloc(&d_act, 3));                        // act, then the runner's order and row
-    MBAR_TRY(buf.alloc(&d_lags, (size_t)batch + ACF_MAX_CHUNKS + 1));   // lags, then the row offsets
     MBAR_TRY(buf.alloc(&d_S, (size_t)batch));
     MBAR_TRY(buf.alloc(&d_C, (size_t)nl));
-    MBAR_TRY(buf.alloc(&d_partial, (size_t)partCap));
-    MBAR_CUDA(cudaMemcpyAsync(d_starts, &start, sizeof(int64_t), cudaMemcpyHostToDevice, o->stream));
-    const AcfSeries v{o->whole.d_off, o->whole.d_NC, o->whole.d_chunkOff, nullptr};
-    AcfLagRunner run{o, &o->whole, v, false, &start, nullptr, d_starts, d_muA, d_muB, d_act, d_act + 1, d_lags,
-                     d_lags + batch, d_partial, partCap};
+    AcfLagRunner run{o, &o->whole, o->cross != 0, false, &start, nullptr};
+    MBAR_TRY(run.alloc(buf, 1, batch, partCap));
     MBAR_CUDA(cudaEventRecord(o->ev0, o->stream));
-    MBAR_TRY(acf_moments(o, buf, d_starts, 1, run, d_muA, d_muB, d_s2, d_status, d_done));
+    MBAR_TRY(acf_moments(o, buf, 1, run, d_s2, d_status, d_done));
     double s2 = 0.0;
     MBAR_CUDA(cudaMemcpyAsync(&s2, d_s2, sizeof(double), cudaMemcpyDeviceToHost, o->stream));
     MBAR_CUDA(cudaStreamSynchronize(o->stream));
@@ -835,15 +835,15 @@ int mbar_b200_acf_correlation(mbar_b200_acf* o, int64_t start, int64_t n_max, do
         lags.resize((size_t)b);
         for (int64_t k = 0; k < b; ++k) lags[k] = l0 + k;
         MBAR_TRY(run.run(&act0, 1, lags.data(), (int)b, d_S, (int)b));
-        acf_corr_kernel<<<(unsigned)((b + 255) / 256), 256, 0, o->stream>>>(d_S, d_lags, (int)b, o->T - start,
+        acf_corr_kernel<<<(unsigned)((b + 255) / 256), 256, 0, o->stream>>>(d_S, run.d_lags, (int)b, o->T - start,
                                                                            o->cross, d_s2, d_C + l0);
         MBAR_CUDA(cudaGetLastError());
         MBAR_CUDA(cudaStreamSynchronize(o->stream));   // d_lags is rewritten by the next batch
     }
     MBAR_CUDA(cudaEventRecord(o->ev1, o->stream));
     MBAR_CUDA(cudaMemcpyAsync(C, d_C, (size_t)nl * sizeof(double), cudaMemcpyDeviceToHost, o->stream));
-    if (mean_a) MBAR_CUDA(cudaMemcpyAsync(mean_a, d_muA, sizeof(double), cudaMemcpyDeviceToHost, o->stream));
-    if (mean_b) MBAR_CUDA(cudaMemcpyAsync(mean_b, d_muB, sizeof(double), cudaMemcpyDeviceToHost, o->stream));
+    if (mean_a) MBAR_CUDA(cudaMemcpyAsync(mean_a, run.d_muA, sizeof(double), cudaMemcpyDeviceToHost, o->stream));
+    if (mean_b) MBAR_CUDA(cudaMemcpyAsync(mean_b, run.d_muB, sizeof(double), cudaMemcpyDeviceToHost, o->stream));
     if (sigma2) MBAR_CUDA(cudaMemcpyAsync(sigma2, d_s2, sizeof(double), cudaMemcpyDeviceToHost, o->stream));
     MBAR_CUDA(cudaStreamSynchronize(o->stream));
     float e = 0.f;
@@ -856,16 +856,17 @@ int mbar_b200_acf_correlation(mbar_b200_acf* o, int64_t start, int64_t n_max, do
 }
 
 // ---- normalized_fluctuation_correlation_function_multiple (timeseries.py:509-658) ----------------------------------
-// Series k of a segmented object (offset o_k, length L_k) is cut into its own chunks of max(512, ceil(L_k / 1024))
-// samples (the object's segment grid, acf_grid): no chunk straddles two series and the bounds depend on the lengths
-// alone.  The sum of a (series, lag) is
-// 0.0 + its chunk partials in order, and a lag's numerator 0.0 + those sums in list order, as the reference adds one
-// np.sum per series; the pooled means are the same construction.
+// Request k is series k of the object's segment grid from start 0, with the pooled means in its mean slots, and its
+// lag sums are the runner's one-sided dA[n] dB[n + t] (on a cross object too): the reference's np.sum of series k.
+// A lag's numerator is 0.0 + those sums in list order, as the reference adds one np.sum per series; the pooled means
+// are the same construction over the chunk totals.
 namespace mbar {
 
-// pooled means (one thread): each series' chunk totals in order, the series in list order, over N
-__global__ void acf_seg_mean_kernel(const double* __restrict__ totA, const double* __restrict__ totB,
-                                    const int64_t* __restrict__ chunkOff, int K, int64_t N, double* mu) {
+// pooled means (one thread): each series' chunk totals in order, the series in list order, over N; written to every
+// request's slot
+__global__ void acf_pooled_mean_kernel(const double* __restrict__ totA, const double* __restrict__ totB,
+                                       const int64_t* __restrict__ chunkOff, int K, int64_t N, double* muA,
+                                       double* muB) {
     if (blockIdx.x != 0 || threadIdx.x != 0) return;
     double pa = 0.0, pb = 0.0;
     for (int k = 0; k < K; ++k) {
@@ -877,76 +878,34 @@ __global__ void acf_seg_mean_kernel(const double* __restrict__ totA, const doubl
         pa = __dadd_rn(pa, sa);
         pb = __dadd_rn(pb, sb);
     }
-    mu[0] = __ddiv_rn(pa, (double)N);
-    mu[1] = __ddiv_rn(pb, (double)N);
+    const double ma = __ddiv_rn(pa, (double)N), mb = __ddiv_rn(pb, (double)N);
+    for (int k = 0; k < K; ++k) {
+        muA[k] = ma;
+        muB[k] = mb;
+    }
 }
 
-struct AcfSegParams {
-    const double* a;
-    const double* b;
-    const int64_t* lo;          // [nChunks] chunk bounds
-    const int64_t* hi;
-    const int64_t* end;         // [nChunks] end of the chunk's series
-    const double* mu;           // [2] pooled means
-    double* partial;            // [nChunks][nLags]
-    int64_t l0;                 // lags l0 .. l0 + nLags - 1
-    int nLags, LG;
-};
-
-// partial[c][jl] = 0.0 + sum over the chunk's n with n + t in its series of dA[n] dB[n + t], t = l0 + jl; one thread
-// per ACF_RL consecutive lags, one chunk per blockIdx.x
-__global__ void __launch_bounds__(ACF_THREADS) acf_seg_partial_kernel(AcfSegParams p) {
-    const int lg = (int)blockIdx.y * ACF_THREADS + threadIdx.x;
-    if (lg >= p.LG) return;
-    const int64_t c = blockIdx.x;
-    const int64_t c0 = p.lo[c], c1 = p.hi[c], end = p.end[c];
-    const double mua = p.mu[0], mub = p.mu[1];
-    const int jl0 = lg * ACF_RL;
-    int64_t t[ACF_RL];
-    double acc[ACF_RL];
-#pragma unroll
-    for (int r = 0; r < ACF_RL; ++r) {
-        t[r] = (jl0 + r < p.nLags) ? p.l0 + jl0 + r : INT64_MAX / 2;
-        acc[r] = 0.0;
-    }
-    const int64_t hi = min(c1, end - t[0]);
-    for (int64_t n = c0; n < hi; ++n) {
-        const double da = __dsub_rn(__ldg(p.a + n), mua);
-#pragma unroll
-        for (int r = 0; r < ACF_RL; ++r)
-            if (n + t[r] < end) acc[r] = __dadd_rn(acc[r], __dmul_rn(da, __dsub_rn(__ldg(p.b + n + t[r]), mub)));
-    }
-#pragma unroll
-    for (int r = 0; r < ACF_RL; ++r)
-        if (jl0 + r < p.nLags) p.partial[c * p.nLags + jl0 + r] = acc[r];
-}
-
-// per lag t = l0 + jl: numerator = 0.0 + the series sums (each 0.0 + its chunk partials in order) of the series with
-// L_k > t in list order, denominator = 0.0 + (double)(L_k - t) over the same series; neg[jl] = 1 when a running
-// numerator is negative (truncate, timeseries.py:641); out[jl] = (numerator / denominator) / sigma2, or the
-// numerator itself where sigma2 is NULL (the lag-0 pass that gives sigma^2)
-__global__ void acf_seg_combine_kernel(const double* __restrict__ partial, const int64_t* __restrict__ chunkOff,
-                                       const int64_t* __restrict__ segLen, int K, int64_t l0, int nLags,
-                                       const double* __restrict__ sigma2, double* out, int8_t* neg) {
+// per lag t = t0 + jl: numerator = 0.0 + S[k * ldS + jl] of the series with L_k > t in list order, denominator =
+// 0.0 + (double)(L_k - t) over the same series; neg[jl] = 1 when a running numerator is negative (truncate,
+// timeseries.py:641); out[jl] = (numerator / denominator) / sigma2, or numerator / denominator where sigma2 is NULL
+// (lag 0, whose denominator is N exactly: sigma^2)
+__global__ void acf_pooled_corr_kernel(const double* __restrict__ S, int ldS, const int64_t* __restrict__ segLen,
+                                       int K, int64_t t0, int nLags, const double* __restrict__ sigma2, double* out,
+                                       int8_t* neg) {
     const int jl = blockIdx.x * blockDim.x + threadIdx.x;
     if (jl >= nLags) return;
-    const int64_t t = l0 + jl;
+    const int64_t t = t0 + jl;
     double num = 0.0, den = 0.0;
     int8_t negative = 0;
     for (int k = 0; k < K; ++k) {
         if (t >= segLen[k]) continue;
-        double s = 0.0;
-        for (int64_t c = chunkOff[k]; c < chunkOff[k + 1]; ++c) s = __dadd_rn(s, partial[c * nLags + jl]);
-        num = __dadd_rn(num, s);
+        num = __dadd_rn(num, S[(int64_t)k * ldS + jl]);
         den = __dadd_rn(den, (double)(segLen[k] - t));
         if (num < 0.0) negative = 1;
     }
-    out[jl] = sigma2 ? __ddiv_rn(__ddiv_rn(num, den), sigma2[0]) : num;
+    const double q = __ddiv_rn(num, den);
+    out[jl] = sigma2 ? __ddiv_rn(q, sigma2[0]) : q;
     if (neg) neg[jl] = negative;
-}
-
-__global__ void acf_seg_sigma_kernel(const double* __restrict__ num0, int64_t N, double* sigma2) {
-    if (blockIdx.x == 0 && threadIdx.x == 0) sigma2[0] = __ddiv_rn(num0[0], (double)N);
 }
 
 // sum over lags t in [t0, t1) of max(L - t, 0): the lag terms of one series
@@ -974,51 +933,46 @@ int mbar_b200_acf_correlation_multiple(mbar_b200_acf* o, int64_t n_max, int32_t 
     const AcfGrid& grid = o->series;
     const int64_t nc = grid.nChunks();
     const int64_t nl = n_max + 1;
-    const int64_t lagStep = std::min<int64_t>(nl, std::max<int64_t>(ACF_RL, ACF_PART_BUDGET / nc / ACF_RL * ACF_RL));
+    // lag sums [K][batch] within a quarter of the partial budget, as the walk's
+    const int64_t batch = std::min<int64_t>(nl, std::max<int64_t>(ACF_RL, ACF_PART_BUDGET / 4 / K));
+    const int64_t partCap = std::min<int64_t>(ACF_PART_BUDGET, nc * batch);
     CallBuffers buf("acf");
-    const int64_t *d_lo = grid.d_lo, *d_hi = grid.d_hi, *d_end = grid.d_end, *d_chunkOff = grid.d_chunkOff;
-    double *d_totA, *d_totB, *d_mu, *d_num0, *d_s2, *d_C, *d_partial;
+    double *d_totA, *d_totB, *d_S, *d_s2, *d_C;
     int8_t* d_neg;
     MBAR_TRY(buf.alloc(&d_totA, (size_t)nc));
     MBAR_TRY(buf.alloc(&d_totB, (size_t)nc));
-    MBAR_TRY(buf.alloc(&d_mu, 2));
-    MBAR_TRY(buf.alloc(&d_num0, 1));
+    MBAR_TRY(buf.alloc(&d_S, (size_t)(K * batch)));
     MBAR_TRY(buf.alloc(&d_s2, 1));
     MBAR_TRY(buf.alloc(&d_C, (size_t)nl));
     MBAR_TRY(buf.alloc(&d_neg, (size_t)nl));
-    MBAR_TRY(buf.alloc(&d_partial, (size_t)(nc * lagStep)));
+    // request k: series k from start 0
+    const std::vector<int64_t> hs((size_t)K, 0);
+    std::vector<int32_t> ser((size_t)K);
+    for (int k = 0; k < K; ++k) ser[k] = k;
+    AcfLagRunner run{o, &grid, false, false, hs.data(), ser.data()};
+    MBAR_TRY(run.alloc(buf, K, batch, partCap));
     MBAR_CUDA(cudaMemsetAsync(d_C, 0xff, (size_t)nl * sizeof(double), o->stream));
-    // lags [t0, t1) in launches whose partials fit the budget; out / neg indexed from t0
+    std::vector<int64_t> lags;
+    // lags [t0, t1) in batches of lag sums; out / neg indexed from t0
     auto evalLags = [&](int64_t t0, int64_t t1, const double* s2, double* out, int8_t* neg) -> int {
-        for (int64_t x = t0; x < t1; x += lagStep) {
-            const int n = (int)std::min(lagStep, t1 - x);
-            AcfSegParams p{};
-            p.a = o->d_a;
-            p.b = o->d_b;
-            p.lo = d_lo;
-            p.hi = d_hi;
-            p.end = d_end;
-            p.mu = d_mu;
-            p.partial = d_partial;
-            p.l0 = x;
-            p.nLags = n;
-            p.LG = (n + ACF_RL - 1) / ACF_RL;
-            const dim3 grid((unsigned)nc, (unsigned)((p.LG + ACF_THREADS - 1) / ACF_THREADS));
-            acf_seg_partial_kernel<<<grid, ACF_THREADS, 0, o->stream>>>(p);
-            acf_seg_combine_kernel<<<(unsigned)((n + 127) / 128), 128, 0, o->stream>>>(
-                d_partial, d_chunkOff, o->d_segLen, K, x, n, s2, out + (x - t0), neg ? neg + (x - t0) : nullptr);
+        for (int64_t x = t0; x < t1; x += batch) {
+            const int n = (int)std::min(batch, t1 - x);
+            lags.resize((size_t)n);
+            for (int k = 0; k < n; ++k) lags[k] = x + k;
+            MBAR_TRY(run.run(ser.data(), K, lags.data(), n, d_S, n));
+            acf_pooled_corr_kernel<<<(unsigned)((n + 127) / 128), 128, 0, o->stream>>>(
+                d_S, n, o->d_segLen, K, x, n, s2, out + (x - t0), neg ? neg + (x - t0) : nullptr);
             MBAR_CUDA(cudaGetLastError());
         }
         return MBAR_B200_OK;
     };
     MBAR_CUDA(cudaEventRecord(o->ev0, o->stream));
-    acf_total_kernel<<<(unsigned)((nc + 127) / 128), 128, 0, o->stream>>>(o->d_a, o->d_b, d_lo, d_hi, nc, d_totA,
-                                                                        d_totB);
-    acf_seg_mean_kernel<<<1, 32, 0, o->stream>>>(d_totA, d_totB, d_chunkOff, K, o->T, d_mu);
+    acf_total_kernel<<<(unsigned)((nc + 127) / 128), 128, 0, o->stream>>>(o->d_a, o->d_b, grid.d_lo, grid.d_hi, nc,
+                                                                        d_totA, d_totB);
+    acf_pooled_mean_kernel<<<1, 32, 0, o->stream>>>(d_totA, d_totB, grid.d_chunkOff, K, o->T, run.d_muA,
+                                                    run.d_muB);
     MBAR_CUDA(cudaGetLastError());
-    MBAR_TRY(evalLags(0, 1, nullptr, d_num0, nullptr));
-    acf_seg_sigma_kernel<<<1, 32, 0, o->stream>>>(d_num0, o->T, d_s2);
-    MBAR_CUDA(cudaGetLastError());
+    MBAR_TRY(evalLags(0, 1, nullptr, d_s2, nullptr));
     double s2 = 0.0;
     MBAR_CUDA(cudaMemcpyAsync(&s2, d_s2, sizeof(double), cudaMemcpyDeviceToHost, o->stream));
     MBAR_CUDA(cudaStreamSynchronize(o->stream));
@@ -1052,12 +1006,10 @@ int mbar_b200_acf_correlation_multiple(mbar_b200_acf* o, int64_t n_max, int32_t 
     }
     MBAR_CUDA(cudaEventRecord(o->ev1, o->stream));
     MBAR_CUDA(cudaMemcpyAsync(C, d_C, (size_t)nl * sizeof(double), cudaMemcpyDeviceToHost, o->stream));
-    double mu[2];
-    MBAR_CUDA(cudaMemcpyAsync(mu, d_mu, 2 * sizeof(double), cudaMemcpyDeviceToHost, o->stream));
+    if (mean_a) MBAR_CUDA(cudaMemcpyAsync(mean_a, run.d_muA, sizeof(double), cudaMemcpyDeviceToHost, o->stream));
+    if (mean_b) MBAR_CUDA(cudaMemcpyAsync(mean_b, run.d_muB, sizeof(double), cudaMemcpyDeviceToHost, o->stream));
     MBAR_CUDA(cudaStreamSynchronize(o->stream));
     *n_out = count;
-    if (mean_a) *mean_a = mu[0];
-    if (mean_b) *mean_b = mu[1];
     if (sigma2) *sigma2 = s2;
     float e = 0.f;
     o->lastMs = event_ms(o->ev0, o->ev1, &e) ? e : 0.0;

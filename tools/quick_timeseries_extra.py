@@ -4,7 +4,8 @@ time (CUDA events of the mbar_b200_acf call, after a warm-up call of the same sh
 pymbar_b200.timeseries call, truncate / lag rounds, the lag terms evaluated and their rate, and the card with its
 power limit read in the same run:
 
-* normalized_fluctuation_correlation_function_multiple, 10 series x 1e5 and 10 x 1e6, with and without truncate;
+* normalized_fluctuation_correlation_function_multiple, 10 series x 1e5, 10 x 1e6 and 1000 x 2000 (many short
+  series: a few chunks each), with and without truncate;
 * statistical_inefficiency_fft at T = 1e8 with tau = 1e3, and at T = 1e6 for a linear drift (crossing near T / 2);
 * detect_equilibration_binary_search at T = 1e6.
 Not run by bench.py.
@@ -89,9 +90,9 @@ def main():
     ap.add_argument("--out", default=None)
     a = ap.parse_args()
     res = dict(card=card(), cases=[])
-    for n in (100_000, 1_000_000):
+    for K, n in ((10, 100_000), (10, 1_000_000), (1000, 2000)):
         for truncate in (False, True):
-            res["cases"].append(correlation_multiple(10, n, truncate))
+            res["cases"].append(correlation_multiple(K, n, truncate))
     res["cases"].append(fft(f"statistical_inefficiency_fft T={a.big} tau=1e3", ar1(7, a.big, 1000.0)))
     T = 1_000_000
     drift = np.linspace(0.0, 1.0, T) + 1e-3 * np.random.RandomState(8).standard_normal(T)
