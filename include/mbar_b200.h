@@ -43,6 +43,10 @@ extern "C" {
 /* Largest number of states a context takes: mbar_b200_create's K and create_augmented's K + n_extra. */
 #define MBAR_B200_MAX_STATES 8192
 
+/* Largest number of rows R_p = K_p + M_p of a batch problem with appended rows (mbar_b200_batch_set_unsampled):
+ * 3 * 64, so the 3K rows of compute_entropy_and_enthalpy fit every problem a batch holds. */
+#define MBAR_B200_BATCH_MAX_ROWS 192
+
 #if defined(__GNUC__)
 #pragma GCC visibility push(default)
 #endif
@@ -452,9 +456,28 @@ int mbar_b200_batch_replicate_moments(mbar_b200_batch* batch, int32_t n_requests
  * [sum over slots of K_p], status and iterations [n_slots]; the same status codes. */
 int mbar_b200_batch_solve_replicates(mbar_b200_batch* batch, double* f_inout, double tol, int32_t maxiter,
                                      int32_t min_sc_iter, double gamma, int32_t* status, int32_t* iterations);
-/* CUDA-event time of the kernels of the last batch_moments, batch_solve, batch_replicate_moments or
- * batch_solve_replicates call, its kernel launches, its iterations (solves) and the bytes of u_kn tiles (and
- * counts) its passes read. */
+/* Appended rows (DESIGN.md 3.5g''): replaces the resident appended rows with those of n problems, problem problem[i]
+ * getting M[i] unsampled rows [M_i][N_p] (rows concatenates them, row-major).  They are stored as tiles of u - x_n,
+ * shifted by the problem's resident x_n and padded with +inf past N_p.  NaN or -inf -> MBAR_B200_ERR_NAN; a bad or
+ * repeated problem index, M_i < 1 or K_p + M_i > MBAR_B200_BATCH_MAX_ROWS -> MBAR_B200_ERR_INVALID; rows that do not
+ * fit in device memory -> MBAR_B200_ERR_NOMEM (the message gives the allocation in bytes).  A failed call leaves no
+ * appended rows.  n = 0 drops them all. */
+int mbar_b200_batch_set_unsampled(mbar_b200_batch* batch, int32_t n, const int32_t* problem, const int32_t* M,
+                                  const double* rows);
+/* The moments of the augmented problems: request r names problem[r], which must hold appended rows, and f its
+ * R_p = K_p + M_p free energies (f concatenates the requests').  L_n is taken over the sampled rows only, as in
+ * mbar_b200_batch_moments.  S and log S [R_p] cover every row (sampled rows as batch_moments with all_rows = 1
+ * gives them; unsampled and appended rows as running (max, sum) pairs), then sum_n L_n, the flag of batch_moments
+ * applied to every row and, when G is not NULL, the N-scaled Gram Ghat [R_p][R_p] of all rows (sampled rows scaled by
+ * N_k, the others by 1).  Appended weights are not shifted: ask for the Gram at a normalised f, where they are at
+ * most 1; a Ghat entry that is not finite sets the flag.  Three kernel launches with the Gram (two without) and one
+ * synchronisation; a request's results are the same bits whichever requests share the call. */
+int mbar_b200_batch_augmented_moments(mbar_b200_batch* batch, int32_t n_requests, const int32_t* problem,
+                                      const double* f, double* S, double* log_S, double* sum_L, int32_t* flag,
+                                      double* G);
+/* CUDA-event time of the kernels of the last batch_moments, batch_solve, batch_replicate_moments,
+ * batch_solve_replicates or batch_augmented_moments call, its kernel launches, its iterations (solves) and the bytes
+ * of u_kn tiles (appended tiles, counts) its passes read. */
 int mbar_b200_last_batch_stats(mbar_b200_batch* batch, double* kernel_ms, int32_t* launches, int32_t* iterations,
                                int64_t* bytes_read);
 

@@ -11,7 +11,9 @@ Public surface:
     Gaussian EXP; :mod:`pymbar_b200.other_estimators`, including ``bar_many`` for many pairs in lockstep);
   * :class:`pymbar_b200.DeviceMbarBatch` — many small MBAR problems (up to 64 states each) resident together;
     :func:`pymbar_b200.mbar_many.mbar_many` solves all of them in lockstep, one device call per iteration, and
-    returns each problem's free energies and uncertainties;
+    returns each problem's free energies and uncertainties, and :class:`pymbar_b200.MbarMany` keeps them resident
+    for batched expectations, perturbed free energies, entropies and enthalpies, overlaps and effective sample
+    numbers;
   * :func:`pymbar_b200.install` — rebind ``pymbar.mbar_solvers`` so unmodified ``pymbar.MBAR`` uses it.
 
 Everything numerical runs in libmbar_b200.so (C ABI in include/mbar_b200.h).  No CPU fallback.
@@ -20,7 +22,7 @@ from . import _lib
 from .problem import DeviceAcf, DeviceBSpline, DeviceKde, DeviceMbarBatch, DeviceProblem, DeviceWork, PinnedArray
 from .utils import ParameterError
 
-__all__ = ["DeviceProblem", "DeviceKde", "DeviceBSpline", "DeviceAcf", "DeviceWork", "DeviceMbarBatch", "PinnedArray", "ParameterError", "install", "uninstall", "trim", "mbar_solvers"]
+__all__ = ["DeviceProblem", "DeviceKde", "DeviceBSpline", "DeviceAcf", "DeviceWork", "DeviceMbarBatch", "PinnedArray", "ParameterError", "install", "uninstall", "trim", "mbar_solvers", "MbarMany"]
 
 _SAVED = {}
 _PATCHED = (
@@ -149,6 +151,10 @@ def __getattr__(name):
         import importlib
 
         return importlib.import_module(".mbar_solvers", __name__)
+    if name == "MbarMany":
+        from .mbar_many import MbarMany
+
+        return MbarMany
     raise AttributeError(name)
 
 

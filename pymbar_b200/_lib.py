@@ -10,6 +10,7 @@ LIB_PATH = os.path.join(_HERE, "libmbar_b200.so")
 
 UNIQUE_ID_BYTES = 128
 MAX_STATES = 8192            # MBAR_B200_MAX_STATES: largest K of a context, augmented ones included
+BATCH_MAX_ROWS = 192         # MBAR_B200_BATCH_MAX_ROWS: largest K_p + M_p of a batch problem with appended rows
 KERNEL_AUTO, KERNEL_FUSED, KERNEL_GENERIC = 0, 1, 2
 
 STATUS = {
@@ -117,6 +118,9 @@ SIGNATURES = {
                                                     _dp, C.POINTER(C.c_int32), _dp]),
     "mbar_b200_batch_solve_replicates": (C.c_int, [_ctx, _dp, C.c_double, C.c_int32, C.c_int32, C.c_double,
                                                    C.POINTER(C.c_int32), C.POINTER(C.c_int32)]),
+    "mbar_b200_batch_set_unsampled": (C.c_int, [_ctx, C.c_int32, C.POINTER(C.c_int32), C.POINTER(C.c_int32), _dp]),
+    "mbar_b200_batch_augmented_moments": (C.c_int, [_ctx, C.c_int32, C.POINTER(C.c_int32), _dp, _dp, _dp, _dp,
+                                                    C.POINTER(C.c_int32), _dp]),
     "mbar_b200_last_batch_stats": (C.c_int, [_ctx, _dp, C.POINTER(C.c_int32), C.POINTER(C.c_int32),
                                              C.POINTER(C.c_int64)]),
     "mbar_b200_solve_sci":(C.c_int, [_ctx, _dp, C.c_double, C.c_int32, C.POINTER(SolveResult)]),

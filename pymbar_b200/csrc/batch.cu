@@ -84,6 +84,41 @@ struct BatchProbDev {
     int32_t K;
 };
 
+// ---- appended rows and the augmented moments (DESIGN.md 3.5g'') ----
+constexpr int AUG_MAX_R = MBAR_B200_BATCH_MAX_ROWS;
+constexpr int AUG_BLOCK = 32;                       // Gram rows per block: a work item is one pair of row blocks
+constexpr int AUG_SW_LD = BATCH_ROUND + 1;          // leading dimension of a staged weight block
+constexpr int64_t AUG_GRAM_MIN_TILES = 512;         // a Gram chunk holds at least 16384 samples ...
+constexpr int64_t AUG_GRAM_MAX_CHUNKS = 64;         // ... and a problem at most 64 Gram chunks
+constexpr size_t AUG_GRAM_SMEM = 2 * AUG_BLOCK * AUG_SW_LD * sizeof(double);
+
+__host__ __device__ __forceinline__ int64_t aug_gram_tiles(int64_t nT) {
+    const int64_t need = (nT + AUG_GRAM_MAX_CHUNKS - 1) / AUG_GRAM_MAX_CHUNKS;
+    return need > AUG_GRAM_MIN_TILES ? need : AUG_GRAM_MIN_TILES;
+}
+__host__ __device__ __forceinline__ int aug_blocks(int R) { return (R + AUG_BLOCK - 1) / AUG_BLOCK; }
+
+// one augmented request: the problem's K_p resident rows followed by its M_p appended rows, R_p = K_p + M_p
+struct AugReq {
+    int64_t uoff, aoff;      // first double of the problem's tiles and of its appended tiles
+    int64_t N, nT;           // samples and tiles of the problem
+    int64_t ct, gct;         // tiles per pass chunk and per Gram chunk
+    int64_t item0, gitem0;   // first (request, chunk) item of the pass and first (request, block pair, chunk) item
+    int64_t poff, gpoff;     // first double of the request's pass partials and Gram partials
+    int64_t ooff, voff, foff, loff;  // packed output, K-vectors (N_k, log N_k), f [R_p], L'_n scratch
+    int32_t K, M, prob, wantG;
+};
+
+// packed output: [0, R) S, [R, 2R) log S, [2R] sum L, [2R + 1] flag, then R x R Ghat when asked for
+__host__ __device__ __forceinline__ int64_t aug_out_size(int R, bool G) { return 2 * R + 2 + (G ? (int64_t)R * R : 0); }
+
+// one problem's appended rows for the upload kernel: raw offset, appended tile offset, first tile of the problem
+// (indexes x_n), first tile among the appended problems, samples, rows
+struct AugProbDev {
+    int64_t roff, aoff, tile0, atile0, N;
+    int32_t M;
+};
+
 }  // namespace mbar
 
 struct mbar_b200_batch : mbar::Resident {
@@ -103,6 +138,12 @@ struct mbar_b200_batch : mbar::Resident {
     mbar::DevArray<int64_t> d_slotCoff;
     mbar::DevArray<int32_t> d_slotProb;
     mbar::DevArray<double> d_sumxw;             // sum_n c_n x_n of each slot
+    // appended rows (mbar_b200_batch_set_unsampled)
+    std::vector<int> M;                         // appended rows of each problem (0: none)
+    std::vector<int64_t> aoff;                  // first double of each problem's appended tiles
+    mbar::DevArray<double> d_ua;                // appended tiles [nT_p][M_p][32] of u - x_n
+    mbar::DevArray<mbar::AugReq> d_areq;
+    mbar::DevArray<double> d_L, d_gpart;        // L'_n of each Gram request, Gram chunk partials
     // per-call buffers, grown on demand
     mbar::DevArray<mbar::BatchReq> d_req;
     mbar::DevArray<double> d_f, d_part, d_out;
@@ -694,6 +735,361 @@ static int batch_moments_call(mbar_b200_batch* b, bool weighted, int32_t n, cons
     return MBAR_B200_OK;
 }
 
+// ---- appended rows and the augmented moments (DESIGN.md 3.5g'') ---------------------------------------------------
+// Three kernels.  The pass, over (request, chunk) items with chunks of batch_chunk_tiles(nT, R) tiles, sums every
+// row as batch_moments_kernel<false> does with all rows asked for (sampled rows linearly, every other row as a running
+// (max, sum) pair) and, when the Gram is wanted, writes L'_n to a per-request scratch.  The Gram kernel takes
+// (request, pair of 32-row blocks, Gram chunk) items: it rebuilds the two blocks' weights of 128 samples at a time
+// from the tiles and L'_n, stages them in shared memory and accumulates a 2 x 4 patch of the 32 x 32 block per thread
+// with DFMA, samples in order.  The finalize kernel adds both kinds of partials in chunk order.  No atomics, and every
+// geometry is a function of (N_p, R_p) alone.
+
+// upload: one warp per appended tile, one lane per sample
+__global__ void __launch_bounds__(256) batch_aug_retile_kernel(const double* __restrict__ raw,
+                                                               const AugProbDev* __restrict__ pr, int n,
+                                                               int64_t nTiles, const double* __restrict__ x,
+                                                               double* __restrict__ ua) {
+    const int64_t tile = (int64_t)blockIdx.x * 8 + (threadIdx.x >> 5);
+    if (tile >= nTiles) return;
+    const int lane = threadIdx.x & 31;
+    int lo = 0, hi = n - 1;
+    while (lo < hi) {
+        const int mid = (lo + hi + 1) >> 1;
+        if (pr[mid].atile0 <= tile) lo = mid;
+        else hi = mid - 1;
+    }
+    const AugProbDev q = pr[lo];
+    const int64_t t = tile - q.atile0;
+    const int64_t s = t * 32 + lane;
+    const bool valid = s < q.N;
+    const double xn = x[(q.tile0 + t) * 32 + lane];
+    double* dst = ua + q.aoff + t * q.M * 32 + lane;
+    for (int m = 0; m < q.M; ++m) dst[m * 32] = valid ? raw[q.roff + (int64_t)m * q.N + s] - xn : INFINITY;
+}
+
+// the request of a pass item (gram = false) or of a Gram item (gram = true)
+__device__ __forceinline__ int aug_find(const AugReq* __restrict__ req, int nReq, int64_t item, bool gram) {
+    int lo = 0, hi = nReq - 1;
+    while (lo < hi) {
+        const int mid = (lo + hi + 1) >> 1;
+        if ((gram ? req[mid].gitem0 : req[mid].item0) <= item) lo = mid;
+        else hi = mid - 1;
+    }
+    return lo;
+}
+
+// row k of a request at tile t: resident tiles for k < K, appended tiles after
+__device__ __forceinline__ const double* aug_row(const double* __restrict__ u, const double* __restrict__ ua,
+                                                 const AugReq& q, int64_t t, int k, int lane) {
+    return k < q.K ? u + q.uoff + (t * q.K + k) * 32 + lane : ua + q.aoff + (t * q.M + (k - q.K)) * 32 + lane;
+}
+
+// per-chunk partial: R (max, sum) pairs, sum L', bad flag
+__global__ void __launch_bounds__(BATCH_THREADS) batch_aug_kernel(
+    const double* __restrict__ u, const double* __restrict__ ua, const AugReq* __restrict__ req, int nReq,
+    const double* __restrict__ fAll, const double* __restrict__ NkAll, const double* __restrict__ logNkAll,
+    double* __restrict__ part, double* __restrict__ Lbuf) {
+    __shared__ double sM[BATCH_WARPS][AUG_MAX_R], sS[BATCH_WARPS][AUG_MAX_R];
+    __shared__ double sF[AUG_MAX_R], sC[BATCH_MAX_K];
+    __shared__ int sRow[AUG_MAX_R];                              // 1 sampled, 2 every other row
+    __shared__ double sRed[BATCH_THREADS];
+    __shared__ int sBad;
+    const int64_t item = blockIdx.x;
+    const AugReq q = req[aug_find(req, nReq, item, false)];
+    const int64_t chunk = item - q.item0;
+    const int K = q.K, R = q.K + q.M;
+    const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+    for (int k = tid; k < R; k += BATCH_THREADS) {
+        sF[k] = fAll[q.foff + k];
+        const bool s = k < K && NkAll[q.voff + k] > 0.0;
+        sRow[k] = s ? 1 : 2;
+        if (k < K) sC[k] = s ? sF[k] + logNkAll[q.voff + k] : -INFINITY;
+    }
+    for (int k = tid; k < BATCH_WARPS * AUG_MAX_R; k += BATCH_THREADS) {
+        (&sM[0][0])[k] = -INFINITY;
+        (&sS[0][0])[k] = 0.0;
+    }
+    if (tid == 0) sBad = 0;
+    __syncthreads();
+    const int64_t t0 = chunk * q.ct, t1 = min(q.nT, t0 + q.ct);
+    double sumL = 0.0;
+    bool bad = false;
+    for (int64_t t = t0 + warp; t < t1; t += BATCH_WARPS) {         // warp-uniform
+        const int64_t n = t * 32 + lane;
+        const bool valid = n < q.N;
+        const double* ut = u + q.uoff + t * (int64_t)K * 32 + lane;
+        double Lp = 0.0;
+        if (valid) {
+            double m = -INFINITY;
+            for (int k = 0; k < K; ++k)
+                if (sRow[k] == 1) m = fmax(m, sC[k] - __ldg(ut + k * 32));
+            double D = 0.0;
+            for (int k = 0; k < K; ++k)
+                if (sRow[k] == 1) D += exp(sC[k] - __ldg(ut + k * 32) - m);
+            Lp = m + log(D);
+            sumL += Lp;
+        }
+        if (q.wantG) Lbuf[q.loff + n] = Lp;
+        for (int k = 0; k < R; ++k) {
+            double a = valid ? sF[k] - __ldg(aug_row(u, ua, q, t, k, lane)) - Lp : -INFINITY;
+            if (a != a) {
+                bad = true;
+                a = -INFINITY;
+            }
+            const double wm = sRow[k] == 1 ? 0.0 : warp_max(a);
+            const double e = wm > -INFINITY ? exp(a - wm) : 0.0;
+            const double ws = warp_sum(e);
+            if (lane == 0) pair_merge(sM[warp][k], sS[warp][k], wm, ws);
+        }
+    }
+    if (bad) sBad = 1;
+    sRed[tid] = sumL;
+    __syncthreads();
+    for (int o = BATCH_THREADS / 2; o > 0; o >>= 1) {
+        if (tid < o) sRed[tid] += sRed[tid + o];
+        __syncthreads();
+    }
+    double* pc = part + q.poff + chunk * (2 * R + 2);
+    for (int k = tid; k < R; k += BATCH_THREADS) {
+        double m = sM[0][k], s = sS[0][k];
+        for (int w = 1; w < BATCH_WARPS; ++w) pair_merge(m, s, sM[w][k], sS[w][k]);
+        pc[2 * k] = m;
+        pc[2 * k + 1] = s;
+    }
+    if (tid == 0) {
+        pc[2 * R] = sRed[0];
+        pc[2 * R + 1] = sBad ? 1.0 : 0.0;
+    }
+}
+
+// one 32 x 32 block (bi, bj), bi >= bj, of Ghat over one Gram chunk: thread (ti, tj) = (tid / 8, tid % 8) owns rows
+// 2 ti, 2 ti + 1 of block bi and columns tj + 8 c (c < 4) of block bj
+__global__ void __launch_bounds__(BATCH_THREADS) batch_aug_gram_kernel(
+    const double* __restrict__ u, const double* __restrict__ ua, const AugReq* __restrict__ req, int nReq,
+    const double* __restrict__ fAll, const double* __restrict__ NkAll, const double* __restrict__ logNkAll,
+    const double* __restrict__ Lbuf, double* __restrict__ gpart) {
+    extern __shared__ __align__(16) double sAug[];               // [2][AUG_BLOCK][AUG_SW_LD] staged weights
+    __shared__ double sF[2][AUG_BLOCK], sLs[2][AUG_BLOCK];
+    const int64_t item = blockIdx.x;
+    const AugReq q = req[aug_find(req, nReq, item, true)];
+    const int R = q.K + q.M;
+    const int64_t ngc = (q.nT + q.gct - 1) / q.gct;
+    const int64_t local = item - q.gitem0;
+    const int pair = (int)(local / ngc);
+    const int64_t gc = local - (int64_t)pair * ngc;
+    int bi = (int)((sqrt(8.0 * pair + 1.0) - 1.0) * 0.5);
+    while ((bi + 1) * (bi + 2) / 2 <= pair) ++bi;
+    while (bi * (bi + 1) / 2 > pair) --bi;
+    const int bj = pair - bi * (bi + 1) / 2;
+    const int nh = bi == bj ? 1 : 2;                             // a diagonal block stages one row block
+    const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+    if (tid < 2 * AUG_BLOCK) {
+        const int h = tid / AUG_BLOCK, i = tid % AUG_BLOCK;
+        const int k = (h ? bj : bi) * AUG_BLOCK + i;
+        const bool s = k < q.K && NkAll[q.voff + k] > 0.0;
+        sF[h][i] = k < R ? fAll[q.foff + k] : 0.0;
+        sLs[h][i] = s ? logNkAll[q.voff + k] : 0.0;
+    }
+    double* sWi = sAug;
+    double* sWj = nh == 2 ? sAug + AUG_BLOCK * AUG_SW_LD : sAug;
+    const int ti = tid >> 3, tj = tid & 7;
+    double acc[2][4];
+#pragma unroll
+    for (int e = 0; e < 2; ++e)
+#pragma unroll
+        for (int c = 0; c < 4; ++c) acc[e][c] = 0.0;
+    __syncthreads();
+    const int64_t t0 = gc * q.gct, t1 = min(q.nT, t0 + q.gct);
+    const int64_t rounds = (t1 - t0 + BATCH_WARPS - 1) / BATCH_WARPS;
+    for (int64_t r = 0; r < rounds; ++r) {
+        const int64_t t = t0 + r * BATCH_WARPS + warp;
+        const int64_t n = t * 32 + lane;
+        const bool valid = t < t1 && n < q.N;
+        const double Lp = valid ? Lbuf[q.loff + n] : 0.0;
+        for (int h = 0; h < nh; ++h) {
+            const int b = h ? bj : bi;
+            double* w = h ? sWj : sWi;
+            for (int i = 0; i < AUG_BLOCK; ++i) {
+                const int k = b * AUG_BLOCK + i;
+                double x = 0.0;
+                if (valid && k < R) x = exp(sF[h][i] - __ldg(aug_row(u, ua, q, t, k, lane)) - Lp + sLs[h][i]);
+                w[i * AUG_SW_LD + tid] = x;
+            }
+        }
+        __syncthreads();
+        const double* wa = sWi + (2 * ti) * AUG_SW_LD;
+        const double* wb = sWj + tj * AUG_SW_LD;
+#pragma unroll 4
+        for (int s = 0; s < BATCH_ROUND; ++s) {
+            const double a0 = wa[s], a1 = wa[AUG_SW_LD + s];
+#pragma unroll
+            for (int c = 0; c < 4; ++c) {
+                const double bc = wb[c * 8 * AUG_SW_LD + s];
+                acc[0][c] = fma(a0, bc, acc[0][c]);
+                acc[1][c] = fma(a1, bc, acc[1][c]);
+            }
+        }
+        __syncthreads();
+    }
+    double* pg = gpart + q.gpoff + local * (AUG_BLOCK * AUG_BLOCK);
+#pragma unroll
+    for (int e = 0; e < 2; ++e)
+#pragma unroll
+        for (int c = 0; c < 4; ++c) pg[(2 * ti + e) * AUG_BLOCK + tj + 8 * c] = acc[e][c];
+}
+
+// A request's partials in chunk order -> its packed output, with the flag rules of batch_finalize_kernel applied to
+// every row (a sampled row's S outside (1e-280, 1e300); any other row's S NaN or overflowing; a NaN in a sum; a Ghat
+// entry that is not finite).  Gram partials of block pair (bi, bj) and chunk c sit at gpoff + (pair * nGc + c) * 1024.
+__global__ void __launch_bounds__(256) batch_aug_finalize_kernel(const AugReq* __restrict__ req,
+                                                                 const double* __restrict__ part,
+                                                                 const double* __restrict__ gpart,
+                                                                 const double* __restrict__ NkAll,
+                                                                 const double* __restrict__ sumx,
+                                                                 double* __restrict__ out) {
+    __shared__ int sFlag;
+    const AugReq q = req[blockIdx.x];
+    const int K = q.K, R = q.K + q.M, tid = threadIdx.x;
+    const int64_t stride = 2 * R + 2;
+    const int64_t nc = (q.nT + q.ct - 1) / q.ct;
+    const double* p0 = part + q.poff;
+    double* o = out + q.ooff;
+    if (tid == 0) sFlag = 0;
+    __syncthreads();
+    for (int k = tid; k < R; k += blockDim.x) {
+        double m = -INFINITY, s = 0.0;
+        for (int64_t c = 0; c < nc; ++c) pair_merge(m, s, p0[c * stride + 2 * k], p0[c * stride + 2 * k + 1]);
+        const double logS = s > 0.0 ? m + log(s) : -INFINITY;
+        const double S = m == 0.0 ? s : exp(logS);
+        o[k] = S;
+        o[R + k] = logS;
+        const bool sampled = k < K && NkAll[q.voff + k] > 0.0;
+        if (sampled && !(S > 1e-280 && S < 1e300)) sFlag = 1;
+        if (!sampled && (logS != logS || !(S < INFINITY))) sFlag = 1;
+    }
+    if (tid == 0) {
+        double sl = 0.0, bad = 0.0;
+        for (int64_t c = 0; c < nc; ++c) {
+            sl += p0[c * stride + 2 * R];
+            bad = fmax(bad, p0[c * stride + 2 * R + 1]);
+        }
+        o[2 * R] = sl - sumx[q.prob];
+        if (bad > 0.0 || sl != sl) sFlag = 1;
+    }
+    if (q.wantG) {
+        const int64_t ngc = (q.nT + q.gct - 1) / q.gct;
+        const int E = R * (R + 1) / 2;
+        for (int e = tid; e < E; e += blockDim.x) {
+            int i = (int)((sqrt(8.0 * e + 1.0) - 1.0) * 0.5);
+            while ((i + 1) * (i + 2) / 2 <= e) ++i;
+            while (i * (i + 1) / 2 > e) --i;
+            const int j = e - i * (i + 1) / 2;
+            const int bi = i / AUG_BLOCK, bj = j / AUG_BLOCK;
+            const double* pg = gpart + q.gpoff + (int64_t)(bi * (bi + 1) / 2 + bj) * ngc * (AUG_BLOCK * AUG_BLOCK) +
+                               (i % AUG_BLOCK) * AUG_BLOCK + j % AUG_BLOCK;
+            double g = 0.0;
+            for (int64_t c = 0; c < ngc; ++c) g += pg[c * (AUG_BLOCK * AUG_BLOCK)];
+            if (!isfinite(g)) sFlag = 1;
+            o[2 * R + 2 + (int64_t)i * R + j] = g;
+            o[2 * R + 2 + (int64_t)j * R + i] = g;
+        }
+    }
+    __syncthreads();
+    if (tid == 0) o[2 * R + 1] = sFlag ? 1.0 : 0.0;
+}
+
+static int aug_smem_attr(int device) {
+    static bool done[16] = {false};
+    if (!done[device & 15]) {
+        MBAR_CUDA(cudaFuncSetAttribute(batch_aug_gram_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                       (int)AUG_GRAM_SMEM));
+        done[device & 15] = true;
+    }
+    return MBAR_B200_OK;
+}
+
+// The augmented requests (problem[r], f: R_p values each) in one launch of each kernel and one synchronisation;
+// request r's packed output is at b->h_out + offsets[r].
+static int batch_aug_run(mbar_b200_batch* b, int nReq, const int32_t* problem, const double* f, bool wantG,
+                         std::vector<int64_t>& offsets) {
+    std::vector<AugReq> req((size_t)nReq);
+    int64_t items = 0, gitems = 0, parts = 0, gparts = 0, outs = 0, fs = 0, Ls = 0, bytes = 0;
+    offsets.resize(nReq);
+    for (int r = 0; r < nReq; ++r) {
+        const int p = problem[r];
+        AugReq& q = req[r];
+        q.K = b->K[p];
+        q.M = b->M[p];
+        q.prob = p;
+        q.wantG = wantG ? 1 : 0;
+        const int R = q.K + q.M;
+        q.N = b->N[p];
+        q.nT = b->nT[p];
+        q.ct = batch_chunk_tiles(q.nT, R);
+        q.gct = aug_gram_tiles(q.nT);
+        q.uoff = b->uoff[p];
+        q.aoff = b->aoff[p];
+        q.voff = b->voff[p];
+        q.item0 = items;
+        q.gitem0 = gitems;
+        q.poff = parts;
+        q.gpoff = gparts;
+        q.ooff = outs;
+        q.foff = fs;
+        q.loff = Ls;
+        const int64_t nc = (q.nT + q.ct - 1) / q.ct;
+        items += nc;
+        parts += nc * (2 * R + 2);
+        bytes += q.nT * 32 * R * 8;
+        if (wantG) {
+            const int nb = aug_blocks(R);
+            const int64_t ngc = (q.nT + q.gct - 1) / q.gct;
+            gitems += (int64_t)nb * (nb + 1) / 2 * ngc;
+            gparts += (int64_t)nb * (nb + 1) / 2 * ngc * AUG_BLOCK * AUG_BLOCK;
+            Ls += q.nT * 32;
+            bytes += q.nT * 32 * 8 * (int64_t)nb * R;             // every row is staged by nb block pairs
+        }
+        offsets[r] = outs;
+        outs += aug_out_size(R, wantG);
+        fs += R;
+    }
+    MBAR_REQUIRE(items < INT32_MAX && gitems < INT32_MAX, MBAR_B200_ERR_INVALID, "batch: %lld chunks in one call",
+                 (long long)(items + gitems));
+    MBAR_TRY(batch_grow(b->d_areq, nReq));
+    MBAR_TRY(batch_grow(b->d_f, fs));
+    MBAR_TRY(batch_grow(b->d_part, parts));
+    MBAR_TRY(batch_grow(b->d_out, outs));
+    if (wantG) {
+        MBAR_TRY(batch_grow(b->d_gpart, gparts));
+        MBAR_TRY(batch_grow(b->d_L, Ls));
+        MBAR_TRY(aug_smem_attr(b->device));
+    }
+    MBAR_TRY(pinned_grow(&b->h_f, &b->h_fCap, (size_t)fs + (size_t)nReq * sizeof(AugReq) / 8 + 1));
+    MBAR_TRY(pinned_grow(&b->h_out, &b->h_outCap, (size_t)outs));
+    std::memcpy(b->h_f, f, (size_t)fs * sizeof(double));
+    AugReq* hreq = reinterpret_cast<AugReq*>(b->h_f + fs);
+    std::memcpy(hreq, req.data(), req.size() * sizeof(AugReq));
+    MBAR_CUDA(cudaMemcpyAsync(b->d_f, b->h_f, (size_t)fs * sizeof(double), cudaMemcpyHostToDevice, b->stream));
+    MBAR_CUDA(cudaMemcpyAsync(b->d_areq, hreq, req.size() * sizeof(AugReq), cudaMemcpyHostToDevice, b->stream));
+    MBAR_CUDA(cudaEventRecord(b->ev0, b->stream));
+    batch_aug_kernel<<<(unsigned)items, BATCH_THREADS, 0, b->stream>>>(b->d_u, b->d_ua, b->d_areq, nReq, b->d_f,
+                                                                      b->d_Nk, b->d_logNk, b->d_part, b->d_L);
+    if (wantG)
+        batch_aug_gram_kernel<<<(unsigned)gitems, BATCH_THREADS, AUG_GRAM_SMEM, b->stream>>>(
+            b->d_u, b->d_ua, b->d_areq, nReq, b->d_f, b->d_Nk, b->d_logNk, b->d_L, b->d_gpart);
+    batch_aug_finalize_kernel<<<(unsigned)nReq, 256, 0, b->stream>>>(b->d_areq, b->d_part, b->d_gpart, b->d_Nk,
+                                                                     b->d_sumx, b->d_out);
+    MBAR_CUDA(cudaGetLastError());
+    MBAR_CUDA(cudaEventRecord(b->ev1, b->stream));
+    MBAR_CUDA(cudaMemcpyAsync(b->h_out, b->d_out, (size_t)outs * sizeof(double), cudaMemcpyDeviceToHost, b->stream));
+    MBAR_CUDA(cudaStreamSynchronize(b->stream));
+    float e = 0.f;
+    b->lastMs = event_ms(b->ev0, b->ev1, &e) ? e : 0.0;
+    b->lastLaunches = wantG ? 3 : 2;
+    b->lastBytes = bytes;
+    return MBAR_B200_OK;
+}
+
 }  // namespace mbar
 
 using namespace mbar;
@@ -840,6 +1236,96 @@ int mbar_b200_batch_solve_replicates(mbar_b200_batch* b, double* f, double tol, 
     NvtxRange nvtx_("mbar_b200::batch_solve_replicates");
     return batch_solve_units(b, true, f, tol, maxiter, min_sc_iter, gamma, status, iterations,
                              "batch_solve_replicates");
+}
+
+int mbar_b200_batch_set_unsampled(mbar_b200_batch* b, int32_t n, const int32_t* problem, const int32_t* M,
+                                  const double* rows) {
+    MBAR_REQUIRE(b, MBAR_B200_ERR_INVALID, "batch_set_unsampled: NULL object");
+    b->M.assign((size_t)b->P, 0);             // a failed call leaves no appended rows
+    b->aoff.assign((size_t)b->P, 0);
+    MBAR_REQUIRE(n >= 0 && (n == 0 || (problem && M && rows)), MBAR_B200_ERR_INVALID,
+                 "batch_set_unsampled: %d problems", (int)n);
+    std::vector<AugProbDev> pr((size_t)n);
+    std::vector<char> seen((size_t)b->P, 0);
+    std::vector<int64_t> tile0((size_t)b->P, 0);  // first tile of each problem: indexes x_n
+    for (int p = 1; p < b->P; ++p) tile0[p] = tile0[p - 1] + b->nT[p - 1];
+    int64_t raw = 0, total = 0, tiles = 0;
+    for (int i = 0; i < n; ++i) {
+        const int p = problem[i];
+        MBAR_REQUIRE(p >= 0 && p < b->P && !seen[p], MBAR_B200_ERR_INVALID,
+                     "batch_set_unsampled: entry %d names problem %d of %d%s", i, p, b->P,
+                     p >= 0 && p < b->P ? " twice" : "");
+        seen[p] = 1;
+        MBAR_REQUIRE(M[i] >= 1 && b->K[p] + M[i] <= AUG_MAX_R, MBAR_B200_ERR_INVALID,
+                     "batch_set_unsampled: problem %d has K=%d states and M=%d appended rows (K + M: at most %d)", p,
+                     b->K[p], (int)M[i], AUG_MAX_R);
+        pr[i] = AugProbDev{raw, total, tile0[p], tiles, b->N[p], M[i]};
+        raw += (int64_t)M[i] * b->N[p];
+        total += b->nT[p] * 32 * M[i];
+        tiles += b->nT[p];
+    }
+    int64_t bad = 0;
+    for (int64_t j = 0; j < raw; ++j) bad += rows[j] != rows[j] || rows[j] == -INFINITY;
+    MBAR_REQUIRE(bad == 0, MBAR_B200_ERR_NAN, "batch_set_unsampled: %lld appended energies are NaN or -inf",
+                 (long long)bad);
+    if (n == 0) return MBAR_B200_OK;
+    MBAR_CUDA(cudaSetDevice(b->device));
+    NvtxRange nvtx_("mbar_b200::batch_set_unsampled");
+    MBAR_TRY(b->d_ua.reserve((size_t)total, "batch_set_unsampled (appended tiles)"));
+    {
+        CallBuffers cb("batch_set_unsampled (staging)");
+        double* draw = nullptr;
+        AugProbDev* dpr = nullptr;
+        MBAR_TRY(cb.alloc(&draw, (size_t)raw));
+        MBAR_TRY(cb.alloc(&dpr, pr.size()));
+        MBAR_CUDA(cudaMemcpyAsync(draw, rows, (size_t)raw * sizeof(double), cudaMemcpyHostToDevice, b->stream));
+        MBAR_CUDA(cudaMemcpyAsync(dpr, pr.data(), pr.size() * sizeof(AugProbDev), cudaMemcpyHostToDevice, b->stream));
+        batch_aug_retile_kernel<<<(unsigned)((tiles + 7) / 8), 256, 0, b->stream>>>(draw, dpr, n, tiles, b->d_x,
+                                                                                    b->d_ua);
+        MBAR_CUDA(cudaGetLastError());
+        MBAR_CUDA(cudaStreamSynchronize(b->stream));
+    }
+    for (int i = 0; i < n; ++i) {
+        b->M[problem[i]] = M[i];
+        b->aoff[problem[i]] = pr[i].aoff;
+    }
+    return MBAR_B200_OK;
+}
+
+int mbar_b200_batch_augmented_moments(mbar_b200_batch* b, int32_t n_requests, const int32_t* problem,
+                                      const double* f, double* S, double* logS, double* sumL, int32_t* flag,
+                                      double* G) {
+    const char* who = "batch_augmented_moments";
+    MBAR_REQUIRE(b, MBAR_B200_ERR_INVALID, "%s: NULL object", who);
+    MBAR_REQUIRE(n_requests >= 1 && problem && f, MBAR_B200_ERR_INVALID, "%s: %d requests", who, (int)n_requests);
+    for (int r = 0; r < n_requests; ++r) {
+        const int p = problem[r];
+        MBAR_REQUIRE(p >= 0 && p < b->P, MBAR_B200_ERR_INVALID, "%s: request %d names problem %d of %d", who, r, p,
+                     b->P);
+        MBAR_REQUIRE(p < (int)b->M.size() && b->M[p] > 0, MBAR_B200_ERR_INVALID,
+                     "%s: request %d names problem %d, which holds no appended rows", who, r, p);
+    }
+    MBAR_CUDA(cudaSetDevice(b->device));
+    NvtxRange nvtx_("mbar_b200::batch_augmented_moments");
+    b->lastLaunches = 0;
+    b->lastBytes = 0;
+    b->lastIterations = 0;
+    b->lastMs = 0.0;
+    std::vector<int64_t> off;
+    MBAR_TRY(batch_aug_run(b, n_requests, problem, f, G != nullptr, off));
+    int64_t ko = 0, go = 0;
+    for (int r = 0; r < n_requests; ++r) {
+        const int R = b->K[problem[r]] + b->M[problem[r]];
+        const double* o = b->h_out + off[r];
+        if (S) std::memcpy(S + ko, o, R * sizeof(double));
+        if (logS) std::memcpy(logS + ko, o + R, R * sizeof(double));
+        if (sumL) sumL[r] = o[2 * R];
+        if (flag) flag[r] = o[2 * R + 1] != 0.0;
+        if (G) std::memcpy(G + go, o + 2 * R + 2, (size_t)R * R * sizeof(double));
+        ko += R;
+        go += (int64_t)R * R;
+    }
+    return MBAR_B200_OK;
 }
 
 int mbar_b200_last_batch_stats(mbar_b200_batch* b, double* ms, int32_t* launches, int32_t* iterations,

@@ -28,6 +28,10 @@ solved by `bootstrap.bootstrap_f_k` on one DeviceProblem per problem instead whe
 or a sum of it is flagged, when its problem has more than 64 states, or when its problem's multiplicities overflow
 uint16.  Each problem's dict then adds f_k_boots [B, K] and boot_single, the number of its replicates that took that
 path.
+
+`MbarMany` is the same solve kept resident: its estimators (expectations, perturbed free energies, entropy and
+enthalpy, overlap, effective sample numbers) append each problem's extra rows to the batch it already holds and
+evaluate every problem in one augmented moments pass (DESIGN.md 3.5g'').  `mbar_many` is `MbarMany(...).results`.
 """
 from __future__ import annotations
 
@@ -38,6 +42,7 @@ import numpy as np
 
 from . import bootstrap
 from . import estimators
+from . import expectations as ex
 from . import mbar_solvers as ms
 from .utils import ParameterError
 
@@ -48,6 +53,9 @@ MAX_BATCH_K = 64
 UNCERTAINTY_METHODS = (None, "svd-ew", "approximate", "bootstrap")
 DEFAULT_OPTIONS = dict(min_sc_iter=0, gamma=1.0, maxiter=10000)
 BOOT_WAVE_BYTES = 2 << 30   # device footprint of one wave of replicate slots
+MAX_BATCH_ROWS = 192        # DeviceMbarBatch.MAX_ROWS: K_p plus appended rows of a batched estimator request
+AUG_WAVE_BYTES = 2 << 30    # device footprint of one wave of appended rows
+ESTIMATOR_METHODS = (None, "svd-ew", "approximate")
 
 
 def _classes():
@@ -120,6 +128,18 @@ def slot_bytes(K, N):
     part = 2 * K + 2 + K * (K + 1) // 2
     out = 2 * K + 2 + K * K
     return 2 * nT * 32 + 2 * 8 * (nc * part + out + K)
+
+
+def augmented_bytes(K, N, M):
+    """Device bytes of one problem's M appended rows in a wave: its appended tiles, L_n scratch, the pass and Gram
+    partials and packed output of its augmented request, and its f (batch.cu's geometry)."""
+    nT = -(-int(N) // 32)
+    R = int(K) + int(M)
+    nc = -(-nT // _chunk_tiles(nT, R))
+    gct = max(512, -(-nT // 64))
+    ngc = -(-nT // gct)
+    nb = -(-R // 32)
+    return 8 * (nT * 32 * (M + 1) + nc * (2 * R + 2) + nb * (nb + 1) // 2 * ngc * 1024 + 2 * R + 2 + R * R + R)
 
 
 def _validate_boot(n_bootstraps, rseed, P):
@@ -248,48 +268,83 @@ def _single(u_kn, N_k, f_k, tol, want_G):
     return f, G
 
 
-def mbar_many(u_kn_list, N_k_list, f_k_init=None, compute_uncertainty=True, uncertainty_method=None,
-              return_theta=False, solver_tolerance=1.0e-12, options=None, n_bootstraps=0, rseed=None):
-    """MBAR on every problem (u_kn_list[p], N_k_list[p]): one dict per problem, in input order, with f_k, Delta_f,
-    dDelta_f (compute_uncertainty), Theta (return_theta), iterations (of the batched solve; None on the single path),
-    success and path ("batch" or "single").
+class MbarMany:
+    """MBAR on every problem (u_kn_list[p], N_k_list[p]), kept resident for the estimators that follow.
 
-    f_k_init: None (zeros) or one starting vector per problem.  options update the adaptive solver's defaults
-    (min_sc_iter=0, gamma=1, maxiter=10000).  uncertainty_method: None, "svd-ew", "approximate" or "bootstrap".  Every
-    problem is validated before any device work; an invalid problem raises for the lowest failing index.
+    The constructor solves as `mbar_many` does (same arguments) and `.results` is its list of dicts.  The batch of
+    problems with at most 64 states stays on the device until `close()` (or the end of a `with` block), so that
+    `compute_expectations`, `compute_perturbed_free_energies`, `compute_entropy_and_enthalpy`, `compute_overlap` and
+    `compute_effective_sample_number` serve every problem without a new upload or a new solve (DESIGN.md 3.5g'').
 
-    n_bootstraps = B > 0 adds f_k_boots [B, K] (replicate b of problem p is the one pymbar.MBAR(u_kn_list[p],
-    N_k_list[p], n_bootstraps=B, rseed=rseed[p]) draws) and boot_single (how many of them the single-problem path
-    solved) to every dict.  rseed: one seed per problem, or None for one np.random.randint(2**31 - 1) per problem in
-    problem order, as P constructions of MBAR would draw.  uncertainty_method="bootstrap" gives
-    dDelta_f = std over b of f_b - f_b^T and needs B > 0; its Theta is "svd-ew"."""
-    if uncertainty_method not in UNCERTAINTY_METHODS:
-        raise ParameterError(f"uncertainty_method {uncertainty_method!r} is not supported by mbar_many "
-                             f"(one of {UNCERTAINTY_METHODS})")
-    if len(u_kn_list) != len(N_k_list):
-        raise ValueError("u_kn_list and N_k_list must have the same length")
-    P = len(u_kn_list)
-    if f_k_init is not None and len(f_k_init) != P:
-        raise ValueError("f_k_init must hold one vector per problem")
-    seeds = _validate_boot(n_bootstraps, rseed, P)
-    B = int(n_bootstraps)
-    if uncertainty_method == "bootstrap" and B <= 0:
-        raise ParameterError("Cannot request bootstrap sampling of free energy differences without any bootstraps.")
-    opts = dict(DEFAULT_OPTIONS)
-    opts.update(options or {})
-    probs = [_validate(u_kn_list[p], N_k_list[p], None if f_k_init is None else f_k_init[p]) for p in range(P)]
-    if B > 0 and seeds is None:
-        seeds = [np.random.randint(np.iinfo(np.int32).max) for _ in range(P)]
-    want_G = bool((compute_uncertainty and uncertainty_method != "bootstrap") or return_theta)
-    results = [None] * P
-    batch = [p for p in range(P) if probs[p][0].shape[0] <= MAX_BATCH_K]
-    single = [p for p in range(P) if probs[p][0].shape[0] > MAX_BATCH_K]
-    with contextlib.ExitStack() as stack:
+    Each estimator takes one entry per problem, or None to skip a problem, and returns one dict per problem (None for
+    a skipped one) with the keys of the pymbar.MBAR method of the same name and `path`, "batch" or "single".  Every
+    request is validated before any device work; an invalid one raises ParameterError for the lowest failing index.
+    Analytic uncertainties only: uncertainty_method is None, "svd-ew" or "approximate".
+
+    The appended rows of expectations.augmentation go on top of the resident problems in waves whose device footprint
+    stays under AUG_WAVE_BYTES; a problem's result is the same bits in any wave.  Each wave takes one
+    augmented_moments call at (f_k, 0), whose log S gives the appended rows' f = -log S (the self-consistent update
+    of the single path), and, when a Theta is needed, one at the full f with the Gram.  A problem takes the single
+    path (expectations.expectations_inner on a DeviceProblem of it) when it took the single path in the solve, when
+    K_p plus its appended rows exceed MAX_BATCH_ROWS, or when either call flags it."""
+
+    def __init__(self, u_kn_list, N_k_list, f_k_init=None, compute_uncertainty=True, uncertainty_method=None,
+                 return_theta=False, solver_tolerance=1.0e-12, options=None, n_bootstraps=0, rseed=None):
+        if uncertainty_method not in UNCERTAINTY_METHODS:
+            raise ParameterError(f"uncertainty_method {uncertainty_method!r} is not supported by mbar_many "
+                                 f"(one of {UNCERTAINTY_METHODS})")
+        if len(u_kn_list) != len(N_k_list):
+            raise ValueError("u_kn_list and N_k_list must have the same length")
+        P = len(u_kn_list)
+        if f_k_init is not None and len(f_k_init) != P:
+            raise ValueError("f_k_init must hold one vector per problem")
+        seeds = _validate_boot(n_bootstraps, rseed, P)
+        B = int(n_bootstraps)
+        if uncertainty_method == "bootstrap" and B <= 0:
+            raise ParameterError("Cannot request bootstrap sampling of free energy differences without any "
+                                 "bootstraps.")
+        opts = dict(DEFAULT_OPTIONS)
+        opts.update(options or {})
+        probs = [_validate(u_kn_list[p], N_k_list[p], None if f_k_init is None else f_k_init[p]) for p in range(P)]
+        if B > 0 and seeds is None:
+            seeds = [np.random.randint(np.iinfo(np.int32).max) for _ in range(P)]
+        self._probs = probs
+        self._stack = contextlib.ExitStack()
+        self._dev = None
+        self._slot = {}              # problem -> its index in the device batch
+        self._G = {}                 # problem -> W^T W at its final f, where the solve computed it
+        self.device_stats = dict(ms=0.0, launches=0, calls=0)
+        try:
+            self.results = self._solve(probs, seeds, B, compute_uncertainty, uncertainty_method, return_theta,
+                                       solver_tolerance, opts)
+        except BaseException:
+            self.close()
+            raise
+
+    def close(self):
+        """Free the device batch.  The results stay."""
+        self._dev = None
+        self._stack.close()
+
+    def __enter__(self):
+        return self
+
+    def __exit__(self, *exc):
+        self.close()
+
+    def _solve(self, probs, seeds, B, compute_uncertainty, uncertainty_method, return_theta, solver_tolerance, opts):
+        P = len(probs)
+        want_G = bool((compute_uncertainty and uncertainty_method != "bootstrap") or return_theta)
+        results = [None] * P
+        batch = [p for p in range(P) if probs[p][0].shape[0] <= MAX_BATCH_K]
+        single = [p for p in range(P) if probs[p][0].shape[0] > MAX_BATCH_K]
         dev = None
         if batch:
             Batch, _ = _classes()
-            dev = stack.enter_context(Batch([probs[p][0] for p in batch], [probs[p][1] for p in batch],
-                                            device=ms._DEVICE))
+            dev = self._stack.enter_context(Batch([probs[p][0] for p in batch], [probs[p][1] for p in batch],
+                                                  device=ms._DEVICE))
+            self._dev = dev
+            self._slot = {p: i for i, p in enumerate(batch)}
             f_list, status, iters = dev.solve([probs[p][2] for p in batch], tol=solver_tolerance,
                                               maxiter=int(opts["maxiter"]), min_sc_iter=int(opts["min_sc_iter"]),
                                               gamma=float(opts["gamma"]))
@@ -318,11 +373,15 @@ def mbar_many(u_kn_list, N_k_list, f_k_init=None, compute_uncertainty=True, unce
                 if want_G and i not in G:
                     continue
                 p = batch[i]
+                if i in G:
+                    self._G[p] = G[i]
                 results[p] = _result(f_final[i], G.get(i), probs[p][1], "batch", int(iters[i]), True,
                                      compute_uncertainty, uncertainty_method, return_theta)
         for p in sorted(single):
             u, N_k, f0 = probs[p]
             f, G = _single(u, N_k, f0, solver_tolerance, want_G)
+            if G is not None:
+                self._G[p] = G
             success = bool(np.all(np.isfinite(f)))
             results[p] = _result(f, G, N_k, "single", None, success, compute_uncertainty, uncertainty_method,
                                  return_theta)
@@ -334,4 +393,239 @@ def mbar_many(u_kn_list, N_k_list, f_k_init=None, compute_uncertainty=True, unce
                 r["boot_single"] = ns
                 if compute_uncertainty and uncertainty_method == "bootstrap":
                     r["dDelta_f"] = _bootstrap_std(fb)
-    return results
+        return results
+
+    # ---- estimators on the resident problems ----
+    def _entries(self, values, name):
+        P = len(self._probs)
+        if values is None:
+            return [None] * P
+        if len(values) != P:
+            raise ValueError(f"{name} must hold one entry (or None) per problem ({P}), got {len(values)}")
+        return list(values)
+
+    def _rows(self, p, a, name, allow_1d=True):
+        """a as float64 rows [L, N_p]; ParameterError for a shape that does not match N_p or for NaN."""
+        N = self._probs[p][0].shape[1]
+        a = np.asarray(a, dtype=np.float64)
+        if a.ndim == 1 and allow_1d:
+            a = a.reshape(1, -1)
+        if a.ndim != 2 or a.shape[1] != N or a.shape[0] < 1:
+            raise ParameterError(f"problem {p}: {name} has shape {a.shape}, the problem has N={N} samples")
+        if np.isnan(a).any():
+            raise ParameterError(f"problem {p}: {name} holds NaN")
+        return a
+
+    def _inner_many(self, requests, uncertainty_method, return_theta):
+        """expectations_inner of every request (requests[p] = (A_n, u_ln, state_map) or None): ([inner or None] per
+        problem, [path or None] per problem)."""
+        P = len(self._probs)
+        plans = {p: ex.augmentation(self._probs[p][0].shape[0], *req) for p, req in enumerate(requests)
+                 if req is not None}
+        batched, single = [], []
+        for p in sorted(plans):
+            R = self._probs[p][0].shape[0] + plans[p]["extra"].shape[0]
+            on_batch = self.results[p]["path"] == "batch" and p in self._slot
+            (batched if on_batch and R <= MAX_BATCH_ROWS else single).append(p)
+        inner = [None] * P
+        path = [None] * P
+        i = 0
+        while i < len(batched):
+            wave, used = [], 0
+            while i < len(batched):
+                p = batched[i]
+                need = augmented_bytes(*self._probs[p][0].shape, plans[p]["extra"].shape[0])
+                if wave and used + need > AUG_WAVE_BYTES:
+                    break
+                wave.append(p)
+                used += need
+                i += 1
+            single += self._wave(wave, plans, uncertainty_method, return_theta, inner, path)
+        if batched:
+            self._dev.set_unsampled([], [])
+        _, Prob = _classes()
+        for p in sorted(single):
+            u, N_k, _ = self._probs[p]
+            with Prob(u, N_k, device=ms._DEVICE) as q:
+                inner[p] = ex.expectations_inner(u, N_k, self.results[p]["f_k"], *requests[p],
+                                                 uncertainty_method=uncertainty_method, return_theta=return_theta,
+                                                 problem=q)
+            path[p] = "single"
+        return inner, path
+
+    def _count(self):
+        s = self._dev.last_stats()
+        self.device_stats["ms"] += s["ms"]
+        self.device_stats["launches"] += s["launches"]
+        self.device_stats["calls"] += 1
+
+    def _wave(self, wave, plans, uncertainty_method, return_theta, inner, path):
+        """One wave of batched problems: fills inner and path, returns the problems the device flagged."""
+        dev = self._dev
+        ids = [self._slot[p] for p in wave]
+        dev.set_unsampled(ids, [plans[p]["extra"] for p in wave])
+        f0 = [np.concatenate([self.results[p]["f_k"], np.zeros(plans[p]["extra"].shape[0])]) for p in wave]
+        sums = dev.augmented_moments(f0, problems=ids)
+        self._count()
+        flagged, ok, f_aug = [], [], {}
+        for p, f, m in zip(wave, f0, sums):
+            if m["flag"]:
+                flagged.append(p)
+                continue
+            K = self._probs[p][0].shape[0]
+            fa = f.copy()
+            fa[K:] = (f - m["log_S"])[K:]          # appended rows: the self-consistent update from f = 0
+            f_aug[p] = fa
+            ok.append(p)
+        G = {}
+        if ok and return_theta:
+            sums = dev.augmented_moments([f_aug[p] for p in ok], want_G=True, problems=[self._slot[p] for p in ok])
+            self._count()
+            for p, m in zip(ok, sums):
+                if m["flag"]:
+                    flagged.append(p)
+                    continue
+                G[p] = _gram_to_G(m["G"], self._N_aug(p, plans[p]))
+        for p in ok:
+            if return_theta and p not in G:
+                continue
+            inner[p] = ex.finish(plans[p], f_aug[p], G.get(p), self._N_aug(p, plans[p]),
+                                 uncertainty_method=uncertainty_method, return_theta=return_theta)
+            path[p] = "batch"
+        return flagged
+
+    def _N_aug(self, p, plan):
+        return np.concatenate([np.asarray(self._probs[p][1], dtype=np.float64), np.zeros(plan["extra"].shape[0])])
+
+    @staticmethod
+    def _method(uncertainty_method):
+        if uncertainty_method not in ESTIMATOR_METHODS:
+            raise ParameterError(f"uncertainty_method {uncertainty_method!r} is not served by MbarMany's estimators "
+                                 f"(one of {ESTIMATOR_METHODS}); bootstrap and 'svd' uncertainties are not served here")
+
+    def compute_perturbed_free_energies(self, u_ln_list, compute_uncertainty=True, uncertainty_method=None,
+                                        warning_cutoff=1.0e-10):
+        """Delta_f, dDelta_f (compute_uncertainty) of the states u_ln_list[p] [L, N_p] of each problem
+        (MBAR.compute_perturbed_free_energies)."""
+        self._method(uncertainty_method)
+        reqs = []
+        for p, u_ln in enumerate(self._entries(u_ln_list, "u_ln_list")):
+            if u_ln is None:
+                reqs.append(None)
+                continue
+            u_ln = self._rows(p, u_ln, "u_ln")
+            reqs.append((np.array([0.0]), u_ln, np.arange(u_ln.shape[0])))
+        inner, path = self._inner_many(reqs, uncertainty_method, bool(compute_uncertainty))
+        return [None if r is None else dict(ex.perturbed_result(r, compute_uncertainty, warning_cutoff), path=w)
+                for r, w in zip(inner, path)]
+
+    def compute_expectations(self, A_n_list, u_ln_list=None, output="averages", state_dependent=False,
+                             compute_uncertainty=True, uncertainty_method=None, warning_cutoff=1.0e-10,
+                             return_theta=False):
+        """mu, sigma (compute_uncertainty) and Theta (return_theta) of the observables A_n_list[p] ([N_p], or [L, N_p]
+        when state_dependent) at the states u_ln_list[p] [L, N_p] (the problem's own states when None)
+        (MBAR.compute_expectations)."""
+        self._method(uncertainty_method)
+        if output not in ("averages", "differences"):
+            raise ParameterError(f"output={output!r} must be 'averages' or 'differences'")
+        u_lns = self._entries(u_ln_list, "u_ln_list")
+        reqs, Ks = [], []
+        for p, A_n in enumerate(self._entries(A_n_list, "A_n_list")):
+            if A_n is None:
+                reqs.append(None)
+                Ks.append(0)
+                continue
+            u = self._probs[p][0] if u_lns[p] is None else self._rows(p, u_lns[p], "u_ln")
+            A = self._rows(p, A_n, "A_n")
+            if A.shape[0] != (u.shape[0] if state_dependent else 1):
+                raise ParameterError(f"problem {p}: A_n has {A.shape[0]} rows for {u.shape[0]} states "
+                                     f"(state_dependent={state_dependent})")
+            reqs.append((A, u, ex.expectation_state_map(u.shape[0], state_dependent)))
+            Ks.append(u.shape[0])
+        inner, path = self._inner_many(reqs, uncertainty_method, bool(compute_uncertainty or return_theta))
+        return [None if r is None else dict(ex.expectations_result(r, Ks[p], output, compute_uncertainty,
+                                                                   return_theta, warning_cutoff), path=path[p])
+                for p, r in enumerate(inner)]
+
+    def compute_entropy_and_enthalpy(self, u_ln_list=None, uncertainty_method=None, warning_cutoff=1.0e-10):
+        """Delta_f, dDelta_f, Delta_u, dDelta_u, Delta_s, dDelta_s of each problem at the states u_ln_list[p]
+        [L, N_p] (every problem at its own states when u_ln_list is None; an entry None skips its problem)
+        (MBAR.compute_entropy_and_enthalpy).  A problem's augmented rows number 3L; up to L = 64 they stay batched."""
+        self._method(uncertainty_method)
+        own = u_ln_list is None
+        u_lns = [None] * len(self._probs) if own else self._entries(u_ln_list, "u_ln_list")
+        reqs, Ls = [], []
+        for p, u_ln in enumerate(u_lns):
+            if u_ln is None and not own:
+                reqs.append(None)
+                Ls.append(0)
+                continue
+            u = self._probs[p][0] if own else self._rows(p, u_ln, "u_ln")
+            L = u.shape[0]
+            state_map = np.array([np.arange(L), np.arange(L)])
+            reqs.append((u, u, state_map))
+            Ls.append(L)
+        inner, path = self._inner_many(reqs, uncertainty_method, True)
+        return [None if r is None else dict(ex.entropy_enthalpy_result(r, Ls[p], warning_cutoff), path=path[p])
+                for p, r in enumerate(inner)]
+
+    def _grams(self):
+        """W^T W at the final f of every problem: the solve's where it computed one, one batched moments call for
+        the other batched problems, DeviceProblem.weight_moments for the rest."""
+        P = len(self._probs)
+        need = [p for p in range(P) if p not in self._G]
+        batched = [p for p in need if self.results[p]["path"] == "batch"]
+        if batched:
+            sums = self._dev.moments([self.results[p]["f_k"] for p in batched], want_G=True, all_rows=True,
+                                     problems=[self._slot[p] for p in batched])
+            self._count()
+            for p, m in zip(batched, sums):
+                if not m["flag"]:
+                    self._G[p] = _gram_to_G(m["G"], self._probs[p][1])
+        _, Prob = _classes()
+        for p in need:
+            if p not in self._G:
+                u, N_k, _ = self._probs[p]
+                with Prob(u, N_k, device=ms._DEVICE) as q:
+                    _, self._G[p] = q.weight_moments(self.results[p]["f_k"])
+        return [self._G[p] for p in range(P)]
+
+    def compute_overlap(self):
+        """scalar, eigenvalues, matrix of every problem (MBAR.compute_overlap), from W^T W at the final f.  A
+        one-state problem has no second eigenvalue: its scalar is NaN, where the reference raises."""
+        out = []
+        for p, G in enumerate(self._grams()):
+            N_k = self._probs[p][1]
+            if len(N_k) > 1:
+                d = estimators.overlap(G, N_k)
+            else:
+                O = np.asarray(N_k, dtype=np.float64) * np.asarray(G)
+                d = {"scalar": np.nan, "eigenvalues": np.linalg.eigvals(O), "matrix": O}
+            out.append(dict(d, path=self.results[p]["path"]))
+        return out
+
+    def compute_effective_sample_number(self):
+        """N_eff [K_p] of every problem (MBAR.compute_effective_sample_number), from W^T W at the final f."""
+        return [dict(N_eff=estimators.effective_sample_number(G), path=self.results[p]["path"])
+                for p, G in enumerate(self._grams())]
+
+
+def mbar_many(u_kn_list, N_k_list, f_k_init=None, compute_uncertainty=True, uncertainty_method=None,
+              return_theta=False, solver_tolerance=1.0e-12, options=None, n_bootstraps=0, rseed=None):
+    """MBAR on every problem (u_kn_list[p], N_k_list[p]): one dict per problem, in input order, with f_k, Delta_f,
+    dDelta_f (compute_uncertainty), Theta (return_theta), iterations (of the batched solve; None on the single path),
+    success and path ("batch" or "single").
+
+    f_k_init: None (zeros) or one starting vector per problem.  options update the adaptive solver's defaults
+    (min_sc_iter=0, gamma=1, maxiter=10000).  uncertainty_method: None, "svd-ew", "approximate" or "bootstrap".  Every
+    problem is validated before any device work; an invalid problem raises for the lowest failing index.
+
+    n_bootstraps = B > 0 adds f_k_boots [B, K] (replicate b of problem p is the one pymbar.MBAR(u_kn_list[p],
+    N_k_list[p], n_bootstraps=B, rseed=rseed[p]) draws) and boot_single (how many of them the single-problem path
+    solved) to every dict.  rseed: one seed per problem, or None for one np.random.randint(2**31 - 1) per problem in
+    problem order, as P constructions of MBAR would draw.  uncertainty_method="bootstrap" gives
+    dDelta_f = std over b of f_b - f_b^T and needs B > 0; its Theta is "svd-ew"."""
+    with MbarMany(u_kn_list, N_k_list, f_k_init=f_k_init, compute_uncertainty=compute_uncertainty,
+                  uncertainty_method=uncertainty_method, return_theta=return_theta, solver_tolerance=solver_tolerance,
+                  options=options, n_bootstraps=n_bootstraps, rseed=rseed) as m:
+        return m.results

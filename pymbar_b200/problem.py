@@ -718,6 +718,7 @@ class DeviceMbarBatch(_Resident):
 
     _destroy = "mbar_b200_batch_destroy"
     MAX_K = 64
+    MAX_ROWS = _lib.BATCH_MAX_ROWS     # K_p + M_p of a problem with appended rows
 
     def __init__(self, u_kn_list, N_k_list, device=0):
         self._lib = _lib.load()
@@ -731,6 +732,7 @@ class DeviceMbarBatch(_Resident):
                 raise ValueError(f"problem {p}: u_kn {u.shape} and N_k {n.shape} do not match")
         self.P = len(us)
         self.slot_problems = np.zeros(0, np.int32)
+        self.appended = np.zeros(self.P, np.int64)     # M_p: appended rows of each problem (set_unsampled)
         self.K = np.ascontiguousarray([u.shape[0] for u in us], dtype=np.int32)
         self.N = np.ascontiguousarray([u.shape[1] for u in us], dtype=np.int64)
         self.N_k = nks
@@ -829,9 +831,57 @@ class DeviceMbarBatch(_Resident):
                                                          _i32p(iters)))
         return np.split(f, np.cumsum(Ks)[:-1]), status, iters
 
+    def set_unsampled(self, problems, rows_list):
+        """Replace the resident appended rows: problem problems[i] gets the unsampled rows rows_list[i] [M_i, N_p]
+        on top of its own K_p (K_p + M_i <= MAX_ROWS), stored shifted by the problem's x_n.  NaN or -inf, a bad or
+        repeated problem index or too many rows raise the library's error and leave no appended rows.  An empty
+        `problems` drops them all."""
+        problems = np.ascontiguousarray(problems, dtype=np.int32).reshape(-1)
+        if len(rows_list) != problems.size:
+            raise ValueError(f"need one row block per problem: {problems.size} problems, {len(rows_list)} blocks")
+        parts = [np.asarray(r, dtype=np.float64) for r in rows_list]
+        parts = [r.reshape(1, -1) if r.ndim == 1 else r for r in parts]
+        for i, (p, r) in enumerate(zip(problems, parts)):
+            if r.ndim != 2 or (0 <= p < self.P and r.shape[1] != self.N[p]):
+                raise ValueError(f"entry {i}: rows {r.shape} do not match problem {p}")
+        M = np.ascontiguousarray([r.shape[0] for r in parts], dtype=np.int32)
+        flat = np.ascontiguousarray(np.concatenate([r.ravel() for r in parts]) if parts else np.zeros(0))
+        self.appended = np.zeros(self.P, np.int64)
+        check(self._lib.mbar_b200_batch_set_unsampled(self._h, problems.size, _i32p(problems), _i32p(M),
+                                                      _dptr(flat)))
+        self.appended[problems] = M
+
+    def augmented_moments(self, f_list, want_G=False, problems=None):
+        """One dict per request (f_list[r] [R_p] at problem problems[r], by default problem r; R_p = K_p + M_p rows,
+        the problem's own first): S [R_p], log_S [R_p], sum_L, flag and, with want_G, G = Ghat [R_p, R_p] (rows
+        scaled by N_k where sampled, by 1 otherwise).  L_n comes from the sampled rows alone.  Appended weights are not
+        shifted: ask for the Gram at a normalised f.  Two launches (three with the Gram) and one synchronisation for
+        all requests."""
+        ids = np.ascontiguousarray(np.arange(len(f_list)) if problems is None else problems, dtype=np.int32)
+        if ids.shape != (len(f_list),) or len(f_list) == 0:
+            raise ValueError("need one problem index per f vector, and at least one")
+        Rs = [int(self.K[i] + self.appended[i]) if 0 <= i < self.P else -1 for i in ids]
+        f = np.ascontiguousarray(np.concatenate([_f64(v, R) for v, R in zip(f_list, Rs)]))
+        S, logS = np.empty(f.size), np.empty(f.size)
+        sumL = np.empty(len(Rs))
+        flag = np.empty(len(Rs), np.int32)
+        G = np.empty(sum(R * R for R in Rs)) if want_G else None
+        check(self._lib.mbar_b200_batch_augmented_moments(self._h, len(Rs), _i32p(ids), _dptr(f), _dptr(S),
+                                                          _dptr(logS), _dptr(sumL), _i32p(flag),
+                                                          _dptr(G) if want_G else None))
+        out, o, g = [], 0, 0
+        for r, R in enumerate(Rs):
+            d = dict(S=S[o:o + R], log_S=logS[o:o + R], sum_L=float(sumL[r]), flag=bool(flag[r]))
+            if want_G:
+                d["G"] = G[g:g + R * R].reshape(R, R)
+            out.append(d)
+            o += R
+            g += R * R
+        return out
+
     def last_stats(self):
-        """CUDA-event time (ms) of the last moments, solve or solve_replicates call's kernels, its launches,
-        iterations and the bytes of u_kn tiles (and replicate counts) it read."""
+        """CUDA-event time (ms) of the last moments, solve, solve_replicates or augmented_moments call's kernels,
+        its launches, iterations and the bytes of u_kn tiles (appended tiles, replicate counts) it read."""
         ms, launches, iters, nbytes = C.c_double(0), C.c_int32(0), C.c_int32(0), C.c_int64(0)
         check(self._lib.mbar_b200_last_batch_stats(self._h, C.byref(ms), C.byref(launches), C.byref(iters),
                                                    C.byref(nbytes)))
