@@ -503,6 +503,19 @@ int mbar_b200_get_loop_stats(const mbar_b200_ctx* ctx, int64_t* polls, int32_t* 
 /* The adaptive iteration is captured into a CUDA graph after the first batch a context runs and relaunched once
  * per iteration: how often it was captured / launched (MBAR_B200_NO_GRAPH=1 disables the capture). */
 int mbar_b200_get_graph_stats(const mbar_b200_ctx* ctx, int64_t* captures, int64_t* launches);
+/* How the last mbar_b200_solve_adaptive on this context ran.  The Newton counters cover the device-resident loop
+ * only (the host-stepped loop retries its own factorisations, up to four times with a growing additive ridge). */
+typedef struct mbar_b200_adaptive_stats {
+    int32_t device_iterations;  /* iterations the device-resident loop completed and kept                       */
+    int32_t fell_back;          /* 1: the host-stepped loop finished the solve from the last polled f           */
+    int32_t ridge_retries;      /* factorisations of H[1:,1:] retried with the 1e-10 relative ridge             */
+    int32_t newton_failed;      /* iterations without a Newton candidate: the retry was not positive definite  */
+    int32_t newton_rejected;    /* Newton candidates rejected as non-finite or outside 0.5 C_RANGE              */
+    int32_t newton_threads;     /* CTA size of the Newton kernel, 0 when it never ran                            */
+    int32_t newton_smem;        /* 1: the matrix sat in shared memory, 0: the L2-resident variant ran           */
+    int32_t reserved;
+} mbar_b200_adaptive_stats;
+int mbar_b200_get_adaptive_stats(const mbar_b200_ctx* ctx, mbar_b200_adaptive_stats* stats);
 /* Run exactly `iters` self-consistent passes back to back with no host round trip (bench). */
 int mbar_b200_sci_iterate(mbar_b200_ctx* ctx, double* f_inout, int32_t iters);
 

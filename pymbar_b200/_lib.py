@@ -31,6 +31,11 @@ class SolveResult(C.Structure):
                 ("max_delta", C.c_double), ("gnorm", C.c_double), ("device_ms", C.c_double)]
 
 
+class AdaptiveStats(C.Structure):
+    _fields_ = [(name, C.c_int32) for name in ("device_iterations", "fell_back", "ridge_retries", "newton_failed",
+                                                 "newton_rejected", "newton_threads", "newton_smem", "reserved")]
+
+
 class Synth(C.Structure):
     _fields_ = [("seed", C.c_uint64), ("n_offset", C.c_int64), ("N_global", C.c_int64),
                 ("O_k", C.POINTER(C.c_double)), ("k_k", C.POINTER(C.c_double))]
@@ -129,6 +134,7 @@ SIGNATURES = {
     "mbar_b200_set_loop_mode": (C.c_int, [_ctx, C.c_int32, C.c_int32]),
     "mbar_b200_get_loop_stats": (C.c_int, [_ctx, C.POINTER(C.c_int64), C.POINTER(C.c_int32), C.POINTER(C.c_int32)]),
     "mbar_b200_get_graph_stats": (C.c_int, [_ctx, C.POINTER(C.c_int64), C.POINTER(C.c_int64)]),
+    "mbar_b200_get_adaptive_stats": (C.c_int, [_ctx, C.POINTER(AdaptiveStats)]),
     "mbar_b200_last_kernels": (C.c_int, [_ctx, C.c_char_p, C.c_char_p, C.c_int32]),
     "mbar_b200_last_hessian_ms": (C.c_int, [_ctx, _dp, _dp]),
     "mbar_b200_last_bin_stats": (C.c_int, [_ctx, _dp, C.POINTER(C.c_int32)]),

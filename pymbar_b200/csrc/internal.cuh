@@ -93,6 +93,9 @@ struct LoopState {
     int maxiter, min_sc_iter;
     int haveNr;          // this iteration has a valid Newton candidate
     int cholFail;        // last Cholesky attempt met a non-positive pivot
+    // per solve, for mbar_b200_get_adaptive_stats: factorisations retried with the ridge, iterations whose retry
+    // failed too, Newton candidates rejected as non-finite or out of range
+    int ridgeRetries, nrFailed, nrRejected, pad_;
     double tol, gamma;
     double max_delta, max_diff, gnorm;
     double gn_sci, gn_nr;
@@ -185,6 +188,7 @@ struct mbar_b200_ctx {
     int loopMode = 0;                    // 0 device-resident, 1 host-stepped (round-1 behaviour)
     int loopBatch = 4;                   // iterations enqueued between two polls of LoopState
     int64_t loopPolls = 0;               // host synchronisations spent polling LoopState
+    mbar_b200_adaptive_stats lastAdaptive{};   // how the last mbar_b200_solve_adaptive ran (loops.cu)
     // the adaptive iteration as a CUDA graph (captured once, relaunched per iteration; see loops.cu)
     bool capturing = false;              // stream capture in progress: no timing events, no allocations
     bool graphWarm = false;              // one uncaptured iteration has sized every buffer / kernel attribute

@@ -12,7 +12,7 @@
 //   adaptive:         pass(f) -> adapt_pre (g, f_sci) -> Hessian -> newton_build -> newton (Cholesky + solves,
 //                     f_nr) -> pass(f_sci), pass(f_nr) -> adapt_post (step choice :607, convergence :627-640)
 // Every kernel starts with `if (loop->done) return;`, so the host enqueues `loopBatch` iterations at a time and
-// reads the 96-byte LoopState once per batch.  Anything the fast path cannot represent (range flag of the fused
+// reads the 112-byte LoopState once per batch.  Anything the fast path cannot represent (range flag of the fused
 // kernel, an underflowing S_k, non-finite candidates) sets status = 1 and the host finishes on the robust
 // host-stepped loop, starting from the last good f.
 //
@@ -193,6 +193,7 @@ newton_kernel(double* __restrict__ Ag, int na, int K, const int* __restrict__ ac
               LoopState* loop) {
     if (loop_done(loop)) return;
     if (onlyIfFail && !*reinterpret_cast<volatile int*>(&loop->cholFail)) return;
+    if (onlyIfFail && threadIdx.x == 0) loop->ridgeRetries++;
     extern __shared__ __align__(16) double sm[];
     const int n = na - 1;
     const int tid = threadIdx.x, nt = blockDim.x;
@@ -245,7 +246,10 @@ newton_kernel(double* __restrict__ Ag, int na, int K, const int* __restrict__ ac
     if (s_fail) {
         if (tid == 0) {
             loop->cholFail = 1;
-            if (lastAttempt) loop->haveNr = 0;
+            if (lastAttempt) {
+                loop->haveNr = 0;
+                loop->nrFailed++;
+            }
         }
         if (lastAttempt)   // no Newton candidate this iteration: it coincides with the self-consistent one
             for (int k = tid; k < K; k += nt) {
@@ -293,6 +297,7 @@ newton_kernel(double* __restrict__ Ag, int na, int K, const int* __restrict__ ac
         if (tid == 0) {
             loop->haveNr = 0;
             loop->cholFail = 0;
+            loop->nrRejected++;
         }
         return;
     }
@@ -742,13 +747,14 @@ static int enqueue_sci(mbar_b200_ctx* c, FusedParams p, bool inKernel, int n, Lo
 // The batches of a device-resident solver.  batch(f, &ok) configures the fused pass at f (ok = false: it does not
 // apply), uploads f and enqueues one batch of iterations; then LoopState and f come back in the batch's one
 // synchronisation.  On return cur holds the last f the device reported.  *fallback: the fast path gave up, cur is
-// the f that batch started from, after *itersBefore iterations, and the caller finishes on its host-stepped loop.
-static int poll_batches(mbar_b200_ctx* c, std::vector<double>& cur, int* itersBefore, bool* fallback,
+// the f that batch started from and *good the LoopState polled with it (its iteration counters are the ones that
+// led to cur; a failed batch's own steps are redone), and the caller finishes on its host-stepped loop.
+static int poll_batches(mbar_b200_ctx* c, std::vector<double>& cur, LoopState* good, bool* fallback,
                         const std::function<int(const double*, bool*)>& batch) {
     const int K = c->K;
     *fallback = false;
     for (;;) {
-        *itersBefore = c->h_loop->iterations;
+        *good = *c->h_loop;
         bool ok = false;
         MBAR_TRY(batch(cur.data(), &ok));
         if (!ok) {
@@ -787,9 +793,9 @@ static int solve_sci_device(mbar_b200_ctx* c, double* f, double tol, int32_t max
     MBAR_TRY(loop_begin(c, tol, maxiter, 0, 1.0));
     const bool inKernel = sci_epilogue_in_kernel(c);
     if (c->peerReady && inKernel) MBAR_TRY(comm_rendezvous(c));
-    int itersBefore = 0;
+    LoopState good{};
     bool fallback = false;
-    MBAR_TRY(poll_batches(c, cur, &itersBefore, &fallback, [&](const double* fb, bool* ok) -> int {
+    MBAR_TRY(poll_batches(c, cur, &good, &fallback, [&](const double* fb, bool* ok) -> int {
         FusedParams p;
         MBAR_TRY(fused_prepare(c, fb, false, false, &p, ok));
         if (!*ok) return MBAR_B200_OK;
@@ -800,6 +806,7 @@ static int solve_sci_device(mbar_b200_ctx* c, double* f, double tol, int32_t max
     int rc;
     if (fallback) {
         // redo from the last good f on the robust path (generic kernel, log-domain sums)
+        const int itersBefore = good.iterations;
         rc = solve_sci_stepped(c, cur.data(), tol, std::max(maxiter - itersBefore, 1), &r);
         r.iterations += itersBefore;
         r.sci_iterations += itersBefore;
@@ -819,6 +826,11 @@ static int solve_sci_device(mbar_b200_ctx* c, double* f, double tol, int32_t max
     return rc;
 }
 
+// Launch plan of newton_kernel for an n x n system: the matrix in shared memory when it fits (n <= 158), and a CTA of
+// 256, 512 or 1024 threads (four per row of the column update).
+static bool newton_in_smem(int n) { return (size_t)n * n * 8 + 2 * ((size_t)n + 2) * 8 <= 200 * 1024; }
+static int newton_threads(int n) { return n >= 96 ? 1024 : n >= 32 ? 512 : 256; }
+
 // One adaptive iteration, enqueued with no host synchronisation.
 static int enqueue_adaptive_iteration(mbar_b200_ctx* c, const FusedParams& pF, const FusedParams& pS,
                                       const FusedParams& pN, const FusedParams* pM) {
@@ -837,7 +849,7 @@ static int enqueue_adaptive_iteration(mbar_b200_ctx* c, const FusedParams& pF, c
     MBAR_TRY(launch_hessian_dev(c, av + AV_CH * K, false, c->d_loop, pF.Wout != nullptr));
     if (c->nranks > 1) MBAR_TRY(comm_allreduce(c, c->d_out + lay.G(), K * K, 0));
     // (3) Newton candidate: build, factorise, solve; one retry with a relative ridge if not positive definite
-    const bool smem = (size_t)n * n * 8 + 2 * ((size_t)n + 2) * 8 <= 200 * 1024;
+    const bool smem = newton_in_smem(n);
     const size_t shBytes = 2 * ((size_t)n + 2) * 8 + (smem ? (size_t)n * n * 8 : 0);
     auto kern = smem ? newton_kernel<true> : newton_kernel<false>;
     static size_t attr[16][2] = {{0}};
@@ -847,7 +859,7 @@ static int enqueue_adaptive_iteration(mbar_b200_ctx* c, const FusedParams& pF, c
         a = shBytes;
     }
     const int bgrid = (int)std::min<int64_t>(((int64_t)n * n + 255) / 256, 4 * c->smCount);
-    const int nthreads = n >= 96 ? 1024 : n >= 32 ? 512 : 256;
+    const int nthreads = newton_threads(n);
     for (int attempt = 0; attempt < 2; ++attempt) {
         newton_build_kernel<<<bgrid, 256, 0, c->stream>>>(c->d_out + lay.G(), av, c->d_active, na, K, c->d_A,
                                                          attempt ? 1.0e-10 : 0.0, attempt, c->d_loop);
@@ -968,9 +980,9 @@ static int solve_adaptive_device(mbar_b200_ctx* c, double* f, double tol, int32_
     MBAR_TRY(loop_begin(c, tol, maxiter, min_sc_iter, gamma));
     if (c->peerReady) MBAR_TRY(comm_rendezvous(c));
     bool usedM2 = false;
-    int itersBefore = 0;
+    LoopState good{};
     bool fallback = false;
-    MBAR_TRY(poll_batches(c, cur, &itersBefore, &fallback, [&](const double* fb, bool* ok) -> int {
+    MBAR_TRY(poll_batches(c, cur, &good, &fallback, [&](const double* fb, bool* ok) -> int {
         FusedParams pF;
         MBAR_TRY(fused_prepare(c, fb, true, false, &pF, ok, nullptr, nullptr, true, 1, 16.0));
         if (!*ok) return MBAR_B200_OK;
@@ -1010,12 +1022,27 @@ static int solve_adaptive_device(mbar_b200_ctx* c, double* f, double tol, int32_
     const LoopState st = *c->h_loop;
     mbar_b200_solve_result r{};
     int rc = MBAR_B200_OK;
+    mbar_b200_adaptive_stats& as = c->lastAdaptive;
+    as.ridge_retries = st.ridgeRetries;
+    as.newton_failed = st.nrFailed;
+    as.newton_rejected = st.nrRejected;
+    as.fell_back = fallback;
+    as.device_iterations = fallback ? good.iterations : st.iterations;
+    if (st.iterations > 0) {
+        const int n = (int)c->active.size() - 1;
+        as.newton_threads = newton_threads(n);
+        as.newton_smem = newton_in_smem(n);
+    }
     if (fallback) {
-        const int msi = std::max(min_sc_iter - st.sci_iterations, 0);
-        rc = solve_adaptive_stepped(c, cur.data(), tol, std::max(maxiter - itersBefore, 1), msi, gamma, &r);
-        r.iterations += itersBefore;
-        r.passes += passesPerIter * itersBefore;
-        r.hessian_passes += itersBefore;
+        // the stepped loop continues from the last good poll: its counters, and what is left of min_sc_iter,
+        // start from that poll's (a failed batch's steps are redone, so they are not counted)
+        const int msi = std::max(min_sc_iter - good.sci_iterations, 0);
+        rc = solve_adaptive_stepped(c, cur.data(), tol, std::max(maxiter - good.iterations, 1), msi, gamma, &r);
+        r.iterations += good.iterations;
+        r.nr_iterations += good.nr_iterations;
+        r.sci_iterations += good.sci_iterations;
+        r.passes += passesPerIter * good.iterations;
+        r.hessian_passes += good.iterations;
     } else {
         r.iterations = st.iterations;
         r.nr_iterations = st.nr_iterations;
@@ -1050,6 +1077,7 @@ int mbar_b200_solve_adaptive(mbar_b200_ctx* c, double* f, double tol, int32_t ma
                              double gamma, mbar_b200_solve_result* res) {
     MBAR_REQUIRE(c && f, MBAR_B200_ERR_INVALID, "NULL argument");
     NvtxRange nvtx_("mbar_b200::solve_adaptive");
+    c->lastAdaptive = mbar_b200_adaptive_stats{};
     if (c->loopMode == 1) return solve_adaptive_stepped(c, f, tol, maxiter, min_sc_iter, gamma, res);
     return solve_adaptive_device(c, f, tol, maxiter, min_sc_iter, gamma, res);
 }
@@ -1074,6 +1102,12 @@ int mbar_b200_get_graph_stats(const mbar_b200_ctx* c, int64_t* captures, int64_t
     MBAR_REQUIRE(c, MBAR_B200_ERR_INVALID, "ctx is NULL");
     if (captures) *captures = c->graphCaptures;
     if (launches) *launches = c->graphLaunches;
+    return MBAR_B200_OK;
+}
+
+int mbar_b200_get_adaptive_stats(const mbar_b200_ctx* c, mbar_b200_adaptive_stats* stats) {
+    MBAR_REQUIRE(c && stats, MBAR_B200_ERR_INVALID, "NULL argument");
+    *stats = c->lastAdaptive;
     return MBAR_B200_OK;
 }
 

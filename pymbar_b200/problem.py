@@ -10,7 +10,7 @@ import ctypes as C
 import numpy as np
 
 from . import _lib
-from ._lib import SolveResult, check
+from ._lib import AdaptiveStats, SolveResult, check
 
 
 def _dptr(a):
@@ -410,6 +410,17 @@ class DeviceProblem(_Resident):
         check(self._lib.mbar_b200_get_graph_stats(self._h, C.byref(cap), C.byref(lau)))
         return dict(polls=polls.value, mode="stepped" if mode.value else "device", batch=batch.value,
                     graph_captures=cap.value, graph_launches=lau.value)
+
+    def adaptive_stats(self):
+        """How the last solve_adaptive ran: iterations the device-resident loop kept, whether the host-stepped loop
+        finished the solve, the device Newton step's ridge retries, failed and rejected candidates, and its launch
+        plan (CTA size, matrix in shared memory or not)."""
+        st = AdaptiveStats()
+        check(self._lib.mbar_b200_get_adaptive_stats(self._h, C.byref(st)))
+        d = {name: getattr(st, name) for name, _ in AdaptiveStats._fields_ if name != "reserved"}
+        d["fell_back"] = bool(d["fell_back"])
+        d["newton_smem"] = bool(d["newton_smem"])
+        return d
 
     def last_kernels(self):
         a, b = C.create_string_buffer(256), C.create_string_buffer(256)
