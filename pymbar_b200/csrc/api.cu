@@ -169,7 +169,7 @@ int run_pass(mbar_b200_ctx* c, const double* f, PassWant want) {
         MBAR_CUDA(cudaStreamSynchronize(c->stream));
         c->d2hBytes += (int64_t)lay.size(false) * 8;
         float ms = 0.f;
-        if (event_ms(c->evA, c->evB, &ms)) c->lastPassMs = ms;
+        if (event_ms(c->ev0, c->ev1, &ms)) c->lastPassMs = ms;
         if (fused && c->h_out[lay.flag()] != 0.0) continue;   // range assumption failed on a sample
         if (fused && needUnsampled) {
             // unsampled states rode along with weight e^-80: valid only while their weight sums are
@@ -347,8 +347,8 @@ int mbar_b200_last_hessian_ms(mbar_b200_ctx* c, double* weights_ms, double* hess
     MBAR_CUDA(cudaSetDevice(c->device));
     MBAR_CUDA(cudaStreamSynchronize(c->stream));
     float a = 0.f, b = 0.f;
-    if (cudaEventElapsedTime(&a, c->evH0, c->evH1) != cudaSuccess) { cudaGetLastError(); a = 0.f; }
-    if (cudaEventElapsedTime(&b, c->evH1, c->evH2) != cudaSuccess) { cudaGetLastError(); b = 0.f; }
+    if (cudaEventElapsedTime(&a, c->evH[0], c->evH[1]) != cudaSuccess) { cudaGetLastError(); a = 0.f; }
+    if (cudaEventElapsedTime(&b, c->evH[1], c->evH[2]) != cudaSuccess) { cudaGetLastError(); b = 0.f; }
     if (weights_ms) *weights_ms = a;
     if (hessian_ms) *hessian_ms = b;
     return MBAR_B200_OK;
@@ -509,9 +509,10 @@ int mbar_b200_peer_export(mbar_b200_ctx* c, void* handle_out) {
     MBAR_REQUIRE(c && handle_out, MBAR_B200_ERR_INVALID, "NULL argument");
     MBAR_CUDA(cudaSetDevice(c->device));
     if (!c->d_inbox) {
-        const size_t bytes = inbox_doubles(c->K) * sizeof(double) + 2 * MAX_PEERS * sizeof(unsigned long long);
-        MBAR_CUDA(cudaMalloc((void**)&c->d_inbox, bytes));
-        MBAR_CUDA(cudaMemset(c->d_inbox, 0, bytes));
+        // the inbox, then the [2][MAX_PEERS] flags (8 bytes each, like a double)
+        const size_t count = inbox_doubles(c->K) + 2 * MAX_PEERS;
+        MBAR_TRY(c->d_inbox.reserve(count, "peer_export"));
+        MBAR_CUDA(cudaMemset(c->d_inbox, 0, count * sizeof(double)));
     }
     cudaIpcMemHandle_t h;
     MBAR_CUDA(cudaIpcGetMemHandle(&h, c->d_inbox));

@@ -147,16 +147,11 @@ struct mbar_b200_batch : mbar::Resident {
     // per-call buffers, grown on demand
     mbar::DevArray<mbar::BatchReq> d_req;
     mbar::DevArray<double> d_f, d_part, d_out;
-    double* h_f = nullptr;                      // pinned staging of f and of the packed output
-    double* h_out = nullptr;
-    size_t h_fCap = 0, h_outCap = 0;
+    mbar::HostPinned<double> h_f;               // pinned staging of f and of the packed output
+    mbar::HostPinned<double> h_out;
     // the last moments / solve call
     int32_t lastLaunches = 0, lastIterations = 0;
     int64_t lastBytes = 0;
-    ~mbar_b200_batch() {
-        if (h_f) cudaFreeHost(h_f);
-        if (h_out) cudaFreeHost(h_out);
-    }
 };
 
 namespace mbar {
@@ -462,24 +457,6 @@ __global__ void __launch_bounds__(BATCH_THREADS) batch_finalize_kernel(const Bat
     if (tid == 0) o[2 * K + 1] = sFlag ? 1.0 : 0.0;
 }
 
-template <class T>
-static int batch_grow(DevArray<T>& a, int64_t count) {
-    if ((size_t)count <= a.cap) return MBAR_B200_OK;
-    return a.reserve((size_t)(count + count / 2 + 64), "batch");
-}
-
-static int pinned_grow(double** p, size_t* cap, size_t count) {
-    if (count <= *cap) return MBAR_B200_OK;
-    if (*p) cudaFreeHost(*p);
-    *p = nullptr;
-    *cap = 0;
-    const size_t n = count + count / 2 + 64;
-    MBAR_REQUIRE(cudaMallocHost((void**)p, n * sizeof(double)) == cudaSuccess, MBAR_B200_ERR_NOMEM,
-                 "batch: cannot allocate %zu bytes of pinned host memory", n * sizeof(double));
-    *cap = n;
-    return MBAR_B200_OK;
-}
-
 // One request of a moments launch: f (K_p values) at unit `id` — problem id, or replicate slot id when the launch is
 // weighted.
 struct Ask {
@@ -541,12 +518,12 @@ static int batch_run(mbar_b200_batch* b, const std::vector<Ask>& asks, bool allR
         if (q.wantG) maxKG = std::max(maxKG, q.K);
     }
     MBAR_REQUIRE(items < INT32_MAX, MBAR_B200_ERR_INVALID, "batch: %lld chunks in one call", (long long)items);
-    MBAR_TRY(batch_grow(b->d_req, nReq));
-    MBAR_TRY(batch_grow(b->d_f, fs));
-    MBAR_TRY(batch_grow(b->d_part, parts));
-    MBAR_TRY(batch_grow(b->d_out, outs));
-    MBAR_TRY(pinned_grow(&b->h_f, &b->h_fCap, (size_t)fs + (size_t)nReq * sizeof(BatchReq) / 8 + 1));
-    MBAR_TRY(pinned_grow(&b->h_out, &b->h_outCap, (size_t)outs));
+    MBAR_TRY(b->d_req.grow(nReq, "batch"));
+    MBAR_TRY(b->d_f.grow(fs, "batch"));
+    MBAR_TRY(b->d_part.grow(parts, "batch"));
+    MBAR_TRY(b->d_out.grow(outs, "batch"));
+    MBAR_TRY(b->h_f.grow((size_t)fs + (size_t)nReq * sizeof(BatchReq) / 8 + 1, "batch"));
+    MBAR_TRY(b->h_out.grow((size_t)outs, "batch"));
     for (int r = 0; r < nReq; ++r) std::memcpy(b->h_f + req[r].foff, asks[r].f, (size_t)req[r].K * sizeof(double));
     BatchReq* hreq = reinterpret_cast<BatchReq*>(b->h_f + fs);
     std::memcpy(hreq, req.data(), req.size() * sizeof(BatchReq));
@@ -1055,17 +1032,17 @@ static int batch_aug_run(mbar_b200_batch* b, int nReq, const int32_t* problem, c
     }
     MBAR_REQUIRE(items < INT32_MAX && gitems < INT32_MAX, MBAR_B200_ERR_INVALID, "batch: %lld chunks in one call",
                  (long long)(items + gitems));
-    MBAR_TRY(batch_grow(b->d_areq, nReq));
-    MBAR_TRY(batch_grow(b->d_f, fs));
-    MBAR_TRY(batch_grow(b->d_part, parts));
-    MBAR_TRY(batch_grow(b->d_out, outs));
+    MBAR_TRY(b->d_areq.grow(nReq, "batch"));
+    MBAR_TRY(b->d_f.grow(fs, "batch"));
+    MBAR_TRY(b->d_part.grow(parts, "batch"));
+    MBAR_TRY(b->d_out.grow(outs, "batch"));
     if (wantG) {
-        MBAR_TRY(batch_grow(b->d_gpart, gparts));
-        MBAR_TRY(batch_grow(b->d_L, Ls));
+        MBAR_TRY(b->d_gpart.grow(gparts, "batch"));
+        MBAR_TRY(b->d_L.grow(Ls, "batch"));
         MBAR_TRY(aug_smem_attr(b->device));
     }
-    MBAR_TRY(pinned_grow(&b->h_f, &b->h_fCap, (size_t)fs + (size_t)nReq * sizeof(AugReq) / 8 + 1));
-    MBAR_TRY(pinned_grow(&b->h_out, &b->h_outCap, (size_t)outs));
+    MBAR_TRY(b->h_f.grow((size_t)fs + (size_t)nReq * sizeof(AugReq) / 8 + 1, "batch"));
+    MBAR_TRY(b->h_out.grow((size_t)outs, "batch"));
     std::memcpy(b->h_f, f, (size_t)fs * sizeof(double));
     AugReq* hreq = reinterpret_cast<AugReq*>(b->h_f + fs);
     std::memcpy(hreq, req.data(), req.size() * sizeof(AugReq));

@@ -322,16 +322,9 @@ int mbar_b200_bin_moments(mbar_b200_ctx* c, const double* f_k, const double* u_n
     MBAR_CUDA(cudaMemsetAsync(d_flag, 0, sizeof(int), s));
     MBAR_CUDA(cudaMemsetAsync(d_keys, 0, (size_t)nbins * sizeof(unsigned long long), s));
     c->h2dBytes += N * 12 + K * 8;
-    struct Events {
-        cudaEvent_t e[2] = {nullptr, nullptr};
-        ~Events() {
-            for (cudaEvent_t x : e)
-                if (x) cudaEventDestroy(x);
-        }
-    } ev;
-    MBAR_CUDA(cudaEventCreate(&ev.e[0]));
-    MBAR_CUDA(cudaEventCreate(&ev.e[1]));
-    MBAR_CUDA(cudaEventRecord(ev.e[0], s));
+    Events ev;
+    MBAR_TRY(ev.create(2));
+    MBAR_CUDA(cudaEventRecord(ev[0], s));
     bin_prep_kernel<<<(unsigned)((nPad + 255) / 256), 256, 0, s>>>(N, nPad, nbins, d_bin, d_lw, c->d_L, c->d_xshift,
                                                                    c->d_wgt, d_keys, d_flag);
     bin_max_kernel<<<(nbins + 255) / 256, 256, 0, s>>>(nbins, d_keys, d_m, d_o, d_flag);
@@ -360,12 +353,12 @@ int mbar_b200_bin_moments(mbar_b200_ctx* c, const double* f_k, const double* u_n
         p.nrows = K + 1;
         MBAR_TRY(run_accum(c, p, nbins, d_out, d_partial, momPlan));
     }
-    MBAR_CUDA(cudaEventRecord(ev.e[1], s));
+    MBAR_CUDA(cudaEventRecord(ev[1], s));
     int flag = 0;
     MBAR_CUDA(cudaMemcpyAsync(&flag, d_flag, sizeof(int), cudaMemcpyDeviceToHost, s));
     MBAR_CUDA(cudaStreamSynchronize(s));
     float ms = 0.f;
-    if (event_ms(ev.e[0], ev.e[1], &ms)) c->lastBinMs = ms;
+    if (event_ms(ev[0], ev[1], &ms)) c->lastBinMs = ms;
     c->lastBinChunks = wantC ? momPlan.chunks : 0;
     MBAR_REQUIRE(!(flag & BINF_INVALID), MBAR_B200_ERR_INVALID, "bin_moments: a bin index lies outside [0, %d)",
                  (int)nbins);

@@ -14,6 +14,7 @@
 #include <cstdlib>
 #include <condition_variable>
 #include <functional>
+#include <memory>
 #include <mutex>
 #include <thread>
 
@@ -169,28 +170,28 @@ struct Parked {
     void* ptr = nullptr;
     size_t bytes = 0;
 };
-struct DevicePool {
-    Parked u, stageDev[2], stagePin[2];
-};
-static DevicePool g_pool[16];
+static Parked g_pool[16][POOL_KINDS];   // per device: POOL_U, POOL_STAGE_DEV + i, POOL_STAGE_PIN + i
 static std::mutex g_poolMutex;
-static bool pool_enabled() {
+bool pool_enabled() {
     static const bool off = std::getenv("MBAR_B200_NO_POOL") != nullptr;
     return !off;
 }
 // take a parked buffer of at least `bytes` (and at most 2x, so a small problem never pins a huge buffer)
-static void* pool_take(Parked& slot, size_t bytes) {
+void* pool_take(int device, int kind, size_t bytes, size_t* got) {
     std::lock_guard<std::mutex> g(g_poolMutex);
+    Parked& slot = g_pool[device & 15][kind];
     if (slot.ptr && slot.bytes >= bytes && slot.bytes <= 2 * bytes + (1u << 20)) {
         void* p = slot.ptr;
+        *got = slot.bytes;
         slot = Parked{};
         return p;
     }
     return nullptr;
 }
 // park `ptr`; whatever was parked there before is returned to the caller for release
-static void* pool_park(Parked& slot, void* ptr, size_t bytes) {
+void* pool_park(int device, int kind, void* ptr, size_t bytes) {
     std::lock_guard<std::mutex> g(g_poolMutex);
+    Parked& slot = g_pool[device & 15][kind];
     void* old = slot.ptr;
     slot.ptr = ptr;
     slot.bytes = bytes;
@@ -358,23 +359,31 @@ __global__ void __launch_bounds__(256) wprep_kernel(const double* __restrict__ w
     }
 }
 
+// d_wgt and d_sqrtw exist together or not at all: reduce_sumxw writes d_sqrtw whenever d_wgt is set
+static int reserve_weights(mbar_b200_ctx* ctx) {
+    const size_t nPad = (size_t)ctx->nTiles * TILE_N;
+    int rc = ctx->d_wgt.reserve(nPad, "sample weights");
+    if (rc == MBAR_B200_OK) rc = ctx->d_sqrtw.reserve(nPad, "sample weights");
+    if (rc != MBAR_B200_OK) {
+        ctx->d_wgt.reset();
+        ctx->d_sqrtw.reset();
+    }
+    return rc;
+}
+
 int set_weights(mbar_b200_ctx* ctx, const double* w_host) {
     if (!w_host) {
-        cudaFree(ctx->d_wgt);
-        cudaFree(ctx->d_sqrtw);
-        ctx->d_wgt = ctx->d_sqrtw = nullptr;
+        ctx->d_wgt.reset();
+        ctx->d_sqrtw.reset();
         return MBAR_B200_OK;
     }
     const size_t nPad = (size_t)ctx->nTiles * TILE_N;
-    if (!ctx->d_wgt) {
-        MBAR_CUDA(cudaMalloc((void**)&ctx->d_wgt, nPad * sizeof(double)));
-        MBAR_CUDA(cudaMalloc((void**)&ctx->d_sqrtw, nPad * sizeof(double)));
-    }
     double sw = 0.0;
     for (int64_t i = 0; i < ctx->N; ++i) {
         MBAR_REQUIRE(w_host[i] >= 0.0, MBAR_B200_ERR_INVALID, "sample weight %lld is negative or NaN", (long long)i);
         sw += w_host[i];
     }
+    MBAR_TRY(reserve_weights(ctx));
     ctx->sumW = sw;
     MBAR_CUDA(cudaMemsetAsync(ctx->d_wgt, 0, nPad * sizeof(double), ctx->stream));
     MBAR_CUDA(cudaMemsetAsync(ctx->d_sqrtw, 0, nPad * sizeof(double), ctx->stream));
@@ -557,12 +566,13 @@ int mbar_b200_host_alloc(void** ptr, uint64_t bytes) {
     MBAR_REQUIRE(ptr, MBAR_B200_ERR_INVALID, "ptr is NULL");
     int dev = 0;
     cudaGetDevice(&dev);
-    NumaPrefer numa(dev);
-    MBAR_CUDA(cudaHostAlloc(ptr, bytes, cudaHostAllocDefault));
+    unsigned char* p = nullptr;
+    MBAR_TRY(host_alloc(&p, (size_t)bytes, "mbar_b200_host_alloc", dev));
+    *ptr = p;
     return MBAR_B200_OK;
 }
 int mbar_b200_host_free(void* ptr) {
-    if (ptr) MBAR_CUDA(cudaFreeHost(ptr));
+    MBAR_CUDA(mem_free(ptr, true));
     return MBAR_B200_OK;
 }
 
@@ -617,8 +627,7 @@ int mbar_b200_create(mbar_b200_ctx** out, int device, int32_t K, int64_t N_local
     MBAR_REQUIRE(N_local >= 1, MBAR_B200_ERR_INVALID, "N_local=%lld must be >= 1", (long long)N_local);
     cudaDeviceProp prop;
     MBAR_TRY(open_device(device, &prop));
-    mbar_b200_ctx* c = new mbar_b200_ctx();
-    c->device = device;
+    std::unique_ptr<mbar_b200_ctx> c(new mbar_b200_ctx());
     c->K = K;
     c->N = N_local;
     c->nTiles = (N_local + TILE_N - 1) / TILE_N;
@@ -628,11 +637,7 @@ int mbar_b200_create(mbar_b200_ctx** out, int device, int32_t K, int64_t N_local
     c->h_logNkEff.resize(K);
     std::vector<unsigned long long> mask((K + 63) / 64, 0ull);
     for (int k = 0; k < K; ++k) {
-        if (!(N_k[k] >= 0.0)) {
-            delete c;
-            set_error("N_k[%d]=%g is negative or NaN", k, N_k[k]);
-            return MBAR_B200_ERR_INVALID;
-        }
+        MBAR_REQUIRE(N_k[k] >= 0.0, MBAR_B200_ERR_INVALID, "N_k[%d]=%g is negative or NaN", k, N_k[k]);
         c->N_total_states += N_k[k];
         if (N_k[k] > 0) {
             c->active.push_back(k);
@@ -644,153 +649,75 @@ int mbar_b200_create(mbar_b200_ctx** out, int device, int32_t K, int64_t N_local
             c->h_logNkEff[k] = LOG_EPS_UNSAMPLED;
         }
     }
-    if (c->active.empty()) {
-        delete c;
-        set_error("all N_k are zero");
-        return MBAR_B200_ERR_INVALID;
-    }
+    MBAR_REQUIRE(!c->active.empty(), MBAR_B200_ERR_INVALID, "all N_k are zero");
     c->firstActive = c->active[0];
 
-    const size_t uBytes = (size_t)c->nTiles * K * TILE_N * sizeof(double);
     const size_t nPad = (size_t)c->nTiles * TILE_N;
     const PassLayout lay{K};
-#define ALLOC(p, bytes)                                                        \
-    do {                                                                       \
-        cudaError_t e = cudaMalloc((void**)&(p), (bytes));                     \
-        if (e != cudaSuccess) {                                                \
-            set_error("cudaMalloc(%zu bytes) failed: %s", (size_t)(bytes), cudaGetErrorString(e)); \
-            mbar_b200_destroy(c);                                              \
-            return MBAR_B200_ERR_NOMEM;                                        \
-        }                                                                      \
-    } while (0)
-    c->uBytes = uBytes;
-    if (pool_enabled()) {
-        c->d_u = static_cast<double*>(pool_take(g_pool[device & 15].u, uBytes));
-        if (c->d_u) c->uBytes = 0;   // size unknown to this context; keep parking the original size
-    }
-    if (!c->d_u) ALLOC(c->d_u, uBytes);
-    ALLOC(c->d_xshift, nPad * sizeof(double));
-    ALLOC(c->d_c, DC_ROWS * (size_t)K * sizeof(double));
-    ALLOC(c->d_Nk, (size_t)K * sizeof(double));
-    ALLOC(c->d_NkEff, (size_t)K * sizeof(double));
-    ALLOC(c->d_rowmask, mask.size() * sizeof(unsigned long long));
-    ALLOC(c->d_zeromask, mask.size() * sizeof(unsigned long long));
-    ALLOC(c->d_onesmask, mask.size() * sizeof(unsigned long long));
-    ALLOC(c->d_partial, (size_t)MAX_GRID * (3 * (size_t)K + 2) * sizeof(double));
-    ALLOC(c->d_out, (size_t)lay.size(true) * sizeof(double));
-    ALLOC(c->d_ticket, 4 * sizeof(unsigned int));
-    ALLOC(c->d_flag, 4 * sizeof(int));
-    ALLOC(c->d_urowmin, 2 * (size_t)K * sizeof(int));
-    ALLOC(c->d_urowfar, (size_t)K * sizeof(unsigned long long));
+    const char* who = "mbar_b200_create";
+    MBAR_TRY(c->d_u.acquire(device, POOL_U, (size_t)c->nTiles * K * TILE_N, who));
+    MBAR_TRY(c->d_xshift.reserve(nPad, who));
+    MBAR_TRY(c->d_c.reserve(DC_ROWS * (size_t)K, who));
+    MBAR_TRY(c->d_Nk.reserve((size_t)K, who));
+    MBAR_TRY(c->d_NkEff.reserve((size_t)K, who));
+    MBAR_TRY(c->d_rowmask.reserve(mask.size(), who));
+    MBAR_TRY(c->d_zeromask.reserve(mask.size(), who));
+    MBAR_TRY(c->d_onesmask.reserve(mask.size(), who));
+    MBAR_TRY(c->d_partial.reserve((size_t)MAX_GRID * (3 * (size_t)K + 2), who));
+    MBAR_TRY(c->d_out.reserve((size_t)lay.size(true), who));
+    MBAR_TRY(c->d_ticket.reserve(4, who));
+    MBAR_TRY(c->d_flag.reserve(4, who));
+    MBAR_TRY(c->d_urowmin.reserve(2 * (size_t)K, who));
+    MBAR_TRY(c->d_urowfar.reserve((size_t)K, who));
     c->h_urowmin.assign(K, 0.0);
     c->h_uclamp.assign(K, 0.0);
     c->h_ufar.assign(K, 0.0);
-    ALLOC(c->d_f, (size_t)K * sizeof(double));
-    ALLOC(c->d_scratch, (scratch_rendezvous(K) + 1024) * sizeof(double));
-    ALLOC(c->d_loop, sizeof(mbar::LoopState));
-    ALLOC(c->d_av, 8 * (size_t)K * sizeof(double));
-    ALLOC(c->d_outM, 2 * (size_t)lay.size(false) * sizeof(double));
-    ALLOC(c->d_A, (size_t)K * K * sizeof(double));
-    ALLOC(c->d_active, (size_t)K * sizeof(int));
-    ALLOC(c->d_seq, sizeof(unsigned long long));
-#undef ALLOC
-    // failures past this point must release what was allocated above (ADVICE r1)
-#define CREATE_CUDA(call)                                                                   \
-    do {                                                                                    \
-        cudaError_t e__ = (call);                                                           \
-        if (e__ != cudaSuccess) {                                                           \
-            set_error("%s failed at %s:%d: %s", #call, __FILE__, __LINE__,                  \
-                      cudaGetErrorString(e__));                                             \
-            mbar_b200_destroy(c);                                                           \
-            return MBAR_B200_ERR_CUDA;                                                      \
-        }                                                                                   \
-    } while (0)
-    CREATE_CUDA(cudaHostAlloc((void**)&c->h_loop, sizeof(mbar::LoopState), cudaHostAllocDefault));
-    CREATE_CUDA(cudaMemset(c->d_loop, 0, sizeof(mbar::LoopState)));
-    CREATE_CUDA(cudaMemset(c->d_seq, 0, sizeof(unsigned long long)));
-    CREATE_CUDA(cudaMemcpy(c->d_active, c->active.data(), c->active.size() * sizeof(int), cudaMemcpyHostToDevice));
-    CREATE_CUDA(cudaEventCreate(&c->evH0));
-    CREATE_CUDA(cudaEventCreate(&c->evH1));
-    CREATE_CUDA(cudaEventCreate(&c->evH2));
+    MBAR_TRY(c->d_f.reserve((size_t)K, who));
+    MBAR_TRY(c->d_scratch.reserve(scratch_rendezvous(K) + 1024, who));
+    MBAR_TRY(c->d_loop.reserve(1, who));
+    MBAR_TRY(c->d_av.reserve(8 * (size_t)K, who));
+    MBAR_TRY(c->d_outM.reserve(2 * (size_t)lay.size(false), who));
+    MBAR_TRY(c->d_A.reserve((size_t)K * K, who));
+    MBAR_TRY(c->d_active.reserve((size_t)K, who));
+    MBAR_TRY(c->d_seq.reserve(1, who));
+    MBAR_TRY(c->h_loop.reserve(1, who));
+    MBAR_CUDA(cudaMemset(c->d_loop, 0, sizeof(mbar::LoopState)));
+    MBAR_CUDA(cudaMemset(c->d_seq, 0, sizeof(unsigned long long)));
+    MBAR_CUDA(cudaMemcpy(c->d_active, c->active.data(), c->active.size() * sizeof(int), cudaMemcpyHostToDevice));
+    MBAR_TRY(c->evH.create(3));
     // (holds one packed result with G, or the two candidate results of mbar_b200_pass_multi)
-    CREATE_CUDA(cudaHostAlloc((void**)&c->h_out,
-                              (size_t)std::max(lay.size(true), 2 * lay.size(false)) * sizeof(double),
-                              cudaHostAllocDefault));
-    CREATE_CUDA(cudaHostAlloc((void**)&c->h_f, HF_ROWS * (size_t)K * sizeof(double), cudaHostAllocDefault));
-    CREATE_CUDA(cudaStreamCreateWithFlags(&c->stream, cudaStreamNonBlocking));
-    CREATE_CUDA(cudaStreamCreateWithFlags(&c->copyStream, cudaStreamNonBlocking));
-    CREATE_CUDA(cudaEventCreate(&c->evA));
-    CREATE_CUDA(cudaEventCreate(&c->evB));
-    CREATE_CUDA(cudaEventCreateWithFlags(&c->evCopy[0], cudaEventDisableTiming));
-    CREATE_CUDA(cudaEventCreateWithFlags(&c->evCopy[1], cudaEventDisableTiming));
-    CREATE_CUDA(cudaMemcpy(c->d_Nk, N_k, (size_t)K * sizeof(double), cudaMemcpyHostToDevice));
+    MBAR_TRY(c->h_out.reserve((size_t)std::max(lay.size(true), 2 * lay.size(false)), who));
+    MBAR_TRY(c->h_f.reserve(HF_ROWS * (size_t)K, who));
+    MBAR_TRY(c->open(device, who));
+    MBAR_TRY(c->copyStream.create(who));
+    MBAR_TRY(c->evCopy.create(2, cudaEventDisableTiming));
+    MBAR_CUDA(cudaMemcpy(c->d_Nk, N_k, (size_t)K * sizeof(double), cudaMemcpyHostToDevice));
     {
         std::vector<double> eff(K);
         for (int k = 0; k < K; ++k) eff[k] = std::exp(c->h_logNkEff[k]);
-        CREATE_CUDA(cudaMemcpy(c->d_NkEff, eff.data(), (size_t)K * sizeof(double), cudaMemcpyHostToDevice));
+        MBAR_CUDA(cudaMemcpy(c->d_NkEff, eff.data(), (size_t)K * sizeof(double), cudaMemcpyHostToDevice));
     }
-    CREATE_CUDA(cudaMemcpy(c->d_rowmask, mask.data(), mask.size() * sizeof(unsigned long long),
-                         cudaMemcpyHostToDevice));
-    CREATE_CUDA(cudaMemset(c->d_zeromask, 0, mask.size() * sizeof(unsigned long long)));
-    CREATE_CUDA(cudaMemset(c->d_onesmask, 0xff, mask.size() * sizeof(unsigned long long)));
-    CREATE_CUDA(cudaMemset(c->d_ticket, 0, 4 * sizeof(unsigned int)));
-    CREATE_CUDA(cudaMemset(c->d_flag, 0, 4 * sizeof(int)));
-    CREATE_CUDA(cudaMemset(c->d_urowmin, 0, 2 * (size_t)K * sizeof(int)));
-    CREATE_CUDA(cudaMemset(c->d_urowfar, 0, (size_t)K * sizeof(unsigned long long)));
-#undef CREATE_CUDA
-    *out = c;
+    MBAR_CUDA(cudaMemcpy(c->d_rowmask, mask.data(), mask.size() * sizeof(unsigned long long), cudaMemcpyHostToDevice));
+    MBAR_CUDA(cudaMemset(c->d_zeromask, 0, mask.size() * sizeof(unsigned long long)));
+    MBAR_CUDA(cudaMemset(c->d_onesmask, 0xff, mask.size() * sizeof(unsigned long long)));
+    MBAR_CUDA(cudaMemset(c->d_ticket, 0, 4 * sizeof(unsigned int)));
+    MBAR_CUDA(cudaMemset(c->d_flag, 0, 4 * sizeof(int)));
+    MBAR_CUDA(cudaMemset(c->d_urowmin, 0, 2 * (size_t)K * sizeof(int)));
+    MBAR_CUDA(cudaMemset(c->d_urowfar, 0, (size_t)K * sizeof(unsigned long long)));
+    *out = c.release();
     return MBAR_B200_OK;
 }
 
+// Members free themselves (the pooled ones go back to the pool); what remains is what no member can own: the
+// communicator and the peers' mappings go first, and the stream drains before any buffer is released.
 int mbar_b200_destroy(mbar_b200_ctx* c) {
     if (!c) return MBAR_B200_OK;
     cudaSetDevice(c->device);
     if (c->comm) mbar_b200_comm_destroy(c);
     for (void* pm : c->peerMapped) cudaIpcCloseMemHandle(pm);
-    cudaFree(c->d_inbox);
-    if (c->stream) cudaStreamSynchronize(c->stream);
-    if (pool_enabled() && c->d_u) {
-        // (a buffer taken from the pool may be larger than this context needed: park it with the size
-        // it is known to cover at least)
-        const size_t need = (size_t)c->nTiles * c->K * TILE_N * sizeof(double);
-        cudaFree(pool_park(g_pool[c->device & 15].u, c->d_u, c->uBytes ? c->uBytes : need));
-        for (int i = 0; i < 2; ++i) {
-            const size_t sb = (size_t)c->stageCols * c->K * sizeof(double);
-            if (c->stage_dev[i]) cudaFree(pool_park(g_pool[c->device & 15].stageDev[i], c->stage_dev[i], sb));
-            if (c->stage_pinned[i]) {
-                void* old = pool_park(g_pool[c->device & 15].stagePin[i], c->stage_pinned[i], sb);
-                if (old) cudaFreeHost(old);
-            }
-            c->stage_dev[i] = nullptr;
-            c->stage_pinned[i] = nullptr;
-        }
-    } else {
-        cudaFree(c->d_u);
-    }
-    cudaFree(c->d_xshift); cudaFree(c->d_wgt); cudaFree(c->d_sqrtw); cudaFree(c->d_c); cudaFree(c->d_Nk); cudaFree(c->d_NkEff);
-    cudaFree(c->d_rowmask); cudaFree(c->d_zeromask); cudaFree(c->d_onesmask); cudaFree(c->d_partial); cudaFree(c->d_out); cudaFree(c->d_L);
-    cudaFree(c->d_W); cudaFree(c->d_ticket); cudaFree(c->d_flag); cudaFree(c->d_urowmin); cudaFree(c->d_urowfar); cudaFree(c->d_f);
-    cudaFree(c->d_scratch);
-    cudaFree(c->d_loop); cudaFree(c->d_av); cudaFree(c->d_outM); cudaFree(c->d_A); cudaFree(c->d_active);
-    cudaFree(c->d_seq); cudaFree(c->d_Wt);
     if (c->loopGraph) cudaGraphExecDestroy(c->loopGraph);
-    if (c->h_loop) cudaFreeHost(c->h_loop);
-    if (c->evH0) cudaEventDestroy(c->evH0);
-    if (c->evH1) cudaEventDestroy(c->evH1);
-    if (c->evH2) cudaEventDestroy(c->evH2);
-    for (int i = 0; i < 2; ++i) {
-        if (c->stage_pinned[i]) cudaFreeHost(c->stage_pinned[i]);
-        cudaFree(c->stage_dev[i]);
-        if (c->evCopy[i]) cudaEventDestroy(c->evCopy[i]);
-    }
-    if (c->h_out) cudaFreeHost(c->h_out);
-    if (c->h_f) cudaFreeHost(c->h_f);
-    if (c->evA) cudaEventDestroy(c->evA);
-    if (c->evB) cudaEventDestroy(c->evB);
-    if (c->stream) cudaStreamDestroy(c->stream);
-    if (c->copyStream) cudaStreamDestroy(c->copyStream);
+    destroy_resident(c);
     cudaGetLastError();
-    delete c;
     return MBAR_B200_OK;
 }
 
@@ -798,21 +725,19 @@ int mbar_b200_trim(void) {
     int cur = 0;
     cudaGetDevice(&cur);
     for (int d = 0; d < 16; ++d) {
-        DevicePool old;
+        Parked old[POOL_KINDS];
+        bool any = false;
         {
             std::lock_guard<std::mutex> g(g_poolMutex);
-            old = g_pool[d];
-            g_pool[d] = DevicePool{};
+            for (int k = 0; k < POOL_KINDS; ++k) {
+                old[k] = g_pool[d][k];
+                g_pool[d][k] = Parked{};
+                any |= old[k].ptr != nullptr;
+            }
         }
-        if (!old.u.ptr && !old.stageDev[0].ptr && !old.stageDev[1].ptr && !old.stagePin[0].ptr &&
-            !old.stagePin[1].ptr)
-            continue;
+        if (!any) continue;
         cudaSetDevice(d);
-        cudaFree(old.u.ptr);
-        for (int i = 0; i < 2; ++i) {
-            cudaFree(old.stageDev[i].ptr);
-            if (old.stagePin[i].ptr) cudaFreeHost(old.stagePin[i].ptr);
-        }
+        for (int k = 0; k < POOL_KINDS; ++k) mem_free(old[k].ptr, k >= POOL_STAGE_PIN);
     }
     cudaSetDevice(cur);
     cudaGetLastError();
@@ -849,7 +774,7 @@ int mbar_b200_last_pass_ms(mbar_b200_ctx* c, double* ms) {
     // launched it)
     cudaSetDevice(c->device);
     float t = 0.f;
-    if (c->stream && cudaStreamSynchronize(c->stream) == cudaSuccess && event_ms(c->evA, c->evB, &t))
+    if (c->stream && cudaStreamSynchronize(c->stream) == cudaSuccess && event_ms(c->ev0, c->ev1, &t))
         c->lastPassMs = t;
     else
         cudaGetLastError();
@@ -867,17 +792,10 @@ static int ensure_staging(mbar_b200_ctx* c, bool needPinned) {
         if (cols > padN) cols = padN;
         c->stageCols = cols;
     }
-    const size_t bytes = (size_t)c->stageCols * c->K * sizeof(double);
+    const size_t count = (size_t)c->stageCols * c->K;
     for (int i = 0; i < 2; ++i) {
-        if (!c->stage_dev[i] && pool_enabled())
-            c->stage_dev[i] = static_cast<double*>(pool_take(g_pool[c->device & 15].stageDev[i], bytes));
-        if (!c->stage_dev[i]) MBAR_CUDA(cudaMalloc((void**)&c->stage_dev[i], bytes));
-        if (needPinned && !c->stage_pinned[i] && pool_enabled())
-            c->stage_pinned[i] = static_cast<double*>(pool_take(g_pool[c->device & 15].stagePin[i], bytes));
-        if (needPinned && !c->stage_pinned[i]) {
-            NumaPrefer numa(c->device);
-            MBAR_CUDA(cudaHostAlloc((void**)&c->stage_pinned[i], bytes, cudaHostAllocDefault));
-        }
+        MBAR_TRY(c->stage_dev[i].acquire(c->device, POOL_STAGE_DEV + i, count, "upload_u_kn"));
+        if (needPinned) MBAR_TRY(c->stage_pinned[i].acquire(c->device, POOL_STAGE_PIN + i, count, "upload_u_kn"));
     }
     return MBAR_B200_OK;
 }
@@ -979,11 +897,10 @@ int mbar_b200_upload_u_kn(mbar_b200_ctx* c, const double* u_host, int64_t ld) {
                                     (size_t)srcLd * sizeof(double), (size_t)w * sizeof(double), K,
                                     cudaMemcpyHostToDevice, c->copyStream));
         c->h2dBytes += (int64_t)w * K * 8;
-        cudaEvent_t copied;
-        MBAR_CUDA(cudaEventCreateWithFlags(&copied, cudaEventDisableTiming));
-        MBAR_CUDA(cudaEventRecord(copied, c->copyStream));
-        MBAR_CUDA(cudaStreamWaitEvent(c->stream, copied, 0));
-        MBAR_CUDA(cudaEventDestroy(copied));
+        Events copied;
+        MBAR_TRY(copied.create(1, cudaEventDisableTiming));
+        MBAR_CUDA(cudaEventRecord(copied[0], c->copyStream));
+        MBAR_CUDA(cudaStreamWaitEvent(c->stream, copied[0], 0));
         const int64_t nT = (w + TILE_N - 1) / TILE_N;
         MBAR_TRY(retile_chunk(c, c->stage_dev[buf], cols, n0 / TILE_N, nT, w, c->stream));
         MBAR_CUDA(cudaEventRecord(c->evCopy[buf], c->stream));
@@ -1048,30 +965,19 @@ int mbar_b200_create_augmented(mbar_b200_ctx* base, int32_t n_extra, const doubl
     const int K = base->K, E = n_extra, Kn = K + E;
     std::vector<double> Nk(base->h_Nk);
     Nk.resize(Kn, 0.0);
-    mbar_b200_ctx* c = nullptr;
-    MBAR_TRY(mbar_b200_create(&c, base->device, Kn, base->N, Nk.data()));
-    auto fail = [&](int rc) {
-        mbar_b200_destroy(c);
-        return rc;
-    };
-#define AUG_CUDA(call)                                                                         \
-    do {                                                                                       \
-        cudaError_t e__ = (call);                                                              \
-        if (e__ != cudaSuccess) {                                                              \
-            set_error("%s failed at %s:%d: %s", #call, __FILE__, __LINE__, cudaGetErrorString(e__)); \
-            return fail(MBAR_B200_ERR_CUDA);                                                   \
-        }                                                                                      \
-    } while (0)
-    AUG_CUDA(cudaStreamSynchronize(base->stream));
+    mbar_b200_ctx* raw = nullptr;
+    MBAR_TRY(mbar_b200_create(&raw, base->device, Kn, base->N, Nk.data()));
+    std::unique_ptr<mbar_b200_ctx, int (*)(mbar_b200_ctx*)> c(raw, mbar_b200_destroy);
+    MBAR_CUDA(cudaStreamSynchronize(base->stream));
     const size_t nPad = (size_t)c->nTiles * TILE_N;
-    AUG_CUDA(cudaMemcpyAsync(c->d_xshift, base->d_xshift, nPad * sizeof(double), cudaMemcpyDeviceToDevice, c->stream));
+    MBAR_CUDA(cudaMemcpyAsync(c->d_xshift, base->d_xshift, nPad * sizeof(double), cudaMemcpyDeviceToDevice, c->stream));
     c->sumX = base->sumX;
     {
         int64_t grid = (int64_t)c->smCount * 8;
         if (grid > c->nTiles) grid = c->nTiles;
         widen_tiles_kernel<<<(unsigned)grid, 256, 0, c->stream>>>(base->d_u, K, Kn, c->nTiles, c->d_u);
         c->launches++;
-        AUG_CUDA(cudaGetLastError());
+        MBAR_CUDA(cudaGetLastError());
     }
     // the E new rows: column chunks through a pinned + a device staging block (pageable sources are packed by
     // the host first, exactly like mbar_b200_upload_u_kn)
@@ -1085,63 +991,48 @@ int mbar_b200_create_augmented(mbar_b200_ctx* base, int32_t n_extra, const doubl
         pinned = (attr.type == cudaMemoryTypeHost);
     else
         cudaGetLastError();
-    double* d_stage = nullptr;
-    double* h_stage = nullptr;
-    AUG_CUDA(cudaMalloc((void**)&d_stage, (size_t)cols * E * sizeof(double)));
-    if (!pinned) {
-        NumaPrefer numa(c->device);
-        cudaError_t e = cudaHostAlloc((void**)&h_stage, (size_t)cols * E * sizeof(double), cudaHostAllocDefault);
-        if (e != cudaSuccess) {
-            cudaFree(d_stage);
-            set_error("cudaHostAlloc failed: %s", cudaGetErrorString(e));
-            return fail(MBAR_B200_ERR_NOMEM);
+    {
+        CallBuffers buf("create_augmented");
+        double* d_stage = nullptr;
+        HostPinned<double> h_stage;
+        StreamDrain guard{c.get()};
+        MBAR_TRY(buf.alloc(&d_stage, (size_t)cols * E));
+        if (!pinned) MBAR_TRY(h_stage.reserve((size_t)cols * E, "create_augmented", c->device));
+        for (int64_t n0 = 0; n0 < c->N; n0 += cols) {
+            const int64_t w = (c->N - n0 < cols) ? (c->N - n0) : cols;
+            const double* src = u_extra_host + n0;
+            int64_t srcLd = ld;
+            if (!pinned) {
+                cudaStreamSynchronize(c->stream);        // the staging block of the previous chunk has been consumed
+                for (int r = 0; r < E; ++r)
+                    std::memcpy(h_stage + (size_t)r * w, u_extra_host + (size_t)r * ld + n0, (size_t)w * sizeof(double));
+                src = h_stage;
+                srcLd = w;
+            }
+            cudaError_t e = cudaMemcpy2DAsync(d_stage, (size_t)cols * sizeof(double), src, (size_t)srcLd * sizeof(double),
+                                              (size_t)w * sizeof(double), E, cudaMemcpyHostToDevice, c->stream);
+            MBAR_REQUIRE(e == cudaSuccess, MBAR_B200_ERR_CUDA, "append rows: H2D failed: %s", cudaGetErrorString(e));
+            c->h2dBytes += (int64_t)w * E * 8;
+            const int64_t nT = (w + TILE_N - 1) / TILE_N;
+            append_rows_kernel<<<(unsigned)nT, 256, 0, c->stream>>>(d_stage, cols, E, K, Kn, n0 / TILE_N, w,
+                                                                  c->d_xshift, c->d_u, c->d_flag, c->d_urowmin,
+                                                                  c->d_urowfar);
+            c->launches++;
+            if (pinned) cudaStreamSynchronize(c->stream);   // one device staging block: consume before refilling
         }
     }
-    int rc = MBAR_B200_OK;
-    for (int64_t n0 = 0; n0 < c->N && rc == MBAR_B200_OK; n0 += cols) {
-        const int64_t w = (c->N - n0 < cols) ? (c->N - n0) : cols;
-        const double* src = u_extra_host + n0;
-        int64_t srcLd = ld;
-        if (!pinned) {
-            cudaStreamSynchronize(c->stream);        // the staging block of the previous chunk has been consumed
-            for (int r = 0; r < E; ++r)
-                std::memcpy(h_stage + (size_t)r * w, u_extra_host + (size_t)r * ld + n0, (size_t)w * sizeof(double));
-            src = h_stage;
-            srcLd = w;
-        }
-        cudaError_t e = cudaMemcpy2DAsync(d_stage, (size_t)cols * sizeof(double), src, (size_t)srcLd * sizeof(double),
-                                          (size_t)w * sizeof(double), E, cudaMemcpyHostToDevice, c->stream);
-        if (e != cudaSuccess) {
-            set_error("append rows: H2D failed: %s", cudaGetErrorString(e));
-            rc = MBAR_B200_ERR_CUDA;
-            break;
-        }
-        c->h2dBytes += (int64_t)w * E * 8;
-        const int64_t nT = (w + TILE_N - 1) / TILE_N;
-        append_rows_kernel<<<(unsigned)nT, 256, 0, c->stream>>>(d_stage, cols, E, K, Kn, n0 / TILE_N, w,
-                                                              c->d_xshift, c->d_u, c->d_flag, c->d_urowmin,
-                                                              c->d_urowfar);
-        c->launches++;
-        if (pinned) cudaStreamSynchronize(c->stream);   // one device staging block: consume before refilling
-    }
-    cudaStreamSynchronize(c->stream);
-    cudaFree(d_stage);
-    if (h_stage) cudaFreeHost(h_stage);
-    if (rc != MBAR_B200_OK) return fail(rc);
-    int flags[4] = {0, 0, 0, 0};
-    AUG_CUDA(cudaMemcpy(flags, c->d_flag, sizeof(flags), cudaMemcpyDeviceToHost));
-    AUG_CUDA(cudaMemset(c->d_flag, 0, 4 * sizeof(int)));
-    if (flags[0]) {
-        set_error(flags[0] & BAD_NAN ? "appended energies contain NaN"
-                                     : "an appended state has an energy of -inf (its free energy would be -inf)");
-        return fail(MBAR_B200_ERR_NAN);
-    }
+    int flags[4] = {0, 0, 0, 0};   // (the appends have drained with the staging)
+    MBAR_CUDA(cudaMemcpy(flags, c->d_flag, sizeof(flags), cudaMemcpyDeviceToHost));
+    MBAR_CUDA(cudaMemset(c->d_flag, 0, 4 * sizeof(int)));
+    MBAR_REQUIRE(!flags[0], MBAR_B200_ERR_NAN, "%s",
+                 flags[0] & BAD_NAN ? "appended energies contain NaN"
+                                    : "an appended state has an energy of -inf (its free energy would be -inf)");
     {
         std::vector<int> m(2 * (size_t)Kn);
         std::vector<unsigned long long> far(Kn);
-        AUG_CUDA(cudaMemcpy(m.data(), c->d_urowmin, m.size() * sizeof(int), cudaMemcpyDeviceToHost));
-        AUG_CUDA(cudaMemcpy(far.data(), c->d_urowfar, far.size() * sizeof(unsigned long long), cudaMemcpyDeviceToHost));
-        if (reset_row_stats(c) != MBAR_B200_OK) return fail(MBAR_B200_ERR_CUDA);
+        MBAR_CUDA(cudaMemcpy(m.data(), c->d_urowmin, m.size() * sizeof(int), cudaMemcpyDeviceToHost));
+        MBAR_CUDA(cudaMemcpy(far.data(), c->d_urowfar, far.size() * sizeof(unsigned long long), cudaMemcpyDeviceToHost));
+        MBAR_TRY(reset_row_stats(c.get()));
         for (int k = 0; k < K; ++k) {
             c->h_urowmin[k] = base->h_urowmin[k];
             c->h_uclamp[k] = base->h_uclamp[k];
@@ -1155,16 +1046,14 @@ int mbar_b200_create_augmented(mbar_b200_ctx* base, int32_t n_extra, const doubl
     }
     if (base->d_wgt) {
         // bootstrap multiplicities travel with the samples
-        AUG_CUDA(cudaMalloc((void**)&c->d_wgt, nPad * sizeof(double)));
-        AUG_CUDA(cudaMalloc((void**)&c->d_sqrtw, nPad * sizeof(double)));
-        AUG_CUDA(cudaMemcpy(c->d_wgt, base->d_wgt, nPad * sizeof(double), cudaMemcpyDeviceToDevice));
-        AUG_CUDA(cudaMemcpy(c->d_sqrtw, base->d_sqrtw, nPad * sizeof(double), cudaMemcpyDeviceToDevice));
+        MBAR_TRY(reserve_weights(c.get()));
+        MBAR_CUDA(cudaMemcpy(c->d_wgt, base->d_wgt, nPad * sizeof(double), cudaMemcpyDeviceToDevice));
+        MBAR_CUDA(cudaMemcpy(c->d_sqrtw, base->d_sqrtw, nPad * sizeof(double), cudaMemcpyDeviceToDevice));
         c->sumW = base->sumW;
         c->sumXw = base->sumXw;
     }
-#undef AUG_CUDA
     c->ready = true;
-    *out = c;
+    *out = c.release();
     return MBAR_B200_OK;
 }
 
@@ -1207,7 +1096,8 @@ int mbar_b200_download_u_kn(mbar_b200_ctx* c, int64_t n0, int64_t n, double* u_h
     const int64_t maxCols = (32ll << 20) / (8ll * c->K) / TILE_N * TILE_N + TILE_N;
     double* d_tmp = nullptr;
     const int64_t cols = n < maxCols ? n : maxCols;
-    MBAR_CUDA(cudaMalloc((void**)&d_tmp, (size_t)cols * c->K * sizeof(double)));
+    CallBuffers buf("download_u_kn");
+    MBAR_TRY(buf.alloc(&d_tmp, (size_t)cols * c->K));
     int rc = MBAR_B200_OK;
     for (int64_t j = 0; j < n && rc == MBAR_B200_OK; j += cols) {
         const int64_t w = (n - j < cols) ? (n - j) : cols;
@@ -1223,7 +1113,6 @@ int mbar_b200_download_u_kn(mbar_b200_ctx* c, int64_t n0, int64_t n, double* u_h
         }
         c->d2hBytes += (int64_t)w * c->K * 8;
     }
-    cudaFree(d_tmp);
     return rc;
 }
 

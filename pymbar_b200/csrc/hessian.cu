@@ -582,26 +582,12 @@ hessian_small_reduce_kernel(const double* __restrict__ Gpart, int K, int KP, int
     }
 }
 
-static int ensure_gpart(mbar_b200_ctx* ctx, size_t bytes) {
-    // partial-block scratch of the Hessian kernels (kept across calls; grows on demand)
-    static_assert(sizeof(size_t) == 8, "64-bit build");
-    if (ctx->d_W && ctx->gpartBytes >= bytes) return MBAR_B200_OK;
-    if (ctx->d_W) cudaFree(ctx->d_W);
-    ctx->d_W = nullptr;
-    MBAR_CUDA(cudaMalloc((void**)&ctx->d_W, bytes));
-    ctx->gpartBytes = bytes;
-    return MBAR_B200_OK;
-}
-
 bool ensure_weight_buffer(mbar_b200_ctx* ctx) {
     static const bool forceOld = std::getenv("MBAR_B200_HESSIAN_INPLACE") != nullptr;
     if (forceOld) return false;
     if (ctx->d_Wt) return true;
     if (ctx->wtAllocFailed) return false;
-    const size_t bytes = (size_t)ctx->nTiles * ctx->K * TILE_N * sizeof(double);
-    if (cudaMalloc((void**)&ctx->d_Wt, bytes) != cudaSuccess) {
-        cudaGetLastError();
-        ctx->d_Wt = nullptr;
+    if (ctx->d_Wt.reserve((size_t)ctx->nTiles * ctx->K * TILE_N, "hessian") != MBAR_B200_OK) {
         ctx->wtAllocFailed = true;
         return false;
     }
@@ -616,7 +602,7 @@ int launch_hessian_dev(mbar_b200_ctx* ctx, const double* d_ch, bool allRows, Loo
     const PassLayout lay{K};
     const unsigned long long* mask = allRows ? ctx->d_onesmask : ctx->d_rowmask;
     static const bool forceOld = std::getenv("MBAR_B200_HESSIAN_INPLACE") != nullptr;
-    if (!ctx->capturing) MBAR_CUDA(cudaEventRecord(ctx->evH0, ctx->stream));
+    if (!ctx->capturing) MBAR_CUDA(cudaEventRecord(ctx->evH[0], ctx->stream));
     if (K <= 64 && !forceOld) {
         const int KT = K <= 16 ? 2 : K <= 32 ? 4 : 8;
         const int KP = KT * 8;
@@ -626,7 +612,7 @@ int launch_hessian_dev(mbar_b200_ctx* ctx, const double* d_ch, bool allRows, Loo
         int64_t grid = ctx->smCount;
         if (grid > (ctx->nTiles + 3) / 4) grid = (ctx->nTiles + 3) / 4;
         if (grid < 1) grid = 1;
-        MBAR_TRY(ensure_gpart(ctx, (size_t)grid * KP * KP * sizeof(double)));
+        MBAR_TRY(ctx->d_W.reserve((size_t)grid * KP * KP, "hessian"));
         const size_t smem = 1024 + (size_t)nslot * slotBytes;
         const bool win = weightsReady && !allRows && ctx->d_Wt;
         void (*kern)(const double*, const double*, const double*, const unsigned long long*, int, int64_t, int64_t,
@@ -641,14 +627,14 @@ int launch_hessian_dev(mbar_b200_ctx* ctx, const double* d_ch, bool allRows, Loo
             MBAR_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
             a = smem;
         }
-        if (!ctx->capturing) MBAR_CUDA(cudaEventRecord(ctx->evH1, ctx->stream));
+        if (!ctx->capturing) MBAR_CUDA(cudaEventRecord(ctx->evH[1], ctx->stream));
         kern<<<(unsigned)grid, 256, smem, ctx->stream>>>(win ? ctx->d_Wt : ctx->d_u, ctx->d_L, d_ch, mask, K, ctx->N,
                                                         ctx->nTiles, nslot, ctx->d_W, ctx->d_sqrtw, loop);
         MBAR_CUDA(cudaGetLastError());
         hessian_small_reduce_kernel<<<(KP * KP + 255) / 256, 256, 0, ctx->stream>>>(ctx->d_W, K, KP, (int)grid,
                                                                                     ctx->d_out + lay.G(), loop);
         MBAR_CUDA(cudaGetLastError());
-        if (!ctx->capturing) MBAR_CUDA(cudaEventRecord(ctx->evH2, ctx->stream));
+        if (!ctx->capturing) MBAR_CUDA(cudaEventRecord(ctx->evH[2], ctx->stream));
         snprintf(ctx->lastHessKernel, sizeof(ctx->lastHessKernel), "hessian_small_kernel<KT=%d, %s> grid=%lld NSLOT=%d",
                  KT, win ? "weights stored by the fused pass (WST)" : "in-register conversion", (long long)grid, nslot);
         ctx->launches += 2;
@@ -674,7 +660,7 @@ int launch_hessian_dev(mbar_b200_ctx* ctx, const double* d_ch, bool allRows, Loo
         MBAR_CUDA(cudaGetLastError());
         ctx->launches++;
     }
-    if (!ctx->capturing) MBAR_CUDA(cudaEventRecord(ctx->evH1, ctx->stream));
+    if (!ctx->capturing) MBAR_CUDA(cudaEventRecord(ctx->evH[1], ctx->stream));
     // pairs in launches of at most 128 (K <= 2048: one launch; the split table is a kernel parameter)
     int totalCtas = 0;
     for (int base = 0; base < nPairsAll; base += 128) {
@@ -723,7 +709,7 @@ int launch_hessian_dev(mbar_b200_ctx* ctx, const double* d_ch, bool allRows, Loo
         split.pairStart[nPairs] = used;
         const int nCtas = used;
         totalCtas += nCtas;
-        MBAR_TRY(ensure_gpart(ctx, (size_t)nCtas * HB * HB * sizeof(double)));
+        MBAR_TRY(ctx->d_W.reserve((size_t)nCtas * HB * HB, "hessian"));
         if (materialise) {
             if (!attr[ctx->device & 15][0]) {
                 MBAR_CUDA(cudaFuncSetAttribute(hessian_big_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
@@ -755,7 +741,7 @@ int launch_hessian_dev(mbar_b200_ctx* ctx, const double* d_ch, bool allRows, Loo
                  totalCtas);
     else
         snprintf(ctx->lastHessKernel, sizeof(ctx->lastHessKernel), "hessian_inplace_kernel (round 1), CTAs %d", totalCtas);
-    if (!ctx->capturing) MBAR_CUDA(cudaEventRecord(ctx->evH2, ctx->stream));
+    if (!ctx->capturing) MBAR_CUDA(cudaEventRecord(ctx->evH[2], ctx->stream));
     ctx->passes++;
     return MBAR_B200_OK;
 }

@@ -106,10 +106,273 @@ struct LoopState {
 // f of log W, c of a second candidate; pinned only: f to and from d_f, f of each LoopState poll.
 enum { ROW_C, ROW_GEN_F, ROW_HESS_C, ROW_LOGW_F, ROW_C2, DC_ROWS, ROW_F = DC_ROWS, ROW_POLL, HF_ROWS };
 
+// Elapsed ms between two events.  False when either was never recorded (e.g. no pass has run yet); the runtime's
+// error is then cleared, or the next MBAR_CUDA(cudaGetLastError()) of an unrelated call would report it.
+inline bool event_ms(cudaEvent_t a, cudaEvent_t b, float* ms) {
+    if (cudaEventElapsedTime(ms, a, b) == cudaSuccess) return true;
+    cudaGetLastError();
+    return false;
+}
+
+// ---- host scaffold of the device objects (mbar_b200_ctx, _batch, _kde, _bspline, _acf, _work) ----
+// Every device buffer, pinned buffer, event and stream of the library has an owner defined here; outside this file only
+// the buffer pool of ctx.cu calls the runtime's allocator.
+
+// Checks that `device` is visible and is an sm_90 part, makes it current and fills *prop unless it is NULL (ctx.cu).
+int open_device(int device, cudaDeviceProp* prop);
+
+// Prefer the GPU's NUMA node for host allocations made while this object lives (ctx.cu).
+int gpu_numa_node(int device);
+struct NumaPrefer {
+    bool active = false;
+    explicit NumaPrefer(int device);
+    ~NumaPrefer();
+};
+
+// cudaMalloc of max(count, 1) elements.  On failure *p is NULL, the runtime's error is cleared and the status is
+// ERR_NOMEM when the device is out of memory, ERR_CUDA otherwise.
+template <class T>
+int dev_alloc(T** p, size_t count, const char* who) {
+    const cudaError_t e = cudaMalloc((void**)p, (count > 0 ? count : 1) * sizeof(T));
+    if (e == cudaSuccess) return MBAR_B200_OK;
+    *p = nullptr;
+    cudaGetLastError();
+    set_error("%s: cannot allocate %zu bytes", who, count * sizeof(T));
+    return e == cudaErrorMemoryAllocation ? MBAR_B200_ERR_NOMEM : MBAR_B200_ERR_CUDA;
+}
+
+// The same for pinned host memory.  numaDevice >= 0: the pages come from that GPU's NUMA node (NumaPrefer), which
+// keeps the large staging buffers of uploads and downloads off the inter-socket link.
+template <class T>
+int host_alloc(T** p, size_t count, const char* who, int numaDevice = -1) {
+    const size_t bytes = (count > 0 ? count : 1) * sizeof(T);
+    cudaError_t e;
+    if (numaDevice >= 0) {
+        NumaPrefer numa(numaDevice);
+        e = cudaHostAlloc((void**)p, bytes, cudaHostAllocDefault);
+    } else {
+        e = cudaHostAlloc((void**)p, bytes, cudaHostAllocDefault);
+    }
+    if (e == cudaSuccess) return MBAR_B200_OK;
+    *p = nullptr;
+    cudaGetLastError();
+    set_error("%s: cannot allocate %zu bytes of pinned host memory", who, count * sizeof(T));
+    return e == cudaErrorMemoryAllocation ? MBAR_B200_ERR_NOMEM : MBAR_B200_ERR_CUDA;
+}
+
+// Releases what dev_alloc (pinned = false) or host_alloc (pinned = true) returned; NULL is a no-op.
+inline cudaError_t mem_free(void* p, bool pinned) {
+    if (!p) return cudaSuccess;
+    return pinned ? cudaFreeHost(p) : cudaFree(p);
+}
+
+// Device buffers of one call, freed on every return path.
+struct CallBuffers {
+    const char* who;
+    std::vector<void*> ptrs;
+    explicit CallBuffers(const char* who_) : who(who_) {}
+    CallBuffers(const CallBuffers&) = delete;
+    CallBuffers& operator=(const CallBuffers&) = delete;
+    ~CallBuffers() {
+        for (void* p : ptrs) mem_free(p, false);
+    }
+    template <class T>
+    int alloc(T** p, size_t count) {
+        MBAR_TRY(dev_alloc(p, count, who));
+        ptrs.push_back((void*)*p);
+        return MBAR_B200_OK;
+    }
+};
+
+// An array owned by an object or a call and freed with it: device memory (DevArray) or pinned host memory
+// (HostPinned).  reserve(n) keeps the buffer when it already holds n elements; otherwise it drops the contents and
+// allocates n, and a failure leaves the array empty with capacity 0.  grow(n) reserves with room to spare
+// (n + n/2 + 64) for per-call buffers whose next call may be somewhat larger.  numaDevice: see host_alloc.
+template <class T, bool Pinned>
+struct OwnedArray {
+    T* ptr = nullptr;
+    size_t cap = 0;
+    OwnedArray() = default;
+    OwnedArray(OwnedArray&& o) noexcept : ptr(o.ptr), cap(o.cap) {
+        o.ptr = nullptr;
+        o.cap = 0;
+    }
+    OwnedArray& operator=(OwnedArray&& o) noexcept {
+        std::swap(ptr, o.ptr);
+        std::swap(cap, o.cap);
+        return *this;
+    }
+    ~OwnedArray() { reset(); }
+    void reset() {
+        mem_free(ptr, Pinned);
+        ptr = nullptr;
+        cap = 0;
+    }
+    int reserve(size_t n, const char* who, int numaDevice = -1) {
+        if (ptr && n <= cap) return MBAR_B200_OK;
+        reset();
+        MBAR_TRY(Pinned ? host_alloc(&ptr, n, who, numaDevice) : dev_alloc(&ptr, n, who));
+        cap = n;
+        return MBAR_B200_OK;
+    }
+    int grow(size_t n, const char* who) { return n <= cap ? MBAR_B200_OK : reserve(n + n / 2 + 64, who); }
+    operator T*() const { return ptr; }
+};
+template <class T>
+using DevArray = OwnedArray<T, false>;
+template <class T>
+using HostPinned = OwnedArray<T, true>;
+
+// The per-device pool of the context's largest buffers (ctx.cu), one slot per kind and device.  pool_take hands out
+// the parked buffer when it holds [bytes, 2 bytes + 1 MiB] (a small problem never pins a huge buffer) and sets *got to
+// its size, else NULL; pool_park parks a buffer and returns the one parked there before, for the caller to release.
+enum { POOL_U, POOL_STAGE_DEV, POOL_STAGE_PIN = POOL_STAGE_DEV + 2, POOL_KINDS = POOL_STAGE_PIN + 2 };
+bool pool_enabled();   // false under MBAR_B200_NO_POOL
+void* pool_take(int device, int kind, size_t bytes, size_t* got);
+void* pool_park(int device, int kind, void* ptr, size_t bytes);
+
+// An array of a context that comes from the pool when a parked buffer fits, and goes back to it at the size it really
+// has when the context is destroyed (released instead when the pool is off).
+template <class T, bool Pinned>
+struct PooledArray {
+    OwnedArray<T, Pinned> a;
+    int device = 0, kind = 0;
+    PooledArray() = default;
+    PooledArray(const PooledArray&) = delete;
+    PooledArray& operator=(const PooledArray&) = delete;
+    ~PooledArray() {
+        if (a.ptr && pool_enabled()) {
+            mem_free(pool_park(device, kind, a.ptr, a.cap * sizeof(T)), Pinned);
+            a.ptr = nullptr;
+        }
+    }
+    // at least n elements, allocated once (pinned: on the GPU's NUMA node)
+    int acquire(int dev, int k, size_t n, const char* who) {
+        if (a.ptr) return MBAR_B200_OK;
+        device = dev;
+        kind = k;
+        size_t got = 0;
+        if (pool_enabled() && (a.ptr = static_cast<T*>(pool_take(dev, k, n * sizeof(T), &got)))) {
+            a.cap = got / sizeof(T);
+            return MBAR_B200_OK;
+        }
+        return a.reserve(n, who, Pinned ? dev : -1);
+    }
+    operator T*() const { return a.ptr; }
+};
+
+// CUDA events, destroyed with the object on every return path.  As the timer of a solve: start() creates two and
+// records the first on the stream, stop() records the second, waits for it and returns the elapsed ms.
+struct Events {
+    std::vector<cudaEvent_t> ev;
+    cudaStream_t s = nullptr;
+    Events() = default;
+    Events(const Events&) = delete;
+    Events& operator=(const Events&) = delete;
+    ~Events() {
+        for (cudaEvent_t e : ev) cudaEventDestroy(e);
+    }
+    // flags: cudaEventDisableTiming for events that only order work
+    int create(size_t n, unsigned flags = cudaEventDefault) {
+        for (size_t i = 0; i < n; ++i) {
+            cudaEvent_t e;
+            MBAR_CUDA(cudaEventCreateWithFlags(&e, flags));
+            ev.push_back(e);
+        }
+        return MBAR_B200_OK;
+    }
+    cudaEvent_t operator[](size_t i) const { return ev[i]; }
+    float ms(size_t a, size_t b) const {
+        float m = 0.f;
+        event_ms(ev[a], ev[b], &m);
+        return m;
+    }
+    int start(cudaStream_t stream) {
+        s = stream;
+        MBAR_TRY(create(2));
+        MBAR_CUDA(cudaEventRecord(ev[0], s));
+        return MBAR_B200_OK;
+    }
+    float stop() {
+        cudaEventRecord(ev[1], s);
+        cudaEventSynchronize(ev[1]);
+        return ms(0, 1);
+    }
+};
+
+// A non-blocking stream (work on the legacy stream does not serialise with it), destroyed with its owner.
+struct Stream {
+    cudaStream_t s = nullptr;
+    Stream() = default;
+    Stream(const Stream&) = delete;
+    Stream& operator=(const Stream&) = delete;
+    ~Stream() {
+        if (s) cudaStreamDestroy(s);
+    }
+    int create(const char* who) {
+        if (cudaStreamCreateWithFlags(&s, cudaStreamNonBlocking) == cudaSuccess) return MBAR_B200_OK;
+        s = nullptr;
+        set_error("%s: %s", who, cudaGetErrorString(cudaGetLastError()));
+        return MBAR_B200_ERR_CUDA;
+    }
+    operator cudaStream_t() const { return s; }
+};
+
+// Device, stream and timing events of a resident device object.  The u_kn context and mbar_b200_batch, _kde,
+// _bspline, _acf and _work derive from it and hold their memory in the owners above; each create holds its object in a
+// std::unique_ptr until it succeeds, and each destroy waits for the stream before the delete (destroy_resident).
+struct Resident {
+    int device = 0;
+    Stream stream;
+    cudaEvent_t ev0 = nullptr, ev1 = nullptr; // the timed window of the last call
+    double lastMs = 0.0;
+
+    Resident() = default;
+    Resident(const Resident&) = delete;
+    Resident& operator=(const Resident&) = delete;
+    ~Resident() {
+        if (ev0) cudaEventDestroy(ev0);
+        if (ev1) cudaEventDestroy(ev1);
+    }
+    // the stream and the events, on `dev` (made current by open_device)
+    int open(int dev, const char* who) {
+        device = dev;
+        MBAR_TRY(stream.create(who));
+        if (cudaEventCreate(&ev0) != cudaSuccess || cudaEventCreate(&ev1) != cudaSuccess) {
+            set_error("%s: %s", who, cudaGetErrorString(cudaGetLastError()));
+            return MBAR_B200_ERR_CUDA;
+        }
+        return MBAR_B200_OK;
+    }
+    // count elements of src into dst (allocated to fit).  The copy goes on the object's own stream and is waited for:
+    // a pageable cudaMemcpy on the legacy stream may return before its DMA lands, and the kernels' stream would not
+    // wait for it.
+    template <class T>
+    int upload(DevArray<T>& dst, const T* src, size_t count, const char* who) {
+        MBAR_TRY(dst.reserve(count, who));
+        if (cudaMemcpyAsync(dst, src, count * sizeof(T), cudaMemcpyHostToDevice, stream) != cudaSuccess ||
+            cudaStreamSynchronize(stream) != cudaSuccess) {
+            set_error("%s: %s", who, cudaGetErrorString(cudaGetLastError()));
+            return MBAR_B200_ERR_CUDA;
+        }
+        return MBAR_B200_OK;
+    }
+};
+
+// Deletes a resident object once its stream has drained.  C++ destroys the derived object's arrays before ~Resident
+// runs, so the wait has to come before the delete.
+template <class T>
+int destroy_resident(T* o) {
+    if (!o) return MBAR_B200_OK;
+    cudaSetDevice(o->device);
+    if (o->stream) cudaStreamSynchronize(o->stream);
+    delete o;
+    return MBAR_B200_OK;
+}
+
 }  // namespace mbar
 
-struct mbar_b200_ctx {
-    int device = 0;
+struct mbar_b200_ctx : mbar::Resident {
     int K = 0;
     int64_t N = 0;        // local samples
     int64_t nTiles = 0;   // ceil(N / 32)
@@ -120,7 +383,7 @@ struct mbar_b200_ctx {
     std::vector<double> h_Nk;       // [K]
     std::vector<double> h_logNk;    // [K], -inf for unsampled
     std::vector<double> h_logNkEff; // [K], LOG_EPS_UNSAMPLED for unsampled
-    double* d_NkEff = nullptr;      // [K], exp(LOG_EPS_UNSAMPLED) for unsampled
+    mbar::DevArray<double> d_NkEff; // [K], exp(LOG_EPS_UNSAMPLED) for unsampled
     // [K] min over samples of each row's shifted energy u'_kn, rounded down, 0 when none is negative (only
     // unsampled rows can be): bounds the exp argument an unsampled row presents to the fused pass
     std::vector<double> h_urowmin;
@@ -130,45 +393,43 @@ struct mbar_b200_ctx {
     // unsampled row with both flags cannot be answered (ERR_RANGE, check_unsampled_clamp); with this one alone it is
     // all +inf: S = 0, f = +inf
     std::vector<double> h_ufar;
-    int* d_urowmin = nullptr;       // [2K] the row minima, then the clamp flags, accumulated during upload / append
-    unsigned long long* d_urowfar = nullptr;  // [K] entries per row at or above U_NEAR_CLAMP (+inf included)
+    mbar::DevArray<int> d_urowmin;  // [2K] the row minima, then the clamp flags, accumulated during upload / append
+    mbar::DevArray<unsigned long long> d_urowfar;  // [K] entries per row at or above U_NEAR_CLAMP (+inf included)
     std::vector<int> active;        // indices of sampled states
     int firstActive = 0;
     double N_total_states = 0;      // sum_k N_k (global N)
 
-    double* d_u = nullptr;          // [nTiles][K][32] shifted, clamped
-    size_t uBytes = 0;              // bytes this context allocated for d_u (0: came from the pool)
-    double* d_xshift = nullptr;     // [nTiles*32] per-sample shift x_n = min over sampled k of u_kn
-    double* d_wgt = nullptr;        // [nTiles*32] per-sample multiplicities w_n (bootstrap), or NULL = all 1
-    double* d_sqrtw = nullptr;      // [nTiles*32] sqrt(w_n) for the second-moment kernel
+    mbar::PooledArray<double, false> d_u;  // [nTiles][K][32] shifted, clamped
+    mbar::DevArray<double> d_xshift;  // [nTiles*32] per-sample shift x_n = min over sampled k of u_kn
+    mbar::DevArray<double> d_wgt;     // [nTiles*32] per-sample multiplicities w_n (bootstrap), or NULL = all 1
+    mbar::DevArray<double> d_sqrtw;   // [nTiles*32] sqrt(w_n) for the second-moment kernel (with d_wgt or neither)
     double sumW = 0.0;              // sum_n w_n over valid local samples (= N when unweighted)
     double sumXw = 0.0;             // sum_n w_n x_n
     double sumX = 0.0;              // sum_n x_n over valid local samples
-    double* d_c = nullptr;          // [DC_ROWS][K] pass constants, rows ROW_*
-    double* d_Nk = nullptr;         // [K]
-    unsigned long long* d_rowmask = nullptr;  // [ceil(K/64)] bit per sampled state
-    unsigned long long* d_zeromask = nullptr; // same size, all zero (log-domain for every row)
-    unsigned long long* d_onesmask = nullptr; // same size, all one (second moments of every state)
-    double* d_partial = nullptr;    // [MAX_GRID][K+2] per-CTA partials
-    double* d_out = nullptr;        // PassLayout packed result (with G)
-    double* h_out = nullptr;        // pinned mirror of d_out
-    double* d_L = nullptr;          // [nTiles*32] per-sample L_n (lazy)
-    double* d_W = nullptr;          // per-CTA partial blocks of the Hessian kernels (gpartBytes)
-    unsigned int* d_ticket = nullptr;
-    int* d_flag = nullptr;          // [4] error/diagnostic flags
-    double* d_f = nullptr;          // [K] device-resident f of the native loops
-    double* h_f = nullptr;          // pinned [HF_ROWS][K] staging, rows ROW_*
-    double* d_scratch = nullptr;    // misc scratch (see scratch_rendezvous)
-    cudaStream_t stream = nullptr;
-    cudaStream_t copyStream = nullptr;
-    cudaEvent_t evA = nullptr, evB = nullptr;
-    cudaEvent_t evCopy[2] = {nullptr, nullptr};
-    double* stage_pinned[2] = {nullptr, nullptr};
-    double* stage_dev[2] = {nullptr, nullptr};
+    mbar::DevArray<double> d_c;     // [DC_ROWS][K] pass constants, rows ROW_*
+    mbar::DevArray<double> d_Nk;    // [K]
+    mbar::DevArray<unsigned long long> d_rowmask;   // [ceil(K/64)] bit per sampled state
+    mbar::DevArray<unsigned long long> d_zeromask;  // same size, all zero (log-domain for every row)
+    mbar::DevArray<unsigned long long> d_onesmask;  // same size, all one (second moments of every state)
+    mbar::DevArray<double> d_partial;  // [MAX_GRID][K+2] per-CTA partials
+    mbar::DevArray<double> d_out;   // PassLayout packed result (with G)
+    mbar::HostPinned<double> h_out; // pinned mirror of d_out
+    mbar::DevArray<double> d_L;     // [nTiles*32] per-sample L_n (lazy, ensure_L)
+    mbar::DevArray<double> d_W;     // per-CTA partial blocks of the Hessian kernels (grown on demand)
+    mbar::DevArray<unsigned int> d_ticket;
+    mbar::DevArray<int> d_flag;     // [4] error/diagnostic flags
+    mbar::DevArray<double> d_f;     // [K] device-resident f of the native loops
+    mbar::HostPinned<double> h_f;   // pinned [HF_ROWS][K] staging, rows ROW_*
+    mbar::DevArray<double> d_scratch;  // misc scratch (see scratch_rendezvous)
+    // upload staging: copies on copyStream, evCopy[buf] marks the re-tile that last read stage_dev[buf]
+    mbar::Stream copyStream;
+    mbar::Events evCopy;
+    mbar::PooledArray<double, true> stage_pinned[2];
+    mbar::PooledArray<double, false> stage_dev[2];
     int64_t stageCols = 0;
 
     // peer-memory exchange (cudaIpc): this rank's inbox + flags and the peers' mappings
-    double* d_inbox = nullptr;
+    mbar::DevArray<double> d_inbox;
     mbar::PeerCfg peer;
     bool peerReady = false;
     std::vector<void*> peerMapped;
@@ -178,13 +439,13 @@ struct mbar_b200_ctx {
     int nranks = 1, rank = 0;
 
     // device-resident solver loops
-    mbar::LoopState* d_loop = nullptr;   // device
-    mbar::LoopState* h_loop = nullptr;   // pinned mirror
-    double* d_av = nullptr;              // [8][K] adaptive work vectors, rows AV_* (loops.cu)
-    double* d_outM = nullptr;            // [2][2K+2] pass outputs of the two candidates
-    double* d_A = nullptr;               // [K*K] Newton matrix / Cholesky factor
-    int* d_active = nullptr;             // [K] indices of the sampled states
-    unsigned long long* d_seq = nullptr; // peer-exchange sequence number (device-side, see PeerCfg::seq)
+    mbar::DevArray<mbar::LoopState> d_loop;    // device
+    mbar::HostPinned<mbar::LoopState> h_loop;  // pinned mirror
+    mbar::DevArray<double> d_av;         // [8][K] adaptive work vectors, rows AV_* (loops.cu)
+    mbar::DevArray<double> d_outM;       // [2][2K+2] pass outputs of the two candidates
+    mbar::DevArray<double> d_A;          // [K*K] Newton matrix / Cholesky factor
+    mbar::DevArray<int> d_active;        // [K] indices of the sampled states
+    mbar::DevArray<unsigned long long> d_seq;  // peer-exchange sequence number (device-side, see PeerCfg::seq)
     int loopMode = 0;                    // 0 device-resident, 1 host-stepped (round-1 behaviour)
     int loopBatch = 4;                   // iterations enqueued between two polls of LoopState
     int64_t loopPolls = 0;               // host synchronisations spent polling LoopState
@@ -195,9 +456,8 @@ struct mbar_b200_ctx {
     cudaGraphExec_t loopGraph = nullptr;
     std::vector<uint64_t> loopGraphKey;
     int64_t graphLaunches = 0, graphCaptures = 0;
-    double* d_Wt = nullptr;              // [nTiles][K][32] materialised N_k W_nk (swizzled) for the Hessian
+    mbar::DevArray<double> d_Wt;         // [nTiles][K][32] materialised N_k W_nk (swizzled) for the Hessian
     bool wtAllocFailed = false;
-    size_t gpartBytes = 0;               // size of d_W (per-CTA partial blocks of the Hessian kernels)
     char lastKernel[200] = "";           // description of the pass-kernel variant launched last
     char lastHessKernel[200] = "";       // ... and of the Hessian kernel path
     double lastHessMs = 0.0, lastWeightsMs = 0.0;
@@ -206,7 +466,7 @@ struct mbar_b200_ctx {
     double lastRepMs = 0.0;              // mbar_b200_replicate_unsampled: its kernels (CUDA events),
     int lastRepBatches = 0;              // ... its replicate batches
     int64_t lastRepExps = 0;             // ... and the exps it evaluated
-    cudaEvent_t evH0 = nullptr, evH1 = nullptr, evH2 = nullptr;
+    mbar::Events evH;                    // [3] bounds of the Hessian's weights and kernel windows
 
     // counters
     int64_t launches = 0, passes = 0, h2dBytes = 0, d2hBytes = 0;
@@ -218,6 +478,24 @@ struct mbar_b200_ctx {
     double* dc(int row) const { return d_c + (size_t)row * K; }
     double* hf(int row) const { return h_f + (size_t)row * K; }
 };
+
+namespace mbar {
+
+// Waits for the context's streams when it goes out of scope.  Declared after the call-scoped staging (buffers, events)
+// it protects, it runs before their destructors on every return path: staging is never freed under an in-flight copy.
+struct StreamDrain {
+    const mbar_b200_ctx* c;
+    ~StreamDrain() {
+        cudaStreamSynchronize(c->copyStream);
+        cudaStreamSynchronize(c->stream);
+    }
+};
+
+// The per-sample L'_n of the passes, allocated by the first pass that keeps it (never under stream capture: the
+// uncaptured warm-up iteration comes first)
+inline int ensure_L(mbar_b200_ctx* c) { return c->d_L.reserve((size_t)c->nTiles * TILE_N, "pass"); }
+
+}  // namespace mbar
 
 namespace mbar {
 
@@ -270,14 +548,6 @@ struct NvtxRange {
 // fn(0..n-1) on the pool plus the calling thread and returns when all are done.
 void host_parallel(int nTasks, const std::function<void(int)>& fn);
 int host_parallel_width();
-
-// Prefer the GPU's NUMA node for host allocations made while this object lives (ctx.cu).
-int gpu_numa_node(int device);
-struct NumaPrefer {
-    bool active = false;
-    explicit NumaPrefer(int device);
-    ~NumaPrefer();
-};
 
 // ---- host-side helpers implemented across the .cu files ----
 int check_range(mbar_b200_ctx* c, const double* f);
@@ -449,137 +719,9 @@ __host__ __device__ __forceinline__ double rel_change(double a, double b, double
     return fabs(a - b) / div;
 }
 
-// Elapsed ms between two events.  False when either was never recorded (e.g. no pass has run yet); the runtime's
-// error is then cleared, or the next MBAR_CUDA(cudaGetLastError()) of an unrelated call would report it.
-inline bool event_ms(cudaEvent_t a, cudaEvent_t b, float* ms) {
-    if (cudaEventElapsedTime(ms, a, b) == cudaSuccess) return true;
-    cudaGetLastError();
-    return false;
-}
-
 // d_scratch holds K*K + 4K + 1024 doubles of call-local scratch; the rendezvous all-reduce of the device-resident
 // loops owns the word at this offset
 inline size_t scratch_rendezvous(int K) { return (size_t)K * K + 4 * (size_t)K; }
-
-// ---- host scaffold of the resident device objects (mbar_b200_kde, _bspline, _acf, _work) ----
-
-// Checks that `device` is visible and is an sm_90 part, makes it current and fills *prop unless it is NULL (ctx.cu).
-int open_device(int device, cudaDeviceProp* prop);
-
-// cudaMalloc of max(count, 1) elements.  On failure *p is NULL, the runtime's error is cleared and the status is
-// ERR_NOMEM when the device is out of memory, ERR_CUDA otherwise.
-template <class T>
-int dev_alloc(T** p, size_t count, const char* who) {
-    const cudaError_t e = cudaMalloc((void**)p, (count > 0 ? count : 1) * sizeof(T));
-    if (e == cudaSuccess) return MBAR_B200_OK;
-    *p = nullptr;
-    cudaGetLastError();
-    set_error("%s: cannot allocate %zu bytes", who, count * sizeof(T));
-    return e == cudaErrorMemoryAllocation ? MBAR_B200_ERR_NOMEM : MBAR_B200_ERR_CUDA;
-}
-
-// Device buffers of one call, freed on every return path.
-struct CallBuffers {
-    const char* who;
-    std::vector<void*> ptrs;
-    explicit CallBuffers(const char* who_) : who(who_) {}
-    CallBuffers(const CallBuffers&) = delete;
-    CallBuffers& operator=(const CallBuffers&) = delete;
-    ~CallBuffers() {
-        for (void* p : ptrs) cudaFree(p);
-    }
-    template <class T>
-    int alloc(T** p, size_t count) {
-        MBAR_TRY(dev_alloc(p, count, who));
-        ptrs.push_back((void*)*p);
-        return MBAR_B200_OK;
-    }
-};
-
-// A device array owned by a resident object and freed with it.  reserve(n) keeps the buffer when it already holds n
-// elements; otherwise it drops the contents and allocates n, and a failure leaves the array empty with capacity 0.
-template <class T>
-struct DevArray {
-    T* ptr = nullptr;
-    size_t cap = 0;
-    DevArray() = default;
-    DevArray(DevArray&& o) noexcept : ptr(o.ptr), cap(o.cap) {
-        o.ptr = nullptr;
-        o.cap = 0;
-    }
-    DevArray& operator=(DevArray&& o) noexcept {
-        std::swap(ptr, o.ptr);
-        std::swap(cap, o.cap);
-        return *this;
-    }
-    ~DevArray() { reset(); }
-    void reset() {
-        if (ptr) cudaFree(ptr);
-        ptr = nullptr;
-        cap = 0;
-    }
-    int reserve(size_t n, const char* who) {
-        if (ptr && n <= cap) return MBAR_B200_OK;
-        reset();
-        MBAR_TRY(dev_alloc(&ptr, n, who));
-        cap = n;
-        return MBAR_B200_OK;
-    }
-    operator T*() const { return ptr; }
-};
-
-// Device, stream and timing events of a resident device object.  mbar_b200_kde, _bspline, _acf and _work derive from
-// it and hold their device memory in DevArray members; each create holds its object in a std::unique_ptr until it
-// succeeds, and each destroy goes through destroy_resident.
-struct Resident {
-    int device = 0;
-    cudaStream_t stream = nullptr;            // non-blocking: work on the legacy stream does not serialise with it
-    cudaEvent_t ev0 = nullptr, ev1 = nullptr; // the timed window of the last call
-    double lastMs = 0.0;
-
-    Resident() = default;
-    Resident(const Resident&) = delete;
-    Resident& operator=(const Resident&) = delete;
-    ~Resident() {
-        if (ev0) cudaEventDestroy(ev0);
-        if (ev1) cudaEventDestroy(ev1);
-        if (stream) cudaStreamDestroy(stream);
-    }
-    // the stream and the events, on `dev` (made current by open_device)
-    int open(int dev, const char* who) {
-        device = dev;
-        if (cudaStreamCreateWithFlags(&stream, cudaStreamNonBlocking) != cudaSuccess ||
-            cudaEventCreate(&ev0) != cudaSuccess || cudaEventCreate(&ev1) != cudaSuccess) {
-            set_error("%s: %s", who, cudaGetErrorString(cudaGetLastError()));
-            return MBAR_B200_ERR_CUDA;
-        }
-        return MBAR_B200_OK;
-    }
-    // count elements of src into dst (allocated to fit).  The copy goes on the object's own stream and is waited for:
-    // a pageable cudaMemcpy on the legacy stream may return before its DMA lands, and the kernels' stream would not
-    // wait for it.
-    template <class T>
-    int upload(DevArray<T>& dst, const T* src, size_t count, const char* who) {
-        MBAR_TRY(dst.reserve(count, who));
-        if (cudaMemcpyAsync(dst, src, count * sizeof(T), cudaMemcpyHostToDevice, stream) != cudaSuccess ||
-            cudaStreamSynchronize(stream) != cudaSuccess) {
-            set_error("%s: %s", who, cudaGetErrorString(cudaGetLastError()));
-            return MBAR_B200_ERR_CUDA;
-        }
-        return MBAR_B200_OK;
-    }
-};
-
-// Deletes a resident object once its stream has drained.  C++ destroys the derived object's DevArrays before ~Resident
-// runs, so the wait has to come before the delete.
-template <class T>
-int destroy_resident(T* o) {
-    if (!o) return MBAR_B200_OK;
-    cudaSetDevice(o->device);
-    if (o->stream) cudaStreamSynchronize(o->stream);
-    delete o;
-    return MBAR_B200_OK;
-}
 
 // The replicate weights V [B, N] of mbar_b200_kde_set_replicates and mbar_b200_bspline_set_replicates: B >= 1 and
 // every V_bn finite and >= 0.

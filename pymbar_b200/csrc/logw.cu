@@ -76,19 +76,17 @@ int launch_logw(mbar_b200_ctx* ctx, const double* h_f, double* logW_host, int64_
     int64_t tilesPerChunk = (64ll << 20) / ((int64_t)K * TILE_N * 8);
     if (tilesPerChunk < 1) tilesPerChunk = 1;
     if (tilesPerChunk > tilesTotal) tilesPerChunk = tilesTotal;
-    double* d_out[2] = {nullptr, nullptr};
-    double* h_stage[2] = {nullptr, nullptr};
-    const size_t chunkBytes = (size_t)tilesPerChunk * TILE_N * K * sizeof(double);
+    const size_t chunkElems = (size_t)tilesPerChunk * TILE_N * K;
+    DevArray<double> d_out[2];
+    HostPinned<double> h_stage[2];
     for (int i = 0; i < 2; ++i) {
-        MBAR_CUDA(cudaMalloc((void**)&d_out[i], chunkBytes));
-        if (!pinnedDst) {
-            NumaPrefer numa(ctx->device);
-            MBAR_CUDA(cudaHostAlloc((void**)&h_stage[i], chunkBytes, cudaHostAllocDefault));
-        }
+        MBAR_TRY(d_out[i].reserve(chunkElems, "log_W"));
+        if (!pinnedDst) MBAR_TRY(h_stage[i].reserve(chunkElems, "log_W", ctx->device));
     }
+    Events done;
+    MBAR_TRY(done.create(2, cudaEventDisableTiming));
+    StreamDrain guard{ctx};
     int rc = MBAR_B200_OK;
-    cudaEvent_t done[2];
-    for (int i = 0; i < 2; ++i) cudaEventCreateWithFlags(&done[i], cudaEventDisableTiming);
     struct Pending { int64_t row0 = 0, rows = 0; bool live = false; } pend[2];
     // drain staging buffer `b` into the caller's (pageable) array with several threads
     auto drain = [&](int b) {
@@ -120,11 +118,10 @@ int launch_logw(mbar_b200_ctx* ctx, const double* h_f, double* logW_host, int64_
         logw_kernel<<<(unsigned)nt, 128, 0, ctx->stream>>>(ctx->d_u, ctx->d_L, ctx->dc(ROW_LOGW_F), K, ctx->N,
                                                           tileFirst + t0, d_out[buf], expo);
         ctx->launches++;
-        cudaEvent_t ready;
-        cudaEventCreateWithFlags(&ready, cudaEventDisableTiming);
-        cudaEventRecord(ready, ctx->stream);
-        cudaStreamWaitEvent(ctx->copyStream, ready, 0);
-        cudaEventDestroy(ready);
+        Events ready;
+        MBAR_TRY(ready.create(1, cudaEventDisableTiming));
+        cudaEventRecord(ready[0], ctx->stream);
+        cudaStreamWaitEvent(ctx->copyStream, ready[0], 0);
         cudaError_t e;
         if (pinnedDst) {
             e = cudaMemcpy2DAsync(logW_host + (row0 - n0) * ld, (size_t)ld * sizeof(double), d_out[buf],
@@ -155,11 +152,6 @@ int launch_logw(mbar_b200_ctx* ctx, const double* h_f, double* logW_host, int64_
     if (!pinnedDst && rc == MBAR_B200_OK) {
         drain(0);
         drain(1);
-    }
-    for (int i = 0; i < 2; ++i) {
-        cudaEventDestroy(done[i]);
-        cudaFree(d_out[i]);
-        if (h_stage[i]) cudaFreeHost(h_stage[i]);
     }
     return rc;
 }

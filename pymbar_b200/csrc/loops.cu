@@ -382,43 +382,6 @@ adapt_post_kernel(const double* __restrict__ outS, const double* __restrict__ ou
 // ------------------------------------------------------------------------------------------------
 // host side
 // ------------------------------------------------------------------------------------------------
-// CUDA events, destroyed with the object on every return path.  As the timer of a solve: start() creates two and
-// records the first on the stream, stop() records the second, waits for it and returns the elapsed ms.
-struct Events {
-    std::vector<cudaEvent_t> ev;
-    cudaStream_t s = nullptr;
-    Events() = default;
-    Events(const Events&) = delete;
-    Events& operator=(const Events&) = delete;
-    ~Events() {
-        for (cudaEvent_t e : ev) cudaEventDestroy(e);
-    }
-    int create(size_t n) {
-        for (size_t i = 0; i < n; ++i) {
-            cudaEvent_t e;
-            MBAR_CUDA(cudaEventCreate(&e));
-            ev.push_back(e);
-        }
-        return MBAR_B200_OK;
-    }
-    float ms(size_t a, size_t b) const {
-        float m = 0.f;
-        event_ms(ev[a], ev[b], &m);
-        return m;
-    }
-    int start(cudaStream_t stream) {
-        s = stream;
-        MBAR_TRY(create(2));
-        MBAR_CUDA(cudaEventRecord(ev[0], s));
-        return MBAR_B200_OK;
-    }
-    float stop() {
-        cudaEventRecord(ev[1], s);
-        cudaEventSynchronize(ev[1]);
-        return ms(0, 1);
-    }
-};
-
 // stream-ordered rendezvous of all ranks (one tiny all-reduce) before the first in-kernel peer exchange of a loop
 static int comm_rendezvous(mbar_b200_ctx* c) {
     if (!c->comm || c->nranks == 1) return MBAR_B200_OK;
@@ -1148,7 +1111,7 @@ int mbar_b200_sci_iterate(mbar_b200_ctx* c, double* f, int32_t iters) {
     MBAR_CUDA(cudaStreamSynchronize(c->stream));
     c->d2hBytes += K * 8 + lay.size(false) * 8;
     float ms = 0.f;
-    if (event_ms(c->evA, c->evB, &ms)) c->lastPassMs = ms;   // (no pass has run on a fresh context with iters = 0)
+    if (event_ms(c->ev0, c->ev1, &ms)) c->lastPassMs = ms;   // (no pass has run on a fresh context with iters = 0)
     MBAR_REQUIRE(!(iters > 0 && c->h_out[lay.flag()] >= 1.0e6), MBAR_B200_ERR_COMM,
                  "peer exchange timed out inside the pass kernel (a rank did not arrive)");
     if (p.debugSkip) return MBAR_B200_OK;   // memory-pipeline probe: the arithmetic was skipped, nothing to return

@@ -866,11 +866,10 @@ int fused_prepare(mbar_b200_ctx* ctx, const double* h_f, bool wantL, bool allSta
     p.partial = ctx->d_partial;
     p.out = ctx->d_out;
     p.ticket = ctx->d_ticket;
-    if (wantL && !ctx->d_L)
-        MBAR_CUDA(cudaMalloc((void**)&ctx->d_L, (size_t)ctx->nTiles * TILE_N * sizeof(double)));
-    p.Lout = wantL ? ctx->d_L : nullptr;
+    if (wantL) MBAR_TRY(ensure_L(ctx));
+    p.Lout = wantL ? ctx->d_L.ptr : nullptr;
     // weights for the K > 64 Hessian path ride along when the caller is about to evaluate the Hessian at this f
-    p.Wout = (wantW && !allStates && M == 1 && ensure_weight_buffer(ctx)) ? ctx->d_Wt : nullptr;
+    p.Wout = (wantW && !allStates && M == 1 && ensure_weight_buffer(ctx)) ? ctx->d_Wt.ptr : nullptr;
     p.wgt = ctx->d_wgt;
     p.sumW = ctx->d_wgt ? ctx->sumW : (double)ctx->N;
     for (int k = 0; k < K; ++k)
@@ -942,7 +941,7 @@ int fused_enqueue(mbar_b200_ctx* ctx, const FusedParams& p) {
         MBAR_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
         attrSet[which] = smem;
     }
-    if (!ctx->capturing) MBAR_CUDA(cudaEventRecord(ctx->evA, ctx->stream));
+    if (!ctx->capturing) MBAR_CUDA(cudaEventRecord(ctx->ev0, ctx->stream));
     if (p.CL == 1) {
         kern<<<(unsigned)grid, p.CW * 32, smem, ctx->stream>>>(p);
     } else {
@@ -960,7 +959,7 @@ int fused_enqueue(mbar_b200_ctx* ctx, const FusedParams& p) {
         cfg.numAttrs = 1;
         MBAR_CUDA(cudaLaunchKernelEx(&cfg, kern, p));
     }
-    if (!ctx->capturing) MBAR_CUDA(cudaEventRecord(ctx->evB, ctx->stream));
+    if (!ctx->capturing) MBAR_CUDA(cudaEventRecord(ctx->ev1, ctx->stream));
     ctx->launches++;
     ctx->passes++;
     MBAR_CUDA(cudaGetLastError());

@@ -231,8 +231,7 @@ int launch_pass_generic(mbar_b200_ctx* ctx, const double* h_f, bool wantL, bool 
     MBAR_REQUIRE(W >= 1, MBAR_B200_ERR_INVALID, "K=%d too large for the generic kernel", K);
     const size_t smem = 256 + (size_t)W * perWarp;
     const bool needUnsampled = logAll || (int)ctx->active.size() < K;
-    if (wantL && !ctx->d_L)
-        MBAR_CUDA(cudaMalloc((void**)&ctx->d_L, (size_t)ctx->nTiles * TILE_N * sizeof(double)));
+    if (wantL) MBAR_TRY(ensure_L(ctx));
     int64_t grid = (ctx->nTiles + W - 1) / W;
     const int64_t maxGrid = (int64_t)ctx->smCount * (smem > 100 * 1024 ? 1 : 2);
     if (grid > maxGrid) grid = maxGrid;
@@ -241,13 +240,13 @@ int launch_pass_generic(mbar_b200_ctx* ctx, const double* h_f, bool wantL, bool 
     MBAR_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
     snprintf(ctx->lastKernel, sizeof(ctx->lastKernel), "pass_generic_kernel<%s> grid=%lld warps=%d",
              needUnsampled ? "log-domain rows" : "linear rows", (long long)grid, W);
-    MBAR_CUDA(cudaEventRecord(ctx->evA, ctx->stream));
+    MBAR_CUDA(cudaEventRecord(ctx->ev0, ctx->stream));
     kern<<<(unsigned)grid, W * 32, smem, ctx->stream>>>(ctx->d_u, K, ctx->N, ctx->nTiles, ctx->dc(ROW_C),
                                                        ctx->dc(ROW_GEN_F), ctx->d_rowmask,
                                                        logAll ? ctx->d_zeromask : ctx->d_rowmask, ctx->d_Nk,
                                                        ctx->d_partial, ctx->d_out, ctx->d_ticket,
-                                                       wantL ? ctx->d_L : nullptr, ctx->d_wgt, W);
-    MBAR_CUDA(cudaEventRecord(ctx->evB, ctx->stream));
+                                                       wantL ? ctx->d_L.ptr : nullptr, ctx->d_wgt, W);
+    MBAR_CUDA(cudaEventRecord(ctx->ev1, ctx->stream));
     ctx->launches++;
     ctx->passes++;
     MBAR_CUDA(cudaGetLastError());

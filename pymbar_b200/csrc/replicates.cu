@@ -188,26 +188,6 @@ __global__ void rep_combine_kernel(const double2* __restrict__ partial, int nGro
 
 using namespace mbar;
 
-namespace {
-
-// Pinned staging of the counts (two batches) and the call's events, released on every return path once the streams
-// have drained.
-struct RepCall {
-    mbar_b200_ctx* c;
-    uint16_t* pinned = nullptr;
-    cudaEvent_t ev[6] = {nullptr, nullptr, nullptr, nullptr, nullptr, nullptr};   // copied[2], used[2], start, end
-    explicit RepCall(mbar_b200_ctx* c_) : c(c_) {}
-    ~RepCall() {
-        cudaStreamSynchronize(c->copyStream);
-        cudaStreamSynchronize(c->stream);
-        if (pinned) cudaFreeHost(pinned);
-        for (cudaEvent_t e : ev)
-            if (e) cudaEventDestroy(e);
-    }
-};
-
-}  // namespace
-
 int mbar_b200_replicate_unsampled(mbar_b200_ctx* c, int64_t B, const uint16_t* counts, const double* F, double* out) {
     MBAR_REQUIRE(c && counts && F && out, MBAR_B200_ERR_INVALID, "replicate_unsampled: NULL argument");
     MBAR_REQUIRE(B >= 1, MBAR_B200_ERR_INVALID, "replicate_unsampled: B = %lld must be at least 1", (long long)B);
@@ -269,12 +249,15 @@ int mbar_b200_replicate_unsampled(mbar_b200_ctx* c, int64_t B, const uint16_t* c
     MBAR_TRY(buf.alloc(&d_act, (size_t)Ks));
     MBAR_TRY(buf.alloc(&d_uns, (size_t)nu));
     MBAR_TRY(buf.alloc(&d_partial, (size_t)groups * chunks * REP_BATCH * JC));
-    RepCall call(c);
+    // pinned staging of the counts (two batches) and the call's events: copied[2], used[2], start, end
     const size_t slotElems = (size_t)REP_BATCH * nPad;
-    MBAR_CUDA(cudaHostAlloc((void**)&call.pinned, 2 * slotElems * sizeof(uint16_t), cudaHostAllocDefault));
-    for (cudaEvent_t& e : call.ev) MBAR_CUDA(cudaEventCreate(&e));
-    cudaEvent_t* copied = call.ev;
-    cudaEvent_t* used = call.ev + 2;
+    HostPinned<uint16_t> pinned;
+    Events ev;
+    StreamDrain guard{c};
+    MBAR_TRY(pinned.reserve(2 * slotElems, "replicate_unsampled"));
+    MBAR_TRY(ev.create(6));
+    const cudaEvent_t* copied = ev.ev.data();
+    const cudaEvent_t* used = copied + 2;
     cudaStream_t s = c->stream;
     MBAR_CUDA(cudaMemcpyAsync(d_c, h_c.data(), h_c.size() * sizeof(double), cudaMemcpyHostToDevice, s));
     MBAR_CUDA(cudaMemcpyAsync(d_act, c->active.data(), (size_t)Ks * sizeof(int), cudaMemcpyHostToDevice, s));
@@ -300,13 +283,13 @@ int mbar_b200_replicate_unsampled(mbar_b200_ctx* c, int64_t B, const uint16_t* c
     // counts go up one batch ahead on the copy stream, through two pinned slots (zero past N once for all)
     for (int slot = 0; slot < 2; ++slot)
         for (int b = 0; b < REP_BATCH; ++b)
-            std::memset(call.pinned + slot * slotElems + (size_t)b * nPad + N, 0, (size_t)(nPad - N) * sizeof(uint16_t));
+            std::memset(pinned + slot * slotElems + (size_t)b * nPad + N, 0, (size_t)(nPad - N) * sizeof(uint16_t));
     for (int64_t i = 0; i < nBatches; ++i) {
         const int slot = (int)(i & 1);
         const int64_t b0 = i * REP_BATCH;
         const int RB = (int)std::min<int64_t>(REP_BATCH, B - b0);
         if (i >= 2) MBAR_CUDA(cudaEventSynchronize(used[slot]));     // batch i - 2 no longer reads this slot
-        uint16_t* hp = call.pinned + slot * slotElems;
+        uint16_t* hp = pinned + slot * slotElems;
         for (int b = 0; b < RB; ++b)
             std::memcpy(hp + (size_t)b * nPad, counts + (size_t)(b0 + b) * N, (size_t)N * sizeof(uint16_t));
         uint16_t* dp = d_counts + slot * slotElems;
@@ -315,7 +298,7 @@ int mbar_b200_replicate_unsampled(mbar_b200_ctx* c, int64_t B, const uint16_t* c
         MBAR_CUDA(cudaEventRecord(copied[slot], c->copyStream));
         c->h2dBytes += (int64_t)RB * nPad * 2;
         MBAR_CUDA(cudaStreamWaitEvent(s, copied[slot], 0));
-        if (i == 0) MBAR_CUDA(cudaEventRecord(call.ev[4], s));
+        if (i == 0) MBAR_CUDA(cudaEventRecord(ev[4], s));
         p.counts = dp;
         p.c = d_c + (size_t)b0 * Ks;
         p.RB = RB;
@@ -327,7 +310,7 @@ int mbar_b200_replicate_unsampled(mbar_b200_ctx* c, int64_t B, const uint16_t* c
         MBAR_CUDA(cudaGetLastError());
         MBAR_CUDA(cudaEventRecord(used[slot], s));
     }
-    MBAR_CUDA(cudaEventRecord(call.ev[5], s));
+    MBAR_CUDA(cudaEventRecord(ev[5], s));
     MBAR_CUDA(cudaMemcpyAsync(out, d_out, (size_t)B * nu * sizeof(double), cudaMemcpyDeviceToHost, s));
     MBAR_CUDA(cudaStreamSynchronize(s));
     c->d2hBytes += (int64_t)B * nu * 8;
@@ -338,7 +321,7 @@ int mbar_b200_replicate_unsampled(mbar_b200_ctx* c, int64_t B, const uint16_t* c
             for (int64_t b = 0; b < B; ++b) out[(size_t)b * nu + q] = INFINITY;
     }
     float ms = 0.f;
-    if (event_ms(call.ev[4], call.ev[5], &ms)) c->lastRepMs = ms;
+    if (event_ms(ev[4], ev[5], &ms)) c->lastRepMs = ms;
     c->lastRepBatches = (int)nBatches;
     c->lastRepExps = pairs * ((int64_t)Ks * chunks + nu);
     return MBAR_B200_OK;

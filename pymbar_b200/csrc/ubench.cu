@@ -53,11 +53,12 @@ extern "C" int mbar_b200_measure_fp64_peak(int device, double* dmma_tflops, doub
     cudaDeviceProp prop;
     MBAR_CUDA(cudaGetDeviceProperties(&prop, device));
     const int sms = prop.multiProcessorCount;
+    CallBuffers buf("measure_fp64_peak");
     double* d = nullptr;
-    MBAR_CUDA(cudaMalloc((void**)&d, (size_t)sms * 512 * sizeof(double)));
-    cudaEvent_t e0, e1;
-    MBAR_CUDA(cudaEventCreate(&e0));
-    MBAR_CUDA(cudaEventCreate(&e1));
+    MBAR_TRY(buf.alloc(&d, (size_t)sms * 512));
+    Events ev;
+    MBAR_TRY(ev.create(2));
+    const cudaEvent_t e0 = ev[0], e1 = ev[1];
     const int iters = 4096;
     double best[2] = {0.0, 0.0};
     for (int which = 0; which < 2; ++which) {
@@ -76,9 +77,6 @@ extern "C" int mbar_b200_measure_fp64_peak(int device, double* dmma_tflops, doub
             if (rep > 0 && tf > best[which]) best[which] = tf;
         }
     }
-    cudaEventDestroy(e0);
-    cudaEventDestroy(e1);
-    cudaFree(d);
     MBAR_CUDA(cudaGetLastError());
     if (dmma_tflops) *dmma_tflops = best[0];
     if (dfma_tflops) *dfma_tflops = best[1];
@@ -96,8 +94,9 @@ extern "C" int mbar_b200_probe_exp(int device, int which, int64_t n, const doubl
     }
     if (n == 0) return MBAR_B200_OK;
     MBAR_CUDA(cudaSetDevice(device));
+    CallBuffers buf("probe_exp");
     double* d = nullptr;
-    MBAR_CUDA(cudaMalloc((void**)&d, 2 * (size_t)n * sizeof(double)));
+    MBAR_TRY(buf.alloc(&d, 2 * (size_t)n));
     int rc = MBAR_B200_OK;
     if (cudaMemcpy(d, a_host, (size_t)n * sizeof(double), cudaMemcpyHostToDevice) != cudaSuccess) {
         set_error("probe_exp: H2D copy failed");
@@ -109,7 +108,6 @@ extern "C" int mbar_b200_probe_exp(int device, int which, int64_t n, const doubl
         set_error("probe_exp: D2H copy failed");
         rc = MBAR_B200_ERR_CUDA;
     }
-    cudaFree(d);
     cudaGetLastError();
     return rc;
 }

@@ -235,13 +235,6 @@ __global__ void work_finalize2_kernel(const WorkReq* __restrict__ req, int nReq,
     }
 }
 
-// grow a per-call buffer to hold `count` elements, with room to spare for a somewhat larger call
-template <class T>
-static int work_grow(DevArray<T>& a, int64_t count) {
-    if ((size_t)count <= a.cap) return MBAR_B200_OK;
-    return a.reserve((size_t)(count + count / 2 + 64), "work");
-}
-
 }  // namespace mbar
 
 using namespace mbar;
@@ -313,10 +306,10 @@ int mbar_b200_work_evaluate(mbar_b200_work* o, int32_t n_requests, const int32_t
     MBAR_REQUIRE(items < INT32_MAX, MBAR_B200_ERR_INVALID, "work_evaluate: %lld chunks in one call", (long long)items);
     MBAR_CUDA(cudaSetDevice(o->device));
     NvtxRange nvtx_("mbar_b200::work_evaluate");
-    MBAR_TRY(work_grow(o->d_req, (int64_t)n_requests));
-    MBAR_TRY(work_grow(o->d_part, 2 * items));
-    MBAR_TRY(work_grow(o->d_shift, 2 * (int64_t)n_requests));
-    MBAR_TRY(work_grow(o->d_out, 3 * (int64_t)n_requests));
+    MBAR_TRY(o->d_req.grow(n_requests, "work"));
+    MBAR_TRY(o->d_part.grow(2 * items, "work"));
+    MBAR_TRY(o->d_shift.grow(2 * (int64_t)n_requests, "work"));
+    MBAR_TRY(o->d_out.grow(3 * (int64_t)n_requests, "work"));
     MBAR_CUDA(cudaMemcpyAsync(o->d_req, req.data(), req.size() * sizeof(WorkReq), cudaMemcpyHostToDevice, o->stream));
     const unsigned rb = (unsigned)((n_requests + 127) / 128);
     MBAR_CUDA(cudaEventRecord(o->ev0, o->stream));
