@@ -21,11 +21,11 @@
 // for that).  A weighted request names a slot and gets exactly what DeviceProblem.set_sample_weights(c) and the
 // matching single-problem call give: S_k = sum_n c_n e^{a_kn}, Ghat_ij = sum_n c_n w_in w_jn and
 // sum L = sum_n c_n L'_n - sum_n c_n x_n, with L'_n itself unweighted (the denominators keep N_k).  It is the same
-// kernel instantiated with W = true; the unweighted instantiation compiles to the code it had before slots existed.
-// Multiplying by c_n = 1 is exact and the order of operations is the same in both instantiations, so all-ones counts
-// give the bits of the unweighted request.  A zero-count sample enters no sum: its L'_n is not added to sum L and its
-// a_kn is -inf before the NaN test and the warp max of an unsampled row, as log c_n = -inf is in the single-problem
-// pass, so an undrawn sample whose sampled energies are all +inf does not flag its replicate.
+// kernel instantiated with W = true.  Multiplying by c_n = 1 is exact and the order of operations is the same in both
+// instantiations, so all-ones counts give the bits of the unweighted request.  A zero-count sample enters no sum: its
+// L'_n is not added to sum L and its a_kn is -inf before the NaN test and the warp max of an unsampled row, as
+// log c_n = -inf is in the single-problem pass, so an undrawn sample whose sampled energies are all +inf does not flag
+// its replicate.
 //
 // Determinism.  Work items are (request, chunk) pairs; a chunk is CT_p tiles with CT_p a function of (N_p, K_p) alone.
 // Warp w of a CTA takes the chunk's tiles w, w + 4, ... in order and folds each tile into its own (max, sum) pairs;
@@ -48,6 +48,7 @@ constexpr int BATCH_WARPS = BATCH_THREADS / 32;
 constexpr int BATCH_ROUND = BATCH_THREADS;          // samples per round
 constexpr int BATCH_SW_LD = BATCH_ROUND + 1;        // leading dimension of the staged weights (bank spread)
 constexpr int BATCH_GSLOTS = (BATCH_MAX_K * (BATCH_MAX_K + 1) / 2 + BATCH_THREADS - 1) / BATCH_THREADS;
+constexpr int BATCH_FINALIZE_THREADS = 256;         // one CTA per request: up to 18528 Gram entries at R = 192
 constexpr int64_t BATCH_MAX_CHUNKS = 4096;
 
 // tiles per chunk: about 64k entries of u' per chunk, at most BATCH_MAX_CHUNKS chunks per problem
@@ -57,6 +58,8 @@ __host__ __device__ __forceinline__ int64_t batch_chunk_tiles(int64_t nT, int K)
     return base > need ? base : need;
 }
 
+// One request: a problem's K rows, a replicate slot's, or a problem's K resident rows followed by its M appended
+// rows; R = K + M rows in all.
 struct BatchReq {
     int64_t uoff;     // first double of the problem's tiles
     int64_t N, nT;    // samples and tiles of the problem
@@ -69,13 +72,23 @@ struct BatchReq {
     int32_t K;
     int32_t prob;     // the problem, or for a weighted request its replicate slot: indexes sum x (sum c x)
     int32_t allRows, wantG;
+    // appended rows (M = 0 for every other request); the Gram of such a request is batch_aug_gram_kernel's
+    int32_t M;
+    int64_t aoff;     // first double of the problem's appended tiles
+    int64_t gct;      // tiles per Gram chunk
+    int64_t gitem0;   // first (request, block pair, Gram chunk) item
+    int64_t gpoff;    // first double of the request's Gram partials
+    int64_t loff;     // first entry of the request's L'_n scratch
 };
 
-// per-request packed output: [0, K) S, [K, 2K) log S, [2K] sum L, [2K + 1] flag, then K x K Ghat when asked for
-__host__ __device__ __forceinline__ int64_t batch_out_size(int K, bool G) { return 2 * K + 2 + (G ? (int64_t)K * K : 0); }
-// per-chunk partial: K (max, sum) pairs, sum L', bad flag, then the K (K + 1) / 2 lower-triangle Gram entries
-__host__ __device__ __forceinline__ int64_t batch_part_size(int K, bool G) {
-    return 2 * K + 2 + (G ? (int64_t)K * (K + 1) / 2 : 0);
+// per-request packed output: [0, R) S, [R, 2R) log S, [2R] sum L, [2R + 1] flag, then R x R Ghat when asked for
+__host__ __device__ __forceinline__ int64_t batch_out_size(int R, bool G) {
+    return 2 * R + 2 + (G ? (int64_t)R * R : 0);
+}
+// per-chunk partial: R (max, sum) pairs, sum L', bad flag, then, with the in-pass Gram, its R (R + 1) / 2
+// lower-triangle entries
+__host__ __device__ __forceinline__ int64_t batch_part_size(int R, bool G) {
+    return 2 * R + 2 + (G ? (int64_t)R * (R + 1) / 2 : 0);
 }
 
 // one problem's layout for the upload kernels: raw offset, tile offset, first tile, samples, K-vector offset, states
@@ -97,20 +110,6 @@ __host__ __device__ __forceinline__ int64_t aug_gram_tiles(int64_t nT) {
     return need > AUG_GRAM_MIN_TILES ? need : AUG_GRAM_MIN_TILES;
 }
 __host__ __device__ __forceinline__ int aug_blocks(int R) { return (R + AUG_BLOCK - 1) / AUG_BLOCK; }
-
-// one augmented request: the problem's K_p resident rows followed by its M_p appended rows, R_p = K_p + M_p
-struct AugReq {
-    int64_t uoff, aoff;      // first double of the problem's tiles and of its appended tiles
-    int64_t N, nT;           // samples and tiles of the problem
-    int64_t ct, gct;         // tiles per pass chunk and per Gram chunk
-    int64_t item0, gitem0;   // first (request, chunk) item of the pass and first (request, block pair, chunk) item
-    int64_t poff, gpoff;     // first double of the request's pass partials and Gram partials
-    int64_t ooff, voff, foff, loff;  // packed output, K-vectors (N_k, log N_k), f [R_p], L'_n scratch
-    int32_t K, M, prob, wantG;
-};
-
-// packed output: [0, R) S, [R, 2R) log S, [2R] sum L, [2R + 1] flag, then R x R Ghat when asked for
-__host__ __device__ __forceinline__ int64_t aug_out_size(int R, bool G) { return 2 * R + 2 + (G ? (int64_t)R * R : 0); }
 
 // one problem's appended rows for the upload kernel: raw offset, appended tile offset, first tile of the problem
 // (indexes x_n), first tile among the appended problems, samples, rows
@@ -142,7 +141,6 @@ struct mbar_b200_batch : mbar::Resident {
     std::vector<int> M;                         // appended rows of each problem (0: none)
     std::vector<int64_t> aoff;                  // first double of each problem's appended tiles
     mbar::DevArray<double> d_ua;                // appended tiles [nT_p][M_p][32] of u - x_n
-    mbar::DevArray<mbar::AugReq> d_areq;
     mbar::DevArray<double> d_L, d_gpart;        // L'_n of each Gram request, Gram chunk partials
     // per-call buffers, grown on demand
     mbar::DevArray<mbar::BatchReq> d_req;
@@ -156,16 +154,27 @@ struct mbar_b200_batch : mbar::Resident {
 
 namespace mbar {
 
-// ---- upload: raw row-major problems -> shifted tiles, x_n, sum x_n -------------------------------------------------
-__device__ __forceinline__ int batch_find_tile(const BatchProbDev* __restrict__ pr, int P, int64_t tile) {
-    int lo = 0, hi = P - 1;
+// the last of n segments whose start(s) <= i, for ascending starts with start(0) <= i
+template <class Start>
+__device__ __forceinline__ int find_segment(int n, int64_t i, Start start) {
+    int lo = 0, hi = n - 1;
     while (lo < hi) {
         const int mid = (lo + hi + 1) >> 1;
-        if (pr[mid].tile0 <= tile) lo = mid;
+        if (start(mid) <= i) lo = mid;
         else hi = mid - 1;
     }
     return lo;
 }
+
+// entry e = i (i + 1) / 2 + j of a lower triangle -> (row i, column j), i >= j
+__device__ __forceinline__ int2 tri_decode(int e) {
+    int i = (int)((sqrt(8.0 * e + 1.0) - 1.0) * 0.5);
+    while ((i + 1) * (i + 2) / 2 <= e) ++i;
+    while (i * (i + 1) / 2 > e) --i;
+    return make_int2(i, e - i * (i + 1) / 2);
+}
+
+// ---- upload: raw row-major problems -> shifted tiles, x_n, sum x_n -------------------------------------------------
 
 // one warp per tile, one lane per sample; bad[0] counts NaN or -inf energies
 __global__ void __launch_bounds__(256) batch_retile_kernel(const double* __restrict__ raw,
@@ -176,7 +185,7 @@ __global__ void __launch_bounds__(256) batch_retile_kernel(const double* __restr
     const int64_t tile = (int64_t)blockIdx.x * 8 + (threadIdx.x >> 5);
     if (tile >= nTiles) return;
     const int lane = threadIdx.x & 31;
-    const int p = batch_find_tile(pr, P, tile);
+    const int p = find_segment(P, tile, [&](int s) { return pr[s].tile0; });
     const BatchProbDev q = pr[p];
     const int64_t t = tile - q.tile0;
     const int64_t n = t * 32 + lane;
@@ -221,17 +230,24 @@ __global__ void __launch_bounds__(256) batch_sumx_kernel(const double* __restric
     if (threadIdx.x == 0) sumx[blockIdx.x] = sh[0];
 }
 
-// ---- the moments pass ---------------------------------------------------------------------------------------------
-__device__ __forceinline__ int batch_find_item(const BatchReq* __restrict__ req, int nReq, int64_t item) {
-    int lo = 0, hi = nReq - 1;
-    while (lo < hi) {
-        const int mid = (lo + hi + 1) >> 1;
-        if (req[mid].item0 <= item) lo = mid;
-        else hi = mid - 1;
-    }
-    return lo;
+// appended rows -> shifted tiles: one warp per appended tile, one lane per sample
+__global__ void __launch_bounds__(256) batch_aug_retile_kernel(const double* __restrict__ raw,
+                                                               const AugProbDev* __restrict__ pr, int n,
+                                                               int64_t nTiles, const double* __restrict__ x,
+                                                               double* __restrict__ ua) {
+    const int64_t tile = (int64_t)blockIdx.x * 8 + (threadIdx.x >> 5);
+    if (tile >= nTiles) return;
+    const int lane = threadIdx.x & 31;
+    const AugProbDev q = pr[find_segment(n, tile, [&](int p) { return pr[p].atile0; })];
+    const int64_t t = tile - q.atile0;
+    const int64_t s = t * 32 + lane;
+    const bool valid = s < q.N;
+    const double xn = x[(q.tile0 + t) * 32 + lane];
+    double* dst = ua + q.aoff + t * q.M * 32 + lane;
+    for (int m = 0; m < q.M; ++m) dst[m * 32] = valid ? raw[q.roff + (int64_t)m * q.N + s] - xn : INFINITY;
 }
 
+// ---- the pass ------------------------------------------------------------------------------------------------------
 __device__ __forceinline__ double warp_max(double x) {
 #pragma unroll
     for (int o = 16; o > 0; o >>= 1) x = fmax(x, __shfl_xor_sync(0xffffffffu, x, o));
@@ -249,48 +265,61 @@ __device__ __forceinline__ void pair_merge(double& m, double& s, double m2, doub
     }
 }
 
-// W: weighted requests (q.prob names a replicate slot; its counts start at slotCoff[q.prob]).  Every request of a
-// launch is weighted or none is.
-template <bool W>
-__global__ void __launch_bounds__(BATCH_THREADS) batch_moments_kernel(
+// row k of a request at tile t: the problem's own tiles for k < K, its appended tiles after
+__device__ __forceinline__ const double* batch_row(const double* __restrict__ u, const double* __restrict__ ua,
+                                                   const BatchReq& q, int64_t t, int k, int lane) {
+    return k < q.K ? u + q.uoff + (t * q.K + k) * 32 + lane : ua + q.aoff + (t * q.M + (k - q.K)) * 32 + lane;
+}
+
+// One CTA per (request, chunk) item; every request of a launch is of one kind:
+//   W: weighted requests (q.prob names a replicate slot; its counts start at slotCoff[q.prob]);
+//   APPENDED: requests with appended rows, every row asked for; with the Gram, L'_n goes to Lbuf for
+//     batch_aug_gram_kernel instead of an in-pass Gram.
+template <bool W, bool APPENDED>
+__global__ void __launch_bounds__(BATCH_THREADS) batch_pass_kernel(
     const double* __restrict__ u, const BatchReq* __restrict__ req, int nReq, const double* __restrict__ fAll,
     const double* __restrict__ NkAll, const double* __restrict__ logNkAll, double* __restrict__ part,
-    const int64_t* __restrict__ slotCoff, const uint16_t* __restrict__ counts) {
+    const int64_t* __restrict__ slotCoff, const uint16_t* __restrict__ counts, const double* __restrict__ ua,
+    double* __restrict__ Lbuf) {
+    constexpr int MAX_R = APPENDED ? AUG_MAX_R : BATCH_MAX_K;
     extern __shared__ __align__(16) double sW[];                  // [K][BATCH_SW_LD] staged Gram weights
-    __shared__ double sM[BATCH_WARPS][BATCH_MAX_K], sS[BATCH_WARPS][BATCH_MAX_K];
-    __shared__ double sF[BATCH_MAX_K], sC[BATCH_MAX_K], sLs[BATCH_MAX_K];
-    __shared__ int sRow[BATCH_MAX_K];                             // 1 sampled, 2 unsampled and asked for, 0 neither
+    __shared__ double sM[BATCH_WARPS][MAX_R], sS[BATCH_WARPS][MAX_R];
+    __shared__ double sF[MAX_R], sC[BATCH_MAX_K], sLs[BATCH_MAX_K];
+    __shared__ int sRow[MAX_R];                                   // 1 sampled, 2 unsampled and asked for, 0 neither
     __shared__ double sRed[BATCH_THREADS];
     __shared__ int sBad;
     const int64_t item = blockIdx.x;
-    const BatchReq q = req[batch_find_item(req, nReq, item)];
+    const BatchReq q = req[find_segment(nReq, item, [&](int r) { return req[r].item0; })];
     const int64_t chunk = item - q.item0;
-    const int K = q.K;
+    const int K = q.K, R = APPENDED ? K + q.M : K;
+    const bool G = !APPENDED && q.wantG;                          // the in-pass Gram
     const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
-    if (tid < K) {
-        const double n = NkAll[q.voff + tid];
-        sF[tid] = fAll[q.foff + tid];
-        sC[tid] = n > 0.0 ? sF[tid] + logNkAll[q.voff + tid] : -INFINITY;
-        sLs[tid] = n > 0.0 ? logNkAll[q.voff + tid] : 0.0;
-        sRow[tid] = n > 0.0 ? 1 : (q.allRows ? 2 : 0);
+#pragma unroll
+    for (int k0 = 0; k0 < MAX_R; k0 += BATCH_THREADS) {            // thread tid takes rows tid, tid + 128, ...
+        const int k = k0 + tid;
+        if (k >= R) break;
+        const bool sampled = k < K && NkAll[q.voff + k] > 0.0;
+        sF[k] = fAll[q.foff + k];
+        if (k < K) {
+            sC[k] = sampled ? sF[k] + logNkAll[q.voff + k] : -INFINITY;
+            if (!APPENDED) sLs[k] = sampled ? logNkAll[q.voff + k] : 0.0;
+        }
+        sRow[k] = sampled ? 1 : (q.allRows ? 2 : 0);
     }
-    for (int k = tid; k < BATCH_WARPS * BATCH_MAX_K; k += BATCH_THREADS) {
+    for (int k = tid; k < BATCH_WARPS * MAX_R; k += BATCH_THREADS) {
         (&sM[0][0])[k] = -INFINITY;
         (&sS[0][0])[k] = 0.0;
     }
     if (tid == 0) sBad = 0;
     // lower-triangle Gram entries of this thread: e = tid + BATCH_THREADS * slot, row i >= column j
-    const int E = q.wantG ? K * (K + 1) / 2 : 0;
+    const int E = G ? K * (K + 1) / 2 : 0;
     int gi[BATCH_GSLOTS], gj[BATCH_GSLOTS];
     double gacc[BATCH_GSLOTS];
 #pragma unroll
     for (int sl = 0; sl < BATCH_GSLOTS; ++sl) {
-        const int e = tid + BATCH_THREADS * sl;
-        int i = (int)((sqrt(8.0 * e + 1.0) - 1.0) * 0.5);
-        while ((i + 1) * (i + 2) / 2 <= e) ++i;
-        while (i * (i + 1) / 2 > e) --i;
-        gi[sl] = i;
-        gj[sl] = e - i * (i + 1) / 2;
+        const int2 ij = tri_decode(tid + BATCH_THREADS * sl);
+        gi[sl] = ij.x;
+        gj[sl] = ij.y;
         gacc[sl] = 0.0;
     }
     __syncthreads();
@@ -314,7 +343,7 @@ __global__ void __launch_bounds__(BATCH_THREADS) batch_moments_kernel(
         double cn = 1.0;
         if constexpr (W) {
             cn = valid ? (double)__ldg(cq + n) : 0.0;
-            if (q.wantG) sCn[tid] = cn;
+            if (G) sCn[tid] = cn;
         }
         double Lp = 0.0;
         if (valid) {
@@ -331,13 +360,15 @@ __global__ void __launch_bounds__(BATCH_THREADS) batch_moments_kernel(
                 sumL += Lp;
             }
         }
-        if (tileOn)
-            for (int k = 0; k < K; ++k) {
+        if (tileOn) {
+            if (APPENDED && q.wantG) Lbuf[q.loff + n] = Lp;
+            for (int k = 0; k < R; ++k) {
                 if (sRow[k] == 0) {
-                    if (q.wantG) sW[k * BATCH_SW_LD + tid] = 0.0;
+                    if (G) sW[k * BATCH_SW_LD + tid] = 0.0;
                     continue;
                 }
-                double a = valid ? sF[k] - __ldg(ut + k * 32) - Lp : -INFINITY;
+                double a = valid ? sF[k] - __ldg(APPENDED ? batch_row(u, ua, q, t, k, lane) : ut + k * 32) - Lp
+                                 : -INFINITY;
                 if constexpr (W)
                     if (cn == 0.0) a = -INFINITY;      // before the NaN test: an undrawn sample enters no sum
                 if (a != a) {
@@ -345,17 +376,17 @@ __global__ void __launch_bounds__(BATCH_THREADS) batch_moments_kernel(
                     a = -INFINITY;
                 }
                 // sampled rows: e^a <= 1 / N_k, summed linearly (the pair keeps max 0) as the single-problem pass
-                // sums them; unsampled rows: shifted by the warp's max
+                // sums them; every other row: shifted by the warp's max
                 const double wm = sRow[k] == 1 ? 0.0 : warp_max(a);
                 double e = wm > -INFINITY ? exp(a - wm) : 0.0;
                 if constexpr (W) e *= cn;
                 const double ws = warp_sum(e);
                 if (lane == 0) pair_merge(sM[warp][k], sS[warp][k], wm, ws);
-                if (q.wantG) sW[k * BATCH_SW_LD + tid] = exp(a + sLs[k]);
+                if (G) sW[k * BATCH_SW_LD + tid] = exp(a + sLs[k]);
             }
-        else if (q.wantG)
+        } else if (G)
             for (int k = 0; k < K; ++k) sW[k * BATCH_SW_LD + tid] = 0.0;
-        if (q.wantG) {
+        if (G) {
             __syncthreads();
 #pragma unroll
             for (int sl = 0; sl < BATCH_GSLOTS; ++sl) {
@@ -380,85 +411,177 @@ __global__ void __launch_bounds__(BATCH_THREADS) batch_moments_kernel(
         if (tid < o) sRed[tid] += sRed[tid + o];
         __syncthreads();
     }
-    const int64_t stride = batch_part_size(K, q.wantG);
+    const int64_t stride = batch_part_size(R, G);
     double* pc = part + q.poff + chunk * stride;
-    if (tid < K) {
-        double m = sM[0][tid], s = sS[0][tid];
-        for (int w = 1; w < BATCH_WARPS; ++w) pair_merge(m, s, sM[w][tid], sS[w][tid]);
-        pc[2 * tid] = m;
-        pc[2 * tid + 1] = s;
+#pragma unroll
+    for (int k0 = 0; k0 < MAX_R; k0 += BATCH_THREADS) {
+        const int k = k0 + tid;
+        if (k >= R) break;
+        double m = sM[0][k], s = sS[0][k];
+        for (int w = 1; w < BATCH_WARPS; ++w) pair_merge(m, s, sM[w][k], sS[w][k]);
+        pc[2 * k] = m;
+        pc[2 * k + 1] = s;
     }
     if (tid == 0) {
-        pc[2 * K] = sRed[0];
-        pc[2 * K + 1] = sBad ? 1.0 : 0.0;
+        pc[2 * R] = sRed[0];
+        pc[2 * R + 1] = sBad ? 1.0 : 0.0;
     }
 #pragma unroll
     for (int sl = 0; sl < BATCH_GSLOTS; ++sl) {
         const int e = tid + BATCH_THREADS * sl;
-        if (e < E) pc[2 * K + 2 + e] = gacc[sl];
+        if (e < E) pc[2 * R + 2 + e] = gacc[sl];
     }
 }
 
-// A request's chunk partials in chunk order -> its packed output.  The flag is set when a NaN reached a sum, when a
-// sampled row's S_k is outside (1e-280, 1e300) (the range the fused pass and the adaptive loop accept), when an
-// unsampled row asked for has a NaN or overflowing S_k, or, with the Gram, when an entry of Ghat is not finite: an
+// The Gram of appended-row requests, over (request, pair of 32-row blocks bi >= bj, Gram chunk) items: it rebuilds the
+// two blocks' weights of 128 samples at a time from the tiles and the pass's L'_n, stages them in shared memory and
+// accumulates a 2 x 4 patch of the 32 x 32 block per thread with DFMA, samples in order: thread
+// (ti, tj) = (tid / 8, tid % 8) owns rows 2 ti, 2 ti + 1 of block bi and columns tj + 8 c (c < 4) of block bj.  No
+// atomics, and the Gram chunking is a function of N_p alone.
+__global__ void __launch_bounds__(BATCH_THREADS) batch_aug_gram_kernel(
+    const double* __restrict__ u, const double* __restrict__ ua, const BatchReq* __restrict__ req, int nReq,
+    const double* __restrict__ fAll, const double* __restrict__ NkAll, const double* __restrict__ logNkAll,
+    const double* __restrict__ Lbuf, double* __restrict__ gpart) {
+    extern __shared__ __align__(16) double sAug[];               // [2][AUG_BLOCK][AUG_SW_LD] staged weights
+    __shared__ double sF[2][AUG_BLOCK], sLs[2][AUG_BLOCK];
+    const int64_t item = blockIdx.x;
+    const BatchReq q = req[find_segment(nReq, item, [&](int r) { return req[r].gitem0; })];
+    const int R = q.K + q.M;
+    const int64_t ngc = (q.nT + q.gct - 1) / q.gct;
+    const int64_t local = item - q.gitem0;
+    const int pair = (int)(local / ngc);
+    const int64_t gc = local - (int64_t)pair * ngc;
+    const int2 b2 = tri_decode(pair);
+    const int bi = b2.x, bj = b2.y;
+    const int nh = bi == bj ? 1 : 2;                             // a diagonal block stages one row block
+    const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+    if (tid < 2 * AUG_BLOCK) {
+        const int h = tid / AUG_BLOCK, i = tid % AUG_BLOCK;
+        const int k = (h ? bj : bi) * AUG_BLOCK + i;
+        const bool s = k < q.K && NkAll[q.voff + k] > 0.0;
+        sF[h][i] = k < R ? fAll[q.foff + k] : 0.0;
+        sLs[h][i] = s ? logNkAll[q.voff + k] : 0.0;
+    }
+    double* sWi = sAug;
+    double* sWj = nh == 2 ? sAug + AUG_BLOCK * AUG_SW_LD : sAug;
+    const int ti = tid >> 3, tj = tid & 7;
+    double acc[2][4];
+#pragma unroll
+    for (int e = 0; e < 2; ++e)
+#pragma unroll
+        for (int c = 0; c < 4; ++c) acc[e][c] = 0.0;
+    __syncthreads();
+    const int64_t t0 = gc * q.gct, t1 = min(q.nT, t0 + q.gct);
+    const int64_t rounds = (t1 - t0 + BATCH_WARPS - 1) / BATCH_WARPS;
+    for (int64_t r = 0; r < rounds; ++r) {
+        const int64_t t = t0 + r * BATCH_WARPS + warp;
+        const int64_t n = t * 32 + lane;
+        const bool valid = t < t1 && n < q.N;
+        const double Lp = valid ? Lbuf[q.loff + n] : 0.0;
+        for (int h = 0; h < nh; ++h) {
+            const int b = h ? bj : bi;
+            double* w = h ? sWj : sWi;
+            for (int i = 0; i < AUG_BLOCK; ++i) {
+                const int k = b * AUG_BLOCK + i;
+                double x = 0.0;
+                if (valid && k < R) x = exp(sF[h][i] - __ldg(batch_row(u, ua, q, t, k, lane)) - Lp + sLs[h][i]);
+                w[i * AUG_SW_LD + tid] = x;
+            }
+        }
+        __syncthreads();
+        const double* wa = sWi + (2 * ti) * AUG_SW_LD;
+        const double* wb = sWj + tj * AUG_SW_LD;
+#pragma unroll 4
+        for (int s = 0; s < BATCH_ROUND; ++s) {
+            const double a0 = wa[s], a1 = wa[AUG_SW_LD + s];
+#pragma unroll
+            for (int c = 0; c < 4; ++c) {
+                const double bc = wb[c * 8 * AUG_SW_LD + s];
+                acc[0][c] = fma(a0, bc, acc[0][c]);
+                acc[1][c] = fma(a1, bc, acc[1][c]);
+            }
+        }
+        __syncthreads();
+    }
+    double* pg = gpart + q.gpoff + local * (AUG_BLOCK * AUG_BLOCK);
+#pragma unroll
+    for (int e = 0; e < 2; ++e)
+#pragma unroll
+        for (int c = 0; c < 4; ++c) pg[(2 * ti + e) * AUG_BLOCK + tj + 8 * c] = acc[e][c];
+}
+
+// A request's partials in chunk order -> its packed output.  The flag is set when a NaN reached a sum, when a
+// sampled row's S_k is outside (1e-280, 1e300) (the range the fused pass and the adaptive loop accept), when any
+// other row asked for has a NaN or overflowing S_k, or, with the Gram, when an entry of Ghat is not finite: an
 // unsampled row's Gram weight e^{a_kn} is not shifted, so a weight above about e^355 overflows Ghat_kk while S_k is
 // still finite.  An unsampled row whose every weight is zero (all its energies +inf) reports S_k = 0,
-// log S_k = -inf, as the single-problem path does.
-__global__ void __launch_bounds__(BATCH_THREADS) batch_finalize_kernel(const BatchReq* __restrict__ req,
-                                                                       const double* __restrict__ part,
-                                                                       const double* __restrict__ NkAll,
-                                                                       const double* __restrict__ sumx,
-                                                                       double* __restrict__ out) {
+// log S_k = -inf, as the single-problem path does.  The Gram partials are the pass's per-chunk lower triangles or,
+// for appended rows, those of batch_aug_gram_kernel: block pair (bi, bj) and Gram chunk c at
+// gpoff + (pair * nGc + c) * 1024.
+__global__ void __launch_bounds__(BATCH_FINALIZE_THREADS) batch_finalize_kernel(const BatchReq* __restrict__ req,
+                                                                                const double* __restrict__ part,
+                                                                                const double* __restrict__ gpart,
+                                                                                const double* __restrict__ NkAll,
+                                                                                const double* __restrict__ sumx,
+                                                                                double* __restrict__ out) {
     __shared__ int sFlag;
     const BatchReq q = req[blockIdx.x];
-    const int K = q.K, tid = threadIdx.x;
-    const int64_t stride = batch_part_size(K, q.wantG);
+    const int K = q.K, R = q.K + q.M, tid = threadIdx.x;
+    const int64_t stride = batch_part_size(R, q.wantG && q.M == 0);
     const int64_t nc = (q.nT + q.ct - 1) / q.ct;
     const double* p0 = part + q.poff;
     double* o = out + q.ooff;
     if (tid == 0) sFlag = 0;
     __syncthreads();
-    if (tid < K) {
+    for (int k = tid; k < R; k += BATCH_FINALIZE_THREADS) {
         double m = -INFINITY, s = 0.0;
-        for (int64_t c = 0; c < nc; ++c) pair_merge(m, s, p0[c * stride + 2 * tid], p0[c * stride + 2 * tid + 1]);
+        for (int64_t c = 0; c < nc; ++c) pair_merge(m, s, p0[c * stride + 2 * k], p0[c * stride + 2 * k + 1]);
         const double logS = s > 0.0 ? m + log(s) : -INFINITY;
         const double S = m == 0.0 ? s : exp(logS);      // sampled rows: the linear sum itself
-        o[tid] = S;
-        o[K + tid] = logS;
-        const bool sampled = NkAll[q.voff + tid] > 0.0;
+        o[k] = S;
+        o[R + k] = logS;
+        const bool sampled = k < K && NkAll[q.voff + k] > 0.0;
         if (sampled && !(S > 1e-280 && S < 1e300)) sFlag = 1;
         if (!sampled && q.allRows && (logS != logS || !(S < INFINITY))) sFlag = 1;
     }
     if (tid == 0) {
         double sl = 0.0, bad = 0.0;
         for (int64_t c = 0; c < nc; ++c) {
-            sl += p0[c * stride + 2 * K];
-            bad = fmax(bad, p0[c * stride + 2 * K + 1]);
+            sl += p0[c * stride + 2 * R];
+            bad = fmax(bad, p0[c * stride + 2 * R + 1]);
         }
-        o[2 * K] = sl - sumx[q.prob];
+        o[2 * R] = sl - sumx[q.prob];
         if (bad > 0.0 || sl != sl) sFlag = 1;
     }
     if (q.wantG) {
-        const int E = K * (K + 1) / 2;
-        for (int e = tid; e < E; e += BATCH_THREADS) {
-            int i = (int)((sqrt(8.0 * e + 1.0) - 1.0) * 0.5);
-            while ((i + 1) * (i + 2) / 2 <= e) ++i;
-            while (i * (i + 1) / 2 > e) --i;
-            const int j = e - i * (i + 1) / 2;
+        const int E = R * (R + 1) / 2;
+        for (int e = tid; e < E; e += BATCH_FINALIZE_THREADS) {
+            const int2 ij = tri_decode(e);
+            const int i = ij.x, j = ij.y;
+            const double* pg = p0 + 2 * R + 2 + e;        // entry e of chunk c at pg[c * gs], c < ngc
+            int64_t gs = stride, ngc = nc;
+            if (q.M > 0) {
+                const int bi = i / AUG_BLOCK, bj = j / AUG_BLOCK;
+                gs = AUG_BLOCK * AUG_BLOCK;
+                ngc = (q.nT + q.gct - 1) / q.gct;
+                pg = gpart + q.gpoff + (int64_t)(bi * (bi + 1) / 2 + bj) * ngc * gs + (i % AUG_BLOCK) * AUG_BLOCK +
+                     j % AUG_BLOCK;
+            }
             double g = 0.0;
-            for (int64_t c = 0; c < nc; ++c) g += p0[c * stride + 2 * K + 2 + e];
+            for (int64_t c = 0; c < ngc; ++c) g += pg[c * gs];
             if (!isfinite(g)) sFlag = 1;
-            o[2 * K + 2 + (int64_t)i * K + j] = g;
-            o[2 * K + 2 + (int64_t)j * K + i] = g;
+            o[2 * R + 2 + (int64_t)i * R + j] = g;
+            o[2 * R + 2 + (int64_t)j * R + i] = g;
         }
     }
     __syncthreads();
-    if (tid == 0) o[2 * K + 1] = sFlag ? 1.0 : 0.0;
+    if (tid == 0) o[2 * R + 1] = sFlag ? 1.0 : 0.0;
 }
 
-// One request of a moments launch: f (K_p values) at unit `id` — problem id, or replicate slot id when the launch is
-// weighted.
+// What the ids of a call name: problems, replicate slots (weighted requests), or problems with their appended rows.
+enum class Units { problems, slots, appended };
+
+// One request of a call: f (R_p values) at unit `id`.
 struct Ask {
     int id;
     const double* f;
@@ -466,42 +589,51 @@ struct Ask {
 };
 
 // the problem of unit `id`
-static inline int unit_problem(const mbar_b200_batch* b, bool weighted, int id) {
-    return weighted ? b->slotProb[id] : id;
+static inline int unit_problem(const mbar_b200_batch* b, Units kind, int id) {
+    return kind == Units::slots ? b->slotProb[id] : id;
 }
 
-// Sets the kernel's dynamic shared memory limit once per device and instantiation.
-template <bool W>
-static int batch_smem_attr(int device) {
-    static size_t attr[16] = {0};
-    const size_t need = BATCH_MAX_K * BATCH_SW_LD * sizeof(double);
-    if (attr[device & 15] < need) {
-        MBAR_CUDA(cudaFuncSetAttribute(batch_moments_kernel<W>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)need));
-        attr[device & 15] = need;
+// the rows of unit `id`: K_p, or K_p + M_p with the appended rows
+static inline int unit_rows(const mbar_b200_batch* b, Units kind, int id) {
+    return b->K[unit_problem(b, kind, id)] + (kind == Units::appended ? b->M[id] : 0);
+}
+
+// Sets a kernel's dynamic shared memory limit once per device.
+template <auto Kernel, size_t Bytes>
+static int smem_limit(int device) {
+    static bool done[16] = {false};
+    if (!done[device & 15]) {
+        MBAR_CUDA(cudaFuncSetAttribute(Kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)Bytes));
+        done[device & 15] = true;
     }
     return MBAR_B200_OK;
 }
 
-// Evaluate the requests in one launch of each kernel and one synchronisation; returns the packed outputs in
-// b->h_out, request r's at offsets[r] (batch_out_size(K_p, G) doubles each).  weighted: every request names a
-// replicate slot.
-static int batch_run(mbar_b200_batch* b, const std::vector<Ask>& asks, bool allRows, bool weighted,
+constexpr size_t BATCH_GRAM_SMEM = BATCH_MAX_K * BATCH_SW_LD * sizeof(double);
+
+// Evaluate the requests, all naming units of one kind, in one launch of each kernel (pass, the appended rows' Gram
+// when asked for, finalize) and one synchronisation; returns the packed outputs in b->h_out, request r's at
+// offsets[r] (batch_out_size(R_p, G) doubles each).
+static int batch_run(mbar_b200_batch* b, Units kind, const std::vector<Ask>& asks, bool allRows,
                      std::vector<int64_t>& offsets, double* msAcc) {
+    const bool weighted = kind == Units::slots, appended = kind == Units::appended;
     const int nReq = (int)asks.size();
     std::vector<BatchReq> req((size_t)nReq);
-    int64_t items = 0, parts = 0, outs = 0, fs = 0, bytes = 0;
+    int64_t items = 0, gitems = 0, parts = 0, gparts = 0, outs = 0, fs = 0, Ls = 0, bytes = 0;
     int maxKG = 0;
     offsets.resize(nReq);
     for (int r = 0; r < nReq; ++r) {
-        const int p = unit_problem(b, weighted, asks[r].id);
+        const int p = unit_problem(b, kind, asks[r].id);
         BatchReq& q = req[r];
         q.K = b->K[p];
+        q.M = appended ? b->M[p] : 0;
         q.prob = asks[r].id;
-        q.allRows = allRows ? 1 : 0;
+        q.allRows = allRows || appended ? 1 : 0;
         q.wantG = asks[r].G ? 1 : 0;
+        const int R = q.K + q.M;
         q.N = b->N[p];
         q.nT = b->nT[p];
-        q.ct = batch_chunk_tiles(q.nT, q.K);
+        q.ct = batch_chunk_tiles(q.nT, R);
         q.uoff = b->uoff[p];
         q.voff = b->voff[p];
         q.item0 = items;
@@ -510,43 +642,70 @@ static int batch_run(mbar_b200_batch* b, const std::vector<Ask>& asks, bool allR
         q.foff = fs;
         const int64_t nc = (q.nT + q.ct - 1) / q.ct;
         items += nc;
-        parts += nc * batch_part_size(q.K, q.wantG);
+        parts += nc * batch_part_size(R, q.wantG && !appended);
+        bytes += q.nT * 32 * R * 8 + (weighted ? q.nT * 32 * 2 : 0);
+        if (appended) {
+            q.aoff = b->aoff[p];
+            q.gct = aug_gram_tiles(q.nT);
+            q.gitem0 = gitems;
+            q.gpoff = gparts;
+            q.loff = Ls;
+        }
+        if (appended && q.wantG) {
+            const int nb = aug_blocks(R);
+            const int64_t ngc = (q.nT + q.gct - 1) / q.gct;
+            gitems += (int64_t)nb * (nb + 1) / 2 * ngc;
+            gparts += (int64_t)nb * (nb + 1) / 2 * ngc * AUG_BLOCK * AUG_BLOCK;
+            Ls += q.nT * 32;
+            bytes += q.nT * 32 * 8 * (int64_t)nb * R;             // every row is staged by nb block pairs
+        } else if (q.wantG) {
+            maxKG = std::max(maxKG, q.K);
+        }
         offsets[r] = outs;
-        outs += batch_out_size(q.K, q.wantG);
-        fs += q.K;
-        bytes += q.nT * 32 * q.K * 8 + (weighted ? q.nT * 32 * 2 : 0);
-        if (q.wantG) maxKG = std::max(maxKG, q.K);
+        outs += batch_out_size(R, q.wantG);
+        fs += R;
     }
-    MBAR_REQUIRE(items < INT32_MAX, MBAR_B200_ERR_INVALID, "batch: %lld chunks in one call", (long long)items);
+    MBAR_REQUIRE(items < INT32_MAX && gitems < INT32_MAX, MBAR_B200_ERR_INVALID, "batch: %lld chunks in one call",
+                 (long long)(items + gitems));
     MBAR_TRY(b->d_req.grow(nReq, "batch"));
     MBAR_TRY(b->d_f.grow(fs, "batch"));
     MBAR_TRY(b->d_part.grow(parts, "batch"));
     MBAR_TRY(b->d_out.grow(outs, "batch"));
+    if (gitems > 0) {
+        MBAR_TRY(b->d_gpart.grow(gparts, "batch"));
+        MBAR_TRY(b->d_L.grow(Ls, "batch"));
+        MBAR_TRY((smem_limit<batch_aug_gram_kernel, AUG_GRAM_SMEM>(b->device)));
+    }
     MBAR_TRY(b->h_f.grow((size_t)fs + (size_t)nReq * sizeof(BatchReq) / 8 + 1, "batch"));
     MBAR_TRY(b->h_out.grow((size_t)outs, "batch"));
-    for (int r = 0; r < nReq; ++r) std::memcpy(b->h_f + req[r].foff, asks[r].f, (size_t)req[r].K * sizeof(double));
+    for (int r = 0; r < nReq; ++r) std::memcpy(b->h_f + req[r].foff, asks[r].f,
+                                             (size_t)(req[r].K + req[r].M) * sizeof(double));
     BatchReq* hreq = reinterpret_cast<BatchReq*>(b->h_f + fs);
     std::memcpy(hreq, req.data(), req.size() * sizeof(BatchReq));
     MBAR_CUDA(cudaMemcpyAsync(b->d_f, b->h_f, (size_t)fs * sizeof(double), cudaMemcpyHostToDevice, b->stream));
     MBAR_CUDA(cudaMemcpyAsync(b->d_req, hreq, req.size() * sizeof(BatchReq), cudaMemcpyHostToDevice, b->stream));
     const size_t shBytes = (size_t)maxKG * BATCH_SW_LD * sizeof(double);
-    if (shBytes > 0) MBAR_TRY(weighted ? batch_smem_attr<true>(b->device) : batch_smem_attr<false>(b->device));
+    if (shBytes > 0)
+        MBAR_TRY((weighted ? smem_limit<batch_pass_kernel<true, false>, BATCH_GRAM_SMEM>(b->device)
+                           : smem_limit<batch_pass_kernel<false, false>, BATCH_GRAM_SMEM>(b->device)));
+    const auto pass = weighted ? batch_pass_kernel<true, false>
+                               : appended ? batch_pass_kernel<false, true> : batch_pass_kernel<false, false>;
     MBAR_CUDA(cudaEventRecord(b->ev0, b->stream));
-    if (weighted)
-        batch_moments_kernel<true><<<(unsigned)items, BATCH_THREADS, shBytes, b->stream>>>(
-            b->d_u, b->d_req, nReq, b->d_f, b->d_Nk, b->d_logNk, b->d_part, b->d_slotCoff, b->d_counts);
-    else
-        batch_moments_kernel<false><<<(unsigned)items, BATCH_THREADS, shBytes, b->stream>>>(
-            b->d_u, b->d_req, nReq, b->d_f, b->d_Nk, b->d_logNk, b->d_part, nullptr, nullptr);
-    batch_finalize_kernel<<<(unsigned)nReq, BATCH_THREADS, 0, b->stream>>>(b->d_req, b->d_part, b->d_Nk,
-                                                                           weighted ? b->d_sumxw : b->d_sumx, b->d_out);
+    pass<<<(unsigned)items, BATCH_THREADS, shBytes, b->stream>>>(b->d_u, b->d_req, nReq, b->d_f, b->d_Nk, b->d_logNk,
+                                                                 b->d_part, b->d_slotCoff, b->d_counts, b->d_ua,
+                                                                 b->d_L);
+    if (gitems > 0)
+        batch_aug_gram_kernel<<<(unsigned)gitems, BATCH_THREADS, AUG_GRAM_SMEM, b->stream>>>(
+            b->d_u, b->d_ua, b->d_req, nReq, b->d_f, b->d_Nk, b->d_logNk, b->d_L, b->d_gpart);
+    batch_finalize_kernel<<<(unsigned)nReq, BATCH_FINALIZE_THREADS, 0, b->stream>>>(
+        b->d_req, b->d_part, b->d_gpart, b->d_Nk, weighted ? b->d_sumxw : b->d_sumx, b->d_out);
     MBAR_CUDA(cudaGetLastError());
     MBAR_CUDA(cudaEventRecord(b->ev1, b->stream));
     MBAR_CUDA(cudaMemcpyAsync(b->h_out, b->d_out, (size_t)outs * sizeof(double), cudaMemcpyDeviceToHost, b->stream));
     MBAR_CUDA(cudaStreamSynchronize(b->stream));
     float e = 0.f;
     if (event_ms(b->ev0, b->ev1, &e)) *msAcc += e;
-    b->lastLaunches += 2;
+    b->lastLaunches += gitems > 0 ? 3 : 2;
     b->lastBytes += bytes;
     return MBAR_B200_OK;
 }
@@ -571,13 +730,14 @@ static int batch_solve_units(mbar_b200_batch* b, bool weighted, double* f, doubl
     b->lastBytes = 0;
     b->lastIterations = 0;
     double ms = 0.0;
+    const Units kind = weighted ? Units::slots : Units::problems;
     const int U = weighted ? b->nSlots : b->P;
     std::vector<BatchSolver> sv((size_t)U);
     std::vector<int64_t> foff((size_t)U + 1, 0);
     std::vector<int> work;                    // units still iterating, in index order
     for (int u = 0; u < U; ++u) {
         BatchSolver& s = sv[u];
-        const int p = unit_problem(b, weighted, u);
+        const int p = unit_problem(b, kind, u);
         const int K = b->K[p];
         foff[u + 1] = foff[u] + K;
         const double* Nk = b->Nk.data() + b->voff[p];
@@ -606,7 +766,7 @@ static int batch_solve_units(mbar_b200_batch* b, bool weighted, double* f, doubl
     };
     // the sums at the starting points
     for (int u : work) asks.push_back(Ask{u, sv[u].cur.data(), true});
-    if (!work.empty()) MBAR_TRY(batch_run(b, asks, false, weighted, off, &ms));
+    if (!work.empty()) MBAR_TRY(batch_run(b, kind, asks, false, off, &ms));
     {
         std::vector<int> next;
         for (size_t i = 0; i < work.size(); ++i) {
@@ -635,7 +795,7 @@ static int batch_solve_units(mbar_b200_batch* b, bool weighted, double* f, doubl
             asks.push_back(Ask{work[i], s.f_sci.data(), true});
             if (s.haveNr) asks.push_back(Ask{work[i], s.f_nr.data(), true});
         }
-        MBAR_TRY(batch_run(b, asks, false, weighted, off, &ms));
+        MBAR_TRY(batch_run(b, kind, asks, false, off, &ms));
         b->lastIterations++;
         std::vector<int> next;
         for (size_t i = 0; i < work.size(); ++i) {
@@ -672,22 +832,24 @@ static int batch_solve_units(mbar_b200_batch* b, bool weighted, double* f, doubl
     return MBAR_B200_OK;
 }
 
-// The moments of mbar_b200_batch_moments (weighted = false, ids name problems) or of
-// mbar_b200_batch_replicate_moments (ids name slots), unpacked into the caller's arrays.
-static int batch_moments_call(mbar_b200_batch* b, bool weighted, int32_t n, const int32_t* ids, const double* f,
+// The moments of mbar_b200_batch_moments (ids name problems), mbar_b200_batch_replicate_moments (ids name slots) or
+// mbar_b200_batch_augmented_moments (ids name problems with appended rows), unpacked into the caller's arrays.
+static int batch_moments_call(mbar_b200_batch* b, Units kind, int32_t n, const int32_t* ids, const double* f,
                               int32_t all_rows, double* S, double* logS, double* sumL, int32_t* flag, double* G,
                               const char* who) {
     MBAR_REQUIRE(b, MBAR_B200_ERR_INVALID, "%s: NULL object", who);
     MBAR_REQUIRE(n >= 1 && ids && f, MBAR_B200_ERR_INVALID, "%s: %d requests", who, (int)n);
-    const int U = weighted ? b->nSlots : b->P;
+    const int U = kind == Units::slots ? b->nSlots : b->P;
     std::vector<Ask> asks((size_t)n);
     int64_t fo = 0;
     for (int r = 0; r < n; ++r) {
         const int id = ids[r];
         MBAR_REQUIRE(id >= 0 && id < U, MBAR_B200_ERR_INVALID, "%s: request %d names %s %d of %d", who, r,
-                     weighted ? "slot" : "problem", id, U);
+                     kind == Units::slots ? "slot" : "problem", id, U);
+        MBAR_REQUIRE(kind != Units::appended || (id < (int)b->M.size() && b->M[id] > 0), MBAR_B200_ERR_INVALID,
+                     "%s: request %d names problem %d, which holds no appended rows", who, r, id);
         asks[r] = Ask{id, f + fo, G != nullptr};
-        fo += b->K[unit_problem(b, weighted, id)];
+        fo += unit_rows(b, kind, id);
     }
     MBAR_CUDA(cudaSetDevice(b->device));
     b->lastLaunches = 0;
@@ -695,375 +857,20 @@ static int batch_moments_call(mbar_b200_batch* b, bool weighted, int32_t n, cons
     b->lastIterations = 0;
     double ms = 0.0;
     std::vector<int64_t> off;
-    MBAR_TRY(batch_run(b, asks, all_rows != 0, weighted, off, &ms));
+    MBAR_TRY(batch_run(b, kind, asks, all_rows != 0, off, &ms));
     b->lastMs = ms;
     int64_t ko = 0, go = 0;
     for (int r = 0; r < n; ++r) {
-        const int K = b->K[unit_problem(b, weighted, asks[r].id)];
+        const int R = unit_rows(b, kind, asks[r].id);
         const double* o = b->h_out + off[r];
-        if (S) std::memcpy(S + ko, o, K * sizeof(double));
-        if (logS) std::memcpy(logS + ko, o + K, K * sizeof(double));
-        if (sumL) sumL[r] = o[2 * K];
-        if (flag) flag[r] = o[2 * K + 1] != 0.0;
-        if (G) std::memcpy(G + go, o + 2 * K + 2, (size_t)K * K * sizeof(double));
-        ko += K;
-        go += (int64_t)K * K;
+        if (S) std::memcpy(S + ko, o, R * sizeof(double));
+        if (logS) std::memcpy(logS + ko, o + R, R * sizeof(double));
+        if (sumL) sumL[r] = o[2 * R];
+        if (flag) flag[r] = o[2 * R + 1] != 0.0;
+        if (G) std::memcpy(G + go, o + 2 * R + 2, (size_t)R * R * sizeof(double));
+        ko += R;
+        go += (int64_t)R * R;
     }
-    return MBAR_B200_OK;
-}
-
-// ---- appended rows and the augmented moments (DESIGN.md 3.5g'') ---------------------------------------------------
-// Three kernels.  The pass, over (request, chunk) items with chunks of batch_chunk_tiles(nT, R) tiles, sums every
-// row as batch_moments_kernel<false> does with all rows asked for (sampled rows linearly, every other row as a running
-// (max, sum) pair) and, when the Gram is wanted, writes L'_n to a per-request scratch.  The Gram kernel takes
-// (request, pair of 32-row blocks, Gram chunk) items: it rebuilds the two blocks' weights of 128 samples at a time
-// from the tiles and L'_n, stages them in shared memory and accumulates a 2 x 4 patch of the 32 x 32 block per thread
-// with DFMA, samples in order.  The finalize kernel adds both kinds of partials in chunk order.  No atomics, and every
-// geometry is a function of (N_p, R_p) alone.
-
-// upload: one warp per appended tile, one lane per sample
-__global__ void __launch_bounds__(256) batch_aug_retile_kernel(const double* __restrict__ raw,
-                                                               const AugProbDev* __restrict__ pr, int n,
-                                                               int64_t nTiles, const double* __restrict__ x,
-                                                               double* __restrict__ ua) {
-    const int64_t tile = (int64_t)blockIdx.x * 8 + (threadIdx.x >> 5);
-    if (tile >= nTiles) return;
-    const int lane = threadIdx.x & 31;
-    int lo = 0, hi = n - 1;
-    while (lo < hi) {
-        const int mid = (lo + hi + 1) >> 1;
-        if (pr[mid].atile0 <= tile) lo = mid;
-        else hi = mid - 1;
-    }
-    const AugProbDev q = pr[lo];
-    const int64_t t = tile - q.atile0;
-    const int64_t s = t * 32 + lane;
-    const bool valid = s < q.N;
-    const double xn = x[(q.tile0 + t) * 32 + lane];
-    double* dst = ua + q.aoff + t * q.M * 32 + lane;
-    for (int m = 0; m < q.M; ++m) dst[m * 32] = valid ? raw[q.roff + (int64_t)m * q.N + s] - xn : INFINITY;
-}
-
-// the request of a pass item (gram = false) or of a Gram item (gram = true)
-__device__ __forceinline__ int aug_find(const AugReq* __restrict__ req, int nReq, int64_t item, bool gram) {
-    int lo = 0, hi = nReq - 1;
-    while (lo < hi) {
-        const int mid = (lo + hi + 1) >> 1;
-        if ((gram ? req[mid].gitem0 : req[mid].item0) <= item) lo = mid;
-        else hi = mid - 1;
-    }
-    return lo;
-}
-
-// row k of a request at tile t: resident tiles for k < K, appended tiles after
-__device__ __forceinline__ const double* aug_row(const double* __restrict__ u, const double* __restrict__ ua,
-                                                 const AugReq& q, int64_t t, int k, int lane) {
-    return k < q.K ? u + q.uoff + (t * q.K + k) * 32 + lane : ua + q.aoff + (t * q.M + (k - q.K)) * 32 + lane;
-}
-
-// per-chunk partial: R (max, sum) pairs, sum L', bad flag
-__global__ void __launch_bounds__(BATCH_THREADS) batch_aug_kernel(
-    const double* __restrict__ u, const double* __restrict__ ua, const AugReq* __restrict__ req, int nReq,
-    const double* __restrict__ fAll, const double* __restrict__ NkAll, const double* __restrict__ logNkAll,
-    double* __restrict__ part, double* __restrict__ Lbuf) {
-    __shared__ double sM[BATCH_WARPS][AUG_MAX_R], sS[BATCH_WARPS][AUG_MAX_R];
-    __shared__ double sF[AUG_MAX_R], sC[BATCH_MAX_K];
-    __shared__ int sRow[AUG_MAX_R];                              // 1 sampled, 2 every other row
-    __shared__ double sRed[BATCH_THREADS];
-    __shared__ int sBad;
-    const int64_t item = blockIdx.x;
-    const AugReq q = req[aug_find(req, nReq, item, false)];
-    const int64_t chunk = item - q.item0;
-    const int K = q.K, R = q.K + q.M;
-    const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
-    for (int k = tid; k < R; k += BATCH_THREADS) {
-        sF[k] = fAll[q.foff + k];
-        const bool s = k < K && NkAll[q.voff + k] > 0.0;
-        sRow[k] = s ? 1 : 2;
-        if (k < K) sC[k] = s ? sF[k] + logNkAll[q.voff + k] : -INFINITY;
-    }
-    for (int k = tid; k < BATCH_WARPS * AUG_MAX_R; k += BATCH_THREADS) {
-        (&sM[0][0])[k] = -INFINITY;
-        (&sS[0][0])[k] = 0.0;
-    }
-    if (tid == 0) sBad = 0;
-    __syncthreads();
-    const int64_t t0 = chunk * q.ct, t1 = min(q.nT, t0 + q.ct);
-    double sumL = 0.0;
-    bool bad = false;
-    for (int64_t t = t0 + warp; t < t1; t += BATCH_WARPS) {         // warp-uniform
-        const int64_t n = t * 32 + lane;
-        const bool valid = n < q.N;
-        const double* ut = u + q.uoff + t * (int64_t)K * 32 + lane;
-        double Lp = 0.0;
-        if (valid) {
-            double m = -INFINITY;
-            for (int k = 0; k < K; ++k)
-                if (sRow[k] == 1) m = fmax(m, sC[k] - __ldg(ut + k * 32));
-            double D = 0.0;
-            for (int k = 0; k < K; ++k)
-                if (sRow[k] == 1) D += exp(sC[k] - __ldg(ut + k * 32) - m);
-            Lp = m + log(D);
-            sumL += Lp;
-        }
-        if (q.wantG) Lbuf[q.loff + n] = Lp;
-        for (int k = 0; k < R; ++k) {
-            double a = valid ? sF[k] - __ldg(aug_row(u, ua, q, t, k, lane)) - Lp : -INFINITY;
-            if (a != a) {
-                bad = true;
-                a = -INFINITY;
-            }
-            const double wm = sRow[k] == 1 ? 0.0 : warp_max(a);
-            const double e = wm > -INFINITY ? exp(a - wm) : 0.0;
-            const double ws = warp_sum(e);
-            if (lane == 0) pair_merge(sM[warp][k], sS[warp][k], wm, ws);
-        }
-    }
-    if (bad) sBad = 1;
-    sRed[tid] = sumL;
-    __syncthreads();
-    for (int o = BATCH_THREADS / 2; o > 0; o >>= 1) {
-        if (tid < o) sRed[tid] += sRed[tid + o];
-        __syncthreads();
-    }
-    double* pc = part + q.poff + chunk * (2 * R + 2);
-    for (int k = tid; k < R; k += BATCH_THREADS) {
-        double m = sM[0][k], s = sS[0][k];
-        for (int w = 1; w < BATCH_WARPS; ++w) pair_merge(m, s, sM[w][k], sS[w][k]);
-        pc[2 * k] = m;
-        pc[2 * k + 1] = s;
-    }
-    if (tid == 0) {
-        pc[2 * R] = sRed[0];
-        pc[2 * R + 1] = sBad ? 1.0 : 0.0;
-    }
-}
-
-// one 32 x 32 block (bi, bj), bi >= bj, of Ghat over one Gram chunk: thread (ti, tj) = (tid / 8, tid % 8) owns rows
-// 2 ti, 2 ti + 1 of block bi and columns tj + 8 c (c < 4) of block bj
-__global__ void __launch_bounds__(BATCH_THREADS) batch_aug_gram_kernel(
-    const double* __restrict__ u, const double* __restrict__ ua, const AugReq* __restrict__ req, int nReq,
-    const double* __restrict__ fAll, const double* __restrict__ NkAll, const double* __restrict__ logNkAll,
-    const double* __restrict__ Lbuf, double* __restrict__ gpart) {
-    extern __shared__ __align__(16) double sAug[];               // [2][AUG_BLOCK][AUG_SW_LD] staged weights
-    __shared__ double sF[2][AUG_BLOCK], sLs[2][AUG_BLOCK];
-    const int64_t item = blockIdx.x;
-    const AugReq q = req[aug_find(req, nReq, item, true)];
-    const int R = q.K + q.M;
-    const int64_t ngc = (q.nT + q.gct - 1) / q.gct;
-    const int64_t local = item - q.gitem0;
-    const int pair = (int)(local / ngc);
-    const int64_t gc = local - (int64_t)pair * ngc;
-    int bi = (int)((sqrt(8.0 * pair + 1.0) - 1.0) * 0.5);
-    while ((bi + 1) * (bi + 2) / 2 <= pair) ++bi;
-    while (bi * (bi + 1) / 2 > pair) --bi;
-    const int bj = pair - bi * (bi + 1) / 2;
-    const int nh = bi == bj ? 1 : 2;                             // a diagonal block stages one row block
-    const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
-    if (tid < 2 * AUG_BLOCK) {
-        const int h = tid / AUG_BLOCK, i = tid % AUG_BLOCK;
-        const int k = (h ? bj : bi) * AUG_BLOCK + i;
-        const bool s = k < q.K && NkAll[q.voff + k] > 0.0;
-        sF[h][i] = k < R ? fAll[q.foff + k] : 0.0;
-        sLs[h][i] = s ? logNkAll[q.voff + k] : 0.0;
-    }
-    double* sWi = sAug;
-    double* sWj = nh == 2 ? sAug + AUG_BLOCK * AUG_SW_LD : sAug;
-    const int ti = tid >> 3, tj = tid & 7;
-    double acc[2][4];
-#pragma unroll
-    for (int e = 0; e < 2; ++e)
-#pragma unroll
-        for (int c = 0; c < 4; ++c) acc[e][c] = 0.0;
-    __syncthreads();
-    const int64_t t0 = gc * q.gct, t1 = min(q.nT, t0 + q.gct);
-    const int64_t rounds = (t1 - t0 + BATCH_WARPS - 1) / BATCH_WARPS;
-    for (int64_t r = 0; r < rounds; ++r) {
-        const int64_t t = t0 + r * BATCH_WARPS + warp;
-        const int64_t n = t * 32 + lane;
-        const bool valid = t < t1 && n < q.N;
-        const double Lp = valid ? Lbuf[q.loff + n] : 0.0;
-        for (int h = 0; h < nh; ++h) {
-            const int b = h ? bj : bi;
-            double* w = h ? sWj : sWi;
-            for (int i = 0; i < AUG_BLOCK; ++i) {
-                const int k = b * AUG_BLOCK + i;
-                double x = 0.0;
-                if (valid && k < R) x = exp(sF[h][i] - __ldg(aug_row(u, ua, q, t, k, lane)) - Lp + sLs[h][i]);
-                w[i * AUG_SW_LD + tid] = x;
-            }
-        }
-        __syncthreads();
-        const double* wa = sWi + (2 * ti) * AUG_SW_LD;
-        const double* wb = sWj + tj * AUG_SW_LD;
-#pragma unroll 4
-        for (int s = 0; s < BATCH_ROUND; ++s) {
-            const double a0 = wa[s], a1 = wa[AUG_SW_LD + s];
-#pragma unroll
-            for (int c = 0; c < 4; ++c) {
-                const double bc = wb[c * 8 * AUG_SW_LD + s];
-                acc[0][c] = fma(a0, bc, acc[0][c]);
-                acc[1][c] = fma(a1, bc, acc[1][c]);
-            }
-        }
-        __syncthreads();
-    }
-    double* pg = gpart + q.gpoff + local * (AUG_BLOCK * AUG_BLOCK);
-#pragma unroll
-    for (int e = 0; e < 2; ++e)
-#pragma unroll
-        for (int c = 0; c < 4; ++c) pg[(2 * ti + e) * AUG_BLOCK + tj + 8 * c] = acc[e][c];
-}
-
-// A request's partials in chunk order -> its packed output, with the flag rules of batch_finalize_kernel applied to
-// every row (a sampled row's S outside (1e-280, 1e300); any other row's S NaN or overflowing; a NaN in a sum; a Ghat
-// entry that is not finite).  Gram partials of block pair (bi, bj) and chunk c sit at gpoff + (pair * nGc + c) * 1024.
-__global__ void __launch_bounds__(256) batch_aug_finalize_kernel(const AugReq* __restrict__ req,
-                                                                 const double* __restrict__ part,
-                                                                 const double* __restrict__ gpart,
-                                                                 const double* __restrict__ NkAll,
-                                                                 const double* __restrict__ sumx,
-                                                                 double* __restrict__ out) {
-    __shared__ int sFlag;
-    const AugReq q = req[blockIdx.x];
-    const int K = q.K, R = q.K + q.M, tid = threadIdx.x;
-    const int64_t stride = 2 * R + 2;
-    const int64_t nc = (q.nT + q.ct - 1) / q.ct;
-    const double* p0 = part + q.poff;
-    double* o = out + q.ooff;
-    if (tid == 0) sFlag = 0;
-    __syncthreads();
-    for (int k = tid; k < R; k += blockDim.x) {
-        double m = -INFINITY, s = 0.0;
-        for (int64_t c = 0; c < nc; ++c) pair_merge(m, s, p0[c * stride + 2 * k], p0[c * stride + 2 * k + 1]);
-        const double logS = s > 0.0 ? m + log(s) : -INFINITY;
-        const double S = m == 0.0 ? s : exp(logS);
-        o[k] = S;
-        o[R + k] = logS;
-        const bool sampled = k < K && NkAll[q.voff + k] > 0.0;
-        if (sampled && !(S > 1e-280 && S < 1e300)) sFlag = 1;
-        if (!sampled && (logS != logS || !(S < INFINITY))) sFlag = 1;
-    }
-    if (tid == 0) {
-        double sl = 0.0, bad = 0.0;
-        for (int64_t c = 0; c < nc; ++c) {
-            sl += p0[c * stride + 2 * R];
-            bad = fmax(bad, p0[c * stride + 2 * R + 1]);
-        }
-        o[2 * R] = sl - sumx[q.prob];
-        if (bad > 0.0 || sl != sl) sFlag = 1;
-    }
-    if (q.wantG) {
-        const int64_t ngc = (q.nT + q.gct - 1) / q.gct;
-        const int E = R * (R + 1) / 2;
-        for (int e = tid; e < E; e += blockDim.x) {
-            int i = (int)((sqrt(8.0 * e + 1.0) - 1.0) * 0.5);
-            while ((i + 1) * (i + 2) / 2 <= e) ++i;
-            while (i * (i + 1) / 2 > e) --i;
-            const int j = e - i * (i + 1) / 2;
-            const int bi = i / AUG_BLOCK, bj = j / AUG_BLOCK;
-            const double* pg = gpart + q.gpoff + (int64_t)(bi * (bi + 1) / 2 + bj) * ngc * (AUG_BLOCK * AUG_BLOCK) +
-                               (i % AUG_BLOCK) * AUG_BLOCK + j % AUG_BLOCK;
-            double g = 0.0;
-            for (int64_t c = 0; c < ngc; ++c) g += pg[c * (AUG_BLOCK * AUG_BLOCK)];
-            if (!isfinite(g)) sFlag = 1;
-            o[2 * R + 2 + (int64_t)i * R + j] = g;
-            o[2 * R + 2 + (int64_t)j * R + i] = g;
-        }
-    }
-    __syncthreads();
-    if (tid == 0) o[2 * R + 1] = sFlag ? 1.0 : 0.0;
-}
-
-static int aug_smem_attr(int device) {
-    static bool done[16] = {false};
-    if (!done[device & 15]) {
-        MBAR_CUDA(cudaFuncSetAttribute(batch_aug_gram_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                       (int)AUG_GRAM_SMEM));
-        done[device & 15] = true;
-    }
-    return MBAR_B200_OK;
-}
-
-// The augmented requests (problem[r], f: R_p values each) in one launch of each kernel and one synchronisation;
-// request r's packed output is at b->h_out + offsets[r].
-static int batch_aug_run(mbar_b200_batch* b, int nReq, const int32_t* problem, const double* f, bool wantG,
-                         std::vector<int64_t>& offsets) {
-    std::vector<AugReq> req((size_t)nReq);
-    int64_t items = 0, gitems = 0, parts = 0, gparts = 0, outs = 0, fs = 0, Ls = 0, bytes = 0;
-    offsets.resize(nReq);
-    for (int r = 0; r < nReq; ++r) {
-        const int p = problem[r];
-        AugReq& q = req[r];
-        q.K = b->K[p];
-        q.M = b->M[p];
-        q.prob = p;
-        q.wantG = wantG ? 1 : 0;
-        const int R = q.K + q.M;
-        q.N = b->N[p];
-        q.nT = b->nT[p];
-        q.ct = batch_chunk_tiles(q.nT, R);
-        q.gct = aug_gram_tiles(q.nT);
-        q.uoff = b->uoff[p];
-        q.aoff = b->aoff[p];
-        q.voff = b->voff[p];
-        q.item0 = items;
-        q.gitem0 = gitems;
-        q.poff = parts;
-        q.gpoff = gparts;
-        q.ooff = outs;
-        q.foff = fs;
-        q.loff = Ls;
-        const int64_t nc = (q.nT + q.ct - 1) / q.ct;
-        items += nc;
-        parts += nc * (2 * R + 2);
-        bytes += q.nT * 32 * R * 8;
-        if (wantG) {
-            const int nb = aug_blocks(R);
-            const int64_t ngc = (q.nT + q.gct - 1) / q.gct;
-            gitems += (int64_t)nb * (nb + 1) / 2 * ngc;
-            gparts += (int64_t)nb * (nb + 1) / 2 * ngc * AUG_BLOCK * AUG_BLOCK;
-            Ls += q.nT * 32;
-            bytes += q.nT * 32 * 8 * (int64_t)nb * R;             // every row is staged by nb block pairs
-        }
-        offsets[r] = outs;
-        outs += aug_out_size(R, wantG);
-        fs += R;
-    }
-    MBAR_REQUIRE(items < INT32_MAX && gitems < INT32_MAX, MBAR_B200_ERR_INVALID, "batch: %lld chunks in one call",
-                 (long long)(items + gitems));
-    MBAR_TRY(b->d_areq.grow(nReq, "batch"));
-    MBAR_TRY(b->d_f.grow(fs, "batch"));
-    MBAR_TRY(b->d_part.grow(parts, "batch"));
-    MBAR_TRY(b->d_out.grow(outs, "batch"));
-    if (wantG) {
-        MBAR_TRY(b->d_gpart.grow(gparts, "batch"));
-        MBAR_TRY(b->d_L.grow(Ls, "batch"));
-        MBAR_TRY(aug_smem_attr(b->device));
-    }
-    MBAR_TRY(b->h_f.grow((size_t)fs + (size_t)nReq * sizeof(AugReq) / 8 + 1, "batch"));
-    MBAR_TRY(b->h_out.grow((size_t)outs, "batch"));
-    std::memcpy(b->h_f, f, (size_t)fs * sizeof(double));
-    AugReq* hreq = reinterpret_cast<AugReq*>(b->h_f + fs);
-    std::memcpy(hreq, req.data(), req.size() * sizeof(AugReq));
-    MBAR_CUDA(cudaMemcpyAsync(b->d_f, b->h_f, (size_t)fs * sizeof(double), cudaMemcpyHostToDevice, b->stream));
-    MBAR_CUDA(cudaMemcpyAsync(b->d_areq, hreq, req.size() * sizeof(AugReq), cudaMemcpyHostToDevice, b->stream));
-    MBAR_CUDA(cudaEventRecord(b->ev0, b->stream));
-    batch_aug_kernel<<<(unsigned)items, BATCH_THREADS, 0, b->stream>>>(b->d_u, b->d_ua, b->d_areq, nReq, b->d_f,
-                                                                      b->d_Nk, b->d_logNk, b->d_part, b->d_L);
-    if (wantG)
-        batch_aug_gram_kernel<<<(unsigned)gitems, BATCH_THREADS, AUG_GRAM_SMEM, b->stream>>>(
-            b->d_u, b->d_ua, b->d_areq, nReq, b->d_f, b->d_Nk, b->d_logNk, b->d_L, b->d_gpart);
-    batch_aug_finalize_kernel<<<(unsigned)nReq, 256, 0, b->stream>>>(b->d_areq, b->d_part, b->d_gpart, b->d_Nk,
-                                                                     b->d_sumx, b->d_out);
-    MBAR_CUDA(cudaGetLastError());
-    MBAR_CUDA(cudaEventRecord(b->ev1, b->stream));
-    MBAR_CUDA(cudaMemcpyAsync(b->h_out, b->d_out, (size_t)outs * sizeof(double), cudaMemcpyDeviceToHost, b->stream));
-    MBAR_CUDA(cudaStreamSynchronize(b->stream));
-    float e = 0.f;
-    b->lastMs = event_ms(b->ev0, b->ev1, &e) ? e : 0.0;
-    b->lastLaunches = wantG ? 3 : 2;
-    b->lastBytes = bytes;
     return MBAR_B200_OK;
 }
 
@@ -1144,7 +951,8 @@ int mbar_b200_batch_destroy(mbar_b200_batch* b) { return destroy_resident(b); }
 int mbar_b200_batch_moments(mbar_b200_batch* b, int32_t n_requests, const int32_t* problem, const double* f,
                             int32_t all_rows, double* S, double* logS, double* sumL, int32_t* flag, double* G) {
     NvtxRange nvtx_("mbar_b200::batch_moments");
-    return batch_moments_call(b, false, n_requests, problem, f, all_rows, S, logS, sumL, flag, G, "batch_moments");
+    return batch_moments_call(b, Units::problems, n_requests, problem, f, all_rows, S, logS, sumL, flag, G,
+                              "batch_moments");
 }
 
 int mbar_b200_batch_solve(mbar_b200_batch* b, double* f, double tol, int32_t maxiter, int32_t min_sc_iter,
@@ -1203,7 +1011,7 @@ int mbar_b200_batch_replicate_moments(mbar_b200_batch* b, int32_t n_requests, co
                                       int32_t all_rows, double* S, double* logS, double* sumL, int32_t* flag,
                                       double* G) {
     NvtxRange nvtx_("mbar_b200::batch_replicate_moments");
-    return batch_moments_call(b, true, n_requests, slot, f, all_rows, S, logS, sumL, flag, G,
+    return batch_moments_call(b, Units::slots, n_requests, slot, f, all_rows, S, logS, sumL, flag, G,
                               "batch_replicate_moments");
 }
 
@@ -1272,37 +1080,9 @@ int mbar_b200_batch_set_unsampled(mbar_b200_batch* b, int32_t n, const int32_t* 
 int mbar_b200_batch_augmented_moments(mbar_b200_batch* b, int32_t n_requests, const int32_t* problem,
                                       const double* f, double* S, double* logS, double* sumL, int32_t* flag,
                                       double* G) {
-    const char* who = "batch_augmented_moments";
-    MBAR_REQUIRE(b, MBAR_B200_ERR_INVALID, "%s: NULL object", who);
-    MBAR_REQUIRE(n_requests >= 1 && problem && f, MBAR_B200_ERR_INVALID, "%s: %d requests", who, (int)n_requests);
-    for (int r = 0; r < n_requests; ++r) {
-        const int p = problem[r];
-        MBAR_REQUIRE(p >= 0 && p < b->P, MBAR_B200_ERR_INVALID, "%s: request %d names problem %d of %d", who, r, p,
-                     b->P);
-        MBAR_REQUIRE(p < (int)b->M.size() && b->M[p] > 0, MBAR_B200_ERR_INVALID,
-                     "%s: request %d names problem %d, which holds no appended rows", who, r, p);
-    }
-    MBAR_CUDA(cudaSetDevice(b->device));
     NvtxRange nvtx_("mbar_b200::batch_augmented_moments");
-    b->lastLaunches = 0;
-    b->lastBytes = 0;
-    b->lastIterations = 0;
-    b->lastMs = 0.0;
-    std::vector<int64_t> off;
-    MBAR_TRY(batch_aug_run(b, n_requests, problem, f, G != nullptr, off));
-    int64_t ko = 0, go = 0;
-    for (int r = 0; r < n_requests; ++r) {
-        const int R = b->K[problem[r]] + b->M[problem[r]];
-        const double* o = b->h_out + off[r];
-        if (S) std::memcpy(S + ko, o, R * sizeof(double));
-        if (logS) std::memcpy(logS + ko, o + R, R * sizeof(double));
-        if (sumL) sumL[r] = o[2 * R];
-        if (flag) flag[r] = o[2 * R + 1] != 0.0;
-        if (G) std::memcpy(G + go, o + 2 * R + 2, (size_t)R * R * sizeof(double));
-        ko += R;
-        go += (int64_t)R * R;
-    }
-    return MBAR_B200_OK;
+    return batch_moments_call(b, Units::appended, n_requests, problem, f, 1, S, logS, sumL, flag, G,
+                              "batch_augmented_moments");
 }
 
 int mbar_b200_last_batch_stats(mbar_b200_batch* b, double* ms, int32_t* launches, int32_t* iterations,

@@ -793,23 +793,8 @@ class DeviceMbarBatch(_Resident):
             raise ValueError("need one problem or slot index per f vector, and at least one")
         owner = self.slot_problems if weighted else np.arange(self.P)
         Ks = [int(self.K[owner[i]]) if 0 <= i < len(owner) else -1 for i in ids]
-        f = np.ascontiguousarray(np.concatenate([_f64(v, K) for v, K in zip(f_list, Ks)]))
-        S, logS = np.empty(f.size), np.empty(f.size)
-        sumL = np.empty(len(Ks))
-        flag = np.empty(len(Ks), np.int32)
-        G = np.empty(sum(K * K for K in Ks)) if want_G else None
         call = self._lib.mbar_b200_batch_replicate_moments if weighted else self._lib.mbar_b200_batch_moments
-        check(call(self._h, len(Ks), _i32p(ids), _dptr(f), int(bool(all_rows)), _dptr(S), _dptr(logS), _dptr(sumL),
-                   _i32p(flag), _dptr(G) if want_G else None))
-        out, o, g = [], 0, 0
-        for r, K in enumerate(Ks):
-            d = dict(S=S[o:o + K], log_S=logS[o:o + K], sum_L=float(sumL[r]), flag=bool(flag[r]))
-            if want_G:
-                d["G"] = G[g:g + K * K].reshape(K, K)
-            out.append(d)
-            o += K
-            g += K * K
-        return out
+        return self._requests(call, ids, f_list, Ks, want_G, int(bool(all_rows)))
 
     def solve(self, f_list=None, tol=1e-12, maxiter=10000, min_sc_iter=0, gamma=1.0):
         """(f_list, status [P], iterations [P]): the adaptive solver from f_list (zeros by default) on every problem.
@@ -872,16 +857,20 @@ class DeviceMbarBatch(_Resident):
         if ids.shape != (len(f_list),) or len(f_list) == 0:
             raise ValueError("need one problem index per f vector, and at least one")
         Rs = [int(self.K[i] + self.appended[i]) if 0 <= i < self.P else -1 for i in ids]
-        f = np.ascontiguousarray(np.concatenate([_f64(v, R) for v, R in zip(f_list, Rs)]))
+        return self._requests(self._lib.mbar_b200_batch_augmented_moments, ids, f_list, Rs, want_G)
+
+    def _requests(self, call, ids, f_list, rows, want_G, *flags):
+        """One batched moments call on requests f_list[r] [rows[r]] at units ids[r], `flags` passed after f; one dict
+        per request: S, log_S, sum_L, flag and, with want_G, G [rows[r], rows[r]]."""
+        f = np.ascontiguousarray(np.concatenate([_f64(v, R) for v, R in zip(f_list, rows)]))
         S, logS = np.empty(f.size), np.empty(f.size)
-        sumL = np.empty(len(Rs))
-        flag = np.empty(len(Rs), np.int32)
-        G = np.empty(sum(R * R for R in Rs)) if want_G else None
-        check(self._lib.mbar_b200_batch_augmented_moments(self._h, len(Rs), _i32p(ids), _dptr(f), _dptr(S),
-                                                          _dptr(logS), _dptr(sumL), _i32p(flag),
-                                                          _dptr(G) if want_G else None))
+        sumL = np.empty(len(rows))
+        flag = np.empty(len(rows), np.int32)
+        G = np.empty(sum(R * R for R in rows)) if want_G else None
+        check(call(self._h, len(rows), _i32p(ids), _dptr(f), *flags, _dptr(S), _dptr(logS), _dptr(sumL), _i32p(flag),
+                   _dptr(G) if want_G else None))
         out, o, g = [], 0, 0
-        for r, R in enumerate(Rs):
+        for r, R in enumerate(rows):
             d = dict(S=S[o:o + R], log_S=logS[o:o + R], sum_L=float(sumL[r]), flag=bool(flag[r]))
             if want_G:
                 d["G"] = G[g:g + R * R].reshape(R, R)
