@@ -475,9 +475,19 @@ int mbar_b200_batch_set_unsampled(mbar_b200_batch* batch, int32_t n, const int32
 int mbar_b200_batch_augmented_moments(mbar_b200_batch* batch, int32_t n_requests, const int32_t* problem,
                                       const double* f, double* S, double* log_S, double* sum_L, int32_t* flag,
                                       double* G);
+/* mbar_b200_batch_augmented_moments with every request naming a replicate slot (slot[r]) whose problem holds
+ * appended rows, and f its R_p = K_p + M_p values: the sums of the augmented problem with sample n counted c_n times,
+ * S_k = sum_n c_n e^{f_k - u_kn - L_n}, log S_k and sum_n c_n L_n, where L_n keeps N_k, and the flag of
+ * batch_augmented_moments.  These are the values DeviceProblem.replicate_unsampled gives for the appended rows.  No
+ * Gram.  A slot out of range or whose problem holds no appended rows -> MBAR_B200_ERR_INVALID.  Two kernel launches
+ * and one synchronisation; all-ones counts give the bits of the unweighted request, a zero-count sample enters no sum
+ * and a request's results are the same bits whichever requests share the call. */
+int mbar_b200_batch_replicate_augmented_moments(mbar_b200_batch* batch, int32_t n_requests, const int32_t* slot,
+                                                const double* f, double* S, double* log_S, double* sum_L,
+                                                int32_t* flag);
 /* CUDA-event time of the kernels of the last batch_moments, batch_solve, batch_replicate_moments,
- * batch_solve_replicates or batch_augmented_moments call, its kernel launches, its iterations (solves) and the bytes
- * of u_kn tiles (appended tiles, counts) its passes read. */
+ * batch_solve_replicates, batch_augmented_moments or batch_replicate_augmented_moments call, its kernel launches, its
+ * iterations (solves) and the bytes of u_kn tiles (appended tiles, counts) its passes read. */
 int mbar_b200_last_batch_stats(mbar_b200_batch* batch, double* kernel_ms, int32_t* launches, int32_t* iterations,
                                int64_t* bytes_read);
 

@@ -58,8 +58,8 @@ __host__ __device__ __forceinline__ int64_t batch_chunk_tiles(int64_t nT, int K)
     return base > need ? base : need;
 }
 
-// One request: a problem's K rows, a replicate slot's, or a problem's K resident rows followed by its M appended
-// rows; R = K + M rows in all.
+// One request: a problem's K rows, a replicate slot's, or a problem's (or a replicate slot's) K resident rows followed
+// by the problem's M appended rows; R = K + M rows in all.
 struct BatchReq {
     int64_t uoff;     // first double of the problem's tiles
     int64_t N, nT;    // samples and tiles of the problem
@@ -274,7 +274,8 @@ __device__ __forceinline__ const double* batch_row(const double* __restrict__ u,
 // One CTA per (request, chunk) item; every request of a launch is of one kind:
 //   W: weighted requests (q.prob names a replicate slot; its counts start at slotCoff[q.prob]);
 //   APPENDED: requests with appended rows, every row asked for; with the Gram, L'_n goes to Lbuf for
-//     batch_aug_gram_kernel instead of an in-pass Gram.
+//     batch_aug_gram_kernel instead of an in-pass Gram;
+//   both: a replicate slot with its problem's appended rows, never with the Gram (DESIGN.md 3.5g''').
 template <bool W, bool APPENDED>
 __global__ void __launch_bounds__(BATCH_THREADS) batch_pass_kernel(
     const double* __restrict__ u, const BatchReq* __restrict__ req, int nReq, const double* __restrict__ fAll,
@@ -361,7 +362,7 @@ __global__ void __launch_bounds__(BATCH_THREADS) batch_pass_kernel(
             }
         }
         if (tileOn) {
-            if (APPENDED && q.wantG) Lbuf[q.loff + n] = Lp;
+            if (APPENDED && !W && q.wantG) Lbuf[q.loff + n] = Lp;      // weighted requests have no Gram
             for (int k = 0; k < R; ++k) {
                 if (sRow[k] == 0) {
                     if (G) sW[k * BATCH_SW_LD + tid] = 0.0;
@@ -578,8 +579,12 @@ __global__ void __launch_bounds__(BATCH_FINALIZE_THREADS) batch_finalize_kernel(
     if (tid == 0) o[2 * R + 1] = sFlag ? 1.0 : 0.0;
 }
 
-// What the ids of a call name: problems, replicate slots (weighted requests), or problems with their appended rows.
-enum class Units { problems, slots, appended };
+// What the ids of a call name: problems, replicate slots (weighted requests), problems with their appended rows, or
+// replicate slots with their problem's appended rows (weighted requests with appended rows).
+enum class Units { problems, slots, appended, slot_appended };
+
+static inline bool units_weighted(Units kind) { return kind == Units::slots || kind == Units::slot_appended; }
+static inline bool units_appended(Units kind) { return kind == Units::appended || kind == Units::slot_appended; }
 
 // One request of a call: f (R_p values) at unit `id`.
 struct Ask {
@@ -590,12 +595,13 @@ struct Ask {
 
 // the problem of unit `id`
 static inline int unit_problem(const mbar_b200_batch* b, Units kind, int id) {
-    return kind == Units::slots ? b->slotProb[id] : id;
+    return units_weighted(kind) ? b->slotProb[id] : id;
 }
 
 // the rows of unit `id`: K_p, or K_p + M_p with the appended rows
 static inline int unit_rows(const mbar_b200_batch* b, Units kind, int id) {
-    return b->K[unit_problem(b, kind, id)] + (kind == Units::appended ? b->M[id] : 0);
+    const int p = unit_problem(b, kind, id);
+    return b->K[p] + (units_appended(kind) ? b->M[p] : 0);
 }
 
 // Sets a kernel's dynamic shared memory limit once per device.
@@ -616,7 +622,7 @@ constexpr size_t BATCH_GRAM_SMEM = BATCH_MAX_K * BATCH_SW_LD * sizeof(double);
 // offsets[r] (batch_out_size(R_p, G) doubles each).
 static int batch_run(mbar_b200_batch* b, Units kind, const std::vector<Ask>& asks, bool allRows,
                      std::vector<int64_t>& offsets, double* msAcc) {
-    const bool weighted = kind == Units::slots, appended = kind == Units::appended;
+    const bool weighted = units_weighted(kind), appended = units_appended(kind);
     const int nReq = (int)asks.size();
     std::vector<BatchReq> req((size_t)nReq);
     int64_t items = 0, gitems = 0, parts = 0, gparts = 0, outs = 0, fs = 0, Ls = 0, bytes = 0;
@@ -688,7 +694,7 @@ static int batch_run(mbar_b200_batch* b, Units kind, const std::vector<Ask>& ask
     if (shBytes > 0)
         MBAR_TRY((weighted ? smem_limit<batch_pass_kernel<true, false>, BATCH_GRAM_SMEM>(b->device)
                            : smem_limit<batch_pass_kernel<false, false>, BATCH_GRAM_SMEM>(b->device)));
-    const auto pass = weighted ? batch_pass_kernel<true, false>
+    const auto pass = weighted ? (appended ? batch_pass_kernel<true, true> : batch_pass_kernel<true, false>)
                                : appended ? batch_pass_kernel<false, true> : batch_pass_kernel<false, false>;
     MBAR_CUDA(cudaEventRecord(b->ev0, b->stream));
     pass<<<(unsigned)items, BATCH_THREADS, shBytes, b->stream>>>(b->d_u, b->d_req, nReq, b->d_f, b->d_Nk, b->d_logNk,
@@ -832,22 +838,26 @@ static int batch_solve_units(mbar_b200_batch* b, bool weighted, double* f, doubl
     return MBAR_B200_OK;
 }
 
-// The moments of mbar_b200_batch_moments (ids name problems), mbar_b200_batch_replicate_moments (ids name slots) or
-// mbar_b200_batch_augmented_moments (ids name problems with appended rows), unpacked into the caller's arrays.
+// The moments of mbar_b200_batch_moments (ids name problems), mbar_b200_batch_replicate_moments (ids name slots),
+// mbar_b200_batch_augmented_moments (ids name problems with appended rows) or
+// mbar_b200_batch_replicate_augmented_moments (ids name slots whose problems hold appended rows), unpacked into the
+// caller's arrays.
 static int batch_moments_call(mbar_b200_batch* b, Units kind, int32_t n, const int32_t* ids, const double* f,
                               int32_t all_rows, double* S, double* logS, double* sumL, int32_t* flag, double* G,
                               const char* who) {
     MBAR_REQUIRE(b, MBAR_B200_ERR_INVALID, "%s: NULL object", who);
     MBAR_REQUIRE(n >= 1 && ids && f, MBAR_B200_ERR_INVALID, "%s: %d requests", who, (int)n);
-    const int U = kind == Units::slots ? b->nSlots : b->P;
+    const int U = units_weighted(kind) ? b->nSlots : b->P;
     std::vector<Ask> asks((size_t)n);
     int64_t fo = 0;
     for (int r = 0; r < n; ++r) {
         const int id = ids[r];
         MBAR_REQUIRE(id >= 0 && id < U, MBAR_B200_ERR_INVALID, "%s: request %d names %s %d of %d", who, r,
-                     kind == Units::slots ? "slot" : "problem", id, U);
-        MBAR_REQUIRE(kind != Units::appended || (id < (int)b->M.size() && b->M[id] > 0), MBAR_B200_ERR_INVALID,
-                     "%s: request %d names problem %d, which holds no appended rows", who, r, id);
+                     units_weighted(kind) ? "slot" : "problem", id, U);
+        const int p = unit_problem(b, kind, id);
+        MBAR_REQUIRE(!units_appended(kind) || (p < (int)b->M.size() && b->M[p] > 0), MBAR_B200_ERR_INVALID,
+                     "%s: request %d names %s %d of problem %d, which holds no appended rows", who, r,
+                     units_weighted(kind) ? "slot" : "problem", id, p);
         asks[r] = Ask{id, f + fo, G != nullptr};
         fo += unit_rows(b, kind, id);
     }
@@ -1083,6 +1093,14 @@ int mbar_b200_batch_augmented_moments(mbar_b200_batch* b, int32_t n_requests, co
     NvtxRange nvtx_("mbar_b200::batch_augmented_moments");
     return batch_moments_call(b, Units::appended, n_requests, problem, f, 1, S, logS, sumL, flag, G,
                               "batch_augmented_moments");
+}
+
+int mbar_b200_batch_replicate_augmented_moments(mbar_b200_batch* b, int32_t n_requests, const int32_t* slot,
+                                                const double* f, double* S, double* logS, double* sumL,
+                                                int32_t* flag) {
+    NvtxRange nvtx_("mbar_b200::batch_replicate_augmented_moments");
+    return batch_moments_call(b, Units::slot_appended, n_requests, slot, f, 1, S, logS, sumL, flag, nullptr,
+                              "batch_replicate_augmented_moments");
 }
 
 int mbar_b200_last_batch_stats(mbar_b200_batch* b, double* ms, int32_t* launches, int32_t* iterations,

@@ -146,12 +146,23 @@ def expectations_inner(u_kn, N_k, f_k, A_n, u_ln, state_map, uncertainty_method=
 
     out = finish(plan, f_aug, G, N_aug, uncertainty_method=uncertainty_method, return_theta=return_theta)
     if replicates is not None:
-        rows_l, rows_s, shift = plan["rows_l"], plan["rows_s"], plan["shift"]
-        fb = boot["f"]
-        obs_b = np.exp(fb[:, rows_l] - fb[:, rows_s]) + shift if len(rows_s) else np.zeros((len(fb), 0))
-        out["bootstrapped_observables"] = obs_b                                             # mbar.py:963-967
-        out["bootstrapped_f"] = fb[:, rows_l]
+        out.update(bootstrap_keys(plan, boot["f"]))
     return out
+
+
+def bootstrap_keys(plan, F_aug):
+    """'bootstrapped_observables' [B, S] and 'bootstrapped_f' [B, len(state_list)] of expectations_inner from every
+    replicate's augmented free energies F_aug [B, K + E] (mbar.py:962-971)."""
+    rows_l, rows_s, shift = plan["rows_l"], plan["rows_s"], plan["shift"]
+    obs_b = np.exp(F_aug[:, rows_l] - F_aug[:, rows_s]) + shift if len(rows_s) else np.zeros((len(F_aug), 0))
+    return {"bootstrapped_observables": obs_b, "bootstrapped_f": F_aug[:, rows_l]}
+
+
+def std_of_differences(X):
+    """The standard deviation over replicates b of X_b - X_b^T, [i, j] = X_bj - X_bi, for X [B, K]: the bootstrap
+    uncertainty of a difference matrix (mbar.py:706-714, :1298-1303, :1623-1643)."""
+    X = np.asarray(X)
+    return np.std(X[:, None, :] - X[:, :, None], axis=0)
 
 
 def expectation_state_map(Ks, state_dependent):
@@ -162,22 +173,29 @@ def expectation_state_map(Ks, state_dependent):
     return state_map
 
 
-def expectations_result(inner, Ks, output, compute_uncertainty, return_theta, warning_cutoff):
-    """compute_expectations' result from expectations_inner's (mbar.py:1274-1312)."""
+def expectations_result(inner, Ks, output, compute_uncertainty, return_theta, warning_cutoff,
+                        uncertainty_method=None):
+    """compute_expectations' result from expectations_inner's (mbar.py:1274-1312).  uncertainty_method="bootstrap":
+    sigma from inner's 'bootstrapped_observables', and Theta (return_theta) is still the b = 0 one."""
     out = {}
-    if compute_uncertainty or return_theta:
+    boot = uncertainty_method == "bootstrap"
+    if (compute_uncertainty and not boot) or return_theta:
         diag = np.ones(2 * Ks)
         diag[:Ks] = diag[Ks:] = inner["observables"] - inner["Amin"]
         Theta = np.diag(diag) @ inner["Theta"] @ np.diag(diag)
         covA = Theta[:Ks, :Ks] + Theta[Ks:, Ks:] - Theta[:Ks, Ks:] - Theta[Ks:, :Ks]
     if output == "averages":
         out["mu"] = inner["observables"]
-        if compute_uncertainty:
+        if compute_uncertainty and boot:
+            out["sigma"] = np.std(inner["bootstrapped_observables"], axis=0)
+        elif compute_uncertainty:
             out["sigma"] = np.sqrt(covA.diagonal())
     elif output == "differences":
         A = inner["observables"]
         out["mu"] = A - np.vstack(A)
-        if compute_uncertainty:
+        if compute_uncertainty and boot:
+            out["sigma"] = std_of_differences(inner["bootstrapped_observables"])
+        elif compute_uncertainty:
             out["sigma"] = est.error_of_differences(covA, warning_cutoff=warning_cutoff)
     else:
         raise ParameterError(f"output={output!r} must be 'averages' or 'differences'")
@@ -186,19 +204,38 @@ def expectations_result(inner, Ks, output, compute_uncertainty, return_theta, wa
     return out
 
 
-def perturbed_result(inner, compute_uncertainty, warning_cutoff):
-    """compute_perturbed_free_energies' result from expectations_inner's (mbar.py:1505-1521)."""
+def perturbed_result(inner, compute_uncertainty, warning_cutoff, uncertainty_method=None):
+    """compute_perturbed_free_energies' result from expectations_inner's (mbar.py:1505-1521).  uncertainty_method=
+    "bootstrap": dDelta_f is the standard deviation over replicates of inner's 'bootstrapped_f', a vector [L] as the
+    reference returns it, not the [L, L] matrix of the analytic methods."""
     f = inner["f"]
     out = {"Delta_f": f - np.vstack(f)}
-    if compute_uncertainty:
+    if compute_uncertainty and uncertainty_method == "bootstrap":
+        out["dDelta_f"] = np.std(inner["bootstrapped_f"], axis=0)
+    elif compute_uncertainty:
         out["dDelta_f"] = est.error_of_differences(inner["Theta"], warning_cutoff=warning_cutoff)
     return out
 
 
-def entropy_enthalpy_result(inner, K, warning_cutoff=1.0e-10):
-    """compute_entropy_and_enthalpy's result (mbar.py:1600-1681, analytic uncertainties) from expectations_inner's
-    with A_n = u_ln = u_kn and the state map (k, k): the reference's 3K x 3K Theta, whose last K rows and columns
-    repeat the states' block, scaled by the observables."""
+def entropy_enthalpy_result(inner, K, warning_cutoff=1.0e-10, f_k_boots=None):
+    """compute_entropy_and_enthalpy's result (mbar.py:1600-1681) from expectations_inner's with A_n = u_ln = u_kn and
+    the state map (k, k).  Analytic uncertainties: the reference's 3K x 3K Theta, whose last K rows and columns
+    repeat the states' block, scaled by the observables.  Bootstrap (f_k_boots [B, K], the problem's replicates): the
+    reference's branch of :1623-1643, dDelta_f from f_k_boots, dDelta_u from inner's 'bootstrapped_observables' and
+    dDelta_s from their difference; inner needs no Theta."""
+    out = {}
+    f_k = inner["f"]
+    out["Delta_f"] = f_k - np.vstack(f_k)
+    u_k = inner["observables"]
+    out["Delta_u"] = u_k - np.vstack(u_k)
+    s_k = u_k - f_k
+    out["Delta_s"] = s_k - np.vstack(s_k)
+    if f_k_boots is not None:
+        u_b = inner["bootstrapped_observables"]
+        out["dDelta_f"] = std_of_differences(f_k_boots)
+        out["dDelta_u"] = std_of_differences(u_b)
+        out["dDelta_s"] = std_of_differences(u_b - f_k_boots)
+        return out
     Theta = np.zeros([3 * K, 3 * K], dtype=np.float64)
     Theta[0:2 * K, 0:2 * K] = inner["Theta"]
     Theta[2 * K:3 * K, :] = Theta[K:2 * K, :]
@@ -208,13 +245,6 @@ def entropy_enthalpy_result(inner, K, warning_cutoff=1.0e-10):
     Adiag = np.zeros([3 * K, 3 * K], dtype=np.float64)
     np.fill_diagonal(Adiag, diag)
     Theta = Adiag @ Theta @ Adiag
-    out = {}
-    f_k = inner["f"]
-    out["Delta_f"] = f_k - np.vstack(f_k)
-    u_k = inner["observables"]
-    out["Delta_u"] = u_k - np.vstack(u_k)
-    s_k = u_k - f_k
-    out["Delta_s"] = s_k - np.vstack(s_k)
     covf = Theta[2 * K:3 * K, 2 * K:3 * K]
     out["dDelta_f"] = est.error_of_differences(covf, warning_cutoff=warning_cutoff)
     covu = Theta[0:K, 0:K] + Theta[K:2 * K, K:2 * K] - Theta[0:K, K:2 * K] - Theta[K:2 * K, 0:K]

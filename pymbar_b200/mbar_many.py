@@ -31,12 +31,15 @@ path.
 
 `MbarMany` is the same solve kept resident: its estimators (expectations, perturbed free energies, entropy and
 enthalpy, overlap, effective sample numbers) append each problem's extra rows to the batch it already holds and
-evaluate every problem in one augmented moments pass (DESIGN.md 3.5g'').  `mbar_many` is `MbarMany(...).results`.
+evaluate every problem in one augmented moments pass (DESIGN.md 3.5g''), and with n_bootstraps > 0 every replicate of
+every problem in one weighted augmented pass for uncertainty_method="bootstrap" (DESIGN.md 3.5g''').  `mbar_many` is
+`MbarMany(...).results`.
 """
 from __future__ import annotations
 
 import contextlib
 import numbers
+import time
 
 import numpy as np
 
@@ -55,7 +58,7 @@ DEFAULT_OPTIONS = dict(min_sc_iter=0, gamma=1.0, maxiter=10000)
 BOOT_WAVE_BYTES = 2 << 30   # device footprint of one wave of replicate slots
 MAX_BATCH_ROWS = 192        # DeviceMbarBatch.MAX_ROWS: K_p plus appended rows of a batched estimator request
 AUG_WAVE_BYTES = 2 << 30    # device footprint of one wave of appended rows
-ESTIMATOR_METHODS = (None, "svd-ew", "approximate")
+ESTIMATOR_METHODS = (None, "svd-ew", "approximate", "bootstrap")
 
 
 def _classes():
@@ -111,8 +114,7 @@ def _result(f, G, N_k, path, iterations, success, compute_uncertainty, uncertain
 
 def _bootstrap_std(f_k_boots):
     """dDelta_f of mbar.py:706-714: the standard deviation over replicates of f_b - f_b^T."""
-    f = np.asarray(f_k_boots)
-    return np.std(f[:, None, :] - f[:, :, None], axis=0)
+    return ex.std_of_differences(f_k_boots)
 
 
 def _chunk_tiles(nT, K):
@@ -142,6 +144,16 @@ def augmented_bytes(K, N, M):
     return 8 * (nT * 32 * (M + 1) + nc * (2 * R + 2) + nb * (nb + 1) // 2 * ngc * 1024 + 2 * R + 2 + R * R + R)
 
 
+def boot_augmented_bytes(K, N, M):
+    """Device bytes of one weighted appended slot in a wave: its counts, the pass partials and packed output of its
+    request (no Gram) and its f (batch.cu's geometry).  The appended tiles are its problem's, counted by
+    augmented_bytes."""
+    nT = -(-int(N) // 32)
+    R = int(K) + int(M)
+    nc = -(-nT // _chunk_tiles(nT, R))
+    return 2 * nT * 32 + 8 * (nc * (2 * R + 2) + 2 * R + 2 + R)
+
+
 def _validate_boot(n_bootstraps, rseed, P):
     if isinstance(n_bootstraps, bool) or not isinstance(n_bootstraps, numbers.Integral) or n_bootstraps < 0:
         raise ParameterError(f"n_bootstraps must be a non-negative int, got {n_bootstraps!r}")
@@ -163,7 +175,7 @@ class _Draws:
 
     def __init__(self, N_k, seed):
         self.N_k = np.asarray(N_k).astype(np.int64)
-        N = int(self.N_k.sum())
+        N = self.N = int(self.N_k.sum())
         self.members = bootstrap.state_members(self.N_k, bootstrap.default_x_kindices(self.N_k))
         self.rng = np.random.default_rng(seed)
         self.rng.choice(np.arange(N), min(50, N))
@@ -177,6 +189,11 @@ class _Draws:
     def rints(self, b):
         return bootstrap.replicate_rints(self.rng, self.states[b], self.N_k, self.members)
 
+    def counts(self, b):
+        """Replicate b's multiplicities [N] as uint16, regenerated from its generator state (they fit: problems whose
+        draws overflow are kept out)."""
+        return np.bincount(self.rints(b), minlength=self.N).astype(np.uint16)
+
 
 def _single_replicates(u_kn, N_k, f_k, rints, protocol):
     """f_k_boots rows of the replicates `rints` on one DeviceProblem, uploaded once."""
@@ -187,7 +204,9 @@ def _single_replicates(u_kn, N_k, f_k, rints, protocol):
 
 
 def _bootstraps(dev, batch, probs, f_main, seeds, B, tol, opts):
-    """(f_k_boots [P][B, K], boot_single [P]) of every problem; dev holds the problems `batch` (None if none)."""
+    """(f_k_boots [P][B, K], boot_single [P], draws [P], overflow) of every problem; dev holds the problems `batch`
+    (None if none).  draws[p] keeps the generator state before each of problem p's replicates; overflow is the set of
+    problems whose multiplicities overflow uint16."""
     P = len(probs)
     draws = [_Draws(probs[p][1], seeds[p]) for p in range(P)]
     boots = [np.zeros((B, probs[p][0].shape[0])) for p in range(P)]
@@ -196,7 +215,8 @@ def _bootstraps(dev, batch, probs, f_main, seeds, B, tol, opts):
     slot_of = {p: i for i, p in enumerate(batch)}
     for p in range(P):
         if p not in slot_of:
-            draws[p].next(B)                    # the generator states of every replicate
+            if draws[p].next(B) is None:        # the generator states of every replicate
+                overflow.add(p)
             single[p] = set(range(B))
     # waves of (problem, replicate) pairs in problem-major order, each under BOOT_WAVE_BYTES on the device
     pairs = [(p, b) for p in batch for b in range(B)]
@@ -252,7 +272,7 @@ def _bootstraps(dev, batch, probs, f_main, seeds, B, tol, opts):
             rints = np.array([draws[p].rints(b) for b in picked])
             u, N_k, _ = probs[p]
             boots[p][picked] = _single_replicates(u, N_k, f_main[p], rints, protocol)
-    return boots, [len(s) for s in single]
+    return boots, [len(s) for s in single], draws, overflow
 
 
 def _single(u_kn, N_k, f_k, tol, want_G):
@@ -279,14 +299,21 @@ class MbarMany:
     Each estimator takes one entry per problem, or None to skip a problem, and returns one dict per problem (None for
     a skipped one) with the keys of the pymbar.MBAR method of the same name and `path`, "batch" or "single".  Every
     request is validated before any device work; an invalid one raises ParameterError for the lowest failing index.
-    Analytic uncertainties only: uncertainty_method is None, "svd-ew" or "approximate".
+    uncertainty_method is None, "svd-ew", "approximate" or, with n_bootstraps > 0 at construction, "bootstrap"
+    (compute_expectations, compute_perturbed_free_energies, compute_entropy_and_enthalpy; DESIGN.md 3.5g''').
 
     The appended rows of expectations.augmentation go on top of the resident problems in waves whose device footprint
     stays under AUG_WAVE_BYTES; a problem's result is the same bits in any wave.  Each wave takes one
     augmented_moments call at (f_k, 0), whose log S gives the appended rows' f = -log S (the self-consistent update
     of the single path), and, when a Theta is needed, one at the full f with the Gram.  A problem takes the single
     path (expectations.expectations_inner on a DeviceProblem of it) when it took the single path in the solve, when
-    K_p plus its appended rows exceed MAX_BATCH_ROWS, or when either call flags it."""
+    K_p plus its appended rows exceed MAX_BATCH_ROWS, or when either call flags it.
+
+    Under bootstrap, every replicate b of a batched problem is a replicate slot with the problem's appended rows,
+    asked at f = [f_k_boots[b], 0 ...] in sub-waves under BOOT_WAVE_BYTES, one weighted augmented_moments call each;
+    the counts are regenerated from the construction's draws.  A flagged replicate sends its problem to the single
+    path, expectations_inner(..., replicates=(f_k_boots, counts)).  A problem whose multiplicities overflow uint16
+    raises ParameterError."""
 
     def __init__(self, u_kn_list, N_k_list, f_k_init=None, compute_uncertainty=True, uncertainty_method=None,
                  return_theta=False, solver_tolerance=1.0e-12, options=None, n_bootstraps=0, rseed=None):
@@ -313,7 +340,11 @@ class MbarMany:
         self._dev = None
         self._slot = {}              # problem -> its index in the device batch
         self._G = {}                 # problem -> W^T W at its final f, where the solve computed it
-        self.device_stats = dict(ms=0.0, launches=0, calls=0)
+        self._B = B
+        self._draws = []             # problem -> its _Draws (n_bootstraps > 0): replicate counts are regenerated
+        self._overflow = set()       # problems whose replicate multiplicities overflow uint16
+        self.device_stats = dict(ms=0.0, launches=0, calls=0, bytes_read=0)
+        self.host_stats = dict(counts_s=0.0)     # host time spent regenerating replicate counts for the estimators
         try:
             self.results = self._solve(probs, seeds, B, compute_uncertainty, uncertainty_method, return_theta,
                                        solver_tolerance, opts)
@@ -386,8 +417,8 @@ class MbarMany:
             results[p] = _result(f, G, N_k, "single", None, success, compute_uncertainty, uncertainty_method,
                                  return_theta)
         if B > 0:
-            boots, nsingle = _bootstraps(dev, batch, probs, [r["f_k"] for r in results], seeds, B, solver_tolerance,
-                                         opts)
+            boots, nsingle, self._draws, self._overflow = _bootstraps(dev, batch, probs, [r["f_k"] for r in results],
+                                                                      seeds, B, solver_tolerance, opts)
             for r, fb, ns in zip(results, boots, nsingle):
                 r["f_k_boots"] = fb
                 r["boot_single"] = ns
@@ -418,8 +449,15 @@ class MbarMany:
 
     def _inner_many(self, requests, uncertainty_method, return_theta):
         """expectations_inner of every request (requests[p] = (A_n, u_ln, state_map) or None): ([inner or None] per
-        problem, [path or None] per problem)."""
+        problem, [path or None] per problem).  uncertainty_method="bootstrap" adds every replicate's keys
+        ('bootstrapped_observables', 'bootstrapped_f')."""
         P = len(self._probs)
+        boot = uncertainty_method == "bootstrap"
+        if boot:
+            for p, req in enumerate(requests):
+                if req is not None and p in self._overflow:
+                    raise ParameterError(f"problem {p}: a bootstrap multiplicity exceeds 65535, so its replicates "
+                                         f"cannot be evaluated")
         plans = {p: ex.augmentation(self._probs[p][0].shape[0], *req) for p, req in enumerate(requests)
                  if req is not None}
         batched, single = [], []
@@ -443,21 +481,34 @@ class MbarMany:
             single += self._wave(wave, plans, uncertainty_method, return_theta, inner, path)
         if batched:
             self._dev.set_unsampled([], [])
+            if boot:
+                self._dev.set_replicates([], [])
         _, Prob = _classes()
         for p in sorted(single):
             u, N_k, _ = self._probs[p]
+            reps = None
+            if boot:
+                reps = (self.results[p]["f_k_boots"], self._replicate_counts([(p, b) for b in range(self._B)]))
             with Prob(u, N_k, device=ms._DEVICE) as q:
                 inner[p] = ex.expectations_inner(u, N_k, self.results[p]["f_k"], *requests[p],
                                                  uncertainty_method=uncertainty_method, return_theta=return_theta,
-                                                 problem=q)
+                                                 problem=q, replicates=reps)
             path[p] = "single"
         return inner, path
+
+    def _replicate_counts(self, pairs):
+        """The multiplicities [len(pairs), N] uint16 of the replicates (problem, b), regenerated from the draws."""
+        t0 = time.perf_counter()
+        out = [self._draws[p].counts(b) for p, b in pairs]
+        self.host_stats["counts_s"] += time.perf_counter() - t0
+        return out
 
     def _count(self):
         s = self._dev.last_stats()
         self.device_stats["ms"] += s["ms"]
         self.device_stats["launches"] += s["launches"]
         self.device_stats["calls"] += 1
+        self.device_stats["bytes_read"] += s["bytes_read"]
 
     def _wave(self, wave, plans, uncertainty_method, return_theta, inner, path):
         """One wave of batched problems: fills inner and path, returns the problems the device flagged."""
@@ -486,28 +537,79 @@ class MbarMany:
                     flagged.append(p)
                     continue
                 G[p] = _gram_to_G(m["G"], self._N_aug(p, plans[p]))
+        ok = [p for p in ok if not return_theta or p in G]
+        F_aug = {}
+        if ok and uncertainty_method == "bootstrap":
+            F_aug = self._replicate_waves(ok, plans, f_aug)
+            flagged += [p for p in ok if p not in F_aug]
+            ok = [p for p in ok if p in F_aug]
         for p in ok:
-            if return_theta and p not in G:
-                continue
             inner[p] = ex.finish(plans[p], f_aug[p], G.get(p), self._N_aug(p, plans[p]),
                                  uncertainty_method=uncertainty_method, return_theta=return_theta)
+            if p in F_aug:
+                inner[p].update(ex.bootstrap_keys(plans[p], F_aug[p]))
             path[p] = "batch"
         return flagged
+
+    def _replicate_waves(self, wave, plans, f_aug):
+        """Every replicate b of every problem p of `wave` (whose appended rows are resident) as a replicate slot at
+        f = [f_k_boots[p][b], 0 ...], in sub-waves under BOOT_WAVE_BYTES, one weighted augmented_moments call each:
+        {p: F_aug [B, R_p]} with F_aug[b, K:] = -log S[K:], for the problems none of whose replicates is flagged."""
+        dev, B = self._dev, self._B
+        F_aug = {}
+        for p in wave:
+            F_aug[p] = np.zeros((B, len(f_aug[p])))
+            F_aug[p][:, :self._probs[p][0].shape[0]] = self.results[p]["f_k_boots"]
+        bad = set()
+        pairs = [(p, b) for p in wave for b in range(B)]
+        i = 0
+        while i < len(pairs):
+            sub, used = [], 0
+            while i < len(pairs):
+                p = pairs[i][0]
+                need = boot_augmented_bytes(*self._probs[p][0].shape, plans[p]["extra"].shape[0])
+                if sub and used + need > BOOT_WAVE_BYTES:
+                    break
+                sub.append(pairs[i])
+                used += need
+                i += 1
+            dev.set_replicates([self._slot[p] for p, _ in sub], self._replicate_counts(sub))
+            f0 = [F_aug[p][b].copy() for p, b in sub]
+            sums = dev.augmented_moments(f0, slots=list(range(len(sub))))
+            self._count()
+            for (p, b), f, m in zip(sub, f0, sums):
+                if m["flag"]:
+                    bad.add(p)
+                    continue
+                K = self._probs[p][0].shape[0]
+                F_aug[p][b, K:] = (f - m["log_S"])[K:]      # appended rows: the replicate's update from f = 0
+        return {p: F for p, F in F_aug.items() if p not in bad}
 
     def _N_aug(self, p, plan):
         return np.concatenate([np.asarray(self._probs[p][1], dtype=np.float64), np.zeros(plan["extra"].shape[0])])
 
-    @staticmethod
-    def _method(uncertainty_method):
+    def _method(self, uncertainty_method):
         if uncertainty_method not in ESTIMATOR_METHODS:
             raise ParameterError(f"uncertainty_method {uncertainty_method!r} is not served by MbarMany's estimators "
-                                 f"(one of {ESTIMATOR_METHODS}); bootstrap and 'svd' uncertainties are not served here")
+                                 f"(one of {ESTIMATOR_METHODS}); 'svd' uncertainties are not served here")
+        if uncertainty_method == "bootstrap" and self._B <= 0:
+            raise ParameterError("Cannot request bootstrap sampling of expectations without any bootstraps.")
+        return uncertainty_method == "bootstrap"
+
+    @staticmethod
+    def _with_boot(out, inner, keys):
+        """out plus inner's bootstrap keys among `keys` (nothing without bootstrap)."""
+        return dict(out, **{k: inner[k] for k in keys if k in inner})
 
     def compute_perturbed_free_energies(self, u_ln_list, compute_uncertainty=True, uncertainty_method=None,
                                         warning_cutoff=1.0e-10):
         """Delta_f, dDelta_f (compute_uncertainty) of the states u_ln_list[p] [L, N_p] of each problem
-        (MBAR.compute_perturbed_free_energies)."""
-        self._method(uncertainty_method)
+        (MBAR.compute_perturbed_free_energies).
+
+        uncertainty_method="bootstrap" (n_bootstraps > 0 at construction): dDelta_f is the standard deviation over
+        replicates of the perturbed free energies, a vector [L] as the reference returns it, not the [L, L] matrix of
+        the analytic methods, and each dict adds bootstrapped_f [B, L]."""
+        boot = self._method(uncertainty_method)
         reqs = []
         for p, u_ln in enumerate(self._entries(u_ln_list, "u_ln_list")):
             if u_ln is None:
@@ -515,8 +617,10 @@ class MbarMany:
                 continue
             u_ln = self._rows(p, u_ln, "u_ln")
             reqs.append((np.array([0.0]), u_ln, np.arange(u_ln.shape[0])))
-        inner, path = self._inner_many(reqs, uncertainty_method, bool(compute_uncertainty))
-        return [None if r is None else dict(ex.perturbed_result(r, compute_uncertainty, warning_cutoff), path=w)
+        inner, path = self._inner_many(reqs, uncertainty_method, bool(compute_uncertainty) and not boot)
+        return [None if r is None else
+                dict(self._with_boot(ex.perturbed_result(r, compute_uncertainty, warning_cutoff, uncertainty_method),
+                                     r, ("bootstrapped_f",)), path=w)
                 for r, w in zip(inner, path)]
 
     def compute_expectations(self, A_n_list, u_ln_list=None, output="averages", state_dependent=False,
@@ -524,8 +628,13 @@ class MbarMany:
                              return_theta=False):
         """mu, sigma (compute_uncertainty) and Theta (return_theta) of the observables A_n_list[p] ([N_p], or [L, N_p]
         when state_dependent) at the states u_ln_list[p] [L, N_p] (the problem's own states when None)
-        (MBAR.compute_expectations)."""
-        self._method(uncertainty_method)
+        (MBAR.compute_expectations).
+
+        uncertainty_method="bootstrap" (n_bootstraps > 0 at construction): sigma is the standard deviation over
+        replicates of the observables ("averages") or of their differences A_b - A_b^T ("differences"), Theta is the
+        "svd-ew" one of the problem's own samples, and each dict adds bootstrapped_observables [B, L] and
+        bootstrapped_f [B, L]."""
+        boot = self._method(uncertainty_method)
         if output not in ("averages", "differences"):
             raise ParameterError(f"output={output!r} must be 'averages' or 'differences'")
         u_lns = self._entries(u_ln_list, "u_ln_list")
@@ -542,16 +651,25 @@ class MbarMany:
                                      f"(state_dependent={state_dependent})")
             reqs.append((A, u, ex.expectation_state_map(u.shape[0], state_dependent)))
             Ks.append(u.shape[0])
-        inner, path = self._inner_many(reqs, uncertainty_method, bool(compute_uncertainty or return_theta))
-        return [None if r is None else dict(ex.expectations_result(r, Ks[p], output, compute_uncertainty,
-                                                                   return_theta, warning_cutoff), path=path[p])
+        theta = bool(return_theta or (compute_uncertainty and not boot))
+        inner, path = self._inner_many(reqs, uncertainty_method, theta)
+        keys = ("bootstrapped_observables", "bootstrapped_f")
+        return [None if r is None else
+                dict(self._with_boot(ex.expectations_result(r, Ks[p], output, compute_uncertainty, return_theta,
+                                                            warning_cutoff, uncertainty_method), r, keys),
+                     path=path[p])
                 for p, r in enumerate(inner)]
 
     def compute_entropy_and_enthalpy(self, u_ln_list=None, uncertainty_method=None, warning_cutoff=1.0e-10):
         """Delta_f, dDelta_f, Delta_u, dDelta_u, Delta_s, dDelta_s of each problem at the states u_ln_list[p]
         [L, N_p] (every problem at its own states when u_ln_list is None; an entry None skips its problem)
-        (MBAR.compute_entropy_and_enthalpy).  A problem's augmented rows number 3L; up to L = 64 they stay batched."""
-        self._method(uncertainty_method)
+        (MBAR.compute_entropy_and_enthalpy).  A problem's augmented rows number 3L; up to L = 64 they stay batched.
+
+        uncertainty_method="bootstrap" (n_bootstraps > 0 at construction) follows the reference: dDelta_f from the
+        problem's f_k_boots, dDelta_u from the bootstrapped observables and dDelta_s from their difference, and each
+        dict adds bootstrapped_observables [B, L] and bootstrapped_f [B, L].  The reference pairs the bootstrapped
+        observables with f_k_boots [B, K_p], so u_ln with L != K_p raises ParameterError."""
+        boot = self._method(uncertainty_method)
         own = u_ln_list is None
         u_lns = [None] * len(self._probs) if own else self._entries(u_ln_list, "u_ln_list")
         reqs, Ls = [], []
@@ -562,11 +680,18 @@ class MbarMany:
                 continue
             u = self._probs[p][0] if own else self._rows(p, u_ln, "u_ln")
             L = u.shape[0]
+            if boot and L != self._probs[p][0].shape[0]:
+                raise ParameterError(f"problem {p}: bootstrap entropies and enthalpies pair u_ln's {L} states with the "
+                                     f"problem's {self._probs[p][0].shape[0]} bootstrapped free energies")
             state_map = np.array([np.arange(L), np.arange(L)])
             reqs.append((u, u, state_map))
             Ls.append(L)
-        inner, path = self._inner_many(reqs, uncertainty_method, True)
-        return [None if r is None else dict(ex.entropy_enthalpy_result(r, Ls[p], warning_cutoff), path=path[p])
+        inner, path = self._inner_many(reqs, uncertainty_method, not boot)
+        keys = ("bootstrapped_observables", "bootstrapped_f")
+        return [None if r is None else
+                dict(self._with_boot(ex.entropy_enthalpy_result(r, Ls[p], warning_cutoff,
+                                                                self.results[p]["f_k_boots"] if boot else None),
+                                     r, keys), path=path[p])
                 for p, r in enumerate(inner)]
 
     def _grams(self):

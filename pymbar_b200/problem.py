@@ -847,28 +847,44 @@ class DeviceMbarBatch(_Resident):
                                                       _dptr(flat)))
         self.appended[problems] = M
 
-    def augmented_moments(self, f_list, want_G=False, problems=None):
+    def augmented_moments(self, f_list, want_G=False, problems=None, slots=None):
         """One dict per request (f_list[r] [R_p] at problem problems[r], by default problem r; R_p = K_p + M_p rows,
         the problem's own first): S [R_p], log_S [R_p], sum_L, flag and, with want_G, G = Ghat [R_p, R_p] (rows
         scaled by N_k where sampled, by 1 otherwise).  L_n comes from the sampled rows alone.  Appended weights are not
         shifted: ask for the Gram at a normalised f.  Two launches (three with the Gram) and one synchronisation for
-        all requests."""
-        ids = np.ascontiguousarray(np.arange(len(f_list)) if problems is None else problems, dtype=np.int32)
+        all requests.
+
+        slots: the requests name replicate slots instead (f_list[r] [R_p] at slot slots[r], whose problem
+        slot_problems[slots[r]] holds appended rows) and every sum counts sample n c_n times, L_n keeping N_k: the
+        appended rows' -log S are the updates DeviceProblem.replicate_unsampled gives.  No Gram; two launches.  All-ones
+        counts give the bits of the unweighted request."""
+        if slots is not None and problems is not None:
+            raise ValueError("an augmented moments call names problems or slots, not both")
+        weighted = slots is not None
+        if weighted and want_G:
+            raise ValueError("weighted augmented moments have no Gram")
+        ids = np.ascontiguousarray(np.arange(len(f_list)) if not weighted and problems is None
+                                   else (slots if weighted else problems), dtype=np.int32)
         if ids.shape != (len(f_list),) or len(f_list) == 0:
-            raise ValueError("need one problem index per f vector, and at least one")
-        Rs = [int(self.K[i] + self.appended[i]) if 0 <= i < self.P else -1 for i in ids]
+            raise ValueError("need one problem or slot index per f vector, and at least one")
+        owner = self.slot_problems if weighted else np.arange(self.P)
+        Rs = [int(self.K[owner[i]] + self.appended[owner[i]]) if 0 <= i < len(owner) else -1 for i in ids]
+        if weighted:
+            return self._requests(self._lib.mbar_b200_batch_replicate_augmented_moments, ids, f_list, Rs, False,
+                                  gram=False)
         return self._requests(self._lib.mbar_b200_batch_augmented_moments, ids, f_list, Rs, want_G)
 
-    def _requests(self, call, ids, f_list, rows, want_G, *flags):
+    def _requests(self, call, ids, f_list, rows, want_G, *flags, gram=True):
         """One batched moments call on requests f_list[r] [rows[r]] at units ids[r], `flags` passed after f; one dict
-        per request: S, log_S, sum_L, flag and, with want_G, G [rows[r], rows[r]]."""
+        per request: S, log_S, sum_L, flag and, with want_G, G [rows[r], rows[r]].  gram=False: `call` takes no Gram
+        argument."""
         f = np.ascontiguousarray(np.concatenate([_f64(v, R) for v, R in zip(f_list, rows)]))
         S, logS = np.empty(f.size), np.empty(f.size)
         sumL = np.empty(len(rows))
         flag = np.empty(len(rows), np.int32)
         G = np.empty(sum(R * R for R in rows)) if want_G else None
         check(call(self._h, len(rows), _i32p(ids), _dptr(f), *flags, _dptr(S), _dptr(logS), _dptr(sumL), _i32p(flag),
-                   _dptr(G) if want_G else None))
+                   *((_dptr(G) if want_G else None,) if gram else ())))
         out, o, g = [], 0, 0
         for r, R in enumerate(rows):
             d = dict(S=S[o:o + R], log_S=logS[o:o + R], sum_L=float(sumL[r]), flag=bool(flag[r]))
