@@ -485,9 +485,26 @@ int mbar_b200_batch_augmented_moments(mbar_b200_batch* batch, int32_t n_requests
 int mbar_b200_batch_replicate_augmented_moments(mbar_b200_batch* batch, int32_t n_requests, const int32_t* slot,
                                                 const double* f, double* S, double* log_S, double* sum_L,
                                                 int32_t* flag);
+/* Histogram FES of many problems (DESIGN.md 3.5h): mbar_b200_bin_moments for every request in one call.  Request r
+ * names problem[r] and gives its converged f [K_p], a target state's reduced potentials u_n [N_p] and dense bin
+ * indices bin_n [N_p] in [0, nbins[r]); f, u_n and bin_n concatenate the requests'.  With L_n = log sum_{k sampled}
+ * N_k exp(f_k - u_kn):
+ *   f_bin [nbins_r]         f_i  = -log sum_{n in i} exp(-u_n - L_n)                          (required)
+ *   C     [K_p * nbins_r]   C_ki = sum_{n in i} W_nk w^_n,  w^_n = exp(-u_n - L_n + f_i)      (row-major, may be NULL)
+ *   D     [nbins_r]         D_i  = sum_{n in i} w^_n^2                                         (may be NULL)
+ * each concatenated by request, W_nk over all K_p rows, sampled or not.  Only u_n and bin_n are uploaded: the
+ * problem's resident tiles, x_n and log N_k serve the rest.  Before any device work: a bad problem index, nbins < 1
+ * or a bin index outside [0, nbins) -> MBAR_B200_ERR_INVALID, a NaN u_n -> MBAR_B200_ERR_NAN.  +inf in u_n is weight
+ * 0.  flag[r] = 1 where an exponent of W_nk or w^_n exceeds 700, a bin has no sample of finite weight, or a sample's
+ * L_n is not a number; the call still succeeds.  Five kernel launches (seven with C or D) and one synchronisation.  No
+ * floating-point atomics: a request's results are the same bits whichever requests share the call, and repeat calls
+ * are bit-identical. */
+int mbar_b200_batch_bin_moments(mbar_b200_batch* batch, int32_t n_requests, const int32_t* problem, const double* f,
+                                const double* u_n, const int32_t* bin_n, const int32_t* nbins, double* f_bin,
+                                double* C, double* D, int32_t* flag);
 /* CUDA-event time of the kernels of the last batch_moments, batch_solve, batch_replicate_moments,
- * batch_solve_replicates, batch_augmented_moments or batch_replicate_augmented_moments call, its kernel launches, its
- * iterations (solves) and the bytes of u_kn tiles (appended tiles, counts) its passes read. */
+ * batch_solve_replicates, batch_augmented_moments, batch_replicate_augmented_moments or batch_bin_moments call, its
+ * kernel launches, its iterations (solves) and the bytes of u_kn tiles (appended tiles, counts) its passes read. */
 int mbar_b200_last_batch_stats(mbar_b200_batch* batch, double* kernel_ms, int32_t* launches, int32_t* iterations,
                                int64_t* bytes_read);
 

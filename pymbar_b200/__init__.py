@@ -12,8 +12,8 @@ Public surface:
   * :class:`pymbar_b200.DeviceMbarBatch` — many small MBAR problems (up to 64 states each) resident together;
     :func:`pymbar_b200.mbar_many.mbar_many` solves all of them in lockstep, one device call per iteration, and
     returns each problem's free energies and uncertainties, and :class:`pymbar_b200.MbarMany` keeps them resident
-    for batched expectations, perturbed free energies, entropies and enthalpies, overlaps and effective sample
-    numbers;
+    for batched expectations, perturbed free energies, entropies and enthalpies, overlaps, effective sample
+    numbers and histogram free-energy surfaces (``generate_fes`` / ``get_fes``);
   * :func:`pymbar_b200.install` — rebind ``pymbar.mbar_solvers`` so unmodified ``pymbar.MBAR`` uses it.
 
 Everything numerical runs in libmbar_b200.so (C ABI in include/mbar_b200.h).  No CPU fallback.

@@ -147,6 +147,7 @@ struct mbar_b200_batch : mbar::Resident {
     mbar::DevArray<double> d_f, d_part, d_out;
     mbar::HostPinned<double> h_f;               // pinned staging of f and of the packed output
     mbar::HostPinned<double> h_out;
+    mbar::HostPinned<int32_t> h_bin;            // pinned staging of the bin indices (mbar_b200_batch_bin_moments)
     // the last moments / solve call
     int32_t lastLaunches = 0, lastIterations = 0;
     int64_t lastBytes = 0;
@@ -884,6 +885,220 @@ static int batch_moments_call(mbar_b200_batch* b, Units kind, int32_t n, const i
     return MBAR_B200_OK;
 }
 
+// ---- histogram bin moments (DESIGN.md 3.5h) -------------------------------------------------------------------------
+// A request names a problem p, its converged f [K_p], a target state's u_n [N_p] and dense bin indices bin_n [N_p] in
+// [0, nbins).  With the shifted tiles u'_kn = u_kn - x_n,
+//   L'_n = log sum_{k sampled} N_k e^{f_k - u'_kn},   log w_n = -(u_n - x_n) - L'_n   (= -u_n - L_n)
+//   f_i  = -log sum_{n in i} w_n,   C_ki = sum_{n in i} W_nk w^_n,   D_i = sum_{n in i} w^_n^2,
+//   W_nk = e^{f_k - u'_kn - L'_n} (every row),   w^_n = e^{log w_n + f_i}
+// as mbar_b200_bin_moments gives them on one context.  Five kernels (seven with C and D), all requests in each:
+//   1. batch_bin_prep_kernel: L'_n and log w_n per sample, each bin's maximum m_i by an atomic max on the
+//      order-preserving key (a maximum does not depend on order);
+//   2. batch_bin_max_kernel: m_i from the keys;
+//   3. batch_bin_accum_kernel<false> + batch_bin_reduce_kernel<false>: s_i = sum_{n in i} e^{log w_n - m_i};
+//   4. batch_bin_f_kernel: f_i = -(m_i + log s_i);
+//   5. batch_bin_accum_kernel<true> + batch_bin_reduce_kernel<true>: the K_p rows of C and the row of D.
+// The accumulation is that of bins.cu (warp_groups): work items are (request, bin chunk, sample chunk); a CTA keeps a
+// [rows x bin chunk] accumulator in shared memory, warps own disjoint rows, and the last lane of each group of equal
+// bins adds the group's sum to its own cell.  Each sample chunk writes its block of partials, and the reduce kernel
+// adds them in chunk order.  The chunking is a function of (N_p, K_p, nbins) alone, there are no floating-point
+// atomics, so a request's results are the same bits whichever requests share the call.
+constexpr int BB_THREADS = 256;
+constexpr int BB_WARPS = BB_THREADS / 32;
+constexpr int BB_MAX_RW = (BATCH_MAX_K + 1 + BB_WARPS - 1) / BB_WARPS;   // rows per warp at K_p + 1 = 65 rows
+constexpr int BB_ACC_DOUBLES = (108 * 1024) / 8;    // shared accumulator per CTA: two CTAs per SM, as bins.cu
+constexpr int64_t BB_MIN_TILES = 64;                // a sample chunk holds at least 2048 samples ...
+constexpr int64_t BB_MAX_CHUNKS = 64;               // ... a request at most 64 sample chunks ...
+constexpr int64_t BB_PARTIAL_BYTES = 4 << 20;       // ... and at most 4 MB of partials (one chunk at least)
+constexpr double BB_MAX_ARG = 700.0;                // range contract of the W_nk and w^_n exponents
+
+// one pass's work items of a request: bin chunks of BC bins, sample chunks of ct tiles
+struct BinGeo {
+    int64_t item0;    // first (request, bin chunk, sample chunk) item
+    int64_t poff;     // first double of the request's partials [nsc][rows][nbins]
+    int64_t ct;       // tiles per sample chunk
+    int32_t BC, nbc, nsc;
+};
+
+static BinGeo bin_geometry(int64_t nT, int rows, int nbins) {
+    BinGeo g{};
+    g.BC = std::min(nbins, BB_ACC_DOUBLES / rows);
+    g.nbc = (nbins + g.BC - 1) / g.BC;
+    const int64_t cap = std::max<int64_t>(1, BB_PARTIAL_BYTES / ((int64_t)rows * nbins * 8));
+    const int64_t nsc = std::min(std::min((nT + BB_MIN_TILES - 1) / BB_MIN_TILES, BB_MAX_CHUNKS), cap);
+    g.ct = (nT + nsc - 1) / nsc;
+    g.nsc = (int32_t)((nT + g.ct - 1) / g.ct);
+    return g;
+}
+
+struct BinReq {
+    int64_t uoff;     // first double of the problem's tiles
+    int64_t xoff;     // first x_n of the problem
+    int64_t soff;     // first sample slot of the request (u_n -> log w_n, L'_n, bin index; nT_p * 32 slots)
+    int64_t N, nT;
+    int64_t boff;     // first bin of the request (keys, m, o, s, f_bin)
+    int64_t ooff;     // first entry of the request's [K_p + 1][nbins] C and D
+    int64_t foff;     // first entry of the request's f
+    int64_t voff;     // first entry of the problem's K-vectors (N_k, log N_k)
+    int32_t K, nbins;
+    BinGeo geo[2];    // 0: the bin sums (one row), 1: C and D (K_p + 1 rows)
+};
+
+// lw [slots]: u_n on entry (+inf past N_p), log w_n on exit (-inf past N_p and where u_n = +inf); Lp [slots]: L'_n.
+// A NaN log w_n (a sample whose sampled energies are all +inf) flags its request.
+__global__ void __launch_bounds__(256) batch_bin_prep_kernel(const double* __restrict__ u,
+                                                             const BinReq* __restrict__ req, int nReq, int64_t slots,
+                                                             const double* __restrict__ fAll,
+                                                             const double* __restrict__ NkAll,
+                                                             const double* __restrict__ logNkAll,
+                                                             const double* __restrict__ x, const int* __restrict__ bin,
+                                                             double* __restrict__ lw, double* __restrict__ Lp,
+                                                             unsigned long long* __restrict__ keys,
+                                                             int* __restrict__ rflag) {
+    const int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= slots) return;
+    const int r = find_segment(nReq, i, [&](int s) { return req[s].soff; });
+    const BinReq& q = req[r];
+    const int64_t n = i - q.soff;
+    if (n >= q.N) {
+        lw[i] = -INFINITY;
+        Lp[i] = 0.0;
+        return;
+    }
+    const double* ut = u + q.uoff + (n >> 5) * (int64_t)q.K * 32 + (n & 31);
+    const double* f = fAll + q.foff;
+    const double* Nk = NkAll + q.voff;
+    const double* logNk = logNkAll + q.voff;
+    double m = -INFINITY;
+    for (int k = 0; k < q.K; ++k)
+        if (Nk[k] > 0.0) m = fmax(m, f[k] + logNk[k] - __ldg(ut + k * 32));
+    double D = 0.0;
+    for (int k = 0; k < q.K; ++k)
+        if (Nk[k] > 0.0) D += exp(f[k] + logNk[k] - __ldg(ut + k * 32) - m);
+    const double L = m + log(D);
+    const double un = lw[i];
+    // u_n = +inf: weight exactly 0, as np.exp(-inf) in the reference
+    const double v = un < INFINITY ? -(un - x[q.xoff + n]) - L : -INFINITY;
+    Lp[i] = L;
+    lw[i] = v;
+    if (v != v) atomicOr(&rflag[r], 1);
+    const unsigned long long key = ordered_key(v);
+    unsigned long long* kb = keys + q.boff + bin[i];
+    if (v > -INFINITY && key > *((volatile unsigned long long*)kb)) atomicMax(kb, key);
+}
+
+// m_i from the keys, o = -m_i (the offset of the bin-sum pass).  A bin without a finite maximum (no sample, every
+// u_n = +inf, or a u_n = -inf) flags its request.
+__global__ void batch_bin_max_kernel(const BinReq* __restrict__ req, int nReq, int64_t bins,
+                                     const unsigned long long* __restrict__ keys, double* __restrict__ m,
+                                     double* __restrict__ o, int* __restrict__ rflag) {
+    const int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= bins) return;
+    const double v = ordered_value(keys[i]);
+    if (!isfinite(v)) atomicOr(&rflag[find_segment(nReq, i, [&](int s) { return req[s].boff; })], 1);
+    m[i] = v;
+    o[i] = -v;
+}
+
+// f_i = -(m_i + log s_i), o = f_i (the offset of the moments pass)
+__global__ void batch_bin_f_kernel(const BinReq* __restrict__ req, int nReq, int64_t bins,
+                                   const double* __restrict__ m, const double* __restrict__ s,
+                                   double* __restrict__ fbin, double* __restrict__ o, int* __restrict__ rflag) {
+    const int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= bins) return;
+    const double fb = -(m[i] + log(s[i]));
+    if (!isfinite(fb)) atomicOr(&rflag[find_segment(nReq, i, [&](int r) { return req[r].boff; })], 1);
+    fbin[i] = fb;
+    o[i] = fb;
+}
+
+// One CTA per (request, bin chunk, sample chunk) item.  MOM = false: one row of ones against e^{log w_n - m_i} (the bin
+// sums); MOM = true: the K_p rows of W_nk and one row of w^_n against w^_n (C and D).
+template <bool MOM>
+__global__ void __launch_bounds__(BB_THREADS, 2) batch_bin_accum_kernel(
+    const double* __restrict__ u, const BinReq* __restrict__ req, int nReq, const double* __restrict__ fAll,
+    const double* __restrict__ lw, const double* __restrict__ Lp, const int* __restrict__ bin,
+    const double* __restrict__ o, double* __restrict__ part, int* __restrict__ rflag) {
+    extern __shared__ double acc[];                     // [rows][BC]
+    __shared__ int perm[BB_WARPS][32];
+    const unsigned FULL = 0xffffffffu;
+    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+    const int r = find_segment(nReq, blockIdx.x, [&](int s) { return req[s].geo[MOM].item0; });
+    const BinReq& q = req[r];
+    const BinGeo g = q.geo[MOM];
+    const int64_t local = blockIdx.x - g.item0;
+    const int sc = (int)(local % g.nsc), bc = (int)(local / g.nsc);
+    const int K = q.K, nbins = q.nbins;
+    const int Kw = MOM ? K : 0, rows = Kw + 1;
+    const int b0 = bc * g.BC, bw = min(g.BC, nbins - b0);
+    for (int i = threadIdx.x; i < rows * g.BC; i += BB_THREADS) acc[i] = 0.0;
+    __syncthreads();
+    const int myRows = (warp < rows) ? (rows - 1 - warp) / BB_WARPS + 1 : 0;   // rows warp, warp + 8, ...
+    const int64_t t0 = (int64_t)sc * g.ct, t1 = min(q.nT, t0 + g.ct);
+    const double* f = fAll + q.foff;
+    const double* ob = o + q.boff;
+    bool range = false;
+    for (int64_t t = t0; t < t1 && myRows > 0; ++t) {
+        const int64_t i = q.soff + t * 32 + lane;
+        const int b = bin[i];
+        if (!__any_sync(FULL, b >= b0 && b < b0 + bw)) continue;
+        // this tile's energies first, so that the loads of all rows are in flight together
+        const double* tp = u + q.uoff + t * (int64_t)K * 32 + lane;
+        double uu[BB_MAX_RW];
+#pragma unroll
+        for (int j = 0; j < BB_MAX_RW; ++j) {
+            const int rl = warp + BB_WARPS * j;
+            uu[j] = (j < myRows && rl < Kw) ? __ldg(tp + rl * 32) : 0.0;
+        }
+        const double L = Lp[i];
+        const double eo = (b >= 0) ? lw[i] + ob[b] : -INFINITY;
+        if (eo > BB_MAX_ARG) range = true;
+        const double e0 = exp(eo);                      // w^_n (moments) | e^{log w_n - m_i} (bin sums)
+        const double aux = MOM ? e0 : 1.0;
+        const WarpGroups grp = warp_groups(b, perm[warp]);
+        const int col = (grp.tail && grp.key >= b0 && grp.key < b0 + bw) ? grp.key - b0 : -1;
+#pragma unroll
+        for (int j = 0; j < BB_MAX_RW; ++j) {
+            const int rl = warp + BB_WARPS * j;
+            if (j >= myRows) continue;                  // warp-uniform
+            double a = aux;
+            if (rl < Kw) {
+                // +inf energies (and the padding past N_p) have weight exactly 0
+                const double e = f[rl] - uu[j] - L;
+                if (b >= 0 && e > BB_MAX_ARG) range = true;
+                a = exp(e);
+            }
+            if (b < 0) a = 0.0;
+            const double v = warp_group_sum(grp, a * e0);
+            if (col >= 0) acc[rl * g.BC + col] += v;
+        }
+        __syncwarp();
+    }
+    if (range) atomicOr(&rflag[r], 1);
+    __syncthreads();
+    double* dst = part + g.poff + (int64_t)sc * rows * nbins + b0;
+    for (int i = threadIdx.x; i < rows * bw; i += BB_THREADS) {
+        const int rl = i / bw, c = i - rl * bw;
+        dst[(int64_t)rl * nbins + c] = acc[rl * g.BC + c];
+    }
+}
+
+// out[i] over every request's [rows][nbins] entries (MOM = false: the bin sums at boff; true: C and D at ooff): the
+// sum over the request's sample chunks, in chunk order
+template <bool MOM>
+__global__ void batch_bin_reduce_kernel(const BinReq* __restrict__ req, int nReq, int64_t total,
+                                        const double* __restrict__ part, double* __restrict__ out) {
+    const int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= total) return;
+    const BinReq& q = req[find_segment(nReq, i, [&](int s) { return MOM ? req[s].ooff : req[s].boff; })];
+    const BinGeo& g = q.geo[MOM];
+    const int rows = MOM ? q.K + 1 : 1;
+    const int64_t e = i - (MOM ? q.ooff : q.boff);    // row * nbins + bin
+    double s = 0.0;
+    for (int c = 0; c < g.nsc; ++c) s += part[g.poff + (int64_t)c * rows * q.nbins + e];
+    out[i] = s;
+}
+
 }  // namespace mbar
 
 using namespace mbar;
@@ -1101,6 +1316,163 @@ int mbar_b200_batch_replicate_augmented_moments(mbar_b200_batch* b, int32_t n_re
     NvtxRange nvtx_("mbar_b200::batch_replicate_augmented_moments");
     return batch_moments_call(b, Units::slot_appended, n_requests, slot, f, 1, S, logS, sumL, flag, nullptr,
                               "batch_replicate_augmented_moments");
+}
+
+int mbar_b200_batch_bin_moments(mbar_b200_batch* b, int32_t n, const int32_t* problem, const double* f,
+                                const double* u_n, const int32_t* bin_n, const int32_t* nbins, double* f_bin,
+                                double* C, double* D, int32_t* flag) {
+    MBAR_REQUIRE(b, MBAR_B200_ERR_INVALID, "batch_bin_moments: NULL object");
+    MBAR_REQUIRE(n >= 1 && problem && f && u_n && bin_n && nbins && f_bin && flag, MBAR_B200_ERR_INVALID,
+                 "batch_bin_moments: %d requests or a NULL argument", (int)n);
+    const bool wantC = C || D;
+    std::vector<BinReq> req((size_t)n);
+    std::vector<int64_t> tile0((size_t)b->P, 0);  // first tile of each problem: indexes x_n
+    for (int p = 1; p < b->P; ++p) tile0[p] = tile0[p - 1] + b->nT[p - 1];
+    int64_t slots = 0, bins = 0, outs = 0, fs = 0, items0 = 0, items1 = 0, parts0 = 0, parts1 = 0, bytes = 0, src = 0;
+    size_t smem1 = 0;
+    for (int r = 0; r < n; ++r) {
+        const int p = problem[r];
+        MBAR_REQUIRE(p >= 0 && p < b->P, MBAR_B200_ERR_INVALID, "batch_bin_moments: request %d names problem %d of %d",
+                     r, p, b->P);
+        MBAR_REQUIRE(nbins[r] >= 1, MBAR_B200_ERR_INVALID, "batch_bin_moments: request %d has nbins = %d", r,
+                     (int)nbins[r]);
+        BinReq& q = req[r];
+        q.K = b->K[p];
+        q.nbins = nbins[r];
+        q.N = b->N[p];
+        q.nT = b->nT[p];
+        q.uoff = b->uoff[p];
+        q.voff = b->voff[p];
+        q.xoff = tile0[p] * 32;
+        q.soff = slots;
+        q.boff = bins;
+        q.ooff = outs;
+        q.foff = fs;
+        for (int64_t i = 0; i < q.N; ++i)
+            MBAR_REQUIRE(bin_n[src + i] >= 0 && bin_n[src + i] < q.nbins, MBAR_B200_ERR_INVALID,
+                         "batch_bin_moments: request %d: bin index %d of sample %lld lies outside [0, %d)", r,
+                         (int)bin_n[src + i], (long long)i, (int)q.nbins);
+        src += q.N;
+        for (int pass = 0; pass < 2; ++pass) {
+            BinGeo& g = q.geo[pass];
+            g = bin_geometry(q.nT, pass ? q.K + 1 : 1, q.nbins);
+            int64_t& items = pass ? items1 : items0;
+            int64_t& parts = pass ? parts1 : parts0;
+            g.item0 = items;
+            g.poff = parts;
+            items += (int64_t)g.nbc * g.nsc;
+            parts += (int64_t)g.nsc * (pass ? q.K + 1 : 1) * q.nbins;
+        }
+        smem1 = std::max(smem1, (size_t)(q.K + 1) * q.geo[1].BC * sizeof(double));
+        bytes += q.nT * 32 * q.K * 8 * (1 + (wantC ? q.geo[1].nbc : 0));   // the prep pass, then C's bin chunks
+        slots += q.nT * 32;
+        bins += q.nbins;
+        outs += (int64_t)(q.K + 1) * q.nbins;
+        fs += q.K;
+    }
+    for (int64_t i = 0; i < src; ++i)
+        MBAR_REQUIRE(u_n[i] == u_n[i], MBAR_B200_ERR_NAN, "batch_bin_moments: NaN in u_n (entry %lld)", (long long)i);
+    MBAR_REQUIRE(items0 < INT32_MAX && items1 < INT32_MAX, MBAR_B200_ERR_INVALID,
+                 "batch_bin_moments: %lld work items in one call", (long long)std::max(items0, items1));
+    MBAR_CUDA(cudaSetDevice(b->device));
+    NvtxRange nvtx_("mbar_b200::batch_bin_moments");
+    b->lastLaunches = 0;
+    b->lastBytes = 0;
+    b->lastIterations = 0;
+    // pinned staging: f, u_n padded with +inf to the tiles and the requests; the bin indices, padded with -1 (no bin)
+    const size_t reqDoubles = ((size_t)n * sizeof(BinReq) + 7) / 8;
+    MBAR_TRY(b->h_f.grow((size_t)fs + (size_t)slots + reqDoubles, "batch_bin_moments"));
+    MBAR_TRY(b->h_bin.grow((size_t)slots, "batch_bin_moments"));
+    double* hu = b->h_f + fs;
+    src = 0;
+    int64_t fo = 0;
+    for (int r = 0; r < n; ++r) {
+        const BinReq& q = req[r];
+        std::memcpy(b->h_f + q.foff, f + fo, (size_t)q.K * sizeof(double));
+        std::memcpy(hu + q.soff, u_n + src, (size_t)q.N * sizeof(double));
+        std::memcpy(b->h_bin + q.soff, bin_n + src, (size_t)q.N * sizeof(int32_t));
+        for (int64_t i = q.N; i < q.nT * 32; ++i) {
+            hu[q.soff + i] = INFINITY;
+            b->h_bin[q.soff + i] = -1;
+        }
+        src += q.N;
+        fo += q.K;
+    }
+    BinReq* hreq = reinterpret_cast<BinReq*>(b->h_f + fs + slots);
+    std::memcpy(hreq, req.data(), req.size() * sizeof(BinReq));
+    CallBuffers buf("batch_bin_moments");
+    BinReq* d_req;
+    int *d_bin, *d_rflag;
+    double *d_f, *d_lw, *d_Lp, *d_m, *d_o, *d_s, *d_fbin, *d_part, *d_out = nullptr;
+    unsigned long long* d_keys;
+    MBAR_TRY(buf.alloc(&d_req, (size_t)n));
+    MBAR_TRY(buf.alloc(&d_f, (size_t)fs));
+    MBAR_TRY(buf.alloc(&d_lw, (size_t)slots));
+    MBAR_TRY(buf.alloc(&d_Lp, (size_t)slots));
+    MBAR_TRY(buf.alloc(&d_bin, (size_t)slots));
+    MBAR_TRY(buf.alloc(&d_keys, (size_t)bins));
+    MBAR_TRY(buf.alloc(&d_m, (size_t)bins));
+    MBAR_TRY(buf.alloc(&d_o, (size_t)bins));
+    MBAR_TRY(buf.alloc(&d_s, (size_t)bins));
+    MBAR_TRY(buf.alloc(&d_fbin, (size_t)bins));
+    MBAR_TRY(buf.alloc(&d_part, (size_t)std::max(parts0, wantC ? parts1 : 0)));
+    MBAR_TRY(buf.alloc(&d_rflag, (size_t)n));
+    if (wantC) MBAR_TRY(buf.alloc(&d_out, (size_t)outs));
+    cudaStream_t s = b->stream;
+    MBAR_CUDA(cudaMemcpyAsync(d_f, b->h_f, (size_t)fs * sizeof(double), cudaMemcpyHostToDevice, s));
+    MBAR_CUDA(cudaMemcpyAsync(d_lw, hu, (size_t)slots * sizeof(double), cudaMemcpyHostToDevice, s));
+    MBAR_CUDA(cudaMemcpyAsync(d_bin, b->h_bin, (size_t)slots * sizeof(int32_t), cudaMemcpyHostToDevice, s));
+    MBAR_CUDA(cudaMemcpyAsync(d_req, hreq, req.size() * sizeof(BinReq), cudaMemcpyHostToDevice, s));
+    MBAR_CUDA(cudaMemsetAsync(d_keys, 0, (size_t)bins * sizeof(unsigned long long), s));
+    MBAR_CUDA(cudaMemsetAsync(d_rflag, 0, (size_t)n * sizeof(int), s));
+    const size_t smem0 = (size_t)BB_ACC_DOUBLES * sizeof(double);
+    MBAR_CUDA(cudaFuncSetAttribute(batch_bin_accum_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                   (int)smem0));
+    MBAR_CUDA(cudaFuncSetAttribute(batch_bin_accum_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                   (int)smem0));
+    // the largest shared-memory carveout, so that two CTAs with the largest accumulator share an SM
+    MBAR_CUDA(cudaFuncSetAttribute(batch_bin_accum_kernel<false>, cudaFuncAttributePreferredSharedMemoryCarveout, 100));
+    MBAR_CUDA(cudaFuncSetAttribute(batch_bin_accum_kernel<true>, cudaFuncAttributePreferredSharedMemoryCarveout, 100));
+    size_t smemS = 0;
+    for (const BinReq& q : req) smemS = std::max(smemS, (size_t)q.geo[0].BC * sizeof(double));
+    MBAR_CUDA(cudaEventRecord(b->ev0, s));
+    batch_bin_prep_kernel<<<(unsigned)((slots + 255) / 256), 256, 0, s>>>(
+        b->d_u, d_req, n, slots, d_f, b->d_Nk, b->d_logNk, b->d_x, d_bin, d_lw, d_Lp, d_keys, d_rflag);
+    batch_bin_max_kernel<<<(unsigned)((bins + 255) / 256), 256, 0, s>>>(d_req, n, bins, d_keys, d_m, d_o, d_rflag);
+    batch_bin_accum_kernel<false><<<(unsigned)items0, BB_THREADS, smemS, s>>>(b->d_u, d_req, n, d_f, d_lw, d_Lp, d_bin,
+                                                                              d_o, d_part, d_rflag);
+    batch_bin_reduce_kernel<false><<<(unsigned)((bins + 255) / 256), 256, 0, s>>>(d_req, n, bins, d_part, d_s);
+    batch_bin_f_kernel<<<(unsigned)((bins + 255) / 256), 256, 0, s>>>(d_req, n, bins, d_m, d_s, d_fbin, d_o, d_rflag);
+    b->lastLaunches = 5;
+    if (wantC) {
+        batch_bin_accum_kernel<true><<<(unsigned)items1, BB_THREADS, smem1, s>>>(b->d_u, d_req, n, d_f, d_lw, d_Lp,
+                                                                                 d_bin, d_o, d_part, d_rflag);
+        batch_bin_reduce_kernel<true><<<(unsigned)((outs + 255) / 256), 256, 0, s>>>(d_req, n, outs, d_part, d_out);
+        b->lastLaunches += 2;
+    }
+    MBAR_CUDA(cudaGetLastError());
+    MBAR_CUDA(cudaEventRecord(b->ev1, s));
+    MBAR_TRY(b->h_out.grow((size_t)bins + (wantC ? (size_t)outs : 0), "batch_bin_moments"));
+    std::vector<int> hflag((size_t)n);
+    MBAR_CUDA(cudaMemcpyAsync(b->h_out, d_fbin, (size_t)bins * sizeof(double), cudaMemcpyDeviceToHost, s));
+    if (wantC)
+        MBAR_CUDA(cudaMemcpyAsync(b->h_out + bins, d_out, (size_t)outs * sizeof(double), cudaMemcpyDeviceToHost, s));
+    MBAR_CUDA(cudaMemcpyAsync(hflag.data(), d_rflag, (size_t)n * sizeof(int), cudaMemcpyDeviceToHost, s));
+    MBAR_CUDA(cudaStreamSynchronize(s));
+    float ms = 0.f;
+    b->lastMs = event_ms(b->ev0, b->ev1, &ms) ? ms : 0.0;
+    b->lastBytes = bytes;
+    int64_t co = 0;
+    for (int r = 0; r < n; ++r) {
+        const BinReq& q = req[r];
+        flag[r] = hflag[r] != 0;
+        std::memcpy(f_bin + q.boff, b->h_out + q.boff, (size_t)q.nbins * sizeof(double));
+        const double* o = b->h_out + bins + q.ooff;
+        if (C) std::memcpy(C + co, o, (size_t)q.K * q.nbins * sizeof(double));
+        if (D) std::memcpy(D + q.boff, o + (size_t)q.K * q.nbins, (size_t)q.nbins * sizeof(double));
+        co += (int64_t)q.K * q.nbins;
+    }
+    return MBAR_B200_OK;
 }
 
 int mbar_b200_last_batch_stats(mbar_b200_batch* b, double* ms, int32_t* launches, int32_t* iterations,

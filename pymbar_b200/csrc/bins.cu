@@ -35,14 +35,6 @@ constexpr size_t BIN_PARTIAL_BYTES = 256ull << 20;     // cap of the per-CTA par
 constexpr double BIN_MAX_ARG = 700.0;                  // range contract of W_nk and w^_n exponents
 enum { BINF_INVALID = 1, BINF_NAN = 2, BINF_RANGE = 4 };
 
-__device__ __forceinline__ unsigned long long ordered_key(double d) {
-    const unsigned long long b = (unsigned long long)__double_as_longlong(d);
-    return (b >> 63) ? ~b : (b | 0x8000000000000000ull);
-}
-__device__ __forceinline__ double ordered_value(unsigned long long k) {
-    return __longlong_as_double((long long)((k >> 63) ? (k & 0x7fffffffffffffffull) : ~k));
-}
-
 // lw [nPad]: u_n on entry (first N), log w_n on exit (-inf for padding and for samples of multiplicity 0);
 // bin [nPad]: the caller's bin index on entry, -1 for padding on exit.
 __global__ void bin_prep_kernel(int64_t N, int64_t nPad, int nbins, int* __restrict__ bin, double* __restrict__ lw,
@@ -146,33 +138,8 @@ __global__ void __launch_bounds__(BIN_THREADS, 2) bin_accum_kernel(BinParams p) 
         const double right = (p.wgt ? p.wgt[n] : 1.0) * e0;
         const double aux = (p.Kw == 0) ? 1.0 : e0;
         // group the lanes by bin and make every group contiguous, groups in the order of their lowest lane
-        const unsigned grp = __match_any_sync(FULL, b);
-        const int leader = __ffs(grp) - 1;
-        const int gsize = __popc(grp);
-        const int own = (lane == leader) ? gsize : 0;
-        int incl = own;
-#pragma unroll
-        for (int d = 1; d < 32; d <<= 1) {
-            const int y = __shfl_up_sync(FULL, incl, d);
-            if (lane >= d) incl += y;
-        }
-        const int start = __shfl_sync(FULL, incl - own, leader);
-        perm[warp][start + __popc(grp & ((1u << lane) - 1u))] = lane;
-        __syncwarp();
-        const int src = perm[warp][lane];
-        __syncwarp();
-        const int key = __shfl_sync(FULL, b, src);
-        const int maxg = (int)__reduce_max_sync(FULL, (unsigned)gsize);
-        int steps = 0;
-        while ((1 << steps) < maxg) ++steps;
-        unsigned same = 0;
-        for (int s = 0; s < steps; ++s) {
-            const int kd = __shfl_up_sync(FULL, key, 1 << s);
-            if (lane >= (1 << s) && kd == key) same |= 1u << s;
-        }
-        const int next = __shfl_down_sync(FULL, key, 1);
-        const bool tail = (lane == 31) || next != key;
-        const int col = (tail && key >= p.b0 && key < p.b0 + p.bw) ? key - p.b0 : -1;
+        const WarpGroups grp = warp_groups(b, perm[warp]);
+        const int col = (grp.tail && grp.key >= p.b0 && grp.key < p.b0 + p.bw) ? grp.key - p.b0 : -1;
         // predicated rather than an early exit, so that the rows' exps and shuffles can interleave
 #pragma unroll
         for (int j = 0; j < BIN_MAX_RW; ++j) {
@@ -187,11 +154,7 @@ __global__ void __launch_bounds__(BIN_THREADS, 2) bin_accum_kernel(BinParams p) 
                 a = (uu[j] >= U_CLAMP) ? 0.0 : exp(e);
             }
             if (b < 0) a = 0.0;
-            double v = __shfl_sync(FULL, a * right, src);
-            for (int s = 0; s < steps; ++s) {
-                const double y = __shfl_up_sync(FULL, v, 1 << s);
-                if ((same >> s) & 1u) v += y;
-            }
+            const double v = warp_group_sum(grp, a * right);
             if (col >= 0) acc[rl * p.BC + col] += v;
         }
         __syncwarp();

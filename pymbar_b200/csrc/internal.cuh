@@ -708,6 +708,68 @@ __device__ __forceinline__ double warp_sum(double x) {
     for (int o = 16; o > 0; o >>= 1) x += __shfl_xor_sync(0xffffffffu, x, o);
     return x;
 }
+
+// The order-preserving integer form of a double, so that a per-bin maximum can be taken by an integer atomicMax (a
+// maximum does not depend on the order of its operands, so the result is deterministic); 0 is below every key.
+__device__ __forceinline__ unsigned long long ordered_key(double d) {
+    const unsigned long long b = (unsigned long long)__double_as_longlong(d);
+    return (b >> 63) ? ~b : (b | 0x8000000000000000ull);
+}
+__device__ __forceinline__ double ordered_value(unsigned long long k) {
+    return __longlong_as_double((long long)((k >> 63) ? (k & 0x7fffffffffffffffull) : ~k));
+}
+
+// The lanes of a warp grouped by an integer key (__match_any_sync) and sorted so that every group is contiguous,
+// groups in the order of their lowest lane.  Lane i of the sorted order holds lane src's value and key; `same` bit s
+// says the lane 2^s below it holds the same key; `tail` marks the last lane of each group.  Computed once per tile and
+// reused for every row summed over that tile; perm is the warp's 32-int shared scratch.
+struct WarpGroups {
+    int src, key, steps;
+    unsigned same;
+    bool tail;
+};
+__device__ __forceinline__ WarpGroups warp_groups(int b, int* perm) {
+    const unsigned FULL = 0xffffffffu;
+    const int lane = threadIdx.x & 31;
+    const unsigned grp = __match_any_sync(FULL, b);
+    const int leader = __ffs(grp) - 1;
+    const int gsize = __popc(grp);
+    const int own = (lane == leader) ? gsize : 0;
+    int incl = own;
+#pragma unroll
+    for (int d = 1; d < 32; d <<= 1) {
+        const int y = __shfl_up_sync(FULL, incl, d);
+        if (lane >= d) incl += y;
+    }
+    const int start = __shfl_sync(FULL, incl - own, leader);
+    perm[start + __popc(grp & ((1u << lane) - 1u))] = lane;
+    __syncwarp();
+    WarpGroups g;
+    g.src = perm[lane];
+    __syncwarp();
+    g.key = __shfl_sync(FULL, b, g.src);
+    const int maxg = (int)__reduce_max_sync(FULL, (unsigned)gsize);
+    g.steps = 0;
+    while ((1 << g.steps) < maxg) ++g.steps;
+    g.same = 0;
+    for (int s = 0; s < g.steps; ++s) {
+        const int kd = __shfl_up_sync(FULL, g.key, 1 << s);
+        if (lane >= (1 << s) && kd == g.key) g.same |= 1u << s;
+    }
+    const int next = __shfl_down_sync(FULL, g.key, 1);
+    g.tail = (lane == 31) || next != g.key;
+    return g;
+}
+// v of lane src, summed over its group by a segmented scan of g.steps steps: a tail lane ends with its group's sum,
+// added in an order fixed by the keys alone
+__device__ __forceinline__ double warp_group_sum(const WarpGroups& g, double v) {
+    v = __shfl_sync(0xffffffffu, v, g.src);
+    for (int s = 0; s < g.steps; ++s) {
+        const double y = __shfl_up_sync(0xffffffffu, v, 1 << s);
+        if ((g.same >> s) & 1u) v += y;
+    }
+    return v;
+}
 #endif
 
 // Relative change |a - b| / |ref| of one entry (mbar_solvers.py:627-632); entries with |ref| below thr = min(1e-8, tol)

@@ -86,21 +86,34 @@ def dense_bins(sample_label, bin_order):
     return order[srt][pos].astype(np.int32)
 
 
+def histogram_bins(x_n, bin_edges):
+    """(histogram_data without "f", dense bin index [N] int32, number of dense bins) of fes.py:476-578."""
+    bins = _edges(bin_edges)
+    bin_n, sample_label, nonzero_bins, bin_label, bin_order = histogram_labels(x_n, bins)
+    dense = dense_bins(sample_label, bin_order)
+    data = {"dims": len(bins), "bins": bins, "bin_n": bin_n, "nonzero_bins": nonzero_bins,
+            "sample_label": sample_label, "bin_order": bin_order, "bin_label": bin_label}
+    return data, dense, len(bin_order)
+
+
+def with_bin_f(data, f_bin):
+    """histogram_data["f"] from the dense bins' free energies f_bin.  fes.py:579 sizes f by the distinct bin TUPLES:
+    when several out-of-grid tuples share the label -1 the trailing entries stay 0, and "from-lowest" can pick one of
+    them, as in the reference."""
+    f = np.zeros(len(data["bin_label"]))
+    f[:len(data["bin_order"])] = f_bin
+    data["f"] = f
+    return data
+
+
 def histogram_fes(problem, f_k, u_n, x_n, bin_edges):
     """The histogram_data dict of fes.py:476-600 for the target state u_n, with f from the device.
 
     `problem` is the DeviceProblem holding (u_kn, N_k); f_k its converged free energies.  The dict has the
     reference's keys and types, so the reference's get_fes code reads it unchanged."""
-    bins = _edges(bin_edges)
-    bin_n, sample_label, nonzero_bins, bin_label, bin_order = histogram_labels(x_n, bins)
-    dense = dense_bins(sample_label, bin_order)
-    f_bin, _, _ = problem.bin_moments(f_k, u_n, dense, len(bin_order), want_C=False)
-    # fes.py:579 sizes f by the distinct bin TUPLES: when several out-of-grid tuples share the label -1 the trailing
-    # entries stay 0, and "from-lowest" can pick one of them, as in the reference
-    f = np.zeros(len(bin_label))
-    f[:len(bin_order)] = f_bin
-    return {"dims": len(bins), "bins": bins, "bin_n": bin_n, "nonzero_bins": nonzero_bins,
-            "sample_label": sample_label, "bin_order": bin_order, "bin_label": bin_label, "f": f}
+    data, dense, nb = histogram_bins(x_n, bin_edges)
+    f_bin, _, _ = problem.bin_moments(f_k, u_n, dense, nb, want_C=False)
+    return with_bin_f(data, f_bin)
 
 
 def augmented_moments(G, C, D):
@@ -122,10 +135,15 @@ def histogram_theta(problem, f_k, N_k, u_n, histogram_data, return_moments=False
     nb = len(histogram_data["bin_order"])
     _, C, D = problem.bin_moments(f_k, u_n, dense, nb)
     S, G = problem.weight_moments(f_k)
-    G_aug = augmented_moments(G, C, D)
-    N_aug = np.concatenate([np.asarray(N_k, dtype=np.float64), np.zeros(nb)])
-    Theta = est.asymptotic_covariance(G_aug, N_aug, method="svd-ew")
+    Theta, G_aug = augmented_theta(G, C, D, N_k)
     return (Theta, S, G_aug) if return_moments else Theta
+
+
+def augmented_theta(G, C, D, N_k):
+    """(Theta, G_aug) of the augmented problem, "svd-ew" (fes.py:1402-1406): the bins are states with N = 0."""
+    G_aug = augmented_moments(G, C, D)
+    N_aug = np.concatenate([np.asarray(N_k, dtype=np.float64), np.zeros(np.shape(C)[1])])
+    return est.asymptotic_covariance(G_aug, N_aug, method="svd-ew"), G_aug
 
 
 def bin_uncertainties(Theta, K, j, n_out=None):

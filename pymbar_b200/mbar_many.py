@@ -46,6 +46,7 @@ import numpy as np
 from . import bootstrap
 from . import estimators
 from . import expectations as ex
+from . import fes as hist
 from . import mbar_solvers as ms
 from .utils import ParameterError
 
@@ -59,6 +60,8 @@ BOOT_WAVE_BYTES = 2 << 30   # device footprint of one wave of replicate slots
 MAX_BATCH_ROWS = 192        # DeviceMbarBatch.MAX_ROWS: K_p plus appended rows of a batched estimator request
 AUG_WAVE_BYTES = 2 << 30    # device footprint of one wave of appended rows
 ESTIMATOR_METHODS = (None, "svd-ew", "approximate", "bootstrap")
+FES_WAVE_BYTES = 2 << 30    # device footprint of one wave of histogram FES requests
+FES_UNCERTAINTY_METHODS = (None, "analytical")
 
 
 def _classes():
@@ -152,6 +155,48 @@ def boot_augmented_bytes(K, N, M):
     R = int(K) + int(M)
     nc = -(-nT // _chunk_tiles(nT, R))
     return 2 * nT * 32 + 8 * (nc * (2 * R + 2) + 2 * R + 2 + R)
+
+
+def _bin_geometry(nT, rows, nbins):
+    """(bins per chunk, bin chunks, sample chunks) of one pass of a batched bin moments request (bin_geometry in
+    batch.cu)."""
+    BC = min(nbins, (108 * 1024 // 8) // rows)
+    cap = max(1, (4 << 20) // (rows * nbins * 8))
+    nsc = min(-(-nT // 64), 64, cap)
+    ct = -(-nT // nsc)
+    return BC, -(-nbins // BC), -(-nT // ct)
+
+
+def bin_bytes(K, N, nbins, want_C):
+    """Device bytes of one histogram request in a wave: its u_n, log w_n, L_n and bin slots, the per-bin arrays, the
+    partials of its larger pass, C and D when asked for, its f and its request record (batch.cu's geometry)."""
+    nT = -(-int(N) // 32)
+    K, nbins = int(K), int(nbins)
+    parts = _bin_geometry(nT, 1, nbins)[2] * nbins
+    if want_C:
+        parts = max(parts, _bin_geometry(nT, K + 1, nbins)[2] * (K + 1) * nbins)
+    return 20 * nT * 32 + 40 * nbins + 8 * parts + (8 * (K + 1) * nbins if want_C else 0) + 8 * K + 164
+
+
+def _waves(items, need, limit):
+    """items split, in order, into waves whose need(item) sum stays under limit (one item at least per wave)."""
+    waves, wave, used = [], [], 0
+    for it in items:
+        n = need(it)
+        if wave and used + n > limit:
+            waves.append(wave)
+            wave, used = [], 0
+        wave.append(it)
+        used += n
+    if wave:
+        waves.append(wave)
+    return waves
+
+
+def _noted(err, p):
+    """err with a note naming problem p, for errors of the single path."""
+    err.add_note(f"raised for problem {p} (MbarMany histogram FES, single path)")
+    return err
 
 
 def _validate_boot(n_bootstraps, rseed, P):
@@ -343,6 +388,8 @@ class MbarMany:
         self._B = B
         self._draws = []             # problem -> its _Draws (n_bootstraps > 0): replicate counts are regenerated
         self._overflow = set()       # problems whose replicate multiplicities overflow uint16
+        self.histogram_datas = [None] * P    # problem -> the reference's histogram_data dict (generate_fes)
+        self._fes = {}                       # problem -> its histogram request, path and cached Theta
         self.device_stats = dict(ms=0.0, launches=0, calls=0, bytes_read=0)
         self.host_stats = dict(counts_s=0.0)     # host time spent regenerating replicate counts for the estimators
         try:
@@ -694,11 +741,12 @@ class MbarMany:
                                      r, keys), path=path[p])
                 for p, r in enumerate(inner)]
 
-    def _grams(self):
-        """W^T W at the final f of every problem: the solve's where it computed one, one batched moments call for
-        the other batched problems, DeviceProblem.weight_moments for the rest."""
+    def _grams(self, problems=None):
+        """W^T W at the final f of every problem (of `problems`): the solve's where it computed one, one batched
+        moments call for the other batched problems, DeviceProblem.weight_moments for the rest."""
         P = len(self._probs)
-        need = [p for p in range(P) if p not in self._G]
+        problems = range(P) if problems is None else problems
+        need = [p for p in problems if p not in self._G]
         batched = [p for p in need if self.results[p]["path"] == "batch"]
         if batched:
             sums = self._dev.moments([self.results[p]["f_k"] for p in batched], want_G=True, all_rows=True,
@@ -713,7 +761,7 @@ class MbarMany:
                 u, N_k, _ = self._probs[p]
                 with Prob(u, N_k, device=ms._DEVICE) as q:
                     _, self._G[p] = q.weight_moments(self.results[p]["f_k"])
-        return [self._G[p] for p in range(P)]
+        return [self._G[p] for p in problems]
 
     def compute_overlap(self):
         """scalar, eigenvalues, matrix of every problem (MBAR.compute_overlap), from W^T W at the final f.  A
@@ -727,6 +775,157 @@ class MbarMany:
                 O = np.asarray(N_k, dtype=np.float64) * np.asarray(G)
                 d = {"scalar": np.nan, "eigenvalues": np.linalg.eigvals(O), "matrix": O}
             out.append(dict(d, path=self.results[p]["path"]))
+        return out
+
+    # ---- histogram free-energy surfaces (DESIGN.md 3.5h) ----
+    def _per_problem(self, value, single):
+        """value for every problem: one entry per problem (a list or tuple of P entries, each None or a valid
+        single value for its problem) or one value for all; single(p, v) tells whether v is a single value."""
+        P = len(self._probs)
+        if isinstance(value, (list, tuple)) and len(value) == P and \
+                all(v is None or single(p, v) for p, v in enumerate(value)):
+            return list(value)
+        return [value] * P
+
+    def generate_fes(self, u_n_list, x_n_list, fes_type="histogram", histogram_parameters=None):
+        """The histogram FES of the target state u_n_list[p] [N_p] over the coordinates x_n_list[p] ([N_p] or
+        [N_p, dims]) of every problem (pymbar.FES.generate_fes with fes_type="histogram"); an entry None skips its
+        problem, whose earlier surface, if any, stays.  histogram_parameters: {"bin_edges": ...} for every problem,
+        or one such dict per problem.  self.histogram_datas[p] becomes the reference's histogram_data dict.
+
+        The batched problems' f comes from one bin_moments call per wave (waves under FES_WAVE_BYTES); a problem that
+        took the single path in the solve, or whose request the batch flags, goes through fes.histogram_fes on a
+        DeviceProblem.  Every argument is checked before any device work."""
+        if fes_type != "histogram":
+            raise ParameterError(f"fes_type {fes_type!r} is not served by MbarMany: only 'histogram' surfaces are")
+        P = len(self._probs)
+        for name, v in (("u_n_list", u_n_list), ("x_n_list", x_n_list)):
+            if v is None or len(v) != P:
+                raise ParameterError(f"{name} must hold one entry (or None) per problem ({P}), got "
+                                     f"{'None' if v is None else len(v)}")
+        params = self._per_problem(histogram_parameters, lambda p, v: isinstance(v, dict))
+        reqs = {}
+        for p in range(P):
+            u, x = u_n_list[p], x_n_list[p]
+            if u is None and x is None:
+                continue
+            if u is None or x is None:
+                raise ParameterError(f"problem {p}: give both u_n and x_n, or neither")
+            par = params[p]
+            if not isinstance(par, dict) or "bin_edges" not in par:
+                raise ParameterError(f"problem {p}: histogram_parameters must be a dict with 'bin_edges', got "
+                                     f"{par!r}")
+            N = self._probs[p][0].shape[1]
+            u = np.asarray(u, dtype=np.float64)
+            if u.shape != (N,):
+                raise ParameterError(f"problem {p}: u_n has shape {u.shape}, the problem has N={N} samples")
+            if np.isnan(u).any():
+                raise ParameterError(f"problem {p}: u_n holds NaN")
+            edges = par["bin_edges"]
+            dims = len(hist._edges(edges))
+            xs = np.shape(x)
+            if not ((len(xs) == 1 and dims == 1 and xs[0] == N) or (len(xs) == 2 and xs == (N, dims))):
+                raise ParameterError(f"problem {p}: x_n has shape {xs}, the problem has N={N} samples and the bins "
+                                     f"{dims} dimension(s)")
+            data, dense, nb = hist.histogram_bins(x, edges)
+            reqs[p] = dict(u_n=u, x_n=x, edges=edges, data=data, dense=dense, nb=nb)
+        batched = [p for p in sorted(reqs) if self.results[p]["path"] == "batch" and p in self._slot]
+        single = [p for p in sorted(reqs) if p not in batched]
+        for wave in _waves(batched, lambda p: bin_bytes(*self._probs[p][0].shape, reqs[p]["nb"], False),
+                           FES_WAVE_BYTES):
+            out, flags = self._dev.bin_moments([self._slot[p] for p in wave], [self.results[p]["f_k"] for p in wave],
+                                               [reqs[p]["u_n"] for p in wave], [reqs[p]["dense"] for p in wave],
+                                               [reqs[p]["nb"] for p in wave], want_C=False)
+            self._count()
+            for p, (f_bin, _, _), flag in zip(wave, out, flags):
+                if flag:
+                    single.append(p)
+                else:
+                    reqs[p]["data"] = hist.with_bin_f(reqs[p]["data"], f_bin)
+                    reqs[p]["path"] = "batch"
+        _, Prob = _classes()
+        for p in sorted(single):
+            u_kn, N_k, _ = self._probs[p]
+            r = reqs[p]
+            try:
+                with Prob(u_kn, N_k, device=ms._DEVICE) as q:
+                    r["data"] = hist.histogram_fes(q, self.results[p]["f_k"], r["u_n"], r["x_n"], r["edges"])
+            except Exception as err:
+                raise _noted(err, p)
+            r["path"] = "single"
+        for p, r in reqs.items():
+            self.histogram_datas[p] = r["data"]
+            self._fes[p] = dict(u_n=r["u_n"], dense=r["dense"], nb=r["nb"], path=r["path"], theta=None)
+
+    def _thetas(self, problems):
+        """Theta of the augmented problem ("svd-ew", fes.py:1382-1406) of every problem of `problems` that lacks
+        one: one bin_moments call for C and D per wave of the batched ones, G from _grams; the single path
+        (fes.histogram_theta) for the rest and for flagged requests."""
+        need = [p for p in problems if self._fes[p]["theta"] is None]
+        batched = [p for p in need if self._fes[p]["path"] == "batch"]
+        single = [p for p in need if p not in batched]
+        if batched:
+            G = dict(zip(batched, self._grams(batched)))
+        for wave in _waves(batched, lambda p: bin_bytes(*self._probs[p][0].shape, self._fes[p]["nb"], True),
+                           FES_WAVE_BYTES):
+            st = [self._fes[p] for p in wave]
+            out, flags = self._dev.bin_moments([self._slot[p] for p in wave], [self.results[p]["f_k"] for p in wave],
+                                               [s["u_n"] for s in st], [s["dense"] for s in st],
+                                               [s["nb"] for s in st], want_C=True)
+            self._count()
+            for p, (_, C, D), flag in zip(wave, out, flags):
+                if flag:
+                    single.append(p)
+                else:
+                    self._fes[p]["theta"], _ = hist.augmented_theta(G[p], C, D, self._probs[p][1])
+        _, Prob = _classes()
+        for p in sorted(single):
+            u_kn, N_k, _ = self._probs[p]
+            s = self._fes[p]
+            try:
+                with Prob(u_kn, N_k, device=ms._DEVICE) as q:
+                    s["theta"] = hist.histogram_theta(q, self.results[p]["f_k"], N_k, s["u_n"],
+                                                      self.histogram_datas[p])
+            except Exception as err:
+                raise _noted(err, p)
+            s["path"] = "single"
+
+    def get_fes(self, x_list, reference_point="from-lowest", fes_reference=None, uncertainty_method=None):
+        """f_i (and df_i with uncertainty_method="analytical") of every problem's surface at the points x_list[p]
+        (pymbar.FES.get_fes of a histogram surface), plus `path`, "batch" or "single"; an entry None skips its
+        problem.  fes_reference: one point for every problem, or one per problem.  Reference points and their
+        errors are those of the reference ("from-lowest", "from-specified"; "all-differences" and
+        "from-normalization" raise what it raises).  The first "analytical" query computes Theta for every problem
+        of the call that lacks one (one bin_moments call per wave) and keeps it."""
+        if uncertainty_method not in FES_UNCERTAINTY_METHODS:
+            raise ParameterError(f"uncertainty_method {uncertainty_method!r} is not served by MbarMany's histogram "
+                                 f"FES (one of {FES_UNCERTAINTY_METHODS}); bootstrap surfaces are not served here")
+        P = len(self._probs)
+        if x_list is None or len(x_list) != P:
+            raise ParameterError(f"x_list must hold one entry (or None) per problem ({P}), got "
+                                 f"{'None' if x_list is None else len(x_list)}")
+        asked = [p for p in range(P) if x_list[p] is not None]
+        for p in asked:
+            if p not in self._fes:
+                raise ParameterError(f"problem {p}: get_fes before generate_fes built its surface")
+
+        def single_ref(p, v):
+            dims = self.histogram_datas[p]["dims"] if p in self._fes else 1
+            return np.ndim(v) == 0 if dims == 1 else (np.shape(v) == (dims,))
+
+        refs = self._per_problem(fes_reference, single_ref)
+        analytical = uncertainty_method == "analytical"
+        out = [None] * P
+        for p in asked:
+            data = self.histogram_datas[p]
+            K = self._probs[p][0].shape[0]
+
+            def df_fn(j, p=p, data=data, K=K):
+                self._thetas(asked)
+                return hist.bin_uncertainties(self._fes[p]["theta"], K, j, len(data["f"]))
+
+            r = hist.query(data, x_list[p], reference_point, refs[p], df_fn if analytical else None)
+            out[p] = dict(r, path=self._fes[p]["path"])
         return out
 
     def compute_effective_sample_number(self):

@@ -874,6 +874,45 @@ class DeviceMbarBatch(_Resident):
                                   gram=False)
         return self._requests(self._lib.mbar_b200_batch_augmented_moments, ids, f_list, Rs, want_G)
 
+    def bin_moments(self, problems, f_list, u_n_list, bin_list, nbins_list, want_C=True):
+        """Histogram FES of every request in one call (mbar_b200_batch_bin_moments): request r is problem problems[r]
+        at its converged f_list[r] [K_p], with the target state's u_n_list[r] [N_p] and dense bin indices bin_list[r]
+        [N_p] in [0, nbins_list[r]).  Returns ([(f_bin [nbins], C [K_p, nbins], D [nbins]) per request], flags
+        [n_requests] bool) with f_i = -log sum_{n in i} exp(-u_n - L_n), C_ki = sum_{n in i} W_nk w^_n,
+        D_i = sum_{n in i} w^_n^2 and w^_n = exp(-u_n - L_n + f_i), what DeviceProblem.bin_moments gives for the
+        problem.  want_C=False skips C and D: (f_bin, None, None).  A flagged request (an exponent above 700, a bin
+        without a sample of finite weight) holds no usable values."""
+        ids = np.ascontiguousarray(problems, dtype=np.int32).reshape(-1)
+        n = ids.size
+        if n == 0 or not (len(f_list) == len(u_n_list) == len(bin_list) == len(nbins_list) == n):
+            raise ValueError("need one problem, f, u_n, bin index vector and bin count per request, and at least one")
+        known = [0 <= p < self.P for p in ids]          # an unknown problem is the library's error
+        Ks = [int(self.K[p]) if ok else 0 for p, ok in zip(ids, known)]
+        us = [_f64(u) for u in u_n_list]
+        bs = [np.asarray(b) for b in bin_list]
+        for r, (u, b, p, ok) in enumerate(zip(us, bs, ids, known)):
+            N = int(self.N[p]) if ok else u.shape[0]
+            if u.shape != (N,) or b.shape != (N,):
+                raise ValueError(f"request {r}: u_n {u.shape} and bin_n {b.shape} must have shape ({N},)")
+        nb = np.ascontiguousarray(nbins_list, dtype=np.int32)
+        f = np.ascontiguousarray(np.concatenate([_f64(v, K) if ok else _f64(v) for v, K, ok in zip(f_list, Ks, known)]))
+        u = np.ascontiguousarray(np.concatenate(us))
+        b = np.ascontiguousarray(np.concatenate(bs), dtype=np.int32)
+        f_bin = np.empty(int(nb.astype(np.int64).sum()))
+        C_ = np.empty(int(np.dot(np.asarray(Ks, np.int64), nb))) if want_C else None
+        D = np.empty(f_bin.size) if want_C else None
+        flag = np.empty(n, np.int32)
+        check(self._lib.mbar_b200_batch_bin_moments(self._h, n, _i32p(ids), _dptr(f), _dptr(u), _i32p(b), _i32p(nb),
+                                                    _dptr(f_bin), _dptr(C_) if want_C else None,
+                                                    _dptr(D) if want_C else None, _i32p(flag)))
+        out, o, c = [], 0, 0
+        for K, m in zip(Ks, nb.tolist()):
+            out.append((f_bin[o:o + m], C_[c:c + K * m].reshape(K, m), D[o:o + m]) if want_C else
+                       (f_bin[o:o + m], None, None))
+            o += m
+            c += K * m
+        return out, flag.astype(bool)
+
     def _requests(self, call, ids, f_list, rows, want_G, *flags, gram=True):
         """One batched moments call on requests f_list[r] [rows[r]] at units ids[r], `flags` passed after f; one dict
         per request: S, log_S, sum_L, flag and, with want_G, G [rows[r], rows[r]].  gram=False: `call` takes no Gram
