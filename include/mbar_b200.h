@@ -502,8 +502,27 @@ int mbar_b200_batch_replicate_augmented_moments(mbar_b200_batch* batch, int32_t 
 int mbar_b200_batch_bin_moments(mbar_b200_batch* batch, int32_t n_requests, const int32_t* problem, const double* f,
                                 const double* u_n, const int32_t* bin_n, const int32_t* nbins, double* f_bin,
                                 double* C, double* D, int32_t* flag);
+/* Histogram FES of bootstrap replicates (DESIGN.md 3.5h'): the f_bin of mbar_b200_batch_bin_moments with sample n
+ * counted c_n times, for replicate slots of many problems in one call.  Target t names target_problem[t] and gives
+ * that problem's target-state u_n [N_p] and dense bin indices bin_n [N_p] in [0, nbins[t]) (u_n and bin_n
+ * concatenate the targets'); each target is uploaded once, however many requests read it.  Request r names a
+ * resident replicate slot slot[r], a target target[r] of the slot's problem and the replicate's converged f [K_p]
+ * (f concatenates the requests').  With L_n = log sum_{k sampled} N_k exp(f_k - u_kn), which keeps N_k:
+ *   f_bin [nbins of target[r]]   f_i = -log sum_{n in i} c_n exp(-u_n - L_n)
+ * concatenated by request: what DeviceProblem.set_sample_weights(c) and mbar_b200_bin_moments(want_C = 0) give.  No
+ * C and no D.  A sample with c_n = 0 enters no sum and no maximum, and its NaN L_n does not flag; all-ones counts give
+ * the bits of batch_bin_moments' f_bin.  flag[r] follows batch_bin_moments' rules over the drawn samples.  Before any
+ * device work: a slot or target out of range, a slot whose problem is not its target's, nbins < 1 or a bin index
+ * outside [0, nbins) -> MBAR_B200_ERR_INVALID, a NaN u_n -> MBAR_B200_ERR_NAN; the batch stays usable.  Five kernel
+ * launches and one synchronisation for all requests; the work split of a request depends on (N_p, K_p, nbins) alone
+ * and there are no floating-point atomics, so its results are the same bits whichever requests share the call. */
+int mbar_b200_batch_replicate_bin_moments(mbar_b200_batch* batch, int32_t n_targets, const int32_t* target_problem,
+                                          const double* u_n, const int32_t* bin_n, const int32_t* nbins,
+                                          int32_t n_requests, const int32_t* slot, const int32_t* target,
+                                          const double* f, double* f_bin, int32_t* flag);
 /* CUDA-event time of the kernels of the last batch_moments, batch_solve, batch_replicate_moments,
- * batch_solve_replicates, batch_augmented_moments, batch_replicate_augmented_moments or batch_bin_moments call, its
+ * batch_solve_replicates, batch_augmented_moments, batch_replicate_augmented_moments, batch_bin_moments or
+ * batch_replicate_bin_moments call, its
  * kernel launches, its iterations (solves) and the bytes of u_kn tiles (appended tiles, counts) its passes read. */
 int mbar_b200_last_batch_stats(mbar_b200_batch* batch, double* kernel_ms, int32_t* launches, int32_t* iterations,
                                int64_t* bytes_read);

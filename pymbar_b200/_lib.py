@@ -130,6 +130,10 @@ SIGNATURES = {
                                                               _dp, C.POINTER(C.c_int32)]),
     "mbar_b200_batch_bin_moments": (C.c_int, [_ctx, C.c_int32, C.POINTER(C.c_int32), _dp, _dp, C.POINTER(C.c_int32),
                                               C.POINTER(C.c_int32), _dp, _dp, _dp, C.POINTER(C.c_int32)]),
+    "mbar_b200_batch_replicate_bin_moments": (C.c_int, [_ctx, C.c_int32, C.POINTER(C.c_int32), _dp,
+                                                        C.POINTER(C.c_int32), C.POINTER(C.c_int32), C.c_int32,
+                                                        C.POINTER(C.c_int32), C.POINTER(C.c_int32), _dp, _dp,
+                                                        C.POINTER(C.c_int32)]),
     "mbar_b200_last_batch_stats": (C.c_int, [_ctx, _dp, C.POINTER(C.c_int32), C.POINTER(C.c_int32),
                                              C.POINTER(C.c_int64)]),
     "mbar_b200_solve_sci":(C.c_int, [_ctx, _dp, C.c_double, C.c_int32, C.POINTER(SolveResult)]),

@@ -944,6 +944,24 @@ struct BinReq {
     BinGeo geo[2];    // 0: the bin sums (one row), 1: C and D (K_p + 1 rows)
 };
 
+// L'_n = log sum_{k sampled} e^{f_k + log N_k - u'_kn} of sample n < N_p of request q (per-sample max shift)
+__device__ __forceinline__ double bin_log_denominator(const double* __restrict__ u, const BinReq& q, int64_t n,
+                                                      const double* __restrict__ fAll,
+                                                      const double* __restrict__ NkAll,
+                                                      const double* __restrict__ logNkAll) {
+    const double* ut = u + q.uoff + (n >> 5) * (int64_t)q.K * 32 + (n & 31);
+    const double* f = fAll + q.foff;
+    const double* Nk = NkAll + q.voff;
+    const double* logNk = logNkAll + q.voff;
+    double m = -INFINITY;
+    for (int k = 0; k < q.K; ++k)
+        if (Nk[k] > 0.0) m = fmax(m, f[k] + logNk[k] - __ldg(ut + k * 32));
+    double D = 0.0;
+    for (int k = 0; k < q.K; ++k)
+        if (Nk[k] > 0.0) D += exp(f[k] + logNk[k] - __ldg(ut + k * 32) - m);
+    return m + log(D);
+}
+
 // lw [slots]: u_n on entry (+inf past N_p), log w_n on exit (-inf past N_p and where u_n = +inf); Lp [slots]: L'_n.
 // A NaN log w_n (a sample whose sampled energies are all +inf) flags its request.
 __global__ void __launch_bounds__(256) batch_bin_prep_kernel(const double* __restrict__ u,
@@ -965,17 +983,7 @@ __global__ void __launch_bounds__(256) batch_bin_prep_kernel(const double* __res
         Lp[i] = 0.0;
         return;
     }
-    const double* ut = u + q.uoff + (n >> 5) * (int64_t)q.K * 32 + (n & 31);
-    const double* f = fAll + q.foff;
-    const double* Nk = NkAll + q.voff;
-    const double* logNk = logNkAll + q.voff;
-    double m = -INFINITY;
-    for (int k = 0; k < q.K; ++k)
-        if (Nk[k] > 0.0) m = fmax(m, f[k] + logNk[k] - __ldg(ut + k * 32));
-    double D = 0.0;
-    for (int k = 0; k < q.K; ++k)
-        if (Nk[k] > 0.0) D += exp(f[k] + logNk[k] - __ldg(ut + k * 32) - m);
-    const double L = m + log(D);
+    const double L = bin_log_denominator(u, q, n, fAll, NkAll, logNkAll);
     const double un = lw[i];
     // u_n = +inf: weight exactly 0, as np.exp(-inf) in the reference
     const double v = un < INFINITY ? -(un - x[q.xoff + n]) - L : -INFINITY;
@@ -984,6 +992,58 @@ __global__ void __launch_bounds__(256) batch_bin_prep_kernel(const double* __res
     if (v != v) atomicOr(&rflag[r], 1);
     const unsigned long long key = ordered_key(v);
     unsigned long long* kb = keys + q.boff + bin[i];
+    if (v > -INFINITY && key > *((volatile unsigned long long*)kb)) atomicMax(kb, key);
+}
+
+// The replicate part of a weighted request (mbar_b200_batch_replicate_bin_moments): its target's first sample in the
+// per-target u_n and bin index arrays, and its slot's first count.
+struct RepBinReq {
+    int64_t toff;
+    int64_t coff;
+};
+
+// batch_bin_prep_kernel for replicate slots.  u_n and the bin index come from the request's target (uploaded once per
+// target); lw, Lp and bin [slots] are the request's own.  A drawn sample (c_n > 0) gets
+// log w_n + log c_n (c_n = 1 adds nothing, so all-ones counts give the unweighted bits) and its bin index; an undrawn
+// one, like the padding, gets lw = -inf and bin -1, so that it enters no maximum and no sum and its L'_n is neither
+// computed nor able to flag the request.
+__global__ void __launch_bounds__(256) batch_rep_bin_prep_kernel(const double* __restrict__ u,
+                                                                 const BinReq* __restrict__ req,
+                                                                 const RepBinReq* __restrict__ rreq, int nReq,
+                                                                 int64_t slots, const double* __restrict__ fAll,
+                                                                 const double* __restrict__ NkAll,
+                                                                 const double* __restrict__ logNkAll,
+                                                                 const double* __restrict__ x,
+                                                                 const uint16_t* __restrict__ counts,
+                                                                 const double* __restrict__ ut,
+                                                                 const int* __restrict__ bt, double* __restrict__ lw,
+                                                                 double* __restrict__ Lp, int* __restrict__ bin,
+                                                                 unsigned long long* __restrict__ keys,
+                                                                 int* __restrict__ rflag) {
+    const int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= slots) return;
+    const int r = find_segment(nReq, i, [&](int s) { return req[s].soff; });
+    const BinReq& q = req[r];
+    const RepBinReq& w = rreq[r];
+    const int64_t n = i - q.soff;
+    const int c = counts[w.coff + n];                   // 0 past N_p: the slot's counts are padded to the tiles
+    if (c == 0) {
+        lw[i] = -INFINITY;
+        Lp[i] = 0.0;
+        bin[i] = -1;
+        return;
+    }
+    const double L = bin_log_denominator(u, q, n, fAll, NkAll, logNkAll);
+    const double un = ut[w.toff + n];
+    double v = un < INFINITY ? -(un - x[q.xoff + n]) - L : -INFINITY;
+    if (c != 1) v += log((double)c);
+    const int b = bt[w.toff + n];
+    Lp[i] = L;
+    lw[i] = v;
+    bin[i] = b;
+    if (v != v) atomicOr(&rflag[r], 1);
+    const unsigned long long key = ordered_key(v);
+    unsigned long long* kb = keys + q.boff + b;
     if (v > -INFINITY && key > *((volatile unsigned long long*)kb)) atomicMax(kb, key);
 }
 
@@ -1472,6 +1532,163 @@ int mbar_b200_batch_bin_moments(mbar_b200_batch* b, int32_t n, const int32_t* pr
         if (D) std::memcpy(D + q.boff, o + (size_t)q.K * q.nbins, (size_t)q.nbins * sizeof(double));
         co += (int64_t)q.K * q.nbins;
     }
+    return MBAR_B200_OK;
+}
+
+int mbar_b200_batch_replicate_bin_moments(mbar_b200_batch* b, int32_t n_targets, const int32_t* target_problem,
+                                          const double* u_n, const int32_t* bin_n, const int32_t* nbins,
+                                          int32_t n, const int32_t* slot, const int32_t* target, const double* f,
+                                          double* f_bin, int32_t* flag) {
+    MBAR_REQUIRE(b, MBAR_B200_ERR_INVALID, "batch_replicate_bin_moments: NULL object");
+    MBAR_REQUIRE(n_targets >= 1 && target_problem && u_n && bin_n && nbins, MBAR_B200_ERR_INVALID,
+                 "batch_replicate_bin_moments: %d targets or a NULL argument", (int)n_targets);
+    MBAR_REQUIRE(n >= 1 && slot && target && f && f_bin && flag, MBAR_B200_ERR_INVALID,
+                 "batch_replicate_bin_moments: %d requests or a NULL argument", (int)n);
+    // targets: u_n and bin indices, each padded to its problem's tiles
+    std::vector<int64_t> toff((size_t)n_targets);
+    int64_t tslots = 0, src = 0;
+    for (int t = 0; t < n_targets; ++t) {
+        const int p = target_problem[t];
+        MBAR_REQUIRE(p >= 0 && p < b->P, MBAR_B200_ERR_INVALID,
+                     "batch_replicate_bin_moments: target %d names problem %d of %d", t, p, b->P);
+        MBAR_REQUIRE(nbins[t] >= 1, MBAR_B200_ERR_INVALID, "batch_replicate_bin_moments: target %d has nbins = %d",
+                     t, (int)nbins[t]);
+        for (int64_t i = 0; i < b->N[p]; ++i)
+            MBAR_REQUIRE(bin_n[src + i] >= 0 && bin_n[src + i] < nbins[t], MBAR_B200_ERR_INVALID,
+                         "batch_replicate_bin_moments: target %d: bin index %d of sample %lld lies outside [0, %d)",
+                         t, (int)bin_n[src + i], (long long)i, (int)nbins[t]);
+        toff[t] = tslots;
+        tslots += b->nT[p] * 32;
+        src += b->N[p];
+    }
+    for (int64_t i = 0; i < src; ++i)
+        MBAR_REQUIRE(u_n[i] == u_n[i], MBAR_B200_ERR_NAN, "batch_replicate_bin_moments: NaN in u_n (entry %lld)",
+                     (long long)i);
+    std::vector<BinReq> req((size_t)n);
+    std::vector<RepBinReq> rreq((size_t)n);
+    std::vector<int64_t> tile0((size_t)b->P, 0);  // first tile of each problem: indexes x_n
+    for (int p = 1; p < b->P; ++p) tile0[p] = tile0[p - 1] + b->nT[p - 1];
+    int64_t slots = 0, bins = 0, fs = 0, items = 0, parts = 0, bytes = 0;
+    for (int r = 0; r < n; ++r) {
+        const int s = slot[r], t = target[r];
+        MBAR_REQUIRE(s >= 0 && s < b->nSlots, MBAR_B200_ERR_INVALID,
+                     "batch_replicate_bin_moments: request %d names slot %d of %d", r, s, b->nSlots);
+        MBAR_REQUIRE(t >= 0 && t < n_targets, MBAR_B200_ERR_INVALID,
+                     "batch_replicate_bin_moments: request %d names target %d of %d", r, t, (int)n_targets);
+        const int p = b->slotProb[s];
+        MBAR_REQUIRE(target_problem[t] == p, MBAR_B200_ERR_INVALID,
+                     "batch_replicate_bin_moments: request %d: slot %d is of problem %d, target %d of problem %d", r,
+                     s, p, t, (int)target_problem[t]);
+        BinReq& q = req[r];
+        q = BinReq{};
+        q.K = b->K[p];
+        q.nbins = nbins[t];
+        q.N = b->N[p];
+        q.nT = b->nT[p];
+        q.uoff = b->uoff[p];
+        q.voff = b->voff[p];
+        q.xoff = tile0[p] * 32;
+        q.soff = slots;
+        q.boff = bins;
+        q.foff = fs;
+        BinGeo& g = q.geo[0];
+        g = bin_geometry(q.nT, 1, q.nbins);
+        g.item0 = items;
+        g.poff = parts;
+        items += (int64_t)g.nbc * g.nsc;
+        parts += (int64_t)g.nsc * q.nbins;
+        rreq[r] = RepBinReq{toff[t], b->slotCoff[s]};
+        bytes += q.nT * 32 * ((int64_t)q.K * 8 + 2);     // the prep pass: tiles and counts
+        slots += q.nT * 32;
+        bins += q.nbins;
+        fs += q.K;
+    }
+    MBAR_REQUIRE(items < INT32_MAX, MBAR_B200_ERR_INVALID, "batch_replicate_bin_moments: %lld work items in one call",
+                 (long long)items);
+    MBAR_CUDA(cudaSetDevice(b->device));
+    NvtxRange nvtx_("mbar_b200::batch_replicate_bin_moments");
+    b->lastLaunches = 0;
+    b->lastBytes = 0;
+    b->lastIterations = 0;
+    // pinned staging: f, the targets' u_n padded with +inf and the requests; the targets' bin indices padded with -1
+    const size_t reqDoubles = ((size_t)n * sizeof(BinReq) + 7) / 8;
+    const size_t rreqDoubles = ((size_t)n * sizeof(RepBinReq) + 7) / 8;
+    MBAR_TRY(b->h_f.grow((size_t)fs + (size_t)tslots + reqDoubles + rreqDoubles, "batch_replicate_bin_moments"));
+    MBAR_TRY(b->h_bin.grow((size_t)tslots, "batch_replicate_bin_moments"));
+    std::memcpy(b->h_f, f, (size_t)fs * sizeof(double));
+    double* hu = b->h_f + fs;
+    src = 0;
+    for (int t = 0; t < n_targets; ++t) {
+        const int p = target_problem[t];
+        std::memcpy(hu + toff[t], u_n + src, (size_t)b->N[p] * sizeof(double));
+        std::memcpy(b->h_bin + toff[t], bin_n + src, (size_t)b->N[p] * sizeof(int32_t));
+        for (int64_t i = b->N[p]; i < b->nT[p] * 32; ++i) {
+            hu[toff[t] + i] = INFINITY;
+            b->h_bin[toff[t] + i] = -1;
+        }
+        src += b->N[p];
+    }
+    BinReq* hreq = reinterpret_cast<BinReq*>(b->h_f + fs + tslots);
+    std::memcpy(hreq, req.data(), req.size() * sizeof(BinReq));
+    RepBinReq* hrreq = reinterpret_cast<RepBinReq*>(b->h_f + fs + tslots + reqDoubles);
+    std::memcpy(hrreq, rreq.data(), rreq.size() * sizeof(RepBinReq));
+    CallBuffers buf("batch_replicate_bin_moments");
+    BinReq* d_req;
+    RepBinReq* d_rreq;
+    int *d_bt, *d_bin, *d_rflag;
+    double *d_f, *d_ut, *d_lw, *d_Lp, *d_m, *d_o, *d_s, *d_fbin, *d_part;
+    unsigned long long* d_keys;
+    MBAR_TRY(buf.alloc(&d_req, (size_t)n));
+    MBAR_TRY(buf.alloc(&d_rreq, (size_t)n));
+    MBAR_TRY(buf.alloc(&d_f, (size_t)fs));
+    MBAR_TRY(buf.alloc(&d_ut, (size_t)tslots));
+    MBAR_TRY(buf.alloc(&d_bt, (size_t)tslots));
+    MBAR_TRY(buf.alloc(&d_lw, (size_t)slots));
+    MBAR_TRY(buf.alloc(&d_Lp, (size_t)slots));
+    MBAR_TRY(buf.alloc(&d_bin, (size_t)slots));
+    MBAR_TRY(buf.alloc(&d_keys, (size_t)bins));
+    MBAR_TRY(buf.alloc(&d_m, (size_t)bins));
+    MBAR_TRY(buf.alloc(&d_o, (size_t)bins));
+    MBAR_TRY(buf.alloc(&d_s, (size_t)bins));
+    MBAR_TRY(buf.alloc(&d_fbin, (size_t)bins));
+    MBAR_TRY(buf.alloc(&d_part, (size_t)parts));
+    MBAR_TRY(buf.alloc(&d_rflag, (size_t)n));
+    cudaStream_t st = b->stream;
+    MBAR_CUDA(cudaMemcpyAsync(d_f, b->h_f, (size_t)fs * sizeof(double), cudaMemcpyHostToDevice, st));
+    MBAR_CUDA(cudaMemcpyAsync(d_ut, hu, (size_t)tslots * sizeof(double), cudaMemcpyHostToDevice, st));
+    MBAR_CUDA(cudaMemcpyAsync(d_bt, b->h_bin, (size_t)tslots * sizeof(int32_t), cudaMemcpyHostToDevice, st));
+    MBAR_CUDA(cudaMemcpyAsync(d_req, hreq, req.size() * sizeof(BinReq), cudaMemcpyHostToDevice, st));
+    MBAR_CUDA(cudaMemcpyAsync(d_rreq, hrreq, rreq.size() * sizeof(RepBinReq), cudaMemcpyHostToDevice, st));
+    MBAR_CUDA(cudaMemsetAsync(d_keys, 0, (size_t)bins * sizeof(unsigned long long), st));
+    MBAR_CUDA(cudaMemsetAsync(d_rflag, 0, (size_t)n * sizeof(int), st));
+    const size_t smem0 = (size_t)BB_ACC_DOUBLES * sizeof(double);
+    MBAR_CUDA(cudaFuncSetAttribute(batch_bin_accum_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                   (int)smem0));
+    MBAR_CUDA(cudaFuncSetAttribute(batch_bin_accum_kernel<false>, cudaFuncAttributePreferredSharedMemoryCarveout, 100));
+    size_t smemS = 0;
+    for (const BinReq& q : req) smemS = std::max(smemS, (size_t)q.geo[0].BC * sizeof(double));
+    MBAR_CUDA(cudaEventRecord(b->ev0, st));
+    batch_rep_bin_prep_kernel<<<(unsigned)((slots + 255) / 256), 256, 0, st>>>(
+        b->d_u, d_req, d_rreq, n, slots, d_f, b->d_Nk, b->d_logNk, b->d_x, b->d_counts, d_ut, d_bt, d_lw, d_Lp, d_bin,
+        d_keys, d_rflag);
+    batch_bin_max_kernel<<<(unsigned)((bins + 255) / 256), 256, 0, st>>>(d_req, n, bins, d_keys, d_m, d_o, d_rflag);
+    batch_bin_accum_kernel<false><<<(unsigned)items, BB_THREADS, smemS, st>>>(b->d_u, d_req, n, d_f, d_lw, d_Lp, d_bin,
+                                                                              d_o, d_part, d_rflag);
+    batch_bin_reduce_kernel<false><<<(unsigned)((bins + 255) / 256), 256, 0, st>>>(d_req, n, bins, d_part, d_s);
+    batch_bin_f_kernel<<<(unsigned)((bins + 255) / 256), 256, 0, st>>>(d_req, n, bins, d_m, d_s, d_fbin, d_o, d_rflag);
+    MBAR_CUDA(cudaGetLastError());
+    MBAR_CUDA(cudaEventRecord(b->ev1, st));
+    MBAR_TRY(b->h_out.grow((size_t)bins, "batch_replicate_bin_moments"));
+    std::vector<int> hflag((size_t)n);
+    MBAR_CUDA(cudaMemcpyAsync(b->h_out, d_fbin, (size_t)bins * sizeof(double), cudaMemcpyDeviceToHost, st));
+    MBAR_CUDA(cudaMemcpyAsync(hflag.data(), d_rflag, (size_t)n * sizeof(int), cudaMemcpyDeviceToHost, st));
+    MBAR_CUDA(cudaStreamSynchronize(st));
+    float ms = 0.f;
+    b->lastMs = event_ms(b->ev0, b->ev1, &ms) ? ms : 0.0;
+    b->lastLaunches = 5;
+    b->lastBytes = bytes;
+    std::memcpy(f_bin, b->h_out, (size_t)bins * sizeof(double));
+    for (int r = 0; r < n; ++r) flag[r] = hflag[r] != 0;
     return MBAR_B200_OK;
 }
 

@@ -47,6 +47,7 @@ from . import bootstrap
 from . import estimators
 from . import expectations as ex
 from . import fes as hist
+from . import fes_bootstrap as fb
 from . import mbar_solvers as ms
 from .utils import ParameterError
 
@@ -61,7 +62,7 @@ MAX_BATCH_ROWS = 192        # DeviceMbarBatch.MAX_ROWS: K_p plus appended rows o
 AUG_WAVE_BYTES = 2 << 30    # device footprint of one wave of appended rows
 ESTIMATOR_METHODS = (None, "svd-ew", "approximate", "bootstrap")
 FES_WAVE_BYTES = 2 << 30    # device footprint of one wave of histogram FES requests
-FES_UNCERTAINTY_METHODS = (None, "analytical")
+FES_UNCERTAINTY_METHODS = (None, "analytical", "bootstrap")
 
 
 def _classes():
@@ -178,6 +179,15 @@ def bin_bytes(K, N, nbins, want_C):
     return 20 * nT * 32 + 40 * nbins + 8 * parts + (8 * (K + 1) * nbins if want_C else 0) + 8 * K + 164
 
 
+def rep_bin_bytes(K, N, nbins):
+    """Device bytes of one replicate histogram request in a wave, beyond its slot (slot_bytes): its log w_n, L_n and
+    bin slots, the per-bin arrays, the partials of its bin-sum pass, its f and its request records (batch.cu's
+    geometry), plus its target's u_n and bin index, counted with every slot as an upper bound."""
+    nT = -(-int(N) // 32)
+    K, nbins = int(K), int(nbins)
+    return 32 * nT * 32 + 40 * nbins + 8 * _bin_geometry(nT, 1, nbins)[2] * nbins + 8 * K + 180
+
+
 def _waves(items, need, limit):
     """items split, in order, into waves whose need(item) sum stays under limit (one item at least per wave)."""
     waves, wave, used = [], [], 0
@@ -197,6 +207,27 @@ def _noted(err, p):
     """err with a note naming problem p, for errors of the single path."""
     err.add_note(f"raised for problem {p} (MbarMany histogram FES, single path)")
     return err
+
+
+def _validate_fes_boot(n_bootstraps, seed, P):
+    """The n_bootstraps rule of pymbar.FES.generate_fes (fes.py:357-360: an integer, 0 or >= 2; ValueError otherwise)
+    and seed: None, or one entry per problem, each an int >= 0, -1 or None."""
+    if not np.issubdtype(type(n_bootstraps), np.integer) or n_bootstraps == 1 or n_bootstraps < 0:
+        raise ValueError(f"n_bootstraps must be an integer of 0 or >=2, it was set to {n_bootstraps}")
+    if seed is None:
+        return [None] * P
+    if np.ndim(seed) != 1:
+        raise ParameterError("seed must be None or one seed per problem: a single seed would give every problem "
+                             "with the same N_k identical replicates")
+    if len(seed) != P:
+        raise ParameterError(f"seed must hold one entry per problem ({P}), got {len(seed)}")
+    out = []
+    for p, v in enumerate(seed):
+        ok = v is None or (np.issubdtype(type(v), np.integer) and (v >= 0 or v == -1))
+        if not ok:
+            raise ParameterError(f"problem {p}: seed must be an int >= 0, -1 or None, got {v!r}")
+        out.append(None if v is None or v < 0 else int(v))
+    return out
 
 
 def _validate_boot(n_bootstraps, rseed, P):
@@ -248,6 +279,25 @@ def _single_replicates(u_kn, N_k, f_k, rints, protocol):
                                        solver_protocol=protocol)
 
 
+def _solve_slots(dev, problems, counts, f_starts, tol, opts):
+    """Replicate slots of a wave (slot s: problem problems[s] of the batch with multiplicities counts[s]) solved in
+    lockstep from f_starts[s] with the adaptive stage, then one weighted all-rows moments call for the all-state update
+    and the gauge f[0] = 0, as bootstrap.bootstrap_f_k does: {s: f [K]} for the slots whose solve converged and whose
+    update is not flagged.  The slots stay resident for the caller's next request."""
+    dev.set_replicates(problems, counts)
+    f_list, status, _ = dev.solve_replicates(f_starts, tol=tol, maxiter=int(opts["maxiter"]),
+                                             min_sc_iter=int(opts["min_sc_iter"]), gamma=float(opts["gamma"]))
+    ok = [s for s in range(len(f_starts)) if status[s] == 0]
+    out = {}
+    if ok:
+        sums = dev.moments([f_list[s] for s in ok], all_rows=True, slots=ok)
+        for s, m in zip(ok, sums):
+            if not m["flag"]:
+                f = f_list[s] - m["log_S"]
+                out[s] = f - f[0]
+    return out
+
+
 def _bootstraps(dev, batch, probs, f_main, seeds, B, tol, opts):
     """(f_k_boots [P][B, K], boot_single [P], draws [P], overflow) of every problem; dev holds the problems `batch`
     (None if none).  draws[p] keeps the generator state before each of problem p's replicates; overflow is the set of
@@ -290,22 +340,14 @@ def _bootstraps(dev, batch, probs, f_main, seeds, B, tol, opts):
         first = {}
         for k, (p, b) in enumerate(wave):
             first.setdefault(p, k)
-        dev.set_replicates([slot_of[p] for p, _ in slots], [counts[p][b - wave[first[p]][1]] for p, b in slots])
-        f_list, status, _ = dev.solve_replicates([f_main[p] for p, _ in slots], tol=tol, maxiter=int(opts["maxiter"]),
-                                                 min_sc_iter=int(opts["min_sc_iter"]), gamma=float(opts["gamma"]))
-        ok = [s for s in range(len(slots)) if status[s] == 0]
-        for s in range(len(slots)):
-            if status[s] != 0:
-                single[slots[s][0]].add(slots[s][1])
-        if ok:
-            sums = dev.moments([f_list[s] for s in ok], all_rows=True, slots=ok)
-            for s, m in zip(ok, sums):
-                p, b = slots[s]
-                if m["flag"]:
-                    single[p].add(b)
-                    continue
-                f = f_list[s] - m["log_S"]
-                boots[p][b] = f - f[0]
+        got = _solve_slots(dev, [slot_of[p] for p, _ in slots],
+                           [counts[p][b - wave[first[p]][1]] for p, b in slots], [f_main[p] for p, _ in slots], tol,
+                           opts)
+        for s, (p, b) in enumerate(slots):
+            if s in got:
+                boots[p][b] = got[s]
+            else:
+                single[p].add(b)
     for p in overflow:
         single[p] = set(range(B))
     protocol = (dict(method="adaptive", tol=tol, options=dict(min_sc_iter=int(opts["min_sc_iter"]),
@@ -389,9 +431,13 @@ class MbarMany:
         self._draws = []             # problem -> its _Draws (n_bootstraps > 0): replicate counts are regenerated
         self._overflow = set()       # problems whose replicate multiplicities overflow uint16
         self.histogram_datas = [None] * P    # problem -> the reference's histogram_data dict (generate_fes)
+        self.replicate_histogram_datas = [None] * P  # problem -> its B ReplicateHistograms (generate_fes, B >= 2)
+        self.fes_boot_single = [0] * P       # problem -> how many of those replicates took the single path
+        self._tol, self._opts = solver_tolerance, opts
         self._fes = {}                       # problem -> its histogram request, path and cached Theta
         self.device_stats = dict(ms=0.0, launches=0, calls=0, bytes_read=0)
-        self.host_stats = dict(counts_s=0.0)     # host time spent regenerating replicate counts for the estimators
+        # host time spent regenerating replicate counts for the estimators, and drawing bootstrap surfaces' replicates
+        self.host_stats = dict(counts_s=0.0, fes_draws_s=0.0)
         try:
             self.results = self._solve(probs, seeds, B, compute_uncertainty, uncertainty_method, return_theta,
                                        solver_tolerance, opts)
@@ -787,7 +833,8 @@ class MbarMany:
             return list(value)
         return [value] * P
 
-    def generate_fes(self, u_n_list, x_n_list, fes_type="histogram", histogram_parameters=None):
+    def generate_fes(self, u_n_list, x_n_list, fes_type="histogram", histogram_parameters=None, n_bootstraps=0,
+                     seed=None):
         """The histogram FES of the target state u_n_list[p] [N_p] over the coordinates x_n_list[p] ([N_p] or
         [N_p, dims]) of every problem (pymbar.FES.generate_fes with fes_type="histogram"); an entry None skips its
         problem, whose earlier surface, if any, stays.  histogram_parameters: {"bin_edges": ...} for every problem,
@@ -795,10 +842,22 @@ class MbarMany:
 
         The batched problems' f comes from one bin_moments call per wave (waves under FES_WAVE_BYTES); a problem that
         took the single path in the solve, or whose request the batch flags, goes through fes.histogram_fes on a
-        DeviceProblem.  Every argument is checked before any device work."""
+        DeviceProblem.  Every argument is checked before any device work.
+
+        n_bootstraps = B >= 2 (DESIGN.md 3.5h') also builds B bootstrap replicates of every requested surface:
+        self.replicate_histogram_datas[p] becomes the reference's FES.histogram_datas, B ReplicateHistograms, and
+        self.fes_boot_single[p] counts those that took the single path.  Replicate b of problem p is the one
+        pymbar.FES(u_kn_p, N_k_p).generate_fes(..., n_bootstraps=B, seed=seed[p]) draws from numpy's global
+        generator; problems draw in increasing order, and the generator ends where P such calls leave it.  seed: None
+        (continue the global stream) or one entry per problem, an int >= 0 (np.random.seed before the problem's
+        draws), -1 or None.  With B = 0 the generator is not touched and replicate_histogram_datas[p] becomes None.
+        A problem with an empty state, or a replicate that draws no sample from a bin tuple of the surface, raises
+        ParameterError; a call that raises restores the generator and changes no surface."""
         if fes_type != "histogram":
             raise ParameterError(f"fes_type {fes_type!r} is not served by MbarMany: only 'histogram' surfaces are")
         P = len(self._probs)
+        seeds = _validate_fes_boot(n_bootstraps, seed, P)
+        B = int(n_bootstraps)
         for name, v in (("u_n_list", u_n_list), ("x_n_list", x_n_list)):
             if v is None or len(v) != P:
                 raise ParameterError(f"{name} must hold one entry (or None) per problem ({P}), got "
@@ -827,6 +886,9 @@ class MbarMany:
             if not ((len(xs) == 1 and dims == 1 and xs[0] == N) or (len(xs) == 2 and xs == (N, dims))):
                 raise ParameterError(f"problem {p}: x_n has shape {xs}, the problem has N={N} samples and the bins "
                                      f"{dims} dimension(s)")
+            if B > 0 and np.any(np.asarray(self._probs[p][1]) == 0):
+                raise ParameterError(f"problem {p}: a state without samples cannot be resampled for bootstrap "
+                                     f"surfaces")
             data, dense, nb = hist.histogram_bins(x, edges)
             reqs[p] = dict(u_n=u, x_n=x, edges=edges, data=data, dense=dense, nb=nb)
         batched = [p for p in sorted(reqs) if self.results[p]["path"] == "batch" and p in self._slot]
@@ -853,9 +915,119 @@ class MbarMany:
             except Exception as err:
                 raise _noted(err, p)
             r["path"] = "single"
+        reps, nsingle = {}, {}
+        if B > 0:
+            state = np.random.get_state()
+            try:
+                reps, nsingle = self._fes_replicates(reqs, B, seeds)
+            except BaseException:
+                np.random.set_state(state)
+                raise
         for p, r in reqs.items():
             self.histogram_datas[p] = r["data"]
             self._fes[p] = dict(u_n=r["u_n"], dense=r["dense"], nb=r["nb"], path=r["path"], theta=None)
+            self.replicate_histogram_datas[p] = reps.get(p)
+            self.fes_boot_single[p] = nsingle.get(p, 0)
+
+    def _fes_replicates(self, reqs, B, seeds):
+        """({p: [B ReplicateHistogram]}, {p: replicates on the single path}) of every request of generate_fes, drawn
+        from numpy's global generator in problem order.  The (problem, replicate) pairs of problems whose b = 0
+        request took the batch path are drawn and evaluated one wave at a time under BOOT_WAVE_BYTES: _solve_slots,
+        then one replicate_bin_moments call on the same resident slots, each problem's target uploaded once.  The
+        others, and replicates the batch does not serve, go through fes_bootstrap.histogram_replicates."""
+        probs, dev = self._probs, self._dev
+        reps = {p: [None] * B for p in reqs}
+        states = {p: [None] * B for p in reqs}
+        single = {p: set() for p in reqs}
+        overflow = set()
+        wave, used = [], 0
+
+        def flush():
+            nonlocal wave, used
+            if wave:
+                self._fes_wave(wave, reqs, reps, single)
+            wave, used = [], 0
+
+        for p in sorted(reqs):
+            r = reqs[p]
+            N_k = np.asarray(probs[p][1]).astype(np.int64)
+            N = int(N_k.sum())
+            tuples, n_tuples = fb.tuple_index(r["data"]["bin_n"])
+            batched = r["path"] == "batch"
+            need = slot_bytes(*probs[p][0].shape) + rep_bin_bytes(*probs[p][0].shape, r["nb"])
+            if seeds[p] is not None:
+                np.random.seed(seeds[p])
+            for b in range(B):
+                t0 = time.perf_counter()
+                drawn = []
+                states[p][b] = fb.draw_replicates(N_k, 1, lambda _, idx: drawn.append(idx))[0]
+                idx = drawn[0]
+                covered = fb.covers_every_tuple(idx, tuples, n_tuples)
+                c = np.bincount(idx, minlength=N) if batched and p not in overflow else None
+                self.host_stats["fes_draws_s"] += time.perf_counter() - t0
+                if not covered:
+                    raise ParameterError(f"problem {p}: bootstrap replicate {b} draws no sample from a bin of the "
+                                         f"surface, so its histogram has fewer bins than the surface")
+                if c is None:
+                    continue
+                if c.max() > 65535:
+                    overflow.add(p)
+                    continue
+                if wave and used + need > BOOT_WAVE_BYTES:
+                    flush()
+                wave.append((p, b, c.astype(np.uint16), states[p][b]))
+                used += need
+        flush()
+        if any(r["path"] == "batch" for r in reqs.values()):
+            dev.set_replicates([], [])
+        _, Prob = _classes()
+        protocol = tuple(dict(st, tol=self._tol) for st in fb.solver_protocol(ms.DEFAULT_SOLVER_PROTOCOL))
+        for p in sorted(reqs):
+            r = reqs[p]
+            picked = list(range(B)) if r["path"] != "batch" or p in overflow else sorted(single[p])
+            if not picked:
+                continue
+            u_kn, N_k, _ = probs[p]
+            try:
+                with Prob(u_kn, N_k, device=ms._DEVICE) as q:
+                    got = fb.histogram_replicates(q, self.results[p]["f_k"], np.asarray(N_k).astype(np.int64),
+                                                  r["u_n"], r["data"], [states[p][b] for b in picked], protocol)
+            except Exception as err:
+                raise _noted(err, p)
+            for b, h in zip(picked, got):
+                reps[p][b] = h
+            single[p] = set(picked)
+        return reps, {p: len(single[p]) for p in reqs}
+
+    def _fes_wave(self, wave, reqs, reps, single):
+        """One wave of (problem, replicate, counts, generator state): the replicates solved on resident slots
+        (_solve_slots) and binned by one replicate_bin_moments call on those slots; replicates either step does not
+        serve go to single."""
+        dev = self._dev
+        got = _solve_slots(dev, [self._slot[p] for p, _, _, _ in wave], [c for _, _, c, _ in wave],
+                           [self.results[p]["f_k"] for p, _, _, _ in wave], self._tol, self._opts)
+        ok = [s for s in range(len(wave)) if s in got]
+        for s in range(len(wave)):
+            if s not in got:
+                single[wave[s][0]].add(wave[s][1])
+        if not ok:
+            return
+        targets = list(dict.fromkeys(wave[s][0] for s in ok))
+        tix = {p: t for t, p in enumerate(targets)}
+        f_bins, flags = dev.replicate_bin_moments([self._slot[p] for p in targets], [reqs[p]["u_n"] for p in targets],
+                                                  [reqs[p]["dense"] for p in targets],
+                                                  [reqs[p]["nb"] for p in targets], ok,
+                                                  [tix[wave[s][0]] for s in ok], [got[s] for s in ok])
+        self._count()
+        for s, f_bin, flag in zip(ok, f_bins, flags):
+            p, b, _, state = wave[s]
+            if flag:
+                single[p].add(b)
+                continue
+            base = reqs[p]["data"]
+            f = np.zeros(len(base["f"]))
+            f[:reqs[p]["nb"]] = f_bin
+            reps[p][b] = fb.ReplicateHistogram(f, base, state, np.asarray(self._probs[p][1]).astype(np.int64))
 
     def _thetas(self, problems):
         """Theta of the augmented problem ("svd-ew", fes.py:1382-1406) of every problem of `problems` that lacks
@@ -891,15 +1063,16 @@ class MbarMany:
             s["path"] = "single"
 
     def get_fes(self, x_list, reference_point="from-lowest", fes_reference=None, uncertainty_method=None):
-        """f_i (and df_i with uncertainty_method="analytical") of every problem's surface at the points x_list[p]
-        (pymbar.FES.get_fes of a histogram surface), plus `path`, "batch" or "single"; an entry None skips its
-        problem.  fes_reference: one point for every problem, or one per problem.  Reference points and their
+        """f_i (and df_i with uncertainty_method="analytical" or "bootstrap") of every problem's surface at the points
+        x_list[p] (pymbar.FES.get_fes of a histogram surface), plus `path`, "batch" or "single"; an entry None skips
+        its problem.  fes_reference: one point for every problem, or one per problem.  Reference points and their
         errors are those of the reference ("from-lowest", "from-specified"; "all-differences" and
         "from-normalization" raise what it raises).  The first "analytical" query computes Theta for every problem
-        of the call that lacks one (one bin_moments call per wave) and keeps it."""
+        of the call that lacks one (one bin_moments call per wave) and keeps it.  "bootstrap" takes df_i from the
+        replicates of generate_fes(..., n_bootstraps=B) (fes.py:1417-1422), with no device work."""
         if uncertainty_method not in FES_UNCERTAINTY_METHODS:
             raise ParameterError(f"uncertainty_method {uncertainty_method!r} is not served by MbarMany's histogram "
-                                 f"FES (one of {FES_UNCERTAINTY_METHODS}); bootstrap surfaces are not served here")
+                                 f"FES (one of {FES_UNCERTAINTY_METHODS})")
         P = len(self._probs)
         if x_list is None or len(x_list) != P:
             raise ParameterError(f"x_list must hold one entry (or None) per problem ({P}), got "
@@ -908,6 +1081,9 @@ class MbarMany:
         for p in asked:
             if p not in self._fes:
                 raise ParameterError(f"problem {p}: get_fes before generate_fes built its surface")
+            if uncertainty_method == "bootstrap" and self.replicate_histogram_datas[p] is None:
+                raise ParameterError(f"problem {p}: Can't calculate uncertainties via bootstrap if bootstrapping was "
+                                     f"not performed when running get_fes")
 
         def single_ref(p, v):
             dims = self.histogram_datas[p]["dims"] if p in self._fes else 1
@@ -924,7 +1100,11 @@ class MbarMany:
                 self._thetas(asked)
                 return hist.bin_uncertainties(self._fes[p]["theta"], K, j, len(data["f"]))
 
-            r = hist.query(data, x_list[p], reference_point, refs[p], df_fn if analytical else None)
+            def boot_fn(j, p=p, data=data):
+                return fb.bootstrap_df(self.replicate_histogram_datas[p], j, len(data["f"]))
+
+            fn = df_fn if analytical else (boot_fn if uncertainty_method == "bootstrap" else None)
+            r = hist.query(data, x_list[p], reference_point, refs[p], fn)
             out[p] = dict(r, path=self._fes[p]["path"])
         return out
 

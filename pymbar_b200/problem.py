@@ -913,6 +913,39 @@ class DeviceMbarBatch(_Resident):
             c += K * m
         return out, flag.astype(bool)
 
+    def replicate_bin_moments(self, target_problems, u_n_list, bin_list, nbins_list, slots, targets, f_list):
+        """Histogram FES of replicate slots in one call (mbar_b200_batch_replicate_bin_moments).  Target t is problem
+        target_problems[t] with the target state's u_n_list[t] [N_p] and dense bin indices bin_list[t] [N_p] in
+        [0, nbins_list[t]), uploaded once; request r is slot slots[r] at its replicate's converged f_list[r] [K_p]
+        against target targets[r] of the slot's problem.  Returns ([f_bin [nbins]] per request, flags bool) with
+        f_i = -log sum_{n in i} c_n exp(-u_n - L_n), L_n keeping N_k: what set_sample_weights(c) and
+        DeviceProblem.bin_moments(want_C=False) give.  A flagged request holds no usable values."""
+        tp = np.ascontiguousarray(target_problems, dtype=np.int32).reshape(-1)
+        if tp.size == 0 or not (len(u_n_list) == len(bin_list) == len(nbins_list) == tp.size):
+            raise ValueError("need one problem, u_n, bin index vector and bin count per target, and at least one")
+        sl = np.ascontiguousarray(slots, dtype=np.int32).reshape(-1)
+        tg = np.ascontiguousarray(targets, dtype=np.int32).reshape(-1)
+        if sl.size == 0 or not (tg.size == len(f_list) == sl.size):
+            raise ValueError("need one slot, target and f vector per request, and at least one")
+        us = [_f64(u) for u in u_n_list]
+        bs = [np.asarray(b) for b in bin_list]
+        for t, (u, b, p) in enumerate(zip(us, bs, tp)):
+            N = int(self.N[p]) if 0 <= p < self.P else u.shape[0]   # an unknown problem is the library's error
+            if u.shape != (N,) or b.shape != (N,):
+                raise ValueError(f"target {t}: u_n {u.shape} and bin_n {b.shape} must have shape ({N},)")
+        nb = np.ascontiguousarray(nbins_list, dtype=np.int32)
+        owner = self.slot_problems
+        Ks = [int(self.K[owner[s]]) if 0 <= s < len(owner) else None for s in sl]
+        f = np.ascontiguousarray(np.concatenate([_f64(v) if K is None else _f64(v, K) for v, K in zip(f_list, Ks)]))
+        out_nb = [int(nb[t]) if 0 <= t < nb.size else 0 for t in tg]
+        f_bin = np.empty(sum(out_nb))
+        flag = np.empty(sl.size, np.int32)
+        check(self._lib.mbar_b200_batch_replicate_bin_moments(
+            self._h, tp.size, _i32p(tp), _dptr(np.ascontiguousarray(np.concatenate(us))),
+            _i32p(np.ascontiguousarray(np.concatenate(bs), dtype=np.int32)), _i32p(nb), sl.size, _i32p(sl), _i32p(tg),
+            _dptr(f), _dptr(f_bin), _i32p(flag)))
+        return np.split(f_bin, np.cumsum(out_nb)[:-1]), flag.astype(bool)
+
     def _requests(self, call, ids, f_list, rows, want_G, *flags, gram=True):
         """One batched moments call on requests f_list[r] [rows[r]] at units ids[r], `flags` passed after f; one dict
         per request: S, log_S, sum_L, flag and, with want_G, G [rows[r], rows[r]].  gram=False: `call` takes no Gram
