@@ -274,6 +274,28 @@ int mbar_b200_kde_log_sum_replicates(mbar_b200_kde* kde, int32_t kernel, double 
 /* CUDA-event time of the kernels of the last mbar_b200_kde_log_sum or mbar_b200_kde_log_sum_replicates, and the number
  * of sample chunks they split N into. */
 int mbar_b200_last_kde_stats(mbar_b200_kde* kde, double* ms, int32_t* chunks);
+/* Many sample sets in one object (DESIGN.md 3.5h''): KDE surfaces of many small problems, and every bootstrap
+ * replicate of each, scored in one call.  Only the coordinates are resident; the weights travel with each request.
+ * Set s holds N[s] >= 1 samples in D[s] dimensions (1..4); x concatenates the sets' row-major [N_s, D_s].  D outside
+ * 1..4 or N < 1 -> MBAR_B200_ERR_INVALID; a NaN or infinite coordinate -> MBAR_B200_ERR_NAN. */
+typedef struct mbar_b200_kde_many mbar_b200_kde_many;
+int mbar_b200_kde_many_create(int device, int32_t n_sets, const int32_t* D, const int64_t* N, const double* x,
+                              mbar_b200_kde_many** out);
+int mbar_b200_kde_many_destroy(mbar_b200_kde_many* kde);
+/* Request r names set[r], a kernel[r] (mbar_b200_kde_kernel), a bandwidth h[r], weights w [N_set] and Q[r] >= 0 query
+ * points y [Q_r, D_set] row-major; w, y and out concatenate the requests'.  out[q] = log sum_n w_n k(d_qn / h): the
+ * same bits mbar_b200_kde_log_sum returns on an mbar_b200_kde created from (x of set[r], that w) for the same kernel, h
+ * and query.  A request gives the same bits alone, among any others, in any order and on repeat calls.  One partial
+ * launch per distinct (D, kernel) and one combine launch for all requests, and one synchronisation; the requests are
+ * cut into sub-batches (more launches, the same results) when their chunk partials would pass 64 MiB.  Before any
+ * device work, leaving the object usable: a bad set or kernel, an h <= 0 or not finite, a negative, NaN or infinite
+ * weight, or weights that sum to 0 -> MBAR_B200_ERR_INVALID; a NaN or infinite query -> MBAR_B200_ERR_NAN.  A call
+ * whose buffers do not fit in device memory -> MBAR_B200_ERR_NOMEM with the byte count in the message. */
+int mbar_b200_kde_many_log_sum(mbar_b200_kde_many* kde, int32_t n_requests, const int32_t* set, const int32_t* kernel,
+                               const double* h, const double* w, const int64_t* Q, const double* y, double* out);
+/* CUDA-event time of the kernels of the last mbar_b200_kde_many_log_sum, its kernel launches and its (query, sample)
+ * pairs. */
+int mbar_b200_last_kde_many_stats(mbar_b200_kde_many* kde, double* ms, int32_t* launches, int64_t* pairs);
 
 /* ---- B-spline basis sums (pymbar FES with fes_type="spline", independent of any u_kn context) --- */
 /* For the resident samples x_n with weights w_n and state labels s_n, and the nb = n_knots - degree - 1 basis
@@ -520,9 +542,18 @@ int mbar_b200_batch_replicate_bin_moments(mbar_b200_batch* batch, int32_t n_targ
                                           const double* u_n, const int32_t* bin_n, const int32_t* nbins,
                                           int32_t n_requests, const int32_t* slot, const int32_t* target,
                                           const double* f, double* f_bin, int32_t* flag);
+/* Target-state log weights of many problems (DESIGN.md 3.5h''): for request r, problem[r] with its converged f [K_p]
+ * and a target state's reduced potentials u_n [N_p] (f and u_n concatenate the requests'),
+ *   log_w [N_p] = -u_n - L_n,   L_n = log sum_{k sampled} N_k exp(f_k - u_kn),
+ * concatenated by request, from the resident tiles: L_n is batch_bin_moments' per-sample denominator.  u_n = +inf
+ * gives -inf.  A NaN log w_n sets flag[r]; the call still succeeds.  Before any device work, leaving the batch usable:
+ * a bad problem index -> MBAR_B200_ERR_INVALID, a NaN u_n -> MBAR_B200_ERR_NAN.  One kernel launch and one
+ * synchronisation. */
+int mbar_b200_batch_log_weights(mbar_b200_batch* batch, int32_t n_requests, const int32_t* problem, const double* f,
+                                const double* u_n, double* log_w, int32_t* flag);
 /* CUDA-event time of the kernels of the last batch_moments, batch_solve, batch_replicate_moments,
- * batch_solve_replicates, batch_augmented_moments, batch_replicate_augmented_moments, batch_bin_moments or
- * batch_replicate_bin_moments call, its
+ * batch_solve_replicates, batch_augmented_moments, batch_replicate_augmented_moments, batch_bin_moments,
+ * batch_replicate_bin_moments or batch_log_weights call, its
  * kernel launches, its iterations (solves) and the bytes of u_kn tiles (appended tiles, counts) its passes read. */
 int mbar_b200_last_batch_stats(mbar_b200_batch* batch, double* kernel_ms, int32_t* launches, int32_t* iterations,
                                int64_t* bytes_read);

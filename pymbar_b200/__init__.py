@@ -4,6 +4,8 @@ Public surface:
   * :mod:`pymbar_b200.mbar_solvers` — same names/signatures as ``pymbar.mbar_solvers``;
   * :class:`pymbar_b200.DeviceProblem` — explicit residency handle (one GPU, one shard of samples);
   * :class:`pymbar_b200.DeviceKde` — weighted samples resident for kernel-density sums (FES with fes_type="kde");
+  * :class:`pymbar_b200.DeviceKdeMany` — many sample sets resident for the kernel-density sums of many problems and
+    their bootstrap replicates in one call;
   * :class:`pymbar_b200.DeviceBSpline` — samples resident for B-spline basis sums (FES with fes_type="spline");
   * :class:`pymbar_b200.DeviceAcf` — a series resident for the lag sums of ``pymbar.timeseries``
     (:mod:`pymbar_b200.timeseries`);
@@ -13,16 +15,16 @@ Public surface:
     :func:`pymbar_b200.mbar_many.mbar_many` solves all of them in lockstep, one device call per iteration, and
     returns each problem's free energies and uncertainties, and :class:`pymbar_b200.MbarMany` keeps them resident
     for batched expectations, perturbed free energies, entropies and enthalpies, overlaps, effective sample
-    numbers and histogram free-energy surfaces (``generate_fes`` / ``get_fes``);
+    numbers and histogram and kernel-density free-energy surfaces (``generate_fes`` / ``get_fes``);
   * :func:`pymbar_b200.install` — rebind ``pymbar.mbar_solvers`` so unmodified ``pymbar.MBAR`` uses it.
 
 Everything numerical runs in libmbar_b200.so (C ABI in include/mbar_b200.h).  No CPU fallback.
 """
 from . import _lib
-from .problem import DeviceAcf, DeviceBSpline, DeviceKde, DeviceMbarBatch, DeviceProblem, DeviceWork, PinnedArray
+from .problem import DeviceAcf, DeviceBSpline, DeviceKde, DeviceKdeMany, DeviceMbarBatch, DeviceProblem, DeviceWork, PinnedArray
 from .utils import ParameterError
 
-__all__ = ["DeviceProblem", "DeviceKde", "DeviceBSpline", "DeviceAcf", "DeviceWork", "DeviceMbarBatch", "PinnedArray", "ParameterError", "install", "uninstall", "trim", "mbar_solvers", "MbarMany"]
+__all__ = ["DeviceProblem", "DeviceKde", "DeviceKdeMany", "DeviceBSpline", "DeviceAcf", "DeviceWork", "DeviceMbarBatch", "PinnedArray", "ParameterError", "install", "uninstall", "trim", "mbar_solvers", "MbarMany"]
 
 _SAVED = {}
 _PATCHED = (

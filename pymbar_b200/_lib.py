@@ -85,6 +85,12 @@ SIGNATURES = {
     "mbar_b200_kde_set_replicates": (C.c_int, [_ctx, C.c_int64, _dp]),
     "mbar_b200_kde_log_sum_replicates": (C.c_int, [_ctx, C.c_int32, C.c_double, C.c_int64, _dp, _dp]),
     "mbar_b200_last_kde_stats": (C.c_int, [_ctx, _dp, C.POINTER(C.c_int32)]),
+    "mbar_b200_kde_many_create": (C.c_int, [C.c_int, C.c_int32, C.POINTER(C.c_int32), C.POINTER(C.c_int64), _dp,
+                                            C.POINTER(_ctx)]),
+    "mbar_b200_kde_many_destroy": (C.c_int, [_ctx]),
+    "mbar_b200_kde_many_log_sum": (C.c_int, [_ctx, C.c_int32, C.POINTER(C.c_int32), C.POINTER(C.c_int32), _dp, _dp,
+                                             C.POINTER(C.c_int64), _dp, _dp]),
+    "mbar_b200_last_kde_many_stats": (C.c_int, [_ctx, _dp, C.POINTER(C.c_int32), C.POINTER(C.c_int64)]),
     "mbar_b200_bspline_create": (C.c_int, [C.c_int, C.c_int64, _dp, _dp, C.POINTER(C.c_int32), C.c_int32,
                                            C.POINTER(_ctx)]),
     "mbar_b200_bspline_destroy": (C.c_int, [_ctx]),
@@ -134,6 +140,8 @@ SIGNATURES = {
                                                         C.POINTER(C.c_int32), C.POINTER(C.c_int32), C.c_int32,
                                                         C.POINTER(C.c_int32), C.POINTER(C.c_int32), _dp, _dp,
                                                         C.POINTER(C.c_int32)]),
+    "mbar_b200_batch_log_weights": (C.c_int, [_ctx, C.c_int32, C.POINTER(C.c_int32), _dp, _dp, _dp,
+                                              C.POINTER(C.c_int32)]),
     "mbar_b200_last_batch_stats": (C.c_int, [_ctx, _dp, C.POINTER(C.c_int32), C.POINTER(C.c_int32),
                                              C.POINTER(C.c_int64)]),
     "mbar_b200_solve_sci":(C.c_int, [_ctx, _dp, C.c_double, C.c_int32, C.POINTER(SolveResult)]),

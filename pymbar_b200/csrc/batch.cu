@@ -155,18 +155,6 @@ struct mbar_b200_batch : mbar::Resident {
 
 namespace mbar {
 
-// the last of n segments whose start(s) <= i, for ascending starts with start(0) <= i
-template <class Start>
-__device__ __forceinline__ int find_segment(int n, int64_t i, Start start) {
-    int lo = 0, hi = n - 1;
-    while (lo < hi) {
-        const int mid = (lo + hi + 1) >> 1;
-        if (start(mid) <= i) lo = mid;
-        else hi = mid - 1;
-    }
-    return lo;
-}
-
 // entry e = i (i + 1) / 2 + j of a lower triangle -> (row i, column j), i >= j
 __device__ __forceinline__ int2 tri_decode(int e) {
     int i = (int)((sqrt(8.0 * e + 1.0) - 1.0) * 0.5);
@@ -995,6 +983,29 @@ __global__ void __launch_bounds__(256) batch_bin_prep_kernel(const double* __res
     if (v > -INFINITY && key > *((volatile unsigned long long*)kb)) atomicMax(kb, key);
 }
 
+// Target-state log weights (mbar_b200_batch_log_weights, DESIGN.md 3.5h''): batch_bin_prep_kernel's log w_n, without
+// bins.  lw [slots]: u_n on entry (+inf past N_p), log w_n on exit (samples past N_p are left as they are).  A NaN
+// log w_n flags its request.
+__global__ void __launch_bounds__(256) batch_log_weights_kernel(const double* __restrict__ u,
+                                                                const BinReq* __restrict__ req, int nReq, int64_t slots,
+                                                                const double* __restrict__ fAll,
+                                                                const double* __restrict__ NkAll,
+                                                                const double* __restrict__ logNkAll,
+                                                                const double* __restrict__ x, double* __restrict__ lw,
+                                                                int* __restrict__ rflag) {
+    const int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= slots) return;
+    const int r = find_segment(nReq, i, [&](int s) { return req[s].soff; });
+    const BinReq& q = req[r];
+    const int64_t n = i - q.soff;
+    if (n >= q.N) return;
+    const double L = bin_log_denominator(u, q, n, fAll, NkAll, logNkAll);
+    const double un = lw[i];
+    const double v = un < INFINITY ? -(un - x[q.xoff + n]) - L : -INFINITY;
+    lw[i] = v;
+    if (v != v) atomicOr(&rflag[r], 1);
+}
+
 // The replicate part of a weighted request (mbar_b200_batch_replicate_bin_moments): its target's first sample in the
 // per-target u_n and bin index arrays, and its slot's first count.
 struct RepBinReq {
@@ -1689,6 +1700,92 @@ int mbar_b200_batch_replicate_bin_moments(mbar_b200_batch* b, int32_t n_targets,
     b->lastBytes = bytes;
     std::memcpy(f_bin, b->h_out, (size_t)bins * sizeof(double));
     for (int r = 0; r < n; ++r) flag[r] = hflag[r] != 0;
+    return MBAR_B200_OK;
+}
+
+int mbar_b200_batch_log_weights(mbar_b200_batch* b, int32_t n, const int32_t* problem, const double* f,
+                                const double* u_n, double* log_w, int32_t* flag) {
+    MBAR_REQUIRE(b, MBAR_B200_ERR_INVALID, "batch_log_weights: NULL object");
+    MBAR_REQUIRE(n >= 1 && problem && f && u_n && log_w && flag, MBAR_B200_ERR_INVALID,
+                 "batch_log_weights: %d requests or a NULL argument", (int)n);
+    std::vector<BinReq> req((size_t)n);
+    std::vector<int64_t> tile0((size_t)b->P, 0);  // first tile of each problem: indexes x_n
+    for (int p = 1; p < b->P; ++p) tile0[p] = tile0[p - 1] + b->nT[p - 1];
+    int64_t slots = 0, fs = 0, src = 0, bytes = 0;
+    for (int r = 0; r < n; ++r) {
+        const int p = problem[r];
+        MBAR_REQUIRE(p >= 0 && p < b->P, MBAR_B200_ERR_INVALID, "batch_log_weights: request %d names problem %d of %d",
+                     r, p, b->P);
+        BinReq& q = req[r];
+        q = BinReq{};
+        q.K = b->K[p];
+        q.N = b->N[p];
+        q.nT = b->nT[p];
+        q.uoff = b->uoff[p];
+        q.voff = b->voff[p];
+        q.xoff = tile0[p] * 32;
+        q.soff = slots;
+        q.foff = fs;
+        bytes += q.nT * 32 * q.K * 8;
+        slots += q.nT * 32;
+        fs += q.K;
+        src += q.N;
+    }
+    for (int64_t i = 0; i < src; ++i)
+        MBAR_REQUIRE(u_n[i] == u_n[i], MBAR_B200_ERR_NAN, "batch_log_weights: NaN in u_n (entry %lld)", (long long)i);
+    MBAR_CUDA(cudaSetDevice(b->device));
+    NvtxRange nvtx_("mbar_b200::batch_log_weights");
+    b->lastLaunches = 0;
+    b->lastBytes = 0;
+    b->lastIterations = 0;
+    // pinned staging: f, u_n padded with +inf to the tiles, the requests; log w_n comes back through the u_n slots
+    const size_t reqDoubles = ((size_t)n * sizeof(BinReq) + 7) / 8;
+    MBAR_TRY(b->h_f.grow((size_t)fs + (size_t)slots + reqDoubles, "batch_log_weights"));
+    std::memcpy(b->h_f, f, (size_t)fs * sizeof(double));
+    double* hu = b->h_f + fs;
+    src = 0;
+    for (int r = 0; r < n; ++r) {
+        const BinReq& q = req[r];
+        std::memcpy(hu + q.soff, u_n + src, (size_t)q.N * sizeof(double));
+        for (int64_t i = q.N; i < q.nT * 32; ++i) hu[q.soff + i] = INFINITY;
+        src += q.N;
+    }
+    BinReq* hreq = reinterpret_cast<BinReq*>(b->h_f + fs + slots);
+    std::memcpy(hreq, req.data(), req.size() * sizeof(BinReq));
+    CallBuffers buf("batch_log_weights");
+    BinReq* d_req;
+    int* d_rflag;
+    double *d_f, *d_lw;
+    MBAR_TRY(buf.alloc(&d_req, (size_t)n));
+    MBAR_TRY(buf.alloc(&d_f, (size_t)fs));
+    MBAR_TRY(buf.alloc(&d_lw, (size_t)slots));
+    MBAR_TRY(buf.alloc(&d_rflag, (size_t)n));
+    cudaStream_t s = b->stream;
+    MBAR_CUDA(cudaMemcpyAsync(d_f, b->h_f, (size_t)fs * sizeof(double), cudaMemcpyHostToDevice, s));
+    MBAR_CUDA(cudaMemcpyAsync(d_lw, hu, (size_t)slots * sizeof(double), cudaMemcpyHostToDevice, s));
+    MBAR_CUDA(cudaMemcpyAsync(d_req, hreq, req.size() * sizeof(BinReq), cudaMemcpyHostToDevice, s));
+    MBAR_CUDA(cudaMemsetAsync(d_rflag, 0, (size_t)n * sizeof(int), s));
+    MBAR_CUDA(cudaEventRecord(b->ev0, s));
+    batch_log_weights_kernel<<<(unsigned)((slots + 255) / 256), 256, 0, s>>>(b->d_u, d_req, n, slots, d_f, b->d_Nk,
+                                                                            b->d_logNk, b->d_x, d_lw, d_rflag);
+    MBAR_CUDA(cudaGetLastError());
+    MBAR_CUDA(cudaEventRecord(b->ev1, s));
+    MBAR_TRY(b->h_out.grow((size_t)slots, "batch_log_weights"));
+    std::vector<int> hflag((size_t)n);
+    MBAR_CUDA(cudaMemcpyAsync(b->h_out, d_lw, (size_t)slots * sizeof(double), cudaMemcpyDeviceToHost, s));
+    MBAR_CUDA(cudaMemcpyAsync(hflag.data(), d_rflag, (size_t)n * sizeof(int), cudaMemcpyDeviceToHost, s));
+    MBAR_CUDA(cudaStreamSynchronize(s));
+    float ms = 0.f;
+    b->lastMs = event_ms(b->ev0, b->ev1, &ms) ? ms : 0.0;
+    b->lastLaunches = 1;
+    b->lastBytes = bytes;
+    src = 0;
+    for (int r = 0; r < n; ++r) {
+        const BinReq& q = req[r];
+        std::memcpy(log_w + src, b->h_out + q.soff, (size_t)q.N * sizeof(double));
+        flag[r] = hflag[r] != 0;
+        src += q.N;
+    }
     return MBAR_B200_OK;
 }
 

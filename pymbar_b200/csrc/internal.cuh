@@ -709,6 +709,18 @@ __device__ __forceinline__ double warp_sum(double x) {
     return x;
 }
 
+// the last of n segments whose start(s) <= i, for ascending starts with start(0) <= i
+template <class Start>
+__device__ __forceinline__ int find_segment(int n, int64_t i, Start start) {
+    int lo = 0, hi = n - 1;
+    while (lo < hi) {
+        const int mid = (lo + hi + 1) >> 1;
+        if (start(mid) <= i) lo = mid;
+        else hi = mid - 1;
+    }
+    return lo;
+}
+
 // The order-preserving integer form of a double, so that a per-bin maximum can be taken by an integer atomicMax (a
 // maximum does not depend on the order of its operands, so the result is deterministic); 0 is below every key.
 __device__ __forceinline__ unsigned long long ordered_key(double d) {

@@ -52,6 +52,17 @@ struct mbar_b200_kde : mbar::Resident {
     mbar::DevArray<double> d_rlw;    // [nPad] log V_bn of one replicate, for the exact pass over flagged queries
 };
 
+// Many sample sets at once (mbar_b200_kde_many_*, DESIGN.md 3.5h''): only the coordinates are resident, each set laid
+// out as mbar_b200_kde lays out its own; the weights come with every request.
+struct mbar_b200_kde_many : mbar::Resident {
+    std::vector<int> D;
+    std::vector<int64_t> N, nPad, chunkLen, xoff;   // per set; xoff: first double of its [D][nPad] block
+    std::vector<int> nChunks;
+    mbar::DevArray<double> d_x;
+    int32_t lastLaunches = 0;
+    int64_t lastPairs = 0;
+};
+
 namespace mbar {
 
 constexpr int KDE_THREADS = 128;              // queries per CTA
@@ -96,17 +107,14 @@ __device__ __forceinline__ double exp_flush(double a, const double* __restrict__
     return q < -1021 ? 0.0 : __hiloint2double(hi, __double2loint(v));
 }
 
-template <int D, int KERN>
-__global__ void __launch_bounds__(KDE_THREADS) kde_partial_kernel(KdeParams p) {
-    __shared__ double sx[D][KDE_TILE];
-    __shared__ double slw[KDE_TILE];
-    __shared__ double tab[MBAR_EXP_NT];
-    if (threadIdx.x < MBAR_EXP_NT) tab[threadIdx.x] = MBAR_EXP_TABLE[threadIdx.x];
-    const int q = blockIdx.x * KDE_THREADS + threadIdx.x;
-    const int64_t n0 = (int64_t)blockIdx.y * p.chunkLen, n1 = min(n0 + p.chunkLen, p.nPad);
-    double y[D];
-#pragma unroll
-    for (int j = 0; j < D; ++j) y[j] = q < p.Qb ? p.y[(int64_t)j * p.Qb + q] : 0.0;
+// One thread's running (m, s) over the samples [n0, n1) of one chunk for its query y: the per-pair arithmetic of every
+// single-replicate KDE pass (kde_partial_kernel, kde_many_partial_kernel), stated once so that both give the same
+// bits.  p holds KdeParams' x [D][nPad], lw [nPad], nPad, h, hh, c and T (the kernel's parameters, or a copy in shared
+// memory); sx, slw and tab are the CTA's shared tiles and exp table.
+template <int D, int KERN, class P>
+__device__ __forceinline__ void kde_chunk_sum(const P& p, int64_t n0, int64_t n1, const double (&y)[D],
+                                              double (&sx)[D][KDE_TILE], double (&slw)[KDE_TILE], const double* tab,
+                                              double& m_out, double& s_out) {
     double m = -INFINITY, s = 0.0;
     for (int64_t t0 = n0; t0 < n1; t0 += KDE_TILE) {
         __syncthreads();
@@ -126,18 +134,18 @@ __global__ void __launch_bounds__(KDE_THREADS) kde_partial_kernel(KdeParams p) {
                 t = __dsub_rn(y[j], sx[j][i]);
                 r = __dadd_rn(r, __dmul_rn(t, t));
             }
-            const double lw = slw[i];
+            const double lwi = slw[i];
             double a, k = 1.0;
             if (KERN == KDE_GAUSSIAN) {
-                a = fma(-r, p.c, lw);
+                a = fma(-r, p.c, lwi);
             } else if (KERN == KDE_TOPHAT) {
-                a = r < p.T ? lw : -INFINITY;
+                a = r < p.T ? lwi : -INFINITY;
             } else if (KERN == KDE_EXPONENTIAL) {
-                a = fma(-__dsqrt_rn(r), p.c, lw);
+                a = fma(-__dsqrt_rn(r), p.c, lwi);
             } else {
                 const double d = __dsqrt_rn(r);
                 const bool in = d < p.h;
-                a = in ? lw : -INFINITY;
+                a = in ? lwi : -INFINITY;
                 if (KERN == KDE_EPANECHNIKOV) k = __dsub_rn(1.0, __ddiv_rn(__dmul_rn(d, d), p.hh));
                 if (KERN == KDE_LINEAR) k = __dsub_rn(1.0, __ddiv_rn(d, p.h));
                 if (KERN == KDE_COSINE) k = cos(__ddiv_rn(__dmul_rn(KDE_HALF_PI, d), p.h));
@@ -153,6 +161,23 @@ __global__ void __launch_bounds__(KDE_THREADS) kde_partial_kernel(KdeParams p) {
             s = (KERN == KDE_EPANECHNIKOV || KERN == KDE_LINEAR || KERN == KDE_COSINE) ? fma(e, k, s) : s + e;
         }
     }
+    m_out = m;
+    s_out = s;
+}
+
+template <int D, int KERN>
+__global__ void __launch_bounds__(KDE_THREADS) kde_partial_kernel(KdeParams p) {
+    __shared__ double sx[D][KDE_TILE];
+    __shared__ double slw[KDE_TILE];
+    __shared__ double tab[MBAR_EXP_NT];
+    if (threadIdx.x < MBAR_EXP_NT) tab[threadIdx.x] = MBAR_EXP_TABLE[threadIdx.x];
+    const int q = blockIdx.x * KDE_THREADS + threadIdx.x;
+    const int64_t n0 = (int64_t)blockIdx.y * p.chunkLen, n1 = min(n0 + p.chunkLen, p.nPad);
+    double y[D];
+#pragma unroll
+    for (int j = 0; j < D; ++j) y[j] = q < p.Qb ? p.y[(int64_t)j * p.Qb + q] : 0.0;
+    double m, s;
+    kde_chunk_sum<D, KERN>(p, n0, n1, y, sx, slw, tab, m, s);
     if (q < p.Qb) {
         p.pm[(int64_t)blockIdx.y * p.Qb + q] = m;
         p.ps[(int64_t)blockIdx.y * p.Qb + q] = s;
@@ -173,6 +198,108 @@ __global__ void kde_combine_kernel(const double* __restrict__ pm, const double* 
     double S = 0.0;
     for (int c = 0; c < nChunks; ++c) S += ps[(int64_t)c * Qb + q] * exp(pm[(int64_t)c * Qb + q] - M);
     out[q] = M + log(S);
+}
+
+// ---- many sample sets (mbar_b200_kde_many_log_sum, DESIGN.md 3.5h'') ----------------------------------------------
+// A piece is up to `cap` queries of one request (cap: the query batch of mbar_b200_kde_log_sum for the set's chunk
+// count).  Its work items are (query block of KDE_THREADS, chunk); a piece's partials are [nChunks][Q] at poff.
+struct KdeManyPiece {
+    int64_t item0;     // first work item of the piece in its partial launch
+    int64_t xoff;      // first double of the set's [D][nPad] coordinates
+    int64_t lwoff;     // first log weight of the request ([nPad], -inf in the padding)
+    int64_t yoff;      // first double of the piece's [D][Q] queries
+    int64_t poff;      // first partial of the piece in its sub-batch
+    int64_t ooff;      // first output of the piece in the call
+    int64_t nPad, chunkLen;
+    int32_t Q, nqb, nChunks;
+    double h, hh, c, T;
+};
+
+// kde_partial_kernel for every piece of one (D, kernel) in a sub-batch: one CTA per work item, found by find_segment
+template <int D, int KERN>
+__global__ void __launch_bounds__(KDE_THREADS, 4) kde_many_partial_kernel(const KdeManyPiece* pc, int n, const double* x,
+                                                                      const double* lw,
+                                                                      const double* __restrict__ yAll,
+                                                                      double* __restrict__ pm, double* __restrict__ ps) {
+    __shared__ double sx[D][KDE_TILE];
+    __shared__ double slw[KDE_TILE];
+    __shared__ double tab[MBAR_EXP_NT];
+    __shared__ KdeParams sp;          // the piece's samples and kernel constants, read from here by the pass
+    if (threadIdx.x < MBAR_EXP_NT) tab[threadIdx.x] = MBAR_EXP_TABLE[threadIdx.x];
+    const int64_t item = blockIdx.x;
+    double m, s;
+    {
+        const KdeManyPiece& p = pc[find_segment(n, item, [&](int i) { return pc[i].item0; })];
+        if (threadIdx.x == 0) {
+            sp.x = x + p.xoff;
+            sp.lw = lw + p.lwoff;
+            sp.nPad = p.nPad;
+            sp.h = p.h;
+            sp.hh = p.hh;
+            sp.c = p.c;
+            sp.T = p.T;
+        }
+        const int local = (int)(item - p.item0);      // a launch has fewer than 2^31 work items
+        const int chunk = local / p.nqb;
+        const int q = (local - chunk * p.nqb) * KDE_THREADS + threadIdx.x;
+        const int64_t n0 = (int64_t)chunk * p.chunkLen, n1 = min(n0 + p.chunkLen, p.nPad);
+        double y[D];
+#pragma unroll
+        for (int j = 0; j < D; ++j) y[j] = q < p.Q ? yAll[p.yoff + (int64_t)j * p.Q + q] : 0.0;
+        kde_chunk_sum<D, KERN>(sp, n0, n1, y, sx, slw, tab, m, s);   // its first barrier publishes sp
+    }
+    // the piece is found and read again after the pass, so that nothing of it stays live across the pass
+    const KdeManyPiece& p = pc[find_segment(n, item, [&](int i) { return pc[i].item0; })];
+    const int local = (int)(item - p.item0);
+    const int chunk = local / p.nqb;
+    const int q = (local - chunk * p.nqb) * KDE_THREADS + threadIdx.x;
+    if (q < p.Q) {
+        pm[p.poff + (int64_t)chunk * p.Q + q] = m;
+        ps[p.poff + (int64_t)chunk * p.Q + q] = s;
+    }
+}
+
+// kde_combine_kernel's rule for the outputs [o0, o0 + nOut) of a sub-batch's pieces (ascending ooff)
+__global__ void kde_many_combine_kernel(const KdeManyPiece* __restrict__ pc, int n, int64_t o0, int64_t nOut,
+                                        const double* __restrict__ pm, const double* __restrict__ ps,
+                                        double* __restrict__ out) {
+    const int64_t i = o0 + (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= o0 + nOut) return;
+    const KdeManyPiece& p = pc[find_segment(n, i, [&](int r) { return pc[r].ooff; })];
+    const int64_t q = i - p.ooff;
+    double M = -INFINITY;
+    for (int c = 0; c < p.nChunks; ++c) M = fmax(M, pm[p.poff + (int64_t)c * p.Q + q]);
+    if (M == -INFINITY) {
+        out[i] = -INFINITY;
+        return;
+    }
+    double S = 0.0;
+    for (int c = 0; c < p.nChunks; ++c) S += ps[p.poff + (int64_t)c * p.Q + q] * exp(pm[p.poff + (int64_t)c * p.Q + q] - M);
+    out[i] = M + log(S);
+}
+
+typedef void (*KdeManyKernelFn)(const KdeManyPiece*, int, const double*, const double*, const double*, double*,
+                                double*);
+
+template <int D>
+static KdeManyKernelFn kde_many_kernel_for(int kernel) {
+    switch (kernel) {
+        case KDE_GAUSSIAN: return kde_many_partial_kernel<D, KDE_GAUSSIAN>;
+        case KDE_TOPHAT: return kde_many_partial_kernel<D, KDE_TOPHAT>;
+        case KDE_EPANECHNIKOV: return kde_many_partial_kernel<D, KDE_EPANECHNIKOV>;
+        case KDE_EXPONENTIAL: return kde_many_partial_kernel<D, KDE_EXPONENTIAL>;
+        case KDE_LINEAR: return kde_many_partial_kernel<D, KDE_LINEAR>;
+        default: return kde_many_partial_kernel<D, KDE_COSINE>;
+    }
+}
+
+static KdeManyKernelFn kde_many_kernel_for(int D, int kernel) {
+    switch (D) {
+        case 1: return kde_many_kernel_for<1>(kernel);
+        case 2: return kde_many_kernel_for<2>(kernel);
+        case 3: return kde_many_kernel_for<3>(kernel);
+        default: return kde_many_kernel_for<4>(kernel);
+    }
 }
 
 // kde_combine_kernel's rule for the W * Qb entries of a replicate batch, and flag[i] = 1 where the entry lies more
@@ -341,6 +468,21 @@ static double sqrt_threshold(double h) {
     return r;
 }
 
+// chunks: a function of N alone (batch independence); at least KDE_MIN_CHUNK samples, at most KDE_MAX_CHUNKS
+static void kde_chunking(int64_t N, int64_t* chunkLen, int* nChunks) {
+    const int64_t nPad = (N + KDE_TILE - 1) / KDE_TILE * KDE_TILE;
+    const int64_t nc = std::min<int64_t>(KDE_MAX_CHUNKS, std::max<int64_t>(1, (N + KDE_MIN_CHUNK - 1) / KDE_MIN_CHUNK));
+    *chunkLen = ((N + nc - 1) / nc + KDE_TILE - 1) / KDE_TILE * KDE_TILE;
+    *nChunks = (int)((nPad + *chunkLen - 1) / *chunkLen);
+}
+
+// the query batch of one call for a sample set cut into nChunks chunks: the partials of a batch stay under
+// KDE_PART_BYTES (one block of KDE_THREADS queries at least); it decides the size of the partials, never a result
+static int64_t kde_query_cap(int nChunks, int64_t perQuery) {
+    const int64_t cap = (int64_t)(KDE_PART_BYTES / (2 * sizeof(double) * (size_t)perQuery * (size_t)nChunks));
+    return std::max<int64_t>(KDE_THREADS, cap / KDE_THREADS * KDE_THREADS);
+}
+
 // per-batch buffers for up to qb queries; on failure the object keeps no (or its previous) buffers and stays usable
 static int kde_reserve(mbar_b200_kde* k, int64_t qb) {
     MBAR_TRY(k->d_y.reserve((size_t)k->D * qb, "kde"));
@@ -396,10 +538,7 @@ int mbar_b200_kde_create(int device, int64_t N, int32_t D, const double* x_host,
     k->D = D;
     k->N = N;
     k->nPad = nPad;
-    // chunks: a function of N alone (batch independence); at least KDE_MIN_CHUNK samples, at most KDE_MAX_CHUNKS
-    int64_t nc = std::min<int64_t>(KDE_MAX_CHUNKS, std::max<int64_t>(1, (N + KDE_MIN_CHUNK - 1) / KDE_MIN_CHUNK));
-    k->chunkLen = ((N + nc - 1) / nc + KDE_TILE - 1) / KDE_TILE * KDE_TILE;
-    k->nChunks = (int)((nPad + k->chunkLen - 1) / k->chunkLen);
+    kde_chunking(N, &k->chunkLen, &k->nChunks);
     MBAR_TRY(k->open(device, "kde_create"));
     MBAR_TRY(k->upload(k->d_x, hx.data(), hx.size(), "kde_create"));
     MBAR_TRY(k->upload(k->d_lw, hlw.data(), hlw.size(), "kde_create"));
@@ -426,9 +565,7 @@ int mbar_b200_kde_log_sum(mbar_b200_kde* k, int32_t kernel, double h, int64_t Q,
     MBAR_CUDA(cudaSetDevice(k->device));
     NvtxRange nvtx_("mbar_b200::kde_log_sum");
     // query batches: only the size of the partials depends on them, never a query's result
-    int64_t cap = (int64_t)(KDE_PART_BYTES / (2 * sizeof(double) * (size_t)k->nChunks));
-    cap = std::max<int64_t>(KDE_THREADS, cap / KDE_THREADS * KDE_THREADS);
-    const int64_t qb = std::min(Q, cap);
+    const int64_t qb = std::min(Q, kde_query_cap(k->nChunks, 1));
     MBAR_TRY(kde_reserve(k, qb));
     KdeParams p{};
     p.x = k->d_x;
@@ -531,9 +668,7 @@ int mbar_b200_kde_log_sum_replicates(mbar_b200_kde* k, int32_t kernel, double h,
                      "(%lld, %d) is %g", (long long)(i / D), (int)(i % D), y_host[i]);
     MBAR_CUDA(cudaSetDevice(k->device));
     NvtxRange nvtx_("mbar_b200::kde_log_sum_replicates");
-    int64_t cap = (int64_t)(KDE_PART_BYTES / (2 * sizeof(double) * KDE_REP_W * (size_t)k->nChunks));
-    cap = std::max<int64_t>(KDE_THREADS, cap / KDE_THREADS * KDE_THREADS);
-    const int64_t qb = std::min(Q, cap);
+    const int64_t qb = std::min(Q, kde_query_cap(k->nChunks, KDE_REP_W));
     MBAR_TRY(kde_reserve(k, qb));
     MBAR_TRY(kde_rep_reserve(k, qb));
     KdeParams p{};
@@ -628,5 +763,249 @@ int mbar_b200_last_kde_stats(mbar_b200_kde* k, double* ms, int32_t* chunks) {
     MBAR_REQUIRE(k, MBAR_B200_ERR_INVALID, "NULL kde object");
     if (ms) *ms = k->lastMs;
     if (chunks) *chunks = k->lastChunks;
+    return MBAR_B200_OK;
+}
+
+int mbar_b200_kde_many_create(int device, int32_t n_sets, const int32_t* D, const int64_t* N, const double* x,
+                              mbar_b200_kde_many** out) {
+    MBAR_REQUIRE(out && D && N && x, MBAR_B200_ERR_INVALID, "kde_many_create: NULL argument");
+    *out = nullptr;
+    MBAR_REQUIRE(n_sets >= 1, MBAR_B200_ERR_INVALID, "kde_many_create: %d sets", (int)n_sets);
+    std::unique_ptr<mbar_b200_kde_many> k(new mbar_b200_kde_many());
+    int64_t total = 0, src = 0;
+    for (int s = 0; s < n_sets; ++s) {
+        MBAR_REQUIRE(N[s] >= 1, MBAR_B200_ERR_INVALID, "kde_many_create: set %d has N=%lld", s, (long long)N[s]);
+        MBAR_REQUIRE(D[s] >= 1 && D[s] <= 4, MBAR_B200_ERR_INVALID, "kde_many_create: set %d has D=%d outside [1, 4]",
+                     s, (int)D[s]);
+        for (int64_t i = 0; i < N[s] * D[s]; ++i)
+            MBAR_REQUIRE(std::isfinite(x[src + i]), MBAR_B200_ERR_NAN, "kde_many_create: set %d: coordinate (%lld, %d) "
+                         "is %g", s, (long long)(i / D[s]), (int)(i % D[s]), x[src + i]);
+        int64_t chunkLen;
+        int nChunks;
+        kde_chunking(N[s], &chunkLen, &nChunks);
+        const int64_t nPad = (N[s] + KDE_TILE - 1) / KDE_TILE * KDE_TILE;
+        k->D.push_back(D[s]);
+        k->N.push_back(N[s]);
+        k->nPad.push_back(nPad);
+        k->chunkLen.push_back(chunkLen);
+        k->nChunks.push_back(nChunks);
+        k->xoff.push_back(total);
+        total += (int64_t)D[s] * nPad;
+        src += N[s] * D[s];
+    }
+    // each set as mbar_b200_kde_create lays it out: [D][nPad], 0 in the padding
+    std::vector<double> hx((size_t)total, 0.0);
+    src = 0;
+    for (int s = 0; s < n_sets; ++s) {
+        for (int64_t n = 0; n < N[s]; ++n)
+            for (int j = 0; j < D[s]; ++j) hx[(size_t)(k->xoff[s] + j * k->nPad[s] + n)] = x[src + n * D[s] + j];
+        src += N[s] * D[s];
+    }
+    MBAR_TRY(open_device(device, nullptr));
+    MBAR_TRY(k->open(device, "kde_many_create"));
+    MBAR_TRY(k->upload(k->d_x, hx.data(), hx.size(), "kde_many_create"));
+    *out = k.release();
+    return MBAR_B200_OK;
+}
+
+int mbar_b200_kde_many_destroy(mbar_b200_kde_many* k) { return destroy_resident(k); }
+
+int mbar_b200_kde_many_log_sum(mbar_b200_kde_many* k, int32_t n_requests, const int32_t* set, const int32_t* kernel,
+                               const double* h, const double* w, const int64_t* Q, const double* y, double* out) {
+    MBAR_REQUIRE(k, MBAR_B200_ERR_INVALID, "kde_many_log_sum: NULL object");
+    MBAR_REQUIRE(n_requests >= 0, MBAR_B200_ERR_INVALID, "kde_many_log_sum: %d requests", (int)n_requests);
+    if (n_requests == 0) return MBAR_B200_OK;
+    MBAR_REQUIRE(set && kernel && h && w && Q, MBAR_B200_ERR_INVALID, "kde_many_log_sum: NULL argument");
+    const int nSets = (int)k->D.size();
+    // every request checked before any device work
+    int64_t wsrc = 0, ysrc = 0, outs = 0, lws = 0;
+    for (int r = 0; r < n_requests; ++r) {
+        const int s = set[r];
+        MBAR_REQUIRE(s >= 0 && s < nSets, MBAR_B200_ERR_INVALID, "kde_many_log_sum: request %d names set %d of %d", r,
+                     s, nSets);
+        MBAR_REQUIRE(kernel[r] >= 0 && kernel[r] < KDE_NKERNELS, MBAR_B200_ERR_INVALID,
+                     "kde_many_log_sum: request %d: unknown kernel %d", r, (int)kernel[r]);
+        MBAR_REQUIRE(std::isfinite(h[r]) && h[r] > 0.0, MBAR_B200_ERR_INVALID,
+                     "kde_many_log_sum: request %d: bandwidth %g must be finite and positive", r, h[r]);
+        MBAR_REQUIRE(Q[r] >= 0, MBAR_B200_ERR_INVALID, "kde_many_log_sum: request %d: Q=%lld", r, (long long)Q[r]);
+        bool any = false;
+        for (int64_t n = 0; n < k->N[s]; ++n) {
+            const double v = w[wsrc + n];
+            MBAR_REQUIRE(v >= 0.0 && v < INFINITY, MBAR_B200_ERR_INVALID, "kde_many_log_sum: request %d: weight %lld "
+                         "is %g (negative, NaN or infinite)", r, (long long)n, v);
+            any |= v > 0.0;
+        }
+        MBAR_REQUIRE(any, MBAR_B200_ERR_INVALID, "kde_many_log_sum: request %d: the weights sum to 0", r);
+        MBAR_REQUIRE(Q[r] == 0 || (y && out), MBAR_B200_ERR_INVALID, "kde_many_log_sum: NULL queries or output");
+        const int D = k->D[s];
+        for (int64_t i = 0; i < Q[r] * D; ++i)
+            MBAR_REQUIRE(std::isfinite(y[ysrc + i]), MBAR_B200_ERR_NAN, "kde_many_log_sum: request %d: query "
+                         "coordinate (%lld, %d) is %g", r, (long long)(i / D), (int)(i % D), y[ysrc + i]);
+        wsrc += k->N[s];
+        ysrc += Q[r] * D;
+        outs += Q[r];
+        lws += k->nPad[s];
+    }
+    // pieces of at most kde_query_cap queries, in request order; sub-batches of pieces whose partials stay under
+    // KDE_PART_BYTES (one piece at least).  Neither decides a result.
+    struct Piece {
+        int r;
+        int64_t q0;
+        int32_t Qp;
+    };
+    std::vector<Piece> pieces;
+    std::vector<std::pair<size_t, size_t>> subs;      // [first, last) piece of each sub-batch
+    size_t first = 0;
+    int64_t used = 0, maxParts = 0, pairs = 0;
+    for (int r = 0; r < n_requests; ++r) {
+        const int s = set[r];
+        const int64_t cap = kde_query_cap(k->nChunks[s], 1);
+        pairs += Q[r] * k->N[s];
+        for (int64_t q0 = 0; q0 < Q[r]; q0 += cap) {
+            const int32_t Qp = (int32_t)std::min(cap, Q[r] - q0);
+            const int64_t parts = (int64_t)k->nChunks[s] * Qp;     // (m, s) pairs
+            if (pieces.size() > first && (size_t)(used + parts) * 2 * sizeof(double) > KDE_PART_BYTES) {
+                subs.emplace_back(first, pieces.size());
+                first = pieces.size();
+                used = 0;
+            }
+            pieces.push_back(Piece{r, q0, Qp});
+            used += parts;
+            maxParts = std::max(maxParts, used);
+        }
+    }
+    if (pieces.size() > first) subs.emplace_back(first, pieces.size());
+    // host staging: log w_n of every request (std::log, as kde_create takes it; -inf in the padding), the queries of
+    // every piece as [D][Qp], and the piece records: per sub-batch, grouped by (D, kernel) for the partial launches,
+    // then in output order for the combine
+    std::vector<double> hlw((size_t)lws, -INFINITY), hy((size_t)ysrc);
+    std::vector<int64_t> lwoff((size_t)n_requests), yoff((size_t)n_requests), ooff((size_t)n_requests);
+    wsrc = 0;
+    ysrc = 0;
+    lws = 0;
+    outs = 0;
+    for (int r = 0; r < n_requests; ++r) {
+        const int s = set[r], D = k->D[s];
+        for (int64_t n = 0; n < k->N[s]; ++n) hlw[(size_t)(lws + n)] = std::log(w[wsrc + n]);
+        lwoff[r] = lws;
+        yoff[r] = ysrc;
+        ooff[r] = outs;
+        wsrc += k->N[s];
+        lws += k->nPad[s];
+        ysrc += Q[r] * D;
+        outs += Q[r];
+    }
+    auto record = [&](const Piece& pc, int64_t poff) {
+        const int r = pc.r, s = set[r], D = k->D[s];
+        KdeManyPiece p{};
+        p.xoff = k->xoff[s];
+        p.lwoff = lwoff[r];
+        p.yoff = yoff[r] + (int64_t)D * pc.q0;        // the piece's own [D][Qp] block
+        p.poff = poff;
+        p.ooff = ooff[r] + pc.q0;
+        p.nPad = k->nPad[s];
+        p.chunkLen = k->chunkLen[s];
+        p.Q = pc.Qp;
+        p.nqb = (pc.Qp + KDE_THREADS - 1) / KDE_THREADS;
+        p.nChunks = k->nChunks[s];
+        p.h = h[r];
+        p.hh = h[r] * h[r];
+        p.c = kernel[r] == KDE_GAUSSIAN ? 0.5 / (h[r] * h[r]) : 1.0 / h[r];
+        p.T = sqrt_threshold(h[r]);
+        return p;
+    };
+    // a piece reads its queries as [D][Qp]: lay every request's queries out piece by piece
+    for (const Piece& pc : pieces) {
+        const int r = pc.r, D = k->D[set[r]];
+        double* dst = hy.data() + yoff[r] + (int64_t)D * pc.q0;
+        for (int64_t i = 0; i < pc.Qp; ++i)
+            for (int j = 0; j < D; ++j) dst[(size_t)j * pc.Qp + i] = y[yoff[r] + (pc.q0 + i) * D + j];
+    }
+    std::vector<KdeManyPiece> hpc;                    // per sub-batch: grouped records, then ordered records
+    struct Launch {
+        size_t rec;       // first record
+        int n;            // records
+        int64_t items;    // CTAs (partial launch) or outputs (combine)
+        int64_t o0;       // first output (combine)
+        KdeManyKernelFn fn;   // NULL: the combine
+    };
+    std::vector<Launch> launches;
+    for (const auto& sb : subs) {
+        std::vector<int64_t> poff(sb.second - sb.first);
+        int64_t parts = 0;
+        for (size_t i = sb.first; i < sb.second; ++i) {
+            poff[i - sb.first] = parts;
+            parts += (int64_t)k->nChunks[set[pieces[i].r]] * pieces[i].Qp;
+        }
+        std::vector<std::pair<int, int>> groups;      // distinct (D, kernel) in order of first appearance
+        for (size_t i = sb.first; i < sb.second; ++i) {
+            const std::pair<int, int> g(k->D[set[pieces[i].r]], kernel[pieces[i].r]);
+            if (std::find(groups.begin(), groups.end(), g) == groups.end()) groups.push_back(g);
+        }
+        for (const auto& g : groups) {
+            Launch L{hpc.size(), 0, 0, 0, kde_many_kernel_for(g.first, g.second)};
+            for (size_t i = sb.first; i < sb.second; ++i) {
+                const Piece& pc = pieces[i];
+                if (k->D[set[pc.r]] != g.first || kernel[pc.r] != g.second) continue;
+                KdeManyPiece p = record(pc, poff[i - sb.first]);
+                p.item0 = L.items;
+                L.items += (int64_t)p.nqb * p.nChunks;
+                hpc.push_back(p);
+                ++L.n;
+            }
+            MBAR_REQUIRE(L.items < INT32_MAX, MBAR_B200_ERR_INVALID, "kde_many_log_sum: %lld work items in one launch",
+                         (long long)L.items);
+            launches.push_back(L);
+        }
+        Launch C{hpc.size(), 0, 0, 0, nullptr};
+        for (size_t i = sb.first; i < sb.second; ++i) {
+            KdeManyPiece p = record(pieces[i], poff[i - sb.first]);
+            if (C.n == 0) C.o0 = p.ooff;
+            C.items += p.Q;
+            hpc.push_back(p);
+            ++C.n;
+        }
+        launches.push_back(C);
+    }
+    MBAR_CUDA(cudaSetDevice(k->device));
+    NvtxRange nvtx_("mbar_b200::kde_many_log_sum");
+    CallBuffers buf("kde_many_log_sum");
+    double *d_lw, *d_y, *d_pm, *d_ps, *d_out;
+    KdeManyPiece* d_pc;
+    MBAR_TRY(buf.alloc(&d_lw, hlw.size()));
+    MBAR_TRY(buf.alloc(&d_y, hy.size()));
+    MBAR_TRY(buf.alloc(&d_pm, (size_t)maxParts));
+    MBAR_TRY(buf.alloc(&d_ps, (size_t)maxParts));
+    MBAR_TRY(buf.alloc(&d_out, (size_t)outs));
+    MBAR_TRY(buf.alloc(&d_pc, hpc.size()));
+    cudaStream_t st = k->stream;
+    MBAR_CUDA(cudaMemcpyAsync(d_lw, hlw.data(), hlw.size() * sizeof(double), cudaMemcpyHostToDevice, st));
+    MBAR_CUDA(cudaMemcpyAsync(d_y, hy.data(), hy.size() * sizeof(double), cudaMemcpyHostToDevice, st));
+    MBAR_CUDA(cudaMemcpyAsync(d_pc, hpc.data(), hpc.size() * sizeof(KdeManyPiece), cudaMemcpyHostToDevice, st));
+    MBAR_CUDA(cudaEventRecord(k->ev0, st));
+    for (const Launch& L : launches) {
+        if (L.fn) {
+            L.fn<<<(unsigned)L.items, KDE_THREADS, 0, st>>>(d_pc + L.rec, L.n, k->d_x, d_lw, d_y, d_pm, d_ps);
+        } else if (L.items > 0) {
+            kde_many_combine_kernel<<<(unsigned)((L.items + 127) / 128), 128, 0, st>>>(d_pc + L.rec, L.n, L.o0, L.items,
+                                                                                      d_pm, d_ps, d_out);
+        }
+    }
+    MBAR_CUDA(cudaGetLastError());
+    MBAR_CUDA(cudaEventRecord(k->ev1, st));
+    if (outs > 0) MBAR_CUDA(cudaMemcpyAsync(out, d_out, (size_t)outs * sizeof(double), cudaMemcpyDeviceToHost, st));
+    MBAR_CUDA(cudaStreamSynchronize(st));
+    float e = 0.f;
+    k->lastMs = event_ms(k->ev0, k->ev1, &e) ? e : 0.0;
+    k->lastLaunches = (int32_t)launches.size();
+    k->lastPairs = pairs;
+    return MBAR_B200_OK;
+}
+
+int mbar_b200_last_kde_many_stats(mbar_b200_kde_many* k, double* ms, int32_t* launches, int64_t* pairs) {
+    MBAR_REQUIRE(k, MBAR_B200_ERR_INVALID, "NULL kde_many object");
+    if (ms) *ms = k->lastMs;
+    if (launches) *launches = k->lastLaunches;
+    if (pairs) *pairs = k->lastPairs;
     return MBAR_B200_OK;
 }

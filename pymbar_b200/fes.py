@@ -313,22 +313,21 @@ def _draw_as_sample(kernel, D):
     rng.normal(size=(1, D))
 
 
-def kde_query(kde, settings, x, reference_point, fes_reference, log_sum_w, with_fmin=False):
-    """_get_fes_kde (fes.py:1523-1609) without uncertainties, from kde.log_sum (a DeviceKde): {"f_i", "df_i": None}
-    with f_i = -score_samples(x) relative to the reference point, log_sum_w = log sum_n w_n of the fitted weights.
-    with_fmin=True also returns the reference's fmin, the -score_samples subtracted for "from-lowest" and
-    "from-specified" (None for "from-normalization"): (out, fmin).
-
-    "from-specified" evaluates its reference point in the same call as the queries (a query's result does not
-    depend on the others).  Raises what the reference raises: IndexError for 1-D x, NotImplementedError for kernels
-    sklearn cannot sample from, DataError on a dimension mismatch, ParameterError for another reference point."""
+def _kde_errors():
     try:
         from pymbar.utils import DataError, ParameterError
     except ImportError:
         from .utils import ParameterError
 
         DataError = ParameterError
-    kernel, h, D = settings["kernel"], settings["h"], settings["D"]
+    return DataError, ParameterError
+
+
+def kde_query_prepare(settings, x, reference_point, fes_reference):
+    """The host steps of kde_query before the device sums: (y [Q, D], or [Q + 1, D] with the "from-specified" point
+    last, and Q).  Draws what KernelDensity.sample() draws and raises what the reference raises before its scoring."""
+    DataError, _ = _kde_errors()
+    kernel, D = settings["kernel"], settings["D"]
     dims = np.shape(x)[1]
     _draw_as_sample(kernel, D)
     if dims != D:
@@ -340,8 +339,15 @@ def kde_query(kde, settings, x, reference_point, fes_reference, log_sum_w, with_
         if ref.shape[1] != D:
             raise ValueError(f"X has {ref.shape[1]} features, but KernelDensity is expecting {D} features as input.")
         y = np.vstack([y, ref])
+    return y, Q
+
+
+def kde_query_finish(settings, log_sums, Q, reference_point, log_sum_w, with_fmin=False):
+    """kde_query from the device's log sums of kde_query_prepare's points."""
+    _, ParameterError = _kde_errors()
+    kernel, h, D = settings["kernel"], settings["h"], settings["D"]
     # sklearn: the tree's log sum, += the kernel's normalisation, -= log of the weight sum
-    score = kde.log_sum(kernel, h, y)
+    score = np.array(log_sums, dtype=np.float64)
     score += kde_log_norm(kernel, D, h)
     score -= log_sum_w
     f_i = -score[:Q]
@@ -358,6 +364,21 @@ def kde_query(kde, settings, x, reference_point, fes_reference, log_sum_w, with_
         raise ParameterError(f"reference point choice {reference_point} for kde is unavailable")
     out = {"f_i": f_i, "df_i": None}
     return (out, fmin) if with_fmin else out
+
+
+def kde_query(kde, settings, x, reference_point, fes_reference, log_sum_w, with_fmin=False):
+    """_get_fes_kde (fes.py:1523-1609) without uncertainties, from kde.log_sum (a DeviceKde): {"f_i", "df_i": None}
+    with f_i = -score_samples(x) relative to the reference point, log_sum_w = log sum_n w_n of the fitted weights.
+    with_fmin=True also returns the reference's fmin, the -score_samples subtracted for "from-lowest" and
+    "from-specified" (None for "from-normalization"): (out, fmin).
+
+    "from-specified" evaluates its reference point in the same call as the queries (a query's result does not
+    depend on the others).  Raises what the reference raises: IndexError for 1-D x, NotImplementedError for kernels
+    sklearn cannot sample from, DataError on a dimension mismatch, ParameterError for another reference point.
+    kde_query_prepare and kde_query_finish are its two host halves, for callers that batch the device sums."""
+    y, Q = kde_query_prepare(settings, x, reference_point, fes_reference)
+    log_sums = kde.log_sum(settings["kernel"], settings["h"], y)
+    return kde_query_finish(settings, log_sums, Q, reference_point, log_sum_w, with_fmin)
 
 
 SPLINE_WEIGHTS = ("unbiasedstate", "biasedstates", "simplesum")

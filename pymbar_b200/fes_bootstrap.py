@@ -248,8 +248,14 @@ def kde_bootstrap_query(kde, settings, x, reference_point, fes_reference, log_su
     out, fmin = hist.kde_query(kde, settings, x, reference_point, fes_reference, log_sum_w, with_fmin=True)
     kernel, h, D = settings["kernel"], settings["h"], settings["D"]
     y = np.asarray(x, dtype=np.float64).reshape(-1, D)
-    score = kde.log_sum_replicates(kernel, h, y)
-    score += hist.kde_log_norm(kernel, D, h)
+    return kde_bootstrap_finish(settings, out, fmin, kde.log_sum_replicates(kernel, h, y), log_sum_w)
+
+
+def kde_bootstrap_finish(settings, out, fmin, log_sums, log_sum_w):
+    """kde_bootstrap_query's df_i from the replicates' log sums [B, Q] at the queries (fes.py:1590-1601); out and fmin
+    are kde_query's (with_fmin=True).  Returns out with df_i set."""
+    score = np.array(log_sums, dtype=np.float64)
+    score += hist.kde_log_norm(settings["kernel"], settings["D"], settings["h"])
     score -= log_sum_w
     fall = -score.T - fmin
     out["df_i"] = np.std(fall, axis=1)

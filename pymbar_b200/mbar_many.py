@@ -53,6 +53,7 @@ from .utils import ParameterError
 
 DeviceMbarBatch = None     # the device classes; resolved on first use (a test may put stand-ins here)
 DeviceProblem = None
+DeviceKdeMany = None
 
 MAX_BATCH_K = 64
 UNCERTAINTY_METHODS = (None, "svd-ew", "approximate", "bootstrap")
@@ -63,6 +64,19 @@ AUG_WAVE_BYTES = 2 << 30    # device footprint of one wave of appended rows
 ESTIMATOR_METHODS = (None, "svd-ew", "approximate", "bootstrap")
 FES_WAVE_BYTES = 2 << 30    # device footprint of one wave of histogram FES requests
 FES_UNCERTAINTY_METHODS = (None, "analytical", "bootstrap")
+FES_TYPES = ("histogram", "kde")
+KDE_WAVE_BYTES = 1 << 30    # device footprint of the requests of one DeviceKdeMany.log_sum call
+KDE_PART_BYTES = 64 << 20   # kde.cu: the chunk partials of one sub-batch of a DeviceKdeMany.log_sum call
+KDE_PIECE_BYTES = 112       # kde.cu: sizeof(KdeManyPiece)
+
+
+def _kde_class():
+    global DeviceKdeMany
+    if DeviceKdeMany is None:
+        from .problem import DeviceKdeMany as K
+
+        DeviceKdeMany = K
+    return DeviceKdeMany
 
 
 def _classes():
@@ -188,6 +202,32 @@ def rep_bin_bytes(K, N, nbins):
     return 32 * nT * 32 + 40 * nbins + 8 * _bin_geometry(nT, 1, nbins)[2] * nbins + 8 * K + 180
 
 
+def log_weight_bytes(K, N):
+    """Device bytes of one request of DeviceMbarBatch.log_weights in a wave: its u_n / log w_n slots, its f, its flag
+    and its request record (batch.cu's geometry)."""
+    nT = -(-int(N) // 32)
+    return 8 * nT * 32 + 8 * int(K) + 4 + 164
+
+
+def _kde_chunks(N):
+    """Chunks of a sample set of N samples (kde_chunking in kde.cu)."""
+    N = int(N)
+    nPad = -(-N // 256) * 256
+    nc = min(1024, max(1, -(-N // 4096)))
+    chunk = -(-(-(-N // nc)) // 256) * 256
+    return nPad, -(-nPad // chunk)
+
+
+def kde_bytes(N, D, Q):
+    """Device bytes of one DeviceKdeMany.log_sum request on a set of N samples in D dimensions with Q queries: its log
+    weights (padded to 256), queries and outputs, and two records for each of its pieces of at most kde_query_cap
+    queries (kde.cu).  The chunk partials of a call take at most KDE_PART_BYTES beyond these, or one piece's."""
+    nPad, nc = _kde_chunks(N)
+    cap = max(128, (KDE_PART_BYTES // (16 * nc)) // 128 * 128)
+    pieces = -(-int(Q) // cap)
+    return 8 * nPad + 8 * int(D) * int(Q) + 8 * int(Q) + 2 * KDE_PIECE_BYTES * pieces
+
+
 def _waves(items, need, limit):
     """items split, in order, into waves whose need(item) sum stays under limit (one item at least per wave)."""
     waves, wave, used = [], [], 0
@@ -228,6 +268,15 @@ def _validate_fes_boot(n_bootstraps, seed, P):
             raise ParameterError(f"problem {p}: seed must be an int >= 0, -1 or None, got {v!r}")
         out.append(None if v is None or v < 0 else int(v))
     return out
+
+
+def _kde_defaults():
+    """KernelDensity().get_params(): the parameters pymbar.FES._setup_fes_kde fills kde_parameters into."""
+    try:
+        from sklearn.neighbors import KernelDensity
+    except ImportError:
+        raise ImportError("Cannot use 'kde' type FES without the scikit-learn module. Could not import sklearn")
+    return KernelDensity().get_params()
 
 
 def _validate_boot(n_bootstraps, rseed, P):
@@ -435,9 +484,14 @@ class MbarMany:
         self.fes_boot_single = [0] * P       # problem -> how many of those replicates took the single path
         self._tol, self._opts = solver_tolerance, opts
         self._fes = {}                       # problem -> its histogram request, path and cached Theta
+        self.fes_types = [None] * P          # problem -> "histogram" or "kde": the surface the last generate_fes built
+        self.kde_settings = [None] * P       # problem -> {"kernel", "h", "D"} of its KDE surface
+        self._kde = {}                       # problem -> its KDE surface: sample set, weights, replicate weights, path
+        self._closed = False
         self.device_stats = dict(ms=0.0, launches=0, calls=0, bytes_read=0)
         # host time spent regenerating replicate counts for the estimators, and drawing bootstrap surfaces' replicates
         self.host_stats = dict(counts_s=0.0, fes_draws_s=0.0)
+        self.kde_stats = dict(ms=0.0, launches=0, calls=0, pairs=0, upload_bytes=0)   # DeviceKdeMany calls
         try:
             self.results = self._solve(probs, seeds, B, compute_uncertainty, uncertainty_method, return_theta,
                                        solver_tolerance, opts)
@@ -446,8 +500,9 @@ class MbarMany:
             raise
 
     def close(self):
-        """Free the device batch.  The results stay."""
+        """Free the device batch and the KDE sample sets.  The results stay."""
         self._dev = None
+        self._closed = True
         self._stack.close()
 
     def __enter__(self):
@@ -834,7 +889,7 @@ class MbarMany:
         return [value] * P
 
     def generate_fes(self, u_n_list, x_n_list, fes_type="histogram", histogram_parameters=None, n_bootstraps=0,
-                     seed=None):
+                     seed=None, kde_parameters=None):
         """The histogram FES of the target state u_n_list[p] [N_p] over the coordinates x_n_list[p] ([N_p] or
         [N_p, dims]) of every problem (pymbar.FES.generate_fes with fes_type="histogram"); an entry None skips its
         problem, whose earlier surface, if any, stays.  histogram_parameters: {"bin_edges": ...} for every problem,
@@ -852,9 +907,22 @@ class MbarMany:
         (continue the global stream) or one entry per problem, an int >= 0 (np.random.seed before the problem's
         draws), -1 or None.  With B = 0 the generator is not touched and replicate_histogram_datas[p] becomes None.
         A problem with an empty state, or a replicate that draws no sample from a bin tuple of the surface, raises
-        ParameterError; a call that raises restores the generator and changes no surface."""
-        if fes_type != "histogram":
-            raise ParameterError(f"fes_type {fes_type!r} is not served by MbarMany: only 'histogram' surfaces are")
+        ParameterError; a call that raises restores the generator and changes no surface.
+
+        fes_type="kde" (DESIGN.md 3.5h'') builds what pymbar.FES(u_kn_p, N_k_p).generate_fes(u_n_p, x_n_p,
+        fes_type="kde", kde_parameters=..., n_bootstraps=B, seed=seed[p]) builds.  kde_parameters: one dict of
+        KernelDensity parameters for every problem, or one per problem; an unknown key raises the reference's
+        ParameterError, and so do parameters fes.kde_settings does not serve (another metric, metric_params, more
+        than 4 dimensions, values sklearn's fit rejects) and None, where the reference raises TypeError.  b = 0's
+        weights come from one log_weights call per wave on the batch (DeviceProblem.log_denominator for problems on
+        the single path or flagged there; self._kde[p]["path"]), normalised as fes.py:411-414 does.  Replicate b puts
+        weight V_bn = sum of w_m over the positions m with idx_b[m] = n on sample n (b = 0's weights by position,
+        fes.py:689-699); the reference's K MBAR constructions per replicate change no KDE output and are not run, but
+        their seed draws are made.  The call's coordinates are uploaded once into one DeviceKdeMany; the surfaces are
+        scored at get_fes.  self.kde_settings[p] becomes {"kernel", "h", "D"} and self.fes_types[p] "kde"; a KDE surface
+        clears the problem's histogram_datas and replicate_histogram_datas, and a histogram surface clears its KDE."""
+        if fes_type not in FES_TYPES:
+            raise ParameterError(f"fes_type {fes_type!r} is not served by MbarMany (one of {FES_TYPES})")
         P = len(self._probs)
         seeds = _validate_fes_boot(n_bootstraps, seed, P)
         B = int(n_bootstraps)
@@ -862,6 +930,8 @@ class MbarMany:
             if v is None or len(v) != P:
                 raise ParameterError(f"{name} must hold one entry (or None) per problem ({P}), got "
                                      f"{'None' if v is None else len(v)}")
+        if fes_type == "kde":
+            return self._generate_kde(u_n_list, x_n_list, kde_parameters, B, seeds)
         params = self._per_problem(histogram_parameters, lambda p, v: isinstance(v, dict))
         reqs = {}
         for p in range(P):
@@ -928,6 +998,131 @@ class MbarMany:
             self._fes[p] = dict(u_n=r["u_n"], dense=r["dense"], nb=r["nb"], path=r["path"], theta=None)
             self.replicate_histogram_datas[p] = reps.get(p)
             self.fes_boot_single[p] = nsingle.get(p, 0)
+            self.fes_types[p] = "histogram"
+            self.kde_settings[p] = None
+            self._kde.pop(p, None)
+
+    def _generate_kde(self, u_n_list, x_n_list, kde_parameters, B, seeds):
+        """generate_fes(..., fes_type="kde") (DESIGN.md 3.5h''): every argument checked, then the target weights, the
+        replicate weights and one DeviceKdeMany upload of the call's coordinates; the surfaces are committed last."""
+        P = len(self._probs)
+        params = self._per_problem(kde_parameters, lambda p, v: isinstance(v, dict))
+        reqs = {}
+        defaults = None
+        for p in range(P):
+            u, x = u_n_list[p], x_n_list[p]
+            if u is None and x is None:
+                continue
+            if u is None or x is None:
+                raise ParameterError(f"problem {p}: give both u_n and x_n, or neither")
+            par = params[p]
+            if not isinstance(par, dict):
+                raise ParameterError(f"problem {p}: fes_type 'kde' needs kde_parameters, a dict of KernelDensity "
+                                     f"parameters, got {par!r}")
+            if defaults is None:
+                defaults = _kde_defaults()
+            for k in par:
+                if k not in defaults:
+                    raise ParameterError(f"problem {p}: Warning: {k} is not a parameter in KernelDensity")
+            N = self._probs[p][0].shape[1]
+            u = np.asarray(u, dtype=np.float64)
+            if u.shape != (N,):
+                raise ParameterError(f"problem {p}: u_n has shape {u.shape}, the problem has N={N} samples")
+            if np.isnan(u).any():
+                raise ParameterError(f"problem {p}: u_n holds NaN")
+            xa = np.asarray(x, dtype=np.float64)
+            if xa.ndim == 1:
+                xa = xa.reshape(-1, 1)
+            if xa.ndim != 2 or xa.shape[0] != N:
+                raise ParameterError(f"problem {p}: x_n has shape {np.shape(x)}, the problem has N={N} samples")
+            if not np.all(np.isfinite(xa)):
+                raise ParameterError(f"problem {p}: x_n holds NaN or infinite coordinates")
+            settings = hist.kde_settings(dict(defaults, **par), N, xa.shape[1])
+            if settings is None:
+                raise ParameterError(f"problem {p}: kde_parameters {par!r} in {xa.shape[1]} dimension(s) are not served "
+                                     f"by MbarMany (euclidean metric, no metric_params, 1 to 4 dimensions, and values "
+                                     f"KernelDensity.fit accepts)")
+            if B > 0 and np.any(np.asarray(self._probs[p][1]) == 0):
+                raise ParameterError(f"problem {p}: a state without samples cannot be resampled for bootstrap "
+                                     f"surfaces")
+            reqs[p] = dict(u_n=u, x=np.ascontiguousarray(xa), settings=settings)
+        if not reqs:
+            return
+        # b = 0: log w_n = -u_n - L_n, one log_weights call per wave on the batch; the single path otherwise
+        log_w = {}
+        batched = [p for p in sorted(reqs) if self.results[p]["path"] == "batch" and p in self._slot]
+        single = [p for p in sorted(reqs) if p not in batched]
+        for wave in _waves(batched, lambda p: log_weight_bytes(*self._probs[p][0].shape), FES_WAVE_BYTES):
+            out, flags = self._dev.log_weights([self._slot[p] for p in wave], [self.results[p]["f_k"] for p in wave],
+                                               [reqs[p]["u_n"] for p in wave])
+            self._count()
+            for p, lw, flag in zip(wave, out, flags):
+                if flag:
+                    single.append(p)
+                else:
+                    log_w[p] = lw
+                    reqs[p]["path"] = "batch"
+        _, Prob = _classes()
+        for p in sorted(single):
+            u_kn, N_k, _ = self._probs[p]
+            with Prob(u_kn, N_k, device=ms._DEVICE) as q:
+                L = q.log_denominator(np.asarray(self.results[p]["f_k"], dtype=np.float64))
+            log_w[p] = -reqs[p]["u_n"] - L            # facade._device_log_weights
+            reqs[p]["path"] = "single"
+        for p in sorted(reqs):
+            lw = log_w[p]
+            with np.errstate(invalid="ignore", over="ignore"):
+                w = np.exp(lw - np.max(lw))           # fes.py:411-414
+                w = w / np.sum(w)
+            if not np.all(np.isfinite(w)):
+                raise ParameterError(f"problem {p}: the target state's weights are not finite (log w_n holds NaN, or "
+                                     f"every sample has weight 0)")
+            reqs[p]["w"] = w
+            reqs[p]["log_sum_w"] = float(np.log(np.sum(w)))
+        order = sorted(reqs)
+        Kde = _kde_class()
+        dev = Kde([reqs[p]["x"] for p in order], device=ms._DEVICE)
+        try:
+            if B > 0:
+                state = np.random.get_state()
+                try:
+                    for p in order:
+                        reqs[p]["V"] = self._kde_replicates(p, reqs[p]["w"], B, seeds[p])
+                except BaseException:
+                    np.random.set_state(state)
+                    raise
+        except BaseException:
+            dev.close()
+            raise
+        self._stack.enter_context(dev)
+        self.kde_stats["upload_bytes"] += int(sum(reqs[p]["x"].nbytes for p in order))
+        for i, p in enumerate(order):
+            r = reqs[p]
+            self._kde[p] = dict(dev=dev, set=i, w=r["w"], log_sum_w=r["log_sum_w"], V=r.get("V"),
+                                settings=r["settings"], path=r["path"])
+            self.kde_settings[p] = r["settings"]
+            self.fes_types[p] = "kde"
+            self.histogram_datas[p] = None
+            self.replicate_histogram_datas[p] = None
+            self.fes_boot_single[p] = 0
+            self._fes.pop(p, None)
+
+    def _kde_replicates(self, p, w, B, seed):
+        """V [B, N_p]: the weight of every sample in each of problem p's B bootstrap replicates, V_bn = sum of w_m over
+        the positions m with idx_b[m] = n (the reference fits replicate b to x_n[idx_b] with b = 0's weights by
+        position, fes.py:689-699), drawn from numpy's global generator as the reference draws them."""
+        t0 = time.perf_counter()
+        N_k = np.asarray(self._probs[p][1]).astype(np.int64)
+        V = np.empty((B, len(w)))
+
+        def each(b, idx):
+            V[b] = np.bincount(idx, weights=w, minlength=len(w))
+
+        if seed is not None:
+            np.random.seed(seed)
+        fb.draw_replicates(N_k, B, each)
+        self.host_stats["fes_draws_s"] += time.perf_counter() - t0
+        return V
 
     def _fes_replicates(self, reqs, B, seeds):
         """({p: [B ReplicateHistogram]}, {p: replicates on the single path}) of every request of generate_fes, drawn
@@ -1064,40 +1259,65 @@ class MbarMany:
 
     def get_fes(self, x_list, reference_point="from-lowest", fes_reference=None, uncertainty_method=None):
         """f_i (and df_i with uncertainty_method="analytical" or "bootstrap") of every problem's surface at the points
-        x_list[p] (pymbar.FES.get_fes of a histogram surface), plus `path`, "batch" or "single"; an entry None skips
-        its problem.  fes_reference: one point for every problem, or one per problem.  Reference points and their
-        errors are those of the reference ("from-lowest", "from-specified"; "all-differences" and
-        "from-normalization" raise what it raises).  The first "analytical" query computes Theta for every problem
-        of the call that lacks one (one bin_moments call per wave) and keeps it.  "bootstrap" takes df_i from the
-        replicates of generate_fes(..., n_bootstraps=B) (fes.py:1417-1422), with no device work."""
+        x_list[p] (pymbar.FES.get_fes), plus `path`, "batch" or "single"; an entry None skips its problem.
+        fes_reference: one point for every problem, or one per problem.
+
+        Histogram surfaces: reference points and their errors are those of the reference ("from-lowest",
+        "from-specified"; "all-differences" and "from-normalization" raise what it raises).  The first "analytical"
+        query computes Theta for every problem of the call that lacks one (one bin_moments call per wave) and keeps
+        it.  "bootstrap" takes df_i from the replicates of generate_fes(..., n_bootstraps=B) (fes.py:1417-1422), with
+        no device work.
+
+        KDE surfaces (DESIGN.md 3.5h''): f_i = -score_samples(x) of the reference's KernelDensity, relative to
+        "from-lowest", "from-specified" or "from-normalization", and df_i None without uncertainties, as
+        _get_fes_kde (fes.py:1523-1609) returns them.  Every KDE problem of the call is answered by one
+        DeviceKdeMany.log_sum call per uploaded sample-set object and wave (waves under KDE_WAVE_BYTES): a request
+        holds a problem's queries and its "from-specified" point and, with "bootstrap", one request per replicate
+        holds its queries under the replicate's weights.  df_i is then np.std over the replicates of
+        -score_b - fmin, every replicate sharing b = 0's weight sum (fes.py:1590-1601).  As in the reference, the
+        gaussian and tophat kernels draw from numpy's global generator at every query (KernelDensity.sample) and the
+        other kernels raise NotImplementedError, and a dimension mismatch raises DataError.  "analytical" raises the
+        reference's ParameterError; "bootstrap" with "from-normalization" raises ParameterError, where the reference
+        fails with UnboundLocalError.  Problems are taken in increasing order; a call that raises, raises for the
+        lowest failing problem and restores numpy's generator.  After close(), a KDE query raises ParameterError."""
         if uncertainty_method not in FES_UNCERTAINTY_METHODS:
-            raise ParameterError(f"uncertainty_method {uncertainty_method!r} is not served by MbarMany's histogram "
-                                 f"FES (one of {FES_UNCERTAINTY_METHODS})")
+            raise ParameterError(f"uncertainty_method {uncertainty_method!r} is not served by MbarMany's FES "
+                                 f"(one of {FES_UNCERTAINTY_METHODS})")
         P = len(self._probs)
         if x_list is None or len(x_list) != P:
             raise ParameterError(f"x_list must hold one entry (or None) per problem ({P}), got "
                                  f"{'None' if x_list is None else len(x_list)}")
         asked = [p for p in range(P) if x_list[p] is not None]
         for p in asked:
-            if p not in self._fes:
+            if self.fes_types[p] is None:
                 raise ParameterError(f"problem {p}: get_fes before generate_fes built its surface")
-            if uncertainty_method == "bootstrap" and self.replicate_histogram_datas[p] is None:
+            if self.fes_types[p] == "histogram" and uncertainty_method == "bootstrap" and \
+                    self.replicate_histogram_datas[p] is None:
                 raise ParameterError(f"problem {p}: Can't calculate uncertainties via bootstrap if bootstrapping was "
                                      f"not performed when running get_fes")
+        kde_asked = [p for p in asked if self.fes_types[p] == "kde"]
+        hist_asked = [p for p in asked if self.fes_types[p] == "histogram"]
 
         def single_ref(p, v):
-            dims = self.histogram_datas[p]["dims"] if p in self._fes else 1
+            if self.fes_types[p] == "kde":
+                dims = self.kde_settings[p]["D"]
+            else:
+                dims = self.histogram_datas[p]["dims"] if p in self._fes else 1
             return np.ndim(v) == 0 if dims == 1 else (np.shape(v) == (dims,))
 
         refs = self._per_problem(fes_reference, single_ref)
-        analytical = uncertainty_method == "analytical"
         out = [None] * P
-        for p in asked:
+        if kde_asked:
+            got = self._kde_get_fes(kde_asked, x_list, reference_point, refs, uncertainty_method)
+            for p in kde_asked:
+                out[p] = got[p]
+        analytical = uncertainty_method == "analytical"
+        for p in hist_asked:
             data = self.histogram_datas[p]
             K = self._probs[p][0].shape[0]
 
             def df_fn(j, p=p, data=data, K=K):
-                self._thetas(asked)
+                self._thetas(hist_asked)
                 return hist.bin_uncertainties(self._fes[p]["theta"], K, j, len(data["f"]))
 
             def boot_fn(j, p=p, data=data):
@@ -1107,6 +1327,83 @@ class MbarMany:
             r = hist.query(data, x_list[p], reference_point, refs[p], fn)
             out[p] = dict(r, path=self._fes[p]["path"])
         return out
+
+    def _kde_get_fes(self, problems, x_list, reference_point, refs, uncertainty_method):
+        """{p: get_fes dict} of the KDE problems `problems` (increasing): kde_query_prepare for each, the device sums of
+        every request in waves, then kde_query_finish (and kde_bootstrap_finish).  numpy's generator is restored when
+        anything raises."""
+        boot = uncertainty_method == "bootstrap"
+        state = np.random.get_state()
+        try:
+            prep = {}
+            for p in problems:
+                if self._closed:
+                    raise ParameterError(f"problem {p}: the KDE surface's samples were freed by close()")
+                k = self._kde[p]
+                x = np.array(x_list[p])
+                if np.ndim(x) <= 1:
+                    x = x.reshape(-1, 1)              # FES.get_fes
+                y, Q = hist.kde_query_prepare(k["settings"], x, reference_point, refs[p])
+                if reference_point not in ("from-lowest", "from-specified", "from-normalization"):
+                    raise hist._kde_errors()[1](f"reference point choice {reference_point} for kde is unavailable")
+                if uncertainty_method == "analytical":
+                    raise ParameterError(f"problem {p}: Uncertainty method {uncertainty_method} for kde is not "
+                                         f"implemented")
+                if boot and k["V"] is None:
+                    raise ParameterError(f"problem {p}: Cannot calculate bootstrap error of bootstrap KDE's not "
+                                         f"determined")
+                if boot and reference_point == "from-normalization":
+                    raise ParameterError(f"problem {p}: bootstrap uncertainties of a KDE surface need a reference "
+                                         f"point: 'from-normalization' has none (the reference fails there)")
+                prep[p] = (y, Q)
+            # requests: (problem, -1) for b = 0 (queries and the reference point), (problem, b) per replicate
+            sums = {}
+            by_dev = {}
+            for p in problems:
+                by_dev.setdefault(id(self._kde[p]["dev"]), []).append(p)
+            for ps in by_dev.values():
+                dev = self._kde[ps[0]]["dev"]
+                items = [(p, -1) for p in ps]
+                if boot:
+                    items += [(p, b) for p in ps for b in range(self._kde[p]["V"].shape[0])]
+
+                def need(it):
+                    p, b = it
+                    k = self._kde[p]
+                    n = prep[p][0].shape[0] if b < 0 else prep[p][1]
+                    return kde_bytes(len(k["w"]), k["settings"]["D"], n)
+
+                for wave in _waves(items, need, KDE_WAVE_BYTES - KDE_PART_BYTES):
+                    reqs = [(p, b) for p, b in wave]
+                    ks = [self._kde[p] for p, _ in reqs]
+                    got = dev.log_sum([k["set"] for k in ks], [k["settings"]["kernel"] for k in ks],
+                                      [k["settings"]["h"] for k in ks],
+                                      [k["w"] if b < 0 else k["V"][b] for (p, b), k in zip(reqs, ks)],
+                                      [prep[p][0] if b < 0 else prep[p][0][:prep[p][1]] for p, b in reqs])
+                    self._count_kde(dev)
+                    for it, l in zip(reqs, got):
+                        sums[it] = l
+            out = {}
+            for p in problems:
+                k = self._kde[p]
+                y, Q = prep[p]
+                r, fmin = hist.kde_query_finish(k["settings"], sums[(p, -1)], Q, reference_point, k["log_sum_w"],
+                                                with_fmin=True)
+                if boot:
+                    reps = np.array([sums[(p, b)] for b in range(k["V"].shape[0])])
+                    r = fb.kde_bootstrap_finish(k["settings"], r, fmin, reps, k["log_sum_w"])
+                out[p] = dict(r, path=k["path"])
+            return out
+        except BaseException:
+            np.random.set_state(state)
+            raise
+
+    def _count_kde(self, dev):
+        s = dev.last_stats()
+        self.kde_stats["ms"] += s["ms"]
+        self.kde_stats["launches"] += s["launches"]
+        self.kde_stats["calls"] += 1
+        self.kde_stats["pairs"] += s["pairs"]
 
     def compute_effective_sample_number(self):
         """N_eff [K_p] of every problem (MBAR.compute_effective_sample_number), from W^T W at the final f."""

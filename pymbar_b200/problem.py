@@ -502,6 +502,73 @@ class DeviceKde(_Resident):
         return dict(ms=ms.value, chunks=chunks.value)
 
 
+class DeviceKdeMany(_Resident):
+    """Many sample sets x_list[s] ([N_s] or [N_s, D_s], D_s = 1..4) resident on one H100 for kernel-density sums of
+    many small problems in one call (mbar_b200_kde_many_*).  Only the coordinates are resident: every request brings
+    its own weights, so a surface and each of its bootstrap replicates are requests on the same set.
+
+    `log_sum(sets, kernels, hs, w_list, y_list)` returns, per request r, l_q = log sum_n w_n k(|y_q - x_n| / h) over
+    set sets[r] with weights w_list[r] [N_s], kernel kernels[r] and bandwidth hs[r] at the queries y_list[r] [Q_r, D_s]:
+    the same bits DeviceKde(x_list[s], w).log_sum gives."""
+
+    _destroy = "mbar_b200_kde_many_destroy"
+
+    def __init__(self, x_list, device=0):
+        self._lib = _lib.load()
+        self._h = C.c_void_p()
+        xs = []
+        for s, x in enumerate(x_list):
+            x = np.asarray(x, dtype=np.float64)
+            if x.ndim == 1:
+                x = x.reshape(-1, 1)
+            if x.ndim != 2:
+                raise ValueError(f"set {s}: x_n must be [N] or [N, D], got shape {x.shape}")
+            xs.append(np.ascontiguousarray(x))
+        if not xs:
+            raise ValueError("need at least one sample set")
+        self.N = np.ascontiguousarray([x.shape[0] for x in xs], dtype=np.int64)
+        self.D = np.ascontiguousarray([x.shape[1] for x in xs], dtype=np.int32)
+        self.device = int(device)
+        flat = np.ascontiguousarray(np.concatenate([x.ravel() for x in xs]))
+        check(self._lib.mbar_b200_kde_many_create(self.device, len(xs), _i32p(self.D), _i64p(self.N), _dptr(flat),
+                                                  C.byref(self._h)))
+
+    def log_sum(self, sets, kernels, hs, w_list, y_list):
+        """[l [Q_r]] per request; kernels are names of KDE_KERNELS or their codes."""
+        sets = np.ascontiguousarray(sets, dtype=np.int32).reshape(-1)
+        n = sets.size
+        if not (len(kernels) == len(hs) == len(w_list) == len(y_list) == n):
+            raise ValueError("need one set, kernel, bandwidth, weight vector and query array per request")
+        codes = np.ascontiguousarray([KDE_KERNELS.index(k) if isinstance(k, str) and k in KDE_KERNELS else
+                                      (-1 if isinstance(k, str) else int(k)) for k in kernels], dtype=np.int32)
+        known = [0 <= s < self.N.size for s in sets]           # an unknown set is the library's error
+        ws, ys = [], []
+        for r, (s, ok, w, y) in enumerate(zip(sets, known, w_list, y_list)):
+            w = _f64(w, int(self.N[s]) if ok else None)
+            y = np.asarray(y, dtype=np.float64)
+            D = int(self.D[s]) if ok else (y.shape[1] if y.ndim == 2 else 1)
+            if y.ndim == 1 and D == 1:
+                y = y.reshape(-1, 1)
+            if y.ndim != 2 or y.shape[1] != D:
+                raise ValueError(f"request {r}: queries must be [Q, {D}], got shape {y.shape}")
+            ws.append(w)
+            ys.append(np.ascontiguousarray(y))
+        Q = np.ascontiguousarray([y.shape[0] for y in ys], dtype=np.int64)
+        w = np.ascontiguousarray(np.concatenate(ws)) if ws else np.zeros(0)
+        y = np.ascontiguousarray(np.concatenate([a.ravel() for a in ys])) if ys else np.zeros(0)
+        h = np.ascontiguousarray(hs, dtype=np.float64).reshape(-1)
+        out = np.empty(int(Q.sum()))
+        check(self._lib.mbar_b200_kde_many_log_sum(self._h, n, _i32p(sets), _i32p(codes), _dptr(h), _dptr(w),
+                                                   _i64p(Q), _dptr(y), _dptr(out)))
+        return np.split(out, np.cumsum(Q)[:-1]) if n else []
+
+    def last_stats(self):
+        """CUDA-event time (ms) of the last log_sum's kernels, its kernel launches and (query, sample) pairs."""
+        ms, launches, pairs = C.c_double(0), C.c_int32(0), C.c_int64(0)
+        check(self._lib.mbar_b200_last_kde_many_stats(self._h, C.byref(ms), C.byref(launches), C.byref(pairs)))
+        return dict(ms=ms.value, launches=launches.value, pairs=pairs.value)
+
+
 class DeviceBSpline(_Resident):
     """Samples x_n [N] with optional weights w_n and state labels state_n in [0, K) resident on one H100 for B-spline
     basis sums (mbar_b200_bspline_*).
@@ -945,6 +1012,29 @@ class DeviceMbarBatch(_Resident):
             _i32p(np.ascontiguousarray(np.concatenate(bs), dtype=np.int32)), _i32p(nb), sl.size, _i32p(sl), _i32p(tg),
             _dptr(f), _dptr(f_bin), _i32p(flag)))
         return np.split(f_bin, np.cumsum(out_nb)[:-1]), flag.astype(bool)
+
+    def log_weights(self, problems, f_list, u_n_list):
+        """Target-state log weights of every request in one call (mbar_b200_batch_log_weights): request r is problem
+        problems[r] at its converged f_list[r] [K_p] with the target state's u_n_list[r] [N_p].  Returns ([log_w [N_p]
+        per request], flags bool) with log w_n = -u_n - L_n, L_n = log sum_{k sampled} N_k exp(f_k - u_kn); u_n = +inf
+        gives -inf.  A flagged request holds a NaN log w_n."""
+        ids = np.ascontiguousarray(problems, dtype=np.int32).reshape(-1)
+        n = ids.size
+        if n == 0 or not (len(f_list) == len(u_n_list) == n):
+            raise ValueError("need one problem, f and u_n per request, and at least one")
+        known = [0 <= p < self.P for p in ids]          # an unknown problem is the library's error
+        us = [_f64(u) for u in u_n_list]
+        for r, (u, p, ok) in enumerate(zip(us, ids, known)):
+            if ok and u.shape != (int(self.N[p]),):
+                raise ValueError(f"request {r}: u_n {u.shape} must have shape ({int(self.N[p])},)")
+        f = np.ascontiguousarray(np.concatenate([_f64(v, int(self.K[p])) if ok else _f64(v)
+                                                 for v, p, ok in zip(f_list, ids, known)]))
+        u = np.ascontiguousarray(np.concatenate(us))
+        out = np.empty(u.size)
+        flag = np.empty(n, np.int32)
+        check(self._lib.mbar_b200_batch_log_weights(self._h, n, _i32p(ids), _dptr(f), _dptr(u), _dptr(out),
+                                                    _i32p(flag)))
+        return np.split(out, np.cumsum([u.size for u in us])[:-1]), flag.astype(bool)
 
     def _requests(self, call, ids, f_list, rows, want_G, *flags, gram=True):
         """One batched moments call on requests f_list[r] [rows[r]] at units ids[r], `flags` passed after f; one dict
